@@ -1,21 +1,21 @@
 #!/usr/bin/env python
-"""bench.py - throughput of the DFQ calibration hot path on B200.
+"""bench.py - throughput of the DFQ calibration hot path on an H100.
 
 One "step" = one pass of the hot path (BN fold -> cross-layer equalization to convergence -> bias correction) over
-one synthetic stack of independent Conv[512,512,3,3]+BN+ReLU -> Conv[512,512,3,3]+BN blocks (BASELINE.json
-configs[4], the configuration the metric's HBM-roofline half is quoted on; it is the largest single-GPU
-configuration: 4096 layer pairs = 38.65 GB of fp32 weights).  Output: ONE JSON line (see README / DESIGN.md).
+one synthetic stack of independent Conv[512,512,3,3]+BN+ReLU -> Conv[512,512,3,3]+BN blocks.  The default of 2048
+layer pairs is 19.3 GB of fp32 weights; with the pristine copy every step restores from, 40.6 GB of an 80 GB H100.
+Output: ONE JSON line (see README / DESIGN.md).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--layers L] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--layers L] [--impl b200|reference] [--dump-outputs DIR]
 
   value      whole-job Conv/BN layer-pairs per second with the stack resident in HBM (device-timed, CUDA events)
   e2e        the same metric through the public API with HOST buffers: pinned host -> device, calibrate, device -> host
-  roofline   the dominant kernel (k_cle_engine): algorithmic bytes (8 B per weight per sweep) / its event-timed
-             duration, against MEASURED_PEAKS.json
+  roofline   the dominant kernel (k_cle_stack): algorithmic bytes (8 B per weight per sweep) / its event-timed
+             duration, against MEASURED_PEAKS.json or else the H100 SXM data sheet's 3.35 TB/s
   cpu_baseline  the oracle (oracle/) timed on the host cores on a bounded sample of the same workload
 
 `--impl reference` times the reference's CPU implementation of the path (its algorithm restated in oracle/, since
-the reference is Python and is not present on the GPU box) on the same workload shape.
+the reference is Python and is not imported by the benchmark) on the same workload shape.
 """
 import argparse
 import json
@@ -38,11 +38,11 @@ N_PER_LAYER = C * C * K * K
 def parse():
     p = argparse.ArgumentParser()
     p.add_argument("--gpus", type=int, default=1)
-    p.add_argument("--steps", type=int, default=10)
+    p.add_argument("--steps", type=int, default=10, help="timed steps (>= 1)")
     p.add_argument("--warmup", type=int, default=3)
-    p.add_argument("--layers", type=int, default=4096, help="Conv/BN pairs in the synthetic stack per GPU")
+    p.add_argument("--layers", type=int, default=2048, help="Conv/BN pairs in the synthetic stack per GPU")
     p.add_argument("--e2e-layers", type=int, default=512, help="pairs moved host->device->host per e2e step")
-    p.add_argument("--e2e-chunk", type=int, default=16, help="pairs per pipelined chunk of the e2e arm (measured: 32 pairs / 4 slots 4.93 k pairs/s, 16 / 6 5.05 k)")
+    p.add_argument("--e2e-chunk", type=int, default=16, help="pairs per pipelined chunk of the e2e arm")
     p.add_argument("--e2e-slots", type=int, default=6, help="arena slots of the e2e pipeline")
     p.add_argument("--cpu-layers", type=int, default=0, help="pairs in the CPU-baseline sample (0 = auto)")
     p.add_argument("--impl", default="b200", choices=["b200", "reference"])
@@ -55,11 +55,16 @@ def parse():
                    help="which curve is the line's headline `value` (the other one is reported next to it): weak = --layers "
                         "pairs PER GPU, strong = --layers pairs IN TOTAL split over the GPUs (SURVEY 8(d) config 5)")
     p.add_argument("--no-strong", action="store_true", help="skip the strong-scaling measurement")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what the last step computed (rank 0's stack) as DIR/<name>.npy")
+    args = p.parse_args()
+    if args.steps < 1:
+        p.error("--steps must be at least 1")
+    return args
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled while the timed region runs (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled while the timed region runs."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -91,24 +96,47 @@ class ClockSampler(threading.Thread):
                 "samples": len(self.rows), "reasons": reasons}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of the equalization kernel (k_cle_stack) from the committed `ncu --set full`
-# capture (profiles/r2_cle_stack_v2.md: 19.346 GB read + 19.292 GB written at 1024 pairs, 2 sweeps; algorithmic 38.655 GB).  The
-# kernel's traffic is linear in the number of pairs (every block is identical), so the figure is scaled to the benched size;
-# None for other sweep counts.  (k_cle_engine, round 1: 38.809 GB, profiles/r1_ncu_full_1024layers.md.)
-NCU_TRAFFIC_1024_PAIRS_2_SWEEPS = 38.638e9
-NCU_TRAFFIC_SOURCE = "ncu --set full capture of k_cle_stack at 1024 pairs (profiles/r2_cle_stack_v2.md), scaled linearly to the benched pairs"
-
-
-def ncu_traffic(layers, sweeps):
-    return NCU_TRAFFIC_1024_PAIRS_2_SWEEPS * layers / 1024.0 if sweeps == 2 else None
-
-
 def measured_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured"
+            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet (HBM3, 700 W card)"
+
+
+DUMP_WEIGHT_SAMPLE = 1 << 22        # weights written by --dump-outputs: 16 MB
+DUMP_VECTOR_CAP = 1 << 21           # elements per per-channel array, at most 8 MB each
+
+
+def dump_outputs(out_dir, stack, res):
+    """What the last timed step computed, as a caller of the path receives it: every block's scale vector S, every layer's
+    corrected bias and BN vectors (fake_weight / fake_bias), the sweeps each block ran, and a sample of the equalized
+    weights at positions fixed by a seeded generator (at most 4 x 8 MB + 16 MB in all).  Arrays larger than the cap are
+    sampled the same way."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    sess, C = stack.sess, stack.C
+
+    def sampled(t, cap, seed):
+        t = t.reshape(-1)
+        if t.numel() > cap:
+            idx = np.unique(np.random.default_rng(seed).integers(0, t.numel(), size=cap, dtype=np.int64))
+            t = t[torch.from_numpy(idx).to(t.device)]
+        return t.detach().cpu().numpy().astype(np.float32)
+
+    s_offs = stack.cle_plan["s_offs"]
+    arrays = {
+        "scale_vectors": torch.stack([sess.view(o, C) for o in s_offs]),
+        "biases": sess.view(stack.bias_begin, stack.n_layers * C),
+        "bn_fake_weight": torch.stack([sess.view(v["fake_w"], C) for v in stack.vec]),
+        "bn_fake_bias": torch.stack([sess.view(v["fake_b"], C) for v in stack.vec]),
+    }
+    for i, (name, t) in enumerate(arrays.items()):
+        np.save(os.path.join(out_dir, name + ".npy"), sampled(t, DUMP_VECTOR_CAP, i))
+    weights = stack.state()[:stack.n_layers * stack.N]
+    np.save(os.path.join(out_dir, "weights_sample.npy"), sampled(weights, DUMP_WEIGHT_SAMPLE, 100))
+    np.save(os.path.join(out_dir, "sweeps_per_block.npy"), np.asarray(res.group_sweeps, dtype=np.float64)[:stack.n_blocks])
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -214,10 +242,10 @@ def one_socket_cores():
 
 def run_reference(args, rank, world):
     """The reference's CPU execution of the path (oracle/eager_port.py: dfq.py's per-channel eager loop, deepcopy per sweep,
-    seven-pass fake quantization) on the box's host cores.  SURVEY 8(d): a 64-pair subsample of the stack; threads = the
+    seven-pass fake quantization) on the host cores.  SURVEY 8(d): a 64-pair subsample of the stack; threads = the
     physical cores of ONE socket with the process pinned to them (the ops are tiny - 4608-element rows - so more threads
-    only add OpenMP spin noise: round 1 saw 1.35 ... 15 pairs/s on the same box type with all 128 logical CPUs); value =
-    median step.  The reference itself is Python and absent on the GPU box: kind "port"."""
+    only add OpenMP spin noise); value = median of --steps steps.  The reference itself is Python and is not imported
+    here: kind "port"."""
     import torch
     if rank != 0:
         return
@@ -233,12 +261,9 @@ def run_reference(args, rank, world):
     for _ in range(min(args.warmup, 1)):
         cpu_pipeline(4, eager=True)
     times = []
-    budget = time.perf_counter() + 150.0           # keep the whole arm within a few minutes on a slow box
-    for _ in range(max(3, min(args.steps, 5))):
+    for _ in range(args.steps):
         dt, sweeps = cpu_pipeline(pairs, eager=True)
         times.append(dt)
-        if time.perf_counter() > budget and len(times) >= 3:
-            break
     times.sort()
     dt = times[len(times) // 2]
     val = pairs / dt
@@ -391,7 +416,7 @@ def run_b200(args, rank, world, local_rank):
 
     def make_step(st, se, saved, xch):
         def step(timers=None):
-            st.state().copy_(saved)                          # untimed: restores (and evicts L2 when the stack is >> 126 MB)
+            st.state().copy_(saved)                          # untimed: restores (and evicts L2 when the stack is >> 50 MB)
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
             ev[0].record()
             se.run_bn_fold(st.fold_plan)
@@ -432,6 +457,8 @@ def run_b200(args, rank, world, local_rank):
         res = step(timers)
     barrier()
     clocks = sampler.stop()
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, stack, res)
 
     # ---- parity of what was just timed: first and last block of this rank's stack vs the oracle (checker only) ---------
     parity = None
@@ -486,7 +513,7 @@ def run_b200(args, rank, world, local_rank):
                   "phases_ms_max_over_ranks": {"bn_fold": float(ts[1]), "equalize": float(ts[2]), "bias_correct": float(ts[3]),
                                                "exchange": float(ts[4])},
                   "exchange_bytes_per_rank": 4 * s_x.n,
-                  "l2": "%.1f GB of weights per GPU >> 126 MB L2; restored from a pristine copy (untimed) before every step"
+                  "l2": "%.1f GB of weights per GPU >> 50 MB L2; restored from a pristine copy (untimed) before every step"
                         % (4e-9 * N_PER_LAYER * 2 * s_blocks),
                   "what": "fixed total of %d pairs split over %d GPUs; speed-up over the 1-GPU weak line at the same total is "
                           "strong-scaling efficiency x N" % (world * 2 * s_blocks, world)}
@@ -498,7 +525,7 @@ def run_b200(args, rank, world, local_rank):
     cle_bytes = 8.0 * N_PER_LAYER * layers * res.n_sweeps          # SURVEY 8(d): 8 B per weight per sweep
     achieved = cle_bytes / (ms_cle * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "k_cle_stack (equalization of the two-layer chains; k_cle_engine when DFQ_CLE_STACK=0)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": ncu_traffic(layers, res.n_sweeps), "traffic_source": NCU_TRAFFIC_SOURCE, "peak_source": peak_src + " (MEASURED_PEAKS.json hbm_gbs, burst copy)",
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": cle_bytes, "ms_per_launch": ms_cle,
                 "whole_step": {"algorithmic_bytes": (26.0 + (12.0 if args.quantize else 0)) * N_PER_LAYER * layers,
                                "GB/s": (26.0 + (12.0 if args.quantize else 0)) * N_PER_LAYER * layers / (ms_step * 1e-3) / 1e9}}
@@ -591,7 +618,7 @@ def run_b200(args, rank, world, local_rank):
             mbv2 = {"error": repr(e)}
     cpu = None
     if not args.no_cpu_baseline and world == 1:
-        pairs = args.cpu_layers or 48          # ~5 s of single-core numpy on the GPU box (plus the input generation)
+        pairs = args.cpu_layers or 48          # a few seconds of single-core numpy (plus the input generation)
         import torch as _t
         _t.set_num_threads(os.cpu_count() or 1)
         dt, sw = cpu_pipeline(pairs)
@@ -604,7 +631,7 @@ def run_b200(args, rank, world, local_rank):
                                    "BN fold + equalization to convergence + bias correction%s" % (layers, " + 8-bit fake-quant" if args.quantize else ""),
                        "layers_per_gpu": layers, "weights_bytes_per_gpu": 4 * N_PER_LAYER * layers, "sweeps": res.n_sweeps,
                        "parallelism": "independent blocks sharded over %d rank(s); one all-gather of the scale vectors" % world,
-                       "l2": "working set %.1f GB >> 126 MB L2; state restored from a pristine copy (untimed) before every step" % (4e-9 * N_PER_LAYER * layers)},
+                       "l2": "working set %.1f GB >> 50 MB L2; state restored from a pristine copy (untimed) before every step" % (4e-9 * N_PER_LAYER * layers)},
             "phases_ms": {"bn_fold": phases[0], "equalize": phases[1], "bias_correct": phases[2], "exchange": phases[3]},
             "exchange": None if exchange is None else {"bytes_per_rank": 4 * exchange.n,
                                                        "carries": "S of every relation + corrected biases + BN vectors (fake_weight, fake_bias) of every layer, one all_gather_into_tensor"},

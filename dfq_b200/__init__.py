@@ -1,4 +1,4 @@
-"""dfq_b200: B200-native (sm_100a) implementation of the DFQ calibration hot path.
+"""dfq_b200: H100-native (sm_90a) implementation of the DFQ calibration hot path.
 
 Cross-layer weight equalization, bias correction, BN folding and fake quantization of
 jakc4103/DFQ, computed by hand-written CUDA kernels behind a C ABI (include/dfq_b200.h).

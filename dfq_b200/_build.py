@@ -1,7 +1,7 @@
-"""Build recipe for libdfq_sm100.so (hand-written sm_100a CUDA behind a C ABI).
+"""Build recipe for libdfq_sm90.so (hand-written sm_90a CUDA behind a C ABI).
 
-The library is built IN-TREE next to this file so that it travels with the repository snapshot to the
-GPU box; it is git-ignored.  nvcc cross-compiles for sm_100a without a GPU.
+The library is built IN-TREE next to this file so that the package is importable from the repository tree; it is
+git-ignored.  nvcc cross-compiles for sm_90a without a GPU.
 """
 import os
 import subprocess
@@ -9,13 +9,13 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.environ.get("DFQ_LIB_OUT") or os.path.join(HERE, "libdfq_sm100.so")
+LIB = os.environ.get("DFQ_LIB_OUT") or os.path.join(HERE, "libdfq_sm90.so")
 SOURCES = ["tensor_ops.cu", "cle_engine.cu", "passes.cu", "distill.cu", "host_copy.cu"]
 HEADERS = [os.path.join(CSRC, h) for h in ("common.cuh", "rowpipe.cuh", "colscan.cuh", "bc_stream.cuh")] + \
     [os.path.join(HERE, "..", "include", "dfq_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--fmad=false",          # every fp32 op of the reference is individually rounded: never contract
     "-Xcompiler", "-fPIC", "-shared",
@@ -41,7 +41,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if verbose or res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)
     if res.returncode != 0:
-        raise RuntimeError("nvcc failed building libdfq_sm100.so")
+        raise RuntimeError("nvcc failed building libdfq_sm90.so")
     with open(os.path.join(HERE, "build.log"), "w") as f:
         f.write(" ".join(cmd) + "\n" + res.stdout + res.stderr)
     return LIB

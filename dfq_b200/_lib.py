@@ -1,4 +1,4 @@
-"""ctypes binding of libdfq_sm100.so (the C ABI declared in include/dfq_b200.h).
+"""ctypes binding of libdfq_sm90.so (the C ABI declared in include/dfq_b200.h).
 
 There is no CPU fallback: if the library is missing and cannot be built, or a call fails, this module
 raises.  The descriptor structs mirror include/dfq_b200.h field for field (numpy structured dtypes
@@ -12,7 +12,7 @@ import os
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm100.so")   # DFQ_LIB: a tuning build
+LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
 ABI_VERSION = 1
 
@@ -124,7 +124,7 @@ def load(build_if_missing: bool = True) -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         if not build_if_missing:
-            raise DfqError("libdfq_sm100.so not built (run python -m dfq_b200._build)")
+            raise DfqError("libdfq_sm90.so not built (run python -m dfq_b200._build)")
         from . import _build
         _build.build()
     try:
@@ -138,7 +138,7 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dfq_last_error.restype = C.c_char_p
     lib.dfq_last_error.argtypes = []
     if lib.dfq_abi_version() != ABI_VERSION:
-        raise DfqError("libdfq_sm100.so ABI %d != binding %d" % (lib.dfq_abi_version(), ABI_VERSION))
+        raise DfqError("libdfq_sm90.so ABI %d != binding %d" % (lib.dfq_abi_version(), ABI_VERSION))
     _lib = lib
     return lib
 
@@ -158,7 +158,7 @@ def require_cuda():
     """The product path needs a GPU; never degrade to the CPU."""
     import torch
     if not torch.cuda.is_available():
-        raise DfqError("dfq_b200 requires a CUDA device (B200, sm_100a); no CPU fallback exists")
+        raise DfqError("dfq_b200 requires a CUDA device (H100, sm_90a); no CPU fallback exists")
 
 
 def stream_ptr():

@@ -1,4 +1,4 @@
-"""Whole-model calibration in ONE arena residency: the B200-native way to run the path.
+"""Whole-model calibration in ONE arena residency: the GPU-native way to run the path.
 
 The reference's drivers call merge_batchnorm / cross_layer_equalization / bias_correction / quantize_targ_layer one
 after the other on CPU-resident parameters (main_cls.py:144-180); the drop-in functions of this package mirror that and

@@ -2,8 +2,8 @@
 //
 // k_bc_engine processes one tile per CTA at a time: every 18 KB row pays two CTA-wide barriers, a serial 8-way fp64
 // sum and three dependent read-modify-writes by thread 0, and every element an IEEE division (MUFU.RCP + FCHK + 5 FFMA)
-// and an FRND - 2.15 TB/s on the synthetic stack (round 1: barrier 4.0 and wait 2.3 of the warp stall samples, issue
-// slots 52 % busy with the XU pipe saturated by MUFU.RCP + FRND: 2 x 4608 quarter-rate ops per row).
+// and an FRND: CTA barriers and waits dominate the warp stalls and the XU pipe saturates on MUFU.RCP + FRND (2 x 4608
+// quarter-rate ops per row).
 //
 // Here every consumer WARP owns whole tiles:
 //   * one CTA per SM: 8 consumer warps + 1 producer warp, a ring of kBcStages 18 KB stages (all of the SM's shared
@@ -17,7 +17,7 @@
 //   * the expectation vector of the current (layer, group) is cached per warp in shared memory (cols <= 512) across tiles;
 //   * the row is read with 32-bit shared-memory addresses (ld.shared, no generic LD + 64-bit address arithmetic) in a
 //     ROLLED column loop: the first version unrolled 16 x 9 taps x 5 variants = 23 800 SASS instructions and stalled on
-//     instruction fetch (ncu: no_instruction 1.39 per issue) - profiles/r2_bc_stream_v1.md;
+//     instruction fetch;
 //   * the quantization error is computed with no XU-pipe instruction:
 //       - the quotient t / scale as Markstein's correction of the product with the correctly rounded reciprocal
 //         (q0 = t*y, r = fma(-q0, s, t), q = fma(r, y, q0); y = __frcp_rn(s)): equal to the IEEE quotient when no
@@ -34,7 +34,6 @@
 namespace dfq {
 
 // 7 consumer warps + the producer = 8 warps = two per SM sub-partition; 11 - 7 = 4 stages loading while all consumers compute.
-// Measured on the stack (bias_correct ms at 4096 pairs): 4 consumers 4.88, 5: 4.89, 6: 4.31-4.54, 7: 4.15, 8: 4.76.
 #ifndef DFQ_BC_CONSUMERS
 #define DFQ_BC_CONSUMERS 7
 #endif
@@ -132,7 +131,7 @@ __device__ __forceinline__ void bc_produce(BcRing& ring, unsigned long long n, c
 // Consumers of this ring own different stages in turn (the stage count is not a multiple of the consumer count), so the warp
 // that is about to wait for use u of stage s may get there while use u-1 of that stage - another warp's item, issued 11 items
 // earlier - is still LOADING: the barrier is then in phase u-1, its parity differs from u's, and try_wait returns "done" at
-// once.  The warp would process the previous tile's stage a second time and arrive on `empty` a second time (round 2: "Warp
+// once.  The warp would process the previous tile's stage a second time and arrive on `empty` a second time ("Warp
 // Illegal Instruction" at the producer's next arrive, hangs, on stacks of 16-96 blocks whose loads start cold; steady-state
 // runs of 1000+ blocks never hit it).  The producer therefore stamps every item with its sequence number before it arrives,
 // and the consumer re-checks the stamp after every wait (and waits once more after it matched: the stamp is written before

@@ -413,7 +413,7 @@ __device__ __forceinline__ void cle_row_smem(const RowCtx& c, const DfqCleParams
 
 // A SHORT row (<= 64 float4 / scalar items) handled by G = 1..16 lanes, 32 / G rows per warp side by side: the depthwise
 // 3x3 rows of a MobileNetV2 are 9 floats and its 1x1 expansion rows 24-160 - a whole warp per row left 23-31 lanes idle and
-// a warp walked through up to 73 rows of a tile one after the other (6-7 us per 18 KB tile; the step's critical path).
+// a warp walked through up to 73 rows of a tile one after the other (the step's critical path).
 // Same arithmetic per element and the same (exact) min / max as cle_row_smem; every lane of the warp executes the
 // shuffles, lanes of a group without a row (`valid` false) only skip the memory accesses.
 #ifndef DFQ_SUB_ITEMS
@@ -650,7 +650,7 @@ struct PassIter {
   int q_live;   // last task whose group was checked and found still iterating (one uncached read per layer, not per tile)
   int g_seen, g_done;   // ... and per run of layers of the same group, not per layer
   // shape of the layer in hand, fetched once per layer: fill() runs in the single producer lane for EVERY tile, and a 64-byte
-  // descriptor load from global memory there (~0.4 us of L2 latency) was what k_cle_stack waited for (round 2)
+  // descriptor load from global memory there (an L2 latency) was what k_cle_stack waited for
   int f_q; int f_li, f_rows, f_row_len; long long f_w_off;
   __device__ __forceinline__ void settle() {
     while (cur.valid()) {
@@ -823,8 +823,8 @@ __device__ __noinline__ void ws_produce(float* arena, const DfqLayer* L, const D
 // point).  A layer's weights are only ever written in its own step, by the CTA that owns the tile (the tile -> CTA map is
 // static), so these loads need nothing from the barrier; what does depend on it - 1/s of the in-relation, the column
 // extrema - is read by the consumers behind it.  The mailbox of such a tile stays invalid: the consumers fetch and publish
-// the row themselves.  On a MobileNetV2 the first tile used to arrive 2.3-2.6 us after the barrier (iterator start + L2 ->
-// shared memory), of ~12 us per step.  Returns the number of tiles issued (sequence numbers count .. count + a - 1).
+// the row themselves.  On a MobileNetV2 the first tile used to arrive a large part of a step after the barrier (iterator
+// start + L2 -> shared memory).  Returns the number of tiles issued (sequence numbers count .. count + a - 1).
 __device__ __noinline__ int ws_issue_ahead(float* arena, PassIter& pit, WsPipe& ws, unsigned long long count) {
   const int lane = threadIdx.x & 31;
   int a = 0;
@@ -1215,8 +1215,7 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
 //
 // k_cle_engine keeps one tile per consumer TEAM: every first-layer row pays a CTA-wide reduction barrier and its
 // bookkeeping goes through the producer warp's mailbox; with 3 stages per CTA only ~one 18 KB load per CTA is in flight
-// while a tile is consumed and another one stored (round 1: 26 % of the warp samples wait for data, first-layer pass
-// 5.2 TB/s, second-layer pass 5.8 TB/s, the fold on the plain pipe 6.3 TB/s).  Here, like k_bc_stream:
+// while a tile is consumed and another one stored (the warps of the plain pipe waited for data).  Here, like k_bc_stream:
 //   * one CTA per SM, kStackConsumers consumer WARPS + a producer warp, 11 stages; a warp owns whole tiles: no CTA barrier per tile;
 //   * first-layer rows: two passes over the row in shared memory (min/max, then rescale in place) by the warp alone, the
 //     per-channel bookkeeping of dfq.py:62-70 (publish_row) done lane-parallel - lane r retires row r - instead of by one
@@ -1383,7 +1382,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           // the rescaled tile: generic-proxy writes -> visible to the bulk store, issued by this warp
           fence_proxy_async_smem();
           __syncwarp();
-          // ... and the stage goes back to the producer as soon as the store has READ it (~0.1 us for 18 KB; the store itself
+          // ... and the stage goes back to the producer as soon as the store has READ it (the store itself
           // completes in the background).  Holding it until the next tile instead (tried first) left every consumer with two
           // stages and the ring with almost nothing loading.
           if (lane == 0) {

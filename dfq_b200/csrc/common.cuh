@@ -1,4 +1,4 @@
-// Shared device/host helpers for libdfq_sm100.so (sm_100a only).
+// Shared device/host helpers for libdfq_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,8 +47,8 @@ int sm_count();
 // All descriptor tables of one call are packed into a MAPPED page-locked staging slot (ring of 4, reused after the copy
 // that read it has completed) and moved into ONE stream-ordered device allocation by a small KERNEL that reads the slot over
 // PCIe - not by cudaMemcpyAsync: a copy of a few KB queues on the H2D copy engine behind whatever bulk copy is running, and
-// in the pipelined host-streaming use (300 MB chunks each way) every launch's tables waited ~6 ms for the NEXT chunk's
-// upload to finish, which in turn kept the host from enqueueing the chunk after that (bench.py e2e: 41.7 of 47 GB/s).
+// in the pipelined host-streaming use (300 MB chunks each way) every launch's tables waited for the NEXT chunk's
+// upload to finish, which in turn kept the host from enqueueing the chunk after that.
 // DFQ_TABLES_COPY_ENGINE=1 restores the memcpy path.
 struct TablePack {
   struct Item { const void* src; size_t bytes; size_t off; };
@@ -166,7 +166,7 @@ __device__ __forceinline__ TileSpan tile_span(const long long* __restrict__ ptr,
 
 // Block-cyclic walk over the tiles [first, end) of a phase: CTA b visits blocks j*G + b (j = 0, 1, ...) of kTileBlock
 // consecutive tiles.  Compared with one contiguous span per CTA this keeps the set of pages all CTAs touch at any time
-// within G*kTileBlock tiles (TLB reach; measured: the contiguous split loses 30 % at a 39 GB arena), while a CTA still
+// within G*kTileBlock tiles (TLB reach: the contiguous split was slower on a multi-GB arena), while a CTA still
 // stays on one layer for kTileBlock tiles.
 #ifndef DFQ_TILE_BLOCK
 #define DFQ_TILE_BLOCK 64
@@ -219,7 +219,7 @@ struct QuantScalars {
   float min_v;     // fp32(min_value)        operand of the final add_(min_value)
   float scale;     // fp32(scale)            operand of div_/mul_
   float inv_scale; // fp32(1.0 / double scale): reciprocal-multiply mode.  PyTorch CUDA eager computes x.div_(python_float)
-                   // as x * float(1.0 / scale) with the reciprocal formed in DOUBLE from the Python scalar [probed on B200
+                   // as x * float(1.0 / scale) with the reciprocal formed in DOUBLE from the Python scalar [probed on the GPU
                    // with torch 2.11: 0 mismatches in 4M elements for five scales; float(1.0f / float(scale)) mismatches]
   float qmin, qmax;
 };

@@ -1,12 +1,12 @@
 // Host side of the residency: gather a model's scattered parameter tensors into the page-locked staging image that one
 // H2D copy moves (and scatter the results back after the one D2H copy).  A whole MobileNetV2 is ~310 tensors / 14 MB; one
-// tensor-library copy call per tensor (or one batched call that still dispatches per tensor) costs 1.6-2.0 ms each way on the
-// GPU box - several times the PCIe transfer itself (0.35 ms).  No CUDA call in here.
+// tensor-library copy call per tensor (or one batched call that still dispatches per tensor) costs several times the PCIe
+// transfer itself.  No CUDA call in here.
 //
 // The caller's thread does the work in 256 KB chunks; a small pool of helper threads, parked on a condition variable,
-// takes chunks too WHEN the scheduler runs them in time.  Measured inside bench.py (right after a tensor-library parallel
-// region whose OpenMP workers were still spinning), freshly spawned-and-joined threads made the gather 3x SLOWER than one
-// thread about half of the time; with chunk stealing a late helper simply finds nothing left, and nobody waits for it.
+// takes chunks too WHEN the scheduler runs them in time.  Right after a tensor-library parallel region whose OpenMP
+// workers are still spinning, freshly spawned-and-joined threads can make the gather several times SLOWER than one
+// thread; with chunk stealing a late helper simply finds nothing left, and nobody waits for it.
 #include <algorithm>
 #include <condition_variable>
 #include <cstring>

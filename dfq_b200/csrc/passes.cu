@@ -640,7 +640,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         // (Tried: copying a [512,3,3] row to registers - 144 per lane, 224 registers per thread - and handing the stage back
         // BEFORE the arithmetic, so that the whole ring is loading.  The straight-line code that needs (16 columns x 9 taps
         // fully unrolled, ~1900 instructions, every warp at a different place in it) misses the instruction cache like the very
-        // first version of this kernel did: 1.31 ms instead of 1.14 ms at 1024 pairs.  The rolled shared-memory loop stays.)
+        // first version of this kernel did, and was slower.  The rolled shared-memory loop stays.)
         for (int r = 0; r < d.nrows; ++r) {
           const int g = (d.row0 + r) / so;
           const float* ex = arena + b.expect_off + (size_t)g * l.cols;
@@ -767,7 +767,7 @@ extern "C" int dfq_quantize_tensors(float* arena, int64_t arena_floats, const Df
   const int iT = tp.add(ft.data(), n_tasks), iP = tp.add(tptr.data(), n_tasks + 1);
   if ((rc = tp.upload(st))) return rc;
   FlatTask* dT = tp.ptr<FlatTask>(iT); long long* dP = tp.ptr<long long>(iP);
-  k_minmax_init<<<std::min(148, (n_tasks + 255) / 256), 256, 0, st>>>(arena, dT, n_tasks);
+  k_minmax_init<<<std::min(std::max(1, sm_count()), (n_tasks + 255) / 256), 256, 0, st>>>(arena, dT, n_tasks);
   k_minmax_tasks<<<grid, kThreads, 0, st>>>(arena, dT, n_tasks, dP);
   if (div_mode) k_quant_tasks<true><<<grid, kThreads, 0, st>>>(arena, dT, n_tasks, dP);
   else          k_quant_tasks<false><<<grid, kThreads, 0, st>>>(arena, dT, n_tasks, dP);
@@ -858,7 +858,7 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
 extern "C" int dfq_selftest_bc_arithmetic(const float* w, float* eps_fast, float* eps_div, int64_t n, const float* minmax2,
                                           int num_bits, int symmetric, int* ok_dev, void* stream) {
   DFQ_REQUIRE(w && eps_fast && eps_div && minmax2 && ok_dev && n > 0, "bad argument");
-  k_bc_selftest<<<(int)std::min<int64_t>(148 * 8, (n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, eps_fast, eps_div, n, minmax2,
+  k_bc_selftest<<<(int)std::min<int64_t>((int64_t)std::max(1, sm_count()) * 8, (n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(w, eps_fast, eps_div, n, minmax2,
                                                                                                    num_bits, symmetric, ok_dev);
   DFQ_CUDA(cudaGetLastError());
   return 0;

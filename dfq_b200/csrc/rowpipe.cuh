@@ -180,7 +180,7 @@ struct RowPipe {
 
 // Walks this CTA's tiles (block-cyclic, TileCursor) over a list of matrices.  Geo(q, base, rows, row_len) describes task q.
 // CACHE: keep the geometry of the task in hand in the iterator (the streaming kernels' single producer lane; costs four
-// registers per iterator, which the 80-register RowPipe kernels do not have: k_bn_fold 12.5 -> 13.4 ms with it).
+// registers per iterator, which the 80-register RowPipe kernels do not have: k_bn_fold ran slower with it).
 template <typename Geo, bool CACHE = false>
 struct MatIter {
   const long long* ptr;
@@ -188,7 +188,7 @@ struct MatIter {
   TileCursor cur;
   Geo geo;
   // geometry of task `gq`, fetched once per task: geo() chases two dependent global loads (task -> layer -> shape), and the
-  // single producer lane of a streaming kernel would otherwise pay that latency (~0.6 us) for EVERY tile it issues
+  // single producer lane of a streaming kernel would otherwise pay that latency for EVERY tile it issues
   int gq;
   float* g_base; int g_rows, g_row_len;
   __device__ __forceinline__ void start(const long long* p, int q_begin, int q_end_, Geo g) {

@@ -617,8 +617,8 @@ extern "C" int dfq_range_cols(const float* w, int64_t O, int64_t J, int64_t kk, 
   cudaStream_t st = (cudaStream_t)stream;
   DFQ_REQUIRE(w && out_min && out_max && O > 0 && J > 0 && kk > 0 && groups > 0 && O % groups == 0, "bad argument");
   const int64_t C = groups * J;
-  k_fill<<<(int)std::min<int64_t>(148, (C + 255) / 256), 256, 0, st>>>(out_min, C, INFINITY);
-  k_fill<<<(int)std::min<int64_t>(148, (C + 255) / 256), 256, 0, st>>>(out_max, C, -INFINITY);
+  k_fill<<<(int)std::min<int64_t>(std::max(1, sm_count()), (C + 255) / 256), 256, 0, st>>>(out_min, C, INFINITY);
+  k_fill<<<(int)std::min<int64_t>(std::max(1, sm_count()), (C + 255) / 256), 256, 0, st>>>(out_max, C, -INFINITY);
   const int64_t nt = groups * ((O / groups + 31) / 32);
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(nt, (int64_t)std::max(1, sm_count()) * 8));
   k_range_cols<<<grid, kThreads, 0, st>>>(w, O, J, kk, groups, out_min, out_max);

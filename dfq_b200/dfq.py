@@ -10,7 +10,7 @@ Same public names, signatures, prints and in-place semantics as jakc4103/DFQ ``d
     bias_correction            dfq.py:173-293
 
 Host code walks the graph and builds descriptor tables; every tensor operation runs in
-libdfq_sm100.so (include/dfq_b200.h).  Parameters may live on the CPU (as in main_cls.py, where
+libdfq_sm90.so (include/dfq_b200.h).  Parameters may live on the CPU (as in main_cls.py, where
 calibration happens before ``model.cuda()``) or on the GPU: they are staged into a device arena, the
 kernels run there, and the results are written back into the SAME parameter storages.
 """

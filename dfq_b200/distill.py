@@ -4,7 +4,7 @@ The step immediately BEFORE the ``--distill_range`` path (main_cls.py:97-98, mai
 batches of synthetic images are optimised (Adam on the pixels, 1000 iterations, ReduceLROnPlateau, early break) until the
 statistics of every BatchNorm INPUT match that layer's running mean / standard deviation (distill_data.py:75-227).
 
-Same signature, same algorithm and same random-number consumption as the reference; what is B200-native:
+Same signature, same algorithm and same random-number consumption as the reference; what is GPU-native:
 
 * the statistics-matching loss of every BatchNorm layer - per-(sample, channel) mean and unbiased std over H*W, two squared
   distances - is ONE fused forward kernel and ONE fused backward kernel (dfq_bnstat_loss_fwd / _bwd, csrc/distill.cu) instead

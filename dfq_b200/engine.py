@@ -2,7 +2,7 @@
 
 A :class:`Session` owns one fp32 device *arena* holding every weight, bias and per-channel vector of
 the layers being calibrated, plus the scratch the kernels need.  Host logic (graph walks, which layer
-pairs with which) produces small descriptor tables; all arithmetic happens in libdfq_sm100.so.
+pairs with which) produces small descriptor tables; all arithmetic happens in libdfq_sm90.so.
 
 The session is the object behind the drop-in functions of :mod:`dfq_b200.dfq` and
 :mod:`dfq_b200.utils.layer_transform`; it can also be driven directly (bench.py, tests) with tensors
@@ -23,9 +23,8 @@ from ._lib import DfqError
 
 # threads of the host gather/scatter (dfq_host_copy_segments); 0 = the library's default
 _HOST_COPY_THREADS = int(os.environ.get("DFQ_HOST_COPY_THREADS", "0"))
-# parts the upload of a model is cut into (gather of part i+1 overlaps the H2D copy of part i).  Measured on MobileNetV2
-# inside bench.py: 1 part 1.5 ms, 2 parts 1.4 ms, 4 parts 2.1 ms of upload() - the H2D copy (0.35 ms) is not worth hiding
-# behind extra library calls, so one part is the default.
+# parts the upload of a model is cut into (gather of part i+1 overlaps the H2D copy of part i).  The H2D copy of a
+# MobileNetV2 is short next to a library call, not worth hiding behind extra calls, so one part is the default.
 _UPLOAD_PARTS = int(os.environ.get("DFQ_UPLOAD_PARTS", "1"))
 
 
@@ -198,7 +197,7 @@ class Session:
 
     def _host_copy(self, x: dict, which: str, direction: int, i0: int = 0, i1: Optional[int] = None) -> bool:
         """Gather (0) / scatter (1) between the bound host tensors [i0, i1) and the staging image with the library's
-        memcpy loop (dfq_host_copy_segments; ~0.6-1.4 ms for a MobileNetV2 instead of 1.6-2.0 ms of per-tensor copy
+        memcpy loop (dfq_host_copy_segments; faster for a MobileNetV2 than the per-tensor copy
         dispatch).  The addresses are read per call (a caller may have re-pointed a parameter's .data); returns False -
         the caller then takes the tensor-library path - when a tensor is not a contiguous fp32 host tensor of the bound size."""
         fn = getattr(self.lib, "dfq_host_copy_segments", None)

@@ -2,7 +2,7 @@
 
 Same public names, constructor signatures and call semantics (UniformQuantize, quantize, QuantMeasure,
 QConv2d, QuantConv2d, QuantNConv2d, QLinear, QuantLinear, QuantNLinear, set_layer_bits); the tensor
-arithmetic runs in libdfq_sm100.so:
+arithmetic runs in libdfq_sm90.so:
 
   utils/quantize.py:23-76    UniformQuantize.forward -> dfq_quant_dequant / dfq_quant_dequant_dev
   utils/quantize.py:102-119  QuantMeasure.forward    -> dfq_observe_quant: statistic + running update + quantization in
@@ -13,7 +13,7 @@ arithmetic runs in libdfq_sm100.so:
 Numerics (SURVEY.md H1).  The reference runs the same Python on CPU tensors (weights during
 calibration) and on CUDA tensors (activations, per-forward weights during inference), and PyTorch's two
 backends differ in ONE op: ``div_(python_float)`` is a true division on CPU and, on CUDA, a multiply by
-``fp32(1.0 / scale)`` - the reciprocal formed in DOUBLE from the Python scalar, then rounded (probed on B200).  ``quantize`` follows the device of its input: CPU tensors are staged through the GPU
+``fp32(1.0 / scale)`` - the reciprocal formed in DOUBLE from the Python scalar, then rounded (probed on the GPU).  ``quantize`` follows the device of its input: CPU tensors are staged through the GPU
 and computed with true division (bit-identical to the reference's CPU result), CUDA tensors use the
 reciprocal form (bit-identical to the reference's CUDA result).  There is no CPU implementation.
 """

@@ -1,5 +1,5 @@
 /*
- * dfq_b200.h  -  C ABI of libdfq_sm100.so: the B200 (sm_100a) implementation of the data-free
+ * dfq_b200.h  -  C ABI of libdfq_sm90.so: the H100 (sm_90a) implementation of the data-free
  * quantization calibration hot path of jakc4103/DFQ.
  *
  * The reference is pure Python on PyTorch-eager CPU tensors and has NO foreign-function interface
@@ -222,7 +222,7 @@ int dfq_minmax(const float* x, int64_t n, float* out2, void* stream);
  *   t = rint(t) [-> codes, if non-null];  y = t * fp32(scale);  y = y + min_value.
  * Four separately rounded fp32 ops, no FMA contraction.  div_mode 0 = IEEE division (PyTorch CPU), 1 = multiply by
  * the reciprocal formed in double and rounded to fp32 - what PyTorch CUDA eager computes for `div_(python_float)`
- * [probed on B200, torch 2.11].  y may alias x. */
+ * [probed with torch 2.11].  y may alias x. */
 int dfq_quant_dequant(const float* x, float* y, int64_t n, float min_value, double scale,
                       float qmin, float qmax, int div_mode, float* codes, void* stream);
 

@@ -1,8 +1,8 @@
 """CPU oracle for the DFQ calibration hot path  --  TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
 Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline / ``--impl reference``
-leg may import this module.  The product package ``dfq_b200`` never does: it runs the sm_100a CUDA
-kernels behind ``libdfq_sm100.so`` and raises when that library is missing.
+leg may import this module.  The product package ``dfq_b200`` never does: it runs the sm_90a CUDA
+kernels behind ``libdfq_sm90.so`` and raises when that library is missing.
 
 What it is: a numpy (IEEE fp32, explicit op order) restatement of the arithmetic of the reference
 jakc4103/DFQ (commit 6f15805c) for the path SURVEY.md section 8 names.  Each function cites the
@@ -67,7 +67,7 @@ def quantize(x: np.ndarray, num_bits: int = 8, min_value: Optional[float] = None
 
     div_mode "div"   : true IEEE division  (PyTorch CPU, ``div_(python_float)``)
     div_mode "recip" : ``t * fp32(1.0 / scale)`` with the reciprocal formed in double from the Python scalar - what PyTorch
-                       CUDA eager computes for ``div_(python_float)`` [probed on B200 with torch 2.11]
+                       CUDA eager computes for ``div_(python_float)`` [probed with torch 2.11]
     """
     x = np.ascontiguousarray(x, dtype=f32)
     if min_value is None:

@@ -1,4 +1,4 @@
-"""A stand-in for libdfq_sm100.so that EXECUTES THE SAME DESCRIPTOR TABLES WITH THE NUMPY ORACLE on host memory.
+"""A stand-in for libdfq_sm90.so that EXECUTES THE SAME DESCRIPTOR TABLES WITH THE NUMPY ORACLE on host memory.
 
 Test infrastructure only (it lives under tests/ and imports oracle/).  It lets the `-m "not gpu"` suite drive
 the product's host logic - graph walks, arena planning, descriptor construction, write-back - end to end on a

@@ -6,7 +6,7 @@
     python tests/main_harness.py --impl reference --out tests/golden/main_cls.npz cls --quantize --relu --equalize --correction
 
 --impl dropin      tools/run_main.py exactly as a user would start it: `dropin/` shadows the reference's dfq / utils.* /
-                   improve_dfq modules with dfq_b200.  With a CUDA device the real libdfq_sm100.so runs; without one the
+                   improve_dfq modules with dfq_b200.  With a CUDA device the real libdfq_sm90.so runs; without one the
                    oracle-backed executor of tests/fakelib.py stands in for the library (test infrastructure).
 --impl reference   the same script on the reference's own modules (fixture generation, build container only).
 

@@ -2,10 +2,10 @@
 --equalize` on the bundled MobileNetV2 checkpoint, written by convert_ncnn.py:178-201) - reproduced through THIS package's
 entry points: merge_batchnorm, create_relation, signed cross_layer_equalization, set_quant_minmax, export.ncnn_scales.
 
-Shared by the CPU test (oracle-backed executor, tests/test_host_logic.py) and the -m gpu test (libdfq_sm100.so,
+Shared by the CPU test (oracle-backed executor, tests/test_host_logic.py) and the -m gpu test (libdfq_sm90.so,
 tests/test_gpu_pipeline.py).  Data: the 53 + 53 expected rows are committed (tests/golden/ncnn_table_rows.npz, extracted
-from the reference's table by tools/make_golden.py); the checkpoint (14 MB) is DATA of the reference, copied by
-`__graft_entry__.build()` into the git-ignored oracle/_ref/ so that it travels to the GPU box with the snapshot.
+from the reference's table by tools/make_golden.py); the checkpoint (14 MB) is DATA of the reference, staged by
+`__graft_entry__.build()` (oracle/ref_data.py) into the git-ignored oracle/_ref/ where a reference checkout is readable.
 """
 import os
 
@@ -21,11 +21,8 @@ CKPT_NAME = "mobilenetv2_1.0-f2a8633.pth.tar"
 
 
 def checkpoint_path():
-    for p in (os.path.join(os.path.dirname(HERE), "oracle", "_ref", CKPT_NAME),
-              os.path.join(os.environ.get("DFQ_REFERENCE_ROOT", "/root/reference"), "modeling", "classification", CKPT_NAME)):
-        if os.path.isfile(p):
-            return p
-    return None
+    p = os.path.join(os.path.dirname(HERE), "oracle", "_ref", CKPT_NAME)
+    return p if os.path.isfile(p) else None
 
 
 def run(monkeypatch):

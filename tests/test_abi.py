@@ -20,7 +20,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     names = _declared_functions()
     assert len(names) >= 18
     for n in names:
-        assert hasattr(lib, n), "libdfq_sm100.so does not export %s" % n
+        assert hasattr(lib, n), "libdfq_sm90.so does not export %s" % n
     # and the binding covers every declared function (dfq_last_error is bound separately)
     for n in names:
         assert n in _lib.SIGNATURES or n == "dfq_last_error", "dfq_b200/_lib.py has no signature for %s" % n

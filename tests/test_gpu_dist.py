@@ -7,7 +7,7 @@ the owners' equalized tensors), then sharded bias correction.  Every rank must e
 on the same GPU: S, weights bit for bit, biases / fake_bias within 1e-5.  (With replicas="replay" the weights of non-owned
 chains are within ~3e-6 and - bias correction being ill-conditioned in the last bit of the weights, DESIGN.md section 4 - the
 biases only within 5e-2: the second test.)
-The NCCL flavour of the same check (one process per GPU) is tools/dist_check.py, profiles/r2_dist_check.txt."""
+The NCCL flavour of the same check (one process per GPU) is tools/dist_check.py."""
 import os
 import sys
 

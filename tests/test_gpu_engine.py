@@ -1,4 +1,4 @@
-"""-m gpu parity tests of the arena engine (libdfq_sm100.so through dfq_b200.engine.Session) against
+"""-m gpu parity tests of the arena engine (libdfq_sm90.so through dfq_b200.engine.Session) against
 the numpy oracle on seeded inputs.  Equalization, BN fold factors and fake-quant are compared
 bit-exactly; bias correction to 1e-5 normwise (fp32 mat-vec has no defined order in the reference)."""
 import numpy as np

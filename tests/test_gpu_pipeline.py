@@ -351,13 +351,13 @@ def test_resnet18_activation_ranges_over_64_images():
 
 
 def test_golden_ncnn_table_through_the_cuda_library(monkeypatch):
-    """The reference's golden artefact through libdfq_sm100.so: BN fold (dfq_bn_fold), signed equalization to convergence
+    """The reference's golden artefact through libdfq_sm90.so: BN fold (dfq_bn_fold), signed equalization to convergence
     (dfq_cle_run) and the per-tensor extrema of the export (dfq_minmax) run on the GPU on the bundled checkpoint; the 53
     weight-scale rows and 53 activation-scale rows of model_quant_relu_equal.table must come out to 1e-5 (the table was
     written by a host whose sqrt differs from IEEE in the last bit: S is only determined to ~1e-6, DESIGN.md section 4)."""
     import ncnn_table_case as case
     if case.checkpoint_path() is None:
-        pytest.skip("checkpoint not shipped: run __graft_entry__.build() where /root/reference exists")
+        pytest.skip("checkpoint not staged: run __graft_entry__.build() with a readable reference checkout")
     got_w, gold_w, got_a, gold_a = case.run(monkeypatch)
     assert got_w.shape == gold_w.shape == (53,) and got_a.shape == gold_a.shape == (53,)
     ew, ea = np.abs(got_w / gold_w - 1).max(), np.abs(got_a / gold_a - 1).max()
@@ -414,5 +414,5 @@ def export_round_trip(tmp_path, monkeypatch=None):
 
 
 def test_export_round_trip_on_cuda_results(tmp_path):
-    """write_ncnn_table / save_calibration on a model calibrated by libdfq_sm100.so (convert_ncnn.py:178-201 format)."""
+    """write_ncnn_table / save_calibration on a model calibrated by libdfq_sm90.so (convert_ncnn.py:178-201 format)."""
     assert export_round_trip(tmp_path) == 42

@@ -267,10 +267,10 @@ def test_set_quant_minmax_matches_reference_fixture(monkeypatch, name, seed):
 def test_live_ncnn_table_through_the_product_host_path(monkeypatch):
     """The reference's checked-in calibration table reproduced by THIS package's entry points end to end (53 weight-scale
     rows and 53 activation-scale rows; tests/ncnn_table_case.py).  Arithmetic by the oracle-backed executor; the -m gpu twin
-    in tests/test_gpu_pipeline.py runs the same case on libdfq_sm100.so."""
+    in tests/test_gpu_pipeline.py runs the same case on libdfq_sm90.so."""
     import ncnn_table_case as case
     if case.checkpoint_path() is None:
-        pytest.skip("MobileNetV2 checkpoint not present (oracle/_ref or the reference tree)")
+        pytest.skip("MobileNetV2 checkpoint not staged in oracle/_ref")
     fakelib.install(monkeypatch, fakelib.torch_sqrt)
     got_w, gold_w, got_a, gold_a = case.run(monkeypatch)
     assert got_w.shape == gold_w.shape == (53,) and got_a.shape == gold_a.shape == (53,)

@@ -3,13 +3,13 @@ tools/run_main.py's environment (dropin/ ahead of the reference on sys.path) and
 the same model the same scripts produce on the reference's own modules.
 
 How: tests/main_harness.py starts the script in a subprocess (synthetic datasets instead of the hard-coded ImageNet/VOC
-paths; without a GPU the oracle-backed executor stands in for libdfq_sm100.so and is given the host's torch.sqrt, as the
+paths; without a GPU the oracle-backed executor stands in for libdfq_sm90.so and is given the host's torch.sqrt, as the
 fixture's reference run used it) and dumps (a) every Conv/Linear weight digest, bias, BN fake_weight/fake_bias, every
 observer range, (b) how many observers fired during the script's own inference loop (layer inputs and - through
 replace_op() - the patched Tensor.__add__/torch.cat/torch.mean/F.interpolate calls), (c) the model outputs.  The expected
 values (tests/golden/main_<which>.npz) were produced by `main_harness.py --impl reference`, i.e. by the reference.
 
-Needs the reference checkout (skipped where /root/reference is absent, e.g. on the GPU box).
+Needs the reference checkout (skipped where it is absent).
 """
 import ast
 import os

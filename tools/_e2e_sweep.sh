@@ -1,5 +1,5 @@
 #!/bin/bash
-# Development helper (run on the GPU box): the end-to-end arm of bench.py against chunk size (pairs) and arena slots.
+# Development helper (run on a GPU): the end-to-end arm of bench.py against chunk size (pairs) and arena slots.
 #   CFGS="32:4 16:6" bash tools/_e2e_sweep.sh
 for cfg in ${CFGS:-32:4 16:4 16:6 64:4}; do
   c=${cfg%%:*}; s=${cfg##*:}

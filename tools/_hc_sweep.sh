@@ -1,5 +1,5 @@
 #!/bin/bash
-# Development helper (run on the GPU box): MobileNetV2 e2e inside bench.py's process environment (NUMA binding, clock sampler)
+# Development helper (run on a GPU): MobileNetV2 e2e inside bench.py's process environment (NUMA binding, clock sampler)
 # against the host-copy thread count (DFQ_HOST_COPY_THREADS) and the number of upload parts (DFQ_UPLOAD_PARTS).
 #   CFGS="0:1 1:1" bash tools/_hc_sweep.sh
 for cfg in ${CFGS:-0:1 0:1 1:1}; do

@@ -16,7 +16,10 @@ build container.  Committed next to its outputs so every fixture can be regenera
                           every post-correction bias and fake_bias vector + sha256 of every input tensor
   main_<cls|seg|ssd>.npz  made by tests/main_harness.py --impl reference (the unmodified main scripts end to end)
 
-usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax]
+  ref_live_pins.npz       the reference's _layer_equalization, replace_op forward and getDistilData on the inputs of the
+                          pin tests (tests/test_oracle_pins.py, test_op_patching.py, test_distill.py)
+
+usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
 """
 import hashlib
 import json
@@ -315,3 +318,57 @@ def ncnn_table_rows():
 
 if __name__ == "__main__" and "table" in sys.argv[1:]:
     ncnn_table_rows()
+
+
+# ---------------------------------------------------------------------------------------------------------
+def live_pins():
+    """What the pin tests used to compute by importing the reference at test time, stored so that they run anywhere:
+    _layer_equalization on the CASES of tests/test_oracle_pins.py (sha256 of every output tensor), the replace_op forward of
+    tests/test_op_patching.py (outputs and observer order) and getDistilData on tests/test_distill.py's tiny model (a seeded
+    sample of 4096 pixels per batch plus each batch's fp64 sum)."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_oracle_pins as P
+    out = {}
+    for ci, (s1, s2, opt) in enumerate(P.CASES):
+        for signed in (False, True):
+            torch.manual_seed(hash((s1, s2, signed)) % 1000)
+            opt_ = dict(opt)
+            degenerate = opt_.pop("degenerate", False)
+            w1 = torch.randn(*s1) * (10 ** torch.empty(s1[0]).uniform_(-1, 1)).view(-1, *([1] * (len(s1) - 1)))
+            w2 = torch.randn(*s2)
+            if degenerate:
+                w1[1] = 0; w1[3] = 0.5
+                w2.view(s2[0], s2[1], -1)[:, 2] = 0
+            b1, bw, bb = torch.randn(s1[0]), torch.rand(s1[0]) + 0.5, torch.randn(s1[0])
+            key = "eq_%d_%d" % (ci, int(signed))
+            out[key + "_in"] = np.array([P.sha256(t.numpy()) for t in (w1, w2, b1, bw, bb)])
+            r = ref.dfq._layer_equalization(w1, w2, b1, bw, bb, signed=signed, **opt_)
+            out[key + "_out"] = np.array([P.sha256(t.numpy()) for t in (w1, w2, b1, bw, bb, r[3])])
+
+    import test_op_patching as T
+    torch.manual_seed(0)
+    model = T.Net().eval()
+    x = torch.randn(2, 3, 6, 6)
+    theirs, seen, _ = T._run_patched(ref.layer_transform, ref.quantize.QuantMeasure, model, x)
+    out["patch_seen"] = np.array([i for i, _ in seen])
+    for k, t in enumerate(theirs):
+        out["patch_out_%d" % k] = t.numpy()
+
+    import run_main
+    import test_distill as D
+    run_main.prepare_environment(use_dropin=False)
+    from ZeroQ.distill_data import getDistilData as ref_get
+    model = D._tiny()
+    torch.manual_seed(123)
+    theirs = ref_get(model, "imagenet", 2, num_batch=2, gpu=False, value_range=[-2.11790393, 2.64], early_break_factor=1e9)
+    for k, t in enumerate(theirs):
+        a = t.detach().numpy()
+        out["distill_shape_%d" % k] = np.array(a.shape)
+        out["distill_sum_%d" % k] = np.array(a.astype(np.float64).sum())
+        out["distill_sample_%d" % k] = a.reshape(-1)[D.sample_index(a.size)]
+    np.savez_compressed(os.path.join(GOLD, "ref_live_pins.npz"), **out)
+    print("live pins:", len(out), "arrays")
+
+
+if __name__ == "__main__" and "live" in sys.argv[1:]:
+    live_pins()

@@ -1,6 +1,6 @@
-// Microbenchmark: cost of one grid-wide barrier in a cooperative kernel on B200 - cooperative_groups grid.sync() against
+// Microbenchmark: cost of one grid-wide barrier in a cooperative kernel on an H100 - cooperative_groups grid.sync() against
 // hand-written counter barriers (the small-model equalization pays ~7 of them per sweep, 49 sweeps on MobileNetV2).
-// build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/microbench/gridbar tools/microbench/gridbar.cu
+// build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/microbench/gridbar tools/microbench/gridbar.cu
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,11 +1,11 @@
-"""Import helper for the UNMODIFIED reference tree (jakc4103/DFQ) in the build container.
+"""Import helper for the UNMODIFIED reference tree (jakc4103/DFQ), wherever a checkout exists.
 
 Test/fixture infrastructure only.  Nothing in the product package (``dfq_b200``), ``bench.py``,
-``__graft_entry__.smoke()`` or the ``-m gpu`` tests imports this file: the reference tree does not
-exist on the GPU box.  It is used by
+``__graft_entry__.smoke()`` or the ``-m gpu`` tests imports this file: none of them needs the reference
+tree.  It is used by
 
 * ``tools/make_golden.py``  - generates ``tests/golden/*`` by running the reference here, and
-* the ``-m "not gpu"`` pin tests, which are skipped when ``/root/reference`` is absent.
+* ``oracle/ref_data.py`` (``REF_ROOT`` only), which stages the reference's data files for the tests.
 
 The shims are the ones SURVEY.md section 8(b) lists for torch 2.11 / python 3.12: stub the optional
 visualisation deps *after* ``import torch``, alias ``collections.Mapping``.

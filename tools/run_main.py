@@ -5,7 +5,7 @@
 
 `dropin/` is placed ahead of the reference tree on sys.path, so `from dfq import ...`, `from utils.quantize import ...`,
 `from utils.layer_transform import ...`, `from utils.relation import ...` and `from improve_dfq import ...` bind to the
-B200 implementation while models, datasets, the tracer (PyTransformer) and the evaluation code stay the reference's.
+H100 implementation while models, datasets, the tracer (PyTransformer) and the evaluation code stay the reference's.
 Needs the reference checkout (DFQ_REFERENCE_ROOT, default /root/reference), a CUDA device and - for the evaluation the
 scripts run at the end - the datasets at the paths hard-coded in those scripts.
 
