@@ -93,6 +93,27 @@ __device__ __forceinline__ bool exit_rule(double& diff, int& count, double diff_
   return !cont || n >= cap;
 }
 
+// Threads tid of nthreads per CTA stride over the groups.  `diff` = 10 of dfq.py:81 for every group.
+__device__ __forceinline__ void groups_init(GroupState* G, int nG, int tid, int nthreads) {
+  for (int g = blockIdx.x * nthreads + tid; g < nG; g += gridDim.x * nthreads) G[g].diff = 10.0;
+}
+// The exit rule after sweep `sweep` for every group still iterating; ctl->active[n & 1] counts those that go on.
+__device__ __forceinline__ void groups_exit_rule(GroupState* G, int nG, CleCtl* ctl, const DfqCleParams& P, int sweep, int tid,
+                                                 int nthreads) {
+  const int slot = sweep % 3, n = sweep + 1;
+  for (int g = blockIdx.x * nthreads + tid; g < nG; g += gridDim.x * nthreads) {
+    GroupState& st = G[g];
+    if (st.done) continue;
+    const double diff_tmp = st.acc[slot];
+    st.acc[(slot + 2) % 3] = 0.0;   // last read before this sweep's final barrier, next used in sweep+2
+    if (g == 0 && sweep < 64) ctl->diffs[sweep] = diff_tmp;
+    bool converged;
+    if (exit_rule(st.diff, st.count, diff_tmp, P, n, &converged)) { st.n_sweeps = n; st.converged = converged; st.done = 1; }
+    else atomicAdd(&ctl->active[n & 1], 1);
+  }
+  if (blockIdx.x == 0 && tid == 0) ctl->active[sweep & 1] = 0;   // read at the end of the previous sweep
+}
+
 // pass tiles: contiguous chunks of rows moved by the RowPipe (rowpipe.cuh)
 __host__ __device__ inline int pass_tiles(const DfqLayer& l) { return pipe_tiles(l.rows, l.cols * l.kk); }
 // Everything a row pass needs to know about its layer; uniform across the CTA.
@@ -167,9 +188,9 @@ __device__ __forceinline__ void cta_minmax(float& mn, float& mx, float* red, int
 struct StagePub { float cmn, cmx, s, inv; int valid; int pad[3]; };
 
 // The per-channel bookkeeping of dfq.py:62-70 + relation.py:20-24 + the derived column extrema, for ONE channel.
-// All loads are issued before the first store (the stores would otherwise fence the loads one global latency apart).
-// The per-channel operands of publish_row: only the row's own publisher ever writes them, so they may be requested together
-// with the row's inputs, one global-memory latency before they are needed.
+// All loads (fetch_row_pub) are issued before the first store (the stores would otherwise fence the loads one global
+// latency apart).  Only the row's own publisher ever writes these operands, so they may also be requested together with
+// the row's inputs, one global-memory latency before they are needed.
 struct RowPub { float a0, b0, w0, w1, o0, o1; };
 __device__ __forceinline__ RowPub fetch_row_pub(const RowCtx& c, const DfqCleParams P, int o) {
   RowPub q;
@@ -182,8 +203,8 @@ __device__ __forceinline__ RowPub fetch_row_pub(const RowCtx& c, const DfqClePar
   q.o1 = c.own_cmin_wr ? __ldcg(c.own_cmax_wr + o) : 0.f;
   return q;
 }
-__device__ __forceinline__ void publish_row_with(const RowCtx& c, const DfqCleParams P, int o, float s, float inv, float cmn,
-                                                 float cmx, const RowPub& q) {
+__device__ __forceinline__ void publish_row(const RowCtx& c, const DfqCleParams P, int o, float s, float inv, float cmn, float cmx,
+                                            const RowPub& q) {
   c.s_step[o] = s;
   __stcg(c.inv_out + o, inv);
   if (!P.apply_only) c.s_acc[o] = c.first_sweep ? s : __fmul_rn(q.a0, s);
@@ -199,39 +220,23 @@ __device__ __forceinline__ void publish_row_with(const RowCtx& c, const DfqClePa
     __stcg(c.own_cmax_wr + o, __fmul_rn(q.o1, s));
   }
 }
-__device__ __forceinline__ void publish_row(const RowCtx& c, const DfqCleParams P, int o, float s, float inv, float cmn, float cmx) {
-  const bool acc = !P.apply_only && !c.first_sweep;
-  const float a0 = acc ? __ldcg(c.s_acc + o) : 1.f;
-  const float b0 = __ldcg(c.bias + o);
-  const float w0 = c.bnw ? __ldcg(c.bnw + o) : 0.f;
-  const float w1 = c.bnb ? __ldcg(c.bnb + o) : 0.f;
-  const float o0 = c.own_cmin_wr ? __ldcg(c.own_cmin_wr + o) : 0.f;
-  const float o1 = c.own_cmin_wr ? __ldcg(c.own_cmax_wr + o) : 0.f;
-  c.s_step[o] = s;
-  __stcg(c.inv_out + o, inv);
-  if (!P.apply_only) c.s_acc[o] = c.first_sweep ? s : __fmul_rn(a0, s);
-  __stcg(c.bias + o, __fmul_rn(b0, s));
-  if (c.bnw) __stcg(c.bnw + o, __fmul_rn(w0, s));
-  if (c.bnb) __stcg(c.bnb + o, __fmul_rn(w1, s));
-  if (c.cmin_wr) {  // derived column extrema of the second layer after its column scaling
-    __stcg(c.cmin_wr + o, __fmul_rn(cmn, inv));
-    __stcg(c.cmax_wr + o, __fmul_rn(cmx, inv));
-  }
-  if (c.own_cmin_wr) {  // depthwise middle layer: its single-row column is this row
-    __stcg(c.own_cmin_wr + o, __fmul_rn(o0, s));
-    __stcg(c.own_cmax_wr + o, __fmul_rn(o1, s));
-  }
-}
 
 // What a row needs from global memory, fetched ahead of the row by whoever can hide the latency (producer warp for
-// single-row tiles, one lane per row for a warp's batch of rows).
+// single-row tiles, one lane per row for a warp's batch of rows).  Default-constructed: the neutral values.
 struct RowIn {
-  float cmn, cmx;   // column extrema of the second layer for this channel (HAS_OUT)
-  float u;          // the row-uniform input factor (IN_UNIFORM)
-  float s_given;    // apply_only: the scale to replay
+  float cmn = 0.f, cmx = 0.f;   // column extrema of the second layer for this channel (HAS_OUT)
+  float u = 1.f;                // the row-uniform input factor (IN_UNIFORM)
+  float s_given = 1.f;          // apply_only: the scale to replay
 };
+// lane src's RowIn, in every lane of the warp
+__device__ __forceinline__ RowIn shfl_row_in(const RowIn& v, int src) {
+  RowIn r;
+  r.cmn = __shfl_sync(0xffffffffu, v.cmn, src); r.cmx = __shfl_sync(0xffffffffu, v.cmx, src);
+  r.u = __shfl_sync(0xffffffffu, v.u, src); r.s_given = __shfl_sync(0xffffffffu, v.s_given, src);
+  return r;
+}
 __device__ __forceinline__ RowIn fetch_row_in(const RowCtx& c, const DfqCleParams P, int o, bool uniform) {
-  RowIn in; in.cmn = in.cmx = 0.f; in.u = 1.f; in.s_given = 1.f;
+  RowIn in;
   if (c.has_out) {
     in.cmn = __ldcg(c.cmin_rd + o); in.cmx = __ldcg(c.cmax_rd + o);
     if (P.apply_only) in.s_given = __ldcg(c.s_acc + o);
@@ -336,11 +341,7 @@ __device__ __forceinline__ void cle_row_smem(const RowCtx& c, const DfqCleParams
 #pragma unroll
       for (int k = 0; k < kRowRegs; ++k) {
         const int i4 = lane + k * TPR;
-        if (i4 < n4) {
-          const float4 t = in_scale4<MODE>(v[k], i4 * 4, inv, u, kk);
-          mn = fminf(mn, fminf(fminf(t.x, t.y), fminf(t.z, t.w)));
-          mx = fmaxf(mx, fmaxf(fmaxf(t.x, t.y), fmaxf(t.z, t.w)));
-        }
+        if (i4 < n4) minmax4(mn, mx, in_scale4<MODE>(v[k], i4 * 4, inv, u, kk));
       }
       solve(mn, mx);
     }
@@ -349,10 +350,9 @@ __device__ __forceinline__ void cle_row_smem(const RowCtx& c, const DfqCleParams
       const int i4 = lane + k * TPR;
       if (i4 < n4) {
         float4 t = in_scale4<MODE>(v[k], i4 * 4, inv, u, kk);
-        if (HAS_OUT) { t.x = __fmul_rn(t.x, s); t.y = __fmul_rn(t.y, s); t.z = __fmul_rn(t.z, s); t.w = __fmul_rn(t.w, s); }
+        if (HAS_OUT) t = mul4(t, s);
         put4(i4, t);
-        dsum += fabsf(__fsub_rn(t.x, v[k].x)) + fabsf(__fsub_rn(t.y, v[k].y)) + fabsf(__fsub_rn(t.z, v[k].z)) +
-                fabsf(__fsub_rn(t.w, v[k].w));
+        dsum += absdiff4(t, v[k]);
       }
     }
   } else if (vec) {
@@ -360,20 +360,16 @@ __device__ __forceinline__ void cle_row_smem(const RowCtx& c, const DfqCleParams
     if (HAS_OUT) {
       float mn = DFQ_INF, mx = -DFQ_INF;
 #pragma unroll 2
-      for (int i4 = lane; i4 < n4; i4 += TPR) {
-        const float4 t = in_scale4<MODE>(r4[i4], i4 * 4, inv, u, kk);
-        mn = fminf(mn, fminf(fminf(t.x, t.y), fminf(t.z, t.w)));
-        mx = fmaxf(mx, fmaxf(fmaxf(t.x, t.y), fmaxf(t.z, t.w)));
-      }
+      for (int i4 = lane; i4 < n4; i4 += TPR) minmax4(mn, mx, in_scale4<MODE>(r4[i4], i4 * 4, inv, u, kk));
       solve(mn, mx);
     }
 #pragma unroll 2
     for (int i4 = lane; i4 < n4; i4 += TPR) {
       const float4 v = r4[i4];
       float4 t = in_scale4<MODE>(v, i4 * 4, inv, u, kk);
-      if (HAS_OUT) { t.x = __fmul_rn(t.x, s); t.y = __fmul_rn(t.y, s); t.z = __fmul_rn(t.z, s); t.w = __fmul_rn(t.w, s); }
+      if (HAS_OUT) t = mul4(t, s);
       put4(i4, t);
-      dsum += fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
+      dsum += absdiff4(t, v);
     }
   } else {
     if (HAS_OUT) {
@@ -418,11 +414,7 @@ __device__ __forceinline__ void cle_row_sub(const RowCtx& c, const DfqCleParams 
     if (valid) {
       if (vec) {
         const float4* r4 = (const float4*)row;
-        for (int i4 = sub; i4 < n4; i4 += G) {
-          const float4 t = in_scale4<MODE>(r4[i4], i4 * 4, inv, u, kk);
-          mn = fminf(mn, fminf(fminf(t.x, t.y), fminf(t.z, t.w)));
-          mx = fmaxf(mx, fmaxf(fmaxf(t.x, t.y), fmaxf(t.z, t.w)));
-        }
+        for (int i4 = sub; i4 < n4; i4 += G) minmax4(mn, mx, in_scale4<MODE>(r4[i4], i4 * 4, inv, u, kk));
       } else {
         for (int e = sub; e < n; e += G) {
           const float t = in_scale1<MODE>(row[e], e, inv, u, kk);
@@ -444,9 +436,9 @@ __device__ __forceinline__ void cle_row_sub(const RowCtx& c, const DfqCleParams 
       for (int i4 = sub; i4 < n4; i4 += G) {
         const float4 v = r4[i4];
         float4 t = in_scale4<MODE>(v, i4 * 4, inv, u, kk);
-        if (HAS_OUT) { t.x = __fmul_rn(t.x, s); t.y = __fmul_rn(t.y, s); t.z = __fmul_rn(t.z, s); t.w = __fmul_rn(t.w, s); }
+        if (HAS_OUT) t = mul4(t, s);
         r4[i4] = t;
-        dsum += fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
+        dsum += absdiff4(t, v);
       }
     } else {
       for (int e = sub; e < n; e += G) {
@@ -472,7 +464,7 @@ __device__ __forceinline__ void cle_tile_rows(const RowCtx& c, const DfqCleParam
   const int warp = ctid() >> 5, lane = ctid() & 31;
   if (nrows == 1) {
     RowIn in;
-    if (HAS_OUT && pub) { in.cmn = pub->cmn; in.cmx = pub->cmx; in.u = 1.f; in.s_given = 1.f;
+    if (HAS_OUT && pub) { in.cmn = pub->cmn; in.cmx = pub->cmx;
                           if (MODE == IN_UNIFORM) in.u = __ldcg(c.inv_in + (row0 / c.in_go) * c.in_gi);
                           if (P.apply_only) in.s_given = __ldcg(c.s_acc + row0); }
     else in = fetch_row_in(c, P, row0, MODE == IN_UNIFORM);
@@ -480,7 +472,7 @@ __device__ __forceinline__ void cle_tile_rows(const RowCtx& c, const DfqCleParam
     cle_row_smem<kThreads, MODE, HAS_OUT>(c, P, buf, row0, ctid(), s_inv, red, parity, dacc, in, &sv, &iv);
     if (HAS_OUT && ctid() == 0) {
       if (pub) { pub->s = sv; pub->inv = iv; }
-      else publish_row(c, P, row0, sv, iv, in.cmn, in.cmx);
+      else publish_row(c, P, row0, sv, iv, in.cmn, in.cmx, fetch_row_pub(c, P, row0));
     }
   } else {
     const int row_len = c.row_len;
@@ -492,8 +484,8 @@ __device__ __forceinline__ void cle_tile_rows(const RowCtx& c, const DfqCleParam
     for (int base = 0; base < mine; base += 32) {
       const int il = base + lane;
       const int ol = row0 + warp + il * kWarps;
-      RowIn mine_in; mine_in.cmn = mine_in.cmx = 0.f; mine_in.u = 1.f; mine_in.s_given = 1.f;
-      RowPub mine_pub; mine_pub.a0 = mine_pub.b0 = mine_pub.w0 = mine_pub.w1 = mine_pub.o0 = mine_pub.o1 = 0.f;
+      RowIn mine_in;
+      RowPub mine_pub{};
       if (il < mine) {
         mine_in = fetch_row_in(c, P, ol, MODE == IN_UNIFORM);
         if (HAS_OUT) mine_pub = fetch_row_pub(c, P, ol);          // in flight together with the inputs
@@ -506,9 +498,7 @@ __device__ __forceinline__ void cle_tile_rows(const RowCtx& c, const DfqCleParam
           const bool valid = (j + grp < nb);
           const int jj = valid ? j + grp : nb - 1;                 // lanes without a row shadow the last one (no stores)
           const int r = warp + (base + jj) * kWarps;
-          RowIn in;
-          in.cmn = __shfl_sync(0xffffffffu, mine_in.cmn, jj); in.cmx = __shfl_sync(0xffffffffu, mine_in.cmx, jj);
-          in.u = __shfl_sync(0xffffffffu, mine_in.u, jj); in.s_given = __shfl_sync(0xffffffffu, mine_in.s_given, jj);
+          const RowIn in = shfl_row_in(mine_in, jj);
           float sv = 1.f, iv = 1.f;
           cle_row_sub<MODE, HAS_OUT>(c, P, buf + (size_t)r * row_len, row0 + r, sub, G, valid, vec, s_inv, dacc, in, &sv, &iv);
           // row j + g was solved by lane group g: its publisher is lane j + g
@@ -519,14 +509,12 @@ __device__ __forceinline__ void cle_tile_rows(const RowCtx& c, const DfqCleParam
       } else
       for (int j = 0; j < nb; ++j) {
         const int r = warp + (base + j) * kWarps;
-        RowIn in;
-        in.cmn = __shfl_sync(0xffffffffu, mine_in.cmn, j); in.cmx = __shfl_sync(0xffffffffu, mine_in.cmx, j);
-        in.u = __shfl_sync(0xffffffffu, mine_in.u, j); in.s_given = __shfl_sync(0xffffffffu, mine_in.s_given, j);
+        const RowIn in = shfl_row_in(mine_in, j);
         float sv = 1.f, iv = 1.f;
         cle_row_smem<32, MODE, HAS_OUT>(c, P, buf + (size_t)r * row_len, row0 + r, lane, s_inv, red, parity, dacc, in, &sv, &iv);
         if (lane == j) { ks = sv; kinv = iv; }
       }
-      if (HAS_OUT && il < mine) publish_row_with(c, P, ol, ks, kinv, mine_in.cmn, mine_in.cmx, mine_pub);
+      if (HAS_OUT && il < mine) publish_row(c, P, ol, ks, kinv, mine_in.cmn, mine_in.cmx, mine_pub);
     }
   }
 }
@@ -563,7 +551,7 @@ __device__ __noinline__ void cle_row_generic(const RowCtx& c, const DfqCleParams
     RowIn in = fetch_row_in(c, P, o, false);
     float iv;
     s = solve_row(P, in, mn, mx, &iv);
-    if (ctid() == 0) publish_row(c, P, o, s, iv, in.cmn, in.cmx);
+    if (ctid() == 0) publish_row(c, P, o, s, iv, in.cmn, in.cmx, fetch_row_pub(c, P, o));
   }
   float dsum = 0.f;
   for (int e = ctid(); e < c.row_len; e += kThreads) {
@@ -687,6 +675,10 @@ struct PassIter {
 // The consumers never wait for global-memory latency of the small vectors nor for the TMA bookkeeping, and the producer is
 // off their critical path: ONE consumer barrier per tile (the block reduction).
 // ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+
 struct WsPipe {
   unsigned char* base;   // everything is derived from it: no pointer arrays (a runtime-indexed array would live in local memory)
   __device__ __forceinline__ float* stage(int i) const { return (float*)(base + (size_t)i * kStageBytes); }
@@ -707,12 +699,25 @@ struct WsPipe {
   __host__ __device__ static constexpr size_t smem_bytes() {
     return (size_t)kCleStages * kStageBytes + 256 + kCleStages * (sizeof(TileDesc) + sizeof(StagePub)) + 64;
   }
+  // Producer warp: tile d goes into stage si.  Lane 0 writes the descriptor and starts the bulk load (TK_BULK) first; lane 2
+  // then writes the stage mailbox, invalid unless mail(pb) fills it in.  The caller then arrives on full(si).
+  template <typename Mail>
+  __device__ __forceinline__ void issue(int si, const TileDesc& d, int lane, Mail mail) const {
+    if (lane == 0) {
+      *desc(si) = d;
+      if (d.kind == TK_BULK) {
+        mbar_expect_tx(full(si), (uint32_t)d.floats * 4u);
+        bulk_g2s(stage(si), d.gptr, (uint32_t)d.floats * 4u, full(si));
+      }
+    }
+    if (lane == 2) {
+      StagePub pb; pb.valid = 0; pb.cmn = pb.cmx = pb.s = pb.inv = 0.f;
+      mail(pb);
+      *pub(si) = pb;
+    }
+  }
 };
 static_assert(kCleStages <= 16, "barrier arrays are 128 bytes");
-
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.expect_tx.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 
 // Producer WARP: issue / retire the tiles of one step.  `count` = tiles this CTA has moved since kernel start.
 // One iteration retires tile m (the consumers no longer need its stage) and issues tile m + kCleStages into that stage;
@@ -761,7 +766,7 @@ __device__ __noinline__ void ws_produce(float* arena, const DfqLayer* L, const D
         }
         if (lane == 1 && pb.valid) {
           if (d.task != li) { make_ctx(ctx, arena, L, R, d.task, sweep); li = d.task; }
-          publish_row(ctx, P, d.row0, pb.s, pb.inv, pb.cmn, pb.cmx);
+          publish_row(ctx, P, d.row0, pb.s, pb.inv, pb.cmn, pb.cmx, fetch_row_pub(ctx, P, d.row0));
         }
       }
       m++;
@@ -771,21 +776,12 @@ __device__ __noinline__ void ws_produce(float* arena, const DfqLayer* L, const D
       if (pit.valid()) { pit.fill(d, arena); pit.next(); }
       else { d.gptr = nullptr; d.task = -1; d.row0 = d.floats = d.nrows = 0; d.kind = TK_END; --end_pending; }
       const int si = (int)(n % kCleStages);
-      if (lane == 0) {
-        *ws.desc(si) = d;
-        if (d.kind == TK_BULK) {
-          mbar_expect_tx(ws.full(si), (uint32_t)d.floats * 4u);
-          bulk_g2s(ws.stage(si), d.gptr, (uint32_t)d.floats * 4u, ws.full(si));
-        }
-      }
-      if (lane == 2) {
-        StagePub pb; pb.valid = 0; pb.cmn = pb.cmx = pb.s = pb.inv = 0.f;
+      ws.issue(si, d, lane, [&](StagePub& pb) {
         if (!scan && d.nrows == 1 && (d.kind == TK_BULK || d.kind == TK_PLAIN)) {
           if (d.task != li) { make_ctx(ctx, arena, L, R, d.task, sweep); li = d.task; }
           if (ctx.has_out) { pb.cmn = __ldcg(ctx.cmin_rd + d.row0); pb.cmx = __ldcg(ctx.cmax_rd + d.row0); pb.valid = 1; }
         }
-        *ws.pub(si) = pb;
-      }
+      });
       __syncwarp();
       if (lane == 0) mbar_arrive(ws.full(si));   // phase completes when this arrival AND the bulk bytes have landed
       n++;
@@ -810,22 +806,20 @@ __device__ __noinline__ int ws_issue_ahead(float* arena, PassIter& pit, WsPipe& 
     pit.fill(d, arena);
     pit.next();
     const int si = (int)((count + (unsigned long long)a) % kCleStages);
-    if (lane == 0) {
-      *ws.desc(si) = d;
-      if (d.kind == TK_BULK) {
-        mbar_expect_tx(ws.full(si), (uint32_t)d.floats * 4u);
-        bulk_g2s(ws.stage(si), d.gptr, (uint32_t)d.floats * 4u, ws.full(si));
-      }
-    }
-    if (lane == 2) {
-      StagePub pb; pb.valid = 0; pb.cmn = pb.cmx = pb.s = pb.inv = 0.f;
-      *ws.pub(si) = pb;
-    }
+    ws.issue(si, d, lane, [](StagePub&) {});
     __syncwarp();
     if (lane == 0) mbar_arrive(ws.full(si));
   }
   __syncwarp();
   return a;
+}
+
+// A TK_PLAIN tile (one the TMA unit cannot move): the consumers fetch it into its stage themselves.  The stage's next refill
+// may be a bulk load (async proxy), hence the proxy fence; the barrier makes the whole tile visible to every consumer.
+__device__ __forceinline__ void consumers_fetch_tile(float* buf, const float* gptr, int floats) {
+  for (int i = ctid(); i < floats; i += kThreads) buf[i] = ldg_stream1(gptr + i);
+  fence_proxy_async_smem();
+  cbar();
 }
 
 __global__ void __launch_bounds__(kCtaThreads, kCleCtas)
@@ -880,7 +874,7 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
 
   // ---- phase 0: column extrema of every `second` layer (buffer 0) -----------------------------
   if (!producer) {
-    for (int g = blockIdx.x * kThreads + ctid(); g < nG; g += gridDim.x * kThreads) G[g].diff = 10.0;   // dfq.py:81
+    groups_init(G, nG, ctid(), kThreads);
     for (int j = ctid(); j < rs_cols; j += kThreads) { rs_min[j] = DFQ_INF; rs_max[j] = -DFQ_INF; }
     for (int li = blockIdx.x; li < nL; li += gridDim.x)
       if (L[li].rel_in >= 0 && !(L[li].flags & DFQ_LAYER_COLS_READY)) reset_cols(arena, L[li], R[L[li].rel_in], 0);
@@ -910,11 +904,7 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
         const TileDesc d = *ws.desc(sidx);
         if (d.kind == TK_END) { mbar_arrive(ws.done(sidx)); ++count; break; }
         float* buf = ws.stage(sidx);
-        if (d.kind == TK_PLAIN) {
-          for (int i = ctid(); i < d.floats; i += kThreads) buf[i] = ldg_stream1(d.gptr + i);
-          fence_proxy_async_smem();
-          cbar();
-        }
+        if (d.kind == TK_PLAIN) consumers_fetch_tile(buf, d.gptr, d.floats);
         if (d.task != cur_li) {
           flush();
           cur_li = d.task;
@@ -996,11 +986,7 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
           const volatile TileDesc& d = *ws.desc(sidx);
           if (d.kind == TK_END) { mbar_arrive(ws.done(sidx)); ++count; break; }
           float* buf = ws.stage(sidx);
-          if (d.kind == TK_PLAIN) {            // a tile the TMA unit cannot move: cooperative fetch
-            for (int i = ctid(); i < d.floats; i += kThreads) buf[i] = ldg_stream1(d.gptr + i);
-            fence_proxy_async_smem();          // the stage's next refill may be a bulk load (async proxy)
-            cbar();
-          }
+          if (d.kind == TK_PLAIN) consumers_fetch_tile(buf, d.gptr, d.floats);
           if (d.task != cur_li) {
             cur_li = d.task;
             const int g = L[cur_li].group;
@@ -1100,19 +1086,7 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
       __syncthreads();          // s_rule_stop is rewritten one sweep from now
       continue;
     }
-    if (!producer) {
-      for (int g = blockIdx.x * kThreads + ctid(); g < nG; g += gridDim.x * kThreads) {
-        GroupState& st = G[g];
-        if (st.done) continue;
-        const double diff_tmp = st.acc[slot];
-        st.acc[(slot + 2) % 3] = 0.0;   // last read before this sweep's final barrier, next used in sweep+2
-        if (g == 0 && sweep < 64) ctl->diffs[sweep] = diff_tmp;
-        bool converged;
-        if (exit_rule(st.diff, st.count, diff_tmp, P, n, &converged)) { st.n_sweeps = n; st.converged = converged; st.done = 1; }
-        else atomicAdd(&ctl->active[n & 1], 1);
-      }
-      if (blockIdx.x == 0 && threadIdx.x == 0) ctl->active[sweep & 1] = 0;   // read at the end of the previous sweep
-    }
+    if (!producer) groups_exit_rule(G, nG, ctl, P, sweep, ctid(), kThreads);
     __threadfence();
     grid.sync();
     if (*((volatile int*)&ctl->active[n & 1]) == 0) break;
@@ -1164,6 +1138,21 @@ __device__ __forceinline__ void sts_f4(uint32_t a, const float4& v) {
   asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
+// One second-layer row of n4 float4 at shared address a0, its columns scaled in place by the cached reciprocals inv_s
+// (MODE IN_KK9 or IN_KK1); returns this lane's sum of |new - old|.
+template <int MODE>
+__device__ __forceinline__ float stack_scale_cols(uint32_t a0, int n4, const float* __restrict__ inv_s, int lane) {
+  float dsum = 0.f;
+#pragma unroll 4
+  for (int i4 = lane; i4 < n4; i4 += 32) {
+    const float4 v = lds_f4(a0 + 16u * i4);
+    const float4 t = in_scale4<MODE>(v, i4 * 4, inv_s, 1.f, MODE == IN_KK9 ? 9 : 1);
+    sts_f4(a0 + 16u * i4, t);
+    dsum += absdiff4(t, v);
+  }
+  return dsum;
+}
+
 // Producer lane: this CTA's tiles of one step (layers of converged groups skipped), SKIP padding, one END per consumer.
 __device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n, float* arena, PassIter it) {
   TileDesc d;
@@ -1188,7 +1177,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool producer = (warp == kBcConsumers);
   unsigned long long n = producer ? 0 : (unsigned long long)warp;       // (warps >= kStackConsumers never use it)
-  for (int g = blockIdx.x * kBcThreads + threadIdx.x; g < nG; g += gridDim.x * kBcThreads) G[g].diff = 10.0;   // dfq.py:81
+  groups_init(G, nG, threadIdx.x, kBcThreads);
   __threadfence();
   grid.sync();
 
@@ -1238,7 +1227,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           const int row_len = c.row_len, n4 = row_len >> 2;
           const uint32_t sbase = smem_u32(ring.stage(s));
           const double inv_n = c.inv_n;
-          RowIn mine; mine.cmn = mine.cmx = 0.f; mine.u = 1.f; mine.s_given = 1.f;
+          RowIn mine;
           float ks = 1.f, kinv = 1.f;
           const bool has_out = c.has_out != 0;
           if (has_out) {
@@ -1248,26 +1237,18 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
               const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
               float mn = DFQ_INF, mx = -DFQ_INF;
 #pragma unroll 4
-              for (int i4 = lane; i4 < n4; i4 += 32) {
-                const float4 t = lds_f4(a0 + 16u * i4);
-                mn = fminf(mn, fminf(fminf(t.x, t.y), fminf(t.z, t.w)));
-                mx = fmaxf(mx, fmaxf(fmaxf(t.x, t.y), fmaxf(t.z, t.w)));
-              }
+              for (int i4 = lane; i4 < n4; i4 += 32) minmax4(mn, mx, lds_f4(a0 + 16u * i4));
               mn = warp_min(mn); mx = warp_max(mx);
-              RowIn in;
-              in.cmn = __shfl_sync(0xffffffffu, mine.cmn, r); in.cmx = __shfl_sync(0xffffffffu, mine.cmx, r);
-              in.u = 1.f; in.s_given = 1.f;
               float iv;
-              const float sv = solve_row(P, in, mn, mx, &iv);
+              const float sv = solve_row(P, shfl_row_in(mine, r), mn, mx, &iv);
               if (lane == r) { ks = sv; kinv = iv; }
               float dsum = 0.f;
 #pragma unroll 4
               for (int i4 = lane; i4 < n4; i4 += 32) {
                 const float4 v = lds_f4(a0 + 16u * i4);
-                float4 t;
-                t.x = __fmul_rn(v.x, sv); t.y = __fmul_rn(v.y, sv); t.z = __fmul_rn(v.z, sv); t.w = __fmul_rn(v.w, sv);
+                const float4 t = mul4(v, sv);
                 sts_f4(a0 + 16u * i4, t);
-                dsum += fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
+                dsum += absdiff4(t, v);
               }
               dacc += (double)dsum * inv_n;
             }
@@ -1275,24 +1256,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
             // ---- second layer: columns scaled by 1/s of the relation (dfq.py:73) ------------------------------------
             for (int r = 0; r < d.nrows; ++r) {
               const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
-              float dsum = 0.f;
-              if (kk == 9) {
-#pragma unroll 4
-                for (int i4 = lane; i4 < n4; i4 += 32) {
-                  const float4 v = lds_f4(a0 + 16u * i4);
-                  const float4 t = in_scale4<IN_KK9>(v, i4 * 4, inv_s, 1.f, 9);
-                  sts_f4(a0 + 16u * i4, t);
-                  dsum += fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
-                }
-              } else {
-#pragma unroll 4
-                for (int i4 = lane; i4 < n4; i4 += 32) {
-                  const float4 v = lds_f4(a0 + 16u * i4);
-                  const float4 t = in_scale4<IN_KK1>(v, i4 * 4, inv_s, 1.f, 1);
-                  sts_f4(a0 + 16u * i4, t);
-                  dsum += fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
-                }
-              }
+              const float dsum = kk == 9 ? stack_scale_cols<IN_KK9>(a0, n4, inv_s, lane) : stack_scale_cols<IN_KK1>(a0, n4, inv_s, lane);
               dacc += (double)dsum * inv_n;
             }
           }
@@ -1310,7 +1274,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           }
           // per-channel bookkeeping of dfq.py:62-70 (S, 1/s, bias, BN vectors, derived column extrema), lane r for row r - after
           // the stage is on its way back: a dozen dependent global accesses that the ring does not have to wait for
-          if (has_out && lane < d.nrows) publish_row(c, P, d.row0 + lane, ks, kinv, mine.cmn, mine.cmx);
+          if (has_out && lane < d.nrows) publish_row(c, P, d.row0 + lane, ks, kinv, mine.cmn, mine.cmx, fetch_row_pub(c, P, d.row0 + lane));
         }
         flush_metric();
         if (lane == 0) { bulk_wait_all(); fence_proxy_async_all(); }
@@ -1319,21 +1283,10 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
       grid.sync();
     }
     // ---- exit rule of dfq.py:105-115, one thread per group (as in k_cle_engine) ---------------------------------------
-    const int nsw = sweep + 1;
-    for (int g = blockIdx.x * kBcThreads + threadIdx.x; g < nG; g += gridDim.x * kBcThreads) {
-      GroupState& st = G[g];
-      if (st.done) continue;
-      const double diff_tmp = st.acc[slot];
-      st.acc[(slot + 2) % 3] = 0.0;
-      if (g == 0 && sweep < 64) ctl->diffs[sweep] = diff_tmp;
-      bool converged;
-      if (exit_rule(st.diff, st.count, diff_tmp, P, nsw, &converged)) { st.n_sweeps = nsw; st.converged = converged; st.done = 1; }
-      else atomicAdd(&ctl->active[nsw & 1], 1);
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0) ctl->active[sweep & 1] = 0;
+    groups_exit_rule(G, nG, ctl, P, sweep, threadIdx.x, kBcThreads);
     __threadfence();
     grid.sync();
-    if (*((volatile int*)&ctl->active[nsw & 1]) == 0) break;
+    if (*((volatile int*)&ctl->active[(sweep + 1) & 1]) == 0) break;
   }
 }
 
@@ -1408,10 +1361,16 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     DFQ_REQUIRE(l.bias_off >= 0 && l.bias_off + l.rows <= arena_floats, "bias outside arena");
     if (l.rel_in >= 0 && l.rel_out >= 0) DFQ_REQUIRE(l.rel_in < l.rel_out, "relations must be in forward chain order");
   }
-  int64_t scan_total = 0;
+  // layers whose column extrema the engine scans before the first sweep (the others arrive with buffer 0 filled)
+  std::vector<int32_t> scan_layers;
+  std::vector<long long> scan_ptr(1, 0);    // pass-tile prefix over scan_layers
   for (int i = 0; i < n_layers; ++i)
-    if (layers[i].rel_in >= 0 && !(layers[i].flags & DFQ_LAYER_COLS_READY)) scan_total += pass_tiles(layers[i]);
-  max_tiles = std::max(max_tiles, scan_total);
+    if (layers[i].rel_in >= 0 && !(layers[i].flags & DFQ_LAYER_COLS_READY)) {
+      scan_layers.push_back(i);
+      scan_ptr.push_back(scan_ptr.back() + pass_tiles(layers[i]));
+    }
+  const int n_scan = (int)scan_layers.size();
+  max_tiles = std::max<int64_t>(max_tiles, scan_ptr.back());
   for (int p = 0; p < n_steps; ++p) {
     int64_t t = 0;
     for (int q = step_ptr[p]; q < step_ptr[p + 1]; ++q) {
@@ -1438,7 +1397,7 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
                       l.cols <= kBcExCols;
       stack_tiles += pass_tiles(l);
     }
-  int dev = 0, sms = 0, per_sm = 0, coop = 0;
+  int dev = 0, sms = 0, coop = 0, grid = 0, rc;
   DFQ_CUDA(cudaGetDevice(&dev));
   DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int n_entries = step_ptr[n_steps];
@@ -1449,14 +1408,10 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
   if (const char* e = getenv("DFQ_CLE_STACK")) stack_ok = stack_eligible && atoi(e) != 0;   // 0: never, 1: whenever eligible (tests)
   if (stack_ok) {
     const size_t dyn_s = BcRing::smem_bytes();
-    DFQ_CUDA(cudaFuncSetAttribute(k_cle_stack, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_s));
-    DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cle_stack, kBcThreads, dyn_s));
-    if (per_sm < 1) { set_error("k_cle_stack does not fit on an SM"); return DFQ_E_NOT_COOPERATIVE; }
-    const int grid = (int)std::min<int64_t>((int64_t)sms * per_sm, std::max<int64_t>(1, max_tiles));
+    if ((rc = coop_grid((const void*)k_cle_stack, "k_cle_stack", kBcThreads, dyn_s, max_tiles, &grid))) return rc;
     TablePack tp;
     const int iL = tp.add(layers, n_layers), iR = tp.add(rels, n_rels), iSP = tp.add(step_ptr, n_steps + 1);
     const int iSL = tp.add(step_layers, n_entries), iPP = tp.add(pass_ptr.data(), n_entries + 1);
-    int rc;
     if ((rc = tp.upload(st))) return rc;
     DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqRelation* dR = tp.ptr<DfqRelation>(iR);
     int32_t *dSP = tp.ptr<int32_t>(iSP), *dSL = tp.ptr<int32_t>(iSL);
@@ -1472,42 +1427,20 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
   bool any_rescan = false;
   for (int i = 0; i < n_layers; ++i) any_rescan |= (layers[i].rel_in >= 0 && layers[i].col_mode == 2);
   int rs_cols = any_rescan ? kRescanCols : 0;
-  // table mirror for small models (see the kernel); its size must be known before the occupancy query
-  size_t tbl_est = 0;
-  {
-    int n_scan_est = 0;
-    for (int i = 0; i < n_layers; ++i) n_scan_est += (layers[i].rel_in >= 0 && !(layers[i].flags & DFQ_LAYER_COLS_READY));
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    tbl_est = al(sizeof(DfqLayer) * n_layers) + al(sizeof(DfqRelation) * n_rels) + al(4 * (n_steps + 1)) + al(4 * n_entries) +
-              al(8 * (n_entries + 1)) + al(8 * (n_scan_est + 1)) + al(4 * n_scan_est);
-  }
-  const bool cache_tables = tbl_est <= kTableCacheBytes;
-  const size_t dyn_smem = ((WsPipe::smem_bytes() + 15) & ~(size_t)15) + (size_t)2 * rs_cols * sizeof(float) +
-                          (cache_tables ? tbl_est : 0);
-  DFQ_CUDA(cudaFuncSetAttribute(k_cle_engine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem));
-  DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cle_engine, kCtaThreads, dyn_smem));
-  if (per_sm < 1) { set_error("persistent kernel does not fit on an SM"); return DFQ_E_NOT_COOPERATIVE; }
-  const int grid = (int)std::min<int64_t>((int64_t)sms * per_sm, max_tiles);
-
-  std::vector<int32_t> scan_layers;
-  std::vector<long long> scan_ptr(1, 0);
-  for (int i = 0; i < n_layers; ++i)
-    if (layers[i].rel_in >= 0 && !(layers[i].flags & DFQ_LAYER_COLS_READY)) {   // the others arrive with buffer 0 filled
-      scan_layers.push_back(i);
-      scan_ptr.push_back(scan_ptr.back() + pass_tiles(layers[i]));
-    }
-  int n_scan = (int)scan_layers.size();
   TablePack tp;
   const int iL = tp.add(layers, n_layers), iR = tp.add(rels, n_rels), iSP = tp.add(step_ptr, n_steps + 1);
   const int iSL = tp.add(step_layers, n_entries);
   const int iPP = tp.add(pass_ptr.data(), n_entries + 1), iSCP = tp.add(scan_ptr.data(), n_scan + 1);
   const int iSCL = tp.add(scan_layers.data(), n_scan);
-  int rc;
+  // table mirror for small models (see the kernel): part of the dynamic shared memory the occupancy query is asked about
+  const bool cache_tables = tp.total <= kTableCacheBytes;
+  const size_t dyn_smem = ((WsPipe::smem_bytes() + 15) & ~(size_t)15) + (size_t)2 * rs_cols * sizeof(float) +
+                          (cache_tables ? tp.total : 0);
+  if ((rc = coop_grid((const void*)k_cle_engine, "k_cle_engine", kCtaThreads, dyn_smem, max_tiles, &grid))) return rc;
   if ((rc = tp.upload(st))) return rc;
   DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqRelation* dR = tp.ptr<DfqRelation>(iR);
   int32_t *dSP = tp.ptr<int32_t>(iSP), *dSL = tp.ptr<int32_t>(iSL), *dSCL = tp.ptr<int32_t>(iSCL);
   long long *dPP = tp.ptr<long long>(iPP), *dSCP = tp.ptr<long long>(iSCP);
-  if (cache_tables && tp.total != tbl_est) { set_error("internal: table pack size mismatch"); return DFQ_E_ARG; }
   CleCtl* dctl = nullptr;
   GroupState* dG = nullptr;
   DfqCleParams P = *params;

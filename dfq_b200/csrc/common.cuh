@@ -43,6 +43,10 @@ inline void free_async(void* p, cudaStream_t st) {
 }
 
 int sm_count();
+// Grid of a cooperative kernel launched with `threads` threads and `dyn_smem` bytes of dynamic shared memory per CTA: as
+// many CTAs as fit on the device at once, at most max_tiles and at least one.  Raises the kernel's dynamic shared-memory
+// limit first when dyn_smem > 0.  DFQ_E_NOT_COOPERATIVE (message names `kernel_name`) when not one CTA fits on an SM.
+int coop_grid(const void* kernel, const char* kernel_name, int threads, size_t dyn_smem, int64_t max_tiles, int* grid);
 
 // All descriptor tables of one call are packed into a MAPPED page-locked staging slot (ring of 4, reused after the copy
 // that read it has completed) and moved into ONE stream-ordered device allocation by a small KERNEL that reads the slot over
@@ -128,6 +132,39 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// CTA-wide min/max of THREADS threads; every thread gets the result.  red: 2 * THREADS / 32 floats of shared memory.
+template <int THREADS>
+__device__ __forceinline__ void block_minmax(float& mn, float& mx, float* red) {
+  constexpr int W = THREADS / 32;
+  mn = warp_min(mn); mx = warp_max(mx);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) { red[w] = mn; red[W + w] = mx; }
+  __syncthreads();
+  float a = red[l & (W - 1)], b = red[W + (l & (W - 1))];
+#pragma unroll
+  for (int o = W / 2; o > 0; o >>= 1) {
+    a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
+    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
+  }
+  mn = a; mx = b;
+}
+
+// Element-wise float4 steps, each element an individually rounded fp32 op.
+// (mn, mx) <- the extrema of (mn, mx) and the four elements of v
+__device__ __forceinline__ void minmax4(float& mn, float& mx, const float4& v) {
+  mn = fminf(mn, fminf(fminf(v.x, v.y), fminf(v.z, v.w)));
+  mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+}
+__device__ __forceinline__ float4 mul4(float4 v, float s) {
+  v.x = __fmul_rn(v.x, s); v.y = __fmul_rn(v.y, s); v.z = __fmul_rn(v.z, s); v.w = __fmul_rn(v.w, s);
+  return v;
+}
+// ((|t.x - v.x| + |t.y - v.y|) + |t.z - v.z|) + |t.w - v.w|: the summation order is part of the equalization's convergence
+// metric, which is compared bit for bit
+__device__ __forceinline__ float absdiff4(const float4& t, const float4& v) {
+  return fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
 }
 
 // float atomic min/max through the integer ordering of IEEE bit patterns (works in global and shared).
@@ -259,6 +296,13 @@ __device__ __forceinline__ float fake_quant(float x, const QuantScalars& q, floa
   if (code) *code = t;
   t = __fmul_rn(t, q.scale);
   return __fadd_rn(t, q.min_v);
+}
+template <bool RECIP>
+__device__ __forceinline__ float4 fake_quant4(const float4& v, const QuantScalars& q, float4* codes = nullptr) {
+  float4 r;
+  r.x = fake_quant<RECIP>(v.x, q, codes ? &codes->x : nullptr); r.y = fake_quant<RECIP>(v.y, q, codes ? &codes->y : nullptr);
+  r.z = fake_quant<RECIP>(v.z, q, codes ? &codes->z : nullptr); r.w = fake_quant<RECIP>(v.w, q, codes ? &codes->w : nullptr);
+  return r;
 }
 
 }  // namespace dfq

@@ -52,11 +52,7 @@ __device__ __forceinline__ void fold_row(float* arena, const DfqLayer& l, const 
   const float fac = __fdiv_rn(gamma, den);
   if (!GLOBAL && (n & 3) == 0) {
     float4* r4 = (float4*)row;
-    for (int i = lane; i < (n >> 2); i += TPR) {
-      float4 v = r4[i];
-      v.x = __fmul_rn(v.x, fac); v.y = __fmul_rn(v.y, fac); v.z = __fmul_rn(v.z, fac); v.w = __fmul_rn(v.w, fac);
-      r4[i] = v;
-    }
+    for (int i = lane; i < (n >> 2); i += TPR) r4[i] = mul4(r4[i], fac);
   } else if (GLOBAL) {
     for (int i = lane; i < n; i += TPR) stg_stream1(row + i, __fmul_rn(ldg_stream1(row + i), fac));
   } else {
@@ -163,21 +159,11 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
 // ------------------------------------------------------------------------------------------------
 struct FlatTask { int64_t off; int64_t n; int64_t minmax_off; int32_t num_bits; int32_t symmetric; };
 
+// the CTA's (mn, mx) folded into dst2[0..1]; the leading barrier lets `red` be reused from one call to the next
 __device__ __forceinline__ void cta_minmax_atomic(float mn, float mx, float* dst2, float* red) {
-  mn = warp_min(mn); mx = warp_max(mx);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   __syncthreads();
-  if (l == 0) { red[w] = mn; red[kWarps + w] = mx; }
-  __syncthreads();
-  if (w == 0) {
-    float a = red[l & (kWarps - 1)], b = red[kWarps + (l & (kWarps - 1))];
-#pragma unroll
-    for (int o = kWarps / 2; o > 0; o >>= 1) {
-      a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-      b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-    }
-    if (l == 0) { atomic_min_f(dst2, a); atomic_max_f(dst2 + 1, b); }
-  }
+  block_minmax<kThreads>(mn, mx, red);
+  if (threadIdx.x == 0) { atomic_min_f(dst2, mn); atomic_max_f(dst2 + 1, mx); }
 }
 
 __device__ __forceinline__ void tile_minmax(const float* x, int64_t n, int64_t t, float& mn, float& mx) {
@@ -186,11 +172,7 @@ __device__ __forceinline__ void tile_minmax(const float* x, int64_t n, int64_t t
   if ((((uintptr_t)x) & 15) == 0) {
     const float4* x4 = (const float4*)x;
     const int64_t lo4 = lo >> 2, hi4 = hi >> 2;
-    for (int64_t i = lo4 + threadIdx.x; i < hi4; i += kThreads) {
-      const float4 v = ldg_stream(x4 + i);
-      mn = fminf(mn, fminf(fminf(v.x, v.y), fminf(v.z, v.w)));
-      mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
-    }
+    for (int64_t i = lo4 + threadIdx.x; i < hi4; i += kThreads) minmax4(mn, mx, ldg_stream(x4 + i));
     for (int64_t i = (hi4 << 2) + threadIdx.x; i < hi; i += kThreads) {
       const float v = ldg_stream1(x + i); mn = fminf(mn, v); mx = fmaxf(mx, v);
     }
@@ -241,12 +223,7 @@ k_quant_tasks(float* arena, const FlatTask* __restrict__ T, int nT, const long l
         if ((t.off & 3) == 0) {
           float4* x4 = (float4*)x;
           const int64_t lo4 = lo >> 2, hi4 = hi >> 2;
-          for (int64_t i = lo4 + threadIdx.x; i < hi4; i += kThreads) {
-            float4 v = ldg_stream(x4 + i);
-            v.x = fake_quant<RECIP>(v.x, q); v.y = fake_quant<RECIP>(v.y, q);
-            v.z = fake_quant<RECIP>(v.z, q); v.w = fake_quant<RECIP>(v.w, q);
-            stg_stream(x4 + i, v);
-          }
+          for (int64_t i = lo4 + threadIdx.x; i < hi4; i += kThreads) stg_stream(x4 + i, fake_quant4<RECIP>(ldg_stream(x4 + i), q));
           for (int64_t i = (hi4 << 2) + threadIdx.x; i < hi; i += kThreads) stg_stream1(x + i, fake_quant<RECIP>(ldg_stream1(x + i), q));
         } else {
           for (int64_t i = lo + threadIdx.x; i < hi; i += kThreads) stg_stream1(x + i, fake_quant<RECIP>(ldg_stream1(x + i), q));
@@ -292,6 +269,46 @@ struct BcGeo {
 
 constexpr int kExpectCache = 2048;
 
+// every corrected weight's per-tensor (min, max) slot <- (+inf, -inf); THREADS threads per CTA
+template <int THREADS>
+__device__ __forceinline__ void bc_reset_minmax(float* arena, const DfqBcLayer* __restrict__ B, int nB) {
+  for (int i = blockIdx.x * THREADS + threadIdx.x; i < nB; i += gridDim.x * THREADS) {
+    __stcg(arena + B[i].minmax_off, DFQ_INF);
+    __stcg(arena + B[i].minmax_off + 1, -DFQ_INF);
+  }
+}
+
+// E[x] of one layer (dfq.py:228-278) into ex: its terms in order, each written to or (accumulate) added into its slice.
+// SMEM: ex is this CTA's shared-memory copy; otherwise it lies in the arena and is accessed with .cg.
+template <int THREADS, bool SMEM>
+__device__ __forceinline__ void bc_expect(float* arena, const DfqBcLayer& b, const DfqExpectTerm* __restrict__ T, float* ex) {
+  for (int ti = b.term_begin; ti < b.term_end; ++ti) {
+    const DfqExpectTerm t = T[ti];
+    for (int ch = threadIdx.x; ch < t.n; ch += THREADS) {
+      const float fb = __ldcg(arena + t.bn_b_off + ch);
+      const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
+      float* d = ex + t.dst_off + ch;
+      if (SMEM) *d = t.accumulate ? __fadd_rn(*d, v) : v;
+      else __stcg(d, t.accumulate ? __fadd_rn(__ldcg(d), v) : v);
+    }
+    __syncthreads();
+  }
+}
+
+// Output row o's read-modify-write operands, requested before the row is processed so that their latency is hidden
+__device__ __forceinline__ void bc_fetch_row(const float* arena, const DfqLayer& l, const DfqBcLayer& b, int o, float& old_bias,
+                                             float& old_next) {
+  old_bias = __ldcg(arena + l.bias_off + o);
+  if (b.next_bn_b_off >= 0) old_next = __ldcg(arena + b.next_bn_b_off + o);
+}
+// ... and its retirement with the row's correction dl
+__device__ __forceinline__ void bc_retire_row(float* arena, const DfqLayer& l, const DfqBcLayer& b, int o, float dl, float old_bias,
+                                              float old_next) {
+  __stcg(arena + b.delta_off + o, dl);
+  __stcg(arena + l.bias_off + o, __fadd_rn(old_bias, (b.flags & 2) ? dl : -dl));              // dfq.py:292 / :164
+  if (b.next_bn_b_off >= 0) __stcg(arena + b.next_bn_b_off + o, __fadd_rn(old_next, -dl));   // dfq.py:204-206,293
+}
+
 // eps . E[x] of one output row held in shared (or, for rows larger than a stage, global) memory.
 // Returns the row's dot product in every thread of the row's group.
 template <int TPR, bool RAW>
@@ -329,10 +346,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
   TileDesc nd;
 
   // ---- per-tensor min/max of every corrected weight (dfq.py:14 via :218), streamed through the pipe ----------
-  for (int i = blockIdx.x * kThreads + threadIdx.x; i < nB; i += gridDim.x * kThreads) {
-    __stcg(arena + B[i].minmax_off, DFQ_INF);
-    __stcg(arena + B[i].minmax_off + 1, -DFQ_INF);
-  }
+  bc_reset_minmax<kThreads>(arena, B, nB);
   grid.sync();
   // layers whose column extrema the caller vouches for (DfqBcLayer.n_col > 0): reduce those, do not stream the weights
   for (int bi = blockIdx.x; bi < nB; bi += gridDim.x) {
@@ -363,11 +377,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         for (int i = threadIdx.x; i < d.floats; i += kThreads) { const float v = ldg_stream1(d.gptr + i); mn = fminf(mn, v); mx = fmaxf(mx, v); }
       } else if ((d.floats & 3) == 0) {
         const float4* b4 = (const float4*)pipe.stage[sidx];
-        for (int i = threadIdx.x; i < (d.floats >> 2); i += kThreads) {
-          const float4 v = b4[i];
-          mn = fminf(mn, fminf(fminf(v.x, v.y), fminf(v.z, v.w)));
-          mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
-        }
+        for (int i = threadIdx.x; i < (d.floats >> 2); i += kThreads) minmax4(mn, mx, b4[i]);
       } else {
         const float* bf = pipe.stage[sidx];
         for (int i = threadIdx.x; i < d.floats; i += kThreads) { mn = fminf(mn, bf[i]); mx = fmaxf(mx, bf[i]); }
@@ -387,21 +397,11 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
     // every CTA evaluates the recipe itself, straight into its shared-memory copy, when it reaches the layer below.
     const bool local = level_local[lev] != 0;
     if (!local) {
-    for (int bi = level_ptr[lev] + blockIdx.x; bi < level_ptr[lev + 1]; bi += gridDim.x) {
-      const DfqBcLayer b = B[bi];
-      float* ex = arena + b.expect_off;
-      for (int ti = b.term_begin; ti < b.term_end; ++ti) {
-        const DfqExpectTerm t = T[ti];
-        for (int ch = threadIdx.x; ch < t.n; ch += kThreads) {
-          const float fb = __ldcg(arena + t.bn_b_off + ch);
-          const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
-          float* d = ex + t.dst_off + ch;
-          __stcg(d, t.accumulate ? __fadd_rn(__ldcg(d), v) : v);
-        }
-        __syncthreads();
+      for (int bi = level_ptr[lev] + blockIdx.x; bi < level_ptr[lev + 1]; bi += gridDim.x) {
+        const DfqBcLayer b = B[bi];
+        bc_expect<kThreads, false>(arena, b, T, arena + b.expect_off);
       }
-    }
-    grid.sync();
+      grid.sync();
     }
     // ---- eps . E[x] per output row (dfq.py:216-219,281-293): rows streamed through the pipe, read only ---------
     MatIter<BcGeo> it;
@@ -422,16 +422,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         ex_cached = (b.expect_len <= kExpectCache);
         __syncthreads();
         if (local) {             // host guarantees expect_len <= kExpectCache for every layer of a local level
-          for (int ti = b.term_begin; ti < b.term_end; ++ti) {
-            const DfqExpectTerm t = T[ti];
-            for (int ch = threadIdx.x; ch < t.n; ch += kThreads) {
-              const float fb = __ldcg(arena + t.bn_b_off + ch);
-              const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
-              float* dst = s_ex + t.dst_off + ch;
-              *dst = t.accumulate ? __fadd_rn(*dst, v) : v;
-            }
-            __syncthreads();
-          }
+          bc_expect<kThreads, true>(arena, b, T, s_ex);
         } else if (ex_cached) {
           for (int j = threadIdx.x; j < b.expect_len; j += kThreads) s_ex[j] = __ldcg(arena + b.expect_off + j);
           __syncthreads();
@@ -445,10 +436,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         const float* ex = (ex_cached ? s_ex : arena + b.expect_off) + (size_t)(o / so) * l.cols;
         // the leader's read-modify-write operands are requested before the row is processed: their latency is hidden
         float old_bias = 0.f, old_next = 0.f;
-        if (threadIdx.x == 0) {
-          old_bias = __ldcg(arena + l.bias_off + o);
-          if (b.next_bn_b_off >= 0) old_next = __ldcg(arena + b.next_bn_b_off + o);
-        }
+        if (threadIdx.x == 0) bc_fetch_row(arena, l, b, o, old_bias, old_next);
         double acc = raw ? bc_row<kThreads, true>(row, l.cols, l.kk, ex, q, threadIdx.x)
                          : bc_row<kThreads, false>(row, l.cols, l.kk, ex, q, threadIdx.x);
         if (lane == 0) dred[warp] = acc;
@@ -457,10 +445,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
           acc = 0.0;
 #pragma unroll
           for (int i = 0; i < kWarps; ++i) acc += dred[i];
-          const float dl = (float)acc;
-          __stcg(arena + b.delta_off + o, dl);
-          __stcg(arena + l.bias_off + o, __fadd_rn(old_bias, (b.flags & 2) ? dl : -dl));              // dfq.py:292 / :164
-          if (b.next_bn_b_off >= 0) __stcg(arena + b.next_bn_b_off + o, __fadd_rn(old_next, -dl));   // dfq.py:204-206,293
+          bc_retire_row(arena, l, b, o, (float)acc, old_bias, old_next);
         }
       } else {
         // a warp per row, 32 rows per batch: lane j requests row j's read-modify-write operands before the batch and
@@ -470,10 +455,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
           const int il = base + lane;
           const int ol = d.row0 + warp + il * kWarps;
           float old_bias = 0.f, old_next = 0.f, dl = 0.f;
-          if (il < mine) {
-            old_bias = __ldcg(arena + l.bias_off + ol);
-            if (b.next_bn_b_off >= 0) old_next = __ldcg(arena + b.next_bn_b_off + ol);
-          }
+          if (il < mine) bc_fetch_row(arena, l, b, ol, old_bias, old_next);
           const int nb = min(32, mine - base);
           for (int j = 0; j < nb; ++j) {
             const int r = warp + (base + j) * kWarps;
@@ -483,11 +465,7 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
             const double acc = raw ? bc_row<32, true>(row, l.cols, l.kk, ex, q, lane) : bc_row<32, false>(row, l.cols, l.kk, ex, q, lane);
             if (lane == j) dl = (float)acc;
           }
-          if (il < mine) {
-            __stcg(arena + b.delta_off + ol, dl);
-            __stcg(arena + l.bias_off + ol, __fadd_rn(old_bias, (b.flags & 2) ? dl : -dl));              // dfq.py:292 / :164
-            if (b.next_bn_b_off >= 0) __stcg(arena + b.next_bn_b_off + ol, __fadd_rn(old_next, -dl));   // dfq.py:204-206,293
-          }
+          if (il < mine) bc_retire_row(arena, l, b, ol, dl, old_bias, old_next);
         }
       }
       bool more = false;
@@ -534,10 +512,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
   const BcGeo geo{arena, L, B};
 
   // ---- per-tensor min/max of every corrected weight (dfq.py:14 via :218) --------------------------------------
-  for (int i = blockIdx.x * kBcThreads + threadIdx.x; i < nB; i += gridDim.x * kBcThreads) {
-    __stcg(arena + B[i].minmax_off, DFQ_INF);
-    __stcg(arena + B[i].minmax_off + 1, -DFQ_INF);
-  }
+  bc_reset_minmax<kBcThreads>(arena, B, nB);
   grid.sync();
   // caller-vouched column extrema (DfqBcLayer.n_col > 0): a warp per layer reduces them
   for (int bi = blockIdx.x * (kBcThreads / 32) + warp; bi < nB; bi += gridDim.x * (kBcThreads / 32)) {
@@ -562,11 +537,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
           float mn = DFQ_INF, mx = -DFQ_INF;
           if (d.kind == TK_BULK && (d.floats & 3) == 0) {
             const float4* b4 = (const float4*)ring.stage(s);
-            for (int i = lane; i < (d.floats >> 2); i += 32) {
-              const float4 v = b4[i];
-              mn = fminf(mn, fminf(fminf(v.x, v.y), fminf(v.z, v.w)));
-              mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
-            }
+            for (int i = lane; i < (d.floats >> 2); i += 32) minmax4(mn, mx, b4[i]);
           } else if (d.kind == TK_BULK) {
             for (int i = lane; i < d.floats; i += 32) { const float v = ring.stage(s)[i]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
           } else {
@@ -585,17 +556,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
     // ---- E[x] of every layer of this level (dfq.py:228-278); one CTA per layer, terms in order ----
     for (int bi = level_ptr[lev] + blockIdx.x; bi < level_ptr[lev + 1]; bi += gridDim.x) {
       const DfqBcLayer b = B[bi];
-      float* ex = arena + b.expect_off;
-      for (int ti = b.term_begin; ti < b.term_end; ++ti) {
-        const DfqExpectTerm t = T[ti];
-        for (int ch = threadIdx.x; ch < t.n; ch += kBcThreads) {
-          const float fb = __ldcg(arena + t.bn_b_off + ch);
-          const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
-          float* d = ex + t.dst_off + ch;
-          __stcg(d, t.accumulate ? __fadd_rn(__ldcg(d), v) : v);
-        }
-        __syncthreads();
-      }
+      bc_expect<kBcThreads, false>(arena, b, T, arena + b.expect_off);
     }
     grid.sync();
     // ---- eps . E[x] per output row (dfq.py:216-219,281-293) ---------------------------------------------------
@@ -628,10 +589,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         }
         // lane r requests row r's read-modify-write operands before the tile and retires them after it
         float old_bias = 0.f, old_next = 0.f, dl = 0.f;
-        if (lane < d.nrows) {
-          old_bias = __ldcg(arena + l.bias_off + d.row0 + lane);
-          if (b.next_bn_b_off >= 0) old_next = __ldcg(arena + b.next_bn_b_off + d.row0 + lane);
-        }
+        if (lane < d.nrows) bc_fetch_row(arena, l, b, d.row0 + lane, old_bias, old_next);
         const uint32_t sbase = smem_u32(ring.stage(s));
         // (Tried: copying a [512,3,3] row to registers - 144 per lane, 224 registers per thread - and handing the stage back
         // BEFORE the arithmetic, so that the whole ring is loading.  The straight-line code that needs (16 columns x 9 taps
@@ -667,12 +625,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
           }
           if (lane == r) dl = (float)acc;
         }
-        if (lane < d.nrows) {
-          const int ol = d.row0 + lane;
-          __stcg(arena + b.delta_off + ol, dl);
-          __stcg(arena + l.bias_off + ol, __fadd_rn(old_bias, (b.flags & 2) ? dl : -dl));              // dfq.py:292 / :164
-          if (b.next_bn_b_off >= 0) __stcg(arena + b.next_bn_b_off + ol, __fadd_rn(old_next, -dl));   // dfq.py:204-206,293
-        }
+        if (lane < d.nrows) bc_retire_row(arena, l, b, d.row0 + lane, dl, old_bias, old_next);
         bc_give_back(ring, s, lane);
       }
     }
@@ -698,16 +651,6 @@ __global__ void k_bc_selftest(const float* __restrict__ w, float* eps_fast, floa
 
 using namespace dfq;
 
-static int pick_grid(const void* kernel, int64_t max_tiles, int* grid, size_t dyn_smem = 0) {
-  int dev = 0, sms = 0, per_sm = 0;
-  DFQ_CUDA(cudaGetDevice(&dev));
-  DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, dyn_smem));
-  if (per_sm < 1) { set_error("kernel does not fit on an SM"); return DFQ_E_NOT_COOPERATIVE; }
-  *grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sms * per_sm, max_tiles));
-  return 0;
-}
-
 extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
                            const DfqFold* folds, int32_t n_folds, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
@@ -731,8 +674,7 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
   }
   int grid, rc;
   const size_t dyn = RowPipe::smem_bytes();
-  DFQ_CUDA(cudaFuncSetAttribute(k_bn_fold, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-  if ((rc = pick_grid((const void*)k_bn_fold, tptr[n_folds], &grid, dyn))) return rc;
+  if ((rc = coop_grid((const void*)k_bn_fold, "k_bn_fold", kThreads, dyn, tptr[n_folds], &grid))) return rc;
   TablePack tp;
   const int iL = tp.add(layers, n_layers), iF = tp.add(folds, n_folds), iP = tp.add(tptr.data(), n_folds + 1);
   if ((rc = tp.upload(st))) return rc;
@@ -758,7 +700,7 @@ extern "C" int dfq_quantize_tensors(float* arena, int64_t arena_floats, const Df
     tptr[i + 1] = tptr[i] + (tasks[i].n + kChunk - 1) / kChunk;
   }
   int grid, rc;
-  if ((rc = pick_grid((const void*)k_minmax_tasks, tptr[n_tasks], &grid))) return rc;
+  if ((rc = coop_grid((const void*)k_minmax_tasks, "k_minmax_tasks", kThreads, 0, tptr[n_tasks], &grid))) return rc;
   TablePack tp;
   const int iT = tp.add(ft.data(), n_tasks), iP = tp.add(tptr.data(), n_tasks + 1);
   if ((rc = tp.upload(st))) return rc;
@@ -814,19 +756,10 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
   const int iL = tp.add(layers, n_layers), iB = tp.add(bc, n_bc), iT = tp.add(terms, n_terms);
   const int iLP = tp.add(level_ptr, n_levels + 1), iRP = tp.add(row_ptr.data(), n_bc + 1), iMP = tp.add(mm_ptr.data(), n_bc + 1);
   const int iLL = stream_variant ? -1 : tp.add(level_local.data(), n_levels);
-  size_t dyn;
-  if (stream_variant) {
-    dyn = BcRing::smem_bytes();
-    DFQ_CUDA(cudaFuncSetAttribute(k_bc_stream, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    int per_sm = 0;
-    DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_bc_stream, kBcThreads, dyn));
-    if (per_sm < 1) { set_error("k_bc_stream does not fit on an SM"); return DFQ_E_NOT_COOPERATIVE; }
-    grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sms * per_sm, max_tiles));
-  } else {
-    dyn = RowPipe::smem_bytes();
-    DFQ_CUDA(cudaFuncSetAttribute(k_bc_engine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    if ((rc = pick_grid((const void*)k_bc_engine, max_tiles, &grid, dyn))) return rc;
-  }
+  const size_t dyn = stream_variant ? BcRing::smem_bytes() : RowPipe::smem_bytes();
+  if (stream_variant) rc = coop_grid((const void*)k_bc_stream, "k_bc_stream", kBcThreads, dyn, max_tiles, &grid);
+  else                rc = coop_grid((const void*)k_bc_engine, "k_bc_engine", kThreads, dyn, max_tiles, &grid);
+  if (rc) return rc;
   if ((rc = tp.upload(st))) return rc;
   DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqBcLayer* dB = tp.ptr<DfqBcLayer>(iB); DfqExpectTerm* dT = tp.ptr<DfqExpectTerm>(iT);
   int32_t* dLP = tp.ptr<int32_t>(iLP); long long* dRP = tp.ptr<long long>(iRP); long long* dMP = tp.ptr<long long>(iMP);

@@ -30,6 +30,16 @@ int sm_count() {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
 }
+int coop_grid(const void* kernel, const char* kernel_name, int threads, size_t dyn_smem, int64_t max_tiles, int* grid) {
+  int dev = 0, sms = 0, per_sm = 0;
+  DFQ_CUDA(cudaGetDevice(&dev));
+  DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (dyn_smem > 0) DFQ_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem));
+  DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, dyn_smem));
+  if (per_sm < 1) { set_error("%s does not fit on an SM", kernel_name); return DFQ_E_NOT_COOPERATIVE; }
+  *grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sms * per_sm, max_tiles));
+  return 0;
+}
 
 namespace {
 struct Slot { unsigned char* host = nullptr; unsigned char* dev = nullptr; size_t cap = 0; cudaEvent_t ev = nullptr; bool used = false; };
@@ -133,20 +143,6 @@ int TablePack::upload(cudaStream_t st) {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 
-__device__ __forceinline__ void block_minmax(float& mn, float& mx, float* red) {
-  mn = warp_min(mn); mx = warp_max(mx);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { red[w] = mn; red[kWarps + w] = mx; }
-  __syncthreads();
-  float a = red[l & (kWarps - 1)], b = red[kWarps + (l & (kWarps - 1))];
-#pragma unroll
-  for (int o = kWarps / 2; o > 0; o >>= 1) {
-    a = fminf(a, __shfl_xor_sync(0xffffffffu, a, o));
-    b = fmaxf(b, __shfl_xor_sync(0xffffffffu, b, o));
-  }
-  mn = a; mx = b;
-}
-
 // grid-stride min/max of a flat tensor, 4 independent 128-bit loads in flight per thread
 __device__ __forceinline__ void flat_minmax(const float* __restrict__ x, int64_t n, int64_t start, int64_t stride,
                                             float& mn, float& mx) {
@@ -162,11 +158,7 @@ __device__ __forceinline__ void flat_minmax(const float* __restrict__ x, int64_t
       mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)), fmaxf(fmaxf(b.x, b.y), fmaxf(b.z, b.w))));
       mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(c.x, c.y), fmaxf(c.z, c.w)), fmaxf(fmaxf(d.x, d.y), fmaxf(d.z, d.w))));
     }
-    for (; i < n4; i += stride) {
-      const float4 a = ldg_stream(x4 + i);
-      mn = fminf(mn, fminf(fminf(a.x, a.y), fminf(a.z, a.w)));
-      mx = fmaxf(mx, fmaxf(fmaxf(a.x, a.y), fmaxf(a.z, a.w)));
-    }
+    for (; i < n4; i += stride) minmax4(mn, mx, ldg_stream(x4 + i));
     for (int64_t j = (n4 << 2) + start; j < n; j += stride) { const float v = x[j]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
   } else {
     for (int64_t j = start; j < n; j += stride) { const float v = x[j]; mn = fminf(mn, v); mx = fmaxf(mx, v); }
@@ -183,7 +175,7 @@ __global__ void __launch_bounds__(kThreads) k_minmax(const float* __restrict__ x
   __shared__ float red[2 * kWarps];
   float mn = DFQ_INF, mx = -DFQ_INF;
   flat_minmax(x, n, blockIdx.x * (int64_t)kThreads + threadIdx.x, (int64_t)gridDim.x * kThreads, mn, mx);
-  block_minmax(mn, mx, red);
+  block_minmax<kThreads>(mn, mx, red);
   if (threadIdx.x == 0) { atomic_min_f(out2, mn); atomic_max_f(out2 + 1, mx); }
 }
 
@@ -193,7 +185,7 @@ __global__ void __launch_bounds__(kThreads) k_sample_minmax(const float* __restr
   const float* xs = x + (int64_t)blockIdx.y * per;
   float mn = DFQ_INF, mx = -DFQ_INF;
   flat_minmax(xs, per, blockIdx.x * (int64_t)kThreads + threadIdx.x, (int64_t)gridDim.x * kThreads, mn, mx);
-  block_minmax(mn, mx, red);
+  block_minmax<kThreads>(mn, mx, red);
   if (threadIdx.x == 0) { atomic_min_f(scratch + 2 * blockIdx.y, mn); atomic_max_f(scratch + 2 * blockIdx.y + 1, mx); }
 }
 
@@ -268,9 +260,8 @@ k_quant(const float* __restrict__ x, float* __restrict__ y, int64_t n, QuantScal
     const int64_t n4 = n >> 2;
     for (int64_t i = start; i < n4; i += stride) {
       const float4 v = ldg_stream((const float4*)x + i);
-      float4 r, c;
-      r.x = fake_quant<RECIP>(v.x, q, &c.x); r.y = fake_quant<RECIP>(v.y, q, &c.y);
-      r.z = fake_quant<RECIP>(v.z, q, &c.z); r.w = fake_quant<RECIP>(v.w, q, &c.w);
+      float4 c;
+      float4 r = fake_quant4<RECIP>(v, q, &c);
       if (ERR) { r.x = __fsub_rn(r.x, v.x); r.y = __fsub_rn(r.y, v.y); r.z = __fsub_rn(r.z, v.z); r.w = __fsub_rn(r.w, v.w); }
       stg_stream((float4*)y + i, r);
       if (codes) stg_stream((float4*)codes + i, c);
@@ -328,7 +319,7 @@ k_observe_quant(const float* __restrict__ x, float* __restrict__ y, int64_t batc
     float mn = DFQ_INF, mx = -DFQ_INF;
     if (hi > lo) flat_minmax(x + b * per + lo, hi - lo, threadIdx.x, kThreads, mn, mx);
     __syncthreads();
-    block_minmax(mn, mx, red);
+    block_minmax<kThreads>(mn, mx, red);
     if (threadIdx.x == 0) { __stcg(scratch + 2 * it, mn); __stcg(scratch + 2 * it + 1, mx); }
   }
   __threadfence();
@@ -372,10 +363,7 @@ k_observe_quant(const float* __restrict__ x, float* __restrict__ y, int64_t batc
   if (((((uintptr_t)x) | ((uintptr_t)y)) & 15) == 0) {
     const int64_t n4 = n >> 2;
     for (int64_t i = start; i < n4; i += stride) {
-      const float4 v = ldg_stream((const float4*)x + i);
-      float4 r;
-      r.x = fake_quant<RECIP>(v.x, q); r.y = fake_quant<RECIP>(v.y, q); r.z = fake_quant<RECIP>(v.z, q); r.w = fake_quant<RECIP>(v.w, q);
-      stg_stream((float4*)y + i, r);
+      stg_stream((float4*)y + i, fake_quant4<RECIP>(ldg_stream((const float4*)x + i), q));
     }
     for (int64_t j = (n4 << 2) + start; j < n; j += stride) y[j] = fake_quant<RECIP>(x[j], q);
   } else {
@@ -393,7 +381,7 @@ k_range_rows(const float* __restrict__ w, int64_t rows, int64_t row_len, float* 
       float mn = DFQ_INF, mx = -DFQ_INF;
       flat_minmax(w + o * row_len, row_len, threadIdx.x, kThreads, mn, mx);
       __syncthreads();
-      block_minmax(mn, mx, red);
+      block_minmax<kThreads>(mn, mx, red);
       if (threadIdx.x == 0) { out_min[o] = mn; out_max[o] = mx; }
     }
   } else {
