@@ -1384,28 +1384,41 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
   }
 
   // ---- streaming variant for stacks of two-layer chains (k_cle_stack) ----------------------------------------------
-  bool stack_ok = (n_steps == 2) && !params->apply_only;
-  for (int i = 0; stack_ok && i < n_rels; ++i) stack_ok = rels[i].groups == 1;
+  // not_stack: the first eligibility condition the problem fails (nullptr: eligible)
+  const char* not_stack = nullptr;
+  if (n_steps != 2) not_stack = "step count (two steps: every chain has exactly two layers)";
+  else if (params->apply_only) not_stack = "apply_only";
+  for (int i = 0; !not_stack && i < n_rels; ++i)
+    if (rels[i].groups != 1) not_stack = "groups (every relation ungrouped)";
   int64_t stack_tiles = 0;
-  for (int p = 0; stack_ok && p < n_steps; ++p)
-    for (int q = step_ptr[p]; stack_ok && q < step_ptr[p + 1]; ++q) {
+  for (int p = 0; !not_stack && p < n_steps; ++p)
+    for (int q = step_ptr[p]; !not_stack && q < step_ptr[p + 1]; ++q) {
       const DfqLayer& l = layers[step_layers[q]];
       const int row_len = l.cols * l.kk;
-      stack_ok = (row_len % 4 == 0) && row_len <= kStageFloats && (l.w_off % 4 == 0) && (l.kk == 9 || l.kk == 1);
-      if (p == 0) stack_ok = stack_ok && l.rel_in < 0 && l.rel_out >= 0;
-      else stack_ok = stack_ok && l.rel_in >= 0 && l.rel_out < 0 && l.col_mode == 0 && (l.flags & DFQ_LAYER_COLS_READY) &&
-                      l.cols <= kBcExCols;
+      if (row_len % 4 != 0 || row_len > kStageFloats || l.w_off % 4 != 0)
+        not_stack = "row length or alignment (rows of a multiple of 4 floats, at most a stage, 16-byte aligned)";
+      else if (l.kk != 9 && l.kk != 1) not_stack = "taps (3x3 or 1x1)";
+      else if (p == 0 && !(l.rel_in < 0 && l.rel_out >= 0)) not_stack = "step count (a first layer that is also a second)";
+      else if (p == 1 && !(l.rel_in >= 0 && l.rel_out < 0 && l.col_mode == 0)) not_stack = "step count (a second layer that is also a first)";
+      else if (p == 1 && !(l.flags & DFQ_LAYER_COLS_READY)) not_stack = "column extrema not ready (second layers need COLS_READY)";
+      else if (p == 1 && l.cols > kBcExCols) not_stack = "columns (at most kBcExCols = 512 per second layer)";
       stack_tiles += pass_tiles(l);
     }
+  // DFQ_CLE_STACK: 0 never takes k_cle_stack, 1 always does and rejects a problem it cannot take (tests compare the two kernels:
+  // a silent fall-back would compare k_cle_engine with itself)
+  const char* force_stack = getenv("DFQ_CLE_STACK");
+  if (force_stack && atoi(force_stack) != 0 && not_stack) {
+    set_error("DFQ_CLE_STACK=1: problem not eligible for k_cle_stack: %s", not_stack);
+    return DFQ_E_ARG;
+  }
   int dev = 0, sms = 0, coop = 0, grid = 0, rc;
   DFQ_CUDA(cudaGetDevice(&dev));
   DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int n_entries = step_ptr[n_steps];
   std::vector<long long> pass_ptr(n_entries + 1, 0);    // pass-tile prefix over step_layers
   for (int q = 0; q < n_entries; ++q) pass_ptr[q + 1] = pass_ptr[q] + pass_tiles(layers[step_layers[q]]);
-  const bool stack_eligible = stack_ok;
-  stack_ok = stack_eligible && stack_tiles >= (int64_t)64 * sms;                              // large phases only: small models are latency-bound
-  if (const char* e = getenv("DFQ_CLE_STACK")) stack_ok = stack_eligible && atoi(e) != 0;   // 0: never, 1: whenever eligible (tests)
+  bool stack_ok = !not_stack && stack_tiles >= (int64_t)64 * sms;                     // large phases only: small models are latency-bound
+  if (force_stack) stack_ok = !not_stack && atoi(force_stack) != 0;
   if (stack_ok) {
     const size_t dyn_s = BcRing::smem_bytes();
     if ((rc = coop_grid((const void*)k_cle_stack, "k_cle_stack", kBcThreads, dyn_s, max_tiles, &grid))) return rc;

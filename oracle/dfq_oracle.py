@@ -331,6 +331,42 @@ def bias_delta(w: np.ndarray, expect: np.ndarray, signed: bool = False, num_bits
     return out
 
 
+def bias_delta_bound(w: np.ndarray, expect: np.ndarray, signed: bool = False, num_bits: int = 8, raw: bool = False):
+    """Per-row acceptance bound for a bias-correction kernel: returns (exact, bound), both float64 [O].
+
+    ``exact[o]`` = sum over (c, t) of eps[o, c, t] * E[c] in float64 from the bit-exact per-element errors
+    eps = Q(W) - W (``raw``: the bias-absorption form, W itself in place of eps).  The documented arithmetic (fp32 sum over the
+    kk taps of one column, float64 dot with E[x], one rounding to fp32) stays within
+
+        (kk - 1) * 2^-24 * sum_c |E_c| * sum_t |eps_oct|      fp32 sum of the taps, any order
+      + n * 2^-53 * sum_c |E_c * sum_t eps_oct|               float64 dot over the n = cols columns
+      + 2^-24 * |exact[o]|                                     final rounding to fp32
+
+    of ``exact[o]``.  Unlike a normwise gate over the whole layer this sees an error confined to one row, column or tap.
+    """
+    w = np.ascontiguousarray(w, f32)
+    eps = w if raw else quantize_error(w, num_bits, signed)
+    O, J = w.shape[0], w.shape[1]
+    e3 = eps.reshape(O, J, -1).astype(np.float64)
+    kk = e3.shape[2]
+    expect = np.asarray(expect, f32).astype(np.float64)
+    G = expect.shape[0] // J
+    so = O // G
+    ex = expect.reshape(G, J)[np.arange(O) // so]                  # [O, J]: the E[x] slice each row reads
+    colsum = e3.sum(axis=2)                                         # float64: its rounding is far below the bound
+    exact = (colsum * ex).sum(axis=1)
+    bound = ((kk - 1) * 2.0 ** -24 * (np.abs(ex) * np.abs(e3).sum(axis=2)).sum(axis=1)
+             + J * 2.0 ** -53 * np.abs(colsum * ex).sum(axis=1)
+             + 2.0 ** -24 * np.abs(exact))
+    return exact, bound
+
+
+def rows_outside_bound(got: np.ndarray, exact: np.ndarray, bound: np.ndarray) -> np.ndarray:
+    """Indices of the rows where a kernel's delta ``got`` leaves the bias_delta_bound interval."""
+    err = np.abs(np.asarray(got, np.float64) - exact)
+    return np.nonzero(~(err <= bound))[0]
+
+
 # --------------------------------------------------------------------------------------------
 # activation observer: utils/quantize.py:102-119
 # --------------------------------------------------------------------------------------------

@@ -1,6 +1,9 @@
 """-m gpu parity tests of the arena engine (libdfq_sm90.so through dfq_b200.engine.Session) against
 the numpy oracle on seeded inputs.  Equalization, BN fold factors and fake-quant are compared
-bit-exactly; bias correction to 1e-5 normwise (fp32 mat-vec has no defined order in the reference)."""
+bit-exactly; bias correction row by row within oracle.dfq_oracle.bias_delta_bound where the kernel and the oracle see
+identical inputs, and to 1e-5 normwise downstream of an earlier correction (inputs differ in the last bits).
+Boundary cases name, in a comment, the kernel branch they target and the constant that puts them there
+(tests/test_boundary_guards.py pins those constants)."""
 import numpy as np
 import pytest
 import torch
@@ -35,6 +38,24 @@ PAIRS = [
     ((8, 2500, 1, 1), (12, 8, 1, 1)),      # rows of 2500 floats (cta vec path, partial)
     ((6, 9001), (5, 6)),                   # row longer than the register tile: generic path, odd length
     ((7, 33, 1, 1), (9, 7, 1, 1)),         # scalar path, 33 elements
+    ((2044, 64), (10, 2044)),              # second-layer cols 2044 <= DFQ_INV_CACHE 2044: 1/s cached in shared memory (IN_KK1)
+    ((2048, 64), (10, 2048)),              # cols 2048 > DFQ_INV_CACHE 2044: 1/s read from global memory (IN_GENERIC)
+    ((32, 16, 3, 3), (24, 32, 2, 2)),      # kk 4 (not 1 or 9): IN_GENERIC, 128-float rows through the vector path
+    ((32, 16, 3, 3), (24, 32, 5, 5)),      # kk 25: IN_GENERIC, 800-float rows
+    ((32, 16, 3, 3), (24, 32, 7, 7)),      # kk 49: IN_GENERIC, 1568-float rows
+    ((66, 3, 7, 7), (24, 66, 1, 1)),       # 7x7 stem, 147-float rows: 28 per tile, last tile 10 rows = 1470 floats (TK_PLAIN)
+    ((24, 256, 3, 3), (16, 24, 3, 3)),     # 2304-float rows: kStageFloats 4608 / 2304 = 2 rows per tile
+    ((20, 4612), (12, 20)),                # 4612 floats > kStageFloats 4608: TK_DIRECT (4608 above: one row per tile, mailbox)
+    ((40, 4, 1, 1), (16, 40, 1, 1)),       # 4-float rows: 4608 / 4 = 1152 fit a stage, the 32-rows-per-tile cap binds
+    # short rows: items = floats / 4 on G lanes, the smallest power of two with DFQ_SUB_ITEMS 8 x G >= items; > 64 items: a warp
+    ((40, 32, 1, 1), (16, 40, 1, 1)),      # 8 items: G = 1
+    ((40, 36, 1, 1), (16, 40, 1, 1)),      # 9 items: G = 2
+    ((40, 64, 1, 1), (16, 40, 1, 1)),      # 16 items: G = 2
+    ((40, 68, 1, 1), (16, 40, 1, 1)),      # 17 items: G = 4
+    ((40, 128, 1, 1), (16, 40, 1, 1)),     # 32 items: G = 4
+    ((40, 132, 1, 1), (16, 40, 1, 1)),     # 33 items: G = 8
+    ((40, 256, 1, 1), (16, 40, 1, 1)),     # 64 items: G = 8
+    ((40, 260, 1, 1), (16, 40, 1, 1)),     # 65 items > 64: a warp per row
 ]
 
 
@@ -96,6 +117,9 @@ CHAINS = [
     [(144, 24, 1, 1), (144, 1, 3, 3), (32, 144, 1, 1)],                                               # inverted residual
     [(64, 32, 3, 3), (64, 64, 3, 3), (48, 64, 3, 3), (10, 48)],                                       # dense chain: re-scanned middles
     [(16, 8, 3, 3), (32, 8, 3, 3), (32, 1, 3, 3), (20, 32, 1, 1)],                                    # grouped (G=2) then depthwise
+    [(1024, 16, 1, 1), (64, 1024, 1, 1), (24, 64, 1, 1)],   # 1024 channels <= kScanCols, kRescanCols 1024: scan, col_mode 2 re-scan in smem
+    [(1028, 16, 1, 1), (64, 1028, 1, 1), (24, 64, 1, 1)],   # 1028 > 1024: initial scan and col_mode 2 re-scan with global atomics
+    [(1152, 16, 1, 1), (1152, 1, 3, 3), (32, 1152, 1, 1)],  # depthwise middle (col_mode 1) and 1x1 at 1152 > kScanCols: global atomics
 ]
 
 
@@ -137,6 +161,76 @@ def test_chain_to_convergence_matches_oracle(shapes, signed):
         assert np.array_equal(a.numpy(), obns[i][0]) and np.array_equal(b.numpy(), obns[i][1])
     for i, r in enumerate(rels):
         assert np.array_equal(S[i], r.S), "S of relation %d" % i
+
+
+@pytest.mark.parametrize("converge_count,min_sweeps", [
+    (3, 40),      # exits through the count branch of dfq.py:110-115 after 45 sweeps
+    (6, 65),      # ... after 69 sweeps: past the 64 sweeps CleResult.diffs records, the exit rule keeps counting
+])
+def test_exit_rule_count_branch_and_past_64_sweeps(converge_count, min_sweeps):
+    """converge_thres far below any reachable diff: the sweeps end only when the diff stops moving by more than 1e-9 for
+    converge_count sweeps in a row.  Sweep count, weights, biases, BN vectors and S equal the oracle bit for bit."""
+    from dfq_b200.engine import Session
+    shapes, thres = CHAINS[3], 1e-30
+    ws, bs, bns = _chain_case(shapes, 11)
+    layers = [O.OLayer(w.clone().numpy(), b.clone().numpy()) for w, b in zip(ws, bs)]
+    obns = [(a.clone().numpy(), b.clone().numpy()) for a, b in bns]
+    rels = [O.ORelation(i, i + 1, i) for i in range(len(shapes) - 1)]
+    n_ref, diffs_ref = O.cross_layer_equalization(layers, obns, rels, converge_thres=thres, converge_count=converge_count)
+    assert n_ref >= min_sweeps and diffs_ref[-1] > thres            # the oracle itself left through the count branch
+    sess = Session()
+    ids = [sess.add_layer(w, b) for w, b in zip(ws, bs)]
+    offs = [(sess.bind(a), sess.bind(b)) for a, b in bns]
+    sess.upload()
+    res, s_offs = sess.run_cle([(ids[i], ids[i + 1], offs[i][0], offs[i][1]) for i in range(len(shapes) - 1)],
+                               converge_thres=thres, converge_count=converge_count)
+    S = [sess.view(o, shapes[i][0]).cpu().numpy() for i, o in enumerate(s_offs)]
+    sess.download()
+    assert res.n_sweeps == n_ref and res.converged, (res.n_sweeps, n_ref)
+    np.testing.assert_allclose(res.diffs, diffs_ref[:64], rtol=1e-6, atol=1e-12)
+    for w, b, l in zip(ws, bs, layers):
+        assert np.array_equal(w.numpy(), l.w) and np.array_equal(b.numpy(), l.b)
+    for (a, b), (oa, ob) in zip(bns, obns):
+        assert np.array_equal(a.numpy(), oa) and np.array_equal(b.numpy(), ob)
+    for s, r in zip(S, rels):
+        assert np.array_equal(s, r.S)
+
+
+def _table_pack_bytes(n_pairs):
+    """TablePack of dfq_cle_run for n_pairs independent two-layer chains, none scanned ahead (cle_engine.cu: layers, relations,
+    step_ptr, step_layers, pass_ptr, scan_ptr, scan_layers), each table padded to 256 bytes (TablePack::add)."""
+    pad = lambda b: (b + 255) // 256 * 256
+    L, R = 2 * n_pairs, n_pairs
+    return (pad(64 * L) + pad(64 * R) + pad(4 * 3) + pad(4 * L) + pad(8 * (L + 1)) + pad(8 * (n_pairs + 1)) + pad(4 * n_pairs))
+
+
+@pytest.mark.parametrize("n_pairs", [
+    8,      # 8 pairs: 2816 bytes of tables <= kTableCacheBytes 9216: mirrored in shared memory
+    64,     # 64 pairs: 15360 bytes > 9216: read from global memory
+])
+def test_descriptor_table_mirror_both_sides(n_pairs):
+    """The same small pairs with the descriptor tables in shared memory and in global memory: bit-exact to the oracle."""
+    from dfq_b200.engine import Session
+    assert (_table_pack_bytes(n_pairs) <= 9 * 1024) == (n_pairs == 8)
+    ws, bs, bns = [], [], []
+    for p in range(n_pairs):
+        w, b, bn = _chain_case([(16, 8, 3, 3), (8, 16, 3, 3)], 300 + 3 * p)
+        ws += w; bs += b; bns += bn
+    layers = [O.OLayer(w.clone().numpy(), b.clone().numpy()) for w, b in zip(ws, bs)]
+    obns = [(a.clone().numpy(), b.clone().numpy()) for a, b in bns]
+    rels = [O.ORelation(2 * p, 2 * p + 1, p) for p in range(n_pairs)]
+    n_ref, _ = O.cross_layer_equalization(layers, obns, rels, max_sweeps=4)    # (the sum over many pairs keeps moving)
+    sess = Session()
+    ids = [sess.add_layer(w, b) for w, b in zip(ws, bs)]
+    offs = [(sess.bind(a), sess.bind(b)) for a, b in bns]
+    sess.upload()
+    res, _ = sess.run_cle([(ids[2 * p], ids[2 * p + 1], offs[p][0], offs[p][1]) for p in range(n_pairs)], max_sweeps=4)
+    sess.download()
+    assert res.n_sweeps == n_ref == 4
+    for w, b, l in zip(ws, bs, layers):
+        assert np.array_equal(w.numpy(), l.w) and np.array_equal(b.numpy(), l.b)
+    for (a, b), (oa, ob) in zip(bns, obns):
+        assert np.array_equal(a.numpy(), oa) and np.array_equal(b.numpy(), ob)
 
 
 def test_bn_fold_matches_oracle():
@@ -224,7 +318,8 @@ def _bias_correct_chain():
     d2_gpu = sess.view(doffs[0], 48).cpu().numpy(); d3_gpu = sess.view(doffs[1], 20).cpu().numpy()
     b3_gpu = sess.view(sess.layer(l3)["bias_off"], 20).cpu().numpy()
     sess.download()
-    assert _normwise(d2_gpu, d2) < 1e-5 and _normwise(d3_gpu, d3) < 1e-5
+    assert O.rows_outside_bound(d2_gpu, *O.bias_delta_bound(w2.numpy(), e1)).size == 0      # identical inputs: row by row
+    assert _normwise(d3_gpu, d3) < 1e-5                          # downstream of the first correction: inputs differ in the last bits
     assert _normwise(b2.numpy(), b2_ref) < 1e-5
     assert _normwise(bn2[1].numpy(), fb2) < 1e-5
     assert _normwise(b3_gpu, b3_ref) < 1e-5
@@ -347,6 +442,154 @@ def test_mid_size_stacks_run_the_streaming_kernels_and_match_the_oracle(n_blocks
     for b in (0, n_blocks - 1):
         r = stack_check.compare_block(st.block_arrays(pristine, b), st.block_arrays(after, b))
         assert r["weights_bit_exact"] and r["vectors_bit_exact"] and r["bias_normwise"] < 1e-5 and r["sweeps"] == 2, (b, r)
+        assert r["bias_rows_outside_bound"] == 0, (b, r)
+
+
+STACK_BLOCKS = [
+    ((128, 64, 3, 3), (256, 128, 3, 3)),   # non-square 3x3 block
+    ((96, 64, 3, 3), (200, 96, 1, 1)),     # 3x3 next to 1x1
+    ((512, 256, 1, 1), (64, 512, 3, 3)),   # second layer at kBcExCols 512 columns and kStageFloats 4608 floats
+    ((44, 16, 3, 3), (37, 44, 3, 3)),      # 396-float rows: 11 per tile, 37 rows = partial tiles, not a multiple of 32
+    ((100, 4, 3, 3), (24, 100, 1, 1)),     # 36-float rows: 4608 / 36 = 128, capped at 32 rows per tile
+]
+
+
+def _chains_session(chains, one_group, stack, bc_variant, hints, monkeypatch, seed=61):
+    """Fold -> equalize -> bias-correct a list of chains (shapes per chain) in one Session, each layer with a BN: chain i is
+    convergence group i (or all one group); the second layer of every chain is corrected with the first's ReLU expectation.
+    `stack`: DFQ_CLE_STACK value (None: unset).  Returns (before, after, res, deltas, expects) - per chain lists of layer dicts."""
+    from dfq_b200.engine import Session
+    if stack is None:
+        monkeypatch.delenv("DFQ_CLE_STACK", raising=False)
+    else:
+        monkeypatch.setenv("DFQ_CLE_STACK", stack)
+    _force_bc_variant(monkeypatch, bc_variant)
+    g = torch.Generator().manual_seed(seed)
+    sess = Session()
+    lay, rels, groups, folds, items = [], [], [], [], []
+    for ci, shapes in enumerate(chains):
+        cl = []
+        for k, s in enumerate(shapes):
+            d = dict(w=_mk(s, seed + 7 * ci + k, gain=(k % 2 == 0)) * 0.1, bias=torch.randn(s[0], generator=g) * 0.1,
+                     gamma=torch.rand(s[0], generator=g) + 0.5, beta=torch.randn(s[0], generator=g) * 0.2,
+                     mean=torch.randn(s[0], generator=g) * 0.1, var=torch.rand(s[0], generator=g) + 0.5)
+            d["li"] = sess.add_layer(d["w"], d["bias"])
+            for n in ("gamma", "beta", "mean", "var"):
+                d[n + "_off"] = sess.bind(d[n], False)
+            d["fake_w_off"], d["fake_b_off"] = sess.alloc(s[0]), sess.alloc(s[0])
+            folds.append(dict(layer=d["li"], bn_eps=1e-5, gamma_off=d["gamma_off"], beta_off=d["beta_off"], mean_off=d["mean_off"],
+                              var_off=d["var_off"], fake_w_off=d["fake_w_off"], fake_b_off=d["fake_b_off"]))
+            cl.append(d)
+        for k in range(len(shapes) - 1):
+            rels.append((cl[k]["li"], cl[k + 1]["li"], cl[k]["fake_w_off"], cl[k]["fake_b_off"]))
+            groups.append(0 if one_group else ci)
+        items.append(dict(layer=cl[1]["li"], signed=False, level=0, next_bn_b_off=cl[1]["fake_b_off"],
+                          terms=[dict(bn_w_off=cl[0]["fake_w_off"], bn_b_off=cl[0]["fake_b_off"], n=shapes[0][0], relu=True, op="set")]))
+        lay.append(cl)
+    before = [[dict((n, d[n].numpy().copy()) for n in ("w", "bias", "gamma", "beta", "mean", "var")) for d in cl] for cl in lay]
+    cle = sess.plan_cle(rels, groups=groups)
+    fold = sess.plan_bn_fold(folds, cle_plan=cle)
+    bc = sess.plan_bias_correct(items)
+    sess.upload()
+    sess.run_bn_fold(fold)
+    res = sess.run_cle_plan(cle, cols_ready=fold["scanned"])
+    sess.run_bias_correct_plan(bc, 8, col_hints=sess.cle_col_hints(cle, res) if hints else None)
+    view = lambda off, n: sess.view(int(off), int(n)).cpu().numpy().copy()
+    deltas = [view(bc["delta_offs"][i], chains[i][1][0]) for i in range(len(chains))]
+    expects = [view(b["expect_off"], b["expect_len"]) for b in bc["bt"]]          # one level: table order = chain order
+    s = [view(o, sess.layer(r[0])["rows"]) for o, r in zip(cle["s_offs"], rels)]
+    sess.download()
+    after = [[dict(w=d["w"].numpy().copy(), bias=d["bias"].numpy().copy(), fake_w=view(d["fake_w_off"], d["w"].shape[0]),
+                   fake_b=view(d["fake_b_off"], d["w"].shape[0])) for d in cl] for cl in lay]
+    return before, after, res, deltas, expects, s
+
+
+def _oracle_chains(before, one_group):
+    """The oracle of _chains_session: BN fold, equalization (per chain, or one call over all chains), correction of layer 1."""
+    out = []
+    layers, bns, rels = [], [], []
+    for cl in before:
+        base = len(layers)
+        for d in cl:
+            w2, b2, fw, fb = O.bn_fold(d["w"], d["bias"], d["gamma"], d["beta"], d["mean"], d["var"], 1e-5)
+            layers.append(O.OLayer(w2, b2)); bns.append([fw, fb])
+        crel = [O.ORelation(base + k, base + k + 1, base + k) for k in range(len(cl) - 1)]
+        if not one_group:
+            crel_local = [O.ORelation(k, k + 1, k) for k in range(len(cl) - 1)]
+            n, _ = O.cross_layer_equalization(layers[base:], [tuple(x) for x in bns[base:]], crel_local)
+            out.append(n)
+        rels += crel
+    if one_group:
+        n, _ = O.cross_layer_equalization(layers, [tuple(x) for x in bns], rels)
+        out = [n] * len(before)
+    return layers, bns, out
+
+
+@pytest.mark.parametrize("one_group", [False, True])
+@pytest.mark.parametrize("bc_variant", BC_VARIANTS)
+def test_heterogeneous_stack_kernel_equals_engine_and_oracle(one_group, bc_variant, monkeypatch):
+    """k_cle_stack on a stack of unlike two-layer blocks (non-square, 3x3 next to 1x1, partial tiles, the 512-column / 4608-float
+    edge, 36-float rows) in one launch, one convergence group per block and one over all blocks: forced k_cle_stack and forced
+    k_cle_engine on identical bits are bit-identical (weights, biases, BN vectors, S, sweeps, corrected biases - the stack run's
+    correction takes the column-extrema hints, the engine run's streams the weights), and both equal the oracle: equalization
+    bit for bit, the correction row by row within bias_delta_bound."""
+    runs = [_chains_session(STACK_BLOCKS, one_group, v, bc_variant, v == "1", monkeypatch) for v in ("1", "0")]
+    (before, a1, r1, d1, e1, s1), (_, a0, r0, d0, e0, s0) = runs
+    assert r1.converged and r0.converged and np.array_equal(r1.group_sweeps, r0.group_sweeps)
+    for x, y in zip(a1, a0):
+        for p, q in zip(x, y):
+            for k in p:
+                assert np.array_equal(p[k], q[k]), k
+    for x, y in zip(s1 + d1 + e1, s0 + d0 + e0):
+        assert np.array_equal(x, y)
+    layers, bns, sweeps = _oracle_chains(before, one_group)
+    assert list(r1.group_sweeps) == (sweeps[:1] if one_group else sweeps)
+    for b, cl in enumerate(a1):
+        l0, l1 = layers[2 * b], layers[2 * b + 1]
+        assert np.array_equal(cl[0]["w"], l0.w) and np.array_equal(cl[1]["w"], l1.w.reshape(cl[1]["w"].shape)), b
+        assert np.array_equal(cl[0]["bias"], l0.b) and np.array_equal(cl[0]["fake_w"], bns[2 * b][0]), b
+        assert np.array_equal(cl[0]["fake_b"], bns[2 * b][1]) and np.array_equal(cl[1]["fake_w"], bns[2 * b + 1][0]), b
+        ex = O.relu_expectation(*bns[2 * b])
+        np.testing.assert_array_max_ulp(e1[b], ex, maxulp=1)
+        exact, bound = O.bias_delta_bound(l1.w, e1[b])
+        assert O.rows_outside_bound(d1[b], exact, bound).size == 0, b
+        assert np.array_equal(cl[1]["bias"], l1.b + (-d1[b])) and np.array_equal(cl[1]["fake_b"], bns[2 * b + 1][1] + (-d1[b])), b
+
+
+INELIGIBLE = [  # (chains, the condition k_cle_stack refuses them for)
+    ([[(516, 16, 1, 1), (32, 516, 1, 1)]], "columns"),                     # 516 input columns > kBcExCols 512
+    ([[(32, 4612, 1, 1), (24, 32, 3, 3)]], "row length"),                   # first-layer rows of 4612 floats > kStageFloats 4608
+    ([[(32, 16, 5, 5), (24, 32, 3, 3)]], "taps"),                           # 5x5 taps
+    ([[(32, 16, 3, 3), (24, 16, 3, 3)]], "groups"),                         # grouped relation (G = 2)
+    ([[(32, 16, 3, 3), (48, 32, 3, 3), (24, 48, 1, 1)]], "step count"),     # three-layer chain
+]
+
+
+@pytest.mark.parametrize("chains,reason", INELIGIBLE)
+def test_forced_stack_kernel_rejects_what_it_cannot_run(chains, reason, monkeypatch):
+    """DFQ_CLE_STACK=1 on a problem k_cle_stack cannot take is an error naming the failed condition (never a silent run of
+    k_cle_engine); unforced, the same problem runs and equals the oracle."""
+    from dfq_b200._lib import DfqError
+    with pytest.raises(DfqError, match=reason):
+        _chains_session(chains, False, "1", "engine", False, monkeypatch)
+    before, after, res, deltas, _, _ = _chains_session(chains, False, None, "engine", False, monkeypatch)
+    layers, bns, sweeps = _oracle_chains(before, False)
+    assert list(res.group_sweeps) == sweeps
+    for d, l in zip(after[0], layers):
+        assert np.array_equal(d["w"], l.w.reshape(d["w"].shape))
+    exact, bound = O.bias_delta_bound(layers[1].w, O.relu_expectation(*bns[0]))
+    assert O.rows_outside_bound(deltas[0], exact, bound).size == 0
+
+
+def test_forced_stack_kernel_needs_ready_column_extrema(monkeypatch):
+    from dfq_b200._lib import DfqError
+    from dfq_b200.engine import Session
+    monkeypatch.setenv("DFQ_CLE_STACK", "1")
+    sess = Session()
+    l1 = sess.add_layer(_mk((32, 16, 3, 3), 1), None); l2 = sess.add_layer(_mk((24, 32, 3, 3), 2), None)
+    sess.upload()
+    with pytest.raises(DfqError, match="column extrema not ready"):
+        sess.run_cle_plan(sess.plan_cle([(l1, l2, -1, -1)]))
 
 
 def _config5_blocks():
@@ -365,7 +608,7 @@ def _config5_blocks():
     after = st.state()
     for b in (0, 2):
         r = stack_check.compare_block(st.block_arrays(pristine, b), st.block_arrays(after, b))
-        assert r["weights_bit_exact"] and r["vectors_bit_exact"], (b, r)
+        assert r["weights_bit_exact"] and r["vectors_bit_exact"] and r["bias_rows_outside_bound"] == 0, (b, r)
         assert r["bias_normwise"] < 1e-5 and r["sweeps"] == int(res.group_sweeps[b]) == 2, (b, r, res.group_sweeps)
 
 
@@ -493,7 +736,8 @@ def test_bias_correct_variants_on_mixed_layer_kinds(variant, monkeypatch):
     depthwise (cols = 1, groups = C: one expectation value per row), pointwise with more than 512 columns (expectation
     read from global memory), the 27-float rows of a first conv (tiles the TMA unit cannot move), rows longer than a
     stage (processed in global memory), a 'cat' of two BNs and an 'add' of two BNs, signed and unsigned, the raw-sum
-    (bias absorption) flags - against the oracle, 1e-5 normwise, with and without column-extrema hints."""
+    (bias absorption) flags, the expectation-cache, level and row-length boundaries of both kernels and tensors the fast-quotient
+    guard refuses - against the oracle row by row (bias_delta_bound), the kernel's E[x] scratch against relu_expectation."""
     from dfq_b200.engine import Session
     _force_bc_variant(monkeypatch, variant)
     g = torch.Generator().manual_seed(31)
@@ -504,6 +748,14 @@ def test_bias_correct_variants_on_mixed_layer_kinds(variant, monkeypatch):
     bnD = (torch.rand(3, generator=g) + 0.4, R(3) * 0.5)
     bnE = (torch.rand(640, generator=g) + 0.4, R(640) * 0.5)
     bnF = (torch.rand(1200, generator=g) + 0.4, R(1200) * 0.5)
+    bn_n = lambda n: (torch.rand(n, generator=g) + 0.4, R(n) * 0.5)
+    bnG, bnH, bnI, bnJ, bnK, bnL = bn_n(2048), bn_n(2052), bn_n(852), bn_n(512), bn_n(516), bn_n(1153)
+    # scale with an all-ones mantissa: lo = 0, hi = s * 255 (as test_bc_fast_quotient_equals_ieee_division builds it)
+    s_ones = np.uint32((np.float32(0.01).view(np.uint32) & np.uint32(0xff800000)) | np.uint32(0x7fffff)).view(np.float32)
+    w_ones = torch.rand(12, 64, 3, 3, generator=g) * float(np.float32(float(s_ones) * 255.0))
+    w_ones.view(-1)[0] = 0.0; w_ones.view(-1)[1] = float(np.float32(float(s_ones) * 255.0))
+    w_outlier = R(20, 64, 3, 3) * 0.1
+    w_outlier[3, 5, 1, 1] = 1e4
     cases = [  # (weight, signed, terms, flags)
         (R(48, 64, 3, 3) * 0.1, False, [("A", True, "set")], {}),
         (R(64, 1, 3, 3) * 0.3, False, [("A", True, "set")], {}),                          # depthwise
@@ -514,8 +766,25 @@ def test_bias_correct_variants_on_mixed_layer_kinds(variant, monkeypatch):
         (R(20, 64, 1, 1) * 0.2, True, [("A", True, "set"), ("A", False, "add")], {}),      # add
         (R(12, 32, 3, 3) * 0.1, False, [("A", True, "set")], {}),                          # grouped: 2 groups x 32 columns
         (R(30, 64, 3, 3) * 0.1, False, [("A", False, "set")], dict(raw_sum=True, add=True)),
+        # level 1: 4 layers, expect_len <= kExpectCache 2048 -> k_bc_engine evaluates E[x] per CTA in shared memory (level_local)
+        (R(16, 2048) * 0.02, False, [("G", True, "set")], dict(level=1)),                 # Linear, expect_len 2048 = kExpectCache
+        (R(16, 16, 3, 3) * 0.1, True, [("A", True, "set")], dict(level=1)),               # grouped G = 4 (so = 4), signed
+        (torch.zeros(10, 64, 1, 1), False, [("A", True, "set")], dict(level=1)),          # all-zero layer
+        (torch.full((10, 64, 1, 1), 0.3), False, [("A", True, "set")], dict(level=1)),    # constant layer: scale clamps to 1e-8
+        # level 2: 5 layers > 4 -> E[x] phase through the arena
+        (R(16, 2052) * 0.02, False, [("H", True, "set")], dict(level=2)),                 # expect_len 2052 > kExpectCache: global E[x]
+        (R(8, 2052, 1, 1) * 0.02, False, [("F", True, "set"), ("I", True, "cat")], dict(level=2)),   # cat 1200 + 852 crosses 2048
+        (R(20, 512, 1, 1) * 0.05, False, [("J", True, "set")], dict(level=2)),            # 512 cols = kBcExCols: k_bc_stream warp cache
+        (R(20, 516, 1, 1) * 0.05, True, [("K", True, "set")], dict(level=2)),             # 516 > kBcExCols: E[x] from global memory
+        (R(16, 32, 3, 3) * 0.1, True, [("A", True, "set")], dict(level=2)),               # grouped G = 2 (so = 8), signed
+        # level 3: row-length boundaries and tensors the fast-quotient guard of k_bc_stream refuses (IEEE chain)
+        (R(8, 512, 3, 3) * 0.05, False, [("J", True, "set")], dict(level=3)),             # 4608 floats = kStageFloats: one row per tile
+        (R(8, 1153, 2, 2) * 0.05, False, [("L", True, "set")], dict(level=3)),            # 4612 floats > kStageFloats: TK_DIRECT
+        (R(24, 64, 3, 3) * 1e-31, False, [("A", True, "set")], dict(level=3)),            # |w| ~ 1e-31: outside the guard's exponent window
+        (w_ones, False, [("A", True, "set")], dict(level=3)),                             # all-ones mantissa scale: guard refuses
+        (w_outlier, False, [("A", True, "set")], dict(level=3)),                          # one huge outlier: every other code near 0
     ]
-    bns = dict(A=bnA, B=bnB, C=bnC, D=bnD, E=bnE, F=bnF)
+    bns = dict(A=bnA, B=bnB, C=bnC, D=bnD, E=bnE, F=bnF, G=bnG, H=bnH, I=bnI, J=bnJ, K=bnK, L=bnL)
     sess = Session()
     off = {k: (sess.bind(v[0], False), sess.bind(v[1], False)) for k, v in bns.items()}
     items, biases, lids = [], [], []
@@ -524,26 +793,40 @@ def test_bias_correct_variants_on_mixed_layer_kinds(variant, monkeypatch):
         biases.append(b.clone())
         li = sess.add_layer(w, b)
         lids.append(li)
-        items.append(dict(layer=li, signed=signed, level=0, next_bn_b_off=-1,
+        flags = dict(flags)
+        items.append(dict(layer=li, signed=signed, level=flags.pop("level", 0), next_bn_b_off=-1,
                           terms=[dict(bn_w_off=off[k][0], bn_b_off=off[k][1], n=bns[k][0].numel(), relu=relu, op=op) for k, relu, op in terms],
                           **flags))
     sess.upload()
-    doffs = sess.run_bias_correct(items)
-    for (w, signed, terms, flags), b0, li, doff in zip(cases, biases, lids, doffs):
+    plan = sess.plan_bias_correct(items)
+    sess.run_bias_correct_plan(plan, 8)
+    doffs = plan["delta_offs"]
+    slot = {int(l): k for k, l in enumerate(plan["bt"]["layer"])}
+    levels = [it["level"] for it in items]
+    ex_len = [int(plan["bt"][slot[li]]["expect_len"]) for li in lids]
+    # k_bc_engine evaluates E[x] per CTA in shared memory (level_local) for levels of <= 4 layers with expect_len <= 2048
+    local = {lv: variant == "engine" and levels.count(lv) <= 4 and all(n <= 2048 for n, v in zip(ex_len, levels) if v == lv)
+             for lv in set(levels)}
+    assert [local[lv] for lv in sorted(local)] == ([False, True, False, False] if variant == "engine" else [False] * 4)
+    for (w, signed, terms, flags), b0, li, doff, it in zip(cases, biases, lids, doffs, items):
         ex = None
         for k, relu, op in terms:
             v = O.relu_expectation(bns[k][0].numpy(), bns[k][1].numpy()) if relu else bns[k][1].numpy().copy()
             ex = v if ex is None else (np.concatenate([ex, v]) if op == "cat" else ex + v)
-        if flags.get("raw_sum"):
-            d = O.bias_absorb_wc(w.numpy(), ex, ex.shape[0])
-            want = b0.numpy() + d
-        else:
-            d = O.bias_delta(w.numpy(), ex, signed=signed)
-            want = b0.numpy() + (-d)
+        # the kernel's E[x] scratch, where it is written, against the oracle on its own; the bound then takes the kernel's
+        if not local[it["level"]]:
+            b = plan["bt"][slot[li]]
+            got_ex = sess.view(int(b["expect_off"]), int(b["expect_len"])).cpu().numpy()
+            np.testing.assert_array_max_ulp(got_ex, ex, maxulp=1)
+            ex = got_ex
+        raw = bool(it.get("raw_sum"))
+        exact, bound = O.bias_delta_bound(w.numpy(), ex, signed=signed, raw=raw)
         got_d = sess.view(doff, w.shape[0]).cpu().numpy()
         got_b = sess.view(sess.layer(li)["bias_off"], w.shape[0]).cpu().numpy()
-        assert _normwise(got_d, d) < 1e-5, (tuple(w.shape), signed, terms, _normwise(got_d, d))
-        assert _normwise(got_b, want) < 1e-5, (tuple(w.shape), "bias")
+        bad = O.rows_outside_bound(got_d, exact, bound)
+        assert bad.size == 0, (tuple(w.shape), signed, terms, bad[:8], got_d[bad[:4]], exact[bad[:4]], bound[bad[:4]])
+        want = b0.numpy() + got_d if it.get("add") else b0.numpy() + (-got_d)     # the bias update itself is one fp32 add
+        assert np.array_equal(got_b, want), (tuple(w.shape), "bias")
 
 
 def test_bc_fast_quotient_equals_ieee_division():
