@@ -75,11 +75,15 @@ QUANT_TASK_DT = np.dtype([
     ("minmax_off", np.int64),
 ], align=True)
 
+I8_CONV_DT = np.dtype([(f, np.int32) for f in (
+    "N", "C", "H", "W", "O", "kh", "kw", "stride_h", "stride_w", "pad_h", "pad_w", "dil_h", "dil_w", "groups",
+    "OH", "OW", "Cpad", "_pad")], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 64), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
     "DfqCleResult": (CLE_RESULT_DT, 528), "DfqFold": (FOLD_DT, 64), "DfqExpectTerm": (TERM_DT, 32),
-    "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32),
+    "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
 }
 
 _PF = C.c_void_p   # device float*
@@ -112,6 +116,9 @@ SIGNATURES = {
     "dfq_selftest_bc_arithmetic": [_PF, _PF, _PF, _I64, _PF, C.c_int, C.c_int, C.c_void_p, _ST],
     "dfq_clamp": [_PF, _I64, C.c_float, C.c_float, _ST],
     "dfq_host_copy_segments": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int],
+    "dfq_i8_quantize_nhwc": [_PF, C.c_void_p, _I32, _I32, _I32, _I32, _I32, C.c_float, _ST],
+    "dfq_i8_pack_weights": [_PF, _PF, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_conv": [C.c_void_p, C.c_void_p, _PF, _PF, _PF, C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -1,0 +1,337 @@
+// Int8 execution of calibrated Conv2d / Linear layers: ncnn's dequantizing int8 convolution (the scheme of the int8
+// table convert_ncnn.py:178-201 writes) on the H100.  Symmetric codes q(v, s) = clamp(round_half_away(v * s), -127, 127)
+// for activations (one scale per tensor) and weights (one scale per output channel), an exact int32 accumulation and the
+// epilogue  y = fp32(fp32_rn(acc) * dq[o]) + bias[o]  with dq[o] = fp32(1 / fp32(a * w_s[o])) supplied by the caller.
+//
+//   k_i8_quantize_nhwc   fp32 NCHW -> int8 NHWC, channels padded to Cpad (multiple of 16) with zero bytes
+//   k_i8_pack_dense      fp32 [O, C, kh, kw] -> int8 [O][kh][kw][Cpad]: GEMM K = (tap, channel) contiguous
+//   k_i8_pack_dw         fp32 [C, 1, kh, kw] -> int8 [kh*kw][Cpad] (channels last)
+//   k_i8_conv_mma        groups == 1: implicit GEMM on the tensor cores (mma.sync m16n8k32 s8), M = N*OH*OW pixels,
+//                        N = O, K = kh*kw*Cpad; a cp.async ring gathers the im2col rows 16 channels (16 B) at a time
+//   k_i8_conv_dw         groups == C == O: int32 MACs on the CUDA cores over the NHWC codes
+#include <algorithm>
+
+#include "common.cuh"
+
+namespace dfq {
+namespace {
+
+__device__ __forceinline__ int8_t q8(float v, float s) {
+  const float p = roundf(__fmul_rn(v, s));              // roundf: half away from zero
+  return (int8_t)(int)fminf(fmaxf(p, -127.f), 127.f);
+}
+
+__device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
+  return __fadd_rn(__fmul_rn(__int2float_rn(acc), dq), b);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// quantizer and packers
+// ------------------------------------------------------------------------------------------------------------------
+
+// One thread per (n, 16-channel chunk, pixel); pixels fastest so the NCHW reads of each channel are coalesced.
+__global__ void k_i8_quantize_nhwc(const float* __restrict__ x, int8_t* __restrict__ q, int C, int HW, int Cpad, int64_t total,
+                                   float s) {
+  const int chunks = Cpad / 16;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i % HW;
+    const int64_t t = i / HW;
+    const int ch = (int)(t % chunks);
+    const int64_t n = t / chunks;
+    alignas(16) int8_t v[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = ch * 16 + j;
+      v[j] = c < C ? q8(x[(n * C + c) * HW + p], s) : (int8_t)0;
+    }
+    *reinterpret_cast<int4*>(q + (n * HW + p) * Cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+  }
+}
+
+__global__ void k_i8_pack_dense(const float* __restrict__ w, const float* __restrict__ ws, int8_t* __restrict__ out, int C,
+                                int taps, int Cpad, int64_t total) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % Cpad);
+    const int64_t t = i / Cpad;
+    const int tap = (int)(t % taps);
+    const int64_t o = t / taps;
+    out[i] = c < C ? q8(w[(o * C + c) * taps + tap], ws[o]) : (int8_t)0;
+  }
+}
+
+__global__ void k_i8_pack_dw(const float* __restrict__ w, const float* __restrict__ ws, int8_t* __restrict__ out, int C,
+                             int taps, int Cpad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= taps * Cpad) return;
+  const int c = i % Cpad, tap = i / Cpad;
+  out[i] = c < C ? q8(w[c * taps + tap], ws[c]) : (int8_t)0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// dense implicit GEMM on the tensor cores
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int BM = 128, BN = 64, BK = 64, STAGES = 3, THREADS = 128;
+constexpr int A_BYTES = BM * BK, B_BYTES = BN * BK, STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int EPI_LD = BM + 4;                                  // int32 words per staged output-channel row
+static_assert(BN * EPI_LD * 4 <= STAGES * STAGE_BYTES, "epilogue staging must fit in the pipeline's shared memory");
+
+// Rows are 64 B = four 16-byte chunks; chunk c of row r lives at chunk c ^ ((r >> 1) & 3), which keeps the eight rows an
+// ldmatrix phase reads (and the cp.async stores) on eight distinct 16-byte bank groups.
+__device__ __forceinline__ int swz(int row, int chunk) { return row * BK + ((chunk ^ ((row >> 1) & 3)) << 4); }
+
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  const int n = valid ? 16 : 0;                                 // src-size 0: the 16 bytes are zero-filled
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(n));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
+
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+
+__device__ __forceinline__ void mma_s8(int32_t* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+               : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// 4 warps as 2 (M) x 2 (N); each warp owns a 64 x 32 tile = 4 x 4 mma tiles.
+__global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq,
+                                                         const float* __restrict__ dq, const float* __restrict__ bias,
+                                                         float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g) {
+  __shared__ __align__(128) unsigned char smem[STAGES * STAGE_BYTES];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int wm = warp >> 1, wn = warp & 1;
+  const int64_t M = (int64_t)g.N * g.OH * g.OW;
+  const int64_t m0 = (int64_t)blockIdx.x * BM;
+  const int o0 = blockIdx.y * BN;
+  const int K = g.kh * g.kw * g.Cpad;
+  const int KT = (K + BK - 1) / BK;
+  const int OHW = g.OH * g.OW;
+
+  // this thread's gather slots: rows tid/4 + 32 i of the A tile and of the B tile, chunk tid % 4 of each
+  const int chunk = tid & 3;
+  const int8_t* a_img[4];
+  int a_ih[4], a_iw[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int64_t m = m0 + (tid >> 2) + 32 * i;
+    if (m < M) {
+      const int n = (int)(m / OHW), p = (int)(m % OHW);
+      a_img[i] = xq + (int64_t)n * g.H * g.W * g.Cpad;
+      a_ih[i] = (p / g.OW) * g.stride_h - g.pad_h;
+      a_iw[i] = (p % g.OW) * g.stride_w - g.pad_w;
+    } else {
+      a_img[i] = xq;
+      a_ih[i] = -(1 << 29);                                     // never inside the image
+      a_iw[i] = 0;
+    }
+  }
+  const uint32_t s_base = (uint32_t)__cvta_generic_to_shared(smem);
+
+  auto load_tile = [&](int kt, int stage) {
+    const uint32_t sa = s_base + stage * STAGE_BYTES, sb = sa + A_BYTES;
+    const int k = (kt * 4 + chunk) * 16;                        // first of the 16 channels of this chunk
+    const bool k_ok = k < K;
+    const int tap = k / g.Cpad, c0 = k - tap * g.Cpad;
+    const int dr = (tap / g.kw) * g.dil_h, ds = (tap % g.kw) * g.dil_w;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int ih = a_ih[i] + dr, iw = a_iw[i] + ds;
+      const bool ok = k_ok && (unsigned)ih < (unsigned)g.H && (unsigned)iw < (unsigned)g.W;
+      const int8_t* src = ok ? a_img[i] + ((int64_t)ih * g.W + iw) * g.Cpad + c0 : xq;
+      cp_async16(sa + swz((tid >> 2) + 32 * i, chunk), src, ok);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int o = o0 + (tid >> 2) + 32 * i;
+      const bool ok = k_ok && o < g.O;
+      const int8_t* src = ok ? wq + (int64_t)o * K + k : wq;
+      cp_async16(sb + swz((tid >> 2) + 32 * i, chunk), src, ok);
+    }
+  };
+
+  int32_t acc[4][4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) acc[i][j][r] = 0;
+
+#pragma unroll
+  for (int s = 0; s < STAGES - 1; ++s) {
+    if (s < KT) load_tile(s, s);
+    cp_async_commit();
+  }
+  for (int kt = 0; kt < KT; ++kt) {
+    cp_async_wait<STAGES - 2>();
+    __syncthreads();                                            // tile kt landed; everyone is done with tile kt - 1
+    if (kt + STAGES - 1 < KT) load_tile(kt + STAGES - 1, (kt + STAGES - 1) % STAGES);
+    cp_async_commit();
+    const uint32_t sa = s_base + (kt % STAGES) * STAGE_BYTES, sb = sa + A_BYTES;
+#pragma unroll
+    for (int ks = 0; ks < BK / 32; ++ks) {
+      uint32_t a[4][4], b[4][2];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {                             // matrices: rows 0-7 / 8-15 x k bytes 0-15 / 16-31
+        const int row = wm * 64 + i * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+        ldmatrix_x4(sa + swz(row, ks * 2 + (lane >> 4)), a[i][0], a[i][1], a[i][2], a[i][3]);
+      }
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {                             // matrices: n 0-7 x k 0-15 / 16-31, then n 8-15
+        const int row = wn * 32 + j * 16 + (lane & 7) + (lane >> 4) * 8;
+        ldmatrix_x4(sb + swz(row, ks * 2 + ((lane >> 3) & 1)), b[2 * j][0], b[2 * j][1], b[2 * j + 1][0], b[2 * j + 1][1]);
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) mma_s8(acc[i][j], a[i], b[j][0], b[j][1]);
+    }
+  }
+  cp_async_wait<0>();
+  __syncthreads();
+
+  // stage the tile as [o][m] so the NCHW stores run along the pixels
+  int32_t* st = reinterpret_cast<int32_t*>(smem);
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int m = wm * 64 + i * 16 + (lane >> 2) + (r >> 1) * 8;
+        const int o = wn * 32 + j * 8 + (lane & 3) * 2 + (r & 1);
+        st[o * EPI_LD + m] = acc[i][j][r];
+      }
+  __syncthreads();
+  for (int e = tid; e < BM * BN; e += THREADS) {
+    const int ml = e % BM, ol = e / BM;
+    const int64_t m = m0 + ml;
+    const int o = o0 + ol;
+    if (m >= M || o >= g.O) continue;
+    const int32_t v = st[ol * EPI_LD + ml];
+    const int64_t n = m / OHW, p = m % OHW;
+    const int64_t idx = (n * g.O + o) * OHW + p;
+    y[idx] = dequant(v, dq[o], bias ? bias[o] : 0.f);
+    if (acc_out) acc_out[idx] = v;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// depthwise on the CUDA cores: one thread per (n, 16 channels, output pixel), pixels fastest
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq, const float* __restrict__ dq,
+                             const float* __restrict__ bias, float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
+                             int64_t total) {
+  const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int p = (int)(i % OHW);
+    const int64_t t = i / OHW;
+    const int ch = (int)(t % chunks);
+    const int64_t n = t / chunks;
+    const int oh = p / g.OW, ow = p % g.OW;
+    int32_t acc[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = 0;
+    const int8_t* img = xq + n * g.H * g.W * g.Cpad + ch * 16;
+    for (int r = 0; r < g.kh; ++r) {
+      const int ih = oh * g.stride_h - g.pad_h + r * g.dil_h;
+      if ((unsigned)ih >= (unsigned)g.H) continue;
+      for (int s = 0; s < g.kw; ++s) {
+        const int iw = ow * g.stride_w - g.pad_w + s * g.dil_w;
+        if ((unsigned)iw >= (unsigned)g.W) continue;
+        const int4 xv = __ldg(reinterpret_cast<const int4*>(img + ((int64_t)ih * g.W + iw) * g.Cpad));
+        const int4 wv = __ldg(reinterpret_cast<const int4*>(wq + (r * g.kw + s) * g.Cpad + ch * 16));
+        const int8_t* xb = reinterpret_cast<const int8_t*>(&xv);
+        const int8_t* wb = reinterpret_cast<const int8_t*>(&wv);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = ch * 16 + j;
+      if (c >= g.C) break;
+      const int64_t idx = (n * g.C + c) * OHW + p;
+      y[idx] = dequant(acc[j], dq[c], bias ? bias[c] : 0.f);
+      if (acc_out) acc_out[idx] = acc[j];
+    }
+  }
+}
+
+inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+int check_geometry(const DfqI8Conv* g) {
+  DFQ_REQUIRE(g != nullptr, "dfq_i8: null geometry");
+  DFQ_REQUIRE(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->O > 0 && g->kh > 0 && g->kw > 0, "dfq_i8: empty dimension");
+  DFQ_REQUIRE(g->stride_h > 0 && g->stride_w > 0 && g->dil_h > 0 && g->dil_w > 0 && g->pad_h >= 0 && g->pad_w >= 0,
+              "dfq_i8: bad stride / padding / dilation");
+  DFQ_REQUIRE(g->Cpad >= g->C && g->Cpad % 16 == 0, "dfq_i8: Cpad must be a multiple of 16 that holds C");
+  DFQ_REQUIRE(g->OH == (g->H + 2 * g->pad_h - g->dil_h * (g->kh - 1) - 1) / g->stride_h + 1 &&
+                  g->OW == (g->W + 2 * g->pad_w - g->dil_w * (g->kw - 1) - 1) / g->stride_w + 1 && g->OH > 0 && g->OW > 0,
+              "dfq_i8: OH / OW do not follow from the geometry");
+  if (g->groups != 1 && !(g->groups == g->C && g->O == g->C)) {
+    set_error("dfq_i8: unsupported grouping: groups=%d C=%d O=%d (needs groups == 1, or groups == C == O)", g->groups, g->C,
+              g->O);
+    return DFQ_E_UNSUPPORTED;
+  }
+  return 0;
+}
+
+int grid_for(int64_t total, int threads) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count() * 32));
+}
+
+}  // namespace
+}  // namespace dfq
+
+using namespace dfq;
+
+extern "C" int dfq_i8_quantize_nhwc(const float* x, int8_t* q, int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cpad,
+                                    float scale, void* stream) {
+  DFQ_REQUIRE(x && q && N > 0 && C > 0 && H > 0 && W > 0, "dfq_i8_quantize_nhwc: bad arguments");
+  DFQ_REQUIRE(Cpad >= C && Cpad % 16 == 0, "dfq_i8_quantize_nhwc: Cpad must be a multiple of 16 that holds C");
+  DFQ_REQUIRE(aligned16(q), "dfq_i8_quantize_nhwc: q must be 16-byte aligned");
+  const int64_t total = (int64_t)N * (Cpad / 16) * H * W;
+  k_i8_quantize_nhwc<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x, q, C, H * W, Cpad, total, scale);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_pack_weights(const float* w, const float* w_scale, int8_t* packed, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(w && w_scale && packed, "dfq_i8_pack_weights: null pointer");
+  const int taps = g->kh * g->kw;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    const int64_t total = (int64_t)g->O * taps * g->Cpad;
+    k_i8_pack_dense<<<grid_for(total, 256), 256, 0, st>>>(w, w_scale, packed, g->C, taps, g->Cpad, total);
+  } else {
+    k_i8_pack_dw<<<(taps * g->Cpad + 255) / 256, 256, 0, st>>>(w, w_scale, packed, g->C, taps, g->Cpad);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, float* y, int32_t* acc_out,
+                           const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(xq && wq && dq && y, "dfq_i8_conv: null pointer");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv: codes must be 16-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    const int64_t M = (int64_t)g->N * g->OH * g->OW;
+    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_conv: too many output pixels");
+    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, total);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}

@@ -471,6 +471,7 @@ extern "C" int dfq_struct_size(int which) {
     case 5: return (int)sizeof(DfqExpectTerm);
     case 6: return (int)sizeof(DfqBcLayer);
     case 7: return (int)sizeof(DfqQuantTask);
+    case 8: return (int)sizeof(DfqI8Conv);
     default: return -1;
   }
 }

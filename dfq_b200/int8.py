@@ -1,0 +1,182 @@
+"""Int8 execution of calibrated Conv2d / Linear layers on the H100.
+
+The reference's end product is "true int8 inference": convert_ncnn.py:109-201 writes the weight and activation scales
+(128 / max|.|) of a calibrated model into an ncnn table and ncnn's runtime then executes the model in int8 on a CPU.  This
+module runs the same dequantizing int8 convolution on the GPU (include/dfq_b200.h, dfq_i8_*), one layer at a time:
+
+    q(v, s) = clamp(round_half_away(fp32(v * s)), -127, 127)       activations: scale a, weights: w_s[o]
+    y       = fp32(fp32_rn(sum q(x) q(w)) * dq[o]) + bias[o],       dq[o] = fp32(1 / fp32(a * w_s[o]))
+
+Each converted layer takes and returns fp32 NCHW like the module it replaces; ReLU, residual adds, pooling and whatever
+else sits between target layers stay in torch (ncnn keeps its elementwise ops in fp32 too).  Dense layers (groups == 1,
+Linear as a 1x1 convolution) run on the tensor cores; depthwise layers (groups == C == O) on the CUDA cores; any other
+grouping is refused.  There is no CPU fallback.
+
+Order of the calibration steps, as in convert_ncnn.py: BN fold, equalization (and bias correction, if used), activation
+ranges (set_quant_minmax or update_stat), then convert_to_int8 - BEFORE quantize_targ_layer, whose fake-quantized weights
+are not the fp32 weights the int8 codes are made from.  The observers replace_op() installs for functional ops are not used:
+tensors between converted layers stay fp32.
+"""
+import ctypes as C
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from . import _lib, engine, export
+
+_f32 = np.float32
+
+
+def _ptr(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _pair(v):
+    return (int(v), int(v)) if isinstance(v, int) else (int(v[0]), int(v[1]))
+
+
+def dequant_scales(act_scale, w_scale):
+    """dq[o] = fp32(1 / fp32(a * w_s[o])); 0 where a * w_s[o] is 0 (a zero range quantizes to codes 0)."""
+    den = _f32(act_scale) * np.asarray(w_scale, _f32)
+    return np.where(den == 0, _f32(0), _f32(1) / np.where(den == 0, _f32(1), den)).astype(_f32)
+
+
+class _Int8Layer(nn.Module):
+    """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves."""
+
+    def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
+        super().__init__()
+        O, Cg, kh, kw = weight.shape
+        self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
+        self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
+        self.cpad = (self.in_channels + 15) // 16 * 16
+        self.act_scale = float(_f32(act_scale))
+        depthwise = self.groups == self.in_channels == self.out_channels and self.groups > 1
+        if self.groups != 1 and not depthwise:
+            raise _lib.DfqError("int8 execution supports groups == 1 or depthwise (groups == C_in == C_out), got groups=%d "
+                                "C_in=%d C_out=%d" % (self.groups, self.in_channels, self.out_channels))
+        dev = engine._default_device()
+        w_scale = np.broadcast_to(np.asarray(w_scale, _f32), (O,)).copy()
+        taps = kh * kw
+        self.register_buffer("weight_codes", torch.zeros((taps * self.cpad,) if depthwise else (O * taps * self.cpad,),
+                                                         dtype=torch.int8, device=dev))
+        self.register_buffer("w_scale", torch.from_numpy(w_scale).to(dev))
+        self.register_buffer("dq", torch.from_numpy(dequant_scales(self.act_scale, w_scale)).to(dev))
+        b = torch.zeros(O) if bias is None else bias.detach().float()
+        self.register_buffer("bias", b.to(dev).contiguous())
+        w = weight.detach().float().to(dev).contiguous()
+        # geometry of a 1-pixel image: the packer only reads O, C, kh, kw, groups and Cpad
+        g = self._geometry(1, (kh - 1) * self.dilation[0] + 1, (kw - 1) * self.dilation[1] + 1, stride=(1, 1), padding=(0, 0))
+        lib = _lib.load()
+        _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes), _lib.table_ptr(g),
+                                           _lib.stream_ptr()), "dfq_i8_pack_weights")
+
+    def _geometry(self, N, H, W, stride=None, padding=None):
+        (sh, sw), (ph, pw), (dh, dw) = stride or self.stride, padding or self.padding, self.dilation
+        kh, kw = self.kernel_size
+        g = np.zeros(1, _lib.I8_CONV_DT)
+        for k, v in dict(N=N, C=self.in_channels, H=H, W=W, O=self.out_channels, kh=kh, kw=kw, stride_h=sh, stride_w=sw,
+                         pad_h=ph, pad_w=pw, dil_h=dh, dil_w=dw, groups=self.groups,
+                         OH=(H + 2 * ph - dh * (kh - 1) - 1) // sh + 1, OW=(W + 2 * pw - dw * (kw - 1) - 1) // sw + 1,
+                         Cpad=self.cpad).items():
+            g[0][k] = v
+        return g
+
+    def run(self, x, with_acc=False):
+        """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue."""
+        if not x.is_cuda or not self.dq.is_cuda:
+            raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
+                                % (x.device, self.dq.device))
+        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
+            raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s %s" % (self.in_channels, x.dtype, tuple(x.shape)))
+        x = x.contiguous()
+        N, Cn, H, W = x.shape
+        g = self._geometry(N, H, W)
+        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
+        if OH <= 0 or OW <= 0:
+            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        lib, st = _lib.load(), _lib.stream_ptr()
+        xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
+        y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=x.device)
+        acc = torch.empty(y.shape, dtype=torch.int32, device=x.device) if with_acc else None
+        _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, Cn, H, W, self.cpad, C.c_float(self.act_scale), st),
+                   "dfq_i8_quantize_nhwc")
+        _lib.check(lib.dfq_i8_conv(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(y), _ptr(acc),
+                                   _lib.table_ptr(g), st), "dfq_i8_conv")
+        return y, acc
+
+
+class Int8Conv2d(_Int8Layer):
+    """nn.Conv2d executed in int8 (zero padding; groups == 1 or depthwise)."""
+
+    @classmethod
+    def from_conv(cls, conv: nn.Conv2d, act_scale, w_scale):
+        if isinstance(conv.padding, str) or conv.padding_mode != "zeros":
+            raise _lib.DfqError("int8 execution supports numeric zero padding only (padding=%r, padding_mode=%r)"
+                                % (conv.padding, conv.padding_mode))
+        return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
+
+    def forward(self, x):
+        return self.run(x)[0]
+
+    def extra_repr(self):
+        return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act_scale=%g" % (
+            self.in_channels, self.out_channels, self.kernel_size, self.stride, self.padding, self.dilation, self.groups,
+            self.act_scale)
+
+
+class Int8Linear(_Int8Layer):
+    """nn.Linear executed in int8: the 1x1 convolution of [B, I, 1, 1]."""
+
+    @classmethod
+    def from_linear(cls, lin: nn.Linear, act_scale, w_scale):
+        return cls(lin.weight.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias, act_scale, w_scale)
+
+    def forward(self, x):
+        lead = x.shape[:-1]
+        y, _ = self.run(x.reshape(-1, self.in_channels, 1, 1))
+        return y.reshape(*lead, self.out_channels)
+
+    def extra_repr(self):
+        return "in_features=%d, out_features=%d, act_scale=%g" % (self.in_channels, self.out_channels, self.act_scale)
+
+
+def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
+    """Replace every target layer of `graph` (types in targ_type, Conv2d or Linear) inside `model` by its int8 executor, in
+    place (by parent attribute); returns the replaced modules' names in graph order.
+
+    Weight scales are export.ncnn_scales' 128 / max|W|, one per layer repeated per output channel.  Activation scales are
+    ncnn_scales' 128 / max(|running_min|, |running_max|) of each layer's `quant` observer, or act_scales[i] (a list in graph
+    order, one per target layer, e.g. the rows of read_ncnn_table).  A zero range gives scale 0.  Call after equalization /
+    bias correction and the activation ranges, before quantize_targ_layer (module docstring).  A layer that cannot run in
+    int8 raises DfqError naming it, before anything is replaced."""
+    rows = export.ncnn_scales(graph, targ_type, zero_range_ok=True)
+    layers = [graph[k] for k in graph if type(graph[k]) in targ_type]
+    if act_scales is not None and len(act_scales) != len(layers):
+        raise _lib.DfqError("act_scales has %d entries for %d target layers" % (len(act_scales), len(layers)))
+    names = {id(m): n for n, m in model.named_modules()}
+    plan = []
+    for i, (layer, (w_scale, _, a_scale)) in enumerate(zip(layers, rows)):
+        name = names.get(id(layer))
+        if name is None:
+            raise _lib.DfqError("target layer %d (%s) is not a submodule of the model" % (i, type(layer).__name__))
+        a = act_scales[i] if act_scales is not None else a_scale
+        if a is None:
+            raise _lib.DfqError("layer %s has no activation range (no `quant` observer and no act_scales entry)" % name)
+        if isinstance(layer, nn.Conv2d):
+            ok = (layer.groups == 1 or layer.groups == layer.in_channels == layer.out_channels) and \
+                layer.padding_mode == "zeros" and not isinstance(layer.padding, str)
+        else:
+            ok = isinstance(layer, nn.Linear)
+        if not ok:
+            raise _lib.DfqError("layer %s (%s, groups=%s) cannot run in int8: needs a Linear, or a zero-padded Conv2d with "
+                                "groups == 1 or depthwise" % (name, type(layer).__name__, getattr(layer, "groups", "-")))
+        plan.append((name, layer, a, w_scale))
+    done = []
+    for name, layer, a, w_scale in plan:
+        new = (Int8Conv2d.from_conv if isinstance(layer, nn.Conv2d) else Int8Linear.from_linear)(layer, a, w_scale)
+        parent_name, _, attr = name.rpartition(".")
+        setattr(model.get_submodule(parent_name) if parent_name else model, attr, new)
+        done.append(name)
+    return done

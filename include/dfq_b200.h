@@ -43,7 +43,7 @@ enum {
 int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
- * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask): lets a binding verify
+ * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -311,6 +311,41 @@ int dfq_selftest_bc_arithmetic(const float* w, float* eps_fast, float* eps_div, 
 
 /* x = clamp(x, lo, hi) in place (dfq.py:167-170 clip_weight). */
 int dfq_clamp(float* x, int64_t n, float lo, float hi, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Int8 execution of calibrated layers
+ *
+ * The reference's "true int8 inference" writes the scales of convert_ncnn.py:178-201 into an ncnn table and lets ncnn's
+ * runtime execute the model in int8 on a CPU (ncnn2int8, inference_cls.cpp).  These entries run the same dequantizing
+ * int8 convolution on the H100, one layer at a time with fp32 NCHW in and out:
+ *   q(v, s) = clamp(round_half_away(fp32(v * s)), -127, 127)    activations: one scale a; weights: w_s[o] per channel
+ *   acc     = exact int32 sum of q(x) * q(w) over the receptive field (padding contributes 0)
+ *   y       = fp32(fp32_rn(acc) * dq[o]) + bias[o],   dq[o] = fp32(1 / fp32(a * w_s[o]))  (computed by the caller)
+ * Supported: groups == 1 (implicit GEMM on the tensor cores; Linear is the 1x1 case on [B, I, 1, 1]) and depthwise
+ * groups == C == O (CUDA cores).  Any other grouping returns DFQ_E_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct DfqI8Conv {
+  int32_t N, C, H, W;          /* input [N, C, H, W]                                                           */
+  int32_t O, kh, kw;           /* output channels, kernel size                                                 */
+  int32_t stride_h, stride_w;
+  int32_t pad_h, pad_w;        /* zero padding                                                                 */
+  int32_t dil_h, dil_w;
+  int32_t groups;
+  int32_t OH, OW;              /* (H + 2 pad - dil (k - 1) - 1) / stride + 1, checked                          */
+  int32_t Cpad;                /* channel stride of the int8 NHWC codes and packed weights: C rounded up to 16 */
+  int32_t _pad;
+} DfqI8Conv;
+
+/* Activation quantizer: fp32 NCHW x -> int8 NHWC q[N, H, W, Cpad], pad channels 0.  q must be 16-byte aligned. */
+int dfq_i8_quantize_nhwc(const float* x, int8_t* q, int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cpad, float scale,
+                         void* stream);
+/* Weight packer (once per layer, at conversion): fp32 w[O, C/groups, kh, kw] with per-output-channel scales w_scale[O]
+ * -> groups == 1: int8 [O][kh][kw][Cpad]; depthwise: int8 [kh*kw][Cpad].  Pad channels 0.  Uses g's O, C, kh, kw, groups, Cpad. */
+int dfq_i8_pack_weights(const float* w, const float* w_scale, int8_t* packed, const DfqI8Conv* g, void* stream);
+/* Convolution of quantized codes with the epilogue above: xq from dfq_i8_quantize_nhwc, wq from dfq_i8_pack_weights, dq[O],
+ * bias[O] (NULL: none), y fp32 [N, O, OH, OW].  acc_out (NULL: not written) receives the int32 sums, [N, O, OH, OW]. */
+int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, float* y, int32_t* acc_out,
+                const DfqI8Conv* g, void* stream);
 
 #ifdef __cplusplus
 }

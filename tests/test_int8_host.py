@@ -1,0 +1,212 @@
+"""Int8 execution without a GPU: the integer oracle (tests/int8_oracle.py), the reference's int8 ncnn model against the
+calibration this package computes, and the host path of dfq_b200.int8 (packing plan, scale choice, module swap,
+read_ncnn_table) through the oracle-backed fake library."""
+import os
+from collections import OrderedDict
+
+import numpy as np
+import pytest
+import torch
+import torch.nn as nn
+import torch.nn.functional as F
+
+import fakelib
+import fakelib_int8
+import int8_oracle as O
+
+f32 = np.float32
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def test_quantizer_rounds_ties_away_from_zero_and_clamps():
+    s = f32(0.5)
+    v = np.array([1, 3, 5, -1, -3, -5, 253, -253, 255, -255, 1e30, -1e30, 0.0, -0.0], f32)   # v * 0.5 = k + 0.5 exactly
+    assert np.all((v[:10] * s) % 1 == 0.5)
+    got = O.i8_quantize(v, s)
+    assert got.dtype == np.int8
+    assert got.tolist() == [1, 2, 3, -1, -2, -3, 127, -127, 127, -127, 127, -127, 0, 0]
+    # the product is rounded to fp32 first: 0.49999997 * 1 stays below the tie, 2.5 - ulp rounds down
+    assert O.i8_quantize(np.array([np.nextafter(f32(0.5), f32(0)), np.nextafter(f32(2.5), f32(0))], f32), 1.0).tolist() == [0, 2]
+    assert O.i8_quantize(np.array([-128.0, 126.5], f32), 1.0).tolist() == [-127, 127]
+
+
+GRID = [  # (N, C, H, W, O, k, stride, pad, dil, groups)
+    (1, 3, 9, 9, 8, 3, 1, 1, 1, 1), (3, 16, 8, 7, 24, 1, 2, 0, 1, 1), (1, 24, 11, 10, 100, 7, 2, 3, 1, 1),
+    (2, 5, 13, 13, 6, 3, 1, 3, 6, 1), (1, 12, 7, 7, 12, 3, 2, 1, 1, 12), (2, 8, 10, 9, 8, 5, 1, 4, 2, 8),
+    (1, 6, 3, 3, 4, 3, 1, 0, 1, 1), (1, 8, 6, 6, 8, 3, 1, 1, 1, 2),
+]
+
+
+@pytest.mark.parametrize("case", GRID)
+def test_integer_conv_oracle_equals_float64_conv(case):
+    N, Cn, H, W, Oc, k, s, p, d, g = case
+    rng = np.random.default_rng(hash(case) % 2 ** 32)
+    x = rng.integers(-127, 128, (N, Cn, H, W))
+    w = rng.integers(-127, 128, (Oc, Cn // g, k, k))
+    acc = O.i8_conv(x, w, (s, s), (p, p), (d, d), g)
+    ref = F.conv2d(torch.from_numpy(x).double(), torch.from_numpy(w).double(), None, s, p, d, g).numpy()
+    assert acc.dtype == np.int64 and np.array_equal(acc, ref.astype(np.int64))
+
+
+def test_dequant_epilogue_is_two_rounded_fp32_ops():
+    acc = np.array([[[[2 ** 24 + 1]], [[-7]], [[5]]]], np.int64)           # 2^24 + 1 is not an fp32: rounds to even
+    a, ws, b = f32(48.484846), np.array([163.08817, 0.0, 3.0], f32), np.array([0.25, 1.0, -0.0], f32)
+    y = O.i8_dequant(acc, a, ws, b)
+    dq0 = f32(1) / (a * ws[0])
+    assert y[0, 0, 0, 0] == f32(f32(2 ** 24) * dq0) + f32(0.25)
+    assert y[0, 1, 0, 0] == f32(1.0)                                        # zero scale: dq 0, the bias remains
+    assert y[0, 2, 0, 0] == f32(5) * (f32(1) / (a * ws[2]))
+
+
+# ---- the reference's int8 ncnn model -------------------------------------------------------------------------------
+def _staged():
+    import ncnn_int8_case as case
+    import ncnn_table_case
+    if case.paths() is None or ncnn_table_case.checkpoint_path() is None:
+        pytest.skip("reference int8 model / checkpoint not staged in oracle/_ref")
+    return case
+
+
+def test_reference_int8_model_parses_completely():
+    case = _staged()
+    layers = case.parse()
+    assert len(layers) == 53 and sum(l["codes"].size for l in layers) == 3_469_760
+    assert min(int(l["codes"].min()) for l in layers) == -127                  # never -128: the clamp is +-127
+    rows = np.load(os.path.join(GOLD, "ncnn_table_rows.npz"))
+    assert np.array_equal(np.array([l["w_scales"][0] for l in layers]), rows["weight_scales"].astype(f32))
+    assert np.abs(np.array([l["in_scale"] for l in layers]) / rows["activation_scales"] - 1).max() < 1e-6
+
+
+def test_reference_codes_and_biases_from_this_calibration(monkeypatch):
+    """Oracle-calibrated weights (BN fold + signed CLE on the bundled checkpoint) quantized with the table's weight scales
+    reproduce the reference's int8 codes but for last-bit weight differences (DESIGN.md section 4); its biases agree."""
+    case = _staged()
+    fakelib.install(monkeypatch, fakelib.torch_sqrt)
+    graph, targ = case.calibrated_graph(monkeypatch)
+    layers = [graph[k] for k in graph if type(graph[k]) in targ]
+    ref = case.parse()
+    rows = np.load(os.path.join(GOLD, "ncnn_table_rows.npz"))
+    same = total = 0
+    worst_bias = 0.0
+    for m, r, ws in zip(layers, ref, rows["weight_scales"]):
+        codes = O.i8_quantize(m.weight.detach().numpy().reshape(-1), f32(ws)).astype(np.int16)
+        d = np.abs(codes - r["codes"].astype(np.int16))
+        assert d.max() <= 1, r["name"]
+        same += int((d == 0).sum()); total += d.size
+        b = m.bias.detach().numpy()
+        worst_bias = max(worst_bias, float(np.abs(b - r["bias"]).max() / np.abs(b).max()))
+    print("reference int8 codes reproduced: %d of %d; worst bias error %.3g of the layer's max|bias|" % (same, total, worst_bias))
+    assert total == 3_469_760 and same >= 3_469_750
+    assert worst_bias < 2e-6
+
+
+# ---- host path of dfq_b200.int8 ------------------------------------------------------------------------------------
+class _Net(nn.Module):
+    def __init__(self):
+        super().__init__()
+        self.features = nn.Sequential(nn.Conv2d(3, 16, 3, 2, 1), nn.ReLU(), nn.Conv2d(16, 16, 3, 1, 2, 2, groups=16), nn.ReLU())
+        self.head = nn.Linear(16, 10)
+
+    def forward(self, x):
+        return self.head(self.features(x).mean((2, 3)))
+
+
+def _graph(model):
+    """The target-layer nodes of the tracer's graph (keys id(module), graph order) - all that the converter reads."""
+    return OrderedDict((id(m), m) for m in model.modules() if isinstance(m, (nn.Conv2d, nn.Linear)))
+
+
+def test_convert_to_int8_packs_scales_and_swaps_through_the_fake_library(monkeypatch):
+    from dfq_b200 import _lib, int8
+    fake = fakelib_int8.install(monkeypatch)
+    torch.manual_seed(0)
+    model = _Net().eval()
+    w = [model.features[0].weight, model.features[2].weight, model.head.weight]
+    with torch.no_grad():
+        model.features[2].weight[3].zero_()                                    # a zero channel packs to zeros
+    graph = _graph(model)
+    targ = [nn.Conv2d, nn.Linear]
+    acts = [40.0, 12.5, 3.0]
+    ws_ref = [f32(128. / float(t.detach().abs().max())) for t in w]
+    names = int8.convert_to_int8(model, graph, targ, act_scales=acts)
+    assert names == ["features.0", "features.2", "head"]
+    assert isinstance(model.features[0], int8.Int8Conv2d) and isinstance(model.features[2], int8.Int8Conv2d)
+    assert isinstance(model.head, int8.Int8Linear) and fake.calls.count("dfq_i8_pack_weights") == 3
+    dense, dw, fc = model.features[0], model.features[2], model.head
+    assert dense.cpad == 16 and dw.cpad == 16 and fc.cpad == 16
+    codes = dense.weight_codes.numpy().reshape(16, 3, 3, 16)                   # [O][kh][kw][Cpad]
+    assert np.array_equal(codes[..., :3], O.i8_quantize(w[0].detach().numpy(), ws_ref[0]).transpose(0, 2, 3, 1))
+    assert not codes[..., 3:].any()
+    dcodes = dw.weight_codes.numpy().reshape(9, 16)                            # [kh*kw][Cpad]
+    assert np.array_equal(dcodes, O.i8_quantize(w[1].detach().numpy(), ws_ref[1]).reshape(16, 9).T)
+    assert not dcodes[:, 3].any()
+    for mod, a, ws in zip((dense, dw, fc), acts, ws_ref):
+        assert mod.act_scale == float(f32(a)) and np.all(mod.w_scale.numpy() == ws)
+        assert np.array_equal(mod.dq.numpy(), (f32(1) / (f32(a) * np.full(mod.out_channels, ws, f32))).astype(f32))
+    with pytest.raises(_lib.DfqError, match="GPU"):
+        model(torch.randn(1, 3, 8, 8))
+
+
+def test_convert_to_int8_uses_the_observers_and_refuses_what_it_cannot_run(monkeypatch):
+    from dfq_b200 import _lib, export, int8
+    from dfq_b200.utils import quantize as Q
+    fakelib_int8.install(monkeypatch)
+    model = nn.Sequential(Q.QuantNConv2d(8, 16, 3, padding=1), nn.ReLU(), Q.QuantNConv2d(16, 16, 1, groups=2))
+    graph = _graph(model)
+    targ = [Q.QuantNConv2d]
+    for m, (lo, hi) in zip((model[0], model[2]), ((-2.0, 3.2), (0.0, 0.0))):
+        m.quant.running_min.fill_(lo); m.quant.running_max.fill_(hi)
+    with pytest.raises(_lib.DfqError, match=r"layer 2 .*cannot run in int8"):
+        int8.convert_to_int8(model, graph, targ)
+    assert isinstance(model[0], Q.QuantNConv2d)                                # nothing replaced
+    with pytest.raises(_lib.DfqError, match="act_scales has 1 entries"):
+        int8.convert_to_int8(model, graph, targ, act_scales=[1.0])
+    model2 = nn.Sequential(Q.QuantNConv2d(8, 16, 3, padding=1), nn.ReLU(), Q.QuantNConv2d(16, 16, 1))
+    model2[0].quant.running_min.fill_(-2.0); model2[0].quant.running_max.fill_(3.2)      # model2[2]: zero range
+    g2 = _graph(model2)
+    assert int8.convert_to_int8(model2, g2, targ) == ["0", "2"]
+    assert model2[0].act_scale == float(f32(128. / 3.2)) and model2[2].act_scale == 0.0
+    with pytest.raises(ZeroDivisionError):                                     # export's default is unchanged
+        export.ncnn_scales(g2, targ)
+    assert not model2[2].dq.numpy().any()
+    with pytest.raises(_lib.DfqError, match="no activation range"):
+        m3 = nn.Sequential(nn.Conv2d(4, 4, 1))
+        int8.convert_to_int8(m3, _graph(m3), [nn.Conv2d])
+
+
+def test_fake_library_runs_the_abi_end_to_end(monkeypatch):
+    """The three entries' host twins compose: quantize -> pack -> conv equals the oracle chain (a CPU rehearsal of the -m gpu
+    tests' comparison)."""
+    from dfq_b200 import int8
+    fakelib_int8.install(monkeypatch)
+    torch.manual_seed(1)
+    conv = nn.Conv2d(5, 7, 3, 2, 1)
+    layer = int8.Int8Conv2d.from_conv(conv, 30.0, f32(128. / float(conv.weight.abs().max())))
+    monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True))
+    x = torch.randn(2, 5, 9, 8)
+    y, acc = layer.run(x, with_acc=True)
+    xq = O.i8_quantize(x.numpy(), f32(30.0))
+    wq = O.i8_quantize(conv.weight.detach().numpy(), layer.w_scale.numpy()[0])
+    ref_acc = O.i8_conv(xq, wq, (2, 2), (1, 1), (1, 1), 1)
+    assert np.array_equal(acc.numpy(), ref_acc)
+    assert np.array_equal(y.numpy(), O.i8_dequant(ref_acc, 30.0, layer.w_scale.numpy(), conv.bias.detach().numpy()))
+
+
+def test_read_ncnn_table_inverts_write_ncnn_table(monkeypatch, tmp_path):
+    from dfq_b200 import export
+    from dfq_b200.utils import quantize as Q
+    fakelib_int8.install(monkeypatch)
+    torch.manual_seed(2)
+    model = nn.Sequential(Q.QuantNConv2d(3, 8, 3), nn.ReLU(), Q.QuantNConv2d(8, 4, 1), nn.Flatten(), Q.QuantNLinear(4 * 4, 3))
+    for i, m in enumerate((model[0], model[2], model[4])):
+        m.quant.running_min.fill_(-1.0 - i); m.quant.running_max.fill_(0.5 + 3 * i)
+    graph = _graph(model)
+    path = str(tmp_path / "t.table")
+    rows = export.write_ncnn_table(graph, path, [Q.QuantNConv2d, Q.QuantNLinear], ["a", "b", "c"])
+    names, back = export.read_ncnn_table(path)
+    assert names == ["a", "b", "c"] and back == rows
+    with open(path, "a") as f:
+        f.write("d_param_0 1.0 2.0\n")
+    with pytest.raises(ValueError, match="differ"):
+        export.read_ncnn_table(path)
+

@@ -1,0 +1,151 @@
+"""Throughput of int8 execution (dfq_b200.int8) on the H100: prints one JSON line.
+
+    python tools/bench_int8.py [--batch 256] [--reps 10]
+
+images/s of torchvision MobileNetV2 and ResNet-18 (seeded weights, 224x224) run three ways - int8 execution, the fake-quant path
+of the reference's QuantN* layers, plain fp32 with TF32 off - and the achieved int8 TOPS of dfq_i8_conv on ResNet-18's largest
+GEMM layers against the data-sheet dense peak.  The card's name and power limit are read in the same run and reported beside
+the numbers.  Needs a CUDA device; writes nothing.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+
+
+def int8_inference(dev, reps=10, batch=256):
+    """images/s of int8 execution (dfq_b200.int8) vs the fake-quant path (QuantN* layers) vs fp32 with TF32 off, for
+    torchvision MobileNetV2 and ResNet-18 (seeded weights, batch 256, 224x224), and the achieved int8 TOPS of dfq_i8_conv
+    on ResNet-18's largest GEMM layers against the data-sheet dense peak."""
+    import copy
+    import ctypes as C
+    import torch
+    import torch.nn as nn
+    import torchvision
+    from dfq_b200 import _lib, int8
+    from dfq_b200.utils import quantize as Q
+
+    def timed(fn):
+        for _ in range(2):
+            fn()
+        torch.cuda.synchronize(dev)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def fake_quant(model, amax):
+        for name, m in list(model.named_modules()):
+            if type(m) in (nn.Conv2d, nn.Linear):
+                q = (Q.QuantNConv2d(m.in_channels, m.out_channels, m.kernel_size, m.stride, m.padding, m.dilation, m.groups,
+                                    m.bias is not None) if isinstance(m, nn.Conv2d) else
+                     Q.QuantNLinear(m.in_features, m.out_features, m.bias is not None)).to(dev).eval()
+                q.load_state_dict(m.state_dict(), strict=False)
+                q.quant.running_min.fill_(-amax[name]); q.quant.running_max.fill_(amax[name])
+                parent, _, attr = name.rpartition(".")
+                setattr(model.get_submodule(parent) if parent else model, attr, q)
+        return model
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps}
+    try:
+        x = torch.randn(batch, 3, 224, 224, device=dev)
+        for net in ("mobilenet_v2", "resnet18"):
+            torch.manual_seed(0)
+            fp32 = getattr(torchvision.models, net)(num_classes=1000).to(dev).eval()
+            graph, amax, hooks = {}, {}, []
+            for name, m in fp32.named_modules():
+                if type(m) in (nn.Conv2d, nn.Linear):
+                    graph[id(m)] = m
+                    hooks.append(m.register_forward_pre_hook(
+                        lambda m, i, name=name: amax.__setitem__(name, max(amax.get(name, 0.0), float(i[0].abs().max())))))
+            with torch.no_grad():
+                fp32(x[:32])
+            for h in hooks:
+                h.remove()
+            fq = fake_quant(copy.deepcopy(fp32), amax)
+            i8 = copy.deepcopy(fp32)
+            graph = {id(m): m for n, m in i8.named_modules() if type(m) in (nn.Conv2d, nn.Linear)}
+            int8.convert_to_int8(i8, graph, [nn.Conv2d, nn.Linear], act_scales=[128. / amax[n] for n, m in fp32.named_modules()
+                                                                                 if type(m) in (nn.Conv2d, nn.Linear)])
+            with torch.no_grad():
+                ms = {k: timed(lambda mod=mod: mod(x)) for k, mod in (("int8", i8), ("fake_quant", fq), ("fp32_no_tf32", fp32))}
+                top1 = float((i8(x[:64]).argmax(1) == fq(x[:64]).argmax(1)).float().mean())
+            out[net] = {k: batch / (v * 1e-3) for k, v in ms.items()}
+            out[net]["ms_per_batch"] = ms
+            out[net]["top1_agreement_int8_vs_fake_quant_64_random_images"] = top1
+            if net == "resnet18":
+                lib, layers = _lib.load(), []
+                shapes = {}
+                hooks = [m.register_forward_pre_hook(lambda m, i: shapes.__setitem__(id(m), tuple(i[0].shape)))
+                         for m in i8.modules() if isinstance(m, int8.Int8Conv2d)]
+                with torch.no_grad():
+                    i8(x)
+                for h in hooks:
+                    h.remove()
+                for name, m in i8.named_modules():
+                    if isinstance(m, int8.Int8Conv2d):
+                        N, Cn, H, W = shapes[id(m)]
+                        g = m._geometry(N, H, W)
+                        M = N * int(g[0]["OH"]) * int(g[0]["OW"])
+                        K = m.kernel_size[0] * m.kernel_size[1] * m.cpad
+                        layers.append((2 * M * m.out_channels * K, name, m, g, (N, Cn, H, W)))
+                tops = []
+                for ops, name, m, g, shp in sorted(layers, key=lambda t: -t[0])[:4]:
+                    xq = torch.zeros(shp[0] * shp[2] * shp[3] * m.cpad, dtype=torch.int8, device=dev)
+                    y = torch.empty(shp[0], m.out_channels, int(g[0]["OH"]), int(g[0]["OW"]), device=dev)
+                    st = _lib.stream_ptr()
+                    call = lambda: lib.dfq_i8_conv(C.c_void_p(xq.data_ptr()), C.c_void_p(m.weight_codes.data_ptr()),
+                                                   C.c_void_p(m.dq.data_ptr()), C.c_void_p(m.bias.data_ptr()),
+                                                   C.c_void_p(y.data_ptr()), None, _lib.table_ptr(g), st)
+                    t = timed(call)
+                    tops.append({"layer": name, "input": list(shp), "out_channels": m.out_channels, "gemm_ops": ops,
+                                 "ms": t, "TOPS": ops / (t * 1e-3) / 1e12})
+                out["resnet18_largest_gemm_layers"] = {
+                    "kernel": "k_i8_conv_mma (dfq_i8_conv, mma.sync m16n8k32 s8; epilogue and fp32 NCHW store included)",
+                    "layers": tops, "datasheet_peak_int8_dense_TOPS": 1979.0,
+                    "peak_note": "NVIDIA H100 SXM data-sheet figure (700 W), not a measured peak"}
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
+
+def card():
+    """Name and power limit of the GPU (read only)."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30)
+        if q.returncode == 0:
+            out["power_limit_and_max_sm_clock"] = q.stdout.strip()
+    except (OSError, subprocess.TimeoutExpired):
+        pass
+    return out
+
+
+def main():
+    p = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    p.add_argument("--batch", type=int, default=256)
+    p.add_argument("--reps", type=int, default=10, help="timed forward passes per arm (after 2 warm-up passes)")
+    args = p.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_int8.py needs a CUDA device (H100)")
+    dev = torch.device("cuda", 0)
+    res = int8_inference(dev, reps=args.reps, batch=args.batch)
+    res["gpu"] = card()
+    print(json.dumps({"int8": res}))
+
+
+if __name__ == "__main__":
+    main()
