@@ -42,6 +42,19 @@ def dequant_scales(act_scale, w_scale):
     return np.where(den == 0, _f32(0), _f32(1) / np.where(den == 0, _f32(1), den)).astype(_f32)
 
 
+def check_scale(what, scale, layer):
+    """Refuse an activation or weight scale (128 / range) that is not a finite, non-negative fp32 number.  A range below about
+    3.8e-37 gives a scale that is inf in fp32, and inf * 0 would quantize every zero input to NaN and then to -127."""
+    s = np.asarray(scale, np.float64).reshape(-1)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        s32 = s.astype(_f32)
+        bad = ~np.isfinite(s32) | (s32 < 0)
+        if bad.any():
+            i = int(np.argmax(bad))
+            raise _lib.DfqError("layer %s: %s scale %g%s (range 128 / scale = %g) is not a finite non-negative fp32 number"
+                                % (layer, what, float(s[i]), " of channel %d" % i if s.size > 1 else "", 128. / s[i]))
+
+
 class _Int8Layer(nn.Module):
     """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves."""
 
@@ -51,6 +64,9 @@ class _Int8Layer(nn.Module):
         self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
         self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
         self.cpad = (self.in_channels + 15) // 16 * 16
+        who = "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, int(O), self.kernel_size)
+        check_scale("activation", act_scale, who)
+        check_scale("weight", w_scale, who)
         self.act_scale = float(_f32(act_scale))
         depthwise = self.groups == self.in_channels == self.out_channels and self.groups > 1
         if self.groups != 1 and not depthwise:
@@ -150,7 +166,8 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
     ncnn_scales' 128 / max(|running_min|, |running_max|) of each layer's `quant` observer, or act_scales[i] (a list in graph
     order, one per target layer, e.g. the rows of read_ncnn_table).  A zero range gives scale 0.  Call after equalization /
     bias correction and the activation ranges, before quantize_targ_layer (module docstring).  A layer that cannot run in
-    int8 raises DfqError naming it, before anything is replaced."""
+    int8, or whose activation or weight scale is not a finite non-negative fp32 number (check_scale), raises DfqError naming
+    it, before anything is replaced."""
     rows = export.ncnn_scales(graph, targ_type, zero_range_ok=True)
     layers = [graph[k] for k in graph if type(graph[k]) in targ_type]
     if act_scales is not None and len(act_scales) != len(layers):
@@ -164,6 +181,8 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
         a = act_scales[i] if act_scales is not None else a_scale
         if a is None:
             raise _lib.DfqError("layer %s has no activation range (no `quant` observer and no act_scales entry)" % name)
+        check_scale("activation", a, name)
+        check_scale("weight", w_scale, name)
         if isinstance(layer, nn.Conv2d):
             ok = (layer.groups == 1 or layer.groups == layer.in_channels == layer.out_channels) and \
                 layer.padding_mode == "zeros" and not isinstance(layer.padding, str)

@@ -1,7 +1,7 @@
 """CPU guards of the GPU boundary tests.
 
-* The kernel constants the boundary cases of tests/test_gpu_engine.py were built around: a retune must fail here, loudly,
-  instead of quietly moving every case off its boundary.
+* The kernel constants the boundary cases of tests/test_gpu_engine.py and tests/test_gpu_int8.py were built around: a
+  retune must fail here, loudly, instead of quietly moving every case off its boundary.
 * The per-row acceptance bound of bias correction (oracle.dfq_oracle.bias_delta_bound) accepts the oracle's own deltas and
   rejects errors that a normwise gate over the whole layer lets through."""
 import os
@@ -24,6 +24,12 @@ CONSTANTS = {
     "DFQ_SUB_ITEMS": ("cle_engine.cu", 8),
     "kExpectCache": ("passes.cu", 2048),
     "kBcExCols": ("bc_stream.cuh", 512),
+    # k_i8_conv_mma's CTA tile and ring (tests/test_gpu_int8.py TILES)
+    "BM": ("int8_conv.cu", 128),
+    "BN": ("int8_conv.cu", 64),
+    "BK": ("int8_conv.cu", 64),
+    "STAGES": ("int8_conv.cu", 3),
+    "THREADS": ("int8_conv.cu", 128),
 }
 
 
@@ -32,8 +38,14 @@ def _source_value(fname, name):
         src = f.read()
     m = (re.search(r"^\s*#define\s+%s\s+([^\s/]+)" % name, src, re.M)
          or re.search(r"constexpr\s+[\w:]+\s+%s\s*=\s*([^;]+);" % name, src))
-    assert m, "%s not found in %s" % (name, fname)
-    expr = m.group(1).strip()
+    expr = m.group(1) if m else None
+    if expr is None or "," in expr:                 # one name of a list: constexpr int BM = 128, BN = 64, ...;
+        for decl in re.findall(r"constexpr\s+[\w:]+\s+([^;]+);", src):
+            items = [i.split("=", 1) for i in decl.split(",")]
+            if all(len(i) == 2 for i in items):
+                expr = {k.strip(): v for k, v in items}.get(name, expr)
+    assert expr is not None, "%s not found in %s" % (name, fname)
+    expr = expr.strip()
     assert re.fullmatch(r"[0-9 *+()]+", expr), "%s = %r is not a plain integer expression" % (name, expr)
     return eval(expr)
 
@@ -43,6 +55,27 @@ def test_kernel_constants_match_the_boundary_cases(name):
     fname, want = CONSTANTS[name]
     assert _source_value(fname, name) == want, \
         "%s changed: move the boundary cases of tests/test_gpu_engine.py that are built from it, then update this table" % name
+
+
+def test_source_value_reads_one_name_of_a_constexpr_list():
+    with open(os.path.join(CSRC, "int8_conv.cu")) as f:
+        assert "constexpr int BM = 128, BN = 64, BK = 64, STAGES = 3, THREADS = 128;" in f.read()
+    assert [_source_value("int8_conv.cu", n) for n in ("BN", "STAGES")] == [64, 3]
+
+
+def test_int8_tile_cases_cover_both_sides_of_every_tile_size():
+    """tests/test_gpu_int8.py TILES: M = N*OH*OW around BM, O around BN and 2 BN, C around 16 and BK, KT = 1 to STAGES + 1,
+    and an image boundary inside an M tile."""
+    import test_gpu_int8 as G
+    bm, bn, bk, stages = (CONSTANTS[k][1] for k in ("BM", "BN", "BK", "STAGES"))
+    assert G.TILE_EDGES == dict(M={1, 31, bm - 1, bm, bm + 1}, O={1, 7, 9, bn - 1, bn, bn + 1, 2 * bn + 1},
+                                C={1, 15, 16, 17, bk, bk + 1}, KT=set(range(1, stages + 2)))
+    geo = [G.tile_geometry(c) for c in G.TILES]
+    for i, key in enumerate(("M", "O", "C", "KT")):
+        assert G.TILE_EDGES[key] <= {g[i] for g in geo}, key
+    # an M tile holding the last pixels of one image and the first of the next
+    assert any(c[0] > 1 and any((m0 // (g[0] // c[0])) != ((min(m0 + bm, g[0]) - 1) // (g[0] // c[0]))
+                                for m0 in range(0, g[0], bm)) for c, g in zip(G.TILES, geo))
 
 
 def test_scan_columns_derive_from_the_inverse_cache():

@@ -30,22 +30,42 @@ def test_quantizer_rounds_ties_away_from_zero_and_clamps():
     assert O.i8_quantize(np.array([-128.0, 126.5], f32), 1.0).tolist() == [-127, 127]
 
 
-GRID = [  # (N, C, H, W, O, k, stride, pad, dil, groups)
+def _pair(v):
+    return (v, v) if isinstance(v, int) else tuple(v)
+
+
+GRID = [  # (N, C, H, W, O, k, stride, pad, dil, groups); k / stride / pad / dil: an int, or (h, w)
     (1, 3, 9, 9, 8, 3, 1, 1, 1, 1), (3, 16, 8, 7, 24, 1, 2, 0, 1, 1), (1, 24, 11, 10, 100, 7, 2, 3, 1, 1),
     (2, 5, 13, 13, 6, 3, 1, 3, 6, 1), (1, 12, 7, 7, 12, 3, 2, 1, 1, 12), (2, 8, 10, 9, 8, 5, 1, 4, 2, 8),
     (1, 6, 3, 3, 4, 3, 1, 0, 1, 1), (1, 8, 6, 6, 8, 3, 1, 1, 1, 2),
+    # off the square: every pair below has different h and w values, so a swapped axis changes the sums
+    (2, 5, 9, 11, 7, (1, 7), 1, (0, 3), 1, 1), (1, 6, 11, 8, 6, (7, 1), 1, (3, 0), 1, 6),             # 1x7 dense, 7x1 dw
+    (2, 4, 10, 13, 5, (3, 5), (2, 1), (1, 2), (1, 2), 1), (1, 9, 12, 10, 9, (3, 5), (2, 1), (1, 2), (1, 2), 9),
+    (1, 3, 13, 14, 4, (5, 3), (1, 3), 0, (2, 1), 1), (2, 7, 13, 14, 7, (5, 3), (1, 3), 0, (2, 1), 7),
+    (2, 10, 5, 6, 10, 1, (1, 2), 0, 1, 10),                                                           # 1x1 dw
+    (2, 6, 7, 5, 8, (2, 3), (3, 2), (2, 1), (2, 1), 2),                                               # grouped
 ]
 
 
 @pytest.mark.parametrize("case", GRID)
 def test_integer_conv_oracle_equals_float64_conv(case):
     N, Cn, H, W, Oc, k, s, p, d, g = case
+    k, s, p, d = map(_pair, (k, s, p, d))
     rng = np.random.default_rng(hash(case) % 2 ** 32)
     x = rng.integers(-127, 128, (N, Cn, H, W))
-    w = rng.integers(-127, 128, (Oc, Cn // g, k, k))
-    acc = O.i8_conv(x, w, (s, s), (p, p), (d, d), g)
+    w = rng.integers(-127, 128, (Oc, Cn // g) + k)
+    acc = O.i8_conv(x, w, s, p, d, g)
     ref = F.conv2d(torch.from_numpy(x).double(), torch.from_numpy(w).double(), None, s, p, d, g).numpy()
-    assert acc.dtype == np.int64 and np.array_equal(acc, ref.astype(np.int64))
+    assert acc.dtype == np.int64 and acc.shape == ref.shape and np.array_equal(acc, ref.astype(np.int64))
+
+
+def test_quantizer_maps_nan_products_to_minus_127():
+    """NaN (a NaN input, inf * 0, 0 * inf) -> -127 like the kernel's fminf(fmaxf(NaN, -127), 127); +-inf and products that
+    overflow fp32 clamp to +-127; subnormal inputs are not flushed: 1e-38 * 3e38 = 3."""
+    v = np.array([np.nan, -np.nan, np.inf, -np.inf, 0.0, 1e30, -1e30, 1.1e-38, -1.1e-38], f32)
+    s = np.array([1.0, 1.0, 0.0, 0.0, np.inf, 1e10, 1e10, 3e38, 3e38], f32)
+    assert O.i8_quantize(v, s).tolist() == [-127, -127, -127, -127, -127, 127, -127, 3, -3]
+    assert O.i8_quantize(np.array([np.nan, 2.0], f32), f32(np.nan)).tolist() == [-127, -127]
 
 
 def test_dequant_epilogue_is_two_rounded_fp32_ops():
@@ -98,6 +118,69 @@ def test_reference_codes_and_biases_from_this_calibration(monkeypatch):
     print("reference int8 codes reproduced: %d of %d; worst bias error %.3g of the layer's max|bias|" % (same, total, worst_bias))
     assert total == 3_469_760 and same >= 3_469_750
     assert worst_bias < 2e-6
+
+
+def test_interpreter_walks_all_112_layers_in_the_order_of_the_topology():
+    """Int8Net consumes every layer of the .param; its Convolution / ConvolutionDepthWise / InnerProduct sequence is the 53
+    target layers of topology_mobilenetv2.json, in order and geometry."""
+    import json
+    case = _staged()
+    net = case.Int8Net()
+    assert len(net.layers) == 112 and len(net.specs) == 53
+    topo = json.load(open(os.path.join(GOLD, "topology_mobilenetv2.json")))
+    targets = [n for n in topo["nodes"] if n["type"] in ("Conv2d", "Linear")]
+    assert len(targets) == 53
+    for s, n in zip(net.specs, targets):
+        a = n["args"]
+        if n["type"] == "Linear":
+            got = (s["type"], s["C"], s["O"], s["k"], s["groups"])
+            assert got == ("InnerProduct", a["in_features"], a["out_features"], (1, 1), 1), s["name"]
+        else:
+            assert s["type"] == ("ConvolutionDepthWise" if a["groups"] > 1 else "Convolution"), s["name"]
+            assert (s["C"], s["O"], s["groups"]) == (a["in_channels"], a["out_channels"], a["groups"]), s["name"]
+            assert (s["k"], s["stride"], s["pad"], s["dilation"]) == tuple(tuple(a[k]) for k in (
+                "kernel_size", "stride", "padding", "dilation")), s["name"]
+
+
+def test_interpreter_refuses_what_it_does_not_implement(monkeypatch):
+    case = _staged()
+    layers = case.parse_param()
+    for edit, msg in ((lambda l: l[4]["params"].__setitem__(11, 5), r"keys \[11\]"),
+                      (lambda l: l[4].__setitem__("type", "Pooling"), "type Pooling"),
+                      (lambda l: [x for x in l if x["type"] == "BinaryOp"][0]["params"].__setitem__(0, 2), "BinaryOp")):
+        changed = [dict(x, params=dict(x["params"])) for x in layers]
+        edit(changed)
+        monkeypatch.setattr(case, "parse_param", lambda changed=changed: changed)
+        with pytest.raises(NotImplementedError, match=msg):
+            case.Int8Net()
+
+
+def test_reference_int8_mobilenetv2_rehearsal_on_the_cpu(monkeypatch):
+    """The comparisons of the -m gpu end-to-end tests with the oracle executor and the oracle-backed library: the
+    reference's int8 model and this package's calibration converted to int8 against the calibrated fp32 model.  The
+    thresholds are test_gpu_int8.py's (measured here: 0.26-0.27, 0.10, top-1 4 of 4)."""
+    import test_gpu_int8 as G
+    from dfq_b200 import int8
+    case = _staged()
+    net = case.Int8Net()
+    fakelib_int8.install(monkeypatch, fakelib.torch_sqrt)
+    graph, targ = case.calibrated_graph(monkeypatch)
+    layers = [graph[k] for k in graph if type(graph[k]) in targ]
+    x = G._ref_images()
+    with torch.no_grad():
+        fp32 = net.forward(x, case.fp32_executor(layers))["781"]
+        theirs = net.forward(x, case.oracle_executor)["781"]
+        holder = nn.ModuleList(layers)
+        rows = np.load(os.path.join(GOLD, "ncnn_table_rows.npz"))
+        int8.convert_to_int8(holder, graph, targ, act_scales=list(rows["activation_scales"]))
+        monkeypatch.setattr(torch.Tensor, "is_cuda", property(lambda self: True))
+        ours = net.forward(x, lambda s, v: holder[s["index"]].run(v)[0])["781"]
+    top1 = lambda a, b: float((a.argmax(1) == b.argmax(1)).float().mean())
+    print("int8 vs fp32: reference codes %.4g, this calibration %.4g; this calibration vs reference codes %.4g" % (
+        G._rel(theirs, fp32), G._rel(ours, fp32), G._rel(ours, theirs)))
+    assert G._rel(theirs, fp32) < G.INT8_VS_FP32_REL and G._rel(ours, fp32) < G.INT8_VS_FP32_REL
+    assert G._rel(ours, theirs) < G.PKG_VS_REF_REL
+    assert top1(theirs, fp32) >= G.TOP1_AGREE and top1(ours, fp32) >= G.TOP1_AGREE
 
 
 # ---- host path of dfq_b200.int8 ------------------------------------------------------------------------------------
@@ -210,3 +293,27 @@ def test_read_ncnn_table_inverts_write_ncnn_table(monkeypatch, tmp_path):
     with pytest.raises(ValueError, match="differ"):
         export.read_ncnn_table(path)
 
+
+
+@pytest.mark.parametrize("bad", [float("inf"), float("nan"), -2.0, 1.28e40])
+def test_non_finite_or_negative_scales_are_refused(monkeypatch, bad):
+    """128 / range of a range below about 3.8e-37 is inf in fp32: refused, by the layer and by the converter, naming the
+    layer and the range, before anything is replaced."""
+    from dfq_b200 import _lib, int8
+    from dfq_b200.utils import quantize as Q
+    fakelib_int8.install(monkeypatch)
+    conv = nn.Conv2d(4, 6, 3)
+    with pytest.raises(_lib.DfqError, match=r"activation scale .*\(range 128 / scale"):
+        int8.Int8Conv2d.from_conv(conv, bad, 1.0)
+    ws = np.ones(6, f32)
+    ws[4] = bad
+    with pytest.raises(_lib.DfqError, match="weight scale .* of channel 4"):
+        int8.Int8Conv2d.from_conv(conv, 1.0, ws)
+    model = nn.Sequential(Q.QuantNConv2d(4, 8, 3, padding=1), nn.ReLU(), Q.QuantNConv2d(8, 8, 1))
+    model[0].quant.running_min.fill_(-1.0); model[0].quant.running_max.fill_(1.0)
+    model[2].quant.running_min.fill_(0.0); model[2].quant.running_max.fill_(1e-38)        # 128 / 1e-38: inf in fp32
+    with pytest.raises(_lib.DfqError, match=r"layer 2: activation scale 1.28e\+40 \(range 128 / scale = 1e-38\)"):
+        int8.convert_to_int8(model, _graph(model), [Q.QuantNConv2d])
+    with pytest.raises(_lib.DfqError, match="layer 0: activation scale"):
+        int8.convert_to_int8(model, _graph(model), [Q.QuantNConv2d], act_scales=[bad, 1.0])
+    assert isinstance(model[0], Q.QuantNConv2d) and isinstance(model[2], Q.QuantNConv2d)   # nothing replaced

@@ -4,8 +4,9 @@
 
 images/s of torchvision MobileNetV2 and ResNet-18 (seeded weights, 224x224) run three ways - int8 execution, the fake-quant path
 of the reference's QuantN* layers, plain fp32 with TF32 off - and the achieved int8 TOPS of dfq_i8_conv on ResNet-18's largest
-GEMM layers against the data-sheet dense peak.  The card's name and power limit are read in the same run and reported beside
-the numbers.  Needs a CUDA device; writes nothing.
+GEMM layers against the data-sheet dense peak, and the relative logit error (2-norm over 64 random images) of int8 and of
+fake-quant against fp32.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a
+CUDA device; writes nothing.
 """
 import argparse
 import json
@@ -20,8 +21,8 @@ if ROOT not in sys.path:
 
 def int8_inference(dev, reps=10, batch=256):
     """images/s of int8 execution (dfq_b200.int8) vs the fake-quant path (QuantN* layers) vs fp32 with TF32 off, for
-    torchvision MobileNetV2 and ResNet-18 (seeded weights, batch 256, 224x224), and the achieved int8 TOPS of dfq_i8_conv
-    on ResNet-18's largest GEMM layers against the data-sheet dense peak."""
+    torchvision MobileNetV2 and ResNet-18 (seeded weights, batch 256, 224x224), their relative logit errors against fp32, and
+    the achieved int8 TOPS of dfq_i8_conv on ResNet-18's largest GEMM layers against the data-sheet dense peak."""
     import copy
     import ctypes as C
     import torch
@@ -78,10 +79,11 @@ def int8_inference(dev, reps=10, batch=256):
                                                                                  if type(m) in (nn.Conv2d, nn.Linear)])
             with torch.no_grad():
                 ms = {k: timed(lambda mod=mod: mod(x)) for k, mod in (("int8", i8), ("fake_quant", fq), ("fp32_no_tf32", fp32))}
-                top1 = float((i8(x[:64]).argmax(1) == fq(x[:64]).argmax(1)).float().mean())
+                ref = fp32(x[:64])
+                err = {k: float((mod(x[:64]) - ref).norm() / ref.norm()) for k, mod in (("int8", i8), ("fake_quant", fq))}
             out[net] = {k: batch / (v * 1e-3) for k, v in ms.items()}
             out[net]["ms_per_batch"] = ms
-            out[net]["top1_agreement_int8_vs_fake_quant_64_random_images"] = top1
+            out[net]["rel_logit_error_vs_fp32_64_random_images"] = err
             if net == "resnet18":
                 lib, layers = _lib.load(), []
                 shapes = {}
