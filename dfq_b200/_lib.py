@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
@@ -87,6 +87,17 @@ EXPECTED_SIZES = {
 }
 
 _PF = C.c_void_p   # device float*
+
+
+class _Momentum(object):
+    """ctypes argument type of the EMA momentum, a C double since ABI 2.  A Python number is passed as is, so 1 - m is formed
+    from the same double the reference uses; a c_float or c_double (what callers of ABI 1 pass) is widened exactly."""
+
+    @classmethod
+    def from_param(cls, v):
+        return C.c_double(v.value if isinstance(v, (C.c_float, C.c_double)) else float(v))
+
+
 _I64 = C.c_int64
 _I32 = C.c_int32
 _ST = C.c_void_p   # cudaStream_t
@@ -105,8 +116,8 @@ SIGNATURES = {
     "dfq_quant_dequant": [_PF, _PF, _I64, C.c_float, C.c_double, C.c_float, C.c_float, C.c_int, _PF, _ST],
     "dfq_quant_dequant_dev": [_PF, _PF, _I64, _PF, _PF, C.c_int, C.c_int, C.c_int, C.c_int, _PF, _ST],
     "dfq_act_minmax_per_sample": [_PF, _I64, _I64, _PF, _PF, _ST],
-    "dfq_observer_update": [_PF, _PF, _PF, C.c_int, C.c_float, _ST],
-    "dfq_observe_quant": [_PF, _PF, _I64, _I64, _PF, _PF, _PF, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, _ST],
+    "dfq_observer_update": [_PF, _PF, _PF, C.c_int, _Momentum, _ST],
+    "dfq_observe_quant": [_PF, _PF, _I64, _I64, _PF, _PF, _PF, C.c_int, _Momentum, C.c_int, C.c_int, C.c_int, C.c_int, _ST],
     "dfq_bnstat_loss_fwd": [_PF, _I64, _I64, _I64, _PF, _PF, C.c_float, _PF, _PF, C.c_void_p, _ST],
     "dfq_bnstat_loss_bwd": [_PF, _PF, _I64, _I64, _I64, _PF, _PF, C.c_float, _PF, _PF, _PF, C.c_int, _ST],
     "dfq_range_rows": [_PF, _I64, _I64, _PF, _PF, _ST],

@@ -286,12 +286,20 @@ __host__ __device__ inline QuantScalars quant_scalars(double mn, double mx, int 
   return q;
 }
 
+// clamp(t, lo, hi) that keeps a NaN, as torch's clamp_ does (fminf/fmaxf would turn it into lo)
+__device__ __forceinline__ float clamp_nan(float t, float lo, float hi) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(t), "f"(lo));
+  asm("min.NaN.f32 %0, %0, %1;" : "+f"(r) : "f"(hi));
+  return r;
+}
+
 // quantize.py:70-74, one element.  Every op is individually rounded (no FMA contraction).
 template <bool RECIP>
 __device__ __forceinline__ float fake_quant(float x, const QuantScalars& q, float* code = nullptr) {
   float t = __fadd_rn(x, q.neg_min);
   t = RECIP ? __fmul_rn(t, q.inv_scale) : __fdiv_rn(t, q.scale);
-  t = fminf(fmaxf(t, q.qmin), q.qmax);
+  t = clamp_nan(t, q.qmin, q.qmax);
   t = rintf(t);
   if (code) *code = t;
   t = __fmul_rn(t, q.scale);

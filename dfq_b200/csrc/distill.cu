@@ -19,6 +19,8 @@
 namespace dfq {
 
 constexpr int kDThreads = 256;
+// dfq_bnstat_loss_fwd: rows of at least this many elements get a CTA each, shorter ones a warp
+constexpr int kBnstatCtaRow = 2048;
 
 __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
@@ -32,12 +34,14 @@ __global__ void __launch_bounds__(kDThreads)
 k_bnstat_fwd(const float* __restrict__ x, int64_t rows, int64_t hw, int C, const float* __restrict__ mu,
              const float* __restrict__ sigma, float eps, float* __restrict__ m_out, float* __restrict__ s_out, double* loss2) {
   __shared__ double red[3][kDThreads / 32];
+  __shared__ float redf[2][kDThreads / 32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   double lm = 0.0, ls = 0.0;
   const int64_t step = CTA_ROW ? gridDim.x : (int64_t)gridDim.x * (kDThreads / 32);
   for (int64_t r = CTA_ROW ? blockIdx.x : blockIdx.x * (int64_t)(kDThreads / 32) + warp; r < rows; r += step) {
     const float* p = x + r * hw;
     double a = 0.0, b = 0.0, sx = 0.0;       // sum(y), sum(y^2) with y = x + eps, and sum(x)
+    float ylo = DFQ_INF, yhi = -DFQ_INF;     // extrema of y: a constant row gets s = 0 exactly
     const int tid = CTA_ROW ? threadIdx.x : lane, nt = CTA_ROW ? kDThreads : 32;
     if ((hw & 3) == 0 && ((((uintptr_t)p) & 15) == 0)) {
       const float4* p4 = (const float4*)p;
@@ -47,26 +51,32 @@ k_bnstat_fwd(const float* __restrict__ x, int64_t rows, int64_t hw, int C, const
         a += ((double)y0 + (double)y1) + ((double)y2 + (double)y3);
         b += ((double)y0 * y0 + (double)y1 * y1) + ((double)y2 * y2 + (double)y3 * y3);
         sx += ((double)v.x + (double)v.y) + ((double)v.z + (double)v.w);
+        ylo = fminf(ylo, fminf(fminf(y0, y1), fminf(y2, y3))); yhi = fmaxf(yhi, fmaxf(fmaxf(y0, y1), fmaxf(y2, y3)));
       }
     } else {
       for (int64_t i = tid; i < hw; i += nt) {
         const float v = __ldg(p + i), y = __fadd_rn(v, eps);
         a += (double)y; b += (double)y * y; sx += (double)v;
+        ylo = fminf(ylo, y); yhi = fmaxf(yhi, y);
       }
     }
     a = warp_sum_d(a); b = warp_sum_d(b); sx = warp_sum_d(sx);
+    ylo = warp_min(ylo); yhi = warp_max(yhi);
     if (CTA_ROW) {
       __syncthreads();
-      if (lane == 0) { red[0][warp] = a; red[1][warp] = b; red[2][warp] = sx; }
+      if (lane == 0) { red[0][warp] = a; red[1][warp] = b; red[2][warp] = sx; redf[0][warp] = ylo; redf[1][warp] = yhi; }
       __syncthreads();
       a = 0.0; b = 0.0; sx = 0.0;
-      for (int i = 0; i < kDThreads / 32; ++i) { a += red[0][i]; b += red[1][i]; sx += red[2][i]; }
+      for (int i = 0; i < kDThreads / 32; ++i) {
+        a += red[0][i]; b += red[1][i]; sx += red[2][i]; ylo = fminf(ylo, redf[0][i]); yhi = fmaxf(yhi, redf[1][i]);
+      }
     }
     if (tid == 0) {
       const double n = (double)hw;
       const double mean_y = a / n;
       double var = (b - a * mean_y) / (n - 1.0);       // unbiased; hw == 1 -> 0/0 = NaN like torch.std
-      if (var < 0.0) var = 0.0;
+      // the single-pass variance of a constant row rounds to a tiny value of either sign instead of 0 (a NaN stays)
+      if (var < 0.0 || (var > 0.0 && ylo == yhi)) var = 0.0;
       const float m = (float)(sx / n), s = (float)sqrt(var);
       m_out[r] = m; s_out[r] = s;
       const int c = (int)(r % C);
@@ -86,6 +96,16 @@ k_bnstat_fwd(const float* __restrict__ x, int64_t rows, int64_t hw, int C, const
   }
 }
 
+// dL/dm per element of a row, and the coefficient of (y_i - mean(y)) in dL/ds per element.  A zero-variance row (a dead
+// channel) has no std gradient: torch's std backward masks std == 0 to 0, where 1/s would give inf (or NaN for x == 0).
+__device__ __forceinline__ double bnstat_mean_coef(double gm, float m, float mu, double inv_c, int64_t hw) {
+  return gm * 2.0 * ((double)m - (double)mu) * inv_c / (double)hw;
+}
+__device__ __forceinline__ double bnstat_std_coef(double gs, float s, float sigma, double inv_c, int64_t hw) {
+  if (s == 0.f) return 0.0;
+  return gs * 2.0 * ((double)s - (double)sigma) * inv_c / ((double)(hw - 1) * (double)s);
+}
+
 __global__ void __launch_bounds__(kDThreads)
 k_bnstat_bwd(const float* __restrict__ x, float* __restrict__ gx, int64_t rows, int64_t hw, int C, const float* __restrict__ mu,
              const float* __restrict__ sigma, float eps, const float* __restrict__ m_in, const float* __restrict__ s_in,
@@ -101,14 +121,14 @@ k_bnstat_bwd(const float* __restrict__ x, float* __restrict__ gx, int64_t rows, 
     int64_t off = i - r * hw;
     float m = m_in[r], s = s_in[r];
     int c = (int)(r % C);
-    double ka = gm * 2.0 * ((double)m - (double)mu[c]) * inv_c / (double)hw;
-    double kb = gs * 2.0 * ((double)s - (double)sigma[c]) * inv_c / ((double)(hw - 1) * (double)s);
+    double ka = bnstat_mean_coef(gm, m, mu[c], inv_c, hw);
+    double kb = bnstat_std_coef(gs, s, sigma[c], inv_c, hw);
     for (int k = 0; k < lim; ++k) {
       if (off == hw) {
         ++r; off = 0;
         m = m_in[r]; s = s_in[r]; c = (int)(r % C);
-        ka = gm * 2.0 * ((double)m - (double)mu[c]) * inv_c / (double)hw;
-        kb = gs * 2.0 * ((double)s - (double)sigma[c]) * inv_c / ((double)(hw - 1) * (double)s);
+        ka = bnstat_mean_coef(gm, m, mu[c], inv_c, hw);
+        kb = bnstat_std_coef(gs, s, sigma[c], inv_c, hw);
       }
       const float y = __fadd_rn(x[i + k], eps);
       const double g = ka + kb * ((double)y - ((double)m + (double)eps));
@@ -131,7 +151,7 @@ extern "C" int dfq_bnstat_loss_fwd(const float* x, int64_t n, int64_t c, int64_t
   DFQ_CUDA(cudaMemsetAsync(loss2, 0, 2 * sizeof(double), st));
   const int64_t rows = n * c;
   const int sms = std::max(1, sm_count());
-  if (hw >= 2048) {
+  if (hw >= kBnstatCtaRow) {
     const int grid = (int)std::min<int64_t>(rows, (int64_t)sms * 8);
     k_bnstat_fwd<true><<<grid, kDThreads, 0, st>>>(x, rows, hw, (int)c, bn_mean, bn_std, eps, mean_out, std_out, loss2);
   } else {

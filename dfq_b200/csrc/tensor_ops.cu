@@ -142,6 +142,10 @@ int TablePack::upload(cudaStream_t st) {
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
+// floats per thread of one (sample, split) work item of the per-sample statistics, and of one k_minmax thread
+constexpr int kItemFloats = 16;
+// dfq_range_rows: rows longer than this get a CTA each, shorter ones a warp
+constexpr int kRangeCtaRow = 2048;
 
 // grid-stride min/max of a flat tensor, 4 independent 128-bit loads in flight per thread
 __device__ __forceinline__ void flat_minmax(const float* __restrict__ x, int64_t n, int64_t start, int64_t stride,
@@ -206,17 +210,18 @@ __global__ void k_batch_mean(const float* __restrict__ scratch, int64_t batch, f
   }
 }
 
-__global__ void k_observer_update(float* rmin, float* rmax, const float* __restrict__ stat2, int mode, float momentum) {
+__global__ void k_observer_update(float* rmin, float* rmax, const float* __restrict__ stat2, int mode, double momentum) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     if (mode == 1) {
       // Python min()/max() on 0-d tensors (quantize.py:106-107): the smaller / larger value
       rmin[0] = fminf(rmin[0], stat2[0]);
       rmax[0] = fmaxf(rmax[0], stat2[1]);
     } else {
-      // running.mul_(1 - m).add_(value * m) (quantize.py:112-113), separately rounded
-      const float om = (float)(1.0 - (double)momentum);
-      rmin[0] = __fadd_rn(__fmul_rn(rmin[0], om), __fmul_rn(stat2[0], momentum));
-      rmax[0] = __fadd_rn(__fmul_rn(rmax[0], om), __fmul_rn(stat2[1], momentum));
+      // running.mul_(1 - m).add_(value * m) (quantize.py:112-113), separately rounded; 1 - m is formed in double from the
+      // Python float, like the reference's scalar
+      const float om = (float)(1.0 - momentum), m = (float)momentum;
+      rmin[0] = __fadd_rn(__fmul_rn(rmin[0], om), __fmul_rn(stat2[0], m));
+      rmax[0] = __fadd_rn(__fmul_rn(rmax[0], om), __fmul_rn(stat2[1], m));
     }
   }
 }
@@ -303,7 +308,7 @@ enum { OBS_UPDATE = 1, OBS_EMA = 2, OBS_OWN = 4 };
 template <bool RECIP>
 __global__ void __launch_bounds__(kThreads)
 k_observe_quant(const float* __restrict__ x, float* __restrict__ y, int64_t batch, int64_t per, int splits,
-                float* running_min, float* running_max, float* __restrict__ scratch, float* stat_out, int flags, float momentum,
+                float* running_min, float* running_max, float* __restrict__ scratch, float* stat_out, int flags, double momentum,
                 int num_bits, int symmetric, int prologue) {
   cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   __shared__ float red[2 * kWarps];
@@ -343,9 +348,9 @@ k_observe_quant(const float* __restrict__ x, float* __restrict__ y, int64_t batc
       else {
         if (flags & OBS_UPDATE) { r_min = fminf(r_min, st_min); r_max = fmaxf(r_max, st_max); }
         if (flags & OBS_EMA) {
-          const float om = (float)(1.0 - (double)momentum);
-          r_min = __fadd_rn(__fmul_rn(r_min, om), __fmul_rn(st_min, momentum));
-          r_max = __fadd_rn(__fmul_rn(r_max, om), __fmul_rn(st_max, momentum));
+          const float om = (float)(1.0 - momentum), m = (float)momentum;
+          r_min = __fadd_rn(__fmul_rn(r_min, om), __fmul_rn(st_min, m));
+          r_max = __fadd_rn(__fmul_rn(r_max, om), __fmul_rn(st_max, m));
           q_min = st_min; q_max = st_max;
         } else { q_min = r_min; q_max = r_max; }
         if (blockIdx.x == 0) { __stcg(running_min, r_min); __stcg(running_max, r_max); }
@@ -436,7 +441,7 @@ __global__ void k_fill(float* p, int64_t n, float v) {
 
 __global__ void __launch_bounds__(kThreads) k_clamp(float* x, int64_t n, float lo, float hi) {
   const int64_t start = blockIdx.x * (int64_t)kThreads + threadIdx.x, stride = (int64_t)gridDim.x * kThreads;
-  for (int64_t i = start; i < n; i += stride) x[i] = fminf(fmaxf(x[i], lo), hi);
+  for (int64_t i = start; i < n; i += stride) x[i] = clamp_nan(x[i], lo, hi);
 }
 
 static int flat_grid(int64_t n, int per_thread) {
@@ -480,7 +485,7 @@ extern "C" int dfq_minmax(const float* x, int64_t n, float* out2, void* stream) 
   cudaStream_t st = (cudaStream_t)stream;
   DFQ_REQUIRE(x && out2 && n > 0, "bad argument");
   k_init2<<<1, 32, 0, st>>>(out2, 1);
-  k_minmax<<<flat_grid(n, 16), kThreads, 0, st>>>(x, n, out2);
+  k_minmax<<<flat_grid(n, kItemFloats), kThreads, 0, st>>>(x, n, out2);
   DFQ_CUDA(cudaGetLastError());
   return 0;
 }
@@ -533,7 +538,7 @@ extern "C" int dfq_act_minmax_per_sample(const float* x, int64_t batch, int64_t 
   DFQ_REQUIRE(batch <= 65535, "batch too large for one launch");
   k_init2<<<(int)std::min<int64_t>(64, (batch + 255) / 256), 256, 0, st>>>(scratch_2b, batch);
   const int sms = std::max(1, sm_count());
-  int splits = (int)std::max<int64_t>(1, std::min<int64_t>((per_sample + kThreads * 16 - 1) / (kThreads * 16),
+  int splits = (int)std::max<int64_t>(1, std::min<int64_t>((per_sample + kThreads * kItemFloats - 1) / (kThreads * kItemFloats),
                                                            std::max<int64_t>(1, (int64_t)sms * 8 / batch)));
   k_sample_minmax<<<dim3(splits, (unsigned)batch), kThreads, 0, st>>>(x, per_sample, scratch_2b);
   k_batch_mean<<<1, 256, 0, st>>>(scratch_2b, batch, out2);
@@ -541,7 +546,7 @@ extern "C" int dfq_act_minmax_per_sample(const float* x, int64_t batch, int64_t 
   return 0;
 }
 
-extern "C" int dfq_observer_update(float* running_min, float* running_max, const float* stat2, int mode, float momentum,
+extern "C" int dfq_observer_update(float* running_min, float* running_max, const float* stat2, int mode, double momentum,
                                    void* stream) {
   DFQ_REQUIRE(running_min && running_max && stat2 && (mode == 1 || mode == 2), "bad argument");
   k_observer_update<<<1, 32, 0, (cudaStream_t)stream>>>(running_min, running_max, stat2, mode, momentum);
@@ -551,7 +556,7 @@ extern "C" int dfq_observer_update(float* running_min, float* running_max, const
 
 
 extern "C" int dfq_observe_quant(const float* x, float* y, int64_t batch, int64_t per_sample, float* running_min,
-                                 float* running_max, float* stat_out2, int flags, float momentum, int num_bits, int symmetric,
+                                 float* running_max, float* stat_out2, int flags, double momentum, int num_bits, int symmetric,
                                  int div_mode, int prologue, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   DFQ_REQUIRE(x && y && batch > 0 && per_sample > 0, "bad argument");
@@ -559,15 +564,17 @@ extern "C" int dfq_observe_quant(const float* x, float* y, int64_t batch, int64_
   DFQ_REQUIRE((flags & (OBS_UPDATE | OBS_EMA | OBS_OWN)) != 0, "nothing to observe: use dfq_quant_dequant_dev");
   DFQ_REQUIRE(num_bits >= 1 && num_bits <= 32 && prologue >= 0 && prologue <= 2, "num_bits / prologue");
   static int per_sm_recip = 0, per_sm_div = 0;
-  int& per_sm = div_mode ? per_sm_recip : per_sm_div;
-  const void* fn = div_mode ? (const void*)k_observe_quant<true> : (const void*)k_observe_quant<false>;
+  // a tensor divisor (prologue 1/2) is always a true division, as in dfq_quant_dequant_dev
+  const bool recip = div_mode && prologue == 0;
+  int& per_sm = recip ? per_sm_recip : per_sm_div;
+  const void* fn = recip ? (const void*)k_observe_quant<true> : (const void*)k_observe_quant<false>;
   if (per_sm == 0) DFQ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kThreads, 0));
   if (per_sm < 1) { set_error("k_observe_quant does not fit on an SM"); return DFQ_E_NOT_COOPERATIVE; }
   const int sms = std::max(1, sm_count());
   const int64_t n = batch * per_sample;
   // enough CTAs to fill the machine for big tensors, few for small ones (a grid barrier costs with the grid size)
-  int grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sms * std::min(per_sm, 4), (n + (int64_t)kThreads * 16 - 1) / ((int64_t)kThreads * 16)));
-  int splits = (int)std::max<int64_t>(1, std::min<int64_t>((per_sample + kThreads * 16 - 1) / (kThreads * 16), std::max<int64_t>(1, grid / batch)));
+  int grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sms * std::min(per_sm, 4), (n + (int64_t)kThreads * kItemFloats - 1) / ((int64_t)kThreads * kItemFloats)));
+  int splits = (int)std::max<int64_t>(1, std::min<int64_t>((per_sample + kThreads * kItemFloats - 1) / (kThreads * kItemFloats), std::max<int64_t>(1, grid / batch)));
   float* scratch = nullptr;
   DFQ_CUDA(cudaMallocAsync((void**)&scratch, sizeof(float) * 2 * (size_t)batch * splits, st));
   void* args[] = {(void*)&x, (void*)&y, (void*)&batch, (void*)&per_sample, (void*)&splits, (void*)&running_min, (void*)&running_max,
@@ -580,7 +587,7 @@ extern "C" int dfq_observe_quant(const float* x, float* y, int64_t batch, int64_
 
 extern "C" int dfq_range_rows(const float* w, int64_t rows, int64_t row_len, float* out_min, float* out_max, void* stream) {
   DFQ_REQUIRE(w && out_min && out_max && rows > 0 && row_len > 0, "bad argument");
-  const int cta_row = row_len > 2048;
+  const int cta_row = row_len > kRangeCtaRow;
   const int64_t want = cta_row ? rows : (rows + kWarps - 1) / kWarps;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)std::max(1, sm_count()) * 8));
   k_range_rows<<<grid, kThreads, 0, (cudaStream_t)stream>>>(w, rows, row_len, out_min, out_max, cta_row);

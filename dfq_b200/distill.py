@@ -30,6 +30,15 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
+def _channel_stat(t, x, name):
+    """A BatchNorm statistic as the kernels read it: [C] contiguous fp32 on x's device."""
+    if t.device != x.device:
+        raise _lib.DfqError("%s is on %s, the input on %s" % (name, t.device, x.device))
+    if t.numel() != x.shape[1]:
+        raise _lib.DfqError("%s has %d elements for %d channels" % (name, t.numel(), x.shape[1]))
+    return t.detach().reshape(-1).to(torch.float32).contiguous()
+
+
 class _BNStatLoss(torch.autograd.Function):
     """(x [N,C,H,W], bn_mean [C], bn_std [C]) -> tensor [2] = (own_loss(bn_mean, mean_hw x), own_loss(bn_std, std_hw(x+eps)))
     as distill_data.py:171-185 computes them; gradient w.r.t. x only."""
@@ -39,6 +48,7 @@ class _BNStatLoss(torch.autograd.Function):
         lib = _lib.load()
         xc = x.detach().contiguous()
         n, c = xc.shape[0], xc.shape[1]
+        bn_mean, bn_std = _channel_stat(bn_mean, xc, "bn_mean"), _channel_stat(bn_std, xc, "bn_std")
         hw = xc.numel() // (n * c)
         m = xc.new_empty((n * c,)); s = xc.new_empty((n * c,))
         loss = xc.new_empty((2,), dtype=torch.float64)

@@ -110,6 +110,25 @@ def tensor_minmax(x):
     return out
 
 
+def _per_sample(numel, batch):
+    """Elements per sample of a tensor viewed as [batch, -1]; refuses a batch that does not divide it, as the reference's
+    ``view(B // num_chunks, -1)`` does (quantize.py:26)."""
+    if numel % batch:
+        raise _lib.DfqError("cannot view a tensor of %d elements as [%d, -1]" % (numel, batch))
+    return numel // batch
+
+
+def _running_buffer(t, device, name):
+    """(fp32 contiguous 1-element tensor the kernel may update, the caller's tensor to copy the result back into or None)."""
+    if t.device != device:
+        raise _lib.DfqError("%s is on %s, the input on %s" % (name, t.device, device))
+    if t.numel() != 1:
+        raise _lib.DfqError("%s must hold one element, got %d" % (name, t.numel()))
+    if t.dtype == torch.float32 and t.is_contiguous():
+        return t, None
+    return t.detach().reshape(1).to(torch.float32).contiguous(), t
+
+
 def per_sample_minmax_mean(x, batch=None):
     """Device tensor [2] = (mean_b min(x[b]), mean_b max(x[b])) for x viewed as [batch, -1]
     (quantize.py:106-107,110-111)."""
@@ -117,7 +136,7 @@ def per_sample_minmax_mean(x, batch=None):
     xd, _ = _dev_f32(x.detach())
     if batch is None:
         batch = xd.shape[0]
-    per = xd.numel() // batch
+    per = _per_sample(xd.numel(), batch)
     out = xd.new_empty((2,))
     scratch = xd.new_empty((2 * batch,))
     _lib.check(lib.dfq_act_minmax_per_sample(_ptr(xd), batch, per, _ptr(out), _ptr(scratch), _lib.stream_ptr()),
@@ -139,14 +158,19 @@ def observe_and_quant(x, num_bits, flags, running_min=None, running_max=None, mo
     if batch is None:
         batch = xd.shape[0] if xd.dim() > 0 else 1
     batch = max(1, int(batch))
-    per = xd.numel() // batch
+    per = _per_sample(xd.numel(), batch)
+    rmin, rmin_back = _running_buffer(running_min, xd.device, "running_min") if running_min is not None else (None, None)
+    rmax, rmax_back = _running_buffer(running_max, xd.device, "running_max") if running_max is not None else (None, None)
     yd = out if (out is not None and out.is_cuda and out.is_contiguous()) else torch.empty_like(xd)
     if xd.numel():
         _lib.check(lib.dfq_observe_quant(_ptr(xd), _ptr(yd), batch, per,
-                                         _ptr(running_min) if running_min is not None else None,
-                                         _ptr(running_max) if running_max is not None else None, None, int(flags),
-                                         C.c_float(momentum), int(num_bits), 1 if symmetric else 0, int(div_mode), int(prologue),
+                                         _ptr(rmin) if rmin is not None else None,
+                                         _ptr(rmax) if rmax is not None else None, None, int(flags),
+                                         C.c_double(momentum), int(num_bits), 1 if symmetric else 0, int(div_mode), int(prologue),
                                          _lib.stream_ptr()), "dfq_observe_quant")
+    for back, buf in ((rmin_back, rmin), (rmax_back, rmax)):
+        if back is not None:
+            back.copy_(buf.view(back.shape))
     if out is not None and yd is not out:
         out.copy_(yd.view(out.shape))
         return out
@@ -179,7 +203,8 @@ class UniformQuantize(InplaceFunction):
             res = fake_quant_device_range(input, num_bits, mn_t, mx_t, symmetric, prologue=prologue, out=out)
         else:
             res = fake_quant_explicit(input, num_bits, float(min_value), float(max_value), symmetric, out=out)
-        return res
+        # in place, autograd wants the very tensor it marked dirty back, not a view of it
+        return input if inplace else res
 
     @staticmethod
     def backward(ctx, grad_output):

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 1
+#define DFQ_ABI_VERSION 2
 
 enum {
   DFQ_OK = 0,
@@ -247,7 +247,7 @@ int dfq_act_minmax_per_sample(const float* x, int64_t batch, int64_t per_sample,
 /* QuantMeasure running statistics update on the device (quantize.py:103-113), stat2 = {min, max}:
  * mode 1: running_min = min(running_min, stat_min), running_max = max(running_max, stat_max)  (update_stat)
  * mode 2: running = running*(1-momentum) + stat*momentum                                      (training EMA) */
-int dfq_observer_update(float* running_min, float* running_max, const float* stat2, int mode, float momentum,
+int dfq_observer_update(float* running_min, float* running_max, const float* stat2, int mode, double momentum,
                         void* stream);
 
 /* QuantMeasure.forward in ONE launch (quantize.py:102-119; SURVEY 8(f) rank 1): per-sample min/max -> batch mean -> running
@@ -264,7 +264,7 @@ int dfq_observer_update(float* running_min, float* running_max, const float* sta
 #define DFQ_OBS_EMA 2
 #define DFQ_OBS_OWN 4
 int dfq_observe_quant(const float* x, float* y, int64_t batch, int64_t per_sample, float* running_min, float* running_max,
-                      float* stat_out2, int flags, float momentum, int num_bits, int symmetric, int div_mode, int prologue,
+                      float* stat_out2, int flags, double momentum, int num_bits, int symmetric, int div_mode, int prologue,
                       void* stream);
 
 /* HOST-side helper of the residency (no CUDA call): copies n segments between scattered host buffers and one contiguous

@@ -92,6 +92,37 @@ def quantize(x: np.ndarray, num_bits: int = 8, min_value: Optional[float] = None
     return y.astype(f32)
 
 
+def tensor_range_scalars(num_bits: int, min_value, max_value, symmetric: bool, prologue: int):
+    """Scalar prologue when min/max are fp32 0-d TENSORS (quantize.py:24-35, then :49-66 on tensors): every step an fp32
+    op.  ``prologue`` 1: ``/ qmax`` is a true division (CPU tensors); 2: a multiply by the fp32 reciprocal of qmax (a CUDA
+    tensor divided by a Python scalar).  Returns (qmin, qmax, min_value, scale) as fp32."""
+    mn, mx = f32(min_value), f32(max_value)
+    with np.errstate(over="ignore", invalid="ignore"):
+        if symmetric:
+            qmin, qmax = f32(-2.0 ** (num_bits - 1)), f32(2 ** (num_bits - 1) - 1)
+            mx, mn = abs(mx), abs(mn)
+            if mx < mn:
+                mx = mn
+            d, mn = mx, f32(0)
+        else:
+            qmin, qmax = f32(0), f32(2.0 ** num_bits - 1)
+            d = f32(mx - mn)
+        scale = f32(d * (f32(1) / qmax)) if prologue == 2 else f32(d / qmax)
+    if f32(1e-8) > scale:
+        scale = f32(1e-8)
+    return qmin, qmax, mn, scale
+
+
+def quantize_tensor_range(x: np.ndarray, num_bits: int, min_value, max_value, symmetric: bool = False, prologue: int = 1):
+    """quantize.py:70-74 with the range of ``tensor_range_scalars``.  The element-wise ``div_(scale)`` is by a tensor and
+    therefore a true division on both devices."""
+    qmin, qmax, mn, scale = tensor_range_scalars(num_bits, min_value, max_value, symmetric, prologue)
+    x = np.ascontiguousarray(x, dtype=f32)
+    with np.errstate(over="ignore", invalid="ignore"):
+        t = (x + (-mn)) / scale
+        return (np.rint(np.minimum(np.maximum(t, qmin), qmax)) * scale + mn).astype(f32)
+
+
 def quantize_error(w: np.ndarray, num_bits: int = 8, signed: bool = False) -> np.ndarray:
     """dfq.py:8-25 with ``reduction=None``: Q(W) - W using the tensor's own min/max."""
     w = np.ascontiguousarray(w, dtype=f32)
@@ -370,12 +401,21 @@ def rows_outside_bound(got: np.ndarray, exact: np.ndarray, bound: np.ndarray) ->
 # --------------------------------------------------------------------------------------------
 # activation observer: utils/quantize.py:102-119
 # --------------------------------------------------------------------------------------------
+def flat_minmax(x: np.ndarray) -> Tuple[np.float32, np.float32]:
+    """(min, max) of a tensor as the library's reductions form them: NaN elements are skipped (DESIGN.md section 4), so a
+    tensor of NaN alone gives (+inf, -inf).  Without NaN this is ``x.min()``, ``x.max()``."""
+    x = np.ascontiguousarray(x, f32).reshape(-1)
+    return f32(np.fmin.reduce(x, initial=np.inf)), f32(np.fmax.reduce(x, initial=-np.inf))
+
+
 def per_sample_minmax_mean(x: np.ndarray) -> Tuple[np.float32, np.float32]:
     """``x.view(B,-1).min(-1)[0].mean()`` / ``.max(...)`` (quantize.py:106-107): exact per-sample
-    extrema, fp32 mean over the batch (accumulated in float64, rounded once)."""
+    extrema, fp32 mean over the batch (accumulated in float64, rounded once).  NaN elements are skipped as in
+    ``flat_minmax``: an all-NaN sample contributes +inf to the minimum and -inf to the maximum."""
     x = np.ascontiguousarray(x, f32).reshape(x.shape[0], -1)
-    mn = x.min(axis=1).astype(np.float64).mean()
-    mx = x.max(axis=1).astype(np.float64).mean()
+    with np.errstate(invalid="ignore"):
+        mn = np.fmin.reduce(x, axis=1, initial=np.inf).astype(np.float64).mean()
+        mx = np.fmax.reduce(x, axis=1, initial=-np.inf).astype(np.float64).mean()
     return f32(mn), f32(mx)
 
 
@@ -391,6 +431,34 @@ def observer_ema(running_min: float, running_max: float, x: np.ndarray, momentum
     rmin = f32(running_min) * f32(1 - momentum) + mn * f32(momentum)
     rmax = f32(running_max) * f32(1 - momentum) + mx * f32(momentum)
     return f32(rmin), f32(rmax), mn, mx
+
+
+# --------------------------------------------------------------------------------------------
+# distilled data: the BN-statistics loss of ZeroQ/distill_data.py:171-185
+# --------------------------------------------------------------------------------------------
+def bn_stat_loss(x: np.ndarray, bn_mean: np.ndarray, bn_std: np.ndarray, eps: float = 1e-6):
+    """float64 (L_mean, L_std, dL_mean/dx, dL_std/dx) of one BatchNorm input x [N, C, ...] with more than one element per
+    (n, c) row:  m = mean_hw x,  s = std_hw(x + eps) (unbiased),  L_mean = sum (mu_c - m)^2 / C,  L_std = sum (sigma_c - s)^2 / C.
+    A row with s == 0 has no std gradient, as torch's std backward masks a zero result."""
+    x64 = np.asarray(x, np.float64)
+    n, c = x64.shape[0], x64.shape[1]
+    flat = x64.reshape(n, c, -1)
+    hw = flat.shape[2]
+    assert hw > 1, "hw == 1 takes the reference's view(C, -1) path"
+    mu = np.asarray(bn_mean, np.float64).reshape(1, c)
+    sigma = np.asarray(bn_std, np.float64).reshape(1, c)
+    y = flat + eps
+    m = flat.mean(axis=2)
+    dev = y - y.mean(axis=2, keepdims=True)
+    dev[y.min(axis=2) == y.max(axis=2)] = 0.0          # a constant row: its rounded mean must not leave a residue
+    s = np.sqrt((dev * dev).sum(axis=2) / (hw - 1))
+    l_mean = ((mu - m) ** 2).sum() / c
+    l_std = ((sigma - s) ** 2).sum() / c
+    g_mean = np.broadcast_to((2.0 * (m - mu) / (c * hw))[:, :, None], flat.shape)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        k = np.where(s > 0, 2.0 * (s - sigma) / (c * (hw - 1) * s), 0.0)
+    g_std = k[:, :, None] * dev
+    return l_mean, l_std, g_mean.reshape(x64.shape).copy(), g_std.reshape(x64.shape)
 
 
 # --------------------------------------------------------------------------------------------

@@ -222,8 +222,8 @@ class FakeLib:
 
     # ---- stand-alone tensor ops -------------------------------------------------------------------------
     def dfq_minmax(self, x_p, n, out_p, stream):
-        x = _floats(x_p, n); out = _floats(out_p, 2)
-        out[0] = x.min(); out[1] = x.max()
+        out = _floats(out_p, 2)
+        out[0], out[1] = O.flat_minmax(_floats(x_p, n))
         return 0
 
     def dfq_quant_dequant(self, x_p, y_p, n, mn, scale, qmin, qmax, div_mode, codes_p, stream):
@@ -242,19 +242,7 @@ class FakeLib:
         if prologue == 0:
             y[...] = O.quantize(x.copy(), bits, mn, mx, bool(sym), div_mode="recip" if div_mode else "div")
         else:
-            mn32, mx32 = f32(mn), f32(mx)
-            if sym:
-                qmin, qmax = f32(-2.0 ** (bits - 1)), f32(2 ** (bits - 1) - 1)
-                a = max(abs(mx32), abs(mn32))
-                scale = a * (f32(1) / qmax) if prologue == 2 else a / qmax
-                mn32 = f32(0)
-            else:
-                qmin, qmax = f32(0), f32(2.0 ** bits - 1)
-                d = mx32 - mn32
-                scale = d * (f32(1) / qmax) if prologue == 2 else d / qmax
-            scale = f32(max(scale, f32(1e-8)))
-            t = (x + (-mn32)) / scale
-            y[...] = np.rint(np.minimum(np.maximum(t, qmin), qmax)) * scale + mn32
+            y[...] = O.quantize_tensor_range(x.copy(), bits, mn, mx, bool(sym), prologue)
         return 0
 
     def dfq_quant_error(self, w_p, e_p, n, mm_p, bits, sym, stream):
@@ -278,8 +266,8 @@ class FakeLib:
             if flags & 1:
                 rmin[0] = min(rmin[0], st_min); rmax[0] = max(rmax[0], st_max)
             if flags & 2:
-                m = f32(_val(momentum)); om = f32(1.0 - float(m))
-                rmin[0] = rmin[0] * om + st_min * m; rmax[0] = rmax[0] * om + st_max * m
+                m = float(_val(momentum)); om, mf = f32(1.0 - m), f32(m)
+                rmin[0] = rmin[0] * om + st_min * mf; rmax[0] = rmax[0] * om + st_max * mf
                 q_min, q_max = st_min, st_max
             else:
                 q_min, q_max = rmin[0], rmax[0]
@@ -291,12 +279,12 @@ class FakeLib:
 
     def dfq_observer_update(self, rmin_p, rmax_p, stat_p, mode, momentum, stream):
         rmin = _floats(rmin_p, 1); rmax = _floats(rmax_p, 1); st = _floats(stat_p, 2)
-        m = f32(_val(momentum))
+        m = float(_val(momentum))
         if mode == 1:
             rmin[0] = min(rmin[0], st[0]); rmax[0] = max(rmax[0], st[1])
         else:
-            om = f32(1.0 - float(m))
-            rmin[0] = rmin[0] * om + st[0] * m; rmax[0] = rmax[0] * om + st[1] * m
+            om, mf = f32(1.0 - m), f32(m)
+            rmin[0] = rmin[0] * om + st[0] * mf; rmax[0] = rmax[0] * om + st[1] * mf
         return 0
 
     def dfq_clamp(self, x_p, n, lo, hi, stream):

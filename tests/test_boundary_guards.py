@@ -1,6 +1,7 @@
 """CPU guards of the GPU boundary tests.
 
-* The kernel constants the boundary cases of tests/test_gpu_engine.py and tests/test_gpu_int8.py were built around: a
+* The kernel constants the boundary cases of tests/test_gpu_engine.py, tests/test_gpu_int8.py and
+  tests/test_gpu_activation.py were built around: a
   retune must fail here, loudly, instead of quietly moving every case off its boundary.
 * The per-row acceptance bound of bias correction (oracle.dfq_oracle.bias_delta_bound) accepts the oracle's own deltas and
   rejects errors that a normwise gate over the whole layer lets through."""
@@ -30,6 +31,12 @@ CONSTANTS = {
     "BK": ("int8_conv.cu", 64),
     "STAGES": ("int8_conv.cu", 3),
     "THREADS": ("int8_conv.cu", 128),
+    # the launch formulas of the activation kernels (tests/test_gpu_activation.py)
+    "kThreads": ("tensor_ops.cu", 256),
+    "kItemFloats": ("tensor_ops.cu", 16),
+    "kRangeCtaRow": ("tensor_ops.cu", 2048),
+    "kDThreads": ("distill.cu", 256),
+    "kBnstatCtaRow": ("distill.cu", 2048),
 }
 
 
