@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
@@ -130,6 +130,7 @@ SIGNATURES = {
     "dfq_i8_quantize_nhwc": [_PF, C.c_void_p, _I32, _I32, _I32, _I32, _I32, C.c_float, _ST],
     "dfq_i8_pack_weights": [_PF, _PF, C.c_void_p, C.c_void_p, _ST],
     "dfq_i8_conv": [C.c_void_p, C.c_void_p, _PF, _PF, _PF, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_conv_requant": [C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -9,7 +9,10 @@
 //   k_i8_conv_mma        groups == 1: implicit GEMM on the tensor cores (mma.sync m16n8k32 s8), M = N*OH*OW pixels,
 //                        N = O, K = kh*kw*Cpad; a cp.async ring gathers the im2col rows 16 channels (16 B) at a time
 //   k_i8_conv_dw         groups == C == O: int32 MACs on the CUDA cores over the NHWC codes
+// Both convolutions have two epilogues on one main loop (template parameter Out): fp32 NCHW (dfq_i8_conv), or the next layer's
+// int8 NHWC codes after the activation clamp (dfq_i8_conv_requant), which keeps activations in int8 between chained layers.
 #include <algorithm>
+#include <cmath>
 
 #include "common.cuh"
 
@@ -23,6 +26,24 @@ __device__ __forceinline__ int8_t q8(float v, float s) {
 
 __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
   return __fadd_rn(__fmul_rn(__int2float_rn(acc), dq), b);
+}
+
+// Where the epilogue puts its result.  F32: fp32 NCHW y (and optionally the int32 sums).  I8: the codes of the next layer,
+// int8 NHWC yq[N, OH, OW, cpad] (cpad = O rounded up to 16, pad channels 0), requantized at the next layer's scale after
+// the activation clamp [lo, hi].
+enum class Out { F32, I8 };
+struct Requant {
+  int8_t* yq;
+  float scale, lo, hi;
+  int cpad;
+};
+
+// What the per-layer path computes between two layers, in its order: dequant(), the activation (relu / relu6 / hardtanh,
+// composed into one clamp that keeps NaN as torch does), q8() at the next layer's scale.
+__device__ __forceinline__ int8_t requant(int32_t acc, float dq, float b, const Requant& rq) {
+  float v = dequant(acc, dq, b);
+  v = v < rq.lo ? rq.lo : (v > rq.hi ? rq.hi : v);
+  return q8(v, rq.scale);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -99,9 +120,11 @@ __device__ __forceinline__ void mma_s8(int32_t* c, const uint32_t* a, uint32_t b
 }
 
 // 4 warps as 2 (M) x 2 (N); each warp owns a 64 x 32 tile = 4 x 4 mma tiles.
+template <Out OUT>
 __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq,
                                                          const float* __restrict__ dq, const float* __restrict__ bias,
-                                                         float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g) {
+                                                         float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
+                                                         Requant rq) {
   __shared__ __align__(128) unsigned char smem[STAGES * STAGE_BYTES];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp >> 1, wn = warp & 1;
@@ -195,6 +218,44 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
+  if constexpr (OUT == Out::I8) {
+    // requantize in registers and stage the codes pixel-major, [m][64 channels] with the A tile's swizzle: the 2-byte stores
+    // of a warp (8 pixels x 4 channel pairs) and the 16-byte reads of a quarter warp (2 pixels x 4 chunks) are conflict-free.
+    // Channels O .. o0 + 63 stage as 0, so the last tile writes the zero pad of yq.
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int ol = wn * 32 + j * 8 + (lane & 3) * 2;          // this thread's channel pair ol, ol + 1
+      float d[2], b[2];
+      bool ok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int o = o0 + ol + h;
+        ok[h] = o < g.O;
+        d[h] = ok[h] ? dq[o] : 0.f;
+        b[h] = ok[h] && bias ? bias[o] : 0.f;
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int m = wm * 64 + i * 16 + (lane >> 2) + rr * 8;
+          const uint8_t c0 = ok[0] ? (uint8_t)requant(acc[i][j][2 * rr], d[0], b[0], rq) : 0;
+          const uint8_t c1 = ok[1] ? (uint8_t)requant(acc[i][j][2 * rr + 1], d[1], b[1], rq) : 0;
+          *reinterpret_cast<uint16_t*>(smem + swz(m, ol >> 4) + (ol & 15)) = (uint16_t)(c0 | (c1 << 8));
+        }
+    }
+    __syncthreads();
+    // one 16-byte chunk = 16 channels of one pixel; chunks at or past cpad (= O rounded up to 16) are not written
+    for (int e = tid; e < BM * (BN / 16); e += THREADS) {
+      const int ml = e >> 2, c = e & 3;
+      const int64_t m = m0 + ml;
+      const int o = o0 + c * 16;
+      if (m >= M || o >= rq.cpad) continue;
+      *reinterpret_cast<int4*>(rq.yq + m * rq.cpad + o) = *reinterpret_cast<const int4*>(smem + swz(ml, c));
+    }
+    return;
+  }
+
   // stage the tile as [o][m] so the NCHW stores run along the pixels
   int32_t* st = reinterpret_cast<int32_t*>(smem);
 #pragma unroll
@@ -224,15 +285,21 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
 // ------------------------------------------------------------------------------------------------------------------
 // depthwise on the CUDA cores: one thread per (n, 16 channels, output pixel), pixels fastest
 // ------------------------------------------------------------------------------------------------------------------
+template <Out OUT>
 __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq, const float* __restrict__ dq,
                              const float* __restrict__ bias, float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
-                             int64_t total) {
+                             int64_t total, Requant rq) {
   const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int p = (int)(i % OHW);
     const int64_t t = i / OHW;
     const int ch = (int)(t % chunks);
     const int64_t n = t / chunks;
+    if constexpr (OUT == Out::I8) {
+      // the input's Cpad may be wider than yq's cpad = round_up(O, 16): chunks past it hold only pad channels, and yq has
+      // no room for them
+      if (ch * 16 >= rq.cpad) continue;
+    }
     const int oh = p / g.OW, ow = p % g.OW;
     int32_t acc[16];
 #pragma unroll
@@ -251,6 +318,16 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
 #pragma unroll
         for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
       }
+    }
+    if constexpr (OUT == Out::I8) {                             // the 16 channels of this pixel in one store
+      alignas(16) int8_t v[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        v[j] = c < g.C ? requant(acc[j], dq[c], bias ? bias[c] : 0.f, rq) : (int8_t)0;
+      }
+      *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+      continue;
     }
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -327,10 +404,34 @@ extern "C" int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, 
     const int64_t M = (int64_t)g->N * g->OH * g->OW;
     DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_conv: too many output pixels");
     const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g);
+    k_i8_conv_mma<Out::F32><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, Requant{});
   } else {
     const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, total);
+    k_i8_conv_dw<Out::F32><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, total, Requant{});
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, int8_t* yq,
+                                   float out_scale, float act_lo, float act_hi, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(xq && wq && dq && yq, "dfq_i8_conv_requant: null pointer");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv_requant: codes must be 16-byte aligned");
+  DFQ_REQUIRE(aligned16(yq), "dfq_i8_conv_requant: yq must be 16-byte aligned");
+  DFQ_REQUIRE(!std::isnan(act_lo) && !std::isnan(act_hi) && act_lo <= act_hi,
+              "dfq_i8_conv_requant: activation bounds must be ordered and not NaN");
+  DFQ_REQUIRE(std::isfinite(out_scale) && out_scale >= 0.f, "dfq_i8_conv_requant: out_scale must be finite and non-negative");
+  const Requant rq{yq, out_scale, act_lo, act_hi, (g->O + 15) / 16 * 16};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    const int64_t M = (int64_t)g->N * g->OH * g->OW;
+    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_requant: too many output pixels");
+    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<Out::I8><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, rq);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<Out::I8><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, rq);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;

@@ -21,7 +21,9 @@ import ctypes as C
 
 import numpy as np
 import torch
+import torch.fx as fx
 import torch.nn as nn
+import torch.nn.functional as F
 
 from . import _lib, engine, export
 
@@ -56,7 +58,14 @@ def check_scale(what, scale, layer):
 
 
 class _Int8Layer(nn.Module):
-    """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves."""
+    """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves.
+
+    Two execution modes, set only on the copies chain_int8 makes (`chained`): `codes_in` - the input is already int8 NHWC
+    codes [N, H, W, cpad] at this layer's act_scale; `requant` = (out_scale, lo, hi) - the output is the next layer's int8
+    NHWC codes (dfq_i8_conv_requant) instead of fp32 NCHW.  A layer convert_to_int8 made takes and returns fp32 only."""
+
+    codes_in = False
+    requant = None
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
         super().__init__()
@@ -99,25 +108,65 @@ class _Int8Layer(nn.Module):
             g[0][k] = v
         return g
 
+    def chained(self, codes_in=False, requant=None):
+        """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
+        mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes.  self is not
+        modified."""
+        new = type(self).__new__(type(self))
+        nn.Module.__init__(new)
+        for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad", "act_scale"):
+            setattr(new, k, getattr(self, k))
+        for k, b in self._buffers.items():
+            new.register_buffer(k, b)
+        new.codes_in = bool(codes_in)
+        if requant is not None:
+            s, lo, hi = requant
+            check_scale("output", s, "%s -> next layer" % type(self).__name__)
+            lo, hi = _f32(lo), _f32(hi)
+            if np.isnan(lo) or np.isnan(hi) or lo > hi:
+                raise _lib.DfqError("activation bounds (%g, %g) must be ordered and not NaN" % (lo, hi))
+            requant = (float(_f32(s)), float(lo), float(hi))
+        new.requant = requant
+        return new
+
     def run(self, x, with_acc=False):
-        """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue."""
+        """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue.  In the chained modes
+        x is int8 codes [N, H, W, cpad] (codes_in) and y int8 codes [N, OH, OW, round_up(C_out, 16)] (requant)."""
         if not x.is_cuda or not self.dq.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.dq.device))
-        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
+        if self.codes_in:
+            if x.dtype != torch.int8 or x.dim() != 4 or x.shape[3] != self.cpad:
+                raise _lib.DfqError("chained int8 layer expects int8 codes [N, H, W, %d], got %s %s"
+                                    % (self.cpad, x.dtype, tuple(x.shape)))
+            N, H, W, _ = x.shape
+        elif x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
             raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s %s" % (self.in_channels, x.dtype, tuple(x.shape)))
+        else:
+            N, _, H, W = x.shape
+        if self.requant is not None and with_acc:
+            raise _lib.DfqError("a requantizing int8 layer does not return its int32 sums")
         x = x.contiguous()
-        N, Cn, H, W = x.shape
         g = self._geometry(N, H, W)
         OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
         if OH <= 0 or OW <= 0:
             raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
         lib, st = _lib.load(), _lib.stream_ptr()
-        xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
+        if self.codes_in:
+            xq = x
+        else:
+            xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
+            _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, self.in_channels, H, W, self.cpad,
+                                                C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
+        if self.requant is not None:
+            s, lo, hi = self.requant
+            yq = torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=x.device)
+            _lib.check(lib.dfq_i8_conv_requant(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(yq),
+                                               C.c_float(s), C.c_float(lo), C.c_float(hi), _lib.table_ptr(g), st),
+                       "dfq_i8_conv_requant")
+            return yq, None
         y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=x.device)
         acc = torch.empty(y.shape, dtype=torch.int32, device=x.device) if with_acc else None
-        _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, Cn, H, W, self.cpad, C.c_float(self.act_scale), st),
-                   "dfq_i8_quantize_nhwc")
         _lib.check(lib.dfq_i8_conv(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(y), _ptr(acc),
                                    _lib.table_ptr(g), st), "dfq_i8_conv")
         return y, acc
@@ -199,3 +248,131 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
         setattr(model.get_submodule(parent_name) if parent_name else model, attr, new)
         done.append(name)
     return done
+
+
+# ---- chaining converted convolutions through int8 codes ---------------------------------------------------------------
+_INF = float("inf")
+
+
+class _Int8Tracer(fx.Tracer):
+    """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves"""
+
+    def is_leaf_module(self, m, qualname):
+        return isinstance(m, _Int8Layer) or super().is_leaf_module(m, qualname)
+
+
+def _arg(node, i, name, default):
+    return node.kwargs[name] if name in node.kwargs else (node.args[i] if len(node.args) > i else default)
+
+
+def _is_identity_bn(bn):
+    """True when the eval-mode BatchNorm2d computes x exactly: weight 1, bias 0, mean 0, var 1 and fp32(1 + eps) == 1 (what
+    merge_batchnorm leaves behind, utils/layer_transform.py)."""
+    if bn.training or not bn.track_running_stats or bn.running_mean is None:
+        return False
+    if _f32(1) + _f32(bn.eps) != _f32(1):
+        return False
+    with torch.no_grad():
+        ok = bool((bn.running_mean == 0).all()) and bool((bn.running_var == 1).all())
+        if bn.affine:
+            ok = ok and bool((bn.weight == 1).all()) and bool((bn.bias == 0).all())
+    return ok
+
+
+def _pass_through(node, mods):
+    """(lo, hi) of a node that is the identity or an activation clamp on the edge between two converted convolutions, or
+    None when it ends the chain."""
+    if node.op == "call_module":
+        m = mods[node.target]
+        if type(m) is nn.BatchNorm2d:
+            return (-_INF, _INF) if _is_identity_bn(m) else None
+        if type(m) is nn.ReLU:
+            return (0.0, _INF)
+        if type(m) in (nn.ReLU6, nn.Hardtanh):                  # ReLU6 is Hardtanh(0, 6)
+            return (float(m.min_val), float(m.max_val))
+        if type(m) is nn.Identity:
+            return (-_INF, _INF)
+        if type(m) is nn.Dropout and not m.training:
+            return (-_INF, _INF)
+        return None
+    if node.op == "call_function":
+        if node.target in (F.relu, torch.relu):
+            return (0.0, _INF)
+        if node.target is F.relu6:
+            return (0.0, 6.0)
+        if node.target is F.hardtanh:
+            return (float(_arg(node, 1, "min_val", -1.0)), float(_arg(node, 2, "max_val", 1.0)))
+        return None
+    if node.op == "call_method" and node.target == "relu":
+        return (0.0, _INF)
+    return None
+
+
+def _compose(first, then):
+    """The one clamp equal to clamp(clamp(v, *first), *then); both keep NaN."""
+    (a, b), (c, d) = first, then
+    return (min(max(a, c), d), max(min(b, d), c))
+
+
+def chain_int8(model: nn.Module, concrete_args=None) -> fx.GraphModule:
+    """A torch.fx GraphModule that computes what `model` computes, with activations kept in int8 between converted
+    convolutions.
+
+    An edge from an Int8Conv2d P to an Int8Conv2d Q (dense or depthwise) is fused when every node from P to Q has exactly
+    one user and every node in between is a pass-through: an exact-identity eval BatchNorm2d (merge_batchnorm's leftover),
+    nn.ReLU / F.relu / torch.relu / .relu(), nn.ReLU6 / F.relu6, nn.Hardtanh / F.hardtanh, nn.Identity, or an eval
+    nn.Dropout.  P then writes Q's int8 NHWC codes (dfq_i8_conv_requant at Q's act_scale, the activations as one clamp),
+    Q reads them, and the nodes in between are deleted (nodes, not modules: a module called elsewhere stays there).  The
+    result is bit-identical to the per-layer path.  A skip connection or any other second user, pooling, add / cat, a
+    BatchNorm that is not an identity, a Linear, or a layer called at several sites ends the chain.
+
+    The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
+    edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order."""
+    tracer = _Int8Tracer()
+    graph = tracer.trace(model, concrete_args)
+    gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
+    mods = dict(gm.named_modules())
+    sites = {}
+    for node in gm.graph.nodes:
+        if node.op == "call_module":
+            sites[node.target] = sites.get(node.target, 0) + 1
+
+    def conv(node):
+        return node.op == "call_module" and isinstance(mods[node.target], Int8Conv2d) and sites[node.target] == 1
+
+    edges, between = [], []
+    for q in list(gm.graph.nodes):
+        if not conv(q) or len(q.args) != 1 or q.kwargs or not isinstance(q.args[0], fx.Node):
+            continue
+        node, clamp, path = q.args[0], (-_INF, _INF), []
+        while len(node.users) == 1:
+            if conv(node):
+                break
+            c = _pass_through(node, mods)
+            if c is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
+                break
+            clamp = _compose(c, clamp)                          # walking backwards: this clamp runs first
+            path.append(node)
+            node = node.args[0]
+        if len(node.users) != 1 or not conv(node) or mods[node.target].out_channels != mods[q.target].in_channels:
+            continue
+        edges.append((node.target, q.target, clamp))
+        between.append((node, q, path))
+    producers = {p: c for p, _, c in edges}
+    consumers = {q for _, q, _ in edges}
+    for target in producers.keys() | consumers:
+        requant = None
+        if target in producers:
+            nxt = mods[next(q for p, q, _ in edges if p == target)]
+            requant = (nxt.act_scale,) + tuple(producers[target])
+        parent, _, attr = target.rpartition(".")
+        setattr(gm.get_submodule(parent) if parent else gm, attr,
+                mods[target].chained(codes_in=target in consumers, requant=requant))
+    for p, q, path in between:
+        q.args = (p,)
+        for node in path:                                       # from the consumer side back: each has no user left
+            gm.graph.erase_node(node)
+    gm.graph.lint()
+    gm.recompile()
+    gm.requantized_edges = edges
+    return gm

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 2
+#define DFQ_ABI_VERSION 3
 
 enum {
   DFQ_OK = 0,
@@ -346,6 +346,15 @@ int dfq_i8_pack_weights(const float* w, const float* w_scale, int8_t* packed, co
  * bias[O] (NULL: none), y fp32 [N, O, OH, OW].  acc_out (NULL: not written) receives the int32 sums, [N, O, OH, OW]. */
 int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, float* y, int32_t* acc_out,
                 const DfqI8Conv* g, void* stream);
+/* The same convolution with a requantizing epilogue, for two layers chained through int8 codes (ncnn's fused requantize):
+ *   v  = fp32(fp32_rn(acc) * dq[o]) + bias[o]
+ *   v  = v < act_lo ? act_lo : (v > act_hi ? act_hi : v)       the activation as one clamp; NaN stays NaN
+ *   yq = q(v, out_scale)                                       out_scale: the NEXT layer's activation scale
+ * yq is int8 NHWC [N, OH, OW, round_up(O, 16)], the layout dfq_i8_quantize_nhwc gives the next layer, whatever the input's
+ * g->Cpad; pad channels are written 0 and nothing past them.  ReLU is (0, +inf), ReLU6 (0, 6), no activation (-inf, +inf).  yq must be 16-byte aligned; NaN or
+ * unordered bounds and an out_scale that is not finite and non-negative are DFQ_E_ARG. */
+int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, int8_t* yq,
+                        float out_scale, float act_lo, float act_hi, const DfqI8Conv* g, void* stream);
 
 #ifdef __cplusplus
 }

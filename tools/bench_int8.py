@@ -5,8 +5,9 @@
 images/s of torchvision MobileNetV2 and ResNet-18 (seeded weights, 224x224) run three ways - int8 execution, the fake-quant path
 of the reference's QuantN* layers, plain fp32 with TF32 off - and the achieved int8 TOPS of dfq_i8_conv on ResNet-18's largest
 GEMM layers against the data-sheet dense peak, and the relative logit error (2-norm over 64 random images) of int8 and of
-fake-quant against fp32.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a
-CUDA device; writes nothing.
+fake-quant against fp32.  `chained`: per-layer int8 against int8.chain_int8 (activations kept in int8 between fused
+convolutions) on the same nets with BN folded - images/s, fused edges, fp32 bytes avoided, bit-identity of the logits.  The
+card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
 """
 import argparse
 import json
@@ -120,6 +121,80 @@ def int8_inference(dev, reps=10, batch=256):
     return out
 
 
+def chained_inference(dev, reps=10, batch=256, rounds=5):
+    """Per-layer int8 execution against int8.chain_int8 (activations kept in int8 between fused convolutions) on torchvision
+    MobileNetV2 (ReLU6 kept) and ResNet-18, BN folded by trace_graph + merge_batchnorm, activation scales 128 / max|input|
+    from forward hooks: images/s and ms per batch of both arms (timed alternately, `rounds` rounds of `reps` passes, median),
+    the fused edges, the fp32 traffic they avoid per batch (computed from shapes) and whether the logits are bit-identical."""
+    import statistics
+    from collections import OrderedDict
+    import torch
+    import torch.nn as nn
+    import torchvision
+    from dfq_b200 import int8
+    from dfq_b200.trace import trace_graph
+    from dfq_b200.utils.layer_transform import merge_batchnorm
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds,
+           "fp32_bytes_avoided_note": "per fused edge and element of the carried tensor: the producer's fp32 store and the "
+                                      "quantizer's fp32 read (8 B) plus a read and a write (8 B) per deleted pass-through op; "
+                                      "the int8 codes (1 B) are written either way"}
+    x = torch.randn(batch, 3, 224, 224, device=dev)
+    for net in ("mobilenet_v2", "resnet18"):
+        torch.manual_seed(0)
+        model = getattr(torchvision.models, net)(num_classes=1000).to(dev).eval()
+        graph, bottoms = trace_graph(model)
+        merge_batchnorm(model, graph, bottoms, [nn.Conv2d])
+        layers = OrderedDict((n, m) for n, m in model.named_modules() if type(m) in (nn.Conv2d, nn.Linear))
+        amax = {}
+        hooks = [m.register_forward_pre_hook(lambda m, i, n=n: amax.__setitem__(n, max(amax.get(n, 0.0), float(i[0].abs().max()))))
+                 for n, m in layers.items()]
+        with torch.no_grad():
+            model(x[:32])
+        for h in hooks:
+            h.remove()
+        int8.convert_to_int8(model, OrderedDict((id(m), m) for m in layers.values()), [nn.Conv2d, nn.Linear],
+                             act_scales=[128. / amax[n] for n in layers])
+        gm = int8.chain_int8(model)
+        edges = gm.requantized_edges
+        traced = int8._Int8Tracer().trace(model)
+        node_of = {n.target: n for n in traced.nodes if n.op == "call_module"}
+        numel, mods = {}, dict(model.named_modules())
+        hooks = [mods[q].register_forward_pre_hook(lambda m, i, q=q: numel.__setitem__(q, i[0].numel())) for _, q, _ in edges]
+        with torch.no_grad():
+            ref = model(x)
+            for h in hooks:
+                h.remove()
+            got = gm(x)
+            torch.cuda.synchronize(dev)
+            avoided = 0
+            for p, q, _ in edges:
+                k, node = 0, node_of[q].args[0]
+                while not (node.op == "call_module" and node.target == p):
+                    k, node = k + 1, node.args[0]
+                avoided += numel[q] * (8 + 8 * k)
+            for _ in range(2):
+                model(x), gm(x)
+            torch.cuda.synchronize(dev)
+            ms = {"per_layer": [], "chained": []}
+            for _ in range(rounds):
+                ms["per_layer"].append(timed(lambda: model(x)))
+                ms["chained"].append(timed(lambda: gm(x)))
+        med = {k: statistics.median(v) for k, v in ms.items()}
+        out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                    "ms_per_batch_rounds": ms, "fused_edges": len(edges), "fp32_bytes_avoided_per_batch": avoided,
+                    "logits_bit_identical": bool(torch.equal(ref.view(torch.int32), got.view(torch.int32)))}
+    return out
+
+
 
 def card():
     """Name and power limit of the GPU (read only)."""
@@ -145,6 +220,7 @@ def main():
         raise SystemExit("bench_int8.py needs a CUDA device (H100)")
     dev = torch.device("cuda", 0)
     res = int8_inference(dev, reps=args.reps, batch=args.batch)
+    res["chained"] = chained_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 

@@ -12,13 +12,21 @@ ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "dfq_b200", "libdfq_sm90.so")
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 names = subprocess.run(["c++filt"], input="\n".join(re.findall(r"Function : (\S+)", sass)), capture_output=True, text=True).stdout.split("\n")
+
+
+def short(name):
+    """`void dfq::(anonymous namespace)::k<(dfq::(anonymous namespace)::Out)1>(...)` -> `void k<Out=1>`"""
+    name = name.replace("(anonymous namespace)::", "").replace("dfq::", "")
+    return re.sub(r"\((\w+)\)(\d+)", r"\1=\2", name).split("(")[0]
+
+
 OPS = ["UBLKCP", "SYNCS", "LDL", "STL", "MUFU", "FRND", "LDS", "STS", "BAR"]
 rows, cur, k = [], None, -1
 for line in sass.splitlines():
     m = re.search(r"Function : (\S+)", line)
     if m:
         k += 1
-        nm = names[k].split("(")[0].replace("dfq::", "")
+        nm = short(names[k])
         cur = [nm, 0, collections.Counter()]
         rows.append(cur)
         continue
@@ -41,5 +49,5 @@ if os.path.exists(log):
     print("\nptxas (`dfq_b200/build.log`): registers / spill bytes per kernel\n\n| kernel | registers | spill stores (B) | spill loads (B) |\n|---|---|---|---|")
     text = open(log).read()
     for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n[^\n]*\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n[^\n]*Used (\d+) registers", text):
-        nm = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip().split("(")[0].replace("dfq::", "")
+        nm = short(subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip())
         print("| `%s` | %s | %s | %s |" % (nm, m.group(5), m.group(3), m.group(4)))
