@@ -9,8 +9,10 @@
 //   k_i8_conv_mma        groups == 1: implicit GEMM on the tensor cores (mma.sync m16n8k32 s8), M = N*OH*OW pixels,
 //                        N = O, K = kh*kw*Cpad; a cp.async ring gathers the im2col rows 16 channels (16 B) at a time
 //   k_i8_conv_dw         groups == C == O: int32 MACs on the CUDA cores over the NHWC codes
-// Both convolutions have two epilogues on one main loop (template parameter Out): fp32 NCHW (dfq_i8_conv), or the next layer's
-// int8 NHWC codes after the activation clamp (dfq_i8_conv_requant), which keeps activations in int8 between chained layers.
+// Both convolutions have three epilogues on one main loop (template parameter Out): fp32 NCHW (dfq_i8_conv); the next layer's
+// int8 NHWC codes after the activation clamp (dfq_i8_conv_requant), which keeps activations in int8 between chained layers;
+// and the residual epilogue (dfq_i8_conv_fused): clamp, fp32 residual add, clamp, then fp32 NCHW and / or the codes, so a
+// residual block's add and an output with several consumers need no separate pass over an fp32 tensor.
 #include <algorithm>
 #include <cmath>
 
@@ -31,7 +33,8 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // Where the epilogue puts its result.  F32: fp32 NCHW y (and optionally the int32 sums).  I8: the codes of the next layer,
 // int8 NHWC yq[N, OH, OW, cpad] (cpad = O rounded up to 16, pad channels 0), requantized at the next layer's scale after
 // the activation clamp [lo, hi].
-enum class Out { F32, I8 };
+// FUSED: Fused below.
+enum class Out { F32, I8, FUSED };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -44,6 +47,32 @@ __device__ __forceinline__ int8_t requant(int32_t acc, float dq, float b, const 
   float v = dequant(acc, dq, b);
   v = v < rq.lo ? rq.lo : (v > rq.hi ? rq.hi : v);
   return q8(v, rq.scale);
+}
+
+// requant()'s clamp (NaN stays NaN) as a function.  requant() keeps its own copy: written through this function, nvcc emits
+// a different (smaller, two registers wider) schedule for the I8 kernels.
+__device__ __forceinline__ float clamp_keep_nan(float v, float lo, float hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+// The residual epilogue (DfqI8Epilogue): y = fp32 NCHW [N, O, OH, OW] and / or yq = int8 NHWC [N, OH, OW, cpad] codes at
+// `scale`, either one NULL; r = fp32 NCHW residual of y's shape, or NULL.  yq and cpad come first, as in Requant, so the
+// code store below serves both.
+struct Fused {
+  int8_t* yq;
+  float scale, pre_lo, pre_hi;
+  int cpad;
+  const float* r;
+  float* y;
+  float post_lo, post_hi;
+};
+template <Out OUT> struct EpiOf { using type = Requant; };
+template <> struct EpiOf<Out::FUSED> { using type = Fused; };
+
+// What the per-layer path computes from the convolution to the tensor after a residual block's add, in its order: the
+// pass-throughs before the add as one clamp, the fp32 add (rv = r[n, o, p], ignored without a residual), the ones after it.
+__device__ __forceinline__ float fused_value(int32_t acc, float dq, float b, float rv, const Fused& e) {
+  float v = clamp_keep_nan(dequant(acc, dq, b), e.pre_lo, e.pre_hi);
+  if (e.r) v = __fadd_rn(v, rv);
+  return clamp_keep_nan(v, e.post_lo, e.post_hi);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -124,7 +153,7 @@ template <Out OUT>
 __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq,
                                                          const float* __restrict__ dq, const float* __restrict__ bias,
                                                          float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
-                                                         Requant rq) {
+                                                         typename EpiOf<OUT>::type rq) {
   __shared__ __align__(128) unsigned char smem[STAGES * STAGE_BYTES];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp >> 1, wn = warp & 1;
@@ -218,6 +247,47 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
+  if constexpr (OUT == Out::FUSED) {
+    // Straight from the accumulator layout: for one register, a warp holds 8 consecutive pixels (m) of 4 channels, so the
+    // residual reads and the fp32 stores run in 32-byte pieces along the pixels of one channel.  A piece is one 32-byte
+    // sector when OH * OW is a multiple of 8; otherwise (7x7, 14x14 maps) it can straddle two sectors or two images.
+    // The codes are staged pixel-major as in the I8 epilogue and stored below.
+    float d[4][2], b[4][2];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int o = o0 + wn * 32 + j * 8 + (lane & 3) * 2 + h;
+        d[j][h] = o < g.O ? dq[o] : 0.f;
+        b[j][h] = o < g.O && bias ? bias[o] : 0.f;
+      }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int ml = wm * 64 + i * 16 + (lane >> 2) + rr * 8;
+        const int64_t m = m0 + ml;
+        const int64_t pix = m < M ? (m / OHW) * g.O * OHW + m % OHW : 0;   // NCHW offset of (n, channel 0, p)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int ol = wn * 32 + j * 8 + (lane & 3) * 2;
+          uint8_t c[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int o = o0 + ol + h;
+            c[h] = 0;
+            if (m < M && o < g.O) {
+              const int64_t idx = pix + (int64_t)o * OHW;
+              const float v = fused_value(acc[i][j][2 * rr + h], d[j][h], b[j][h], rq.r ? rq.r[idx] : 0.f, rq);
+              if (rq.y) rq.y[idx] = v;
+              c[h] = (uint8_t)q8(v, rq.scale);
+            }
+          }
+          if (rq.yq) *reinterpret_cast<uint16_t*>(smem + swz(ml, ol >> 4) + (ol & 15)) = (uint16_t)(c[0] | (c[1] << 8));
+        }
+      }
+    if (!rq.yq) return;
+  }
   if constexpr (OUT == Out::I8) {
     // requantize in registers and stage the codes pixel-major, [m][64 channels] with the A tile's swizzle: the 2-byte stores
     // of a warp (8 pixels x 4 channel pairs) and the 16-byte reads of a quarter warp (2 pixels x 4 chunks) are conflict-free.
@@ -244,6 +314,8 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
           *reinterpret_cast<uint16_t*>(smem + swz(m, ol >> 4) + (ol & 15)) = (uint16_t)(c0 | (c1 << 8));
         }
     }
+  }
+  if constexpr (OUT != Out::F32) {
     __syncthreads();
     // one 16-byte chunk = 16 channels of one pixel; chunks at or past cpad (= O rounded up to 16) are not written
     for (int e = tid; e < BM * (BN / 16); e += THREADS) {
@@ -288,14 +360,14 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
 template <Out OUT>
 __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq, const float* __restrict__ dq,
                              const float* __restrict__ bias, float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
-                             int64_t total, Requant rq) {
+                             int64_t total, typename EpiOf<OUT>::type rq) {
   const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int p = (int)(i % OHW);
     const int64_t t = i / OHW;
     const int ch = (int)(t % chunks);
     const int64_t n = t / chunks;
-    if constexpr (OUT == Out::I8) {
+    if constexpr (OUT != Out::F32) {
       // the input's Cpad may be wider than yq's cpad = round_up(O, 16): chunks past it hold only pad channels, and yq has
       // no room for them
       if (ch * 16 >= rq.cpad) continue;
@@ -319,6 +391,22 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
       }
     }
+    if constexpr (OUT == Out::FUSED) {                          // r and y along the pixels, as the F32 stores
+      alignas(16) int8_t v[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        v[j] = 0;
+        if (c < g.C) {
+          const int64_t idx = (n * g.C + c) * OHW + p;
+          const float f = fused_value(acc[j], dq[c], bias ? bias[c] : 0.f, rq.r ? rq.r[idx] : 0.f, rq);
+          if (rq.y) rq.y[idx] = f;
+          v[j] = q8(f, rq.scale);
+        }
+      }
+      if (rq.yq) *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+      continue;
+    }
     if constexpr (OUT == Out::I8) {                             // the 16 channels of this pixel in one store
       alignas(16) int8_t v[16];
 #pragma unroll
@@ -341,6 +429,14 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
 }
 
 inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
+
+// [a, a + na) and [b, b + nb) share a byte; a NULL range shares none
+inline bool overlap(const void* a, int64_t na, const void* b, int64_t nb) {
+  const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+  return a && b && x < y + (uintptr_t)nb && y < x + (uintptr_t)na;
+}
+
+inline bool ordered(float lo, float hi) { return !std::isnan(lo) && !std::isnan(hi) && lo <= hi; }
 
 int check_geometry(const DfqI8Conv* g) {
   DFQ_REQUIRE(g != nullptr, "dfq_i8: null geometry");
@@ -432,6 +528,39 @@ extern "C" int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const flo
   } else {
     const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
     k_i8_conv_dw<Out::I8><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, rq);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                                 const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(xq && wq && dq && e, "dfq_i8_conv_fused: null pointer");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv_fused: codes must be 16-byte aligned");
+  DFQ_REQUIRE(e->y || e->yq, "dfq_i8_conv_fused: no output requested (y and yq are both NULL)");
+  DFQ_REQUIRE(aligned16(e->yq), "dfq_i8_conv_fused: yq must be 16-byte aligned");
+  DFQ_REQUIRE(((uintptr_t)e->residual & 3) == 0 && ((uintptr_t)e->y & 3) == 0,
+              "dfq_i8_conv_fused: residual and y must be 4-byte aligned");
+  DFQ_REQUIRE(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
+              "dfq_i8_conv_fused: pre / post clamp bounds must be ordered and not NaN");
+  DFQ_REQUIRE(!e->yq || (std::isfinite(e->out_scale) && e->out_scale >= 0.f),
+              "dfq_i8_conv_fused: out_scale must be finite and non-negative when yq is written");
+  const int cpad = (g->O + 15) / 16 * 16;
+  const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
+  const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float), yq_bytes = pixels * cpad;
+  DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes),
+              "dfq_i8_conv_fused: residual overlaps y or yq");
+  DFQ_REQUIRE(!overlap(e->y, y_bytes, e->yq, yq_bytes), "dfq_i8_conv_fused: y overlaps yq");
+  const Fused ep{e->yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, e->residual, e->y, e->post_lo, e->post_hi};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    DFQ_REQUIRE((pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_fused: too many output pixels");
+    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<Out::FUSED><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;

@@ -477,6 +477,7 @@ extern "C" int dfq_struct_size(int which) {
     case 6: return (int)sizeof(DfqBcLayer);
     case 7: return (int)sizeof(DfqQuantTask);
     case 8: return (int)sizeof(DfqI8Conv);
+    case 9: return (int)sizeof(DfqI8Epilogue);
     default: return -1;
   }
 }

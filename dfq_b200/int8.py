@@ -18,6 +18,8 @@ are not the fp32 weights the int8 codes are made from.  The observers replace_op
 tensors between converted layers stay fp32.
 """
 import ctypes as C
+import operator
+from typing import NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -57,15 +59,36 @@ def check_scale(what, scale, layer):
                                 % (layer, what, float(s[i]), " of channel %d" % i if s.size > 1 else "", 128. / s[i]))
 
 
+class Epilogue(NamedTuple):
+    """The residual epilogue of a chained layer (dfq_i8_conv_fused): v = clamp(dequant, *pre); v = v + r when `residual`
+    (forward(x, r)); v = clamp(v, *post); then the codes of v at out_scale (None: no codes) and / or v in fp32 (`fp32`).
+    Both clamps keep NaN, (-inf, inf) is none."""
+    out_scale: Optional[float] = None
+    pre: Tuple[float, float] = (-float("inf"), float("inf"))
+    post: Tuple[float, float] = (-float("inf"), float("inf"))
+    residual: bool = False
+    fp32: bool = False
+
+
+def _ordered(lo, hi, what="activation"):
+    lo, hi = _f32(lo), _f32(hi)
+    if np.isnan(lo) or np.isnan(hi) or lo > hi:
+        raise _lib.DfqError("%s bounds (%g, %g) must be ordered and not NaN" % (what, lo, hi))
+    return float(lo), float(hi)
+
+
 class _Int8Layer(nn.Module):
     """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves.
 
-    Two execution modes, set only on the copies chain_int8 makes (`chained`): `codes_in` - the input is already int8 NHWC
-    codes [N, H, W, cpad] at this layer's act_scale; `requant` = (out_scale, lo, hi) - the output is the next layer's int8
-    NHWC codes (dfq_i8_conv_requant) instead of fp32 NCHW.  A layer convert_to_int8 made takes and returns fp32 only."""
+    Execution modes, set only on the copies chain_int8 makes (`chained`): `codes_in` - the input is already int8 NHWC codes
+    [N, H, W, cpad] at this layer's act_scale; `requant` = (out_scale, lo, hi) - the output is the next layer's int8 NHWC
+    codes (dfq_i8_conv_requant) instead of fp32 NCHW; `epilogue` - the residual epilogue (dfq_i8_conv_fused, see Epilogue).
+    A layer convert_to_int8 made takes and returns fp32 only."""
 
     codes_in = False
     requant = None
+    epilogue = None
+    layer_name = None
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
         super().__init__()
@@ -108,10 +131,11 @@ class _Int8Layer(nn.Module):
             g[0][k] = v
         return g
 
-    def chained(self, codes_in=False, requant=None):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None):
         """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
-        mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes.  self is not
-        modified."""
+        mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes; epilogue - an
+        Epilogue: the residual epilogue (not together with requant).  name: the layer's name in error messages.  self is
+        not modified."""
         new = type(self).__new__(type(self))
         nn.Module.__init__(new)
         for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad", "act_scale"):
@@ -119,19 +143,35 @@ class _Int8Layer(nn.Module):
         for k, b in self._buffers.items():
             new.register_buffer(k, b)
         new.codes_in = bool(codes_in)
+        new.layer_name = name
+        if requant is not None and epilogue is not None:
+            raise _lib.DfqError("layer %s: requant and epilogue are two output modes; give one" % new._who())
         if requant is not None:
             s, lo, hi = requant
             check_scale("output", s, "%s -> next layer" % type(self).__name__)
-            lo, hi = _f32(lo), _f32(hi)
-            if np.isnan(lo) or np.isnan(hi) or lo > hi:
-                raise _lib.DfqError("activation bounds (%g, %g) must be ordered and not NaN" % (lo, hi))
-            requant = (float(_f32(s)), float(lo), float(hi))
+            lo, hi = _ordered(lo, hi, "activation")
+            requant = (float(_f32(s)), lo, hi)
         new.requant = requant
+        if epilogue is not None:
+            e = Epilogue(*epilogue)
+            if e.out_scale is None and not e.fp32:
+                raise _lib.DfqError("layer %s: the epilogue returns neither codes nor fp32" % new._who())
+            if e.out_scale is not None:
+                check_scale("output", e.out_scale, "%s -> next layer" % new._who())
+            epilogue = Epilogue(None if e.out_scale is None else float(_f32(e.out_scale)), _ordered(*e.pre, what="pre-add"),
+                                _ordered(*e.post, what="post-add"), bool(e.residual), bool(e.fp32))
+        new.epilogue = epilogue
         return new
 
-    def run(self, x, with_acc=False):
+    def _who(self):
+        return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
+                                                                  self.kernel_size)
+
+    def run(self, x, with_acc=False, residual=None):
         """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue.  In the chained modes
-        x is int8 codes [N, H, W, cpad] (codes_in) and y int8 codes [N, OH, OW, round_up(C_out, 16)] (requant)."""
+        x is int8 codes [N, H, W, cpad] (codes_in) and y int8 codes [N, OH, OW, round_up(C_out, 16)] (requant).  With an
+        epilogue, y is the codes, the fp32 output, or (codes, fp32 output) when it returns both, and `residual` is the fp32
+        tensor [N, C_out, OH, OW] the epilogue adds (exactly that shape, no broadcasting, on x's device)."""
         if not x.is_cuda or not self.dq.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.dq.device))
@@ -144,8 +184,11 @@ class _Int8Layer(nn.Module):
             raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s %s" % (self.in_channels, x.dtype, tuple(x.shape)))
         else:
             N, _, H, W = x.shape
-        if self.requant is not None and with_acc:
+        if (self.requant is not None or self.epilogue is not None) and with_acc:
             raise _lib.DfqError("a requantizing int8 layer does not return its int32 sums")
+        if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
+            raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
+                                                    "takes no residual input"))
         x = x.contiguous()
         g = self._geometry(N, H, W)
         OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
@@ -158,6 +201,8 @@ class _Int8Layer(nn.Module):
             xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
             _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, self.in_channels, H, W, self.cpad,
                                                 C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
+        if self.epilogue is not None:
+            return self._run_fused(xq, residual, g, N, OH, OW), None
         if self.requant is not None:
             s, lo, hi = self.requant
             yq = torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=x.device)
@@ -171,6 +216,28 @@ class _Int8Layer(nn.Module):
                                    _lib.table_ptr(g), st), "dfq_i8_conv")
         return y, acc
 
+    def _run_fused(self, xq, r, g, N, OH, OW):
+        e = self.epilogue
+        shape = (N, self.out_channels, OH, OW)
+        if r is not None:
+            if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
+                    r.device != xq.device:
+                raise _lib.DfqError("layer %s: the residual must be fp32 %s on %s, got %s" % (
+                    self._who(), list(shape), xq.device, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
+                    if isinstance(r, torch.Tensor) else type(r).__name__))
+            r = r.contiguous()
+        yq = None if e.out_scale is None else \
+            torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=xq.device)
+        y = torch.empty(shape, dtype=torch.float32, device=xq.device) if e.fp32 else None
+        d = np.zeros(1, _lib.I8_EPILOGUE_DT)
+        d[0] = (0 if r is None else r.data_ptr(), 0 if y is None else y.data_ptr(), 0 if yq is None else yq.data_ptr(),
+                0.0 if e.out_scale is None else e.out_scale) + e.pre + e.post
+        lib = _lib.load()
+        _lib.check(lib.dfq_i8_conv_fused(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                         _lib.table_ptr(d), _lib.table_ptr(g), _lib.stream_ptr()),
+                   "dfq_i8_conv_fused (layer %s)" % self._who())
+        return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
+
 
 class Int8Conv2d(_Int8Layer):
     """nn.Conv2d executed in int8 (zero padding; groups == 1 or depthwise)."""
@@ -182,8 +249,8 @@ class Int8Conv2d(_Int8Layer):
                                 % (conv.padding, conv.padding_mode))
         return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
 
-    def forward(self, x):
-        return self.run(x)[0]
+    def forward(self, x, r=None):
+        return self.run(x, residual=r)[0]
 
     def extra_repr(self):
         return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act_scale=%g" % (
@@ -314,7 +381,21 @@ def _compose(first, then):
     return (min(max(a, c), d), max(min(b, d), c))
 
 
-def chain_int8(model: nn.Module, concrete_args=None) -> fx.GraphModule:
+def _is_identity(node, mods):
+    """An exact-identity pass-through: an identity eval BatchNorm2d, nn.Identity or an eval nn.Dropout (no clamp)."""
+    return node.op == "call_module" and type(mods[node.target]) in (nn.BatchNorm2d, nn.Identity, nn.Dropout) and \
+        _pass_through(node, mods) == (-_INF, _INF)
+
+
+def _is_add(node):
+    """operator.add / torch.add / Tensor.add of two distinct fx nodes, without alpha or out."""
+    add = (node.op == "call_function" and node.target in (operator.add, torch.add)) or \
+        (node.op == "call_method" and node.target == "add")
+    return add and not node.kwargs and len(node.args) == 2 and all(isinstance(a, fx.Node) for a in node.args) and \
+        node.args[0] is not node.args[1]
+
+
+def chain_int8(model: nn.Module, concrete_args=None, residual=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` computes, with activations kept in int8 between converted
     convolutions.
 
@@ -326,8 +407,25 @@ def chain_int8(model: nn.Module, concrete_args=None) -> fx.GraphModule:
     result is bit-identical to the per-layer path.  A skip connection or any other second user, pooling, add / cat, a
     BatchNorm that is not an identity, a Linear, or a layer called at several sites ends the chain.
 
+    residual=True adds residual blocks and tensors with several consumers (dfq_i8_conv_fused, `Epilogue`), still
+    bit-identical to the per-layer path:
+    - fan-out: from an Int8Conv2d P, forward through single-user pass-throughs to a node with several users.  Its Int8Conv2d
+      users (single-site, channels matching) take P's codes when their act_scale equals, bit for bit, the first such user's
+      in graph order; every other user, a convolution at another scale included, takes P's fp32 output of the same launch.
+    - residual add: operator.add / torch.add / Tensor.add of two distinct nodes, without alpha or out.  The fused operand is
+      the first argument whose chain back to an Int8Conv2d P is all single-user pass-throughs (they give the clamp before
+      the add); the other is P's residual input, with its exact-identity pass-throughs (identity BatchNorm, Identity, eval
+      Dropout, single-user) skipped.  Single-user pass-throughs after the add give the clamp after it, and the fan-out rule
+      applies to the result.  P moves to the add's position (its residual may be computed after it in graph order, as in
+      ResNet's downsample blocks).
+    The deleted pass-throughs' and adds' fp32 value is P's fp32 output.  Adds whose operands differ in shape raise DfqError
+    naming the layer when the module runs (no broadcasting).
+
     The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
-    edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order."""
+    edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) being the
+    clamp the consumer's codes were taken after; with residual=True also the fused adds in `fused_adds`: (producer name,
+    add node name, residual node name, (lo, hi) before the add, (lo, hi) after it) in graph order, node names being those
+    of the traced model (a residual another fusion deleted is that producer's fp32 output in the result)."""
     tracer = _Int8Tracer()
     graph = tracer.trace(model, concrete_args)
     gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
@@ -339,6 +437,9 @@ def chain_int8(model: nn.Module, concrete_args=None) -> fx.GraphModule:
 
     def conv(node):
         return node.op == "call_module" and isinstance(mods[node.target], Int8Conv2d) and sites[node.target] == 1
+
+    if residual:
+        return _chain_residual(gm, mods, conv)
 
     edges, between = [], []
     for q in list(gm.graph.nodes):
@@ -375,4 +476,121 @@ def chain_int8(model: nn.Module, concrete_args=None) -> fx.GraphModule:
     gm.graph.lint()
     gm.recompile()
     gm.requantized_edges = edges
+    return gm
+
+
+def _chain_residual(gm, mods, conv):
+    """chain_int8(..., residual=True) on the traced `gm` (see chain_int8)."""
+    full = (-_INF, _INF)
+    order = {n: i for i, n in enumerate(gm.graph.nodes)}
+
+    def producer(node):
+        return conv(node) and len(node.args) == 1 and not node.kwargs and isinstance(node.args[0], fx.Node)
+
+    def forward(node, clamp):
+        """Walk from node through single-user pass-throughs: (last node, composed clamp, the pass-throughs)."""
+        path = []
+        while len(node.users) == 1:
+            u = next(iter(node.users))
+            c = _pass_through(u, mods)
+            if c is None or len(u.all_input_nodes) != 1 or u.args[0] is not node:
+                break
+            clamp, node = _compose(clamp, c), u
+            path.append(u)
+        return node, clamp, path
+
+    def back_to_producer(node):
+        """The producer whose single-user pass-through chain ends at `node`, or None."""
+        while len(node.users) == 1 and not producer(node):
+            if _pass_through(node, mods) is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
+                return None
+            node = node.args[0]
+        return node if len(node.users) == 1 and producer(node) else None
+
+    plans = []
+    for p in list(gm.graph.nodes):
+        if not producer(p):
+            continue
+        end, pre, path = forward(p, full)
+        add, ri, post, post_path, tail = None, None, full, [], end
+        if len(end.users) == 1:
+            a = next(iter(end.users))
+            if _is_add(a):
+                fused = next((i for i, v in enumerate(a.args) if back_to_producer(v) is not None), None)
+                if fused is not None and a.args[fused] is end:
+                    add, ri = a, 1 - fused
+                    tail, post, post_path = forward(a, full)
+        codes, scale = [], None
+        out_c = mods[p.target].out_channels
+        for u in sorted(tail.users, key=order.get):
+            if producer(u) and u.args[0] is tail and mods[u.target].in_channels == out_c:
+                s = _f32(mods[u.target].act_scale)
+                if scale is None or s.view(np.int32) == scale.view(np.int32):
+                    scale = s
+                    codes.append(u)
+        if add is None and not codes:
+            continue
+        plans.append(dict(p=p, path=path, pre=pre, add=add, ri=ri, post=post, post_path=post_path, tail=tail, codes=codes))
+
+    # the residual's exact identities, skipped once every plan's own nodes are known: a node another plan deletes (an
+    # identity at the end of its post-add chain, say) stays the residual, and that plan replaces it by its fp32 output
+    claimed = {n for pl in plans for n in (pl["p"], *pl["path"], *([pl["add"]] if pl["add"] is not None else []),
+                                            *pl["post_path"])}
+    for pl in plans:
+        pl["skipped"] = []
+        if pl["add"] is None:
+            continue
+        r = pl["add"].args[pl["ri"]]
+        while r not in claimed and len(r.users) == 1 and _is_identity(r, mods) and isinstance(r.args[0], fx.Node):
+            pl["skipped"].append(r)
+            r = r.args[0]
+        pl["r_name"] = r.name
+
+    # rewrite in producer order: a producer's input may be the codes of an earlier one, and a residual its fp32 output
+    g = gm.graph
+    edges, adds, modes = [], [], {}
+    for pl in plans:
+        p, add, tail = pl["p"], pl["add"], pl["tail"]
+        if add is not None:
+            for node in pl["skipped"]:                          # from the add back: each loses its only user
+                node.replace_all_uses_with(node.args[0])
+                g.erase_node(node)
+            add.prepend(p)
+            p.args = (p.args[0], add.args[pl["ri"]])
+        fp32 = any(u not in pl["codes"] for u in tail.users)
+        scale = float(_f32(mods[pl["codes"][0].target].act_scale)) if pl["codes"] else None
+        clamp = pl["post"] if add is not None else pl["pre"]
+        if add is None and not fp32:
+            modes[p.target] = ("requant", (scale,) + tuple(clamp))
+            codes_node = y_node = p
+        else:
+            modes[p.target] = ("epilogue", Epilogue(scale, pl["pre"], pl["post"], add is not None, fp32))
+            codes_node = y_node = p
+            if scale is not None and fp32:
+                with g.inserting_after(p):
+                    y_node = g.call_function(operator.getitem, (p, 1))
+                with g.inserting_after(p):
+                    codes_node = g.call_function(operator.getitem, (p, 0))
+        for u in pl["codes"]:
+            u.replace_input_with(tail, codes_node)
+            edges.append((p.target, u.target, clamp))
+        if tail is not p:
+            tail.replace_all_uses_with(y_node)
+            for node in reversed([*pl["path"], *([add] if add is not None else []), *pl["post_path"]]):
+                g.erase_node(node)
+        else:
+            p.replace_all_uses_with(y_node, delete_user_cb=lambda u: u not in (y_node, codes_node))
+        if add is not None:
+            adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
+    consumers = {q for _, q, _ in edges}
+    for target in modes.keys() | consumers:
+        kind, arg = modes.get(target, (None, None))
+        parent, _, attr = target.rpartition(".")
+        setattr(gm.get_submodule(parent) if parent else gm, attr,
+                mods[target].chained(codes_in=target in consumers, name=target,
+                                     requant=arg if kind == "requant" else None, epilogue=arg if kind == "epilogue" else None))
+    g.lint()
+    gm.recompile()
+    gm.requantized_edges = edges
+    gm.fused_adds = adds
     return gm

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 3
+#define DFQ_ABI_VERSION 4
 
 enum {
   DFQ_OK = 0,
@@ -43,7 +43,7 @@ enum {
 int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
- * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv): lets a binding verify
+ * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -355,6 +355,28 @@ int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, const float
  * unordered bounds and an out_scale that is not finite and non-negative are DFQ_E_ARG. */
 int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, int8_t* yq,
                         float out_scale, float act_lo, float act_hi, const DfqI8Conv* g, void* stream);
+
+/* The residual epilogue of dfq_i8_conv_fused: the convolution, the pass-throughs up to a residual block's add, the add and
+ * the pass-throughs after it, in one launch.  Per output element (n, o, p):
+ *   v  = fp32(fp32_rn(acc) * dq[o]) + bias[o]
+ *   v  = v < pre_lo ? pre_lo : (v > pre_hi ? pre_hi : v)       NaN stays NaN
+ *   v  = fp32(v + residual[n, o, p])                           only when residual != NULL: fp32 NCHW [N, O, OH, OW]
+ *   v  = v < post_lo ? post_lo : (v > post_hi ? post_hi : v)
+ *   y[n, o, p]  = v                                            when y != NULL: fp32 NCHW [N, O, OH, OW]
+ *   yq[n, p, o] = q(v, out_scale)                              when yq != NULL: int8 NHWC [N, OH, OW, round_up(O, 16)], as
+ *                                                              dfq_i8_conv_requant writes it (pad channels 0)
+ * No clamp is (-inf, +inf). */
+typedef struct DfqI8Epilogue {
+  const float* residual;
+  float* y;
+  int8_t* yq;
+  float out_scale, pre_lo, pre_hi, post_lo, post_hi;
+} DfqI8Epilogue;
+/* The convolution of dfq_i8_conv with the epilogue *e.  DFQ_E_ARG, with a reason: y and yq both NULL, yq not 16-byte
+ * aligned, residual or y not 4-byte aligned, NaN or unordered bounds in either clamp, an out_scale that is not finite and non-negative while yq is written,
+ * a residual that overlaps y or yq, or y overlapping yq (extents from the geometry).  Grouping as dfq_i8_conv. */
+int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                      const DfqI8Conv* g, void* stream);
 
 #ifdef __cplusplus
 }

@@ -6,8 +6,9 @@ images/s of torchvision MobileNetV2 and ResNet-18 (seeded weights, 224x224) run 
 of the reference's QuantN* layers, plain fp32 with TF32 off - and the achieved int8 TOPS of dfq_i8_conv on ResNet-18's largest
 GEMM layers against the data-sheet dense peak, and the relative logit error (2-norm over 64 random images) of int8 and of
 fake-quant against fp32.  `chained`: per-layer int8 against int8.chain_int8 (activations kept in int8 between fused
-convolutions) on the same nets with BN folded - images/s, fused edges, fp32 bytes avoided, bit-identity of the logits.  The
-card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
+convolutions) on the same nets with BN folded - images/s, fused edges, fp32 bytes avoided, bit-identity of the logits.
+`residual`: per-layer against chain_int8 and chain_int8(residual=True) (residual adds and tensors with several consumers
+fused too), the same way, with the fused adds.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
 """
 import argparse
 import json
@@ -195,6 +196,98 @@ def chained_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def residual_inference(dev, reps=10, batch=256, rounds=5):
+    """Per-layer int8 execution against int8.chain_int8 and int8.chain_int8(residual=True) on the nets of chained_inference
+    (timed alternately, `rounds` rounds of `reps` passes, median): images/s, ms per batch, edges and fused adds, the fp32
+    traffic the residual arm avoids per batch against the per-layer path (computed from shapes) and bit-identity of the
+    logits."""
+    import statistics
+    from collections import OrderedDict
+    import torch
+    import torch.nn as nn
+    import torchvision
+    from dfq_b200 import int8
+    from dfq_b200.trace import trace_graph
+    from dfq_b200.utils.layer_transform import merge_batchnorm
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds,
+           "fp32_bytes_avoided_note": "fp32 bytes of the per-layer path that the residual arm does not move, per batch: per "
+                                      "element of every carried tensor, the quantizer's fp32 read (4 B) per carried consumer, "
+                                      "plus the producer's fp32 store (4 B) when no fp32 consumer is left; a read and a write "
+                                      "(8 B) per deleted pass-through and per deleted identity on a residual; per fused add, "
+                                      "its two reads and its write (12 B)"}
+    x = torch.randn(batch, 3, 224, 224, device=dev)
+    for net in ("mobilenet_v2", "resnet18"):
+        torch.manual_seed(0)
+        model = getattr(torchvision.models, net)(num_classes=1000).to(dev).eval()
+        graph, bottoms = trace_graph(model)
+        merge_batchnorm(model, graph, bottoms, [nn.Conv2d])
+        layers = OrderedDict((n, m) for n, m in model.named_modules() if type(m) in (nn.Conv2d, nn.Linear))
+        amax = {}
+        hooks = [m.register_forward_pre_hook(lambda m, i, n=n: amax.__setitem__(n, max(amax.get(n, 0.0), float(i[0].abs().max()))))
+                 for n, m in layers.items()]
+        with torch.no_grad():
+            model(x[:32])
+        for h in hooks:
+            h.remove()
+        int8.convert_to_int8(model, OrderedDict((id(m), m) for m in layers.values()), [nn.Conv2d, nn.Linear],
+                             act_scales=[128. / amax[n] for n in layers])
+        chained = int8.chain_int8(model)
+        gm = int8.chain_int8(model, residual=True)
+        # bytes from shapes: every node of the per-layer graph the residual arm deleted or made int8
+        traced = int8._Int8Tracer().trace(model)
+        kept = {n.name for n in gm.graph.nodes}
+        numel, mods = {}, dict(model.named_modules())
+        hooks = [m.register_forward_hook(lambda m, i, o, n=n: numel.__setitem__(n, o.numel())) for n, m in mods.items()
+                 if isinstance(m, int8.Int8Conv2d)]
+        with torch.no_grad():
+            ref = model(x)
+            for h in hooks:
+                h.remove()
+            got = {"chained": chained(x), "residual": gm(x)}
+            torch.cuda.synchronize(dev)
+            avoided = 0
+            for p, q, _ in gm.requantized_edges:
+                avoided += 4 * numel[p]
+            for p, epi in ((n, getattr(m, "epilogue", None)) for n, m in gm.named_modules()):
+                if isinstance(mods.get(p), int8.Int8Conv2d) and (epi is None or not epi.fp32) and \
+                        p in {e[0] for e in gm.requantized_edges}:
+                    avoided += 4 * numel[p]
+            node_out = {n.target: n for n in traced.nodes if n.op == "call_module"}
+            for n in traced.nodes:
+                if n.name in kept or n.op not in ("call_module", "call_function", "call_method"):
+                    continue
+                src = n.args[0] if n.args and isinstance(n.args[0], torch.fx.Node) else None
+                while src is not None and not (src.op == "call_module" and src.target in node_out and
+                                               isinstance(mods.get(src.target), int8.Int8Conv2d)):
+                    src = src.args[0] if src.args and isinstance(src.args[0], torch.fx.Node) else None
+                if src is not None:
+                    avoided += numel[src.target] * (12 if int8._is_add(n) else 8)
+            for _ in range(2):
+                model(x), chained(x), gm(x)
+            torch.cuda.synchronize(dev)
+            ms = {"per_layer": [], "chained": [], "residual": []}
+            for _ in range(rounds):
+                ms["per_layer"].append(timed(lambda: model(x)))
+                ms["chained"].append(timed(lambda: chained(x)))
+                ms["residual"].append(timed(lambda: gm(x)))
+        med = {k: statistics.median(v) for k, v in ms.items()}
+        out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                    "ms_per_batch_rounds": ms, "edges": {"chained": len(chained.requantized_edges),
+                                                         "residual": len(gm.requantized_edges)},
+                    "fused_adds": len(gm.fused_adds), "fp32_bytes_avoided_per_batch": avoided,
+                    "logits_bit_identical": {k: bool(torch.equal(ref.view(torch.int32), v.view(torch.int32)))
+                                             for k, v in got.items()}}
+    return out
+
 
 def card():
     """Name and power limit of the GPU (read only)."""
@@ -221,6 +314,7 @@ def main():
     dev = torch.device("cuda", 0)
     res = int8_inference(dev, reps=args.reps, batch=args.batch)
     res["chained"] = chained_inference(dev, reps=args.reps, batch=args.batch)
+    res["residual"] = residual_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
