@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
@@ -82,12 +82,16 @@ I8_CONV_DT = np.dtype([(f, np.int32) for f in (
 I8_EPILOGUE_DT = np.dtype([("residual", np.uint64), ("y", np.uint64), ("yq", np.uint64)] +
                           [(f, np.float32) for f in ("out_scale", "pre_lo", "pre_hi", "post_lo", "post_hi")], align=True)
 
+I8_POOL_DT = np.dtype([(f, np.int32) for f in (
+    "N", "C", "H", "W", "kh", "kw", "stride_h", "stride_w", "pad_h", "pad_w", "dil_h", "dil_w", "ceil_mode", "OH", "OW",
+    "Cpad")], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 64), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
     "DfqCleResult": (CLE_RESULT_DT, 528), "DfqFold": (FOLD_DT, 64), "DfqExpectTerm": (TERM_DT, 32),
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
-    "DfqI8Epilogue": (I8_EPILOGUE_DT, 48),
+    "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64),
 }
 
 _PF = C.c_void_p   # device float*
@@ -136,6 +140,8 @@ SIGNATURES = {
     "dfq_i8_conv": [C.c_void_p, C.c_void_p, _PF, _PF, _PF, C.c_void_p, C.c_void_p, _ST],
     "dfq_i8_conv_requant": [C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p, _ST],
     "dfq_i8_conv_fused": [C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_conv_slice": [C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _I32, _I32, C.c_void_p, _ST],
+    "dfq_i8_maxpool": [C.c_void_p, _PF, _PF, C.c_void_p, C.c_float, C.c_void_p, _ST],
 }
 
 _lib = None

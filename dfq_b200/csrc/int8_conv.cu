@@ -12,7 +12,9 @@
 // Both convolutions have three epilogues on one main loop (template parameter Out): fp32 NCHW (dfq_i8_conv); the next layer's
 // int8 NHWC codes after the activation clamp (dfq_i8_conv_requant), which keeps activations in int8 between chained layers;
 // and the residual epilogue (dfq_i8_conv_fused): clamp, fp32 residual add, clamp, then fp32 NCHW and / or the codes, so a
-// residual block's add and an output with several consumers need no separate pass over an fp32 tensor.
+// residual block's add and an output with several consumers need no separate pass over an fp32 tensor.  The code stores of
+// the last two can target a channel slice of a wider tensor (dfq_i8_conv_slice), so the producers of a channel
+// concatenation write the consumer's input directly; k_i8_maxpool pools codes, or fp32 to fp32 and / or codes.
 #include <algorithm>
 #include <cmath>
 
@@ -34,11 +36,13 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // int8 NHWC yq[N, OH, OW, cpad] (cpad = O rounded up to 16, pad channels 0), requantized at the next layer's scale after
 // the activation clamp [lo, hi].
 // FUSED: Fused below.
+// Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
+// wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
 enum class Out { F32, I8, FUSED };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
-  int cpad;
+  int cpad, cstride;
 };
 
 // What the per-layer path computes between two layers, in its order: dequant(), the activation (relu / relu6 / hardtanh,
@@ -59,7 +63,7 @@ __device__ __forceinline__ float clamp_keep_nan(float v, float lo, float hi) { r
 struct Fused {
   int8_t* yq;
   float scale, pre_lo, pre_hi;
-  int cpad;
+  int cpad, cstride;
   const float* r;
   float* y;
   float post_lo, post_hi;
@@ -323,7 +327,7 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
       const int64_t m = m0 + ml;
       const int o = o0 + c * 16;
       if (m >= M || o >= rq.cpad) continue;
-      *reinterpret_cast<int4*>(rq.yq + m * rq.cpad + o) = *reinterpret_cast<const int4*>(smem + swz(ml, c));
+      *reinterpret_cast<int4*>(rq.yq + m * rq.cstride + o) = *reinterpret_cast<const int4*>(smem + swz(ml, c));
     }
     return;
   }
@@ -404,7 +408,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
           v[j] = q8(f, rq.scale);
         }
       }
-      if (rq.yq) *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+      if (rq.yq) *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cstride + ch * 16) = *reinterpret_cast<const int4*>(v);
       continue;
     }
     if constexpr (OUT == Out::I8) {                             // the 16 channels of this pixel in one store
@@ -414,7 +418,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         const int c = ch * 16 + j;
         v[j] = c < g.C ? requant(acc[j], dq[c], bias ? bias[c] : 0.f, rq) : (int8_t)0;
       }
-      *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+      *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cstride + ch * 16) = *reinterpret_cast<const int4*>(v);
       continue;
     }
 #pragma unroll
@@ -425,6 +429,72 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
       y[idx] = dequant(acc[j], dq[c], bias ? bias[c] : 0.f);
       if (acc_out) acc_out[idx] = acc[j];
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// max pooling: one thread per (n, 16 channels, output pixel), pixels fastest, as k_i8_conv_dw
+// ------------------------------------------------------------------------------------------------------------------
+// CODES: xq int8 NHWC [N, H, W, Cpad] -> yq int8 NHWC [N, OH, OW, Cpad], a byte-wise signed max of 16-byte taps.  q8() is
+// monotone non-decreasing for a scale >= 0, so the max of the codes is the code of the max for any window without NaN.
+// A window with no tap inside the input (possible with dilation) is -inf in torch, whose code is -127; pad channels 0.
+// !CODES: x fp32 NCHW [N, C, H, W] -> y fp32 NCHW [N, C, OH, OW] and / or yq int8 NHWC at `scale`, with torch's CUDA rule:
+// from -inf, taps row-major, the running max replaced when v > m or v is NaN (so the first of tied values is kept).
+template <bool CODES>
+__global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restrict__ x, float* __restrict__ y,
+                             int8_t* __restrict__ yq, float scale, DfqI8Pool g, int64_t total) {
+  const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int p = (int)(i % OHW);
+    const int64_t t = i / OHW;
+    const int ch = (int)(t % chunks);
+    const int64_t n = t / chunks;
+    const int h0 = (p / g.OW) * g.stride_h - g.pad_h, w0 = (p % g.OW) * g.stride_w - g.pad_w;
+    alignas(16) int8_t v[16];
+    if constexpr (CODES) {
+      const int8_t* img = xq + n * g.H * g.W * g.Cpad + ch * 16;
+      int m[4] = {(int)0x81818181, (int)0x81818181, (int)0x81818181, (int)0x81818181};
+      bool any = false;
+      for (int r = 0; r < g.kh; ++r) {
+        const int ih = h0 + r * g.dil_h;
+        if ((unsigned)ih >= (unsigned)g.H) continue;
+        for (int s = 0; s < g.kw; ++s) {
+          const int iw = w0 + s * g.dil_w;
+          if ((unsigned)iw >= (unsigned)g.W) continue;
+          const int4 q = __ldg(reinterpret_cast<const int4*>(img + ((int64_t)ih * g.W + iw) * g.Cpad));
+          m[0] = __vmaxs4(m[0], q.x), m[1] = __vmaxs4(m[1], q.y), m[2] = __vmaxs4(m[2], q.z), m[3] = __vmaxs4(m[3], q.w);
+          any = true;
+        }
+      }
+      *reinterpret_cast<int4*>(v) = make_int4(m[0], m[1], m[2], m[3]);
+      if (!any) {
+#pragma unroll
+        for (int j = 0; j < 16; ++j) v[j] = ch * 16 + j < g.C ? (int8_t)-127 : (int8_t)0;
+      }
+    } else {
+#pragma unroll 1
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        v[j] = 0;
+        if (c >= g.C) continue;
+        const float* img = x + (n * g.C + c) * g.H * g.W;
+        float mx = -INFINITY;
+        for (int r = 0; r < g.kh; ++r) {
+          const int ih = h0 + r * g.dil_h;
+          if ((unsigned)ih >= (unsigned)g.H) continue;
+          for (int s = 0; s < g.kw; ++s) {
+            const int iw = w0 + s * g.dil_w;
+            if ((unsigned)iw >= (unsigned)g.W) continue;
+            const float f = __ldg(img + (int64_t)ih * g.W + iw);
+            if (f > mx || isnan(f)) mx = f;
+          }
+        }
+        if (y) y[(n * g.C + c) * OHW + p] = mx;
+        v[j] = q8(mx, scale);
+      }
+      if (!yq) continue;
+    }
+    *reinterpret_cast<int4*>(yq + (n * OHW + p) * g.Cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
   }
 }
 
@@ -453,6 +523,14 @@ int check_geometry(const DfqI8Conv* g) {
     return DFQ_E_UNSUPPORTED;
   }
   return 0;
+}
+
+// torch's pooling_output_shape: floor division, and in ceil mode the last window starts inside the input or its left pad
+int pool_extent(int in, int k, int pad, int stride, int dil, bool ceil_mode) {
+  const int64_t num = (int64_t)in + 2 * pad - (int64_t)dil * (k - 1) - 1 + (ceil_mode ? stride - 1 : 0);
+  int64_t out = (num >= 0 ? num / stride : -((-num + stride - 1) / stride)) + 1;
+  if (ceil_mode && (out - 1) * stride >= (int64_t)in + pad) --out;
+  return (int)out;
 }
 
 int grid_for(int64_t total, int threads) {
@@ -518,7 +596,8 @@ extern "C" int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const flo
   DFQ_REQUIRE(!std::isnan(act_lo) && !std::isnan(act_hi) && act_lo <= act_hi,
               "dfq_i8_conv_requant: activation bounds must be ordered and not NaN");
   DFQ_REQUIRE(std::isfinite(out_scale) && out_scale >= 0.f, "dfq_i8_conv_requant: out_scale must be finite and non-negative");
-  const Requant rq{yq, out_scale, act_lo, act_hi, (g->O + 15) / 16 * 16};
+  const int cpad = (g->O + 15) / 16 * 16;
+  const Requant rq{yq, out_scale, act_lo, act_hi, cpad, cpad};
   cudaStream_t st = (cudaStream_t)stream;
   if (g->groups == 1) {
     const int64_t M = (int64_t)g->N * g->OH * g->OW;
@@ -552,7 +631,7 @@ extern "C" int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float
   DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes),
               "dfq_i8_conv_fused: residual overlaps y or yq");
   DFQ_REQUIRE(!overlap(e->y, y_bytes, e->yq, yq_bytes), "dfq_i8_conv_fused: y overlaps yq");
-  const Fused ep{e->yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, e->residual, e->y, e->post_lo, e->post_hi};
+  const Fused ep{e->yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cpad, e->residual, e->y, e->post_lo, e->post_hi};
   cudaStream_t st = (cudaStream_t)stream;
   if (g->groups == 1) {
     DFQ_REQUIRE((pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_fused: too many output pixels");
@@ -561,6 +640,86 @@ extern "C" int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float
   } else {
     const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
     k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                                 int32_t coff, int32_t cstride, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(xq && wq && dq && e, "dfq_i8_conv_slice: null pointer");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv_slice: codes must be 16-byte aligned");
+  DFQ_REQUIRE(e->yq, "dfq_i8_conv_slice: no codes requested (yq is NULL)");
+  DFQ_REQUIRE(aligned16(e->yq), "dfq_i8_conv_slice: yq must be 16-byte aligned");
+  DFQ_REQUIRE(((uintptr_t)e->residual & 3) == 0 && ((uintptr_t)e->y & 3) == 0,
+              "dfq_i8_conv_slice: residual and y must be 4-byte aligned");
+  DFQ_REQUIRE(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
+              "dfq_i8_conv_slice: pre / post clamp bounds must be ordered and not NaN");
+  DFQ_REQUIRE(std::isfinite(e->out_scale) && e->out_scale >= 0.f, "dfq_i8_conv_slice: out_scale must be finite and non-negative");
+  const int cpad = (g->O + 15) / 16 * 16;
+  DFQ_REQUIRE(coff >= 0 && cstride > 0 && coff % 16 == 0 && cstride % 16 == 0,
+              "dfq_i8_conv_slice: coff and cstride must be non-negative multiples of 16");
+  DFQ_REQUIRE((int64_t)coff + cpad <= cstride, "dfq_i8_conv_slice: the slice coff + round_up(O, 16) exceeds cstride");
+  const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
+  const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float);
+  int8_t* yq = e->yq + coff;
+  const int64_t slice_bytes = (pixels - 1) * cstride + cpad;          // first to last byte the slice's chunks cover
+  DFQ_REQUIRE(!overlap(e->residual, y_bytes, yq, slice_bytes), "dfq_i8_conv_slice: residual overlaps the slice");
+  DFQ_REQUIRE(!overlap(e->y, y_bytes, yq, slice_bytes), "dfq_i8_conv_slice: y overlaps the slice");
+  DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes), "dfq_i8_conv_slice: residual overlaps y");
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool dense = g->groups == 1;
+  DFQ_REQUIRE(!dense || (pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_slice: too many output pixels");
+  const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+  const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+  if (!e->residual && !e->y && e->post_lo == -INFINITY && e->post_hi == INFINITY) {
+    // codes only after one clamp: the requantizing epilogue
+    const Requant rq{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride};
+    if (dense) k_i8_conv_mma<Out::I8><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, rq);
+    else k_i8_conv_dw<Out::I8><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, rq);
+  } else {
+    const Fused ep{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride, e->residual, e->y, e->post_lo, e->post_hi};
+    if (dense) k_i8_conv_mma<Out::FUSED><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
+    else k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, float out_scale, const DfqI8Pool* g,
+                              void* stream) {
+  DFQ_REQUIRE(g != nullptr, "dfq_i8_maxpool: null geometry");
+  DFQ_REQUIRE(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->kh > 0 && g->kw > 0, "dfq_i8_maxpool: empty dimension");
+  DFQ_REQUIRE(g->stride_h > 0 && g->stride_w > 0 && g->dil_h > 0 && g->dil_w > 0 && g->pad_h >= 0 && g->pad_w >= 0 &&
+                  (g->ceil_mode == 0 || g->ceil_mode == 1),
+              "dfq_i8_maxpool: bad stride / padding / dilation / ceil_mode");
+  DFQ_REQUIRE(g->pad_h <= g->kh / 2 && g->pad_w <= g->kw / 2 && g->pad_h <= (g->dil_h * (g->kh - 1) + 1) / 2 &&
+                  g->pad_w <= (g->dil_w * (g->kw - 1) + 1) / 2,
+              "dfq_i8_maxpool: padding must be at most half of the kernel and of the effective kernel");
+  DFQ_REQUIRE(g->Cpad >= g->C && g->Cpad % 16 == 0, "dfq_i8_maxpool: Cpad must be a multiple of 16 that holds C");
+  DFQ_REQUIRE(g->OH == pool_extent(g->H, g->kh, g->pad_h, g->stride_h, g->dil_h, g->ceil_mode) &&
+                  g->OW == pool_extent(g->W, g->kw, g->pad_w, g->stride_w, g->dil_w, g->ceil_mode) && g->OH > 0 && g->OW > 0,
+              "dfq_i8_maxpool: OH / OW do not follow from the geometry");
+  DFQ_REQUIRE((xq != nullptr) != (x != nullptr), "dfq_i8_maxpool: give exactly one input, codes xq or fp32 x");
+  const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
+  const int64_t total = out_px * (g->Cpad / 16);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (xq) {
+    DFQ_REQUIRE(yq && !y, "dfq_i8_maxpool: codes in give codes out only (yq, no y)");
+    DFQ_REQUIRE(aligned16(xq) && aligned16(yq), "dfq_i8_maxpool: xq and yq must be 16-byte aligned");
+    DFQ_REQUIRE(!overlap(xq, in_px * g->Cpad, yq, out_px * g->Cpad), "dfq_i8_maxpool: yq overlaps xq");
+    k_i8_maxpool<true><<<grid_for(total, 256), 256, 0, st>>>(xq, nullptr, nullptr, yq, 0.f, *g, total);
+  } else {
+    DFQ_REQUIRE(y || yq, "dfq_i8_maxpool: no output requested (y and yq are both NULL)");
+    DFQ_REQUIRE(aligned16(yq), "dfq_i8_maxpool: yq must be 16-byte aligned");
+    DFQ_REQUIRE(((uintptr_t)x & 3) == 0 && ((uintptr_t)y & 3) == 0, "dfq_i8_maxpool: x and y must be 4-byte aligned");
+    DFQ_REQUIRE(!yq || (std::isfinite(out_scale) && out_scale >= 0.f),
+                "dfq_i8_maxpool: out_scale must be finite and non-negative when yq is written");
+    const int64_t x_bytes = in_px * g->C * 4, y_bytes = out_px * g->C * 4, yq_bytes = out_px * g->Cpad;
+    DFQ_REQUIRE(!overlap(x, x_bytes, y, y_bytes) && !overlap(x, x_bytes, yq, yq_bytes) && !overlap(y, y_bytes, yq, yq_bytes),
+                "dfq_i8_maxpool: x, y and yq overlap");
+    k_i8_maxpool<false><<<grid_for(total, 256), 256, 0, st>>>(nullptr, x, y, yq, out_scale, *g, total);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;

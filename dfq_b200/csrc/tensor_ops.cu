@@ -478,6 +478,7 @@ extern "C" int dfq_struct_size(int which) {
     case 7: return (int)sizeof(DfqQuantTask);
     case 8: return (int)sizeof(DfqI8Conv);
     case 9: return (int)sizeof(DfqI8Epilogue);
+    case 10: return (int)sizeof(DfqI8Pool);
     default: return -1;
   }
 }

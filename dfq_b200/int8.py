@@ -88,6 +88,7 @@ class _Int8Layer(nn.Module):
     codes_in = False
     requant = None
     epilogue = None
+    out_slice = None
     layer_name = None
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
@@ -131,11 +132,13 @@ class _Int8Layer(nn.Module):
             g[0][k] = v
         return g
 
-    def chained(self, codes_in=False, requant=None, epilogue=None, name=None):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None):
         """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
         mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes; epilogue - an
-        Epilogue: the residual epilogue (not together with requant).  name: the layer's name in error messages.  self is
-        not modified."""
+        Epilogue: the residual epilogue (not together with requant); out_slice = (coff, cstride), with requant - write the
+        codes into channels [coff, coff + round_up(C_out, 16)) of an int8 NHWC tensor [N, OH, OW, cstride] (a channel
+        concatenation, dfq_i8_conv_slice), given as forward(x, out=...) or made when out is None.  name: the layer's name
+        in error messages.  self is not modified."""
         new = type(self).__new__(type(self))
         nn.Module.__init__(new)
         for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad", "act_scale"):
@@ -161,17 +164,27 @@ class _Int8Layer(nn.Module):
             epilogue = Epilogue(None if e.out_scale is None else float(_f32(e.out_scale)), _ordered(*e.pre, what="pre-add"),
                                 _ordered(*e.post, what="post-add"), bool(e.residual), bool(e.fp32))
         new.epilogue = epilogue
+        if out_slice is not None:
+            coff, cstride = (int(v) for v in out_slice)
+            if requant is None:
+                raise _lib.DfqError("layer %s: a channel slice needs requant" % new._who())
+            if coff < 0 or coff % 16 or cstride % 16 or coff + (self.out_channels + 15) // 16 * 16 > cstride:
+                raise _lib.DfqError("layer %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
+                                    % (new._who(), coff, cstride))
+            out_slice = (coff, cstride)
+        new.out_slice = out_slice
         return new
 
     def _who(self):
         return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
                                                                   self.kernel_size)
 
-    def run(self, x, with_acc=False, residual=None):
+    def run(self, x, with_acc=False, residual=None, out=None):
         """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue.  In the chained modes
         x is int8 codes [N, H, W, cpad] (codes_in) and y int8 codes [N, OH, OW, round_up(C_out, 16)] (requant).  With an
         epilogue, y is the codes, the fp32 output, or (codes, fp32 output) when it returns both, and `residual` is the fp32
-        tensor [N, C_out, OH, OW] the epilogue adds (exactly that shape, no broadcasting, on x's device)."""
+        tensor [N, C_out, OH, OW] the epilogue adds (exactly that shape, no broadcasting, on x's device).  With out_slice, y
+        is `out` (int8 [N, OH, OW, cstride] on x's device) or a new such tensor, its slice written."""
         if not x.is_cuda or not self.dq.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.dq.device))
@@ -203,6 +216,10 @@ class _Int8Layer(nn.Module):
                                                 C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
         if self.epilogue is not None:
             return self._run_fused(xq, residual, g, N, OH, OW), None
+        if out is not None and self.out_slice is None:
+            raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
+        if self.out_slice is not None:
+            return self._run_slice(xq, out, g, N, OH, OW), None
         if self.requant is not None:
             s, lo, hi = self.requant
             yq = torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=x.device)
@@ -215,6 +232,23 @@ class _Int8Layer(nn.Module):
         _lib.check(lib.dfq_i8_conv(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(y), _ptr(acc),
                                    _lib.table_ptr(g), st), "dfq_i8_conv")
         return y, acc
+
+    def _run_slice(self, xq, out, g, N, OH, OW):
+        (s, lo, hi), (coff, cstride) = self.requant, self.out_slice
+        shape = (N, OH, OW, cstride)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.int8, device=xq.device)
+        elif not isinstance(out, torch.Tensor) or out.dtype != torch.int8 or tuple(out.shape) != shape or \
+                out.device != xq.device or not out.is_contiguous():
+            raise _lib.DfqError("layer %s: the concatenation's codes must be contiguous int8 %s on %s, got %s" % (
+                self._who(), list(shape), xq.device, "%s %s on %s" % (out.dtype, list(out.shape), out.device)
+                if isinstance(out, torch.Tensor) else type(out).__name__))
+        d = np.zeros(1, _lib.I8_EPILOGUE_DT)
+        d[0] = (0, 0, out.data_ptr(), s, lo, hi, -_INF, _INF)
+        _lib.check(_lib.load().dfq_i8_conv_slice(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                                 _lib.table_ptr(d), coff, cstride, _lib.table_ptr(g), _lib.stream_ptr()),
+                   "dfq_i8_conv_slice (layer %s)" % self._who())
+        return out
 
     def _run_fused(self, xq, r, g, N, OH, OW):
         e = self.epilogue
@@ -249,8 +283,8 @@ class Int8Conv2d(_Int8Layer):
                                 % (conv.padding, conv.padding_mode))
         return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
 
-    def forward(self, x, r=None):
-        return self.run(x, residual=r)[0]
+    def forward(self, x, r=None, out=None):
+        return self.run(x, residual=r, out=out)[0]
 
     def extra_repr(self):
         return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act_scale=%g" % (
@@ -272,6 +306,64 @@ class Int8Linear(_Int8Layer):
 
     def extra_repr(self):
         return "in_features=%d, out_features=%d, act_scale=%g" % (self.in_channels, self.out_channels, self.act_scale)
+
+
+def _pool_extent(n, k, p, s, d, ceil_mode):
+    """torch's pooling output size (floor division; in ceil mode the last window starts inside the input or its left pad)."""
+    o = (n + 2 * p - d * (k - 1) - 1 + (s - 1 if ceil_mode else 0)) // s + 1
+    return o - 1 if ceil_mode and (o - 1) * s >= n + p else o
+
+
+class Int8MaxPool2d(nn.Module):
+    """F.max_pool2d of a chained model (dfq_i8_maxpool).  codes_in: int8 NHWC codes [N, H, W, round_up(channels, 16)] in,
+    the pooled codes out (the max of codes is the code of the max, q being monotone).  Otherwise fp32 NCHW in, bit for bit
+    torch's max_pool2d out (`fp32`) and / or its codes at out_scale: (codes, fp32) when both."""
+
+    def __init__(self, kernel_size, stride, padding, dilation, ceil_mode, channels, codes_in, out_scale=None, fp32=False,
+                 name=None):
+        super().__init__()
+        self.kernel_size, self.padding, self.dilation = _pair(kernel_size), _pair(padding), _pair(dilation)
+        self.stride = self.kernel_size if stride is None or stride == [] or stride == () else _pair(stride)
+        self.ceil_mode, self.channels, self.codes_in = bool(ceil_mode), int(channels), bool(codes_in)
+        self.cpad = (self.channels + 15) // 16 * 16
+        self.out_scale = None if out_scale is None else float(_f32(out_scale))
+        self.fp32, self.layer_name = bool(fp32), name
+        if self.out_scale is not None:
+            check_scale("output", self.out_scale, "max pool %s" % name)
+        if not codes_in and self.out_scale is None and not self.fp32:
+            raise _lib.DfqError("max pool %s returns neither codes nor fp32" % name)
+
+    def forward(self, x):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise _lib.DfqError("int8 max pool %s runs on the GPU only (no CPU fallback)" % self.layer_name)
+        if self.codes_in:
+            if x.dtype != torch.int8 or x.dim() != 4 or x.shape[3] != self.cpad:
+                raise _lib.DfqError("int8 max pool %s expects int8 codes [N, H, W, %d], got %s %s"
+                                    % (self.layer_name, self.cpad, x.dtype, tuple(x.shape)))
+            N, H, W, _ = x.shape
+        else:
+            if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.channels:
+                raise _lib.DfqError("int8 max pool %s expects fp32 [N, %d, H, W], got %s %s"
+                                    % (self.layer_name, self.channels, x.dtype, tuple(x.shape)))
+            N, _, H, W = x.shape
+        x = x.contiguous()
+        (kh, kw), (sh, sw), (ph, pw), (dh, dw) = self.kernel_size, self.stride, self.padding, self.dilation
+        OH, OW = _pool_extent(H, kh, ph, sh, dh, self.ceil_mode), _pool_extent(W, kw, pw, sw, dw, self.ceil_mode)
+        g = np.zeros(1, _lib.I8_POOL_DT)
+        g[0] = (N, self.channels, H, W, kh, kw, sh, sw, ph, pw, dh, dw, int(self.ceil_mode), OH, OW, self.cpad)
+        yq = torch.empty((N, OH, OW, self.cpad), dtype=torch.int8, device=x.device) \
+            if self.codes_in or self.out_scale is not None else None
+        y = torch.empty((N, self.channels, OH, OW), dtype=torch.float32, device=x.device) \
+            if not self.codes_in and self.fp32 else None
+        _lib.check(_lib.load().dfq_i8_maxpool(_ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y),
+                                              _ptr(yq), C.c_float(self.out_scale or 0.0), _lib.table_ptr(g),
+                                              _lib.stream_ptr()), "dfq_i8_maxpool (%s)" % self.layer_name)
+        return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
+
+    def extra_repr(self):
+        return "kernel_size=%s, stride=%s, padding=%s, dilation=%s, ceil_mode=%s, channels=%d, %s" % (
+            self.kernel_size, self.stride, self.padding, self.dilation, self.ceil_mode, self.channels,
+            "codes" if self.codes_in else "fp32 in, out_scale=%s, fp32=%s" % (self.out_scale, self.fp32))
 
 
 def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
@@ -395,7 +487,42 @@ def _is_add(node):
         node.args[0] is not node.args[1]
 
 
-def chain_int8(model: nn.Module, concrete_args=None, residual=False) -> fx.GraphModule:
+def _is_const(v):
+    return isinstance(v, (int, bool)) or (isinstance(v, (tuple, list)) and all(isinstance(e, int) for e in v))
+
+
+def _max_pool(node, mods):
+    """(kernel_size, stride, padding, dilation, ceil_mode) of an nn.MaxPool2d / F.max_pool2d / torch.max_pool2d node without
+    return_indices, on one fx node and constant arguments; None otherwise."""
+    if len(node.all_input_nodes) != 1 or not node.args or not isinstance(node.args[0], fx.Node):
+        return None
+    if node.op == "call_module" and type(mods[node.target]) is nn.MaxPool2d:
+        m = mods[node.target]
+        if m.return_indices or len(node.args) != 1 or node.kwargs:
+            return None
+        return m.kernel_size, m.stride, m.padding, m.dilation, m.ceil_mode
+    if node.op == "call_function" and node.target in (F.max_pool2d, torch.max_pool2d):
+        a = (_arg(node, 1, "kernel_size", None), _arg(node, 2, "stride", None), _arg(node, 3, "padding", 0),
+             _arg(node, 4, "dilation", 1), _arg(node, 5, "ceil_mode", False))
+        if _arg(node, 6, "return_indices", False) or not all(v is None or _is_const(v) for v in a) or a[0] is None:
+            return None
+        return a
+    return None
+
+
+def _cat_operands(node):
+    """The operands of torch.cat / torch.concat along the channels (dim 1 or -3) of >= 2 distinct fx nodes, without out;
+    None otherwise."""
+    if node.op != "call_function" or node.target not in (torch.cat, torch.concat) or set(node.kwargs) - {"tensors", "dim"}:
+        return None
+    ops, dim = _arg(node, 0, "tensors", None), _arg(node, 1, "dim", 0)
+    if dim not in (1, -3) or not isinstance(ops, (list, tuple)) or len(ops) < 2 or \
+            not all(isinstance(o, fx.Node) for o in ops) or len(set(ops)) != len(ops):
+        return None
+    return list(ops)
+
+
+def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` computes, with activations kept in int8 between converted
     convolutions.
 
@@ -425,7 +552,28 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False) -> fx.Graph
     edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) being the
     clamp the consumer's codes were taken after; with residual=True also the fused adds in `fused_adds`: (producer name,
     add node name, residual node name, (lo, hi) before the add, (lo, hi) after it) in graph order, node names being those
-    of the traced model (a residual another fusion deleted is that producer's fp32 output in the result)."""
+    of the traced model (a residual another fusion deleted is that producer's fp32 output in the result).
+
+    pool_cat=True (with residual=True) also carries codes through max pools and channel concatenations, still bit-identical
+    to the per-layer path except where noted:
+    - max pool: an nn.MaxPool2d (it may be called at several sites) or F.max_pool2d node without return_indices.  Codes mode
+      (dfq_i8_maxpool on codes): its input is a tail that carries codes - a producer's single-user chain or fan-out tail, a
+      fused concatenation's or another fused pool's - and every user of the pool, past single-user exact identities (which
+      are deleted), takes codes at one scale: an Int8Conv2d at that act_scale, bit for bit, or another such pool.  A clamp
+      after a pool ends it.  Two inputs the per-layer path treats otherwise: a window holding a NaN gives the max of the
+      other codes (per-layer: -127), and an infinite input at scale 0 gives the code of the max (per-layer: -127).
+      Fp32 mode: the pool's input is a producer's single-user pass-through chain and some user needs fp32 (ResNet's stem,
+      whose pooled tensor is a residual).  The producer writes its clamped fp32 output (dfq_i8_conv_fused, fp32 only); the
+      pool writes torch's fp32 max_pool2d for the fp32 users and the codes of the fan-out rule's Int8Conv2d users.
+    - concatenation: torch.cat / torch.concat along dim 1 (or -3) of >= 2 distinct nodes, without out.  Each operand is
+      reached from its own Int8Conv2d producer through single-user pass-throughs, every operand but the last has a multiple
+      of 16 channels, and every user of the cat's tail (the cat and its single-user pass-throughs) takes codes at one scale
+      (Int8Conv2d or codes-mode pool).  Each producer writes its codes, after its operand's clamp composed with the tail's,
+      into its channel slice of the consumers' int8 input (dfq_i8_conv_slice), one buffer per forward, in graph order; the
+      cat and its pass-throughs are deleted.  Any other cat stays in torch, fp32.
+    Edges whose codes come through a fused pool or cat name that node (its traced name) as the producer.  `fused_cats`
+    records (cat node name, producer names, channel offsets) and `fused_pools` (pool node name, "codes" or "fp32", the
+    outputs it writes), in graph order.  pool_cat=True without residual=True raises DfqError."""
     tracer = _Int8Tracer()
     graph = tracer.trace(model, concrete_args)
     gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
@@ -438,8 +586,10 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False) -> fx.Graph
     def conv(node):
         return node.op == "call_module" and isinstance(mods[node.target], Int8Conv2d) and sites[node.target] == 1
 
+    if pool_cat and not residual:
+        raise _lib.DfqError("chain_int8: pool_cat=True builds on residual=True")
     if residual:
-        return _chain_residual(gm, mods, conv)
+        return _chain_residual(gm, mods, conv, pool_cat)
 
     edges, between = [], []
     for q in list(gm.graph.nodes):
@@ -479,8 +629,8 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False) -> fx.Graph
     return gm
 
 
-def _chain_residual(gm, mods, conv):
-    """chain_int8(..., residual=True) on the traced `gm` (see chain_int8)."""
+def _chain_residual(gm, mods, conv, pool_cat=False):
+    """chain_int8(..., residual=True[, pool_cat=True]) on the traced `gm` (see chain_int8)."""
     full = (-_INF, _INF)
     order = {n: i for i, n in enumerate(gm.graph.nodes)}
 
@@ -507,6 +657,60 @@ def _chain_residual(gm, mods, conv):
             node = node.args[0]
         return node if len(node.users) == 1 and producer(node) else None
 
+    def same(a, b):
+        return a.view(np.int32) == b.view(np.int32)
+
+    def after_pool(node):
+        """Walk from a pool through single-user exact identities: (last node, the identities)."""
+        path = []
+        while len(node.users) == 1:
+            u = next(iter(node.users))
+            if not _is_identity(u, mods) or len(u.all_input_nodes) != 1 or u.args[0] is not node:
+                break
+            node = u
+            path.append(u)
+        return node, path
+
+    pool_memo = {}
+
+    def pool_scale(pool, channels):
+        """The scale at which every user of a pool (past exact identities) takes codes, or None."""
+        if pool not in pool_memo:
+            pool_memo[pool] = None
+            tail, _ = after_pool(pool)
+            scales = [user_scale(u, tail, channels) for u in tail.users]
+            if scales and all(s is not None and same(s, scales[0]) for s in scales):
+                pool_memo[pool] = scales[0]
+        return pool_memo[pool]
+
+    def user_scale(u, tail, channels, pools=True):
+        """The scale at which u takes the codes of `tail` (channels wide), or None when it takes fp32."""
+        if producer(u) and u.args[0] is tail and mods[u.target].in_channels == channels:
+            return _f32(mods[u.target].act_scale)
+        if pools and pool_cat and _max_pool(u, mods) is not None and u.args[0] is tail:
+            return pool_scale(u, channels)
+        return None
+
+    def take_codes(tail, channels, pools=True):
+        """The fan-out rule: the users of tail that take codes at the first such user's scale (graph order), and it."""
+        codes, scale = [], None
+        for u in sorted(tail.users, key=order.get):
+            s = user_scale(u, tail, channels, pools)
+            if s is not None and (scale is None or same(s, scale)):
+                scale = s
+                codes.append(u)
+        return codes, scale
+
+    pool_plans = []
+
+    def codes_pool(u, channels, clamp):
+        tail, ids = after_pool(u)
+        pool_plans.append(dict(node=u, mode="codes", tail=tail, path=ids, codes=sorted(tail.users, key=order.get),
+                               scale=pool_scale(u, channels), clamp=clamp, channels=channels))
+        for v in tail.users:
+            if not producer(v):
+                codes_pool(v, channels, clamp)
+
     plans = []
     for p in list(gm.graph.nodes):
         if not producer(p):
@@ -520,22 +724,62 @@ def _chain_residual(gm, mods, conv):
                 if fused is not None and a.args[fused] is end:
                     add, ri = a, 1 - fused
                     tail, post, post_path = forward(a, full)
-        codes, scale = [], None
         out_c = mods[p.target].out_channels
-        for u in sorted(tail.users, key=order.get):
-            if producer(u) and u.args[0] is tail and mods[u.target].in_channels == out_c:
-                s = _f32(mods[u.target].act_scale)
-                if scale is None or s.view(np.int32) == scale.view(np.int32):
-                    scale = s
-                    codes.append(u)
+        codes, scale = take_codes(tail, out_c)
+        clamp = post if add is not None else pre
+        if add is None and not codes and pool_cat and len(tail.users) == 1:
+            u = next(iter(tail.users))                          # fp32-mode pool: a user of the pool needs fp32
+            if _max_pool(u, mods) is not None and u.args[0] is tail:
+                pc, ps = take_codes(u, out_c, pools=False)
+                if pc:
+                    pool_plans.append(dict(node=u, mode="fp32", codes=pc, scale=ps, clamp=clamp, channels=out_c))
+                    plans.append(dict(p=p, path=path, pre=pre, add=None, ri=None, post=full, post_path=[], tail=tail,
+                                      codes=[], scale=None))
+            continue
         if add is None and not codes:
             continue
-        plans.append(dict(p=p, path=path, pre=pre, add=add, ri=ri, post=post, post_path=post_path, tail=tail, codes=codes))
+        plans.append(dict(p=p, path=path, pre=pre, add=add, ri=ri, post=post, post_path=post_path, tail=tail, codes=codes,
+                          scale=scale))
+        for u in codes:
+            if not producer(u):
+                codes_pool(u, out_c, clamp)
+
+    # concatenations whose operands come from their own producers and whose users all take codes at one scale
+    cat_plans = []
+    for c in (list(gm.graph.nodes) if pool_cat else []):
+        ops = _cat_operands(c)
+        if ops is None:
+            continue
+        prods = [back_to_producer(o) for o in ops]
+        if any(q is None for q in prods) or len(set(prods)) != len(prods):
+            continue
+        chans = [mods[q.target].out_channels for q in prods]
+        if any(k % 16 for k in chans[:-1]):
+            continue
+        tail, tclamp, tpath = forward(c, full)
+        codes, scale = take_codes(tail, sum(chans))
+        if not codes or len(codes) != len(tail.users):
+            continue
+        operands = []
+        for o, q, off in zip(ops, prods, np.cumsum([0] + chans[:-1]).tolist()):
+            node, clamp, opath = o, full, []
+            while node is not q:
+                clamp = _compose(_pass_through(node, mods), clamp)
+                opath.append(node)
+                node = node.args[0]
+            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), coff=off))
+        cat_plans.append(dict(cat=c, operands=operands, tail=tail, path=tpath, codes=codes, scale=scale, clamp=tclamp,
+                              cstride=(sum(chans) + 15) // 16 * 16))
+        for u in codes:
+            if not producer(u):
+                codes_pool(u, sum(chans), tclamp)
 
     # the residual's exact identities, skipped once every plan's own nodes are known: a node another plan deletes (an
     # identity at the end of its post-add chain, say) stays the residual, and that plan replaces it by its fp32 output
     claimed = {n for pl in plans for n in (pl["p"], *pl["path"], *([pl["add"]] if pl["add"] is not None else []),
                                             *pl["post_path"])}
+    claimed |= {n for cp in cat_plans for n in (cp["cat"], *cp["path"], *(n for o in cp["operands"] for n in (o["p"], *o["path"])))}
+    claimed |= {n for pp in pool_plans for n in (pp["node"], *pp.get("path", []))}
     for pl in plans:
         pl["skipped"] = []
         if pl["add"] is None:
@@ -548,6 +792,7 @@ def _chain_residual(gm, mods, conv):
 
     # rewrite in producer order: a producer's input may be the codes of an earlier one, and a residual its fp32 output
     g = gm.graph
+    convs = {n for n in g.nodes if producer(n)}                 # before the rewrites give producers a second input
     edges, adds, modes = [], [], {}
     for pl in plans:
         p, add, tail = pl["p"], pl["add"], pl["tail"]
@@ -558,7 +803,7 @@ def _chain_residual(gm, mods, conv):
             add.prepend(p)
             p.args = (p.args[0], add.args[pl["ri"]])
         fp32 = any(u not in pl["codes"] for u in tail.users)
-        scale = float(_f32(mods[pl["codes"][0].target].act_scale)) if pl["codes"] else None
+        scale = float(pl["scale"]) if pl["codes"] else None
         clamp = pl["post"] if add is not None else pl["pre"]
         if add is None and not fp32:
             modes[p.target] = ("requant", (scale,) + tuple(clamp))
@@ -573,7 +818,8 @@ def _chain_residual(gm, mods, conv):
                     codes_node = g.call_function(operator.getitem, (p, 0))
         for u in pl["codes"]:
             u.replace_input_with(tail, codes_node)
-            edges.append((p.target, u.target, clamp))
+            if u in convs:
+                edges.append((p.target, u.target, clamp))
         if tail is not p:
             tail.replace_all_uses_with(y_node)
             for node in reversed([*pl["path"], *([add] if add is not None else []), *pl["post_path"]]):
@@ -582,15 +828,74 @@ def _chain_residual(gm, mods, conv):
             p.replace_all_uses_with(y_node, delete_user_cb=lambda u: u not in (y_node, codes_node))
         if add is not None:
             adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
+
+    # concatenations: the producers write their slices of one buffer in graph order, threaded through `out`
+    cats = []
+    for cp in cat_plans:
+        cstride, prev = cp["cstride"], None
+        for o in sorted(cp["operands"], key=lambda o: order[o["p"]]):
+            q = o["p"]
+            modes[q.target] = ("slice", ((float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride)))
+            if prev is not None:
+                q.kwargs = {"out": prev}
+            prev = q
+        for u in cp["codes"]:
+            u.replace_input_with(cp["tail"], prev)
+            if u in convs:
+                edges.append((cp["cat"].name, u.target, cp["clamp"]))
+        for node in reversed(cp["path"]):
+            g.erase_node(node)
+        g.erase_node(cp["cat"])
+        for o in cp["operands"]:
+            for node in o["path"]:                              # from the cat back to the producer
+                g.erase_node(node)
+        cats.append((cp["cat"].name, [o["p"].target for o in cp["operands"]], [o["coff"] for o in cp["operands"]]))
+
+    # pools, last: each reads its input as the rewrites above left it
+    pools = []
+    for pp in sorted(pool_plans, key=lambda pp: order[pp["node"]]):
+        u = pp["node"]
+        k, s, pad, dil, ceil = _max_pool(u, mods)
+        codes_mode = pp["mode"] == "codes"
+        fp32 = not codes_mode
+        mod = Int8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, None if codes_mode else float(pp["scale"]),
+                            fp32, name=u.name)
+        name = "int8_pool_" + u.name
+        gm.add_submodule(name, mod)
+        inp = u.args[0]
+        u.op, u.target, u.args, u.kwargs = "call_module", name, (inp,), {}
+        if codes_mode:
+            for v in pp["codes"]:
+                v.replace_input_with(pp["tail"], u)
+            for node in reversed(pp["path"]):
+                g.erase_node(node)
+        else:
+            with g.inserting_after(u):
+                y_node = g.call_function(operator.getitem, (u, 1))
+            with g.inserting_after(u):
+                codes_node = g.call_function(operator.getitem, (u, 0))
+            for v in pp["codes"]:
+                v.replace_input_with(u, codes_node)
+            u.replace_all_uses_with(y_node, delete_user_cb=lambda x: x not in (y_node, codes_node))
+        for v in pp["codes"]:
+            if v in convs:
+                edges.append((u.name, v.target, pp["clamp"]))
+        pools.append((u.name, pp["mode"], ("codes",) if codes_mode else ("fp32", "codes")))
+
     consumers = {q for _, q, _ in edges}
     for target in modes.keys() | consumers:
         kind, arg = modes.get(target, (None, None))
         parent, _, attr = target.rpartition(".")
         setattr(gm.get_submodule(parent) if parent else gm, attr,
                 mods[target].chained(codes_in=target in consumers, name=target,
-                                     requant=arg if kind == "requant" else None, epilogue=arg if kind == "epilogue" else None))
+                                     requant=arg if kind == "requant" else (arg[0] if kind == "slice" else None),
+                                     epilogue=arg if kind == "epilogue" else None,
+                                     out_slice=arg[1] if kind == "slice" else None))
     g.lint()
     gm.recompile()
     gm.requantized_edges = edges
     gm.fused_adds = adds
+    if pool_cat:
+        gm.fused_cats = cats
+        gm.fused_pools = pools
     return gm

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 4
+#define DFQ_ABI_VERSION 5
 
 enum {
   DFQ_OK = 0,
@@ -377,6 +377,42 @@ typedef struct DfqI8Epilogue {
  * a residual that overlaps y or yq, or y overlapping yq (extents from the geometry).  Grouping as dfq_i8_conv. */
 int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
                       const DfqI8Conv* g, void* stream);
+
+/* The convolution's codes written into a channel slice of a wider int8 NHWC tensor, for a channel concatenation whose
+ * producers each write their own channels of the consumer's input:  pixel m, channel o < round_up(O, 16) goes to
+ * e->yq[m * cstride + coff + o] (pad channels O .. round_up(O, 16) written 0; the last slice's are the tensor's pad), and
+ * nothing else of e->yq is written.  The codes are those of dfq_i8_conv_fused with the epilogue *e (residual and y as
+ * there; yq required); without residual and y and with post = (-inf, +inf), those of dfq_i8_conv_requant at
+ * (out_scale, pre_lo, pre_hi).  coff = 0, cstride = round_up(O, 16) is the tensor those two entries write.  DFQ_E_ARG, with
+ * a reason: yq NULL or not 16-byte aligned, coff or cstride not a multiple of 16, coff + round_up(O, 16) > cstride, a
+ * residual or y that overlaps the slice's extent or each other, and the epilogue refusals of dfq_i8_conv_fused. */
+int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                      int32_t coff, int32_t cstride, const DfqI8Conv* g, void* stream);
+
+/* Max pooling, with torch's geometry (F.max_pool2d: zero-free padding, dilation, ceil_mode). */
+typedef struct DfqI8Pool {
+  int32_t N, C, H, W;          /* input [N, C, H, W]                                                              */
+  int32_t kh, kw;
+  int32_t stride_h, stride_w;
+  int32_t pad_h, pad_w;        /* at most kh / 2 and (dil_h (kh - 1) + 1) / 2, as torch requires                   */
+  int32_t dil_h, dil_w;
+  int32_t ceil_mode;           /* 0 or 1                                                                          */
+  int32_t OH, OW;              /* torch's formula, checked; in ceil mode the last window starts inside the input   */
+  int32_t Cpad;                /* channel stride of the codes: a multiple of 16 >= C                              */
+} DfqI8Pool;
+/* Two modes, by which input is given (exactly one):
+ *   xq (codes): int8 NHWC [N, H, W, Cpad] -> yq int8 NHWC [N, OH, OW, Cpad], the byte-wise signed max of the taps inside
+ *      the input.  q(v, s) is monotone for s >= 0, so this is q(max_pool2d(v), s) for any window without NaN.  Exceptions
+ *      of the per-layer path, where it quantizes the fp32 max: a window holding a NaN gives -127 there and the max of the
+ *      other codes here; at scale 0 an infinite input gives q(inf * 0) = -127 there.  A window with no tap in the input
+ *      gives -127 (torch's -inf), pad channels 0.  y must be NULL.
+ *   x (fp32): NCHW [N, C, H, W] -> y fp32 NCHW [N, C, OH, OW] (NULL: not written) bit for bit torch's CUDA max_pool2d (from
+ *      -inf, taps row-major, replaced when v > max or v is NaN: the first of tied values, -0.0 before +0.0, is kept), and /
+ *      or yq = q(y, out_scale) int8 NHWC [N, OH, OW, Cpad] (NULL: not written; pad channels 0).
+ * DFQ_E_ARG, with a reason: a bad geometry, both or neither input, no output, misaligned xq / yq (16 B) or x / y (4 B),
+ * an out_scale that is not finite and non-negative while yq is written in fp32 mode, overlapping input and outputs. */
+int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, float out_scale, const DfqI8Pool* g,
+                   void* stream);
 
 #ifdef __cplusplus
 }

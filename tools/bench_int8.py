@@ -8,7 +8,9 @@ GEMM layers against the data-sheet dense peak, and the relative logit error (2-n
 fake-quant against fp32.  `chained`: per-layer int8 against int8.chain_int8 (activations kept in int8 between fused
 convolutions) on the same nets with BN folded - images/s, fused edges, fp32 bytes avoided, bit-identity of the logits.
 `residual`: per-layer against chain_int8 and chain_int8(residual=True) (residual adds and tensors with several consumers
-fused too), the same way, with the fused adds.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
+fused too), the same way, with the fused adds.  `pool_cat`: per-layer against chain_int8(residual=True) and
+chain_int8(residual=True, pool_cat=True) (max pools and channel concatenations carried in int8 too) on ResNet-18, SqueezeNet
+1.1 and GoogLeNet.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
 """
 import argparse
 import json
@@ -289,6 +291,96 @@ def residual_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def pool_cat_inference(dev, reps=10, batch=256, rounds=5):
+    """Per-layer int8 execution against chain_int8(residual=True) and chain_int8(residual=True, pool_cat=True) on ResNet-18,
+    SqueezeNet 1.1 and GoogLeNet (BN folded, scales 128 / max|input|), timed alternately (`rounds` rounds of `reps` passes,
+    median): images/s, ms per batch, fused cats and pools, the fp32 bytes the pool_cat arm avoids against the residual arm
+    (from shapes) and bit-identity of the logits."""
+    import statistics
+    from collections import OrderedDict
+    import torch
+    import torch.nn as nn
+    import torchvision
+    from dfq_b200 import int8
+    from dfq_b200.trace import trace_graph
+    from dfq_b200.utils.layer_transform import merge_batchnorm
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds,
+           "fp32_bytes_avoided_note": "fp32 bytes the residual arm moves through torch.cat, max_pool2d and the pass-throughs "
+                                      "and quantizers around them that the pool_cat arm does not, per batch, from the "
+                                      "traced tensors' sizes: per deleted node a read and a write of its output (cat: of "
+                                      "its output twice), per fused pool its fp32 read and write unless it runs in fp32 mode, "
+                                      "per carried consumer of a pool or cat the quantizer's read"}
+    x = torch.randn(batch, 3, 224, 224, device=dev)
+    for net in ("resnet18", "squeezenet1_1", "googlenet"):
+        torch.manual_seed(0)
+        kw = dict(aux_logits=False, init_weights=True) if net == "googlenet" else {}
+        model = getattr(torchvision.models, net)(num_classes=1000, **kw).to(dev).eval()
+        graph, bottoms = trace_graph(model)
+        merge_batchnorm(model, graph, bottoms, [nn.Conv2d])
+        layers = OrderedDict((n, m) for n, m in model.named_modules() if type(m) in (nn.Conv2d, nn.Linear))
+        amax = {}
+        hooks = [m.register_forward_pre_hook(lambda m, i, n=n: amax.__setitem__(n, max(amax.get(n, 0.0), float(i[0].abs().max()))))
+                 for n, m in layers.items()]
+        with torch.no_grad():
+            model(x[:32])
+        for h in hooks:
+            h.remove()
+        int8.convert_to_int8(model, OrderedDict((id(m), m) for m in layers.values()), [nn.Conv2d, nn.Linear],
+                             act_scales=[128. / amax[n] for n in layers])
+        res = int8.chain_int8(model, residual=True)
+        gm = int8.chain_int8(model, residual=True, pool_cat=True)
+        # sizes of every traced node's output, from one fp32 run of the traced per-layer model
+        traced = torch.fx.GraphModule(model, int8._Int8Tracer().trace(model))
+        size = {}
+        interp = torch.fx.Interpreter(traced)
+        run_node = interp.run_node
+
+        def record(n):
+            v = run_node(n)
+            if isinstance(v, torch.Tensor):
+                size[n.name] = v.numel() * 4
+            return v
+        interp.run_node = record
+        with torch.no_grad():
+            interp.run(x)
+            kept_res = {n.name for n in res.graph.nodes}
+            kept = {n.name for n in gm.graph.nodes}
+            avoided = sum(2 * size.get(n, 0) for n in kept_res - kept)
+            avoided += sum(2 * size.get(c[0], 0) for c in gm.fused_cats)
+            avoided += sum(size.get(p[0], 0) // 4 * 4 for p in gm.fused_pools if p[1] == "codes")
+            avoided += sum(size.get(p, 0) for p, q, _ in gm.requantized_edges
+                           if q not in {e[1] for e in res.requantized_edges})
+            ref = model(x)
+            got = {"residual": res(x), "pool_cat": gm(x)}
+            for _ in range(2):
+                model(x), res(x), gm(x)
+            torch.cuda.synchronize(dev)
+            ms = {"per_layer": [], "residual": [], "pool_cat": []}
+            for _ in range(rounds):
+                ms["per_layer"].append(timed(lambda: model(x)))
+                ms["residual"].append(timed(lambda: res(x)))
+                ms["pool_cat"].append(timed(lambda: gm(x)))
+        med = {k: statistics.median(v) for k, v in ms.items()}
+        out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                    "ms_per_batch_rounds": ms, "fused_cats": len(gm.fused_cats),
+                    "fused_pools": [p[:2] for p in gm.fused_pools],
+                    "carried_conv_inputs": {"residual": len({e[1] for e in res.requantized_edges}),
+                                            "pool_cat": len({e[1] for e in gm.requantized_edges})},
+                    "fp32_bytes_avoided_per_batch_vs_residual": avoided,
+                    "logits_bit_identical": {k: bool(torch.equal(ref.view(torch.int32), v.view(torch.int32)))
+                                             for k, v in got.items()}}
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -315,6 +407,7 @@ def main():
     res = int8_inference(dev, reps=args.reps, batch=args.batch)
     res["chained"] = chained_inference(dev, reps=args.reps, batch=args.batch)
     res["residual"] = residual_inference(dev, reps=args.reps, batch=args.batch)
+    res["pool_cat"] = pool_cat_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
