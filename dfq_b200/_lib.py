@@ -14,10 +14,12 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
+LAYER_FOLD_PENDING = 2
+FOLD_FULL, FOLD_DEFER, FOLD_APPLY = 0, 1, 2   # DfqFold.mode
 
 
 class DfqError(RuntimeError):
@@ -29,7 +31,7 @@ LAYER_DT = np.dtype([
     ("w_off", np.int64), ("bias_off", np.int64),
     ("rows", np.int32), ("cols", np.int32), ("kk", np.int32),
     ("rel_in", np.int32), ("rel_out", np.int32), ("col_mode", np.int32), ("group", np.int32), ("flags", np.int32),
-    ("cmin_off", np.int64), ("cmax_off", np.int64),
+    ("cmin_off", np.int64), ("cmax_off", np.int64), ("fold_off", np.int64),
 ], align=True)
 
 RELATION_DT = np.dtype([
@@ -55,7 +57,7 @@ FOLD_DT = np.dtype([
     ("layer", np.int32), ("bn_eps", np.float32),
     ("gamma_off", np.int64), ("beta_off", np.int64), ("mean_off", np.int64), ("var_off", np.int64),
     ("fake_w_off", np.int64), ("fake_b_off", np.int64),
-    ("scan_go", np.int32), ("scan_gi", np.int32),
+    ("scan_go", np.int32), ("scan_gi", np.int32), ("mode", np.int32), ("_pad", np.int32), ("fac_off", np.int64),
 ], align=True)
 
 TERM_DT = np.dtype([
@@ -88,8 +90,8 @@ I8_POOL_DT = np.dtype([(f, np.int32) for f in (
 
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
-    "DfqLayer": (LAYER_DT, 64), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
-    "DfqCleResult": (CLE_RESULT_DT, 528), "DfqFold": (FOLD_DT, 64), "DfqExpectTerm": (TERM_DT, 32),
+    "DfqLayer": (LAYER_DT, 72), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
+    "DfqCleResult": (CLE_RESULT_DT, 528), "DfqFold": (FOLD_DT, 80), "DfqExpectTerm": (TERM_DT, 32),
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64),
 }
@@ -117,6 +119,7 @@ SIGNATURES = {
     "dfq_device_info": [C.POINTER(C.c_int), C.POINTER(C.c_int)],
     "dfq_cle_run": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32,
                     C.c_void_p, C.c_void_p, _I32, C.c_void_p, _ST],
+    "dfq_cle_takes_stack": [C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32, _I32, C.c_void_p],
     "dfq_bn_fold": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, _ST],
     "dfq_bias_correct": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, _I32, _ST],
     "dfq_quantize_tensors": [_PF, _I64, C.c_void_p, _I32, C.c_int, _ST],

@@ -133,6 +133,7 @@ struct RowCtx {
   double inv_n;
   int first_sweep;
   int inv_cached;        // 1: inv_in[0 .. cols) of the (single) input group is cached in shared memory
+  const float* fold;     // first sweep of a DFQ_LAYER_FOLD_PENDING layer: its [rows] fold factors (k_cle_stack only)
 };
 
 // The column scans are rare in the sweep loop (general middle layers only): kept out of line so that their registers do
@@ -572,6 +573,7 @@ __device__ __forceinline__ void make_ctx(RowCtx& c, float* arena, const DfqLayer
   c.rows = l.rows; c.cols = l.cols; c.kk = l.kk; c.row_len = l.cols * l.kk;
   c.inv_n = 1.0 / ((double)l.rows * (double)c.row_len);
   c.first_sweep = (sweep == 0);
+  c.fold = (sweep == 0 && (l.flags & DFQ_LAYER_FOLD_PENDING)) ? arena + l.fold_off : nullptr;
   const int rd = sweep & 1, wr = rd ^ 1;
   c.inv_in = nullptr; c.in_gi = 1; c.in_go = 1; c.inv_cached = 0;
   c.own_cmin_wr = c.own_cmax_wr = nullptr;
@@ -1116,9 +1118,12 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
 //     has READ it;
 //   * same arithmetic, same exit rule per convergence group (the functions of k_cle_engine are reused): weights, S, biases
 //     and BN vectors are bit-identical to the engine's; the convergence metric is summed in a different order (float64).
-// Eligibility (host, dfq_cle_run): two steps; every layer either `first` only or `second` only (col_mode 0) with its column
-// extrema ready (the fold's scan); ungrouped relations; rows that the TMA unit can move (multiple of 4 floats, <= a stage);
-// at most kBcExCols input columns, 3x3 or 1x1 taps; not apply_only.  Everything else runs on k_cle_engine.
+// Eligibility (host: stack_ineligible + stack_decision, the one decision of dfq_cle_run and dfq_cle_takes_stack): two steps;
+// every layer either `first` only or `second` only (col_mode 0) with its column extrema ready (the fold's scan); ungrouped
+// relations; rows that the TMA unit can move (multiple of 4 floats, <= a stage); at most kBcExCols input columns, 3x3 or 1x1
+// taps; not apply_only.  Everything else runs on k_cle_engine.
+// The first sweep also completes a BN fold deferred into it (DFQ_LAYER_FOLD_PENDING, RowCtx.fold): every row is multiplied by
+// its fold factor as it is read from the stage.
 // ------------------------------------------------------------------------------------------------------------
 // Consumer warps of k_cle_stack (of the kBcConsumers the CTA has): the pass is far from issue-bound (ncu, 7 consumers: issue
 // slots 19 % busy, 45 % of the warp samples waiting for data) - what matters is how many of the 11 stages are LOADING, i.e.
@@ -1138,15 +1143,46 @@ __device__ __forceinline__ void sts_f4(uint32_t a, const float4& v) {
   asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
 
+// FOLD (first sweep of a DFQ_LAYER_FOLD_PENDING layer): the row's BN fold is applied to every element as it is read,
+// v = fl(w * fo) - the value dfq_bn_fold would have stored - and the row is then processed exactly as if it had been.
+
 // One second-layer row of n4 float4 at shared address a0, its columns scaled in place by the cached reciprocals inv_s
 // (MODE IN_KK9 or IN_KK1); returns this lane's sum of |new - old|.
-template <int MODE>
-__device__ __forceinline__ float stack_scale_cols(uint32_t a0, int n4, const float* __restrict__ inv_s, int lane) {
+template <int MODE, bool FOLD>
+__device__ __forceinline__ float stack_scale_cols(uint32_t a0, int n4, const float* __restrict__ inv_s, float fo, int lane) {
   float dsum = 0.f;
 #pragma unroll 4
   for (int i4 = lane; i4 < n4; i4 += 32) {
-    const float4 v = lds_f4(a0 + 16u * i4);
+    float4 v = lds_f4(a0 + 16u * i4);
+    if (FOLD) v = mul4(v, fo);
     const float4 t = in_scale4<MODE>(v, i4 * 4, inv_s, 1.f, MODE == IN_KK9 ? 9 : 1);
+    sts_f4(a0 + 16u * i4, t);
+    dsum += absdiff4(t, v);
+  }
+  return dsum;
+}
+
+// One first-layer row of n4 float4 at shared address a0 (dfq.py:48-73): range -> s (*sv, *iv) -> rescale in place.
+// `in`: the row's column extrema of the pair.  Returns this lane's sum of |new - old|.
+template <bool FOLD>
+__device__ __forceinline__ float stack_scale_row(uint32_t a0, int n4, const DfqCleParams& P, const RowIn& in, float fo, int lane,
+                                                 float* sv, float* iv) {
+  float mn = DFQ_INF, mx = -DFQ_INF;
+#pragma unroll 4
+  for (int i4 = lane; i4 < n4; i4 += 32) {
+    float4 v = lds_f4(a0 + 16u * i4);
+    if (FOLD) v = mul4(v, fo);
+    minmax4(mn, mx, v);
+  }
+  mn = warp_min(mn); mx = warp_max(mx);
+  const float s = solve_row(P, in, mn, mx, iv);
+  *sv = s;
+  float dsum = 0.f;
+#pragma unroll 4
+  for (int i4 = lane; i4 < n4; i4 += 32) {
+    float4 v = lds_f4(a0 + 16u * i4);
+    if (FOLD) v = mul4(v, fo);
+    const float4 t = mul4(v, s);
     sts_f4(a0 + 16u * i4, t);
     dsum += absdiff4(t, v);
   }
@@ -1230,33 +1266,33 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           RowIn mine;
           float ks = 1.f, kinv = 1.f;
           const bool has_out = c.has_out != 0;
+          // first sweep with the BN fold pending: lane r fetches row r's fold factor
+          const float* fold = c.fold;
+          float fo_mine = 1.f;
+          if (fold && lane < d.nrows) fo_mine = __ldcg(fold + d.row0 + lane);
           if (has_out) {
             // ---- first layer of a chain: per-row range -> s -> rescale (dfq.py:48-73) --------------------------------
             if (lane < d.nrows) mine = fetch_row_in(c, P, d.row0 + lane, false);     // this lane's row: column extrema of the pair
             for (int r = 0; r < d.nrows; ++r) {
               const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
-              float mn = DFQ_INF, mx = -DFQ_INF;
-#pragma unroll 4
-              for (int i4 = lane; i4 < n4; i4 += 32) minmax4(mn, mx, lds_f4(a0 + 16u * i4));
-              mn = warp_min(mn); mx = warp_max(mx);
-              float iv;
-              const float sv = solve_row(P, shfl_row_in(mine, r), mn, mx, &iv);
+              const RowIn in = shfl_row_in(mine, r);
+              float sv, iv;
+              const float dsum = fold ? stack_scale_row<true>(a0, n4, P, in, __shfl_sync(0xffffffffu, fo_mine, r), lane, &sv, &iv)
+                                      : stack_scale_row<false>(a0, n4, P, in, 1.f, lane, &sv, &iv);
               if (lane == r) { ks = sv; kinv = iv; }
-              float dsum = 0.f;
-#pragma unroll 4
-              for (int i4 = lane; i4 < n4; i4 += 32) {
-                const float4 v = lds_f4(a0 + 16u * i4);
-                const float4 t = mul4(v, sv);
-                sts_f4(a0 + 16u * i4, t);
-                dsum += absdiff4(t, v);
-              }
               dacc += (double)dsum * inv_n;
             }
           } else {
             // ---- second layer: columns scaled by 1/s of the relation (dfq.py:73) ------------------------------------
             for (int r = 0; r < d.nrows; ++r) {
               const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
-              const float dsum = kk == 9 ? stack_scale_cols<IN_KK9>(a0, n4, inv_s, lane) : stack_scale_cols<IN_KK1>(a0, n4, inv_s, lane);
+              float dsum;
+              if (fold) {
+                const float fo = __shfl_sync(0xffffffffu, fo_mine, r);
+                dsum = kk == 9 ? stack_scale_cols<IN_KK9, true>(a0, n4, inv_s, fo, lane) : stack_scale_cols<IN_KK1, true>(a0, n4, inv_s, fo, lane);
+              } else {
+                dsum = kk == 9 ? stack_scale_cols<IN_KK9, false>(a0, n4, inv_s, 1.f, lane) : stack_scale_cols<IN_KK1, false>(a0, n4, inv_s, 1.f, lane);
+              }
               dacc += (double)dsum * inv_n;
             }
           }
@@ -1321,9 +1357,80 @@ static int launch_cle(const void* kernel, int grid, int threads, size_t dyn_smem
   return 0;
 }
 
+// Why k_cle_stack cannot take a problem (nullptr: it can); *stack_tiles = the pass tiles of its steps.  See "Eligibility"
+// above k_cle_stack.
+static const char* stack_ineligible(const DfqLayer* layers, int32_t n_layers, const DfqRelation* rels, int32_t n_rels,
+                                    const int32_t* step_ptr, const int32_t* step_layers, int32_t n_steps, int32_t apply_only,
+                                    int64_t* stack_tiles) {
+  *stack_tiles = 0;
+  if (n_steps != 2) return "step count (two steps: every chain has exactly two layers)";
+  if (apply_only) return "apply_only";
+  for (int i = 0; i < n_rels; ++i)
+    if (rels[i].groups != 1) return "groups (every relation ungrouped)";
+  for (int p = 0; p < n_steps; ++p)
+    for (int q = step_ptr[p]; q < step_ptr[p + 1]; ++q) {
+      if (step_layers[q] < 0 || step_layers[q] >= n_layers) return "step layer index";
+      const DfqLayer& l = layers[step_layers[q]];
+      const int row_len = l.cols * l.kk;
+      if (row_len % 4 != 0 || row_len > kStageFloats || l.w_off % 4 != 0)
+        return "row length or alignment (rows of a multiple of 4 floats, at most a stage, 16-byte aligned)";
+      if (l.kk != 9 && l.kk != 1) return "taps (3x3 or 1x1)";
+      if (p == 0 && !(l.rel_in < 0 && l.rel_out >= 0)) return "step count (a first layer that is also a second)";
+      if (p == 1 && !(l.rel_in >= 0 && l.rel_out < 0 && l.col_mode == 0)) return "step count (a second layer that is also a first)";
+      if (p == 1 && !(l.flags & DFQ_LAYER_COLS_READY)) return "column extrema not ready (second layers need COLS_READY)";
+      if (p == 1 && l.cols > kBcExCols) return "columns (at most kBcExCols = 512 per second layer)";
+      *stack_tiles += pass_tiles(l);
+    }
+  return nullptr;
+}
+
+// The one decision between k_cle_stack and k_cle_engine (dfq_cle_run, dfq_cle_takes_stack): *take, and *why the problem is
+// not eligible (nullptr: it is).  Large phases only take the stack kernel (small models are latency-bound); DFQ_CLE_STACK:
+// 0 never takes it, 1 takes every eligible problem.
+static int stack_decision(const DfqLayer* layers, int32_t n_layers, const DfqRelation* rels, int32_t n_rels, const int32_t* step_ptr,
+                          const int32_t* step_layers, int32_t n_steps, int32_t apply_only, bool* take, const char** why) {
+  int dev = 0, sms = 0;
+  DFQ_CUDA(cudaGetDevice(&dev));
+  DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int64_t stack_tiles = 0;
+  *why = stack_ineligible(layers, n_layers, rels, n_rels, step_ptr, step_layers, n_steps, apply_only, &stack_tiles);
+  *take = !*why && stack_tiles >= (int64_t)64 * sms;
+  if (const char* force = getenv("DFQ_CLE_STACK")) *take = !*why && atoi(force) != 0;
+  return 0;
+}
+
+// The weight pass of every DFQ_LAYER_FOLD_PENDING layer that k_cle_stack will not complete (skip[i]: it will), as
+// DFQ_FOLD_APPLY folds: a pending fold is never lost, whichever way dfq_cle_run goes.
+static int apply_pending_folds(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
+                               const std::vector<char>& skip, cudaStream_t st) {
+  std::vector<DfqFold> folds;
+  for (int i = 0; i < n_layers; ++i)
+    if ((layers[i].flags & DFQ_LAYER_FOLD_PENDING) && !(i < (int)skip.size() && skip[i])) {
+      DfqFold f;
+      memset(&f, 0, sizeof(f));
+      f.layer = i; f.mode = DFQ_FOLD_APPLY; f.fac_off = layers[i].fold_off;
+      folds.push_back(f);
+    }
+  if (folds.empty()) return 0;
+  return dfq_bn_fold(arena, arena_floats, layers, n_layers, folds.data(), (int32_t)folds.size(), st);
+}
+
 }  // namespace dfq
 
 using namespace dfq;
+
+extern "C" int dfq_cle_takes_stack(const DfqLayer* layers, int32_t n_layers, const DfqRelation* rels, int32_t n_rels,
+                                   const int32_t* step_ptr, const int32_t* step_layers, int32_t n_steps, int32_t apply_only,
+                                   int32_t* takes) {
+  DFQ_REQUIRE(layers && rels && step_ptr && step_layers && takes, "null argument");
+  DFQ_REQUIRE(n_layers > 0 && n_rels > 0 && n_steps > 0, "empty problem");
+  bool take = false;
+  const char* why = nullptr;
+  const int rc = stack_decision(layers, n_layers, rels, n_rels, step_ptr, step_layers, n_steps, apply_only, &take, &why);
+  if (rc) return rc;
+  *takes = take ? 1 : 0;
+  return 0;
+}
 
 extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
                            const DfqRelation* rels, int32_t n_rels, const int32_t* step_ptr,
@@ -1334,7 +1441,13 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
   DFQ_REQUIRE(n_layers > 0 && n_rels > 0 && n_steps > 0 && n_groups > 0, "empty problem");
   memset(result, 0, sizeof(*result));
   // Python `while diff > thres and count < converge_count` with diff = 10, count = 0 (dfq.py:81-83)
-  if (!(10.0 > params->converge_thres) || !(0 < params->converge_count)) { result->converged = 1; result->last_diff = 10.0; return 0; }
+  // - no sweep at all; a pending fold is completed all the same
+  if (!(10.0 > params->converge_thres) || !(0 < params->converge_count)) {
+    const int rc = apply_pending_folds(arena, arena_floats, layers, n_layers, std::vector<char>(), st);
+    if (rc) return rc;
+    result->converged = 1; result->last_diff = 10.0;
+    return 0;
+  }
 
   // ---- validate descriptors, find the widest phase -----------------------------------------------
   int64_t max_tiles = 1;
@@ -1360,6 +1473,7 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     DFQ_REQUIRE(l.w_off >= 0 && l.w_off + (int64_t)l.rows * l.cols * l.kk <= arena_floats, "weight outside arena");
     DFQ_REQUIRE(l.bias_off >= 0 && l.bias_off + l.rows <= arena_floats, "bias outside arena");
     if (l.rel_in >= 0 && l.rel_out >= 0) DFQ_REQUIRE(l.rel_in < l.rel_out, "relations must be in forward chain order");
+    if (l.flags & DFQ_LAYER_FOLD_PENDING) DFQ_REQUIRE(l.fold_off >= 0 && l.fold_off + l.rows <= arena_floats, "fold factors outside arena");
   }
   // layers whose column extrema the engine scans before the first sweep (the others arrive with buffer 0 filled)
   std::vector<int32_t> scan_layers;
@@ -1385,40 +1499,27 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
 
   // ---- streaming variant for stacks of two-layer chains (k_cle_stack) ----------------------------------------------
   // not_stack: the first eligibility condition the problem fails (nullptr: eligible)
+  bool stack_ok = false;
   const char* not_stack = nullptr;
-  if (n_steps != 2) not_stack = "step count (two steps: every chain has exactly two layers)";
-  else if (params->apply_only) not_stack = "apply_only";
-  for (int i = 0; !not_stack && i < n_rels; ++i)
-    if (rels[i].groups != 1) not_stack = "groups (every relation ungrouped)";
-  int64_t stack_tiles = 0;
-  for (int p = 0; !not_stack && p < n_steps; ++p)
-    for (int q = step_ptr[p]; !not_stack && q < step_ptr[p + 1]; ++q) {
-      const DfqLayer& l = layers[step_layers[q]];
-      const int row_len = l.cols * l.kk;
-      if (row_len % 4 != 0 || row_len > kStageFloats || l.w_off % 4 != 0)
-        not_stack = "row length or alignment (rows of a multiple of 4 floats, at most a stage, 16-byte aligned)";
-      else if (l.kk != 9 && l.kk != 1) not_stack = "taps (3x3 or 1x1)";
-      else if (p == 0 && !(l.rel_in < 0 && l.rel_out >= 0)) not_stack = "step count (a first layer that is also a second)";
-      else if (p == 1 && !(l.rel_in >= 0 && l.rel_out < 0 && l.col_mode == 0)) not_stack = "step count (a second layer that is also a first)";
-      else if (p == 1 && !(l.flags & DFQ_LAYER_COLS_READY)) not_stack = "column extrema not ready (second layers need COLS_READY)";
-      else if (p == 1 && l.cols > kBcExCols) not_stack = "columns (at most kBcExCols = 512 per second layer)";
-      stack_tiles += pass_tiles(l);
-    }
-  // DFQ_CLE_STACK: 0 never takes k_cle_stack, 1 always does and rejects a problem it cannot take (tests compare the two kernels:
-  // a silent fall-back would compare k_cle_engine with itself)
+  int dev = 0, coop = 0, grid = 0, rc;
+  if ((rc = stack_decision(layers, n_layers, rels, n_rels, step_ptr, step_layers, n_steps, params->apply_only, &stack_ok, &not_stack)))
+    return rc;
+  // DFQ_CLE_STACK=1 rejects a problem k_cle_stack cannot take (tests compare the two kernels: a silent fall-back would
+  // compare k_cle_engine with itself)
   const char* force_stack = getenv("DFQ_CLE_STACK");
   if (force_stack && atoi(force_stack) != 0 && not_stack) {
     set_error("DFQ_CLE_STACK=1: problem not eligible for k_cle_stack: %s", not_stack);
     return DFQ_E_ARG;
   }
-  int dev = 0, sms = 0, coop = 0, grid = 0, rc;
   DFQ_CUDA(cudaGetDevice(&dev));
-  DFQ_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int n_entries = step_ptr[n_steps];
   std::vector<long long> pass_ptr(n_entries + 1, 0);    // pass-tile prefix over step_layers
   for (int q = 0; q < n_entries; ++q) pass_ptr[q + 1] = pass_ptr[q] + pass_tiles(layers[step_layers[q]]);
-  bool stack_ok = !not_stack && stack_tiles >= (int64_t)64 * sms;                     // large phases only: small models are latency-bound
-  if (force_stack) stack_ok = !not_stack && atoi(force_stack) != 0;
+  // pending BN folds: k_cle_stack completes those of its step layers in its first sweep; everything else gets the weight pass now
+  std::vector<char> completes(n_layers, 0);
+  if (stack_ok)
+    for (int q = 0; q < n_entries; ++q) completes[step_layers[q]] = 1;
+  if ((rc = apply_pending_folds(arena, arena_floats, layers, n_layers, completes, st))) return rc;
   if (stack_ok) {
     const size_t dyn_s = BcRing::smem_bytes();
     if ((rc = coop_grid((const void*)k_cle_stack, "k_cle_stack", kBcThreads, dyn_s, max_tiles, &grid))) return rc;

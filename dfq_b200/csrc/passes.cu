@@ -42,14 +42,31 @@ struct FoldGeo {
   }
 };
 
-// One output row: W[o,:] *= gamma/sqrt(var+eps) in place (shared memory or, for rows larger than a stage, global).
+// The fold factor of output row o, layer_transform.py:251: gamma / sqrt(var + eps), the quotient formed first and then
+// multiplied into the row.  *den = sqrt(var + eps) for the bias shift.  The one place the factor is computed: a full fold
+// uses it directly, a deferred one stores it (DfqFold.fac_off) for the read-only scan and for whoever applies it later.
+__device__ __forceinline__ float bn_fold_factor(const float* arena, const DfqFold& f, int o, float* den) {
+  *den = __fsqrt_rn(__fadd_rn(arena[f.var_off + o], f.bn_eps));
+  return __fdiv_rn(arena[f.gamma_off + o], *den);
+}
+// The [rows]-vector part of the fold for row o: bias and the BN vectors the equalization / bias correction use.
+__device__ __forceinline__ void bn_fold_vectors(float* arena, const DfqLayer& l, const DfqFold& f, int o, float fac, float den) {
+  // layer_transform.py:260-261: b*f + (beta - (gamma*mean)/sqrt(var+eps))
+  const float gamma = arena[f.gamma_off + o], beta = arena[f.beta_off + o], mean = arena[f.mean_off + o];
+  const float b = arena[l.bias_off + o];
+  const float shift = __fsub_rn(beta, __fdiv_rn(__fmul_rn(gamma, mean), den));
+  arena[l.bias_off + o] = __fadd_rn(__fmul_rn(b, fac), shift);
+  arena[f.fake_w_off + o] = fabsf(gamma);   // :264
+  arena[f.fake_b_off + o] = beta;           // :265
+}
+
+// One output row: W[o,:] *= factor in place (shared memory or, for rows larger than a stage, global).  DFQ_FOLD_FULL forms
+// the factor and does the row's vector part too; DFQ_FOLD_DEFER / _APPLY take the factor stored by the deferring call.
 template <int TPR, bool GLOBAL>
 __device__ __forceinline__ void fold_row(float* arena, const DfqLayer& l, const DfqFold& f, float* row, int o, int lane) {
   const int n = l.cols * l.kk;
-  // layer_transform.py:251: gamma / sqrt(var + eps) formed first, then multiplied in
-  const float gamma = arena[f.gamma_off + o], var = arena[f.var_off + o];
-  const float den = __fsqrt_rn(__fadd_rn(var, f.bn_eps));
-  const float fac = __fdiv_rn(gamma, den);
+  float den = 0.f;
+  const float fac = f.mode == DFQ_FOLD_FULL ? bn_fold_factor(arena, f, o, &den) : arena[f.fac_off + o];
   if (!GLOBAL && (n & 3) == 0) {
     float4* r4 = (float4*)row;
     for (int i = lane; i < (n >> 2); i += TPR) r4[i] = mul4(r4[i], fac);
@@ -58,30 +75,34 @@ __device__ __forceinline__ void fold_row(float* arena, const DfqLayer& l, const 
   } else {
     for (int i = lane; i < n; i += TPR) row[i] = __fmul_rn(row[i], fac);
   }
-  if (lane == 0) {
-    // layer_transform.py:260-261: b*f + (beta - (gamma*mean)/sqrt(var+eps))
-    const float beta = arena[f.beta_off + o], mean = arena[f.mean_off + o];
-    const float b = arena[l.bias_off + o];
-    const float shift = __fsub_rn(beta, __fdiv_rn(__fmul_rn(gamma, mean), den));
-    arena[l.bias_off + o] = __fadd_rn(__fmul_rn(b, fac), shift);
-    arena[f.fake_w_off + o] = fabsf(gamma);   // :264
-    arena[f.fake_b_off + o] = beta;           // :265
-  }
+  if (lane == 0 && f.mode == DFQ_FOLD_FULL) bn_fold_vectors(arena, l, f, o, fac, den);
 }
 
 constexpr int kFoldScanCols = 1024;   // columns whose extrema a CTA accumulates in shared memory (more: global atomics)
 
-// buffer 0 of the column-extrema arrays of every fold that scans: +inf / -inf
-__global__ void k_fold_reset_cols(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restrict__ F, int nF) {
+// The [rows]-vector work before the weight pass, a CTA per fold: buffer 0 of the column extrema of every fold that scans
+// <- +inf / -inf, and the whole vector part of every deferred fold (bias, BN vectors, factors).
+__global__ void k_fold_prologue(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restrict__ F, int nF) {
   for (int q = blockIdx.x; q < nF; q += gridDim.x) {
     const DfqFold f = F[q];
-    if (f.scan_go <= 0) continue;
     const DfqLayer l = L[f.layer];
-    const int nch = (l.rows / f.scan_go) * f.scan_gi;
-    for (int j = threadIdx.x; j < nch; j += blockDim.x) { arena[l.cmin_off + j] = DFQ_INF; arena[l.cmax_off + j] = -DFQ_INF; }
+    if (f.scan_go > 0) {
+      const int nch = (l.rows / f.scan_go) * f.scan_gi;
+      for (int j = threadIdx.x; j < nch; j += blockDim.x) { arena[l.cmin_off + j] = DFQ_INF; arena[l.cmax_off + j] = -DFQ_INF; }
+    }
+    if (f.mode == DFQ_FOLD_DEFER)
+      for (int o = threadIdx.x; o < l.rows; o += blockDim.x) {
+        float den;
+        const float fac = bn_fold_factor(arena, f, o, &den);
+        bn_fold_vectors(arena, l, f, o, fac, den);
+        arena[f.fac_off + o] = fac;
+      }
   }
 }
 
+// The weight pass of the fold.  STORE: folds that rewrite the weights (DFQ_FOLD_FULL, DFQ_FOLD_APPLY).  !STORE: the
+// read-only scan of deferred folds (DFQ_FOLD_DEFER, scan_go > 0): each tile is folded in its stage, scanned and dropped.
+template <bool STORE>
 __global__ void __launch_bounds__(kThreads, kPipeCtas)
 k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restrict__ F, int nF,
           const long long* __restrict__ tptr) {
@@ -110,7 +131,7 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
   while (it.valid()) {
     const int sidx = pipe.acquire();
     const TileDesc d = pipe.desc[sidx];
-    const DfqFold f = F[d.task];
+    const DfqFold& f = F[d.task];     // (a reference: the fields are read as needed, a copy spills)
     const DfqLayer l = L[f.layer];
     const int row_len = l.cols * l.kk;
     if (d.task != cur) {
@@ -123,9 +144,10 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
         dmin = arena + l.cmin_off; dmax = arena + l.cmax_off;    // buffer 0
       }
     }
-    if (d.kind == TK_DIRECT) {
-      for (int r = 0; r < d.nrows; ++r)
-        fold_row<kThreads, true>(arena, l, f, d.gptr + (size_t)r * row_len, d.row0 + r, threadIdx.x);
+    if (d.kind == TK_DIRECT) {        // (!STORE: the host admits no row larger than a stage)
+      if (STORE)
+        for (int r = 0; r < d.nrows; ++r)
+          fold_row<kThreads, true>(arena, l, f, d.gptr + (size_t)r * row_len, d.row0 + r, threadIdx.x);
     } else if (d.nrows == 1) {
       fold_row<kThreads, false>(arena, l, f, pipe.stage[sidx], d.row0, threadIdx.x);
     } else {
@@ -147,7 +169,7 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
       more = ahead.valid();
       if (more) { ahead.fill(nd); ahead.next(); }
     }
-    pipe.release<true>(sidx, more, nd);
+    pipe.release<STORE>(sidx, more, nd);
     it.next();
   }
   flush();
@@ -656,30 +678,54 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
   cudaStream_t st = (cudaStream_t)stream;
   DFQ_REQUIRE(arena && layers && folds, "null argument");
   if (n_folds <= 0) return 0;
-  std::vector<long long> tptr(n_folds + 1, 0);
-  bool any_scan = false;
+  // the weight passes: folds that rewrite the weights (FULL, APPLY) and deferred folds that only scan them; a deferred fold
+  // without a scan moves no weight at all
+  std::vector<DfqFold> rw, ro;
+  std::vector<long long> rw_ptr(1, 0), ro_ptr(1, 0);
+  bool prologue = false;
   for (int i = 0; i < n_folds; ++i) {
-    DFQ_REQUIRE(folds[i].layer >= 0 && folds[i].layer < n_layers, "fold layer index");
-    const DfqLayer& l = layers[folds[i].layer];
-    DFQ_REQUIRE(l.w_off >= 0 && l.w_off + (int64_t)l.rows * l.cols * l.kk <= arena_floats, "weight outside arena");
-    tptr[i + 1] = tptr[i] + pipe_tiles(l.rows, l.cols * l.kk);
-    if (folds[i].scan_go > 0) {
-      const DfqFold& f = folds[i];
+    const DfqFold& f = folds[i];
+    DFQ_REQUIRE(f.layer >= 0 && f.layer < n_layers, "fold layer index");
+    DFQ_REQUIRE(f.mode == DFQ_FOLD_FULL || f.mode == DFQ_FOLD_DEFER || f.mode == DFQ_FOLD_APPLY, "fold mode");
+    const DfqLayer& l = layers[f.layer];
+    const int row_len = l.cols * l.kk;
+    DFQ_REQUIRE(l.w_off >= 0 && l.w_off + (int64_t)l.rows * row_len <= arena_floats, "weight outside arena");
+    if (f.mode != DFQ_FOLD_FULL) DFQ_REQUIRE(f.fac_off >= 0 && f.fac_off + l.rows <= arena_floats, "fold factors outside arena");
+    if (f.scan_go > 0) {
+      DFQ_REQUIRE(f.mode != DFQ_FOLD_APPLY, "DFQ_FOLD_APPLY does not scan");
       DFQ_REQUIRE(f.scan_gi > 0 && l.rows % f.scan_go == 0 && f.scan_gi == l.cols, "fold scan geometry (DfqRelation.go / .gi of the layer's rel_in)");
       const int64_t nch = (int64_t)(l.rows / f.scan_go) * f.scan_gi;
       DFQ_REQUIRE(l.cmin_off >= 0 && l.cmax_off >= 0 && l.cmin_off + 2 * nch <= arena_floats && l.cmax_off + 2 * nch <= arena_floats,
                   "fold scan needs the layer's column range scratch");
-      any_scan = true;
+      prologue = true;
+    }
+    if (f.mode == DFQ_FOLD_DEFER) {
+      prologue = true;
+      if (f.scan_go > 0) {
+        // the read-only scan folds each row in its stage: a row must fit one
+        DFQ_REQUIRE(row_len <= kStageFloats, "deferred fold with a scan: rows larger than a pipe stage");
+        ro.push_back(f);
+        ro_ptr.push_back(ro_ptr.back() + pipe_tiles(l.rows, row_len));
+      }
+    } else {
+      rw.push_back(f);
+      rw_ptr.push_back(rw_ptr.back() + pipe_tiles(l.rows, row_len));
     }
   }
-  int grid, rc;
+  const int n_rw = (int)rw.size(), n_ro = (int)ro.size();
+  int grid_rw = 0, grid_ro = 0, rc;
   const size_t dyn = RowPipe::smem_bytes();
-  if ((rc = coop_grid((const void*)k_bn_fold, "k_bn_fold", kThreads, dyn, tptr[n_folds], &grid))) return rc;
+  if (n_rw && (rc = coop_grid((const void*)k_bn_fold<true>, "k_bn_fold", kThreads, dyn, rw_ptr.back(), &grid_rw))) return rc;
+  if (n_ro && (rc = coop_grid((const void*)k_bn_fold<false>, "k_bn_fold", kThreads, dyn, ro_ptr.back(), &grid_ro))) return rc;
   TablePack tp;
-  const int iL = tp.add(layers, n_layers), iF = tp.add(folds, n_folds), iP = tp.add(tptr.data(), n_folds + 1);
+  const int iL = tp.add(layers, n_layers), iF = tp.add(folds, n_folds);
+  const int iRW = n_rw ? tp.add(rw.data(), n_rw) : -1, iRWP = n_rw ? tp.add(rw_ptr.data(), n_rw + 1) : -1;
+  const int iRO = n_ro ? tp.add(ro.data(), n_ro) : -1, iROP = n_ro ? tp.add(ro_ptr.data(), n_ro + 1) : -1;
   if ((rc = tp.upload(st))) return rc;
-  if (any_scan) k_fold_reset_cols<<<std::min(n_folds, 4096), 128, 0, st>>>(arena, tp.ptr<DfqLayer>(iL), tp.ptr<DfqFold>(iF), n_folds);
-  k_bn_fold<<<grid, kThreads, dyn, st>>>(arena, tp.ptr<DfqLayer>(iL), tp.ptr<DfqFold>(iF), n_folds, tp.ptr<long long>(iP));
+  const DfqLayer* dL = tp.ptr<DfqLayer>(iL);
+  if (prologue) k_fold_prologue<<<std::min(n_folds, 4096), 128, 0, st>>>(arena, dL, tp.ptr<DfqFold>(iF), n_folds);
+  if (n_rw) k_bn_fold<true><<<grid_rw, kThreads, dyn, st>>>(arena, dL, tp.ptr<DfqFold>(iRW), n_rw, tp.ptr<long long>(iRWP));
+  if (n_ro) k_bn_fold<false><<<grid_ro, kThreads, dyn, st>>>(arena, dL, tp.ptr<DfqFold>(iRO), n_ro, tp.ptr<long long>(iROP));
   DFQ_CUDA(cudaGetLastError());
   tp.release(st);
   return 0;

@@ -66,6 +66,7 @@ class Session:
         self._staging: Optional[torch.Tensor] = None
         self.h2d_bytes = 0
         self.d2h_bytes = 0
+        self._pending = None        # a fold plan whose weight pass was deferred into the equalization (plan_bn_fold)
 
     # ---- arena planning ---------------------------------------------------------------------------
     def alloc(self, n: int, align: int = 4) -> int:
@@ -217,6 +218,7 @@ class Session:
         """Copy every bound tensor into the arena: host tensors through ONE pinned staging buffer and one H2D copy per
         run of adjacent mirrors, device tensors with device-to-device copies."""
         self._ensure_room()
+        self.finish_fold()
         x = self._transfer_lists()
         with torch.no_grad():
             if x["h2d_bounds"]:
@@ -233,6 +235,7 @@ class Session:
     def download_begin(self):
         """Enqueue the device-to-host copies of every write-back run (asynchronous; host work that does not read the results
         can overlap them).  download_end() waits and writes the tensors."""
+        self.finish_fold()
         x = self._transfer_lists()
         with torch.no_grad():
             lo, st = x["lo"], self._staging
@@ -266,6 +269,7 @@ class Session:
 
     def view(self, off: int, n: int) -> torch.Tensor:
         self._ensure_room()
+        self.finish_fold()
         return self.arena[off: off + n]
 
     # ---- tables ------------------------------------------------------------------------------------
@@ -275,7 +279,7 @@ class Session:
             t[i]["w_off"] = l["w_off"]; t[i]["bias_off"] = l["bias_off"]
             t[i]["rows"] = l["rows"]; t[i]["cols"] = l["cols"]; t[i]["kk"] = l["kk"]
             t[i]["rel_in"] = -1; t[i]["rel_out"] = -1; t[i]["col_mode"] = 0; t[i]["group"] = 0
-            t[i]["cmin_off"] = -1; t[i]["cmax_off"] = -1
+            t[i]["cmin_off"] = -1; t[i]["cmax_off"] = -1; t[i]["fold_off"] = -1
             if roles and i in roles:
                 for k, v in roles[i].items():
                     t[i][k] = v
@@ -288,7 +292,13 @@ class Session:
     def plan_bn_fold(self, folds: Sequence[dict], cle_plan: Optional[dict] = None) -> dict:
         """cle_plan: the equalization plan that will run right after this fold.  The fold then also writes the column
         extrema of every folded `second` layer (it has each tile in shared memory anyway) and `plan["scanned"]` lists those
-        layers: pass it to run_cle_plan(cols_ready=...) so that the equalization skips its initial 4 B/weight scan."""
+        layers: pass it to run_cle_plan(cols_ready=...) so that the equalization skips its initial 4 B/weight scan.
+
+        When the library reports that cle_plan runs on the stack kernel (dfq_cle_takes_stack), the fold of the plan's layers
+        is DEFERRED: run_bn_fold does the [rows]-vector work and a read-only scan of the `second` layers, and the
+        equalization's first sweep multiplies every row by its fold factor as it reads it - one read-write pass over the
+        weights fewer.  Until run_cle_plan(cle_plan) has run, every other call of this session that touches the arena
+        completes the fold first (finish_fold), so nothing ever sees unfolded weights."""
         ft = np.zeros(len(folds), dtype=_lib.FOLD_DT)
         scanned = []
         for i, f in enumerate(folds):
@@ -299,7 +309,32 @@ class Session:
                 if ri >= 0:
                     ft[i]["scan_go"] = cle_plan["rt"][ri]["go"]; ft[i]["scan_gi"] = cle_plan["rt"][ri]["gi"]
                     scanned.append(int(f["layer"]))
-        return dict(ft=ft, lt=cle_plan["lt"] if cle_plan is not None else self._layer_table(), scanned=scanned)
+        deferred = []
+        if cle_plan is not None and self._takes_stack(cle_plan, scanned):
+            in_plan = set(int(x) for x in cle_plan["step_layers"])
+            for i, f in enumerate(folds):
+                li = int(f["layer"])
+                if li in in_plan:
+                    ft[i]["mode"] = _lib.FOLD_DEFER
+                    ft[i]["fac_off"] = self.alloc(self._layers[li]["rows"])
+                    deferred.append((li, int(ft[i]["fac_off"])))
+        return dict(ft=ft, lt=cle_plan["lt"] if cle_plan is not None else self._layer_table(), scanned=scanned,
+                    deferred=deferred, cle_plan=cle_plan)
+
+    def _takes_stack(self, cle_plan: dict, cols_ready: Sequence[int]) -> bool:
+        """Whether dfq_cle_run will take `cle_plan` (with these layers' column extrema ready) on the stack kernel - the
+        library's own decision.  A library without the query (a test stand-in) never defers."""
+        fn = getattr(self.lib, "dfq_cle_takes_stack", None)
+        if fn is None:
+            return False
+        lt = cle_plan["lt"].copy()
+        if cols_ready:
+            lt["flags"][list(cols_ready)] |= _lib.LAYER_COLS_READY
+        takes = np.zeros(1, dtype=np.int32)
+        _lib.check(fn(_lib.table_ptr(lt), len(lt), _lib.table_ptr(cle_plan["rt"]), len(cle_plan["rt"]),
+                      _lib.table_ptr(cle_plan["step_ptr"]), _lib.table_ptr(cle_plan["step_layers"]), cle_plan["n_steps"], 0,
+                      _lib.table_ptr(takes)), "dfq_cle_takes_stack")
+        return bool(takes[0])
 
     def run_bn_fold(self, folds):
         """folds: dicts(layer, bn_eps, gamma_off, beta_off, mean_off, var_off, fake_w_off, fake_b_off), or a plan."""
@@ -307,7 +342,27 @@ class Session:
         if plan is None:
             return
         self._ensure_room()
+        self.finish_fold()
         ft, lt = plan["ft"], plan["lt"]
+        _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
+                                        _lib.table_ptr(ft), len(ft), _lib.stream_ptr()), "dfq_bn_fold")
+        if plan.get("deferred"):
+            self._pending = plan
+
+    @property
+    def fold_pending(self) -> bool:
+        """A deferred fold's weight pass is still outstanding (see plan_bn_fold)."""
+        return self._pending is not None
+
+    def finish_fold(self):
+        """Complete a deferred fold now: W[o,:] *= its stored factor (one read-write pass over the deferred layers)."""
+        plan, self._pending = self._pending, None
+        if plan is None:
+            return
+        ft = np.zeros(len(plan["deferred"]), dtype=_lib.FOLD_DT)
+        for k, (li, fac_off) in enumerate(plan["deferred"]):
+            ft[k]["layer"] = li; ft[k]["mode"] = _lib.FOLD_APPLY; ft[k]["fac_off"] = fac_off
+        lt = plan["lt"]
         _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
                                         _lib.table_ptr(ft), len(ft), _lib.stream_ptr()), "dfq_bn_fold")
 
@@ -381,8 +436,13 @@ class Session:
     def run_cle_plan(self, plan: dict, s_range=(1e-8, 1e8), converge_thres=2e-7, converge_count=20, signed=False,
                      eps=0, max_sweeps=0, apply_only=False, cols_ready: Optional[Sequence[int]] = None) -> CleResult:
         """Run dfq.py:78-117 on a planned relation list; see include/dfq_b200.h dfq_cle_run.
-        cols_ready: layers whose column extrema (buffer 0) a fold planned with cle_plan=plan has JUST written."""
+        cols_ready: layers whose column extrema (buffer 0) a fold planned with cle_plan=plan has JUST written.
+        A fold planned with cle_plan=plan and deferred (plan_bn_fold) is completed by this call."""
         self._ensure_room()
+        pending = self._pending
+        if pending is not None and pending["cle_plan"] is not plan:
+            self.finish_fold()
+            pending = None
         lo, hi = float(s_range[0]), float(s_range[1])
         P = np.zeros(1, dtype=_lib.CLE_PARAMS_DT)
         P[0]["s_lo"] = np.float32(lo); P[0]["s_hi"] = np.float32(hi)
@@ -402,12 +462,25 @@ class Session:
                 lt2["flags"][list(cols_ready)] |= _lib.LAYER_COLS_READY
                 plan["_ready_key"], plan["_ready_lt"] = key, lt2
             lt = plan["_ready_lt"]
+        if pending is not None:
+            # the deferred layers are marked FOLD_PENDING: the stack kernel folds them in its first sweep, any other path of
+            # dfq_cle_run applies the fold before it starts
+            key = (id(lt), tuple(pending["deferred"]))
+            if pending.get("_pending_key") != key:
+                lt2 = lt.copy()
+                li = [d[0] for d in pending["deferred"]]
+                lt2["flags"][li] |= _lib.LAYER_FOLD_PENDING
+                lt2["fold_off"][li] = [d[1] for d in pending["deferred"]]
+                pending["_pending_key"], pending["_pending_lt"], pending["_pending_base"] = key, lt2, lt
+            lt = pending["_pending_lt"]
         gs = np.zeros(plan["n_groups"], dtype=np.int32)
         _lib.check(self.lib.dfq_cle_run(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
                                         _lib.table_ptr(rt), len(rt), _lib.table_ptr(plan["step_ptr"]),
                                         _lib.table_ptr(plan["step_layers"]), plan["n_steps"], _lib.table_ptr(P),
                                         _lib.table_ptr(R), plan["n_groups"], _lib.table_ptr(gs), _lib.stream_ptr()),
                    "dfq_cle_run")
+        if pending is not None:
+            self._pending = None
         n = int(R[0]["n_sweeps"])
         res = CleResult(n, bool(R[0]["converged"]), float(R[0]["last_diff"]), [float(x) for x in R[0]["diffs"][:min(n, 64)]])
         res.group_sweeps = gs
@@ -487,6 +560,7 @@ class Session:
     def run_bias_correct_plan(self, plan: dict, num_bits: int = 8, col_hints: Optional[Dict[str, np.ndarray]] = None):
         """col_hints: see cle_col_hints (only meaningful for the layers' CURRENT weights)."""
         self._ensure_room()
+        self.finish_fold()
         lt, bt, tt = plan["lt"], plan["bt"], plan["tt"]
         if col_hints is not None and len(col_hints["layer"]):
             bt = bt.copy()
@@ -529,5 +603,6 @@ class Session:
                 return
             qt = self.plan_quantize(tasks)["qt"]
         self._ensure_room()
+        self.finish_fold()
         _lib.check(self.lib.dfq_quantize_tensors(self._ptr(), self.arena.numel(), _lib.table_ptr(qt), len(qt),
                                                  int(div_mode), _lib.stream_ptr()), "dfq_quantize_tensors")

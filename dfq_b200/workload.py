@@ -170,9 +170,13 @@ def stack_topology(n_blocks: int, channels: int = 512, k: int = 3, in_channels: 
 class DeviceStack:
     """`n_blocks` independent Conv[C,C,k,k]+BN+ReLU -> Conv[C,C,k,k]+BN blocks living only in a Session arena.
 
-    Pipeline per calibration step (the BASELINE metric's unit of work, per Conv/BN pair):
-      BN fold (8N B) -> equalization to convergence (8N B per sweep, 2 sweeps) -> bias correction of the second
-      conv (4N B read once - its range comes from the equalization's column extrema - = 2N B per pair on average) [-> 8-bit weight fake-quant (8N+4N B)]
+    Pipeline per calibration step (the BASELINE metric's unit of work, per Conv/BN pair), N weights per conv:
+      BN fold: the per-channel vectors and a read-only scan of the second conv's column extrema (4N B per block = 2N B
+      per conv on average; the weight pass itself is deferred into the first sweep, see Session.plan_bn_fold) ->
+      equalization to convergence (8N B per sweep, 2 sweeps; the first sweep also folds) -> bias correction of the second
+      conv (4N B read once - its range comes from the equalization's column extrema - = 2N B per conv on average)
+      [-> 8-bit weight fake-quant (8N+4N B)].  20N B per conv in all (26N B with the fold as a pass of its own: the
+      engine path, where the fold is not deferred).
     """
 
     def __init__(self, sess, n_blocks: int, channels: int = 512, k: int = 3, seed: int = 1234, quantize: bool = False):
@@ -281,9 +285,10 @@ class DeviceStack:
 
     @property
     def launches_per_step(self) -> int:
-        """Kernels of this library per step: column-range reset + fold, equalization engine, correction engine
-        [+ range init, min/max, quantize], plus the small copy kernel (k_copy_words) that moves each call's descriptor tables
-        (fold, equalization, correction [, quantize]) and the equalization's two result blocks through mapped pinned memory."""
+        """Kernels of this library per step: fold prologue (column-range reset, the deferred fold's vectors) + fold pass
+        (the read-only scan when deferred), equalization engine, correction engine [+ range init, min/max, quantize], plus
+        the small copy kernel (k_copy_words) that moves each call's descriptor tables (fold, equalization, correction
+        [, quantize]) and the equalization's two result blocks through mapped pinned memory."""
         return 4 + 5 + (4 if self.quant_plan is not None else 0)
 
 

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 5
+#define DFQ_ABI_VERSION 6
 
 enum {
   DFQ_OK = 0,
@@ -75,15 +75,26 @@ typedef struct DfqLayer {
   int32_t group;      /* convergence group (= model) this layer belongs to, 0 .. n_groups-1    */
   int32_t flags;      /* DFQ_LAYER_COLS_READY: buffer 0 of cmin/cmax already holds the column extrema of the
                          current weights (dfq_bn_fold with DfqFold.scan_go > 0 just produced them): dfq_cle_run
-                         skips its initial scan of this layer                                  */
+                         skips its initial scan of this layer
+                         DFQ_LAYER_FOLD_PENDING: see below                                     */
   int64_t cmin_off;   /* [2][C of rel_in] running column minima, double-buffered by sweep parity
                          (scratch, valid when rel_in >= 0)                                  */
   int64_t cmax_off;   /* [2][C of rel_in] running column maxima                              */
+  int64_t fold_off;   /* DFQ_LAYER_FOLD_PENDING: [rows] fold factors gamma/sqrt(var+eps) (DfqFold.fac_off)      */
 } DfqLayer;
+
+/* Both flags are promises about the call that runs RIGHT AFTER dfq_bn_fold, on the same weights:
+ *   DFQ_LAYER_COLS_READY   the fold (scan_go > 0) has written buffer 0 of the column extrema of the FOLDED weights.
+ *   DFQ_LAYER_FOLD_PENDING the fold ran with DfqFold.mode = DFQ_FOLD_DEFER: biases, BN vectors and the factors at fold_off
+ *                          are final, the weights are NOT yet multiplied by the factors.  dfq_cle_run completes the fold:
+ *                          k_cle_stack multiplies each row by its factor as its first sweep reads it (fl(w * f), the value
+ *                          the fold would have stored); on every other path (the engine, no sweep at all) the fold is
+ *                          applied to the weights before anything else.  Either way the weights are folded on return. */
+#define DFQ_LAYER_COLS_READY 1
+#define DFQ_LAYER_FOLD_PENDING 2
 
 /* One equalization relation (utils/relation.py:5-27): rows of `first` are multiplied by s[c],
  * the matching input columns of `second` by 1/s[c] (dfq.py:62-73). */
-#define DFQ_LAYER_COLS_READY 1
 
 typedef struct DfqRelation {
   int32_t first;
@@ -144,6 +155,14 @@ int dfq_cle_run(float* arena, int64_t arena_floats,
                 int32_t n_groups, int32_t* group_sweeps /* host, [n_groups] sweeps run per group, or NULL */,
                 void* stream);
 
+/* *takes = 1 when dfq_cle_run would run this problem (same tables, DfqCleParams.apply_only = apply_only) on the
+ * streaming stack kernel k_cle_stack on the current device, 0 when on k_cle_engine - the one decision dfq_cle_run makes
+ * (including the DFQ_CLE_STACK override).  A fold may defer its weight pass (DFQ_FOLD_DEFER) only into a k_cle_stack run:
+ * on the engine path the deferred fold costs an extra pass.  No GPU work, no synchronisation. */
+int dfq_cle_takes_stack(const DfqLayer* layers, int32_t n_layers, const DfqRelation* rels, int32_t n_rels,
+                        const int32_t* step_ptr, const int32_t* step_layers, int32_t n_steps, int32_t apply_only,
+                        int32_t* takes);
+
 /* BN fold (utils/layer_transform.py:231-276, merge_batchnorm), batched over layers.
  * W[o,:] *= gamma[o]/sqrt(var[o]+eps); b = b*f + (beta - gamma*mean/sqrt(var+eps));
  * fake_weight = |gamma|, fake_bias = beta. */
@@ -156,7 +175,19 @@ typedef struct DfqFold {
                                  group (DfqRelation.go / .gi): also write the column extrema of the FOLDED weights into
                                  buffer 0 of the layer's cmin_off / cmax_off (layers[] must carry them), saving the
                                  equalization its initial 4 B/weight scan.  0: no scan. */
+  int32_t mode;               /* DFQ_FOLD_FULL / _DEFER / _APPLY, below                                              */
+  int32_t _pad;
+  int64_t fac_off;            /* _DEFER, _APPLY: [rows] fold factors gamma/sqrt(var+eps)                              */
 } DfqFold;
+/* DFQ_FOLD_FULL   the fold above: weights, bias, fake_weight / fake_bias.
+ * DFQ_FOLD_DEFER  everything but the weights: bias, fake_weight / fake_bias, and each row's factor into fac_off.  With
+ *                 scan_go > 0 the weights are READ (not written) and the column extrema of fl(w * factor) - those of the
+ *                 folded weights - go to buffer 0.  The weights stay unfolded until a DFQ_LAYER_FOLD_PENDING layer entry
+ *                 (fold_off = fac_off) hands them to dfq_cle_run, or a DFQ_FOLD_APPLY call completes the fold.
+ * DFQ_FOLD_APPLY  the weights only: W[o,:] = fl(W[o,:] * fac[o]); gamma / beta / mean / var / bias are not read. */
+#define DFQ_FOLD_FULL 0
+#define DFQ_FOLD_DEFER 1
+#define DFQ_FOLD_APPLY 2
 int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
                 const DfqFold* folds, int32_t n_folds, void* stream);
 
