@@ -167,14 +167,17 @@ __device__ __forceinline__ float absdiff4(const float4& t, const float4& v) {
   return fabsf(__fsub_rn(t.x, v.x)) + fabsf(__fsub_rn(t.y, v.y)) + fabsf(__fsub_rn(t.z, v.z)) + fabsf(__fsub_rn(t.w, v.w));
 }
 
-// float atomic min/max through the integer ordering of IEEE bit patterns (works in global and shared).
+// float atomic min/max through the integer ordering of IEEE bit patterns (works in global and shared): signed-int order
+// for values with a clear sign bit, reversed unsigned order for those with it set.  The branch tests the sign BIT: -0.0
+// (0x80000000, INT_MIN as a signed int) compares >= 0.f, and taking the signed branch for it would let a -0.0 minimum
+// overwrite a negative one and a -0.0 maximum lose to one (folded rows of a zero BN scale are +-0.0).
 __device__ __forceinline__ void atomic_min_f(float* addr, float v) {
-  if (v >= 0.f) atomicMin((int*)addr, __float_as_int(v));
-  else          atomicMax((unsigned int*)addr, __float_as_uint(v));
+  if (!(__float_as_uint(v) >> 31)) atomicMin((int*)addr, __float_as_int(v));
+  else                             atomicMax((unsigned int*)addr, __float_as_uint(v));
 }
 __device__ __forceinline__ void atomic_max_f(float* addr, float v) {
-  if (v >= 0.f) atomicMax((int*)addr, __float_as_int(v));
-  else          atomicMin((unsigned int*)addr, __float_as_uint(v));
+  if (!(__float_as_uint(v) >> 31)) atomicMax((int*)addr, __float_as_int(v));
+  else                             atomicMin((unsigned int*)addr, __float_as_uint(v));
 }
 
 // ------------------------------------------------------------------------------------------

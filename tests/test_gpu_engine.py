@@ -9,16 +9,10 @@ import pytest
 import torch
 
 from oracle import dfq_oracle as O
+from stack_cases import DEFAULT_PARAMS, STACK_BLOCKS, VECTORS, chain_layers, oracle_chains
+from stack_cases import mk as _mk
 
 pytestmark = pytest.mark.gpu
-
-
-def _mk(shape, seed, gain=True):
-    g = torch.Generator().manual_seed(seed)
-    w = torch.randn(*shape, generator=g)
-    if gain:
-        w = w * (10 ** torch.empty(shape[0]).uniform_(-1, 1, generator=g)).view(-1, *([1] * (len(shape) - 1)))
-    return w.contiguous()
 
 
 def _normwise(a, b):
@@ -445,58 +439,77 @@ def test_mid_size_stacks_run_the_streaming_kernels_and_match_the_oracle(n_blocks
         assert r["bias_rows_outside_bound"] == 0, (b, r)
 
 
-STACK_BLOCKS = [
-    ((128, 64, 3, 3), (256, 128, 3, 3)),   # non-square 3x3 block
-    ((96, 64, 3, 3), (200, 96, 1, 1)),     # 3x3 next to 1x1
-    ((512, 256, 1, 1), (64, 512, 3, 3)),   # second layer at kBcExCols 512 columns and kStageFloats 4608 floats
-    ((44, 16, 3, 3), (37, 44, 3, 3)),      # 396-float rows: 11 per tile, 37 rows = partial tiles, not a multiple of 32
-    ((100, 4, 3, 3), (24, 100, 1, 1)),     # 36-float rows: 4608 / 36 = 128, capped at 32 rows per tile
-]
-
-
-def _chains_session(chains, one_group, stack, bc_variant, hints, monkeypatch, seed=61):
-    """Fold -> equalize -> bias-correct a list of chains (shapes per chain) in one Session, each layer with a BN: chain i is
-    convergence group i (or all one group); the second layer of every chain is corrected with the first's ReLU expectation.
-    `stack`: DFQ_CLE_STACK value (None: unset).  Returns (before, after, res, deltas, expects) - per chain lists of layer dicts."""
-    from dfq_b200.engine import Session
-    if stack is None:
-        monkeypatch.delenv("DFQ_CLE_STACK", raising=False)
-    else:
-        monkeypatch.setenv("DFQ_CLE_STACK", stack)
-    _force_bc_variant(monkeypatch, bc_variant)
-    g = torch.Generator().manual_seed(seed)
-    sess = Session()
-    lay, rels, groups, folds, items = [], [], [], [], []
-    for ci, shapes in enumerate(chains):
-        cl = []
-        for k, s in enumerate(shapes):
-            d = dict(w=_mk(s, seed + 7 * ci + k, gain=(k % 2 == 0)) * 0.1, bias=torch.randn(s[0], generator=g) * 0.1,
-                     gamma=torch.rand(s[0], generator=g) + 0.5, beta=torch.randn(s[0], generator=g) * 0.2,
-                     mean=torch.randn(s[0], generator=g) * 0.1, var=torch.rand(s[0], generator=g) + 0.5)
+def _bind_chains(sess, lay, one_group, signed=False):
+    """Binds the layer dicts of stack_cases.chain_layers into `sess` (weights, biases, BN vectors; fake_weight / fake_bias scratch)
+    and returns (relations, groups, folds, correction items): chain i is convergence group i (or all one group); the second layer
+    of every chain is corrected with the first's ReLU expectation."""
+    rels, groups, folds, items = [], [], [], []
+    for ci, cl in enumerate(lay):
+        for d in cl:
             d["li"] = sess.add_layer(d["w"], d["bias"])
             for n in ("gamma", "beta", "mean", "var"):
                 d[n + "_off"] = sess.bind(d[n], False)
-            d["fake_w_off"], d["fake_b_off"] = sess.alloc(s[0]), sess.alloc(s[0])
-            folds.append(dict(layer=d["li"], bn_eps=1e-5, gamma_off=d["gamma_off"], beta_off=d["beta_off"], mean_off=d["mean_off"],
+            d["fake_w_off"], d["fake_b_off"] = sess.alloc(d["w"].shape[0]), sess.alloc(d["w"].shape[0])
+            folds.append(dict(layer=d["li"], bn_eps=d["bn_eps"], gamma_off=d["gamma_off"], beta_off=d["beta_off"], mean_off=d["mean_off"],
                               var_off=d["var_off"], fake_w_off=d["fake_w_off"], fake_b_off=d["fake_b_off"]))
-            cl.append(d)
-        for k in range(len(shapes) - 1):
+        for k in range(len(cl) - 1):
             rels.append((cl[k]["li"], cl[k + 1]["li"], cl[k]["fake_w_off"], cl[k]["fake_b_off"]))
             groups.append(0 if one_group else ci)
-        items.append(dict(layer=cl[1]["li"], signed=False, level=0, next_bn_b_off=cl[1]["fake_b_off"],
-                          terms=[dict(bn_w_off=cl[0]["fake_w_off"], bn_b_off=cl[0]["fake_b_off"], n=shapes[0][0], relu=True, op="set")]))
-        lay.append(cl)
-    before = [[dict((n, d[n].numpy().copy()) for n in ("w", "bias", "gamma", "beta", "mean", "var")) for d in cl] for cl in lay]
+        items.append(dict(layer=cl[1]["li"], signed=signed, level=0, next_bn_b_off=cl[1]["fake_b_off"],
+                          terms=[dict(bn_w_off=cl[0]["fake_w_off"], bn_b_off=cl[0]["fake_b_off"], n=cl[0]["w"].shape[0], relu=True,
+                                      op="set")]))
+    return rels, groups, folds, items
+
+
+def _chains_session(chains, one_group, stack, bc_variant, hints, monkeypatch, seed=61, params=None, edit=None, correct=True,
+                    plan_stack="same", extra=None):
+    """Fold -> equalize -> bias-correct a list of chains (shapes per chain) in one Session, each layer with a BN: chain i is
+    convergence group i (or all one group); the second layer of every chain is corrected with the first's ReLU expectation.
+    `stack`: DFQ_CLE_STACK value (None: unset) while the equalization runs; `plan_stack`: its value while the fold is planned
+    (default: the same).  `params`: equalization parameters other than stack_cases.DEFAULT_PARAMS; `edit(ci, k, d)`: changes a
+    layer's w / gamma / beta / mean / var / bn_eps before it is bound (stack_cases.chain_layers); `correct`: False skips the
+    correction (deltas and expects are then empty).  `extra` (a dict): receives the fold plan, the column extrema buffer 0 of
+    every second layer as the fold left them (read without completing a deferred fold) and the column hints.
+    Returns (before, after, res, deltas, expects, s) - per chain lists of layer dicts."""
+    from dfq_b200.engine import Session
+
+    def set_stack(v):
+        if v is None:
+            monkeypatch.delenv("DFQ_CLE_STACK", raising=False)
+        else:
+            monkeypatch.setenv("DFQ_CLE_STACK", v)
+    p = dict(DEFAULT_PARAMS, **(params or {}))
+    set_stack(stack if plan_stack == "same" else plan_stack)
+    _force_bc_variant(monkeypatch, bc_variant)
+    sess = Session()
+    lay = chain_layers(chains, seed, edit)
+    rels, groups, folds, items = _bind_chains(sess, lay, one_group, p["signed"])
+    before = [[dict((n, d[n].numpy().copy()) for n in VECTORS) for d in cl] for cl in lay]
+    for cl, bl in zip(lay, before):
+        for d, b in zip(cl, bl):
+            b["bn_eps"] = d["bn_eps"]
     cle = sess.plan_cle(rels, groups=groups)
     fold = sess.plan_bn_fold(folds, cle_plan=cle)
-    bc = sess.plan_bias_correct(items)
+    bc = sess.plan_bias_correct(items) if correct else None
+    set_stack(stack)
     sess.upload()
     sess.run_bn_fold(fold)
-    res = sess.run_cle_plan(cle, cols_ready=fold["scanned"])
-    sess.run_bias_correct_plan(bc, 8, col_hints=sess.cle_col_hints(cle, res) if hints else None)
+    if extra is not None:
+        raw = lambda off, n: sess.arena[int(off): int(off) + int(n)].cpu().numpy().copy()   # (view() would complete the fold)
+        extra["fold"] = fold
+        extra["cols0"] = [(raw(cle["lt"][cl[1]["li"]]["cmin_off"], cl[0]["w"].shape[0]),
+                           raw(cle["lt"][cl[1]["li"]]["cmax_off"], cl[0]["w"].shape[0])) for cl in lay]
+    res = sess.run_cle_plan(cle, s_range=p["s_range"], converge_thres=p["converge_thres"], converge_count=p["converge_count"],
+                            signed=p["signed"], eps=p["eps"], max_sweeps=p["max_sweeps"], cols_ready=fold["scanned"])
     view = lambda off, n: sess.view(int(off), int(n)).cpu().numpy().copy()
-    deltas = [view(bc["delta_offs"][i], chains[i][1][0]) for i in range(len(chains))]
-    expects = [view(b["expect_off"], b["expect_len"]) for b in bc["bt"]]          # one level: table order = chain order
+    deltas, expects = [], []
+    if correct:
+        col_hints = sess.cle_col_hints(cle, res) if hints else None
+        if extra is not None:
+            extra["hints"] = col_hints
+        sess.run_bias_correct_plan(bc, 8, col_hints=col_hints)
+        deltas = [view(bc["delta_offs"][i], chains[i][1][0]) for i in range(len(chains))]
+        expects = [view(b["expect_off"], b["expect_len"]) for b in bc["bt"]]          # one level: table order = chain order
     s = [view(o, sess.layer(r[0])["rows"]) for o, r in zip(cle["s_offs"], rels)]
     sess.download()
     after = [[dict(w=d["w"].numpy().copy(), bias=d["bias"].numpy().copy(), fake_w=view(d["fake_w_off"], d["w"].shape[0]),
@@ -504,25 +517,10 @@ def _chains_session(chains, one_group, stack, bc_variant, hints, monkeypatch, se
     return before, after, res, deltas, expects, s
 
 
-def _oracle_chains(before, one_group):
-    """The oracle of _chains_session: BN fold, equalization (per chain, or one call over all chains), correction of layer 1."""
-    out = []
-    layers, bns, rels = [], [], []
-    for cl in before:
-        base = len(layers)
-        for d in cl:
-            w2, b2, fw, fb = O.bn_fold(d["w"], d["bias"], d["gamma"], d["beta"], d["mean"], d["var"], 1e-5)
-            layers.append(O.OLayer(w2, b2)); bns.append([fw, fb])
-        crel = [O.ORelation(base + k, base + k + 1, base + k) for k in range(len(cl) - 1)]
-        if not one_group:
-            crel_local = [O.ORelation(k, k + 1, k) for k in range(len(cl) - 1)]
-            n, _ = O.cross_layer_equalization(layers[base:], [tuple(x) for x in bns[base:]], crel_local)
-            out.append(n)
-        rels += crel
-    if one_group:
-        n, _ = O.cross_layer_equalization(layers, [tuple(x) for x in bns], rels)
-        out = [n] * len(before)
-    return layers, bns, out
+def _oracle_chains(before, one_group, params=None):
+    """The oracle of _chains_session (stack_cases.oracle_chains): (layers, bns, sweeps per group, diffs per group, S per
+    relation)."""
+    return oracle_chains(before, one_group, params)
 
 
 @pytest.mark.parametrize("one_group", [False, True])
@@ -542,7 +540,7 @@ def test_heterogeneous_stack_kernel_equals_engine_and_oracle(one_group, bc_varia
                 assert np.array_equal(p[k], q[k]), k
     for x, y in zip(s1 + d1 + e1, s0 + d0 + e0):
         assert np.array_equal(x, y)
-    layers, bns, sweeps = _oracle_chains(before, one_group)
+    layers, bns, sweeps = _oracle_chains(before, one_group)[:3]
     assert list(r1.group_sweeps) == (sweeps[:1] if one_group else sweeps)
     for b, cl in enumerate(a1):
         l0, l1 = layers[2 * b], layers[2 * b + 1]
@@ -573,7 +571,7 @@ def test_forced_stack_kernel_rejects_what_it_cannot_run(chains, reason, monkeypa
     with pytest.raises(DfqError, match=reason):
         _chains_session(chains, False, "1", "engine", False, monkeypatch)
     before, after, res, deltas, _, _ = _chains_session(chains, False, None, "engine", False, monkeypatch)
-    layers, bns, sweeps = _oracle_chains(before, False)
+    layers, bns, sweeps = _oracle_chains(before, False)[:3]
     assert list(res.group_sweeps) == sweeps
     for d, l in zip(after[0], layers):
         assert np.array_equal(d["w"], l.w.reshape(d["w"].shape))
