@@ -14,7 +14,8 @@
 // and the residual epilogue (dfq_i8_conv_fused): clamp, fp32 residual add, clamp, then fp32 NCHW and / or the codes, so a
 // residual block's add and an output with several consumers need no separate pass over an fp32 tensor.  The code stores of
 // the last two can target a channel slice of a wider tensor (dfq_i8_conv_slice), so the producers of a channel
-// concatenation write the consumer's input directly; k_i8_maxpool pools codes, or fp32 to fp32 and / or codes.
+// concatenation write the consumer's input directly; k_i8_maxpool pools codes, or fp32 to fp32 and / or codes;
+// k_i8_upsample_bilinear resizes fp32 as torch does, to fp32 and / or codes in such a channel slice.
 #include <algorithm>
 #include <cmath>
 
@@ -498,6 +499,79 @@ __global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restr
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// bilinear upsampling: one thread per (n, 16 channels, output pixel), pixels fastest, as k_i8_conv_dw
+// ------------------------------------------------------------------------------------------------------------------
+// x fp32 NCHW [N, C, H, W] -> y fp32 NCHW [N, C, OH, OW] and / or the codes q8(clamp(y, lo, hi), out_scale) into channels
+// [coff, coff + round_up(C, 16)) of int8 NHWC yq [N, OH, OW, cstride] (one 16-byte store per thread, pad channels 0).
+// y is bit for bit torch's CUDA upsample_bilinear2d_out_frame<float, float>.  torch compiles that kernel with contraction
+// on; its sm_90 SASS (torch 2.11) is, per axis and per element:
+//   src = align_corners ? FMUL(dst, scale) : FFMA(FADD(dst, 0.5), scale, -0.5), then src < 0 ? 0 : src (NaN kept)
+//   i   = F2I.TRUNC(src), l1 = FADD(src, -i), l0 = FADD(1, -l1), i + 1 only while i < in - 1
+//   row = FFMA(w_l0, x[h][w_i], FMUL(w_l1, x[h][w_i + w_p]))             for h = h_i and h_i + h_p
+//   y   = FFMA(h_l0, row(h_i), FMUL(h_l1, row(h_i + h_p)))
+// The library builds with --fmad=false, so the same operations are spelled out with __fmaf_rn / __fmul_rn / __fadd_rn.
+// An unchanged size is torch's plain copy (0 * inf and -0.0 + 0.0 would make the formula differ from x).
+struct BilinearTap {
+  int i0, i1;
+  float l0, l1;
+};
+
+__device__ __forceinline__ BilinearTap bilinear_tap(int dst, float scale, bool align_corners, int in) {
+  float src = align_corners ? __fmul_rn((float)dst, scale) : __fmaf_rn(__fadd_rn((float)dst, 0.5f), scale, -0.5f);
+  if (!align_corners) src = src < 0.f ? 0.f : src;
+  BilinearTap t;
+  t.i0 = (int)src;
+  t.i1 = t.i0 + (t.i0 < in - 1 ? 1 : 0);
+  t.l1 = __fadd_rn(src, -(float)t.i0);
+  t.l0 = __fadd_rn(1.f, -t.l1);
+  return t;
+}
+
+__global__ void k_i8_upsample_bilinear(const float* __restrict__ x, float* __restrict__ y, int8_t* __restrict__ yq,
+                                       DfqI8Resize g, float scale_h, float scale_w, int64_t total) {
+  const int chunks = (g.C + 15) / 16;
+  const int64_t HW = (int64_t)g.H * g.W, OHW = (int64_t)g.OH * g.OW;    // a plane may exceed 2^31 pixels
+  const bool copy = g.H == g.OH && g.W == g.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i % OHW;
+    const int64_t t = i / OHW;
+    const int ch = (int)(t % chunks);
+    const int64_t n = t / chunks;
+    const int oh = (int)(p / g.OW), ow = (int)(p % g.OW);
+    const BilinearTap th = bilinear_tap(oh, scale_h, g.align_corners, g.H);
+    const BilinearTap tw = bilinear_tap(ow, scale_w, g.align_corners, g.W);
+    alignas(16) int8_t v[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = ch * 16 + j;
+      v[j] = 0;
+      if (c >= g.C) continue;
+      const float* img = x + (n * g.C + c) * HW;
+      float f;
+      if (copy) {
+        f = __ldg(img + (int64_t)oh * g.W + ow);
+      } else {
+        const float* r0 = img + (int64_t)th.i0 * g.W;
+        const float* r1 = img + (int64_t)th.i1 * g.W;
+        const float a = __fmaf_rn(tw.l0, __ldg(r0 + tw.i0), __fmul_rn(tw.l1, __ldg(r0 + tw.i1)));
+        const float b = __fmaf_rn(tw.l0, __ldg(r1 + tw.i0), __fmul_rn(tw.l1, __ldg(r1 + tw.i1)));
+        f = __fmaf_rn(th.l0, a, __fmul_rn(th.l1, b));
+      }
+      if (y) y[(n * g.C + c) * OHW + p] = f;
+      v[j] = q8(clamp_keep_nan(f, g.lo, g.hi), g.out_scale);
+    }
+    if (yq)
+      *reinterpret_cast<int4*>(yq + (n * OHW + p) * g.cstride + g.coff + ch * 16) = *reinterpret_cast<const int4*>(v);
+  }
+}
+
+// torch's area_pixel_compute_scale<float> without a scale_factor, formed on the host as torch forms it
+inline float bilinear_scale(int in, int out, bool align_corners) {
+  if (align_corners) return out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f;
+  return (float)in / (float)out;
+}
+
 inline bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 
 // [a, a + na) and [b, b + nb) share a byte; a NULL range shares none
@@ -721,6 +795,38 @@ extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t
                 "dfq_i8_maxpool: x, y and yq overlap");
     k_i8_maxpool<false><<<grid_for(total, 256), 256, 0, st>>>(nullptr, x, y, yq, out_scale, *g, total);
   }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_upsample_bilinear(const float* x, float* y, int8_t* yq, const DfqI8Resize* g, void* stream) {
+  DFQ_REQUIRE(g != nullptr, "dfq_i8_upsample_bilinear: null geometry");
+  DFQ_REQUIRE(x != nullptr, "dfq_i8_upsample_bilinear: null input");
+  DFQ_REQUIRE(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->OH > 0 && g->OW > 0,
+              "dfq_i8_upsample_bilinear: empty dimension (every size must be positive)");
+  DFQ_REQUIRE(g->align_corners == 0 || g->align_corners == 1, "dfq_i8_upsample_bilinear: align_corners must be 0 or 1");
+  const int cpad = (g->C + 15) / 16 * 16;
+  DFQ_REQUIRE(g->coff >= 0 && g->cstride > 0 && g->coff % 16 == 0 && g->cstride % 16 == 0,
+              "dfq_i8_upsample_bilinear: coff and cstride must be non-negative multiples of 16");
+  DFQ_REQUIRE((int64_t)g->coff + cpad <= g->cstride,
+              "dfq_i8_upsample_bilinear: the slice coff + round_up(C, 16) exceeds cstride");
+  DFQ_REQUIRE(y || yq, "dfq_i8_upsample_bilinear: no output requested (y and yq are both NULL)");
+  DFQ_REQUIRE(aligned16(yq), "dfq_i8_upsample_bilinear: yq must be 16-byte aligned");
+  DFQ_REQUIRE(((uintptr_t)x & 3) == 0 && ((uintptr_t)y & 3) == 0, "dfq_i8_upsample_bilinear: x and y must be 4-byte aligned");
+  DFQ_REQUIRE(!yq || (std::isfinite(g->out_scale) && g->out_scale >= 0.f),
+              "dfq_i8_upsample_bilinear: out_scale must be finite and non-negative when yq is written");
+  DFQ_REQUIRE(ordered(g->lo, g->hi), "dfq_i8_upsample_bilinear: clamp bounds must be ordered and not NaN");
+  const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
+  const int64_t x_bytes = in_px * g->C * 4, y_bytes = out_px * g->C * 4;
+  const int8_t* slice = yq ? yq + g->coff : nullptr;
+  const int64_t slice_bytes = (out_px - 1) * g->cstride + cpad;       // first to last byte the slice's chunks cover
+  DFQ_REQUIRE(!overlap(x, x_bytes, y, y_bytes) && !overlap(x, x_bytes, slice, slice_bytes),
+              "dfq_i8_upsample_bilinear: x overlaps y or the slice");
+  DFQ_REQUIRE(!overlap(y, y_bytes, slice, slice_bytes), "dfq_i8_upsample_bilinear: y overlaps the slice");
+  const int64_t total = out_px * (cpad / 16);
+  const bool ac = g->align_corners == 1;
+  k_i8_upsample_bilinear<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      x, y, yq, *g, bilinear_scale(g->H, g->OH, ac), bilinear_scale(g->W, g->OW, ac), total);
   DFQ_CUDA(cudaGetLastError());
   return 0;
 }

@@ -479,6 +479,7 @@ extern "C" int dfq_struct_size(int which) {
     case 8: return (int)sizeof(DfqI8Conv);
     case 9: return (int)sizeof(DfqI8Epilogue);
     case 10: return (int)sizeof(DfqI8Pool);
+    case 11: return (int)sizeof(DfqI8Resize);
     default: return -1;
   }
 }

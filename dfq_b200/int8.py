@@ -366,6 +366,63 @@ class Int8MaxPool2d(nn.Module):
             "codes" if self.codes_in else "fp32 in, out_scale=%s, fp32=%s" % (self.out_scale, self.fp32))
 
 
+class Int8UpsampleBilinear(nn.Module):
+    """F.interpolate(x, size, mode='bilinear', align_corners=...) of a chained model (dfq_i8_upsample_bilinear): fp32 NCHW
+    [N, channels, H, W] in, the codes q(clamp(y, *clamp), out_scale) of torch's bilinear output y out - int8 NHWC
+    [N, OH, OW, round_up(channels, 16)], or with out_slice = (coff, cstride) channels [coff, coff + round_up(channels, 16))
+    of `out` (int8 [N, OH, OW, cstride], made when None).  The size comes at run time (often a traced value such as
+    x.shape[-2:]) and must be a pair of positive ints."""
+
+    def __init__(self, channels, align_corners, out_scale, clamp=(-float("inf"), float("inf")), out_slice=None, name=None):
+        super().__init__()
+        self.channels, self.align_corners, self.layer_name = int(channels), bool(align_corners), name
+        self.cpad = (self.channels + 15) // 16 * 16
+        check_scale("output", out_scale, "bilinear upsample %s" % name)
+        self.out_scale = float(_f32(out_scale))
+        self.clamp = _ordered(*clamp, what="upsample %s clamp" % name)
+        if out_slice is not None:
+            coff, cstride = (int(v) for v in out_slice)
+            if coff < 0 or coff % 16 or cstride % 16 or coff + self.cpad > cstride:
+                raise _lib.DfqError("bilinear upsample %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
+                                    % (name, coff, cstride))
+            out_slice = (coff, cstride)
+        self.out_slice = out_slice
+
+    def forward(self, x, size, out=None):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise _lib.DfqError("int8 bilinear upsample %s runs on the GPU only (no CPU fallback)" % self.layer_name)
+        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.channels:
+            raise _lib.DfqError("int8 bilinear upsample %s expects fp32 [N, %d, H, W], got %s %s"
+                                % (self.layer_name, self.channels, x.dtype, tuple(x.shape)))
+        if not isinstance(size, (tuple, list)) or len(size) != 2 or \
+                not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in size):
+            raise _lib.DfqError("int8 bilinear upsample %s: size must be a pair of positive ints, got %r"
+                                % (self.layer_name, size))
+        N, _, H, W = x.shape
+        OH, OW = int(size[0]), int(size[1])
+        coff, cstride = self.out_slice or (0, self.cpad)
+        shape = (N, OH, OW, cstride)
+        if out is not None and self.out_slice is None:
+            raise _lib.DfqError("bilinear upsample %s: takes no output tensor" % self.layer_name)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.int8, device=x.device)
+        elif not isinstance(out, torch.Tensor) or out.dtype != torch.int8 or tuple(out.shape) != shape or \
+                out.device != x.device or not out.is_contiguous():
+            raise _lib.DfqError("bilinear upsample %s: the concatenation's codes must be contiguous int8 %s on %s, got %s" % (
+                self.layer_name, list(shape), x.device, "%s %s on %s" % (out.dtype, list(out.shape), out.device)
+                if isinstance(out, torch.Tensor) else type(out).__name__))
+        x = x.contiguous()
+        g = np.zeros(1, _lib.I8_RESIZE_DT)
+        g[0] = (N, self.channels, H, W, OH, OW, int(self.align_corners), coff, cstride, self.out_scale) + self.clamp
+        _lib.check(_lib.load().dfq_i8_upsample_bilinear(_ptr(x), None, _ptr(out), _lib.table_ptr(g), _lib.stream_ptr()),
+                   "dfq_i8_upsample_bilinear (%s)" % self.layer_name)
+        return out
+
+    def extra_repr(self):
+        return "channels=%d, align_corners=%s, out_scale=%g, clamp=%s, out_slice=%s" % (
+            self.channels, self.align_corners, self.out_scale, self.clamp, self.out_slice)
+
+
 def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
     """Replace every target layer of `graph` (types in targ_type, Conv2d or Linear) inside `model` by its int8 executor, in
     place (by parent attribute); returns the replaced modules' names in graph order.
@@ -510,6 +567,47 @@ def _max_pool(node, mods):
     return None
 
 
+def _bilinear_upsample(node, mods):
+    """(size, align_corners) of an F.interpolate / nn.Upsample node that resizes one fx node bilinearly to a given size:
+    mode 'bilinear', size a pair of ints or a traced value, align_corners True or False, no scale_factor,
+    recompute_scale_factor or antialias; None otherwise."""
+    if not node.args or not isinstance(node.args[0], fx.Node):
+        return None
+    if node.op == "call_module" and type(mods[node.target]) is nn.Upsample:
+        m = mods[node.target]
+        if len(node.args) != 1 or node.kwargs:
+            return None
+        size, sf, mode, ac, rsf, aa = m.size, m.scale_factor, m.mode, m.align_corners, m.recompute_scale_factor, False
+    elif node.op == "call_function" and node.target is F.interpolate:
+        size, sf, mode, ac, rsf, aa = (_arg(node, i, k, d) for i, k, d in (
+            (1, "size", None), (2, "scale_factor", None), (3, "mode", "nearest"), (4, "align_corners", None),
+            (5, "recompute_scale_factor", None), (6, "antialias", False)))
+    else:
+        return None
+    if mode != "bilinear" or sf is not None or rsf is not None or aa is not False or (ac is not True and ac is not False):
+        return None
+    if not isinstance(size, fx.Node) and not (isinstance(size, (tuple, list)) and len(size) == 2 and all(
+            isinstance(v, fx.Node) or (isinstance(v, int) and not isinstance(v, bool)) for v in size)):
+        return None
+    return size, ac
+
+
+def _shape_query(u, node):
+    """True when u only reads node's shape: node.size(), node.size(d), node.shape or node.dim()."""
+    if not u.args or u.args[0] is not node or u.kwargs:
+        return False
+    if u.op == "call_method" and u.target in ("size", "dim"):
+        return all(not isinstance(a, fx.Node) for a in u.args[1:])
+    return u.op == "call_function" and u.target is getattr and len(u.args) == 2 and u.args[1] == "shape"
+
+
+def _nchw_view(codes, channels):
+    """A tensor of the shape [N, channels, H, W] of the fp32 tensor whose codes `codes` [N, H, W, *] carry, for the shape
+    queries on a fused concatenation's operand (sizes taken as `x4.size()[2:]`): a zero-stride view, nothing allocated."""
+    N, H, W = codes.shape[:3]
+    return codes.as_strided((N, channels, H, W), (0, 0, 0, 0))
+
+
 def _cat_operands(node):
     """The operands of torch.cat / torch.concat along the channels (dim 1 or -3) of >= 2 distinct fx nodes, without out;
     None otherwise."""
@@ -522,7 +620,7 @@ def _cat_operands(node):
     return list(ops)
 
 
-def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False) -> fx.GraphModule:
+def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False, upsample=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` computes, with activations kept in int8 between converted
     convolutions.
 
@@ -573,7 +671,26 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
       cat and its pass-throughs are deleted.  Any other cat stays in torch, fp32.
     Edges whose codes come through a fused pool or cat name that node (its traced name) as the producer.  `fused_cats`
     records (cat node name, producer names, channel offsets) and `fused_pools` (pool node name, "codes" or "fp32", the
-    outputs it writes), in graph order.  pool_cat=True without residual=True raises DfqError."""
+    outputs it writes), in graph order.  pool_cat=True without residual=True raises DfqError.
+
+    upsample=True (with pool_cat=True) also carries codes out of bilinear upsampling, bit-identical to the per-layer path
+    (no exceptions: the codes are those of torch's fp32 output):
+    - the node: F.interpolate / nn.Upsample with mode='bilinear', size given (constant or traced, e.g. x.shape[-2:]; checked
+      to be a pair of positive ints when the module runs), align_corners True or False, and no scale_factor, antialias or
+      recompute_scale_factor, whose input is the end of an Int8Conv2d producer's single-user pass-through chain.  The
+      producer writes its clamped fp32 output (dfq_i8_conv_fused, fp32 only; other fp32 users of a fan-out take the same
+      tensor), and the upsample (Int8UpsampleBilinear, dfq_i8_upsample_bilinear) writes the codes of torch's output after
+      the clamp of its single-user pass-throughs (deleted), when either
+      (a) it is, through them, an operand of a concatenation: the concatenation rule accepts it in place of a producer, and
+          it writes its slice at the consumers' scale, with the cat tail's clamp composed in.  With upsample=True a user
+          that only reads a cat operand's shape (x4.size()[2:], .shape, .size(d), .dim(), on any node of the operand's
+          chain - where DeepLab-v3+ reads its upsample sizes) does not count as a second user: it reads the shape of a
+          zero-stride view of the slice's writer's output instead (_nchw_view); or
+      (b) every user takes codes: Int8Conv2d consumers (single-site, channels matching) at one act_scale, bit for bit.
+    Any other upsample stays in torch, fp32, as does anything not listed (nearest or bicubic modes, scale_factor,
+    adaptive average pools).  `fused_upsamples` records (node name, producer name, "slice" or "codes", align_corners) in
+    graph order; edges whose codes come out of a fused upsample name it as the producer.  upsample=True without
+    pool_cat=True raises DfqError."""
     tracer = _Int8Tracer()
     graph = tracer.trace(model, concrete_args)
     gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
@@ -588,8 +705,10 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
 
     if pool_cat and not residual:
         raise _lib.DfqError("chain_int8: pool_cat=True builds on residual=True")
+    if upsample and not pool_cat:
+        raise _lib.DfqError("chain_int8: upsample=True builds on pool_cat=True")
     if residual:
-        return _chain_residual(gm, mods, conv, pool_cat)
+        return _chain_residual(gm, mods, conv, pool_cat, upsample)
 
     edges, between = [], []
     for q in list(gm.graph.nodes):
@@ -629,8 +748,8 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     return gm
 
 
-def _chain_residual(gm, mods, conv, pool_cat=False):
-    """chain_int8(..., residual=True[, pool_cat=True]) on the traced `gm` (see chain_int8)."""
+def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
+    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) on the traced `gm` (see chain_int8)."""
     full = (-_INF, _INF)
     order = {n: i for i, n in enumerate(gm.graph.nodes)}
 
@@ -649,16 +768,41 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
             path.append(u)
         return node, clamp, path
 
-    def back_to_producer(node):
-        """The producer whose single-user pass-through chain ends at `node`, or None."""
-        while len(node.users) == 1 and not producer(node):
+    def data_users(node, queries):
+        """node's users, without those that only read its shape when `queries`."""
+        return [u for u in node.users if not (queries and _shape_query(u, node))]
+
+    def back_to_producer(node, queries=False):
+        """The producer whose single-user pass-through chain ends at `node`, or None.  queries: users that only read a
+        node's shape do not count."""
+        while len(data_users(node, queries)) == 1 and not producer(node):
             if _pass_through(node, mods) is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
                 return None
             node = node.args[0]
-        return node if len(node.users) == 1 and producer(node) else None
+        return node if len(data_users(node, queries)) == 1 and producer(node) else None
 
     def same(a, b):
         return a.view(np.int32) == b.view(np.int32)
+
+    # bilinear upsamples: the producer whose single-user pass-through chain ends at the upsample's input
+    ends = {forward(p, full)[0]: p for p in gm.graph.nodes if producer(p)} if upsample else {}
+
+    sources = {}
+
+    def up_source(node):
+        """The producer of a fusable bilinear upsample node, or None (as the traced graph has it: memoized before the
+        rewrites)."""
+        if node not in sources:
+            sources[node] = ends.get(node.args[0]) if ends and _bilinear_upsample(node, mods) is not None else None
+        return sources[node]
+
+    def back_to_upsample(node):
+        """The fusable upsample whose single-user pass-through chain ends at `node` (shape queries not counted), or None."""
+        while len(data_users(node, True)) == 1 and up_source(node) is None:
+            if _pass_through(node, mods) is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
+                return None
+            node = node.args[0]
+        return node if len(data_users(node, True)) == 1 and up_source(node) is not None else None
 
     def after_pool(node):
         """Walk from a pool through single-user exact identities: (last node, the identities)."""
@@ -750,10 +894,10 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
         ops = _cat_operands(c)
         if ops is None:
             continue
-        prods = [back_to_producer(o) for o in ops]
+        prods = [back_to_producer(o, upsample) or (back_to_upsample(o) if upsample else None) for o in ops]
         if any(q is None for q in prods) or len(set(prods)) != len(prods):
             continue
-        chans = [mods[q.target].out_channels for q in prods]
+        chans = [mods[(up_source(q) or q).target].out_channels for q in prods]
         if any(k % 16 for k in chans[:-1]):
             continue
         tail, tclamp, tpath = forward(c, full)
@@ -761,18 +905,40 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
         if not codes or len(codes) != len(tail.users):
             continue
         operands = []
-        for o, q, off in zip(ops, prods, np.cumsum([0] + chans[:-1]).tolist()):
+        for o, q, k, off in zip(ops, prods, chans, np.cumsum([0] + chans[:-1]).tolist()):
             node, clamp, opath = o, full, []
             while node is not q:
                 clamp = _compose(_pass_through(node, mods), clamp)
                 opath.append(node)
                 node = node.args[0]
-            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), coff=off))
+            queries = [(u, n) for n in (q, *opath) for u in n.users if upsample and _shape_query(u, n)]
+            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), coff=off, channels=k, queries=queries))
         cat_plans.append(dict(cat=c, operands=operands, tail=tail, path=tpath, codes=codes, scale=scale, clamp=tclamp,
                               cstride=(sum(chans) + 15) // 16 * 16))
         for u in codes:
             if not producer(u):
                 codes_pool(u, sum(chans), tclamp)
+
+    # upsamples: slice mode through a fused concatenation above, codes mode when every user takes codes at one scale;
+    # either way the producer writes its clamped fp32 output
+    up_plans = [dict(node=o["p"], mode="slice") for cp in cat_plans for o in cp["operands"] if not producer(o["p"])]
+    sliced = {up["node"] for up in up_plans}
+    for u in (list(gm.graph.nodes) if upsample else []):
+        if u in sliced or up_source(u) is None:
+            continue
+        utail, uclamp, upath = forward(u, full)
+        codes, scale = take_codes(utail, mods[up_source(u).target].out_channels, pools=False)
+        if codes and len(codes) == len(utail.users):
+            up_plans.append(dict(node=u, mode="codes", tail=utail, clamp=uclamp, path=upath, codes=codes, scale=scale))
+    planned = {pl["p"] for pl in plans}
+    for up in up_plans:
+        p = up_source(up["node"])
+        if p not in planned:
+            end, pre, path = forward(p, full)
+            plans.append(dict(p=p, path=path, pre=pre, add=None, ri=None, post=full, post_path=[], tail=end, codes=[],
+                              scale=None))
+            planned.add(p)
+    plans.sort(key=lambda pl: order[pl["p"]])
 
     # the residual's exact identities, skipped once every plan's own nodes are known: a node another plan deletes (an
     # identity at the end of its post-add chain, say) stays the residual, and that plan replaces it by its fp32 output
@@ -780,6 +946,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
                                             *pl["post_path"])}
     claimed |= {n for cp in cat_plans for n in (cp["cat"], *cp["path"], *(n for o in cp["operands"] for n in (o["p"], *o["path"])))}
     claimed |= {n for pp in pool_plans for n in (pp["node"], *pp.get("path", []))}
+    claimed |= {n for up in up_plans for n in (up["node"], *up.get("path", []))}
     for pl in plans:
         pl["skipped"] = []
         if pl["add"] is None:
@@ -829,12 +996,26 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
         if add is not None:
             adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
 
+    def fuse_upsample(u, scale, clamp, out_slice=None, out=None):
+        """Turn the upsample node u into a call of its Int8UpsampleBilinear, on its (rewritten) input."""
+        (size, ac), p = _bilinear_upsample(u, mods), up_source(u)
+        mod = Int8UpsampleBilinear(mods[p.target].out_channels, ac, float(scale), clamp, out_slice, name=u.name)
+        name = "int8_up_" + u.name
+        gm.add_submodule(name, mod)
+        ups.append((order[u], (u.name, p.target, "slice" if out_slice else "codes", ac)))
+        u.op, u.target, u.args, u.kwargs = "call_module", name, (u.args[0], size), ({} if out is None else {"out": out})
+
     # concatenations: the producers write their slices of one buffer in graph order, threaded through `out`
-    cats = []
+    cats, ups = [], []
     for cp in cat_plans:
         cstride, prev = cp["cstride"], None
+        names = [o["p"].target if producer(o["p"]) else o["p"].name for o in cp["operands"]]
         for o in sorted(cp["operands"], key=lambda o: order[o["p"]]):
             q = o["p"]
+            if not producer(q):
+                fuse_upsample(q, cp["scale"], o["clamp"], (o["coff"], cstride), prev)
+                prev = q
+                continue
             modes[q.target] = ("slice", ((float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride)))
             if prev is not None:
                 q.kwargs = {"out": prev}
@@ -847,9 +1028,25 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
             g.erase_node(node)
         g.erase_node(cp["cat"])
         for o in cp["operands"]:
+            for u, n in o["queries"]:                           # shape queries read the shape off the slice's writer
+                with g.inserting_before(u):
+                    u.replace_input_with(n, g.call_function(_nchw_view, (o["p"], o["channels"])))
             for node in o["path"]:                              # from the cat back to the producer
                 g.erase_node(node)
-        cats.append((cp["cat"].name, [o["p"].target for o in cp["operands"]], [o["coff"] for o in cp["operands"]]))
+        cats.append((cp["cat"].name, names, [o["coff"] for o in cp["operands"]]))
+
+    # upsamples whose users all take their codes
+    for up in up_plans:
+        if up["mode"] != "codes":
+            continue
+        u = up["node"]
+        fuse_upsample(u, up["scale"], up["clamp"])
+        for v in up["codes"]:
+            v.replace_input_with(up["tail"], u)
+            edges.append((u.name, v.target, up["clamp"]))
+        for node in reversed(up["path"]):
+            g.erase_node(node)
+    ups = [t for _, t in sorted(ups)]
 
     # pools, last: each reads its input as the rewrites above left it
     pools = []
@@ -898,4 +1095,6 @@ def _chain_residual(gm, mods, conv, pool_cat=False):
     if pool_cat:
         gm.fused_cats = cats
         gm.fused_pools = pools
+    if upsample:
+        gm.fused_upsamples = ups
     return gm

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 6
+#define DFQ_ABI_VERSION 7
 
 enum {
   DFQ_OK = 0,
@@ -43,7 +43,8 @@ enum {
 int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
- * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue): lets a binding verify
+ * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
+ * 11 DfqI8Resize): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -444,6 +445,26 @@ typedef struct DfqI8Pool {
  * an out_scale that is not finite and non-negative while yq is written in fp32 mode, overlapping input and outputs. */
 int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, float out_scale, const DfqI8Pool* g,
                    void* stream);
+
+/* Bilinear resize to a given size (F.interpolate(x, size=(OH, OW), mode='bilinear', align_corners=...)). */
+typedef struct DfqI8Resize {
+  int32_t N, C, H, W;          /* fp32 NCHW input                                                                 */
+  int32_t OH, OW;              /* output size (the `size=` of F.interpolate)                                      */
+  int32_t align_corners;       /* 0 or 1                                                                          */
+  int32_t coff, cstride;       /* codes go to channels [coff, coff + round_up(C, 16)) of int8 NHWC [N, OH, OW, cstride] */
+  float out_scale, lo, hi;     /* q(clamp(v, lo, hi), out_scale); (-inf, +inf): no clamp                          */
+} DfqI8Resize;
+/* x fp32 NCHW [N, C, H, W] -> y fp32 NCHW [N, C, OH, OW] (NULL: not written), bit for bit torch's CUDA upsample_bilinear2d
+ * of a contiguous NCHW fp32 tensor with no scale_factor: per axis scale = align_corners ? (in - 1) / (out - 1) (0 when
+ * out == 1) : in / out in fp32, source index scale * dst or max(scale * (dst + 0.5) - 0.5, 0) with torch's fused
+ * multiply-adds, and a plain copy when the size does not change; and / or yq[m * cstride + coff + c] =
+ * q(clamp(y, lo, hi), out_scale) (NULL: not written), the clamp keeping NaN.  The codes are those of the fp32 value, so
+ * NaN, +-inf, -0.0 and subnormal inputs give what the per-layer path gives.  Pad channels C .. round_up(C, 16) of the slice
+ * are written 0 and nothing outside the slice.  DFQ_E_ARG, with a reason: a non-positive size, align_corners not 0 / 1,
+ * coff or cstride not a multiple of 16 or the slice not inside cstride, no output, yq not 16-byte aligned or x / y not
+ * 4-byte aligned, an out_scale that is not finite and non-negative while yq is written, NaN or unordered bounds, x
+ * overlapping y or the slice, y overlapping the slice. */
+int dfq_i8_upsample_bilinear(const float* x, float* y, int8_t* yq, const DfqI8Resize* g, void* stream);
 
 #ifdef __cplusplus
 }

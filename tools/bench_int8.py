@@ -10,7 +10,10 @@ convolutions) on the same nets with BN folded - images/s, fused edges, fp32 byte
 `residual`: per-layer against chain_int8 and chain_int8(residual=True) (residual adds and tensors with several consumers
 fused too), the same way, with the fused adds.  `pool_cat`: per-layer against chain_int8(residual=True) and
 chain_int8(residual=True, pool_cat=True) (max pools and channel concatenations carried in int8 too) on ResNet-18, SqueezeNet
-1.1 and GoogLeNet.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
+1.1 and GoogLeNet.  `upsample`: per-layer against chain_int8(residual=True, pool_cat=True) and chain_int8(..., upsample=True)
+(bilinear upsamples feeding concatenations carried in int8 too) on two segmentation networks at 513x513: the DeepLab-v3+-shaped
+network of tests/deeplab_v3plus_like.py and torchvision's DeepLab-v3 ResNet-50.  The card's name and power limit are read in
+the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
 """
 import argparse
 import json
@@ -381,6 +384,104 @@ def pool_cat_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def upsample_inference(dev, reps=10, batch=8, rounds=5, size=513):
+    """Per-layer int8 execution against chain_int8(residual=True, pool_cat=True) and chain_int8(..., upsample=True) on the
+    DeepLab-v3+-shaped network of tests/deeplab_v3plus_like.py and torchvision's deeplabv3_resnet50 (seeded weights, BN
+    folded, scales 128 / max|input|), `batch` images of size x size, timed alternately (`rounds` rounds of `reps` passes,
+    median): images/s, ms per batch, fused cats and upsamples, carried convolution inputs, the fp32 bytes the upsample arm
+    avoids against the pool_cat arm (from the traced tensors' sizes) and bit-identity of the output."""
+    import statistics
+    from collections import OrderedDict
+    import torch
+    import torch.nn as nn
+    import torchvision
+    from dfq_b200 import int8
+    from dfq_b200.trace import trace_graph
+    from dfq_b200.utils.layer_transform import merge_batchnorm
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from deeplab_v3plus_like import DeepLabV3PlusLike
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def out_of(t):
+        return t["out"] if isinstance(t, dict) else t
+
+    out = {"batch": batch, "image": "3x%dx%d" % (size, size), "unit": "images/s", "reps": reps, "rounds": rounds,
+           "fp32_bytes_avoided_note": "fp32 bytes the pool_cat arm moves that the upsample arm does not, per batch, from the "
+                                      "traced tensors' sizes: per deleted node a read and a write of its output (cat: of its "
+                                      "output twice), per fused upsample its fp32 output's write, per carried consumer of a "
+                                      "fused cat or upsample the quantizer's read"}
+    x = torch.randn(batch, 3, size, size, device=dev)
+    for net in ("deeplab_v3plus_like", "deeplabv3_resnet50"):
+        torch.manual_seed(0)
+        model = (DeepLabV3PlusLike(num_classes=21) if net == "deeplab_v3plus_like" else
+                 torchvision.models.segmentation.deeplabv3_resnet50(weights=None, weights_backbone=None, aux_loss=False))
+        model = model.to(dev).eval()
+        graph, bottoms = trace_graph(model)
+        merge_batchnorm(model, graph, bottoms, [nn.Conv2d])
+        layers = OrderedDict((n, m) for n, m in model.named_modules() if type(m) in (nn.Conv2d, nn.Linear))
+        amax = {}
+        hooks = [m.register_forward_pre_hook(lambda m, i, n=n: amax.__setitem__(n, max(amax.get(n, 0.0), float(i[0].abs().max()))))
+                 for n, m in layers.items()]
+        with torch.no_grad():
+            model(x[:2])
+        for h in hooks:
+            h.remove()
+        int8.convert_to_int8(model, OrderedDict((id(m), m) for m in layers.values()), [nn.Conv2d, nn.Linear],
+                             act_scales=[128. / amax[n] for n in layers])
+        base = int8.chain_int8(model, residual=True, pool_cat=True)
+        gm = int8.chain_int8(model, residual=True, pool_cat=True, upsample=True)
+        traced = torch.fx.GraphModule(model, int8._Int8Tracer().trace(model))
+        nbytes = {}
+        interp = torch.fx.Interpreter(traced)
+        run_node = interp.run_node
+
+        def record(n):
+            v = run_node(n)
+            if isinstance(v, torch.Tensor):
+                nbytes[n.name] = v.numel() * 4
+            return v
+        interp.run_node = record
+        with torch.no_grad():
+            interp.run(x)
+            kept_base, kept = {n.name for n in base.graph.nodes}, {n.name for n in gm.graph.nodes}
+            avoided = sum(2 * nbytes.get(n, 0) for n in kept_base - kept)
+            avoided += sum(2 * nbytes.get(c[0], 0) for c in gm.fused_cats)
+            avoided += sum(nbytes.get(u[0], 0) for u in gm.fused_upsamples)
+            avoided += sum(nbytes.get(p, 0) for p, q, _ in gm.requantized_edges
+                           if q not in {e[1] for e in base.requantized_edges})
+            del interp, nbytes
+            ref = out_of(model(x))
+            got = {"pool_cat": out_of(base(x)), "upsample": out_of(gm(x))}
+            for _ in range(2):
+                model(x), base(x), gm(x)
+            torch.cuda.synchronize(dev)
+            ms = {"per_layer": [], "pool_cat": [], "upsample": []}
+            for _ in range(rounds):
+                ms["per_layer"].append(timed(lambda: model(x)))
+                ms["pool_cat"].append(timed(lambda: base(x)))
+                ms["upsample"].append(timed(lambda: gm(x)))
+        med = {k: statistics.median(v) for k, v in ms.items()}
+        out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                    "ms_per_batch_rounds": ms, "fused_cats": len(gm.fused_cats),
+                    "fused_upsamples": [u[:3] for u in gm.fused_upsamples],
+                    "carried_conv_inputs": {"pool_cat": len({e[1] for e in base.requantized_edges}),
+                                            "upsample": len({e[1] for e in gm.requantized_edges}),
+                                            "convolutions": sum(isinstance(m, int8.Int8Conv2d) for m in model.modules())},
+                    "fp32_bytes_avoided_per_batch_vs_pool_cat": avoided,
+                    "output_bit_identical": {k: bool(torch.equal(ref.view(torch.int32), v.view(torch.int32)))
+                                             for k, v in got.items()}}
+        del model, base, gm, ref, got
+        torch.cuda.empty_cache()
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -399,15 +500,24 @@ def main():
     p = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     p.add_argument("--batch", type=int, default=256)
     p.add_argument("--reps", type=int, default=10, help="timed forward passes per arm (after 2 warm-up passes)")
+    p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample)")
+    p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample",
+                   help="comma-separated sections to run (default: all)")
     args = p.parse_args()
+    want = set(args.sections.split(","))
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_int8.py needs a CUDA device (H100)")
     dev = torch.device("cuda", 0)
-    res = int8_inference(dev, reps=args.reps, batch=args.batch)
-    res["chained"] = chained_inference(dev, reps=args.reps, batch=args.batch)
-    res["residual"] = residual_inference(dev, reps=args.reps, batch=args.batch)
-    res["pool_cat"] = pool_cat_inference(dev, reps=args.reps, batch=args.batch)
+    res = int8_inference(dev, reps=args.reps, batch=args.batch) if "int8" in want else {}
+    if "chained" in want:
+        res["chained"] = chained_inference(dev, reps=args.reps, batch=args.batch)
+    if "residual" in want:
+        res["residual"] = residual_inference(dev, reps=args.reps, batch=args.batch)
+    if "pool_cat" in want:
+        res["pool_cat"] = pool_cat_inference(dev, reps=args.reps, batch=args.batch)
+    if "upsample" in want:
+        res["upsample"] = upsample_inference(dev, reps=args.reps, batch=args.seg_batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
