@@ -24,6 +24,7 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <type_traits>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -74,10 +75,14 @@ struct GroupState {
   int n_sweeps;
   int done;
   int converged;
+  double fuse_lb;  // k_cle_stack's fused pass: lower bound of sweep 1's metric (fuse_guard_scan)
+  int fuse_moves;  // ... some channel has s2 != 1 or inv2 != 1
 };
 struct CleCtl {
   int active[2];   // groups still iterating, double-buffered by sweep parity
   double diffs[64];  // diff_tmp per sweep of group 0
+  int fuse_refused;  // k_cle_stack: the guard sent the launch down the per-sweep path
+  int fused_sweeps;  // DfqCleResult.fused_sweeps
 };
 
 // One sweep of the exit rule of dfq.py:105-115 for one group: folds this sweep's metric `diff_tmp` into `diff` / `count`
@@ -1189,6 +1194,130 @@ __device__ __forceinline__ float stack_scale_row(uint32_t a0, int n4, const DfqC
   return dsum;
 }
 
+// ---- the first two sweeps in one pass ------------------------------------------------------------------------------
+// A two-layer chain's scale of channel c depends on four numbers only: the extrema of row c of the first layer and of
+// column c of the second.  Rounding is monotone, so for s > 0  max_i fl(v_i * s) = fl(max_i(v_i) * s)  (likewise min): after
+// sweep 1 the row extrema are fl(mn * s1), fl(mx * s1) and the column extrema fl(cmn * inv1), fl(cmx * inv1) (the rule the
+// derived column extrema already rest on).  With the row extrema of the folded weights from the fold's scan
+// (DFQ_LAYER_ROWS_READY), s1, inv1, s2, inv2 of every channel are known before any weight is read, and one pass applies
+// both sweeps: t1 = fl(v * s1), t2 = fl(t1 * s2) - the very values, metric terms included, of two passes.
+// Sweep 2 must then be one the per-sweep run makes too, for every group: see fuse_guard.
+struct FuseScales { float s1, inv1, s2, inv2; };
+__device__ __forceinline__ FuseScales fuse_scales(const DfqCleParams& P, float rmn, float rmx, float cmn, float cmx) {
+  FuseScales f;
+  RowIn in;
+  in.cmn = cmn; in.cmx = cmx;
+  f.s1 = solve_row(P, in, rmn, rmx, &f.inv1);
+  in.cmn = __fmul_rn(cmn, f.inv1); in.cmx = __fmul_rn(cmx, f.inv1);     // publish_row's derived column extrema
+  f.s2 = solve_row(P, in, __fmul_rn(rmn, f.s1), __fmul_rn(rmx, f.s1), &f.inv2);
+  return f;
+}
+
+// A lower bound of one channel's term of sweep 1's metric sum |fl(fl(v*s) - v)|: the element of largest magnitude m alone
+// contributes at least |m| (|s - 1| - 2^-24 s) - 2^-149 (the rounding of the product, absolute below the normal range).
+// 0 when m is not finite (its own term is then inf or NaN - the exit rule goes on after a NaN metric as well).
+__device__ __forceinline__ double fuse_term_bound(float mn, float mx, float s) {
+  const double m = fmax(fabs((double)mn), fabs((double)mx)), sd = (double)s;
+  const double t = m * (fabs(sd - 1.0) - 0x1p-24 * sd) - 0x1p-149;
+  return (t > 0.0 && t < 1e300) ? t : 0.0;
+}
+
+// Phase 1 of the guard, a CTA per first layer: per group the lower bound of sweep 1's metric (GroupState.fuse_lb) and whether
+// any channel has s2 != 1 or inv2 != 1 (.fuse_moves); a launch-wide refusal when some s1 is not finite and > 0 (the
+// monotonicity needs s1 > 0; only a user-set s_range can break it).
+__device__ __noinline__ void fuse_guard_scan(const float* arena, const DfqLayer* L, const DfqRelation* R, const int* step_ptr,
+                                             const int* step_layers, const DfqCleParams P, CleCtl* ctl, GroupState* G) {
+  const int lane = threadIdx.x & 31;
+  for (int q = step_ptr[0] + blockIdx.x; q < step_ptr[1]; q += gridDim.x) {
+    const DfqLayer l = L[step_layers[q]];
+    const DfqRelation r = R[l.rel_out];
+    const DfqLayer l2 = L[r.second];
+    const double n1 = (double)l.rows * l.cols * l.kk, n2 = (double)l2.rows * l2.cols * l2.kk;
+    double lb = 0.0;
+    bool bad = false, moves = false;
+    for (int o = threadIdx.x; o < l.rows; o += blockDim.x) {
+      const float rmn = __ldcg(arena + l.rext_off + o), rmx = __ldcg(arena + l.rext_off + l.rows + o);
+      const float cmn = __ldcg(arena + l2.cmin_off + o), cmx = __ldcg(arena + l2.cmax_off + o);
+      const FuseScales f = fuse_scales(P, rmn, rmx, cmn, cmx);
+      bad |= !(f.s1 > 0.f && f.s1 < DFQ_INF);
+      moves |= (f.s2 != 1.f || f.inv2 != 1.f);
+      lb += fuse_term_bound(rmn, rmx, f.s1) / n1 + fuse_term_bound(cmn, cmx, f.inv1) / n2;
+    }
+    lb = warp_sum(lb);
+    bad = __any_sync(0xffffffffu, bad);
+    moves = __any_sync(0xffffffffu, moves);
+    if (lane == 0) {
+      if (lb > 0.0) atomicAdd(&G[l.group].fuse_lb, lb);
+      if (moves) atomicOr(&G[l.group].fuse_moves, 1);
+      if (bad) atomicOr(&ctl->fuse_refused, 1);
+    }
+  }
+}
+
+// Phase 2: a group may take the fused pass when its sweep 2 is certain, i.e. when
+//   * the lower bound exceeds 2x converge_thres: d1 > converge_thres, so the exit rule goes on after sweep 1 (the factor 2
+//     covers the rounding of the metric's fp32 lane sums, ~1e-4 relative at most), or
+//   * s2 = inv2 = 1 on every channel: sweep 2 changes no bit, so a run that stops after sweep 1 ends in the same state.
+// (The host adds converge_count >= 2 and max_sweeps != 1: the other two ways out after sweep 1.)  Any group that fails
+// sends the whole launch down the per-sweep path.
+__device__ __forceinline__ void fuse_guard_groups(const GroupState* G, int nG, CleCtl* ctl, const DfqCleParams& P) {
+  for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < nG; g += gridDim.x * blockDim.x)
+    if (!(G[g].fuse_lb > 2.0 * P.converge_thres) && G[g].fuse_moves) atomicOr(&ctl->fuse_refused, 1);
+}
+
+// Phase 3 (the guard passed): the per-channel bookkeeping of sweeps 1 and 2 (publish_row twice, in the reference's order:
+// S, bias, BN vectors, s_step / 1/s, both buffers of the derived column extrema), then rext <- (s1, inv1), which the fused
+// pass reads next to s_step = s2 and 1/s = inv2.
+__device__ __noinline__ void fuse_publish(float* arena, const DfqLayer* L, const DfqRelation* R, const int* step_ptr,
+                                          const int* step_layers, const DfqCleParams P) {
+  for (int q = step_ptr[0] + blockIdx.x; q < step_ptr[1]; q += gridDim.x) {
+    const int li = step_layers[q];
+    RowCtx c0, c1;
+    make_ctx(c0, arena, L, R, li, 0);
+    make_ctx(c1, arena, L, R, li, 1);
+    float* rext = arena + L[li].rext_off;
+    for (int o = threadIdx.x; o < c0.rows; o += blockDim.x) {
+      const float rmn = __ldcg(rext + o), rmx = __ldcg(rext + c0.rows + o);
+      const float cmn = __ldcg(c0.cmin_rd + o), cmx = __ldcg(c0.cmax_rd + o);
+      const FuseScales f = fuse_scales(P, rmn, rmx, cmn, cmx);
+      publish_row(c0, P, o, f.s1, f.inv1, cmn, cmx, fetch_row_pub(c0, P, o));
+      publish_row(c1, P, o, f.s2, f.inv2, __fmul_rn(cmn, f.inv1), __fmul_rn(cmx, f.inv1), fetch_row_pub(c1, P, o));
+      __stcg(rext + o, f.s1);
+      __stcg(rext + c0.rows + o, f.inv1);
+    }
+  }
+}
+
+// The fused pass over one first-layer row: v (folded as read) -> t1 = fl(v*s1) -> t2 = fl(t1*s2), stored; d1 / d2: this
+// lane's sums of |t1 - v| and |t2 - t1|, in the order the two per-sweep passes sum them.
+template <bool FOLD>
+__device__ __forceinline__ void stack_fused_row(uint32_t a0, int n4, float fo, float s1, float s2, int lane, float& d1, float& d2) {
+#pragma unroll 4
+  for (int i4 = lane; i4 < n4; i4 += 32) {
+    float4 v = lds_f4(a0 + 16u * i4);
+    if (FOLD) v = mul4(v, fo);
+    const float4 t1 = mul4(v, s1), t2 = mul4(t1, s2);
+    sts_f4(a0 + 16u * i4, t2);
+    d1 += absdiff4(t1, v);
+    d2 += absdiff4(t2, t1);
+  }
+}
+// ... and over one second-layer row, columns scaled by inv1 then inv2 (both cached in shared memory)
+template <int MODE, bool FOLD>
+__device__ __forceinline__ void stack_fused_cols(uint32_t a0, int n4, const float* __restrict__ inv1, const float* __restrict__ inv2,
+                                                 float fo, int lane, float& d1, float& d2) {
+#pragma unroll 4
+  for (int i4 = lane; i4 < n4; i4 += 32) {
+    float4 v = lds_f4(a0 + 16u * i4);
+    if (FOLD) v = mul4(v, fo);
+    const float4 t1 = in_scale4<MODE>(v, i4 * 4, inv1, 1.f, MODE == IN_KK9 ? 9 : 1);
+    const float4 t2 = in_scale4<MODE>(t1, i4 * 4, inv2, 1.f, MODE == IN_KK9 ? 9 : 1);
+    sts_f4(a0 + 16u * i4, t2);
+    d1 += absdiff4(t1, v);
+    d2 += absdiff4(t2, t1);
+  }
+}
+
 // Producer lane: this CTA's tiles of one step (layers of converged groups skipped), SKIP padding, one END per consumer.
 __device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n, float* arena, PassIter it) {
   TileDesc d;
@@ -1201,10 +1330,15 @@ __device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n,
   for (int i = 0; i < kStackConsumers; ++i) bc_produce(ring, n++, d);
 }
 
+// Dynamic shared memory of k_cle_stack: the ring, then kBcConsumers reciprocal caches (BcRing::ex_cache) and kStackConsumers
+// more for the fused pass's second vector (ex_cache(kBcConsumers + warp)).
+constexpr size_t kStackSmemBytes = BcRing::smem_bytes() + (size_t)kStackConsumers * (kBcExCols + 4) * 4;
+
+// fuse: the host found every first layer DFQ_LAYER_ROWS_READY, converge_count >= 2 and max_sweeps != 1; the guard decides.
 __global__ void __launch_bounds__(kBcThreads, 1)
 k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelation* __restrict__ R, int nR,
             const int* __restrict__ step_ptr, const int* __restrict__ step_layers, const long long* __restrict__ pass_ptr,
-            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG) {
+            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG, int fuse) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(128) unsigned char ring_smem[];
   __shared__ RowCtx wctx[kBcConsumers];
@@ -1214,10 +1348,26 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
   const bool producer = (warp == kBcConsumers);
   unsigned long long n = producer ? 0 : (unsigned long long)warp;       // (warps >= kStackConsumers never use it)
   groups_init(G, nG, threadIdx.x, kBcThreads);
+  if (fuse) fuse_guard_scan(arena, L, R, step_ptr, step_layers, P, ctl, G);
   __threadfence();
   grid.sync();
+  bool fused = false;
+  if (fuse) {
+    fuse_guard_groups(G, nG, ctl, P);
+    __threadfence();
+    grid.sync();
+    fused = *((volatile int*)&ctl->fuse_refused) == 0;
+    if (fused) {
+      fuse_publish(arena, L, R, step_ptr, step_layers, P);
+      if (blockIdx.x == 0 && threadIdx.x == 0) ctl->fused_sweeps = 2;
+      __threadfence();
+      grid.sync();
+    }
+  }
 
-  for (int sweep = 0;; ++sweep) {
+  // One pass over the weights: sweep `sweep`, or with FUSED sweeps 0 and 1 (metric terms into acc[0] and acc[1]).
+  auto pass = [&](auto fused_tag, int sweep) {
+    constexpr bool FUSED = decltype(fused_tag)::value;
     const int slot = sweep % 3;
     for (int p = 0; p < 2; ++p) {
       if (producer) {
@@ -1229,14 +1379,20 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
       } else if (warp < kStackConsumers) {
         RowCtx& c = wctx[warp];
         float* inv_s = ring.ex_cache(warp);            // reciprocal scales of the current second layer's columns (+ sentinel)
+        float* inv1_s = ring.ex_cache(kBcConsumers + warp);   // FUSED: those of sweep 1 (inv_s: sweep 2)
+        const float* rext = nullptr;                   // FUSED, first layer: s1 per row (fuse_publish)
         int cur_li = -1, cur_g = -1, kk = 1;
-        double dacc = 0.0;
+        double dacc = 0.0, dacc2 = 0.0;
         auto flush_metric = [&]() {
           if (cur_g >= 0) {
             const double t = warp_sum(dacc);
             if (lane == 0 && t != 0.0) atomicAdd(&G[cur_g].acc[slot], t);
+            if (FUSED) {
+              const double t2 = warp_sum(dacc2);
+              if (lane == 0 && t2 != 0.0) atomicAdd(&G[cur_g].acc[slot + 1], t2);
+            }
           }
-          dacc = 0.0;
+          dacc = 0.0; dacc2 = 0.0;
         };
         for (;; n += kStackConsumers) {
           const int s = bc_take(ring, n);
@@ -1257,8 +1413,15 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
             if (c.inv_in) {
               for (int j = lane; j < c.cols; j += 32) inv_s[j] = __ldcg(c.inv_in + j);
               if (lane == 0) inv_s[c.cols] = 1.f;
+              if (FUSED) {
+                const DfqRelation& r = R[L[cur_li].rel_in];
+                const float* inv1 = arena + L[r.first].rext_off + r.channels;
+                for (int j = lane; j < c.cols; j += 32) inv1_s[j] = __ldcg(inv1 + j);
+                if (lane == 0) inv1_s[c.cols] = 1.f;
+              }
               __syncwarp();
             }
+            if (FUSED) rext = arena + L[cur_li].rext_off;
           }
           const int row_len = c.row_len, n4 = row_len >> 2;
           const uint32_t sbase = smem_u32(ring.stage(s));
@@ -1270,7 +1433,36 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           const float* fold = c.fold;
           float fo_mine = 1.f;
           if (fold && lane < d.nrows) fo_mine = __ldcg(fold + d.row0 + lane);
-          if (has_out) {
+          if (FUSED && has_out) {
+            // ---- first layer, sweeps 1 and 2: the scales are known (fuse_publish) -------------------------------------
+            float s1_mine = 1.f, s2_mine = 1.f;
+            if (lane < d.nrows) { s1_mine = __ldcg(rext + d.row0 + lane); s2_mine = __ldcg(c.s_step + d.row0 + lane); }
+            for (int r = 0; r < d.nrows; ++r) {
+              const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
+              const float s1 = __shfl_sync(0xffffffffu, s1_mine, r), s2 = __shfl_sync(0xffffffffu, s2_mine, r);
+              float d1 = 0.f, d2 = 0.f;
+              if (fold) stack_fused_row<true>(a0, n4, __shfl_sync(0xffffffffu, fo_mine, r), s1, s2, lane, d1, d2);
+              else stack_fused_row<false>(a0, n4, 1.f, s1, s2, lane, d1, d2);
+              dacc += (double)d1 * inv_n;
+              dacc2 += (double)d2 * inv_n;
+            }
+          } else if (FUSED) {
+            // ---- second layer, sweeps 1 and 2 ---------------------------------------------------------------------------
+            for (int r = 0; r < d.nrows; ++r) {
+              const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
+              const float fo = __shfl_sync(0xffffffffu, fo_mine, r);
+              float d1 = 0.f, d2 = 0.f;
+              if (fold) {
+                if (kk == 9) stack_fused_cols<IN_KK9, true>(a0, n4, inv1_s, inv_s, fo, lane, d1, d2);
+                else stack_fused_cols<IN_KK1, true>(a0, n4, inv1_s, inv_s, fo, lane, d1, d2);
+              } else {
+                if (kk == 9) stack_fused_cols<IN_KK9, false>(a0, n4, inv1_s, inv_s, 1.f, lane, d1, d2);
+                else stack_fused_cols<IN_KK1, false>(a0, n4, inv1_s, inv_s, 1.f, lane, d1, d2);
+              }
+              dacc += (double)d1 * inv_n;
+              dacc2 += (double)d2 * inv_n;
+            }
+          } else if (has_out) {
             // ---- first layer of a chain: per-row range -> s -> rescale (dfq.py:48-73) --------------------------------
             if (lane < d.nrows) mine = fetch_row_in(c, P, d.row0 + lane, false);     // this lane's row: column extrema of the pair
             for (int r = 0; r < d.nrows; ++r) {
@@ -1310,7 +1502,8 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           }
           // per-channel bookkeeping of dfq.py:62-70 (S, 1/s, bias, BN vectors, derived column extrema), lane r for row r - after
           // the stage is on its way back: a dozen dependent global accesses that the ring does not have to wait for
-          if (has_out && lane < d.nrows) publish_row(c, P, d.row0 + lane, ks, kinv, mine.cmn, mine.cmx, fetch_row_pub(c, P, d.row0 + lane));
+          if (!FUSED && has_out && lane < d.nrows)
+            publish_row(c, P, d.row0 + lane, ks, kinv, mine.cmn, mine.cmx, fetch_row_pub(c, P, d.row0 + lane));
         }
         flush_metric();
         if (lane == 0) { bulk_wait_all(); fence_proxy_async_all(); }
@@ -1318,11 +1511,25 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
       }
       grid.sync();
     }
-    // ---- exit rule of dfq.py:105-115, one thread per group (as in k_cle_engine) ---------------------------------------
+  };
+  // ---- exit rule of dfq.py:105-115, one thread per group (as in k_cle_engine) ---------------------------------------
+  auto exit_rule_all = [&](int sweep) {
     groups_exit_rule(G, nG, ctl, P, sweep, threadIdx.x, kBcThreads);
     __threadfence();
     grid.sync();
-    if (*((volatile int*)&ctl->active[(sweep + 1) & 1]) == 0) break;
+    return *((volatile int*)&ctl->active[(sweep + 1) & 1]) != 0;
+  };
+
+  int sweep = 0;
+  if (fused) {
+    pass(std::true_type{}, 0);
+    exit_rule_all(0);
+    if (!exit_rule_all(1)) return;
+    sweep = 2;         // the state is the per-sweep run's after two sweeps; later sweeps run the per-sweep pass
+  }
+  for (;; ++sweep) {
+    pass(std::false_type{}, sweep);
+    if (!exit_rule_all(sweep)) break;
   }
 }
 
@@ -1354,6 +1561,7 @@ static int launch_cle(const void* kernel, int grid, int threads, size_t dyn_smem
   }
   result->last_diff = hg[0].diff;
   memcpy(result->diffs, h.diffs, sizeof(h.diffs));
+  result->fused_sweeps = h.fused_sweeps;
   return 0;
 }
 
@@ -1474,6 +1682,7 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     DFQ_REQUIRE(l.bias_off >= 0 && l.bias_off + l.rows <= arena_floats, "bias outside arena");
     if (l.rel_in >= 0 && l.rel_out >= 0) DFQ_REQUIRE(l.rel_in < l.rel_out, "relations must be in forward chain order");
     if (l.flags & DFQ_LAYER_FOLD_PENDING) DFQ_REQUIRE(l.fold_off >= 0 && l.fold_off + l.rows <= arena_floats, "fold factors outside arena");
+    if (l.flags & DFQ_LAYER_ROWS_READY) DFQ_REQUIRE(l.rext_off >= 0 && l.rext_off + 2 * (int64_t)l.rows <= arena_floats, "row extrema outside arena");
   }
   // layers whose column extrema the engine scans before the first sweep (the others arrive with buffer 0 filled)
   std::vector<int32_t> scan_layers;
@@ -1521,7 +1730,12 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     for (int q = 0; q < n_entries; ++q) completes[step_layers[q]] = 1;
   if ((rc = apply_pending_folds(arena, arena_floats, layers, n_layers, completes, st))) return rc;
   if (stack_ok) {
-    const size_t dyn_s = BcRing::smem_bytes();
+    // the first two sweeps in one pass (k_cle_stack's guard has the last word): every first layer's row extrema scanned by the
+    // fold, and an exit rule that cannot stop after sweep 1 on the count or the sweep cap
+    int fuse = params->converge_count >= 2 && params->max_sweeps != 1;
+    for (int q = step_ptr[0]; q < step_ptr[1]; ++q)
+      if (!(layers[step_layers[q]].flags & DFQ_LAYER_ROWS_READY)) fuse = 0;
+    const size_t dyn_s = kStackSmemBytes;
     if ((rc = coop_grid((const void*)k_cle_stack, "k_cle_stack", kBcThreads, dyn_s, max_tiles, &grid))) return rc;
     TablePack tp;
     const int iL = tp.add(layers, n_layers), iR = tp.add(rels, n_rels), iSP = tp.add(step_ptr, n_steps + 1);
@@ -1532,7 +1746,7 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     long long* dPP = tp.ptr<long long>(iPP);
     CleCtl* dctl = nullptr; GroupState* dG = nullptr;
     DfqCleParams P = *params;
-    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups};
+    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups, &fuse};
     return launch_cle((const void*)k_cle_stack, grid, kBcThreads, dyn_s, args, &dctl, &dG, tp, n_groups, result, group_sweeps, st);
   }
 

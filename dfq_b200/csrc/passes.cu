@@ -100,14 +100,42 @@ __global__ void k_fold_prologue(float* arena, const DfqLayer* __restrict__ L, co
   }
 }
 
+// Row extrema of a tile's folded rows (DfqFold.scan_rows): rext[o] = min, rext[rows + o] = max of row o.  The same min / max
+// reduction as k_cle_stack's first sweep over a first-layer row (minmax4, warp_min / warp_max), whose extrema these replace.
+// Only values matter there: min and max ignore NaN whatever the order, and the sign of a zero extremum does not change a range.
+__device__ __forceinline__ void rowscan_tile(const float* buf, int row0, int nrows, int row_len, int rows, float* rext, float* red) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  auto scan = [&](const float* row, int t, int nt, float& mn, float& mx) {
+    if ((row_len & 3) == 0)
+      for (int i = t; i < (row_len >> 2); i += nt) minmax4(mn, mx, ((const float4*)row)[i]);
+    else
+      for (int i = t; i < row_len; i += nt) { mn = fminf(mn, row[i]); mx = fmaxf(mx, row[i]); }
+  };
+  if (nrows == 1) {
+    float mn = DFQ_INF, mx = -DFQ_INF;
+    scan(buf, threadIdx.x, kThreads, mn, mx);
+    block_minmax<kThreads>(mn, mx, red);
+    if (threadIdx.x == 0) { rext[row0] = mn; rext[rows + row0] = mx; }
+  } else {
+    for (int r = warp; r < nrows; r += kWarps) {
+      float mn = DFQ_INF, mx = -DFQ_INF;
+      scan(buf + (size_t)r * row_len, lane, 32, mn, mx);
+      mn = warp_min(mn); mx = warp_max(mx);
+      if (lane == 0) { rext[row0 + r] = mn; rext[rows + row0 + r] = mx; }
+    }
+  }
+}
+
 // The weight pass of the fold.  STORE: folds that rewrite the weights (DFQ_FOLD_FULL, DFQ_FOLD_APPLY).  !STORE: the
-// read-only scan of deferred folds (DFQ_FOLD_DEFER, scan_go > 0): each tile is folded in its stage, scanned and dropped.
+// read-only scan of deferred folds (DFQ_FOLD_DEFER, scan_go > 0 or scan_rows): each tile is folded in its stage, scanned
+// and dropped.
 template <bool STORE>
 __global__ void __launch_bounds__(kThreads, kPipeCtas)
 k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restrict__ F, int nF,
           const long long* __restrict__ tptr) {
   extern __shared__ __align__(128) unsigned char pipe_smem[];
   __shared__ float s_cmin[kFoldScanCols], s_cmax[kFoldScanCols];
+  __shared__ float s_red[2 * kWarps];
   RowPipe pipe;
   pipe.init(pipe_smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -153,6 +181,10 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
     } else {
       for (int r = warp; r < d.nrows; r += kWarps)
         fold_row<32, false>(arena, l, f, pipe.stage[sidx] + (size_t)r * row_len, d.row0 + r, lane);
+    }
+    if (!STORE && f.scan_rows) {
+      __syncthreads();     // the tile's rows are final (and every thread is past the last tile's use of s_red)
+      rowscan_tile(pipe.stage[sidx], d.row0, d.nrows, row_len, l.rows, arena + l.rext_off, s_red);
     }
     if (scanning) {
       __syncthreads();     // the tile's rows are final
@@ -691,6 +723,10 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
     const int row_len = l.cols * l.kk;
     DFQ_REQUIRE(l.w_off >= 0 && l.w_off + (int64_t)l.rows * row_len <= arena_floats, "weight outside arena");
     if (f.mode != DFQ_FOLD_FULL) DFQ_REQUIRE(f.fac_off >= 0 && f.fac_off + l.rows <= arena_floats, "fold factors outside arena");
+    if (f.scan_rows) {
+      DFQ_REQUIRE(f.mode == DFQ_FOLD_DEFER, "only DFQ_FOLD_DEFER scans rows");
+      DFQ_REQUIRE(l.rext_off >= 0 && l.rext_off + 2 * (int64_t)l.rows <= arena_floats, "row scan needs the layer's row extrema scratch");
+    }
     if (f.scan_go > 0) {
       DFQ_REQUIRE(f.mode != DFQ_FOLD_APPLY, "DFQ_FOLD_APPLY does not scan");
       DFQ_REQUIRE(f.scan_gi > 0 && l.rows % f.scan_go == 0 && f.scan_gi == l.cols, "fold scan geometry (DfqRelation.go / .gi of the layer's rel_in)");
@@ -701,7 +737,7 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
     }
     if (f.mode == DFQ_FOLD_DEFER) {
       prologue = true;
-      if (f.scan_go > 0) {
+      if (f.scan_go > 0 || f.scan_rows) {
         // the read-only scan folds each row in its stage: a row must fit one
         DFQ_REQUIRE(row_len <= kStageFloats, "deferred fold with a scan: rows larger than a pipe stage");
         ro.push_back(f);

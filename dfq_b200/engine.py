@@ -39,6 +39,7 @@ class CleResult:
     diffs: List[float]       # diff_tmp per sweep of group 0
     group_sweeps: Optional[np.ndarray] = None
     apply_only: bool = False
+    fused_sweeps: int = 0    # 2: k_cle_stack applied the first two sweeps in one pass (plan_bn_fold's row scan), else 0
 
 
 @dataclass
@@ -279,7 +280,7 @@ class Session:
             t[i]["w_off"] = l["w_off"]; t[i]["bias_off"] = l["bias_off"]
             t[i]["rows"] = l["rows"]; t[i]["cols"] = l["cols"]; t[i]["kk"] = l["kk"]
             t[i]["rel_in"] = -1; t[i]["rel_out"] = -1; t[i]["col_mode"] = 0; t[i]["group"] = 0
-            t[i]["cmin_off"] = -1; t[i]["cmax_off"] = -1; t[i]["fold_off"] = -1
+            t[i]["cmin_off"] = -1; t[i]["cmax_off"] = -1; t[i]["fold_off"] = -1; t[i]["rext_off"] = -1
             if roles and i in roles:
                 for k, v in roles[i].items():
                     t[i][k] = v
@@ -298,7 +299,11 @@ class Session:
         is DEFERRED: run_bn_fold does the [rows]-vector work and a read-only scan of the `second` layers, and the
         equalization's first sweep multiplies every row by its fold factor as it reads it - one read-write pass over the
         weights fewer.  Until run_cle_plan(cle_plan) has run, every other call of this session that touches the arena
-        completes the fold first (finish_fold), so nothing ever sees unfolded weights."""
+        completes the fold first (finish_fold), so nothing ever sees unfolded weights.
+
+        A deferred fold also reads the plan's `first` layers and writes their row extrema (`plan["rows_scanned"]`: pairs
+        (layer, offset of its [2][rows] scratch)).  With those and the column extrema, the stack kernel knows the scales of
+        the first two sweeps before it reads a weight and, where its guard allows, applies both in one pass."""
         ft = np.zeros(len(folds), dtype=_lib.FOLD_DT)
         scanned = []
         for i, f in enumerate(folds):
@@ -309,7 +314,8 @@ class Session:
                 if ri >= 0:
                     ft[i]["scan_go"] = cle_plan["rt"][ri]["go"]; ft[i]["scan_gi"] = cle_plan["rt"][ri]["gi"]
                     scanned.append(int(f["layer"]))
-        deferred = []
+        deferred, rows_scanned = [], []
+        lt = cle_plan["lt"] if cle_plan is not None else self._layer_table()
         if cle_plan is not None and self._takes_stack(cle_plan, scanned):
             in_plan = set(int(x) for x in cle_plan["step_layers"])
             for i, f in enumerate(folds):
@@ -318,8 +324,13 @@ class Session:
                     ft[i]["mode"] = _lib.FOLD_DEFER
                     ft[i]["fac_off"] = self.alloc(self._layers[li]["rows"])
                     deferred.append((li, int(ft[i]["fac_off"])))
-        return dict(ft=ft, lt=cle_plan["lt"] if cle_plan is not None else self._layer_table(), scanned=scanned,
-                    deferred=deferred, cle_plan=cle_plan)
+                    if lt[li]["rel_out"] >= 0 and lt[li]["rel_in"] < 0:
+                        ft[i]["scan_rows"] = 1
+                        rows_scanned.append((li, self.alloc(2 * self._layers[li]["rows"])))
+            if rows_scanned:
+                lt = lt.copy()
+                lt["rext_off"][[r[0] for r in rows_scanned]] = [r[1] for r in rows_scanned]
+        return dict(ft=ft, lt=lt, scanned=scanned, deferred=deferred, rows_scanned=rows_scanned, cle_plan=cle_plan)
 
     def _takes_stack(self, cle_plan: dict, cols_ready: Sequence[int]) -> bool:
         """Whether dfq_cle_run will take `cle_plan` (with these layers' column extrema ready) on the stack kernel - the
@@ -465,12 +476,17 @@ class Session:
         if pending is not None:
             # the deferred layers are marked FOLD_PENDING: the stack kernel folds them in its first sweep, any other path of
             # dfq_cle_run applies the fold before it starts
-            key = (id(lt), tuple(pending["deferred"]))
+            # the first layers whose row extrema the fold scanned are marked ROWS_READY
+            key = (id(lt), tuple(pending["deferred"]), tuple(pending["rows_scanned"]))
             if pending.get("_pending_key") != key:
                 lt2 = lt.copy()
                 li = [d[0] for d in pending["deferred"]]
                 lt2["flags"][li] |= _lib.LAYER_FOLD_PENDING
                 lt2["fold_off"][li] = [d[1] for d in pending["deferred"]]
+                if pending["rows_scanned"]:
+                    li = [d[0] for d in pending["rows_scanned"]]
+                    lt2["flags"][li] |= _lib.LAYER_ROWS_READY
+                    lt2["rext_off"][li] = [d[1] for d in pending["rows_scanned"]]
                 pending["_pending_key"], pending["_pending_lt"], pending["_pending_base"] = key, lt2, lt
             lt = pending["_pending_lt"]
         gs = np.zeros(plan["n_groups"], dtype=np.int32)
@@ -485,6 +501,7 @@ class Session:
         res = CleResult(n, bool(R[0]["converged"]), float(R[0]["last_diff"]), [float(x) for x in R[0]["diffs"][:min(n, 64)]])
         res.group_sweeps = gs
         res.apply_only = bool(apply_only)
+        res.fused_sweeps = int(R[0]["fused_sweeps"])
         return res
 
     def cle_col_hints(self, plan: dict, res: CleResult) -> Optional[Dict[str, np.ndarray]]:

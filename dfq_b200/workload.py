@@ -171,12 +171,12 @@ class DeviceStack:
     """`n_blocks` independent Conv[C,C,k,k]+BN+ReLU -> Conv[C,C,k,k]+BN blocks living only in a Session arena.
 
     Pipeline per calibration step (the BASELINE metric's unit of work, per Conv/BN pair), N weights per conv:
-      BN fold: the per-channel vectors and a read-only scan of the second conv's column extrema (4N B per block = 2N B
-      per conv on average; the weight pass itself is deferred into the first sweep, see Session.plan_bn_fold) ->
-      equalization to convergence (8N B per sweep, 2 sweeps; the first sweep also folds) -> bias correction of the second
-      conv (4N B read once - its range comes from the equalization's column extrema - = 2N B per conv on average)
-      [-> 8-bit weight fake-quant (8N+4N B)].  20N B per conv in all (26N B with the fold as a pass of its own: the
-      engine path, where the fold is not deferred).
+      BN fold: the per-channel vectors and a read-only scan of both convs (column extrema of the second, row extrema of
+      the first: 4N B per conv; the weight pass itself is deferred into the first sweep, see Session.plan_bn_fold) ->
+      equalization to convergence (2 sweeps, applied in ONE pass of 8N B that also folds; a later sweep would be 8N B
+      more) -> bias correction of the second conv (4N B read once - its range comes from the equalization's column
+      extrema - = 2N B per conv on average) [-> 8-bit weight fake-quant (8N+4N B)].  14N B per conv in all (26N B with
+      the fold and each sweep as passes of their own: the engine path, where the fold is not deferred).
     """
 
     def __init__(self, sess, n_blocks: int, channels: int = 512, k: int = 3, seed: int = 1234, quantize: bool = False):

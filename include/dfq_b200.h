@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 7
+#define DFQ_ABI_VERSION 8
 
 enum {
   DFQ_OK = 0,
@@ -77,22 +77,29 @@ typedef struct DfqLayer {
   int32_t flags;      /* DFQ_LAYER_COLS_READY: buffer 0 of cmin/cmax already holds the column extrema of the
                          current weights (dfq_bn_fold with DfqFold.scan_go > 0 just produced them): dfq_cle_run
                          skips its initial scan of this layer
-                         DFQ_LAYER_FOLD_PENDING: see below                                     */
+                         DFQ_LAYER_FOLD_PENDING, DFQ_LAYER_ROWS_READY: see below                */
   int64_t cmin_off;   /* [2][C of rel_in] running column minima, double-buffered by sweep parity
                          (scratch, valid when rel_in >= 0)                                  */
   int64_t cmax_off;   /* [2][C of rel_in] running column maxima                              */
   int64_t fold_off;   /* DFQ_LAYER_FOLD_PENDING: [rows] fold factors gamma/sqrt(var+eps) (DfqFold.fac_off)      */
+  int64_t rext_off;   /* DFQ_LAYER_ROWS_READY: [2][rows] scratch, row minima then row maxima (DfqFold.scan_rows)     */
 } DfqLayer;
 
-/* Both flags are promises about the call that runs RIGHT AFTER dfq_bn_fold, on the same weights:
+/* The flags are promises about the call that runs RIGHT AFTER dfq_bn_fold, on the same weights:
  *   DFQ_LAYER_COLS_READY   the fold (scan_go > 0) has written buffer 0 of the column extrema of the FOLDED weights.
  *   DFQ_LAYER_FOLD_PENDING the fold ran with DfqFold.mode = DFQ_FOLD_DEFER: biases, BN vectors and the factors at fold_off
  *                          are final, the weights are NOT yet multiplied by the factors.  dfq_cle_run completes the fold:
  *                          k_cle_stack multiplies each row by its factor as its first sweep reads it (fl(w * f), the value
  *                          the fold would have stored); on every other path (the engine, no sweep at all) the fold is
- *                          applied to the weights before anything else.  Either way the weights are folded on return. */
+ *                          applied to the weights before anything else.  Either way the weights are folded on return.
+ *   DFQ_LAYER_ROWS_READY   the fold (DfqFold.scan_rows) has written the row extrema of the FOLDED weights of this `first`
+ *                          layer to rext_off.  When every first layer of a k_cle_stack run carries it, the kernel may
+ *                          derive the scales of the first two sweeps from these extrema and the column extrema alone and
+ *                          apply both sweeps in one pass over the weights (DfqCleResult.fused_sweeps); the scratch is
+ *                          consumed either way (its content after the call is unspecified). */
 #define DFQ_LAYER_COLS_READY 1
 #define DFQ_LAYER_FOLD_PENDING 2
+#define DFQ_LAYER_ROWS_READY 4
 
 /* One equalization relation (utils/relation.py:5-27): rows of `first` are multiplied by s[c],
  * the matching input columns of `second` by 1/s[c] (dfq.py:62-73). */
@@ -129,6 +136,9 @@ typedef struct DfqCleResult {
   int32_t converged;       /* exit rule of dfq.py:83 fired (as opposed to max_sweeps)            */
   double last_diff;        /* `diff` of dfq.py:110 at exit                                        */
   double diffs[64];        /* diff_tmp of the first 64 sweeps (dfq.py:105-108)                    */
+  int32_t fused_sweeps;    /* 2: k_cle_stack applied sweeps 1 and 2 in one pass (DFQ_LAYER_ROWS_READY), 0: one pass
+                              per sweep.  Results are the same bits either way.                                  */
+  int32_t _pad;
 } DfqCleResult;
 
 /* Cross-layer equalization to convergence.  Replaces dfq.py:78-117 (cross_layer_equalization) and,
@@ -177,13 +187,14 @@ typedef struct DfqFold {
                                  buffer 0 of the layer's cmin_off / cmax_off (layers[] must carry them), saving the
                                  equalization its initial 4 B/weight scan.  0: no scan. */
   int32_t mode;               /* DFQ_FOLD_FULL / _DEFER / _APPLY, below                                              */
-  int32_t _pad;
+  int32_t scan_rows;          /* _DEFER only, 1: also write the row extrema of the FOLDED weights to the layer's rext_off
+                                 ([0, rows) minima, [rows, 2 rows) maxima; layers[] must carry it).  0: no row scan.    */
   int64_t fac_off;            /* _DEFER, _APPLY: [rows] fold factors gamma/sqrt(var+eps)                              */
 } DfqFold;
 /* DFQ_FOLD_FULL   the fold above: weights, bias, fake_weight / fake_bias.
  * DFQ_FOLD_DEFER  everything but the weights: bias, fake_weight / fake_bias, and each row's factor into fac_off.  With
  *                 scan_go > 0 the weights are READ (not written) and the column extrema of fl(w * factor) - those of the
- *                 folded weights - go to buffer 0.  The weights stay unfolded until a DFQ_LAYER_FOLD_PENDING layer entry
+ *                 folded weights - go to buffer 0; with scan_rows the row extrema of fl(w * factor) go to rext_off.  The weights stay unfolded until a DFQ_LAYER_FOLD_PENDING layer entry
  *                 (fold_off = fac_off) hands them to dfq_cle_run, or a DFQ_FOLD_APPLY call completes the fold.
  * DFQ_FOLD_APPLY  the weights only: W[o,:] = fl(W[o,:] * fac[o]); gamma / beta / mean / var / bias are not read. */
 #define DFQ_FOLD_FULL 0

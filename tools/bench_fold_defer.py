@@ -2,10 +2,11 @@
 
 bench.py's `roofline.whole_step` counts the unfused algorithm, 26 B per weight: fold 8 + two sweeps 16 + correction 2.  With
 the fold deferred into the first sweep (plan_bn_fold(..., cle_plan=...) when the stack kernel takes the plan) a step moves
-  fold       read-only scan of the second conv: 4 B per second-conv weight = 2 B per weight averaged over both convs
-  equalize   8 B per weight per sweep (read + write)
-  correct    reads the second conv once: 2 B per weight averaged
-i.e. 20 B per weight at 2 sweeps.  This prints those bytes and the achieved TB/s of the fold scan and of the whole step, per
+  fold       read-only scan of both convs (column extrema of the second, row extrema of the first): 4 B per weight
+  equalize   8 B per weight per pass over the weights (read + write); the first pass applies sweeps 1 and 2 when the
+             stack kernel's guard accepts (CleResult.fused_sweeps = 2), every later sweep is a pass of its own
+  correct    reads the second conv once: 2 B per weight averaged over both convs
+i.e. 14 B per weight at 2 sweeps.  This prints those bytes and the achieved TB/s of the fold scan and of the whole step, per
 phase timed with CUDA events like bench.py (state restored from a pristine copy, untimed, before every step).
 
     python tools/bench_fold_defer.py [--pairs 2048] [--steps 10] [--warmup 3]
@@ -51,12 +52,16 @@ def main():
     fold_ms, cle_ms, bc_ms = (sum(t[k] for t in times) / len(times) for k in range(3))
     n = st.N * st.n_layers                          # weights of the stack
     sweeps = int(res.n_sweeps)
-    fold_b = (2.0 if deferred else 8.0) * n         # scan of the second convs / read + write of every weight
-    cle_b = 8.0 * sweeps * n
+    rows_scanned = bool(st.fold_plan["rows_scanned"])
+    # read-only scan of both convs / of the second convs only / read + write of every weight
+    fold_b = (4.0 if rows_scanned else 2.0 if deferred else 8.0) * n
+    passes = sweeps - 1 if res.fused_sweeps == 2 else sweeps
+    cle_b = 8.0 * passes * n
     bc_b = 2.0 * n
     step_ms = fold_ms + cle_ms + bc_ms
     props = torch.cuda.get_device_properties(torch.cuda.current_device())
     out = {"gpu": props.name, "pairs": st.n_layers, "sweeps": sweeps, "fold_deferred": deferred,
+           "fused_sweeps": res.fused_sweeps, "passes": passes,
            "bytes_per_weight": {"fold": fold_b / n, "equalize": cle_b / n, "correct": bc_b / n,
                                 "step": (fold_b + cle_b + bc_b) / n},
            "ms": {"fold": fold_ms, "equalize": cle_ms, "correct": bc_ms, "step": step_ms},
