@@ -14,13 +14,14 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
 LAYER_FOLD_PENDING = 2
 LAYER_ROWS_READY = 4
 FOLD_FULL, FOLD_DEFER, FOLD_APPLY = 0, 1, 2   # DfqFold.mode
+BC_PREPARED = 4        # DfqBcLayer.flags
 
 
 class DfqError(RuntimeError):
@@ -51,7 +52,7 @@ CLE_PARAMS_DT = np.dtype([
 
 CLE_RESULT_DT = np.dtype([
     ("n_sweeps", np.int32), ("converged", np.int32), ("last_diff", np.float64),
-    ("diffs", np.float64, (64,)), ("fused_sweeps", np.int32), ("_pad", np.int32),
+    ("diffs", np.float64, (64,)), ("fused_sweeps", np.int32), ("bc_prepared", np.int32),
 ], align=True)
 
 FOLD_DT = np.dtype([
@@ -123,6 +124,8 @@ SIGNATURES = {
     "dfq_device_info": [C.POINTER(C.c_int), C.POINTER(C.c_int)],
     "dfq_cle_run": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32,
                     C.c_void_p, C.c_void_p, _I32, C.c_void_p, _ST],
+    "dfq_cle_run_bc": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32,
+                       C.c_void_p, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32, C.c_void_p, _I32, _I32, _ST],
     "dfq_cle_takes_stack": [C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32, _I32, C.c_void_p],
     "dfq_bn_fold": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, _ST],
     "dfq_bias_correct": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, _I32, _ST],

@@ -84,6 +84,47 @@ __device__ __forceinline__ float bc_qerr(float w, const BcFastQuant& f) {
   return __fsub_rn(__fadd_rn(t, f.min_v), w);
 }
 
+// scipy.stats.norm.pdf / cdf in float64 on an fp32 argument, rounded to fp32 (dfq.py:182-183)
+__device__ __forceinline__ float std_pdf(float x32) {
+  const double x = (double)x32;
+  return (float)(exp(-x * x / 2.0) / 2.5066282746310002);   // sqrt(2*pi)
+}
+__device__ __forceinline__ float std_cdf(float x32) {
+  // scipy.special.ndtr (cephes)
+  const double x = (double)x32 * 0.70710678118654752440;
+  const double z = fabs(x);
+  double y;
+  if (z < 0.70710678118654752440) y = 0.5 + 0.5 * erf(x);
+  else { y = 0.5 * erfc(z); if (x > 0) y = 1.0 - y; }
+  return (float)y;
+}
+// dfq.py:184 calculate_mean + :240 clamp; every op an individually rounded fp32 op as in eager PyTorch
+__device__ __forceinline__ float relu_gauss_mean(float g, float b) {
+  const float q = __fdiv_rn(-b, g);
+  const float t1 = __fmul_rn(g, std_pdf(q));
+  const float t2 = __fmul_rn(b, __fsub_rn(1.0f, std_cdf(q)));
+  const float e = __fadd_rn(t1, t2);
+  return e < 0.f ? 0.f : e;      // NaN stays NaN (expect[expect < 0] = 0)
+}
+
+// E[x] of one layer (dfq.py:228-278) into ex: its terms in order, each written to or (accumulate) added into its slice.
+// SMEM: ex is this CTA's shared-memory copy; otherwise it lies in the arena and is accessed with .cg.  (k_bc_engine,
+// k_bc_stream, and k_cle_stack's prologue of an attached correction.)
+template <int THREADS, bool SMEM>
+__device__ __forceinline__ void bc_expect(float* arena, const DfqBcLayer& b, const DfqExpectTerm* __restrict__ T, float* ex) {
+  for (int ti = b.term_begin; ti < b.term_end; ++ti) {
+    const DfqExpectTerm t = T[ti];
+    for (int ch = threadIdx.x; ch < t.n; ch += THREADS) {
+      const float fb = __ldcg(arena + t.bn_b_off + ch);
+      const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
+      float* d = ex + t.dst_off + ch;
+      if (SMEM) *d = t.accumulate ? __fadd_rn(*d, v) : v;
+      else __stcg(d, t.accumulate ? __fadd_rn(__ldcg(d), v) : v);
+    }
+    __syncthreads();
+  }
+}
+
 struct BcRing {
   unsigned char* base;
   __device__ __forceinline__ float* stage(int s) const { return (float*)(base + (size_t)s * kStageBytes); }

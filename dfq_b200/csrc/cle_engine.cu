@@ -1331,14 +1331,27 @@ __device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n,
 }
 
 // Dynamic shared memory of k_cle_stack: the ring, then kBcConsumers reciprocal caches (BcRing::ex_cache) and kStackConsumers
-// more for the fused pass's second vector (ex_cache(kBcConsumers + warp)).
-constexpr size_t kStackSmemBytes = BcRing::smem_bytes() + (size_t)kStackConsumers * (kBcExCols + 4) * 4;
+// more for the fused pass's second vector (ex_cache(kBcConsumers + warp)).  An attached correction caches E[x] per consumer
+// warp (stack_ex_slot): in the ring's caches no consumer uses (kStackConsumers .. kBcConsumers - 1), then behind the others.
+constexpr int kStackExExtra = 2 * kStackConsumers > kBcConsumers ? 2 * kStackConsumers - kBcConsumers : 0;
+constexpr size_t kStackSmemBytes = BcRing::smem_bytes() + (size_t)(kStackConsumers + kStackExExtra) * (kBcExCols + 4) * 4;
+__device__ __forceinline__ int stack_ex_slot(int warp) {
+  return warp < kBcConsumers - kStackConsumers ? kStackConsumers + warp : kBcConsumers + kStackConsumers + warp - (kBcConsumers - kStackConsumers);
+}
+
+// The bias correction attached to the fused pass (dfq_cle_run's bc tables; see "Attached correction" in dfq_cle_run).
+struct StackBc {
+  const DfqBcLayer* B;     // one level, every entry the `second` layer of a relation, expect_len = cols, no flags
+  const DfqExpectTerm* T;
+  const int* of_layer;     // [nL]: the entry of a layer, or -1
+  int n, num_bits;
+};
 
 // fuse: the host found every first layer DFQ_LAYER_ROWS_READY, converge_count >= 2 and max_sweeps != 1; the guard decides.
 __global__ void __launch_bounds__(kBcThreads, 1)
 k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelation* __restrict__ R, int nR,
             const int* __restrict__ step_ptr, const int* __restrict__ step_layers, const long long* __restrict__ pass_ptr,
-            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG, int fuse) {
+            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG, int fuse, StackBc bc) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(128) unsigned char ring_smem[];
   __shared__ RowCtx wctx[kBcConsumers];
@@ -1362,6 +1375,27 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
       if (blockIdx.x == 0 && threadIdx.x == 0) ctl->fused_sweeps = 2;
       __threadfence();
       grid.sync();
+      // Attached correction, what k_bc_stream does before its row phase, a CTA per entry: the per-tensor range from the
+      // column extrema of sweep 2 (buffer 0, the one cle_col_hints names for a group that stops there; reduced as k_bc_stream
+      // reduces such a hint), then E[x] from the BN vectors fuse_publish has just scaled.  Both hold for the final state
+      // only when every group stops after sweep 2 - the host uses the deltas only then (DfqCleResult.bc_prepared).
+      if (bc.n > 0) {
+        for (int bi = blockIdx.x; bi < bc.n; bi += gridDim.x) {
+          const DfqBcLayer b = bc.B[bi];
+          if (warp == 0) {
+            const DfqLayer l = L[b.layer];
+            float mn = DFQ_INF, mx = -DFQ_INF;
+            for (int j = lane; j < l.cols; j += 32) {
+              mn = fminf(mn, __ldcg(arena + l.cmin_off + j)); mx = fmaxf(mx, __ldcg(arena + l.cmax_off + j));
+            }
+            mn = warp_min(mn); mx = warp_max(mx);
+            if (lane == 0) { __stcg(arena + b.minmax_off, mn); __stcg(arena + b.minmax_off + 1, mx); }
+          }
+          bc_expect<kBcThreads, false>(arena, b, bc.T, arena + b.expect_off);
+        }
+        __threadfence();
+        grid.sync();
+      }
     }
   }
 
@@ -1381,6 +1415,12 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
         float* inv_s = ring.ex_cache(warp);            // reciprocal scales of the current second layer's columns (+ sentinel)
         float* inv1_s = ring.ex_cache(kBcConsumers + warp);   // FUSED: those of sweep 1 (inv_s: sweep 2)
         const float* rext = nullptr;                   // FUSED, first layer: s1 per row (fuse_publish)
+        // FUSED, a second layer with an attached correction: its entry (bc_mode -1: none), quantizer and E[x] cache
+        float* bc_ex = ring.ex_cache(stack_ex_slot(warp));
+        float* bc_delta = nullptr;
+        const float* bc_exg = nullptr;
+        BcFastQuant bc_f;
+        int bc_mode = -1;
         int cur_li = -1, cur_g = -1, kk = 1;
         double dacc = 0.0, dacc2 = 0.0;
         auto flush_metric = [&]() {
@@ -1422,6 +1462,20 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
               __syncwarp();
             }
             if (FUSED) rext = arena + L[cur_li].rext_off;
+            if (FUSED) {
+              const int bi = bc.n > 0 ? bc.of_layer[cur_li] : -1;
+              bc_mode = -1;
+              if (bi >= 0) {
+                const DfqBcLayer b = bc.B[bi];
+                bc_f = bc_fast_quant(quant_scalars((double)__ldcg(arena + b.minmax_off), (double)__ldcg(arena + b.minmax_off + 1),
+                                                   bc.num_bits, b.signed_mode), bc.num_bits);
+                bc_mode = bc_f.ok ? 0 : 1;
+                bc_delta = arena + b.delta_off;
+                bc_exg = arena + b.expect_off;
+                for (int j = lane; j < c.cols; j += 32) bc_ex[j] = __ldcg(bc_exg + j);
+                __syncwarp();
+              }
+            }
           }
           const int row_len = c.row_len, n4 = row_len >> 2;
           const uint32_t sbase = smem_u32(ring.stage(s));
@@ -1497,6 +1551,22 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           if (lane == 0) {
             bulk_s2g(d.gptr, ring.stage(s), (uint32_t)d.floats * 4u);
             bulk_commit();
+          }
+          // attached correction: eps . E[x] of the final rows (dfq.py:216-219,281-287), read from the stage while the store
+          // reads it too - k_bc_stream's row reduction on the same bits; lane r writes row r's delta, nothing else
+          if (FUSED && !has_out && bc_mode >= 0) {
+            float dl = 0.f;
+            for (int r = 0; r < d.nrows; ++r) {
+              const uint32_t srow = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
+              const double acc = bc_mode == 1 ? bc_stream_row_smem<1, 0>(srow, c.cols, kk, bc_ex, bc_exg, bc_f, lane)
+                               : kk == 9      ? bc_stream_row_smem<0, 9>(srow, c.cols, 9, bc_ex, bc_exg, bc_f, lane)
+                                              : bc_stream_row_smem<0, 1>(srow, c.cols, 1, bc_ex, bc_exg, bc_f, lane);
+              if (lane == r) dl = (float)acc;
+            }
+            if (lane < d.nrows) __stcg(bc_delta + d.row0 + lane, dl);
+            __syncwarp();
+          }
+          if (lane == 0) {
             bulk_wait_read<0>();
             mbar_arrive(ring.empty + s);
           }
@@ -1536,7 +1606,8 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
 // Cooperative launch of k_cle_engine / k_cle_stack with zeroed convergence state, then the read-back of that state into
 // *result.  `args` holds the addresses of *dctl and *dG, which are allocated here, before the launch reads them.
 static int launch_cle(const void* kernel, int grid, int threads, size_t dyn_smem, void** args, CleCtl** dctl, GroupState** dG,
-                      TablePack& tp, int n_groups, DfqCleResult* result, int32_t* group_sweeps, cudaStream_t st) {
+                      TablePack& tp, int n_groups, DfqCleResult* result, int32_t* group_sweeps, cudaStream_t st,
+                      bool bc_attached = false) {
   DFQ_CUDA(cudaMallocAsync((void**)dctl, sizeof(CleCtl), st));
   DFQ_CUDA(cudaMemsetAsync(*dctl, 0, sizeof(CleCtl), st));
   DFQ_CUDA(cudaMallocAsync((void**)dG, sizeof(GroupState) * n_groups, st));
@@ -1554,14 +1625,18 @@ static int launch_cle(const void* kernel, int grid, int threads, size_t dyn_smem
   rb.finish();
   result->n_sweeps = 0;
   result->converged = 1;
+  bool all_two = true;
   for (int g = 0; g < n_groups; ++g) {
     result->n_sweeps = std::max(result->n_sweeps, hg[g].n_sweeps);
     result->converged &= hg[g].converged;
+    all_two &= (hg[g].n_sweeps == 2);
     if (group_sweeps) group_sweeps[g] = hg[g].n_sweeps;
   }
   result->last_diff = hg[0].diff;
   memcpy(result->diffs, h.diffs, sizeof(h.diffs));
   result->fused_sweeps = h.fused_sweeps;
+  // the attached correction saw the state after sweep 2: it is the final one only if no group went on
+  result->bc_prepared = (bc_attached && h.fused_sweeps == 2 && all_two) ? 1 : 0;
   return 0;
 }
 
@@ -1644,9 +1719,20 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
                            const DfqRelation* rels, int32_t n_rels, const int32_t* step_ptr,
                            const int32_t* step_layers, int32_t n_steps, const DfqCleParams* params,
                            DfqCleResult* result, int32_t n_groups, int32_t* group_sweeps, void* stream) {
+  return dfq_cle_run_bc(arena, arena_floats, layers, n_layers, rels, n_rels, step_ptr, step_layers, n_steps, params, result,
+                        n_groups, group_sweeps, nullptr, 0, nullptr, 0, 0, stream);
+}
+
+extern "C" int dfq_cle_run_bc(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
+                              const DfqRelation* rels, int32_t n_rels, const int32_t* step_ptr,
+                              const int32_t* step_layers, int32_t n_steps, const DfqCleParams* params,
+                              DfqCleResult* result, int32_t n_groups, int32_t* group_sweeps, const DfqBcLayer* bc, int32_t n_bc,
+                              const DfqExpectTerm* bc_terms, int32_t n_bc_terms, int32_t bc_num_bits, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   DFQ_REQUIRE(arena && layers && rels && step_ptr && step_layers && params && result, "null argument");
   DFQ_REQUIRE(n_layers > 0 && n_rels > 0 && n_steps > 0 && n_groups > 0, "empty problem");
+  if (!bc) n_bc = 0;
+  DFQ_REQUIRE(n_bc <= 0 || (bc_terms && n_bc_terms >= 0), "attached correction without its terms");
   memset(result, 0, sizeof(*result));
   // Python `while diff > thres and count < converge_count` with diff = 10, count = 0 (dfq.py:81-83)
   // - no sweep at all; a pending fold is completed all the same
@@ -1720,6 +1806,31 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     set_error("DFQ_CLE_STACK=1: problem not eligible for k_cle_stack: %s", not_stack);
     return DFQ_E_ARG;
   }
+  // Attached correction: computed inside k_cle_stack's fused pass, so it must be one that pass can compute with the
+  // arithmetic of k_bc_stream and that never depends on another entry's result (one level, no raw sums, no added deltas).
+  std::vector<int32_t> bc_of;
+  if (n_bc > 0) {
+    if (!stack_ok) { set_error("attached bias correction: the problem does not run on k_cle_stack"); return DFQ_E_ARG; }
+    DFQ_REQUIRE(bc_num_bits >= 1 && bc_num_bits <= 32, "attached bias correction: num_bits");
+    bc_of.assign(n_layers, -1);
+    for (int i = 0; i < n_bc; ++i) {
+      const DfqBcLayer& b = bc[i];
+      DFQ_REQUIRE(b.layer >= 0 && b.layer < n_layers, "attached bias correction: layer index");
+      const DfqLayer& l = layers[b.layer];
+      DFQ_REQUIRE(l.rel_in >= 0 && l.rel_out < 0, "attached bias correction: every entry must be the `second` layer of a relation");
+      DFQ_REQUIRE(bc_of[b.layer] < 0, "attached bias correction: a layer listed twice");
+      DFQ_REQUIRE(b.flags == 0, "attached bias correction: no raw-sum, add or prepared flags");
+      DFQ_REQUIRE(b.expect_len == l.cols, "attached bias correction: expect_len must equal the layer's columns");
+      DFQ_REQUIRE(b.term_begin >= 0 && b.term_end <= n_bc_terms && b.term_begin <= b.term_end, "attached bias correction: term range");
+      for (int t = b.term_begin; t < b.term_end; ++t)
+        DFQ_REQUIRE(bc_terms[t].dst_off >= 0 && bc_terms[t].dst_off + bc_terms[t].n <= b.expect_len,
+                    "attached bias correction: term outside expectation vector");
+      DFQ_REQUIRE(b.expect_off >= 0 && b.expect_off + b.expect_len <= arena_floats && b.delta_off >= 0 &&
+                  b.delta_off + l.rows <= arena_floats && b.minmax_off >= 0 && b.minmax_off + 2 <= arena_floats,
+                  "attached bias correction: scratch outside arena");
+      bc_of[b.layer] = i;
+    }
+  }
   DFQ_CUDA(cudaGetDevice(&dev));
   const int n_entries = step_ptr[n_steps];
   std::vector<long long> pass_ptr(n_entries + 1, 0);    // pass-tile prefix over step_layers
@@ -1740,14 +1851,25 @@ extern "C" int dfq_cle_run(float* arena, int64_t arena_floats, const DfqLayer* l
     TablePack tp;
     const int iL = tp.add(layers, n_layers), iR = tp.add(rels, n_rels), iSP = tp.add(step_ptr, n_steps + 1);
     const int iSL = tp.add(step_layers, n_entries), iPP = tp.add(pass_ptr.data(), n_entries + 1);
+    int iB = -1, iT = -1, iOf = -1;
+    if (n_bc > 0) {
+      iB = tp.add(bc, n_bc); iOf = tp.add(bc_of.data(), n_layers);
+      if (n_bc_terms > 0) iT = tp.add(bc_terms, n_bc_terms);
+    }
     if ((rc = tp.upload(st))) return rc;
     DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqRelation* dR = tp.ptr<DfqRelation>(iR);
     int32_t *dSP = tp.ptr<int32_t>(iSP), *dSL = tp.ptr<int32_t>(iSL);
     long long* dPP = tp.ptr<long long>(iPP);
+    StackBc sbc{nullptr, nullptr, nullptr, 0, bc_num_bits};
+    if (n_bc > 0) {
+      sbc.B = tp.ptr<DfqBcLayer>(iB); sbc.of_layer = tp.ptr<int32_t>(iOf); sbc.n = n_bc;
+      if (iT >= 0) sbc.T = tp.ptr<DfqExpectTerm>(iT);
+    }
     CleCtl* dctl = nullptr; GroupState* dG = nullptr;
     DfqCleParams P = *params;
-    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups, &fuse};
-    return launch_cle((const void*)k_cle_stack, grid, kBcThreads, dyn_s, args, &dctl, &dG, tp, n_groups, result, group_sweeps, st);
+    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups, &fuse, &sbc};
+    return launch_cle((const void*)k_cle_stack, grid, kBcThreads, dyn_s, args, &dctl, &dG, tp, n_groups, result, group_sweeps, st,
+                      n_bc > 0);
   }
 
   DFQ_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));

@@ -290,29 +290,6 @@ k_quant_tasks(float* arena, const FlatTask* __restrict__ T, int nT, const long l
 // ------------------------------------------------------------------------------------------------
 // bias correction engine (persistent cooperative kernel)
 // ------------------------------------------------------------------------------------------------
-// scipy.stats.norm.pdf / cdf in float64 on an fp32 argument, rounded to fp32 (dfq.py:182-183)
-__device__ __forceinline__ float std_pdf(float x32) {
-  const double x = (double)x32;
-  return (float)(exp(-x * x / 2.0) / 2.5066282746310002);   // sqrt(2*pi)
-}
-__device__ __forceinline__ float std_cdf(float x32) {
-  // scipy.special.ndtr (cephes)
-  const double x = (double)x32 * 0.70710678118654752440;
-  const double z = fabs(x);
-  double y;
-  if (z < 0.70710678118654752440) y = 0.5 + 0.5 * erf(x);
-  else { y = 0.5 * erfc(z); if (x > 0) y = 1.0 - y; }
-  return (float)y;
-}
-// dfq.py:184 calculate_mean + :240 clamp; every op an individually rounded fp32 op as in eager PyTorch
-__device__ __forceinline__ float relu_gauss_mean(float g, float b) {
-  const float q = __fdiv_rn(-b, g);
-  const float t1 = __fmul_rn(g, std_pdf(q));
-  const float t2 = __fmul_rn(b, __fsub_rn(1.0f, std_cdf(q)));
-  const float e = __fadd_rn(t1, t2);
-  return e < 0.f ? 0.f : e;      // NaN stays NaN (expect[expect < 0] = 0)
-}
-
 struct BcGeo {
   float* arena; const DfqLayer* L; const DfqBcLayer* B;
   __device__ __forceinline__ void operator()(int q, float*& base, int& rows, int& row_len) const {
@@ -329,23 +306,6 @@ __device__ __forceinline__ void bc_reset_minmax(float* arena, const DfqBcLayer* 
   for (int i = blockIdx.x * THREADS + threadIdx.x; i < nB; i += gridDim.x * THREADS) {
     __stcg(arena + B[i].minmax_off, DFQ_INF);
     __stcg(arena + B[i].minmax_off + 1, -DFQ_INF);
-  }
-}
-
-// E[x] of one layer (dfq.py:228-278) into ex: its terms in order, each written to or (accumulate) added into its slice.
-// SMEM: ex is this CTA's shared-memory copy; otherwise it lies in the arena and is accessed with .cg.
-template <int THREADS, bool SMEM>
-__device__ __forceinline__ void bc_expect(float* arena, const DfqBcLayer& b, const DfqExpectTerm* __restrict__ T, float* ex) {
-  for (int ti = b.term_begin; ti < b.term_end; ++ti) {
-    const DfqExpectTerm t = T[ti];
-    for (int ch = threadIdx.x; ch < t.n; ch += THREADS) {
-      const float fb = __ldcg(arena + t.bn_b_off + ch);
-      const float v = t.relu ? relu_gauss_mean(__ldcg(arena + t.bn_w_off + ch), fb) : fb;
-      float* d = ex + t.dst_off + ch;
-      if (SMEM) *d = t.accumulate ? __fadd_rn(*d, v) : v;
-      else __stcg(d, t.accumulate ? __fadd_rn(__ldcg(d), v) : v);
-    }
-    __syncthreads();
   }
 }
 
@@ -687,6 +647,21 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
   }
 }
 
+// A prepared correction (DFQ_BC_PREPARED: k_cle_stack computed the deltas of the current weights): what bc_retire_row does,
+// per row, a CTA per entry.  The entries travel as this compact table (32 B instead of the 80 B DfqBcLayer plus the whole
+// layer table: the upload through mapped host memory was most of the call).
+struct BcRetire { int64_t bias_off, delta_off, next_off; int32_t rows, add; };
+__global__ void k_bc_retire(float* arena, const BcRetire* __restrict__ E, int n) {
+  for (int i = blockIdx.x; i < n; i += gridDim.x) {
+    const BcRetire e = E[i];
+    for (int o = threadIdx.x; o < e.rows; o += blockDim.x) {
+      const float dl = __ldcg(arena + e.delta_off + o);
+      __stcg(arena + e.bias_off + o, __fadd_rn(__ldcg(arena + e.bias_off + o), e.add ? dl : -dl));     // dfq.py:292 / :164
+      if (e.next_off >= 0) __stcg(arena + e.next_off + o, __fadd_rn(__ldcg(arena + e.next_off + o), -dl));   // dfq.py:204-206,293
+    }
+  }
+}
+
 // Library self-test hook: the element-wise quantization error Q(w) - w of one tensor computed with the streaming kernel's
 // XU-free arithmetic (eps_fast) and with the plain IEEE chain of quantize.py:70-74 (eps_div); *ok = the per-tensor guard.
 __global__ void k_bc_selftest(const float* __restrict__ w, float* eps_fast, float* eps_div, int64_t n,
@@ -822,6 +797,28 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
     mm_ptr[i + 1] = mm_ptr[i] + (b.n_col > 0 ? 0 : pipe_tiles(l.rows, l.cols * l.kk));
   }
   max_tiles = std::max<int64_t>(max_tiles, row_ptr[n_bc]);
+  std::vector<BcRetire> retire;
+  int max_rows = 1;
+  for (int i = 0; i < n_bc; ++i) {
+    if (!(bc[i].flags & DFQ_BC_PREPARED)) continue;
+    const DfqLayer& l = layers[bc[i].layer];
+    DFQ_REQUIRE(!(bc[i].flags & 1), "DFQ_BC_PREPARED on a raw-sum entry");
+    DFQ_REQUIRE(bc[i].delta_off >= 0 && bc[i].delta_off + l.rows <= arena_floats, "delta scratch outside arena");
+    retire.push_back(BcRetire{l.bias_off, bc[i].delta_off, bc[i].next_bn_b_off, l.rows, (bc[i].flags & 2) ? 1 : 0});
+    max_rows = std::max(max_rows, (int)l.rows);
+  }
+  if (!retire.empty()) {
+    DFQ_REQUIRE((int)retire.size() == n_bc, "a table that mixes DFQ_BC_PREPARED and unprepared entries");
+    TablePack tp;
+    const int iE = tp.add(retire.data(), n_bc);
+    int rc;
+    if ((rc = tp.upload(st))) return rc;
+    const int threads = std::min(512, (max_rows + 31) / 32 * 32);
+    k_bc_retire<<<std::min(n_bc, std::max(1, sm_count()) * 8), threads, 0, st>>>(arena, tp.ptr<BcRetire>(iE), n_bc);
+    DFQ_CUDA(cudaGetLastError());
+    tp.release(st);
+    return 0;
+  }
   std::vector<int32_t> level_local(n_levels, 0);
   for (int lv = 0; lv < n_levels; ++lv) {
     bool ok = (level_ptr[lv + 1] - level_ptr[lv]) <= 4;

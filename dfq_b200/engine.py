@@ -40,6 +40,7 @@ class CleResult:
     group_sweeps: Optional[np.ndarray] = None
     apply_only: bool = False
     fused_sweeps: int = 0    # 2: k_cle_stack applied the first two sweeps in one pass (plan_bn_fold's row scan), else 0
+    bc_prepared: bool = False  # the correction attached to the plan (plan_bias_correct(cle_plan=...)) was computed in that pass
 
 
 @dataclass
@@ -68,6 +69,7 @@ class Session:
         self.h2d_bytes = 0
         self.d2h_bytes = 0
         self._pending = None        # a fold plan whose weight pass was deferred into the equalization (plan_bn_fold)
+        self._bc_ready = None       # (correction plan, num_bits) whose deltas the last equalization computed (plan_bias_correct)
 
     # ---- arena planning ---------------------------------------------------------------------------
     def alloc(self, n: int, align: int = 4) -> int:
@@ -341,6 +343,12 @@ class Session:
         lt = cle_plan["lt"].copy()
         if cols_ready:
             lt["flags"][list(cols_ready)] |= _lib.LAYER_COLS_READY
+        return self._takes_stack_lt(cle_plan, lt)
+
+    def _takes_stack_lt(self, cle_plan: dict, lt: np.ndarray) -> bool:
+        fn = getattr(self.lib, "dfq_cle_takes_stack", None)
+        if fn is None:
+            return False
         takes = np.zeros(1, dtype=np.int32)
         _lib.check(fn(_lib.table_ptr(lt), len(lt), _lib.table_ptr(cle_plan["rt"]), len(cle_plan["rt"]),
                       _lib.table_ptr(cle_plan["step_ptr"]), _lib.table_ptr(cle_plan["step_layers"]), cle_plan["n_steps"], 0,
@@ -366,7 +374,10 @@ class Session:
         return self._pending is not None
 
     def finish_fold(self):
-        """Complete a deferred fold now: W[o,:] *= its stored factor (one read-write pass over the deferred layers)."""
+        """Complete a deferred fold now: W[o,:] *= its stored factor (one read-write pass over the deferred layers).
+        Every session call that touches the arena runs this first; it also forgets a prepared correction (plan_bias_correct),
+        whose deltas may no longer be those of the weights."""
+        self._bc_ready = None
         plan, self._pending = self._pending, None
         if plan is None:
             return
@@ -448,8 +459,11 @@ class Session:
                      eps=0, max_sweeps=0, apply_only=False, cols_ready: Optional[Sequence[int]] = None) -> CleResult:
         """Run dfq.py:78-117 on a planned relation list; see include/dfq_b200.h dfq_cle_run.
         cols_ready: layers whose column extrema (buffer 0) a fold planned with cle_plan=plan has JUST written.
-        A fold planned with cle_plan=plan and deferred (plan_bn_fold) is completed by this call."""
+        A fold planned with cle_plan=plan and deferred (plan_bn_fold) is completed by this call.
+        A bias correction attached to plan (plan_bias_correct(cle_plan=plan)) is computed in the same pass when the stack
+        kernel runs it; CleResult.bc_prepared says whether its deltas are those of the final weights."""
         self._ensure_room()
+        self._bc_ready = None
         pending = self._pending
         if pending is not None and pending["cle_plan"] is not plan:
             self.finish_fold()
@@ -490,11 +504,20 @@ class Session:
                 pending["_pending_key"], pending["_pending_lt"], pending["_pending_base"] = key, lt2, lt
             lt = pending["_pending_lt"]
         gs = np.zeros(plan["n_groups"], dtype=np.int32)
-        _lib.check(self.lib.dfq_cle_run(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
-                                        _lib.table_ptr(rt), len(rt), _lib.table_ptr(plan["step_ptr"]),
-                                        _lib.table_ptr(plan["step_layers"]), plan["n_steps"], _lib.table_ptr(P),
-                                        _lib.table_ptr(R), plan["n_groups"], _lib.table_ptr(gs), _lib.stream_ptr()),
-                   "dfq_cle_run")
+        # the attached correction goes along only where the library accepts it: on the stack kernel (a library without
+        # dfq_cle_run_bc - a test stand-in - never gets it)
+        att = plan.get("bc")
+        run_bc = getattr(self.lib, "dfq_cle_run_bc", None)
+        if att is not None and (run_bc is None or apply_only or not self._takes_stack_lt(plan, lt)):
+            att = None
+        args = (self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt), _lib.table_ptr(rt), len(rt),
+                _lib.table_ptr(plan["step_ptr"]), _lib.table_ptr(plan["step_layers"]), plan["n_steps"], _lib.table_ptr(P),
+                _lib.table_ptr(R), plan["n_groups"], _lib.table_ptr(gs))
+        if att is not None:
+            _lib.check(run_bc(*args, _lib.table_ptr(att["plan"]["bt"]), len(att["plan"]["bt"]), _lib.table_ptr(att["plan"]["tt"]),
+                              att["plan"]["n_terms"], int(att["num_bits"]), _lib.stream_ptr()), "dfq_cle_run_bc")
+        else:
+            _lib.check(self.lib.dfq_cle_run(*args, _lib.stream_ptr()), "dfq_cle_run")
         if pending is not None:
             self._pending = None
         n = int(R[0]["n_sweeps"])
@@ -502,6 +525,9 @@ class Session:
         res.group_sweeps = gs
         res.apply_only = bool(apply_only)
         res.fused_sweeps = int(R[0]["fused_sweeps"])
+        res.bc_prepared = att is not None and bool(R[0]["bc_prepared"])
+        if res.bc_prepared:
+            self._bc_ready = (att["plan"], int(att["num_bits"]))
         return res
 
     def cle_col_hints(self, plan: dict, res: CleResult) -> Optional[Dict[str, np.ndarray]]:
@@ -528,9 +554,17 @@ class Session:
         return res, plan["s_offs"]
 
     # ---- bias correction ----------------------------------------------------------------------------
-    def plan_bias_correct(self, items: Sequence[dict]) -> dict:
+    def plan_bias_correct(self, items: Sequence[dict], cle_plan: Optional[dict] = None, num_bits: int = 8) -> dict:
         """items (in graph order): dict(layer, signed, terms=[dict(bn_w_off, bn_b_off, n, relu, op)], next_bn_b_off,
-        level[, raw_sum, add]) with op in {'set', 'cat', 'add'}."""
+        level[, raw_sum, add]) with op in {'set', 'cat', 'add'}.
+
+        cle_plan: the equalization plan that runs right before this correction.  When the correction is one the stack
+        kernel can compute in its fused pass (one level; every item the `second` layer of one of cle_plan's relations, once;
+        no raw sums or added deltas; an expectation as long as the layer's input), it is attached to cle_plan
+        (`plan["attached"]`): run_cle_plan(cle_plan) then computes the deltas from the rows it holds anyway, and a
+        run_bias_correct_plan(plan, num_bits, col_hints=...) right after it only retires them - no second read of the
+        weights.  Anything else in between (any session call that touches the arena), another num_bits, no col_hints or an
+        equalization that did not stop after two fused sweeps: the full correction runs, as without cle_plan."""
         bt = np.zeros(len(items), dtype=_lib.BC_LAYER_DT)
         terms = []
         order = sorted(range(len(items)), key=lambda i: (items[i]["level"], i))
@@ -571,15 +605,33 @@ class Session:
         level_ptr = np.zeros(len(uniq) + 1, dtype=np.int32)
         for k, lv in enumerate(uniq):
             level_ptr[k + 1] = level_ptr[k] + sum(1 for x in levels if x == lv)
-        return dict(bt=bt, tt=tt, n_terms=len(terms), level_ptr=level_ptr, n_levels=len(uniq), delta_offs=delta_offs,
-                    lt=self._layer_table())
+        plan = dict(bt=bt, tt=tt, n_terms=len(terms), level_ptr=level_ptr, n_levels=len(uniq), delta_offs=delta_offs,
+                    lt=self._layer_table(), attached=False)
+        if cle_plan is not None and self._bc_attachable(bt, len(uniq), cle_plan):
+            cle_plan["bc"] = dict(plan=plan, num_bits=int(num_bits))
+            plan["attached"] = True
+        return plan
+
+    def _bc_attachable(self, bt: np.ndarray, n_levels: int, cle_plan: dict) -> bool:
+        """dfq_cle_run's conditions on an attached correction (include/dfq_b200.h), checked on the host."""
+        lt = cle_plan["lt"]
+        layers = bt["layer"].astype(np.int64)
+        return (n_levels == 1 and len(bt) > 0 and not bt["flags"].any() and len(set(layers.tolist())) == len(layers)
+                and bool(np.all(lt["rel_in"][layers] >= 0)) and bool(np.all(lt["rel_out"][layers] < 0))
+                and bool(np.all(bt["expect_len"] == lt["cols"][layers])))
 
     def run_bias_correct_plan(self, plan: dict, num_bits: int = 8, col_hints: Optional[Dict[str, np.ndarray]] = None):
-        """col_hints: see cle_col_hints (only meaningful for the layers' CURRENT weights)."""
+        """col_hints: see cle_col_hints (only meaningful for the layers' CURRENT weights).
+        Right after the run_cle_plan that computed this plan's correction (plan_bias_correct(cle_plan=...)) at this
+        num_bits, with col_hints (the range that run reduced), only the deltas are retired."""
         self._ensure_room()
+        ready = self._bc_ready
         self.finish_fold()
         lt, bt, tt = plan["lt"], plan["bt"], plan["tt"]
-        if col_hints is not None and len(col_hints["layer"]):
+        if ready is not None and ready[0] is plan and ready[1] == int(num_bits) and col_hints is not None:
+            bt = bt.copy()
+            bt["flags"] |= _lib.BC_PREPARED
+        elif col_hints is not None and len(col_hints["layer"]):
             bt = bt.copy()
             lut = np.full(len(lt), -1, dtype=np.int64)
             lut[col_hints["layer"]] = np.arange(len(col_hints["layer"]))

@@ -173,10 +173,12 @@ class DeviceStack:
     Pipeline per calibration step (the BASELINE metric's unit of work, per Conv/BN pair), N weights per conv:
       BN fold: the per-channel vectors and a read-only scan of both convs (column extrema of the second, row extrema of
       the first: 4N B per conv; the weight pass itself is deferred into the first sweep, see Session.plan_bn_fold) ->
-      equalization to convergence (2 sweeps, applied in ONE pass of 8N B that also folds; a later sweep would be 8N B
-      more) -> bias correction of the second conv (4N B read once - its range comes from the equalization's column
-      extrema - = 2N B per conv on average) [-> 8-bit weight fake-quant (8N+4N B)].  14N B per conv in all (26N B with
-      the fold and each sweep as passes of their own: the engine path, where the fold is not deferred).
+      equalization to convergence (2 sweeps, applied in ONE pass of 8N B that also folds and computes the second conv's
+      bias correction from the rows it holds; a later sweep would be 8N B more) -> the correction's retirement, [C]-sized
+      vectors only [-> 8-bit weight fake-quant (8N+4N B)].  12N B per conv in all.  When the equalization does not stop
+      after its two fused sweeps the correction reads the second conv once more (4N B = 2N B per conv on average, its range
+      from the equalization's column extrema); 26N B with the fold, each sweep and the correction as passes of their own
+      (the engine path, where the fold is not deferred).
     """
 
     def __init__(self, sess, n_blocks: int, channels: int = 512, k: int = 3, seed: int = 1234, quantize: bool = False):
@@ -214,7 +216,8 @@ class DeviceStack:
         items = [dict(layer=self.layers[2 * b + 1], signed=False, level=0, next_bn_b_off=self.vec[2 * b + 1]["fake_b"],
                       terms=[dict(bn_w_off=self.vec[2 * b]["fake_w"], bn_b_off=self.vec[2 * b]["fake_b"], n=C, relu=True, op="set")])
                  for b in range(n_blocks)]
-        self.bc_plan = sess.plan_bias_correct(items)
+        # ... and the correction of the second convs rides on the equalization's pass (Session.plan_bias_correct)
+        self.bc_plan = sess.plan_bias_correct(items, cle_plan=self.cle_plan)
         self.quant_plan = None
         if quantize:
             tasks = []
@@ -286,7 +289,8 @@ class DeviceStack:
     @property
     def launches_per_step(self) -> int:
         """Kernels of this library per step: fold prologue (column-range reset, the deferred fold's vectors) + fold pass
-        (the read-only scan when deferred), equalization engine, correction engine [+ range init, min/max, quantize], plus
+        (the read-only scan when deferred), equalization engine, correction engine (its retirement when the equalization
+        prepared it) [+ range init, min/max, quantize], plus
         the small copy kernel (k_copy_words) that moves each call's descriptor tables (fold, equalization, correction
         [, quantize]) and the equalization's two result blocks through mapped pinned memory."""
         return 4 + 5 + (4 if self.quant_plan is not None else 0)

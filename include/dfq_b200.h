@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 8
+#define DFQ_ABI_VERSION 9
 
 enum {
   DFQ_OK = 0,
@@ -138,7 +138,9 @@ typedef struct DfqCleResult {
   double diffs[64];        /* diff_tmp of the first 64 sweeps (dfq.py:105-108)                    */
   int32_t fused_sweeps;    /* 2: k_cle_stack applied sweeps 1 and 2 in one pass (DFQ_LAYER_ROWS_READY), 0: one pass
                               per sweep.  Results are the same bits either way.                                  */
-  int32_t _pad;
+  int32_t bc_prepared;     /* 1: the attached bias correction (dfq_cle_run's bc tables) holds the results of the final
+                              weights - the fused pass ran and every group stopped after sweep 2.  0: none attached, or
+                              its scratch is stale (all or nothing).                                              */
 } DfqCleResult;
 
 /* Cross-layer equalization to convergence.  Replaces dfq.py:78-117 (cross_layer_equalization) and,
@@ -165,6 +167,25 @@ int dfq_cle_run(float* arena, int64_t arena_floats,
                 const DfqCleParams* params, DfqCleResult* result,
                 int32_t n_groups, int32_t* group_sweeps /* host, [n_groups] sweeps run per group, or NULL */,
                 void* stream);
+
+/* dfq_cle_run with an attached bias correction (bc, n_bc, bc_terms, n_bc_terms, bc_num_bits; NULL or 0: none, which is
+ * dfq_cle_run).  One level of a dfq_bias_correct table (same structs, same meaning, num_bits = bc_num_bits) whose
+ * correction k_cle_stack computes inside its fused pass, from the rows it holds in shared memory - instead of a later pass
+ * that reads the corrected layers again.  The call writes each entry's minmax_off, expect_off and delta_off (eps . E[x])
+ * and nothing else: no bias and no fake_bias changes.  Those are the results of the final weights only when
+ * result->bc_prepared is 1; a dfq_bias_correct of the same table with every entry flagged DFQ_BC_PREPARED then only
+ * retires them.  Refused (DFQ_E_ARG) unless the problem runs on k_cle_stack and every entry is the `second` layer of a
+ * relation, listed once, with flags 0 and expect_len = cols. */
+struct DfqBcLayer;
+struct DfqExpectTerm;
+int dfq_cle_run_bc(float* arena, int64_t arena_floats,
+                   const DfqLayer* layers, int32_t n_layers,
+                   const DfqRelation* rels, int32_t n_rels,
+                   const int32_t* step_ptr, const int32_t* step_layers, int32_t n_steps,
+                   const DfqCleParams* params, DfqCleResult* result,
+                   int32_t n_groups, int32_t* group_sweeps,
+                   const struct DfqBcLayer* bc, int32_t n_bc, const struct DfqExpectTerm* bc_terms, int32_t n_bc_terms,
+                   int32_t bc_num_bits, void* stream);
 
 /* *takes = 1 when dfq_cle_run would run this problem (same tables, DfqCleParams.apply_only = apply_only) on the
  * streaming stack kernel k_cle_stack on the current device, 0 when on k_cle_engine - the one decision dfq_cle_run makes
@@ -226,7 +247,7 @@ typedef struct DfqBcLayer {
   int32_t expect_len;        /* = groups * cols */
   int32_t flags;             /* bit 0: use sum_k W instead of the quantization error (bias absorption,
                                 dfq.py:139-153); bit 1: ADD delta to the bias (dfq.py:164) instead of
-                                subtracting it (dfq.py:292) */
+                                subtracting it (dfq.py:292); DFQ_BC_PREPARED: see below */
   int64_t expect_off;        /* scratch [expect_len] */
   int64_t delta_off;         /* scratch/out [rows]: eps . E[x]                           */
   int64_t next_bn_b_off;     /* fake_bias that receives -delta (dfq.py:204-206), or -1  */
@@ -236,6 +257,11 @@ typedef struct DfqBcLayer {
   int32_t n_col;             /* streamed a second time.  After dfq_cle_run the valid buffer of a `second` layer is      */
   int32_t _pad;              /* cmin_off + (group_sweeps[group] & 1) * C (same for cmax).  0: scan the weights.          */
 } DfqBcLayer;
+/* DFQ_BC_PREPARED: delta_off, expect_off and minmax_off already hold this layer's results for its CURRENT weights (a
+ * dfq_cle_run with this table attached reported bc_prepared, and nothing has touched the arena since).  When every entry
+ * carries it, dfq_bias_correct only retires the deltas: bias = fl(bias - delta), next fake_bias = fl(fake_bias - delta),
+ * no weight is read.  A table that mixes flagged and unflagged entries, or flags a raw-sum entry, is refused. */
+#define DFQ_BC_PREPARED 4
 int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
                      const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
                      const int32_t* level_ptr, int32_t n_levels, int32_t num_bits, void* stream);

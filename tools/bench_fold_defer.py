@@ -5,8 +5,10 @@ the fold deferred into the first sweep (plan_bn_fold(..., cle_plan=...) when the
   fold       read-only scan of both convs (column extrema of the second, row extrema of the first): 4 B per weight
   equalize   8 B per weight per pass over the weights (read + write); the first pass applies sweeps 1 and 2 when the
              stack kernel's guard accepts (CleResult.fused_sweeps = 2), every later sweep is a pass of its own
-  correct    reads the second conv once: 2 B per weight averaged over both convs
-i.e. 14 B per weight at 2 sweeps.  This prints those bytes and the achieved TB/s of the fold scan and of the whole step, per
+  correct    0 B per weight when the equalization computed it in its fused pass (CleResult.bc_prepared: the correction
+             planned with cle_plan=..., every group stopped after sweep 2) and only the deltas are retired; otherwise it
+             reads the second conv once: 2 B per weight averaged over both convs
+i.e. 12 B per weight at 2 fused sweeps (14 B when the correction reads the weights again).  This prints those bytes and the achieved TB/s of the fold scan and of the whole step, per
 phase timed with CUDA events like bench.py (state restored from a pristine copy, untimed, before every step).
 
     python tools/bench_fold_defer.py [--pairs 2048] [--steps 10] [--warmup 3]
@@ -57,16 +59,16 @@ def main():
     fold_b = (4.0 if rows_scanned else 2.0 if deferred else 8.0) * n
     passes = sweeps - 1 if res.fused_sweeps == 2 else sweeps
     cle_b = 8.0 * passes * n
-    bc_b = 2.0 * n
+    bc_b = 0.0 if res.bc_prepared else 2.0 * n
     step_ms = fold_ms + cle_ms + bc_ms
     props = torch.cuda.get_device_properties(torch.cuda.current_device())
     out = {"gpu": props.name, "pairs": st.n_layers, "sweeps": sweeps, "fold_deferred": deferred,
-           "fused_sweeps": res.fused_sweeps, "passes": passes,
+           "fused_sweeps": res.fused_sweeps, "passes": passes, "bc_prepared": res.bc_prepared,
            "bytes_per_weight": {"fold": fold_b / n, "equalize": cle_b / n, "correct": bc_b / n,
                                 "step": (fold_b + cle_b + bc_b) / n},
            "ms": {"fold": fold_ms, "equalize": cle_ms, "correct": bc_ms, "step": step_ms},
            "TB/s": {"fold": fold_b / (fold_ms * 1e-3) / 1e12, "equalize": cle_b / (cle_ms * 1e-3) / 1e12,
-                    "correct": bc_b / (bc_ms * 1e-3) / 1e12, "step": (fold_b + cle_b + bc_b) / (step_ms * 1e-3) / 1e12}}
+                    "correct": (bc_b / (bc_ms * 1e-3) / 1e12) if bc_b else None, "step": (fold_b + cle_b + bc_b) / (step_ms * 1e-3) / 1e12}}
     print(json.dumps(out))
 
 
