@@ -16,6 +16,8 @@
 // the last two can target a channel slice of a wider tensor (dfq_i8_conv_slice), so the producers of a channel
 // concatenation write the consumer's input directly; k_i8_maxpool pools codes, or fp32 to fp32 and / or codes;
 // k_i8_upsample_bilinear resizes fp32 as torch does, to fp32 and / or codes in such a channel slice.
+// A fourth epilogue writes the fp32 output pixel-major into a slice of a detection head's [N, R, k] concatenation
+// (dfq_i8_conv_nhwc), so the permute / contiguous / cat of SSD's heads need no copies.
 #include <algorithm>
 #include <cmath>
 
@@ -36,10 +38,10 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // Where the epilogue puts its result.  F32: fp32 NCHW y (and optionally the int32 sums).  I8: the codes of the next layer,
 // int8 NHWC yq[N, OH, OW, cpad] (cpad = O rounded up to 16, pad channels 0), requantized at the next layer's scale after
 // the activation clamp [lo, hi].
-// FUSED: Fused below.
+// FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED };
+enum class Out { F32, I8, FUSED, ROWS };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -69,8 +71,17 @@ struct Fused {
   float* y;
   float post_lo, post_hi;
 };
+// The pixel-major fp32 epilogue (dfq_i8_conv_nhwc): v = clamp(clamp(dequant, pre), post) goes to
+// y[n * img_stride + off + p * O + o], the permute(0, 2, 3, 1) of the NCHW output placed at `off` inside each image's
+// img_stride floats (a slice along dim 1 of a detection head's [N, R, k] concatenation).
+struct Rows {
+  float* y;
+  int64_t off, img_stride;
+  float pre_lo, pre_hi, post_lo, post_hi;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
+template <> struct EpiOf<Out::ROWS> { using type = Rows; };
 
 // What the per-layer path computes from the convolution to the tensor after a residual block's add, in its order: the
 // pass-throughs before the add as one clamp, the fp32 add (rv = r[n, o, p], ignored without a residual), the ones after it.
@@ -78,6 +89,11 @@ __device__ __forceinline__ float fused_value(int32_t acc, float dq, float b, flo
   float v = clamp_keep_nan(dequant(acc, dq, b), e.pre_lo, e.pre_hi);
   if (e.r) v = __fadd_rn(v, rv);
   return clamp_keep_nan(v, e.post_lo, e.post_hi);
+}
+
+// fused_value without a residual, for the Rows epilogue
+__device__ __forceinline__ float rows_value(int32_t acc, float dq, float b, const Rows& e) {
+  return clamp_keep_nan(clamp_keep_nan(dequant(acc, dq, b), e.pre_lo, e.pre_hi), e.post_lo, e.post_hi);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -252,6 +268,36 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
+  if constexpr (OUT == Out::ROWS) {
+    // Straight from the accumulator layout: for one register pair (h = 0, 1), a warp holds 8 pixels x 8 consecutive
+    // channels, so the stores run in 32-byte pieces along the channels of each pixel's row.  4-byte stores: off and O are
+    // arbitrary, so a row may start at any float.
+    float d[4][2], b[4][2];
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int o = o0 + wn * 32 + j * 8 + (lane & 3) * 2 + h;
+        d[j][h] = o < g.O ? dq[o] : 0.f;
+        b[j][h] = o < g.O && bias ? bias[o] : 0.f;
+      }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int64_t m = m0 + wm * 64 + i * 16 + (lane >> 2) + rr * 8;
+        if (m >= M) continue;
+        float* row = rq.y + (m / OHW) * rq.img_stride + rq.off + (m % OHW) * g.O;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int o = o0 + wn * 32 + j * 8 + (lane & 3) * 2 + h;
+            if (o < g.O) row[o] = rows_value(acc[i][j][2 * rr + h], d[j][h], b[j][h], rq);
+          }
+      }
+    return;
+  }
   if constexpr (OUT == Out::FUSED) {
     // Straight from the accumulator layout: for one register, a warp holds 8 consecutive pixels (m) of 4 channels, so the
     // residual reads and the fp32 stores run in 32-byte pieces along the pixels of one channel.  A piece is one 32-byte
@@ -320,7 +366,7 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
         }
     }
   }
-  if constexpr (OUT != Out::F32) {
+  if constexpr (OUT == Out::I8 || OUT == Out::FUSED) {
     __syncthreads();
     // one 16-byte chunk = 16 channels of one pixel; chunks at or past cpad (= O rounded up to 16) are not written
     for (int e = tid; e < BM * (BN / 16); e += THREADS) {
@@ -372,7 +418,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
     const int64_t t = i / OHW;
     const int ch = (int)(t % chunks);
     const int64_t n = t / chunks;
-    if constexpr (OUT != Out::F32) {
+    if constexpr (OUT == Out::I8 || OUT == Out::FUSED) {
       // the input's Cpad may be wider than yq's cpad = round_up(O, 16): chunks past it hold only pad channels, and yq has
       // no room for them
       if (ch * 16 >= rq.cpad) continue;
@@ -410,6 +456,15 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         }
       }
       if (rq.yq) *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cstride + ch * 16) = *reinterpret_cast<const int4*>(v);
+      continue;
+    }
+    if constexpr (OUT == Out::ROWS) {                           // this pixel's 16 channels of its row
+      float* row = rq.y + n * rq.img_stride + rq.off + (int64_t)p * g.C + ch * 16;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        if (c < g.C) row[j] = rows_value(acc[j], dq[c], bias ? bias[c] : 0.f, rq);
+      }
       continue;
     }
     if constexpr (OUT == Out::I8) {                             // the 16 channels of this pixel in one store
@@ -756,6 +811,37 @@ extern "C" int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float
     const Fused ep{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride, e->residual, e->y, e->post_lo, e->post_hi};
     if (dense) k_i8_conv_mma<Out::FUSED><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
     else k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_conv_nhwc(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                                int64_t off, int64_t img_stride, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE(xq && wq && dq && e, "dfq_i8_conv_nhwc: null pointer");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv_nhwc: codes must be 16-byte aligned");
+  DFQ_REQUIRE(e->y, "dfq_i8_conv_nhwc: no output (y is NULL)");
+  DFQ_REQUIRE(((uintptr_t)e->y & 3) == 0, "dfq_i8_conv_nhwc: y must be 4-byte aligned");
+  DFQ_REQUIRE(!e->residual && !e->yq, "dfq_i8_conv_nhwc: residual and yq must be NULL (fp32 rows only)");
+  DFQ_REQUIRE(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
+              "dfq_i8_conv_nhwc: pre / post clamp bounds must be ordered and not NaN");
+  const int64_t extent = (int64_t)g->OH * g->OW * g->O;              // floats of one image's rows
+  DFQ_REQUIRE(off >= 0, "dfq_i8_conv_nhwc: off must be non-negative");
+  DFQ_REQUIRE(img_stride >= off + extent, "dfq_i8_conv_nhwc: img_stride must be at least off + OH * OW * O");
+  const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
+  const int64_t x_bytes = (int64_t)g->N * g->H * g->W * g->Cpad;
+  const int64_t y_bytes = ((g->N - 1) * img_stride + extent) * (int64_t)sizeof(float);   // first to last row written
+  DFQ_REQUIRE(!overlap(xq, x_bytes, e->y + off, y_bytes), "dfq_i8_conv_nhwc: y overlaps xq");
+  const Rows ep{e->y, off, img_stride, e->pre_lo, e->pre_hi, e->post_lo, e->post_hi};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    DFQ_REQUIRE((pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_nhwc: too many output pixels");
+    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<Out::ROWS><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<Out::ROWS><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;

@@ -82,13 +82,15 @@ class _Int8Layer(nn.Module):
 
     Execution modes, set only on the copies chain_int8 makes (`chained`): `codes_in` - the input is already int8 NHWC codes
     [N, H, W, cpad] at this layer's act_scale; `requant` = (out_scale, lo, hi) - the output is the next layer's int8 NHWC
-    codes (dfq_i8_conv_requant) instead of fp32 NCHW; `epilogue` - the residual epilogue (dfq_i8_conv_fused, see Epilogue).
+    codes (dfq_i8_conv_requant) instead of fp32 NCHW; `epilogue` - the residual epilogue (dfq_i8_conv_fused, see Epilogue);
+    `rows` - the clamped fp32 output pixel-major, a detection head's rows of its concatenation (dfq_i8_conv_nhwc).
     A layer convert_to_int8 made takes and returns fp32 only."""
 
     codes_in = False
     requant = None
     epilogue = None
     out_slice = None
+    rows = False
     layer_name = None
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
@@ -132,13 +134,17 @@ class _Int8Layer(nn.Module):
             g[0][k] = v
         return g
 
-    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None, rows=False):
         """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
         mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes; epilogue - an
         Epilogue: the residual epilogue (not together with requant); out_slice = (coff, cstride), with requant - write the
         codes into channels [coff, coff + round_up(C_out, 16)) of an int8 NHWC tensor [N, OH, OW, cstride] (a channel
-        concatenation, dfq_i8_conv_slice), given as forward(x, out=...) or made when out is None.  name: the layer's name
-        in error messages.  self is not modified."""
+        concatenation, dfq_i8_conv_slice), given as forward(x, out=...) or made when out is None; rows - the fp32 output
+        pixel-major (dfq_i8_conv_nhwc): forward(x, out=y, off=off) writes permute(0, 2, 3, 1) of it as OH * OW * C_out floats
+        at y[n].view(-1)[off:] of a contiguous fp32 y [N, ...] (a detection head's slice of its [N, R, k] concatenation), or
+        returns a new [N, OH * OW, C_out] tensor when out is None; the clamps come from an fp32-only epilogue without
+        residual (none: no clamp), and rows excludes requant.  name: the layer's name in error messages.  self is not
+        modified."""
         new = type(self).__new__(type(self))
         nn.Module.__init__(new)
         for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad", "act_scale"):
@@ -173,18 +179,25 @@ class _Int8Layer(nn.Module):
                                     % (new._who(), coff, cstride))
             out_slice = (coff, cstride)
         new.out_slice = out_slice
+        if rows:
+            if requant is not None or out_slice is not None or \
+                    (epilogue is not None and (epilogue.out_scale is not None or epilogue.residual)):
+                raise _lib.DfqError("layer %s: pixel-major fp32 rows exclude codes and a residual" % new._who())
+            new.epilogue = epilogue or Epilogue(fp32=True)
+        new.rows = bool(rows)
         return new
 
     def _who(self):
         return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
                                                                   self.kernel_size)
 
-    def run(self, x, with_acc=False, residual=None, out=None):
+    def run(self, x, with_acc=False, residual=None, out=None, off=0):
         """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue.  In the chained modes
         x is int8 codes [N, H, W, cpad] (codes_in) and y int8 codes [N, OH, OW, round_up(C_out, 16)] (requant).  With an
         epilogue, y is the codes, the fp32 output, or (codes, fp32 output) when it returns both, and `residual` is the fp32
         tensor [N, C_out, OH, OW] the epilogue adds (exactly that shape, no broadcasting, on x's device).  With out_slice, y
-        is `out` (int8 [N, OH, OW, cstride] on x's device) or a new such tensor, its slice written."""
+        is `out` (int8 [N, OH, OW, cstride] on x's device) or a new such tensor, its slice written.  With rows, y is `out`
+        with this layer's rows written at `off` of each image, or a new [N, OH * OW, C_out] tensor (see chained)."""
         if not x.is_cuda or not self.dq.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.dq.device))
@@ -214,6 +227,8 @@ class _Int8Layer(nn.Module):
             xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
             _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, self.in_channels, H, W, self.cpad,
                                                 C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
+        if self.rows:
+            return self._run_rows(xq, out, off, g, N, OH, OW), None
         if self.epilogue is not None:
             return self._run_fused(xq, residual, g, N, OH, OW), None
         if out is not None and self.out_slice is None:
@@ -250,6 +265,31 @@ class _Int8Layer(nn.Module):
                    "dfq_i8_conv_slice (layer %s)" % self._who())
         return out
 
+    def out_extent(self, x):
+        """OH * OW * C_out: the floats one image of input x (fp32 NCHW, or the codes of a codes_in layer) gives."""
+        H, W = (x.shape[1], x.shape[2]) if self.codes_in else (x.shape[2], x.shape[3])
+        g = self._geometry(1, int(H), int(W))
+        return int(g[0]["OH"]) * int(g[0]["OW"]) * self.out_channels
+
+    def _run_rows(self, xq, out, off, g, N, OH, OW):
+        e, n = self.epilogue, OH * OW * self.out_channels
+        if out is None:
+            out, off = torch.empty((N, OH * OW, self.out_channels), dtype=torch.float32, device=xq.device), 0
+        elif not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.dim() < 2 or out.shape[0] != N or \
+                out.device != xq.device or not out.is_contiguous():
+            raise _lib.DfqError("layer %s: the rows' tensor must be contiguous fp32 [%d, ...] on %s, got %s" % (
+                self._who(), N, xq.device, "%s %s on %s" % (out.dtype, list(out.shape), out.device)
+                if isinstance(out, torch.Tensor) else type(out).__name__))
+        if not 0 <= off <= out[0].numel() - n:
+            raise _lib.DfqError("layer %s: rows [%d, %d) do not fit in the %d floats of an image"
+                                % (self._who(), off, off + n, out[0].numel()))
+        d = np.zeros(1, _lib.I8_EPILOGUE_DT)
+        d[0] = (0, out.data_ptr(), 0, 0.0) + e.pre + e.post
+        _lib.check(_lib.load().dfq_i8_conv_nhwc(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                                _lib.table_ptr(d), int(off), out[0].numel(), _lib.table_ptr(g),
+                                                _lib.stream_ptr()), "dfq_i8_conv_nhwc (layer %s)" % self._who())
+        return out
+
     def _run_fused(self, xq, r, g, N, OH, OW):
         e = self.epilogue
         shape = (N, self.out_channels, OH, OW)
@@ -283,8 +323,8 @@ class Int8Conv2d(_Int8Layer):
                                 % (conv.padding, conv.padding_mode))
         return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
 
-    def forward(self, x, r=None, out=None):
-        return self.run(x, residual=r, out=out)[0]
+    def forward(self, x, r=None, out=None, off=0):
+        return self.run(x, residual=r, out=out, off=off)[0]
 
     def extra_repr(self):
         return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act_scale=%g" % (
@@ -421,6 +461,39 @@ class Int8UpsampleBilinear(nn.Module):
     def extra_repr(self):
         return "channels=%d, align_corners=%s, out_scale=%g, clamp=%s, out_slice=%s" % (
             self.channels, self.align_corners, self.out_scale, self.clamp, self.out_slice)
+
+
+class Int8HeadConcat(nn.Module):
+    """torch.cat(..., 1) of detection heads laid out as `conv(x_i).permute(0, 2, 3, 1).contiguous().view(N, -1, k)` in a
+    chained model: each head (a rows-mode Int8Conv2d, _Int8Layer.chained(rows=True)) writes its pixel-major fp32 output
+    straight into its slice of one [N, R, k] tensor (dfq_i8_conv_nhwc), in order.  R and the offsets follow from the inputs'
+    sizes when the module runs.  batch: the view's constant N (None: the input's batch), checked."""
+
+    def __init__(self, heads, k, batch=None, name=None):
+        super().__init__()
+        self.heads = nn.ModuleList(heads)
+        self.k, self.batch, self.layer_name = int(k), None if batch is None else int(batch), name
+
+    def forward(self, *xs):
+        if len(xs) != len(self.heads):
+            raise _lib.DfqError("head concatenation %s takes %d inputs, got %d" % (self.layer_name, len(self.heads), len(xs)))
+        N = int(xs[0].shape[0])
+        if any(int(x.shape[0]) != N for x in xs) or (self.batch is not None and self.batch != N):
+            raise _lib.DfqError("head concatenation %s: inputs of batch %s do not match the view's batch %s"
+                                % (self.layer_name, [int(x.shape[0]) for x in xs], self.batch or N))
+        ext = [h.out_extent(x) for h, x in zip(self.heads, xs)]
+        if any(e % self.k for e in ext):
+            raise _lib.DfqError("head concatenation %s: head outputs of %s floats per image do not view as rows of %d"
+                                % (self.layer_name, ext, self.k))
+        out = torch.empty((N, sum(ext) // self.k, self.k), dtype=torch.float32, device=xs[0].device)
+        off = 0
+        for h, x, e in zip(self.heads, xs, ext):
+            h(x, out=out, off=off)
+            off += e
+        return out
+
+    def extra_repr(self):
+        return "k=%d, batch=%s" % (self.k, self.batch)
 
 
 def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
@@ -620,7 +693,158 @@ def _cat_operands(node):
     return list(ops)
 
 
-def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False, upsample=False) -> fx.GraphModule:
+def _zero_pad(node):
+    """(t, l) of an F.pad node that zero-pads one fx node symmetrically: pad (l, r) or (l, r, t, b) with l == r >= 0 and
+    t == b >= 0, mode 'constant', value 0 or None; None otherwise."""
+    if node.op != "call_function" or node.target not in (F.pad, torch._C._nn.pad) or len(node.all_input_nodes) != 1 or \
+            not node.args or not isinstance(node.args[0], fx.Node) or set(node.kwargs) - {"pad", "mode", "value"}:
+        return None
+    pad, mode, value = _arg(node, 1, "pad", None), _arg(node, 2, "mode", "constant"), _arg(node, 3, "value", None)
+    if not isinstance(pad, (tuple, list)) or len(pad) not in (2, 4) or \
+            not all(isinstance(v, int) and not isinstance(v, bool) for v in pad):
+        return None
+    l, r, t, b = (tuple(pad) + (0, 0))[:4]
+    if l != r or t != b or l < 0 or t < 0 or mode != "constant" or not (value is None or (
+            isinstance(value, (int, float)) and not isinstance(value, bool) and value == 0)):
+        return None
+    return t, l
+
+
+def _fold_pads(gm, mods, conv):
+    """Rule (a) of chain_int8(layout=True): fold each qualifying zero F.pad into its only user, an Int8Conv2d."""
+    folded = []
+    for node in list(gm.graph.nodes):
+        tl = _zero_pad(node)
+        if tl is None or len(node.users) != 1:
+            continue
+        q = next(iter(node.users))
+        if not conv(q) or q.args != (node,) or q.kwargs:
+            continue
+        m = mods[q.target]
+        new = m.chained(name=q.target)
+        new.padding = (m.padding[0] + tl[0], m.padding[1] + tl[1])
+        parent, _, attr = q.target.rpartition(".")
+        setattr(gm.get_submodule(parent) if parent else gm, attr, new)
+        mods[q.target] = new
+        q.args = (node.args[0],)
+        gm.graph.erase_node(node)
+        folded.append((node.name, q.target, tl))
+    return folded
+
+
+def _head_operand(view, conv, mods):
+    """(producer, clamp, nodes to delete, k, constant N or None) of a cat operand `view(N, -1, k)` / `reshape` of
+    [`.contiguous()` of] `.permute(0, 2, 3, 1)` of an Int8Conv2d producer's single-user pass-through chain; None otherwise.
+    N is a constant or a dim-0 shape query (.size(0), .shape[0], .size()[0]) of a node on that path, used only by the view."""
+    if view.op != "call_method" or view.target not in ("view", "reshape") or view.kwargs or len(view.args) < 2 or \
+            not isinstance(view.args[0], fx.Node) or len(view.users) != 1:
+        return None
+    sizes = view.args[1] if len(view.args) == 2 and isinstance(view.args[1], (tuple, list)) else view.args[1:]
+    if len(sizes) != 3 or sizes[1] != -1 or not isinstance(sizes[2], int) or isinstance(sizes[2], bool) or sizes[2] <= 0:
+        return None
+    n, k = sizes[0], sizes[2]
+    path, node = [view], view.args[0]
+    if node.op == "call_method" and node.target == "contiguous" and len(node.args) == 1 and not node.kwargs:
+        path.append(node)
+        node = node.args[0]
+    if not (node.op == "call_method" and node.target == "permute" and not node.kwargs and isinstance(node.args[0], fx.Node)
+            and tuple(node.args[1:] if len(node.args) == 5 else (node.args[1] if len(node.args) == 2 else ())) == (0, 2, 3, 1)):
+        return None
+    path.append(node)
+    node, clamp = node.args[0], (-_INF, _INF)
+    while not conv(node):
+        c = _pass_through(node, mods)
+        if c is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
+            return None
+        clamp = _compose(c, clamp)
+        path.append(node)
+        node = node.args[0]
+    if len(node.args) != 1 or node.kwargs or not isinstance(node.args[0], fx.Node):
+        return None
+    path.append(node)
+
+    def query_nodes(u, n):
+        """[u, ...] when u reads a shape of n and everything it feeds ends at the view; None otherwise."""
+        if u.op == "call_method" and u.target == "size" and u.args[0] is n and not u.kwargs and len(u.args) <= 2:
+            pass
+        elif u.op == "call_function" and u.target is getattr and u.args == (n, "shape"):
+            pass
+        else:
+            return None
+        if u.users.keys() == {view}:
+            return [u]
+        if all(g.op == "call_function" and g.target is operator.getitem and g.users.keys() == {view} for g in u.users):
+            return [u, *u.users]
+        return None
+
+    queries = []
+    for a, b in zip(path[1:], path):                            # every node but the view: the next node and shape queries
+        for u in a.users:
+            if u is b:
+                continue
+            qn = query_nodes(u, a)
+            if qn is None:
+                return None
+            queries += qn
+    if isinstance(n, fx.Node):
+        base = n.args[0] if n.op == "call_function" and n.target is operator.getitem else None
+        dim0 = (n.op == "call_method" and n.target == "size" and n.args[1:] == (0,)) or \
+            (base is not None and n.args[1] == 0 and base.op in ("call_method", "call_function") and
+             (base.target == "size" and len(base.args) == 1 or base.target is getattr))
+        if n not in queries or not dim0:
+            return None
+        n = None
+    elif not isinstance(n, int) or isinstance(n, bool) or n <= 0:
+        return None
+    if any(q.users.keys() - {view} - set(queries) for q in queries):
+        return None
+    return dict(p=node, clamp=clamp, path=path + queries, k=k, batch=n)
+
+
+def _fuse_heads(gm, conv, mods):
+    """Rule (b) of chain_int8(layout=True): detection-head concatenations written in place by their producers."""
+    plans = []
+    for c in gm.graph.nodes:
+        if c.op != "call_function" or c.target not in (torch.cat, torch.concat) or set(c.kwargs) - {"tensors", "dim"}:
+            continue
+        ops, dim = _arg(c, 0, "tensors", None), _arg(c, 1, "dim", 0)
+        if dim != 1 or not isinstance(ops, (list, tuple)) or len(ops) < 2 or not all(isinstance(o, fx.Node) for o in ops) \
+                or len(set(ops)) != len(ops):
+            continue
+        heads = [_head_operand(o, conv, mods) for o in ops]
+        if any(h is None for h in heads) or len({h["k"] for h in heads}) != 1 or len({h["p"] for h in heads}) != len(heads) \
+                or len({h["batch"] for h in heads} - {None}) > 1:
+            continue
+        plans.append((c, heads, next((h["batch"] for h in heads if h["batch"] is not None), None)))
+    g, fused = gm.graph, []
+    for c, heads, batch in plans:
+        layers = []
+        for h in heads:
+            p = h["p"]
+            layer = gm.get_submodule(p.target).chained(codes_in=gm.get_submodule(p.target).codes_in, name=p.target,
+                                                      epilogue=Epilogue(None, h["clamp"], fp32=True), rows=True)
+            parent, _, attr = p.target.rpartition(".")
+            setattr(gm.get_submodule(parent) if parent else gm, attr, layer)
+            layers.append(layer)
+        name = "int8_heads_" + c.name
+        gm.add_submodule(name, Int8HeadConcat(layers, heads[0]["k"], batch, name=c.name))
+        with g.inserting_before(c):
+            node = g.call_module(name, tuple(h["p"].args[0] for h in heads))
+        c.replace_all_uses_with(node)
+        g.erase_node(c)
+        dead = {n for h in heads for n in h["path"]}
+        while dead:                                             # each node goes once nothing uses it
+            for n in [n for n in dead if not n.users]:
+                g.erase_node(n)
+                dead.discard(n)
+        fused.append((c.name, [h["p"].target for h in heads], heads[0]["k"]))
+    g.lint()
+    gm.recompile()
+    return fused
+
+
+def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False, upsample=False,
+               layout=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` computes, with activations kept in int8 between converted
     convolutions.
 
@@ -690,7 +914,27 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     Any other upsample stays in torch, fp32, as does anything not listed (nearest or bicubic modes, scale_factor,
     adaptive average pools).  `fused_upsamples` records (node name, producer name, "slice" or "codes", align_corners) in
     graph order; edges whose codes come out of a fused upsample name it as the producer.  upsample=True without
-    pool_cat=True raises DfqError."""
+    pool_cat=True raises DfqError.
+
+    layout=True (with upsample=True) also removes the layout copies around converted convolutions, bit-identical to the
+    per-layer path (no exceptions):
+    (a) zero padding: an F.pad node of one fx node with constant arguments - pad (l, r) or (l, r, t, b), l == r >= 0,
+        t == b >= 0, mode 'constant', value 0 or None - whose only user is a single-site Int8Conv2d taking it as its sole
+        argument is folded into that convolution: it becomes a copy on the same packed buffers with padding + (t, l), on the
+        pad's input, and the pad is deleted.  The per-layer path quantizes the padded zeros to code 0, which is what the
+        convolution's out-of-image taps read, so the int32 sums are the same (DeepLab-v3+'s fixed_padding before each
+        inverted residual block; in front of a 1x1 convolution too).  This runs before every other rule, which then see a
+        direct edge.  Any other pad (asymmetric, negative, reflect / replicate, non-zero, several users, not in front of an
+        Int8Conv2d, nn.ZeroPad2d) stays in torch.  `folded_pads` records (pad node name, conv name, (t, l)) in graph order.
+    (b) detection heads: a torch.cat / torch.concat along dim 1 of >= 2 distinct nodes, without out, each of them
+        `view` / `reshape`(N, -1, k) (N a constant, or a dim-0 shape query - .size(0), .shape[0] - of the path below, used
+        only by the view; one k for all) of an optional `.contiguous()` of `.permute(0, 2, 3, 1)` of a single-site Int8Conv2d
+        producer's single-user pass-through chain (SSD's compute_header).  The producers write their clamped fp32 output
+        pixel-major into their slices of one [N, R, k] tensor per forward (dfq_i8_conv_nhwc), run in operand order at the
+        cat's position (Int8HeadConcat), R and the offsets following from the inputs' sizes at run time; the cat becomes
+        that tensor for its users, and the views, permutes, shape queries and pass-throughs are deleted.  If one operand
+        does not qualify the cat stays in torch.  `fused_heads` records (cat node name, producer names, k).
+    layout=True without upsample=True raises DfqError."""
     tracer = _Int8Tracer()
     graph = tracer.trace(model, concrete_args)
     gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
@@ -707,8 +951,15 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
         raise _lib.DfqError("chain_int8: pool_cat=True builds on residual=True")
     if upsample and not pool_cat:
         raise _lib.DfqError("chain_int8: upsample=True builds on pool_cat=True")
+    if layout and not upsample:
+        raise _lib.DfqError("chain_int8: layout=True builds on upsample=True")
+    folded = _fold_pads(gm, mods, conv) if layout else None
     if residual:
-        return _chain_residual(gm, mods, conv, pool_cat, upsample)
+        gm = _chain_residual(gm, mods, conv, pool_cat, upsample)
+        if layout:
+            gm.folded_pads = folded
+            gm.fused_heads = _fuse_heads(gm, conv, mods)
+        return gm
 
     edges, between = [], []
     for q in list(gm.graph.nodes):

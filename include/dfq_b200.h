@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 9
+#define DFQ_ABI_VERSION 10
 
 enum {
   DFQ_OK = 0,
@@ -457,6 +457,18 @@ int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float* dq, const
  * residual or y that overlaps the slice's extent or each other, and the epilogue refusals of dfq_i8_conv_fused. */
 int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
                       int32_t coff, int32_t cstride, const DfqI8Conv* g, void* stream);
+
+/* The convolution's fp32 output in pixel-major rows, for detection heads whose outputs are permuted to [N, OH, OW, O] and
+ * concatenated along the anchors (`permute(0, 2, 3, 1).contiguous().view(N, -1, k)` then `torch.cat(..., 1)`):
+ *   v = clamp(clamp(fp32(fp32_rn(acc) * dq[o]) + bias[o], pre), post)      as dfq_i8_conv_fused computes it
+ *   e->y[n * img_stride + off + p * O + o] = v                             p = oh * OW + ow
+ * Each image's OH * OW * O floats start at `off` inside its img_stride floats, so rows [off / k, off / k + OH * OW * O / k) of
+ * an [N, R, k] tensor (img_stride = R * k) are this layer's slice of the concatenation; nothing else of y is written.  Only
+ * e->y and the two clamps of *e are used.  DFQ_E_ARG, with a reason: y NULL or not 4-byte aligned, residual or yq not NULL,
+ * off < 0, img_stride < off + OH * OW * O, NaN or unordered bounds in either clamp, y's extent overlapping xq.  Grouping
+ * as dfq_i8_conv. */
+int dfq_i8_conv_nhwc(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
+                     int64_t off, int64_t img_stride, const DfqI8Conv* g, void* stream);
 
 /* Max pooling, with torch's geometry (F.max_pool2d: zero-free padding, dilation, ceil_mode). */
 typedef struct DfqI8Pool {

@@ -12,8 +12,11 @@ fused too), the same way, with the fused adds.  `pool_cat`: per-layer against ch
 chain_int8(residual=True, pool_cat=True) (max pools and channel concatenations carried in int8 too) on ResNet-18, SqueezeNet
 1.1 and GoogLeNet.  `upsample`: per-layer against chain_int8(residual=True, pool_cat=True) and chain_int8(..., upsample=True)
 (bilinear upsamples feeding concatenations carried in int8 too) on two segmentation networks at 513x513: the DeepLab-v3+-shaped
-network of tests/deeplab_v3plus_like.py and torchvision's DeepLab-v3 ResNet-50.  The card's name and power limit are read in
-the same run and reported beside the numbers.  Needs a CUDA device; writes nothing.
+network of tests/deeplab_v3plus_like.py and torchvision's DeepLab-v3 ResNet-50.  `layout`: per-layer against
+chain_int8(..., upsample=True) and chain_int8(..., layout=True) (zero pads folded into convolutions, detection heads written
+into their concatenation) on the networks of tests/deeplab_mobilenet_padded.py (8 x 513x513) and tests/ssd_lite_like.py
+(256 x 300x300).  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+device; writes nothing.
 """
 import argparse
 import json
@@ -482,6 +485,107 @@ def upsample_inference(dev, reps=10, batch=8, rounds=5, size=513):
     return out
 
 
+def layout_inference(dev, reps=10, rounds=5, seg_batch=8, ssd_batch=256):
+    """Per-layer int8 execution against chain_int8(residual=True, pool_cat=True, upsample=True) and chain_int8(...,
+    layout=True) on the DeepLab-v3+ (MobileNetV2, fixed padding) of tests/deeplab_mobilenet_padded.py at seg_batch x
+    513x513 and the MobileNetV2-SSD-Lite of tests/ssd_lite_like.py (is_test) at ssd_batch x 300x300 (seeded weights, BN
+    folded, scales 128 / max|input|), timed alternately (`rounds` rounds of `reps` passes, median): images/s, ms per batch,
+    folded pads and fused heads, carried convolution inputs, the fp32 bytes and launches the layout arm avoids against the
+    upsample arm (from the traced tensors' sizes) and bit-identity of the outputs."""
+    import statistics
+    from collections import OrderedDict
+    import torch
+    import torch.nn as nn
+    from dfq_b200 import int8
+    from dfq_b200.trace import trace_graph
+    from dfq_b200.utils.layer_transform import merge_batchnorm
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from deeplab_mobilenet_padded import DeepLabMobileNetPadded
+    from ssd_lite_like import SSDLiteLike
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def same(a, b):
+        a, b = (t if isinstance(t, tuple) else (t,) for t in (a, b))
+        return all(x.shape == y.shape and bool(torch.equal(x.view(torch.int32), y.view(torch.int32))) for x, y in zip(a, b))
+
+    out = {"unit": "images/s", "reps": reps, "rounds": rounds,
+           "avoided_note": "fp32 bytes and launches the upsample arm spends that the layout arm does not, per batch, from the "
+                           "traced tensors' sizes: per folded pad the pad's read of its input, its write and the quantizer's "
+                           "read of the padded tensor (2 launches); per fused head the contiguous copy's read and write and "
+                           "the cat's read and write of its output (1 launch, plus 1 per cat)"}
+    for net, batch, size in (("deeplab_mobilenet_padded", seg_batch, 513), ("ssd_lite", ssd_batch, 300)):
+        torch.manual_seed(0)
+        model = (DeepLabMobileNetPadded(21) if net == "deeplab_mobilenet_padded" else SSDLiteLike(21, is_test=True))
+        model = model.to(dev).eval()
+        x = torch.randn(batch, 3, size, size, device=dev)
+        graph, bottoms = trace_graph(model)
+        merge_batchnorm(model, graph, bottoms, [nn.Conv2d])
+        layers = OrderedDict((n, m) for n, m in model.named_modules() if type(m) in (nn.Conv2d, nn.Linear))
+        amax = {}
+        hooks = [m.register_forward_pre_hook(lambda m, i, n=n: amax.__setitem__(n, max(amax.get(n, 0.0), float(i[0].abs().max()))))
+                 for n, m in layers.items()]
+        with torch.no_grad():
+            model(x[:2])
+        for h in hooks:
+            h.remove()
+        int8.convert_to_int8(model, OrderedDict((id(m), m) for m in layers.values()), [nn.Conv2d, nn.Linear],
+                             act_scales=[128. / amax[n] for n in layers])
+        base = int8.chain_int8(model, residual=True, pool_cat=True, upsample=True)
+        gm = int8.chain_int8(model, residual=True, pool_cat=True, upsample=True, layout=True)
+        traced = torch.fx.GraphModule(model, int8._Int8Tracer().trace(model))
+        numel = {}
+        interp = torch.fx.Interpreter(traced)
+        run_node = interp.run_node
+
+        def record(n):
+            v = run_node(n)
+            if isinstance(v, torch.Tensor):
+                numel[n.name] = v.numel()
+            return v
+        interp.run_node = record
+        with torch.no_grad():
+            interp.run(x[:1])                                   # sizes of one image, scaled to the batch below
+            nodes = {n.name: n for n in traced.graph.nodes}
+            avoided = sum(4 * (numel[nodes[p].args[0].name] + 2 * numel[p]) for p, _, _ in gm.folded_pads)
+            launches = 2 * len(gm.folded_pads)
+            heads = {q: n.name for n in traced.graph.nodes if n.op == "call_module" for q in [n.target]}
+            for _, prods, _ in gm.fused_heads:
+                avoided += sum(16 * numel[heads[q]] for q in prods)
+                launches += len(prods) + 1
+            del interp, numel
+            ref = model(x)
+            got = {"upsample": base(x), "layout": gm(x)}
+            for _ in range(2):
+                model(x), base(x), gm(x)
+            torch.cuda.synchronize(dev)
+            ms = {"per_layer": [], "upsample": [], "layout": []}
+            for _ in range(rounds):
+                ms["per_layer"].append(timed(lambda: model(x)))
+                ms["upsample"].append(timed(lambda: base(x)))
+                ms["layout"].append(timed(lambda: gm(x)))
+        med = {k: statistics.median(v) for k, v in ms.items()}
+        out[net] = {"batch": batch, "image": "3x%dx%d" % (size, size),
+                    "images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                    "ms_per_batch_rounds": ms, "folded_pads": len(gm.folded_pads),
+                    "fused_heads": [(c, len(p), k) for c, p, k in gm.fused_heads],
+                    "carried_conv_inputs": {"upsample": len({e[1] for e in base.requantized_edges}),
+                                            "layout": len({e[1] for e in gm.requantized_edges}),
+                                            "convolutions": sum(isinstance(m, int8.Int8Conv2d) for m in model.modules())},
+                    "fp32_bytes_avoided_per_batch_vs_upsample": avoided * batch,
+                    "launches_avoided_per_forward_vs_upsample": launches,
+                    "output_bit_identical": {k: same(v, ref) for k, v in got.items()}}
+        del model, base, gm, ref, got, x
+        torch.cuda.empty_cache()
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -500,8 +604,9 @@ def main():
     p = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     p.add_argument("--batch", type=int, default=256)
     p.add_argument("--reps", type=int, default=10, help="timed forward passes per arm (after 2 warm-up passes)")
-    p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample)")
-    p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample",
+    p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
+    p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
+    p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
                    help="comma-separated sections to run (default: all)")
     args = p.parse_args()
     want = set(args.sections.split(","))
@@ -518,6 +623,8 @@ def main():
         res["pool_cat"] = pool_cat_inference(dev, reps=args.reps, batch=args.batch)
     if "upsample" in want:
         res["upsample"] = upsample_inference(dev, reps=args.reps, batch=args.seg_batch)
+    if "layout" in want:
+        res["layout"] = layout_inference(dev, reps=args.reps, seg_batch=args.seg_batch, ssd_batch=args.ssd_batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
