@@ -14,12 +14,13 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DFQ_LIB") or os.path.join(_HERE, "libdfq_sm90.so")   # DFQ_LIB: a tuning build
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 LAYER_COLS_READY = 1   # DfqLayer.flags
 LAYER_FOLD_PENDING = 2
 LAYER_ROWS_READY = 4
+ROWS_FULL, ROWS_STREAMED, ROWS_UNDECIDED, ROWS_HOST_FULL = 0, 1, 2, 3   # DfqCleResult.rows_streamed
 FOLD_FULL, FOLD_DEFER, FOLD_APPLY = 0, 1, 2   # DfqFold.mode
 BC_PREPARED = 4        # DfqBcLayer.flags
 
@@ -34,6 +35,7 @@ LAYER_DT = np.dtype([
     ("rows", np.int32), ("cols", np.int32), ("kk", np.int32),
     ("rel_in", np.int32), ("rel_out", np.int32), ("col_mode", np.int32), ("group", np.int32), ("flags", np.int32),
     ("cmin_off", np.int64), ("cmax_off", np.int64), ("fold_off", np.int64), ("rext_off", np.int64),
+    ("rext_rows", np.int32), ("_pad", np.int32),
 ], align=True)
 
 RELATION_DT = np.dtype([
@@ -53,6 +55,7 @@ CLE_PARAMS_DT = np.dtype([
 CLE_RESULT_DT = np.dtype([
     ("n_sweeps", np.int32), ("converged", np.int32), ("last_diff", np.float64),
     ("diffs", np.float64, (64,)), ("fused_sweeps", np.int32), ("bc_prepared", np.int32),
+    ("rows_streamed", np.int32), ("_pad", np.int32),
 ], align=True)
 
 FOLD_DT = np.dtype([
@@ -60,6 +63,7 @@ FOLD_DT = np.dtype([
     ("gamma_off", np.int64), ("beta_off", np.int64), ("mean_off", np.int64), ("var_off", np.int64),
     ("fake_w_off", np.int64), ("fake_b_off", np.int64),
     ("scan_go", np.int32), ("scan_gi", np.int32), ("mode", np.int32), ("scan_rows", np.int32), ("fac_off", np.int64),
+    ("row_prefix", np.int32), ("_pad", np.int32),
 ], align=True)
 
 TERM_DT = np.dtype([
@@ -95,8 +99,8 @@ I8_RESIZE_DT = np.dtype([(f, np.int32) for f in ("N", "C", "H", "W", "OH", "OW",
 
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
-    "DfqLayer": (LAYER_DT, 80), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
-    "DfqCleResult": (CLE_RESULT_DT, 536), "DfqFold": (FOLD_DT, 80), "DfqExpectTerm": (TERM_DT, 32),
+    "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
+    "DfqCleResult": (CLE_RESULT_DT, 544), "DfqFold": (FOLD_DT, 88), "DfqExpectTerm": (TERM_DT, 32),
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64), "DfqI8Resize": (I8_RESIZE_DT, 48),
 }

@@ -23,6 +23,7 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <type_traits>
 #include <cstdlib>
@@ -77,12 +78,15 @@ struct GroupState {
   int converged;
   double fuse_lb;  // k_cle_stack's fused pass: lower bound of sweep 1's metric (fuse_guard_scan)
   int fuse_moves;  // ... some channel has s2 != 1 or inv2 != 1
+  double fuse_lb_prefix;  // ... the same bound over the scanned row prefix only (fuse_guard_scan<true>)
 };
 struct CleCtl {
   int active[2];   // groups still iterating, double-buffered by sweep parity
   double diffs[64];  // diff_tmp per sweep of group 0
   int fuse_refused;  // k_cle_stack: the guard sent the launch down the per-sweep path
   int fused_sweeps;  // DfqCleResult.fused_sweeps
+  int prefix_undecided;  // k_cle_stack: some group's prefix bound does not decide the guard
+  int rows_streamed;     // DfqCleResult.rows_streamed
 };
 
 // One sweep of the exit rule of dfq.py:105-115 for one group: folds this sweep's metric `diff_tmp` into `diff` / `count`
@@ -225,6 +229,19 @@ __device__ __forceinline__ void publish_row(const RowCtx& c, const DfqCleParams 
     __stcg(c.own_cmin_wr + o, __fmul_rn(q.o0, s));
     __stcg(c.own_cmax_wr + o, __fmul_rn(q.o1, s));
   }
+}
+
+// What fetch_row_pub would read right after publish_row(c, P, o, s, ...) - the operands of the NEXT sweep's bookkeeping of
+// the same row, without another round trip to memory.  For a layer without an in-relation only (its own column extrema are
+// double-buffered, and the next sweep reads the other buffer).
+__device__ __forceinline__ RowPub row_pub_after(const RowCtx& c, const DfqCleParams P, float s, const RowPub& q) {
+  RowPub n;
+  n.a0 = P.apply_only ? 1.f : c.first_sweep ? s : __fmul_rn(q.a0, s);
+  n.b0 = __fmul_rn(q.b0, s);
+  n.w0 = c.bnw ? __fmul_rn(q.w0, s) : 0.f;
+  n.w1 = c.bnb ? __fmul_rn(q.w1, s) : 0.f;
+  n.o0 = n.o1 = 0.f;
+  return n;
 }
 
 // What a row needs from global memory, fetched ahead of the row by whoever can hide the latency (producer warp for
@@ -1167,12 +1184,11 @@ __device__ __forceinline__ float stack_scale_cols(uint32_t a0, int n4, const flo
   return dsum;
 }
 
-// One first-layer row of n4 float4 at shared address a0 (dfq.py:48-73): range -> s (*sv, *iv) -> rescale in place.
-// `in`: the row's column extrema of the pair.  Returns this lane's sum of |new - old|.
+// The extrema of one row of n4 float4 at shared address a0 (folded as read), in every lane of the warp.  The same min / max
+// reduction as the fold's row scan (passes.cu rowscan_tile): min and max are exact, so the extrema are the scan's.
 template <bool FOLD>
-__device__ __forceinline__ float stack_scale_row(uint32_t a0, int n4, const DfqCleParams& P, const RowIn& in, float fo, int lane,
-                                                 float* sv, float* iv) {
-  float mn = DFQ_INF, mx = -DFQ_INF;
+__device__ __forceinline__ void stack_row_extrema(uint32_t a0, int n4, float fo, int lane, float& mn, float& mx) {
+  mn = DFQ_INF; mx = -DFQ_INF;
 #pragma unroll 4
   for (int i4 = lane; i4 < n4; i4 += 32) {
     float4 v = lds_f4(a0 + 16u * i4);
@@ -1180,6 +1196,15 @@ __device__ __forceinline__ float stack_scale_row(uint32_t a0, int n4, const DfqC
     minmax4(mn, mx, v);
   }
   mn = warp_min(mn); mx = warp_max(mx);
+}
+
+// One first-layer row of n4 float4 at shared address a0 (dfq.py:48-73): range -> s (*sv, *iv) -> rescale in place.
+// `in`: the row's column extrema of the pair.  Returns this lane's sum of |new - old|.
+template <bool FOLD>
+__device__ __forceinline__ float stack_scale_row(uint32_t a0, int n4, const DfqCleParams& P, const RowIn& in, float fo, int lane,
+                                                 float* sv, float* iv) {
+  float mn, mx;
+  stack_row_extrema<FOLD>(a0, n4, fo, lane, mn, mx);
   const float s = solve_row(P, in, mn, mx, iv);
   *sv = s;
   float dsum = 0.f;
@@ -1222,9 +1247,16 @@ __device__ __forceinline__ double fuse_term_bound(float mn, float mx, float s) {
   return (t > 0.0 && t < 1e300) ? t : 0.0;
 }
 
+// Rows of a first layer whose extrema the fold scanned (DfqLayer.rext_rows)
+__host__ __device__ inline int rext_rows(const DfqLayer& l) { return l.rext_rows > 0 && l.rext_rows < l.rows ? l.rext_rows : l.rows; }
+
 // Phase 1 of the guard, a CTA per first layer: per group the lower bound of sweep 1's metric (GroupState.fuse_lb) and whether
 // any channel has s2 != 1 or inv2 != 1 (.fuse_moves); a launch-wide refusal when some s1 is not finite and > 0 (the
 // monotonicity needs s1 > 0; only a user-set s_range can break it).
+// PREFIX: the bound over the scanned rows only (.fuse_lb_prefix).  Every channel's term is >= 0, so the sum over any subset
+// of channels is a lower bound of the metric as well; the other two clauses need every channel and are not evaluated (the
+// host takes this path only for an s_range that keeps every s1 finite and > 0).
+template <bool PREFIX>
 __device__ __noinline__ void fuse_guard_scan(const float* arena, const DfqLayer* L, const DfqRelation* R, const int* step_ptr,
                                              const int* step_layers, const DfqCleParams P, CleCtl* ctl, GroupState* G) {
   const int lane = threadIdx.x & 31;
@@ -1235,7 +1267,8 @@ __device__ __noinline__ void fuse_guard_scan(const float* arena, const DfqLayer*
     const double n1 = (double)l.rows * l.cols * l.kk, n2 = (double)l2.rows * l2.cols * l2.kk;
     double lb = 0.0;
     bool bad = false, moves = false;
-    for (int o = threadIdx.x; o < l.rows; o += blockDim.x) {
+    const int nr = PREFIX ? rext_rows(l) : l.rows;
+    for (int o = threadIdx.x; o < nr; o += blockDim.x) {
       const float rmn = __ldcg(arena + l.rext_off + o), rmx = __ldcg(arena + l.rext_off + l.rows + o);
       const float cmn = __ldcg(arena + l2.cmin_off + o), cmx = __ldcg(arena + l2.cmax_off + o);
       const FuseScales f = fuse_scales(P, rmn, rmx, cmn, cmx);
@@ -1244,6 +1277,10 @@ __device__ __noinline__ void fuse_guard_scan(const float* arena, const DfqLayer*
       lb += fuse_term_bound(rmn, rmx, f.s1) / n1 + fuse_term_bound(cmn, cmx, f.inv1) / n2;
     }
     lb = warp_sum(lb);
+    if (PREFIX) {
+      if (lane == 0 && lb > 0.0) atomicAdd(&G[l.group].fuse_lb_prefix, lb);
+      continue;
+    }
     bad = __any_sync(0xffffffffu, bad);
     moves = __any_sync(0xffffffffu, moves);
     if (lane == 0) {
@@ -1263,6 +1300,43 @@ __device__ __noinline__ void fuse_guard_scan(const float* arena, const DfqLayer*
 __device__ __forceinline__ void fuse_guard_groups(const GroupState* G, int nG, CleCtl* ctl, const DfqCleParams& P) {
   for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < nG; g += gridDim.x * blockDim.x)
     if (!(G[g].fuse_lb > 2.0 * P.converge_thres) && G[g].fuse_moves) atomicOr(&ctl->fuse_refused, 1);
+}
+// ... from the row prefix: a group passes when its partial bound alone exceeds 2x converge_thres.  Any other group leaves
+// the launch undecided: the remaining rows are scanned (complete_rows) and the guard above decides as with a full scan.
+__device__ __forceinline__ void fuse_prefix_groups(const GroupState* G, int nG, CleCtl* ctl, const DfqCleParams& P) {
+  for (int g = blockIdx.x * blockDim.x + threadIdx.x; g < nG; g += gridDim.x * blockDim.x)
+    if (!(G[g].fuse_lb_prefix > 2.0 * P.converge_thres)) atomicOr(&ctl->prefix_undecided, 1);
+}
+
+// The row extrema the fold did not scan (rows [rext_rows, rows) of every first layer that arrived with a prefix), a warp per
+// row over the whole grid, read-only: the values the fold's scan would have written (fl(w * f) with a pending fold, the
+// reduction of stack_row_extrema).  The rows of all layers are dealt out as one list so that every warp gets a share.
+__device__ __noinline__ void complete_rows(float* arena, const DfqLayer* L, const int* step_ptr, const int* step_layers) {
+  const int lane = threadIdx.x & 31;
+  const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+  const long long gw = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  long long base = 0;   // rows of the earlier layers in the list
+  for (int q = step_ptr[0]; q < step_ptr[1]; ++q) {
+    const DfqLayer l = L[step_layers[q]];
+    if (!(l.flags & DFQ_LAYER_ROWS_READY)) continue;
+    const int p0 = rext_rows(l), rem = l.rows - p0, n4 = (l.cols * l.kk) >> 2;
+    if (rem <= 0) continue;
+    const float* fold = (l.flags & DFQ_LAYER_FOLD_PENDING) ? arena + l.fold_off : nullptr;
+    for (long long i = base + (((gw - base) % nw) + nw) % nw; i < base + rem; i += nw) {
+      const int o = p0 + (int)(i - base);
+      const float4* row = (const float4*)(arena + l.w_off + (size_t)o * (n4 * 4));
+      const float fo = fold ? __ldcg(fold + o) : 1.f;
+      float mn = DFQ_INF, mx = -DFQ_INF;
+      for (int i4 = lane; i4 < n4; i4 += 32) {
+        float4 v = ldg_stream(row + i4);
+        if (fold) v = mul4(v, fo);
+        minmax4(mn, mx, v);
+      }
+      mn = warp_min(mn); mx = warp_max(mx);
+      if (lane == 0) { __stcg(arena + l.rext_off + o, mn); __stcg(arena + l.rext_off + l.rows + o, mx); }
+    }
+    base += rem;
+  }
 }
 
 // Phase 3 (the guard passed): the per-channel bookkeeping of sweeps 1 and 2 (publish_row twice, in the reference's order:
@@ -1348,62 +1422,97 @@ struct StackBc {
 };
 
 // fuse: the host found every first layer DFQ_LAYER_ROWS_READY, converge_count >= 2 and max_sweeps != 1; the guard decides.
+// rows_mode: how complete those row extrema are (DfqLayer.rext_rows): ROWS_COMPLETE every row's; ROWS_PREFIX some layers
+// hold a prefix and the guard may decide from it (fuse, and an s_range that keeps every s1 finite and > 0); ROWS_SCAN_FIRST
+// some layers hold a prefix that the guard may not use: the remaining rows are scanned before anything else.
+enum { ROWS_COMPLETE = 0, ROWS_PREFIX = 1, ROWS_SCAN_FIRST = 2 };
 __global__ void __launch_bounds__(kBcThreads, 1)
 k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelation* __restrict__ R, int nR,
             const int* __restrict__ step_ptr, const int* __restrict__ step_layers, const long long* __restrict__ pass_ptr,
-            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG, int fuse, StackBc bc) {
+            DfqCleParams P, CleCtl* ctl, GroupState* G, int nG, int fuse, int rows_mode, StackBc bc) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(128) unsigned char ring_smem[];
   __shared__ RowCtx wctx[kBcConsumers];
+  __shared__ RowCtx wctx1[kStackConsumers];   // STREAM: the context of sweep 2 of the layer in hand
   BcRing ring;
   ring.init(ring_smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool producer = (warp == kBcConsumers);
   unsigned long long n = producer ? 0 : (unsigned long long)warp;       // (warps >= kStackConsumers never use it)
   groups_init(G, nG, threadIdx.x, kBcThreads);
-  if (fuse) fuse_guard_scan(arena, L, R, step_ptr, step_layers, P, ctl, G);
+  if (rows_mode == ROWS_SCAN_FIRST) complete_rows(arena, L, step_ptr, step_layers);
+  else if (rows_mode == ROWS_PREFIX) fuse_guard_scan<true>(arena, L, R, step_ptr, step_layers, P, ctl, G);
+  else if (fuse) fuse_guard_scan<false>(arena, L, R, step_ptr, step_layers, P, ctl, G);
   __threadfence();
   grid.sync();
-  bool fused = false;
-  if (fuse) {
+  // stream: the prefix decided the guard for every group - the fused pass derives the first layers' row extrema, scales and
+  // bookkeeping row by row as it holds the rows (no fuse_publish).  Otherwise every row's extrema are known before the guard.
+  bool stream = false;
+  if (rows_mode == ROWS_PREFIX) {
+    fuse_prefix_groups(G, nG, ctl, P);
+    __threadfence();
+    grid.sync();
+    stream = *((volatile int*)&ctl->prefix_undecided) == 0;
+    if (!stream) {
+      complete_rows(arena, L, step_ptr, step_layers);
+      __threadfence();
+      grid.sync();
+    }
+  }
+  if (fuse && !stream && rows_mode != ROWS_COMPLETE) {
+    fuse_guard_scan<false>(arena, L, R, step_ptr, step_layers, P, ctl, G);
+    __threadfence();
+    grid.sync();
+  }
+  bool fused = stream;
+  if (fuse && !stream) {
     fuse_guard_groups(G, nG, ctl, P);
     __threadfence();
     grid.sync();
     fused = *((volatile int*)&ctl->fuse_refused) == 0;
     if (fused) {
       fuse_publish(arena, L, R, step_ptr, step_layers, P);
-      if (blockIdx.x == 0 && threadIdx.x == 0) ctl->fused_sweeps = 2;
       __threadfence();
       grid.sync();
-      // Attached correction, what k_bc_stream does before its row phase, a CTA per entry: the per-tensor range from the
-      // column extrema of sweep 2 (buffer 0, the one cle_col_hints names for a group that stops there; reduced as k_bc_stream
-      // reduces such a hint), then E[x] from the BN vectors fuse_publish has just scaled.  Both hold for the final state
-      // only when every group stops after sweep 2 - the host uses the deltas only then (DfqCleResult.bc_prepared).
-      if (bc.n > 0) {
-        for (int bi = blockIdx.x; bi < bc.n; bi += gridDim.x) {
-          const DfqBcLayer b = bc.B[bi];
-          if (warp == 0) {
-            const DfqLayer l = L[b.layer];
-            float mn = DFQ_INF, mx = -DFQ_INF;
-            for (int j = lane; j < l.cols; j += 32) {
-              mn = fminf(mn, __ldcg(arena + l.cmin_off + j)); mx = fmaxf(mx, __ldcg(arena + l.cmax_off + j));
-            }
-            mn = warp_min(mn); mx = warp_max(mx);
-            if (lane == 0) { __stcg(arena + b.minmax_off, mn); __stcg(arena + b.minmax_off + 1, mx); }
-          }
-          bc_expect<kBcThreads, false>(arena, b, bc.T, arena + b.expect_off);
-        }
-        __threadfence();
-        grid.sync();
-      }
     }
   }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (fused) ctl->fused_sweeps = 2;
+    ctl->rows_streamed = rows_mode == ROWS_COMPLETE ? DFQ_ROWS_FULL : rows_mode == ROWS_SCAN_FIRST ? DFQ_ROWS_HOST_FULL
+                       : stream ? DFQ_ROWS_STREAMED : DFQ_ROWS_UNDECIDED;
+  }
 
-  // One pass over the weights: sweep `sweep`, or with FUSED sweeps 0 and 1 (metric terms into acc[0] and acc[1]).
-  auto pass = [&](auto fused_tag, int sweep) {
+  // Attached correction, what k_bc_stream does before its row phase, a CTA per entry: the per-tensor range from the column
+  // extrema of sweep 2 (buffer 0, the one cle_col_hints names for a group that stops there; reduced as k_bc_stream reduces such
+  // a hint), then E[x] from the BN vectors scaled by both sweeps.  The fused pass's first step writes both (in-stream, or
+  // fuse_publish before it), so this runs between its two steps.  Both hold for the final state only when every group stops
+  // after sweep 2 - the host uses the deltas only then (DfqCleResult.bc_prepared).
+  auto bc_setup = [&]() {
+    for (int bi = blockIdx.x; bi < bc.n; bi += gridDim.x) {
+      const DfqBcLayer b = bc.B[bi];
+      if (warp == 0) {
+        const DfqLayer l = L[b.layer];
+        float mn = DFQ_INF, mx = -DFQ_INF;
+        for (int j = lane; j < l.cols; j += 32) {
+          mn = fminf(mn, __ldcg(arena + l.cmin_off + j)); mx = fmaxf(mx, __ldcg(arena + l.cmax_off + j));
+        }
+        mn = warp_min(mn); mx = warp_max(mx);
+        if (lane == 0) { __stcg(arena + b.minmax_off, mn); __stcg(arena + b.minmax_off + 1, mx); }
+      }
+      bc_expect<kBcThreads, false>(arena, b, bc.T, arena + b.expect_off);
+    }
+    __threadfence();
+    grid.sync();
+  };
+
+  // One pass over the weights: sweep `sweep`, or with FUSED sweeps 0 and 1 (metric terms into acc[0] and acc[1]); STREAM (with
+  // FUSED): the first layers' scales come from the rows in the stage, not from fuse_publish.
+  auto pass = [&](auto fused_tag, auto stream_tag, int sweep) {
     constexpr bool FUSED = decltype(fused_tag)::value;
+    constexpr bool STREAM = FUSED && decltype(stream_tag)::value;
     const int slot = sweep % 3;
     for (int p = 0; p < 2; ++p) {
+      if (FUSED && p == 1 && bc.n > 0) bc_setup();
       if (producer) {
         if (lane == 0) {
           PassIter it;
@@ -1414,7 +1523,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
         RowCtx& c = wctx[warp];
         float* inv_s = ring.ex_cache(warp);            // reciprocal scales of the current second layer's columns (+ sentinel)
         float* inv1_s = ring.ex_cache(kBcConsumers + warp);   // FUSED: those of sweep 1 (inv_s: sweep 2)
-        const float* rext = nullptr;                   // FUSED, first layer: s1 per row (fuse_publish)
+        float* rext = nullptr;                         // FUSED, first layer: s1 per row (fuse_publish; STREAM: written here)
         // FUSED, a second layer with an attached correction: its entry (bc_mode -1: none), quantizer and E[x] cache
         float* bc_ex = ring.ex_cache(stack_ex_slot(warp));
         float* bc_delta = nullptr;
@@ -1447,7 +1556,10 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
             const int g = L[cur_li].group;
             if (g != cur_g) { flush_metric(); cur_g = g; }
             __syncwarp();
-            if (lane == 0) make_ctx(c, arena, L, R, cur_li, sweep);
+            if (lane == 0) {
+              make_ctx(c, arena, L, R, cur_li, sweep);
+              if (STREAM) make_ctx(wctx1[warp], arena, L, R, cur_li, sweep + 1);
+            }
             __syncwarp();
             kk = c.kk;
             if (c.inv_in) {
@@ -1481,13 +1593,35 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           const uint32_t sbase = smem_u32(ring.stage(s));
           const double inv_n = c.inv_n;
           RowIn mine;
-          float ks = 1.f, kinv = 1.f;
+          RowPub pub;
+          float ks = 1.f, kinv = 1.f, ks2 = 1.f, kinv2 = 1.f;
           const bool has_out = c.has_out != 0;
           // first sweep with the BN fold pending: lane r fetches row r's fold factor
           const float* fold = c.fold;
           float fo_mine = 1.f;
           if (fold && lane < d.nrows) fo_mine = __ldcg(fold + d.row0 + lane);
-          if (FUSED && has_out) {
+          if (STREAM && has_out) {
+            // ---- first layer, sweeps 1 and 2: the row's extrema from the stage (folded as read), then its scales --------
+            if (lane < d.nrows) {
+              mine = fetch_row_in(c, P, d.row0 + lane, false);     // column extrema of the pair, sweep 1
+              pub = fetch_row_pub(c, P, d.row0 + lane);            // ... and the operands of the bookkeeping, requested now
+            }
+            for (int r = 0; r < d.nrows; ++r) {
+              const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
+              const float fo = __shfl_sync(0xffffffffu, fo_mine, r);
+              const RowIn in = shfl_row_in(mine, r);
+              float mn, mx;
+              if (fold) stack_row_extrema<true>(a0, n4, fo, lane, mn, mx);
+              else stack_row_extrema<false>(a0, n4, 1.f, lane, mn, mx);
+              const FuseScales f = fuse_scales(P, mn, mx, in.cmn, in.cmx);
+              float d1 = 0.f, d2 = 0.f;
+              if (fold) stack_fused_row<true>(a0, n4, fo, f.s1, f.s2, lane, d1, d2);
+              else stack_fused_row<false>(a0, n4, 1.f, f.s1, f.s2, lane, d1, d2);
+              if (lane == r) { ks = f.s1; kinv = f.inv1; ks2 = f.s2; kinv2 = f.inv2; }
+              dacc += (double)d1 * inv_n;
+              dacc2 += (double)d2 * inv_n;
+            }
+          } else if (FUSED && has_out) {
             // ---- first layer, sweeps 1 and 2: the scales are known (fuse_publish) -------------------------------------
             float s1_mine = 1.f, s2_mine = 1.f;
             if (lane < d.nrows) { s1_mine = __ldcg(rext + d.row0 + lane); s2_mine = __ldcg(c.s_step + d.row0 + lane); }
@@ -1574,6 +1708,14 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
           // the stage is on its way back: a dozen dependent global accesses that the ring does not have to wait for
           if (!FUSED && has_out && lane < d.nrows)
             publish_row(c, P, d.row0 + lane, ks, kinv, mine.cmn, mine.cmx, fetch_row_pub(c, P, d.row0 + lane));
+          // STREAM: fuse_publish's bookkeeping of the row, lane r for row r (the operands of sweep 2's from those of sweep 1's)
+          if (STREAM && has_out && lane < d.nrows) {
+            const int o = d.row0 + lane;
+            publish_row(c, P, o, ks, kinv, mine.cmn, mine.cmx, pub);
+            publish_row(wctx1[warp], P, o, ks2, kinv2, __fmul_rn(mine.cmn, kinv), __fmul_rn(mine.cmx, kinv), row_pub_after(c, P, ks, pub));
+            __stcg(rext + o, ks);
+            __stcg(rext + c.rows + o, kinv);
+          }
         }
         flush_metric();
         if (lane == 0) { bulk_wait_all(); fence_proxy_async_all(); }
@@ -1592,13 +1734,14 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
 
   int sweep = 0;
   if (fused) {
-    pass(std::true_type{}, 0);
+    if (stream) pass(std::true_type{}, std::true_type{}, 0);
+    else pass(std::true_type{}, std::false_type{}, 0);
     exit_rule_all(0);
     if (!exit_rule_all(1)) return;
     sweep = 2;         // the state is the per-sweep run's after two sweeps; later sweeps run the per-sweep pass
   }
   for (;; ++sweep) {
-    pass(std::false_type{}, sweep);
+    pass(std::false_type{}, std::false_type{}, sweep);
     if (!exit_rule_all(sweep)) break;
   }
 }
@@ -1635,6 +1778,7 @@ static int launch_cle(const void* kernel, int grid, int threads, size_t dyn_smem
   result->last_diff = hg[0].diff;
   memcpy(result->diffs, h.diffs, sizeof(h.diffs));
   result->fused_sweeps = h.fused_sweeps;
+  result->rows_streamed = h.rows_streamed;
   // the attached correction saw the state after sweep 2: it is the final one only if no group went on
   result->bc_prepared = (bc_attached && h.fused_sweeps == 2 && all_two) ? 1 : 0;
   return 0;
@@ -1769,6 +1913,7 @@ extern "C" int dfq_cle_run_bc(float* arena, int64_t arena_floats, const DfqLayer
     if (l.rel_in >= 0 && l.rel_out >= 0) DFQ_REQUIRE(l.rel_in < l.rel_out, "relations must be in forward chain order");
     if (l.flags & DFQ_LAYER_FOLD_PENDING) DFQ_REQUIRE(l.fold_off >= 0 && l.fold_off + l.rows <= arena_floats, "fold factors outside arena");
     if (l.flags & DFQ_LAYER_ROWS_READY) DFQ_REQUIRE(l.rext_off >= 0 && l.rext_off + 2 * (int64_t)l.rows <= arena_floats, "row extrema outside arena");
+    DFQ_REQUIRE(l.rext_rows >= 0, "row prefix");
   }
   // layers whose column extrema the engine scans before the first sweep (the others arrive with buffer 0 filled)
   std::vector<int32_t> scan_layers;
@@ -1844,8 +1989,16 @@ extern "C" int dfq_cle_run_bc(float* arena, int64_t arena_floats, const DfqLayer
     // the first two sweeps in one pass (k_cle_stack's guard has the last word): every first layer's row extrema scanned by the
     // fold, and an exit rule that cannot stop after sweep 1 on the count or the sweep cap
     int fuse = params->converge_count >= 2 && params->max_sweeps != 1;
-    for (int q = step_ptr[0]; q < step_ptr[1]; ++q)
-      if (!(layers[step_layers[q]].flags & DFQ_LAYER_ROWS_READY)) fuse = 0;
+    bool prefix = false;    // some first layer arrived with the extrema of a row prefix only (DfqLayer.rext_rows)
+    for (int q = step_ptr[0]; q < step_ptr[1]; ++q) {
+      const DfqLayer& l = layers[step_layers[q]];
+      if (!(l.flags & DFQ_LAYER_ROWS_READY)) fuse = 0;
+      else prefix |= rext_rows(l) < l.rows;
+    }
+    // the guard may decide from a prefix only where every s1 is finite and > 0 whatever the rows hold: solve_scale clamps
+    // into [s_lo, s_hi] (NaN -> s_hi)
+    const bool s1_safe = params->s_lo > 0.f && std::isfinite(params->s_lo) && std::isfinite(params->s_hi);
+    int rows_mode = !prefix ? ROWS_COMPLETE : (fuse && s1_safe) ? ROWS_PREFIX : ROWS_SCAN_FIRST;
     const size_t dyn_s = kStackSmemBytes;
     if ((rc = coop_grid((const void*)k_cle_stack, "k_cle_stack", kBcThreads, dyn_s, max_tiles, &grid))) return rc;
     TablePack tp;
@@ -1867,7 +2020,8 @@ extern "C" int dfq_cle_run_bc(float* arena, int64_t arena_floats, const DfqLayer
     }
     CleCtl* dctl = nullptr; GroupState* dG = nullptr;
     DfqCleParams P = *params;
-    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups, &fuse, &sbc};
+    void* args[] = {&arena, &dL, (void*)&n_layers, &dR, (void*)&n_rels, &dSP, &dSL, &dPP, &P, &dctl, &dG, (void*)&n_groups, &fuse,
+                    &rows_mode, &sbc};
     return launch_cle((const void*)k_cle_stack, grid, kBcThreads, dyn_s, args, &dctl, &dG, tp, n_groups, result, group_sweeps, st,
                       n_bc > 0);
   }

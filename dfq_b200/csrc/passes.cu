@@ -34,11 +34,15 @@ __device__ __forceinline__ int first_tile(long long base) {
 // ------------------------------------------------------------------------------------------------
 // BN fold
 // ------------------------------------------------------------------------------------------------
+// Rows the weight pass of a fold visits: all of them, or the prefix of a row scan (DfqFold.row_prefix).
+__host__ __device__ inline int fold_rows(const DfqFold& f, int rows) {
+  return f.scan_rows && f.row_prefix > 0 && f.row_prefix < rows ? f.row_prefix : rows;
+}
 struct FoldGeo {
   float* arena; const DfqLayer* L; const DfqFold* F;
   __device__ __forceinline__ void operator()(int q, float*& base, int& rows, int& row_len) const {
     const DfqLayer l = L[F[q].layer];
-    base = arena + l.w_off; rows = l.rows; row_len = l.cols * l.kk;
+    base = arena + l.w_off; rows = fold_rows(F[q], l.rows); row_len = l.cols * l.kk;
   }
 };
 
@@ -702,6 +706,8 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
       DFQ_REQUIRE(f.mode == DFQ_FOLD_DEFER, "only DFQ_FOLD_DEFER scans rows");
       DFQ_REQUIRE(l.rext_off >= 0 && l.rext_off + 2 * (int64_t)l.rows <= arena_floats, "row scan needs the layer's row extrema scratch");
     }
+    DFQ_REQUIRE(f.row_prefix >= 0, "row prefix");
+    DFQ_REQUIRE(!f.scan_rows || f.row_prefix == 0 || f.scan_go == 0, "a row prefix is for a row scan without a column scan");
     if (f.scan_go > 0) {
       DFQ_REQUIRE(f.mode != DFQ_FOLD_APPLY, "DFQ_FOLD_APPLY does not scan");
       DFQ_REQUIRE(f.scan_gi > 0 && l.rows % f.scan_go == 0 && f.scan_gi == l.cols, "fold scan geometry (DfqRelation.go / .gi of the layer's rel_in)");
@@ -716,7 +722,7 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
         // the read-only scan folds each row in its stage: a row must fit one
         DFQ_REQUIRE(row_len <= kStageFloats, "deferred fold with a scan: rows larger than a pipe stage");
         ro.push_back(f);
-        ro_ptr.push_back(ro_ptr.back() + pipe_tiles(l.rows, row_len));
+        ro_ptr.push_back(ro_ptr.back() + pipe_tiles(fold_rows(f, l.rows), row_len));
       }
     } else {
       rw.push_back(f);

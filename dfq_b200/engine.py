@@ -11,6 +11,7 @@ that already live on the GPU.
 from __future__ import annotations
 
 import ctypes as C
+import os
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -27,6 +28,14 @@ def _default_device() -> torch.device:
     return torch.device("cuda", torch.cuda.current_device())
 
 
+# Rows of each `first` layer whose extrema a deferred fold scans (plan_bn_fold); DFQ_ROW_PREFIX overrides it, 0 = every row.
+ROW_PREFIX = 16
+
+
+def row_prefix() -> int:
+    return max(0, int(os.environ.get("DFQ_ROW_PREFIX", ROW_PREFIX)))
+
+
 def _round_up(x: int, a: int) -> int:
     return (x + a - 1) // a * a
 
@@ -41,6 +50,7 @@ class CleResult:
     apply_only: bool = False
     fused_sweeps: int = 0    # 2: k_cle_stack applied the first two sweeps in one pass (plan_bn_fold's row scan), else 0
     bc_prepared: bool = False  # the correction attached to the plan (plan_bias_correct(cle_plan=...)) was computed in that pass
+    rows_streamed: int = 0   # _lib.ROWS_*: how k_cle_stack completed the row extrema of a prefix scan (plan_bn_fold)
 
 
 @dataclass
@@ -305,7 +315,12 @@ class Session:
 
         A deferred fold also reads the plan's `first` layers and writes their row extrema (`plan["rows_scanned"]`: pairs
         (layer, offset of its [2][rows] scratch)).  With those and the column extrema, the stack kernel knows the scales of
-        the first two sweeps before it reads a weight and, where its guard allows, applies both in one pass."""
+        the first two sweeps before it reads a weight and, where its guard allows, applies both in one pass.
+
+        Only the first row_prefix() rows of each first layer are scanned (`plan["row_prefix"]`, 0 = all): their bound on
+        the first sweep's metric is enough for the stack kernel's guard on ordinary weights, and the fused pass finds the
+        other rows' extrema in the rows it holds anyway.  Where the prefix does not decide, the kernel scans the rest
+        itself; either way the scratch and the results are those of a full scan."""
         ft = np.zeros(len(folds), dtype=_lib.FOLD_DT)
         scanned = []
         for i, f in enumerate(folds):
@@ -317,6 +332,7 @@ class Session:
                     ft[i]["scan_go"] = cle_plan["rt"][ri]["go"]; ft[i]["scan_gi"] = cle_plan["rt"][ri]["gi"]
                     scanned.append(int(f["layer"]))
         deferred, rows_scanned = [], []
+        prefix = row_prefix()
         lt = cle_plan["lt"] if cle_plan is not None else self._layer_table()
         if cle_plan is not None and self._takes_stack(cle_plan, scanned):
             in_plan = set(int(x) for x in cle_plan["step_layers"])
@@ -328,11 +344,13 @@ class Session:
                     deferred.append((li, int(ft[i]["fac_off"])))
                     if lt[li]["rel_out"] >= 0 and lt[li]["rel_in"] < 0:
                         ft[i]["scan_rows"] = 1
+                        ft[i]["row_prefix"] = prefix
                         rows_scanned.append((li, self.alloc(2 * self._layers[li]["rows"])))
             if rows_scanned:
                 lt = lt.copy()
                 lt["rext_off"][[r[0] for r in rows_scanned]] = [r[1] for r in rows_scanned]
-        return dict(ft=ft, lt=lt, scanned=scanned, deferred=deferred, rows_scanned=rows_scanned, cle_plan=cle_plan)
+        return dict(ft=ft, lt=lt, scanned=scanned, deferred=deferred, rows_scanned=rows_scanned, row_prefix=prefix,
+                    cle_plan=cle_plan)
 
     def _takes_stack(self, cle_plan: dict, cols_ready: Sequence[int]) -> bool:
         """Whether dfq_cle_run will take `cle_plan` (with these layers' column extrema ready) on the stack kernel - the
@@ -501,6 +519,7 @@ class Session:
                     li = [d[0] for d in pending["rows_scanned"]]
                     lt2["flags"][li] |= _lib.LAYER_ROWS_READY
                     lt2["rext_off"][li] = [d[1] for d in pending["rows_scanned"]]
+                    lt2["rext_rows"][li] = pending.get("row_prefix", 0)
                 pending["_pending_key"], pending["_pending_lt"], pending["_pending_base"] = key, lt2, lt
             lt = pending["_pending_lt"]
         gs = np.zeros(plan["n_groups"], dtype=np.int32)
@@ -525,6 +544,7 @@ class Session:
         res.group_sweeps = gs
         res.apply_only = bool(apply_only)
         res.fused_sweeps = int(R[0]["fused_sweeps"])
+        res.rows_streamed = int(R[0]["rows_streamed"])
         res.bc_prepared = att is not None and bool(R[0]["bc_prepared"])
         if res.bc_prepared:
             self._bc_ready = (att["plan"], int(att["num_bits"]))

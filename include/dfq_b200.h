@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DFQ_ABI_VERSION 10
+#define DFQ_ABI_VERSION 11
 
 enum {
   DFQ_OK = 0,
@@ -83,6 +83,9 @@ typedef struct DfqLayer {
   int64_t cmax_off;   /* [2][C of rel_in] running column maxima                              */
   int64_t fold_off;   /* DFQ_LAYER_FOLD_PENDING: [rows] fold factors gamma/sqrt(var+eps) (DfqFold.fac_off)      */
   int64_t rext_off;   /* DFQ_LAYER_ROWS_READY: [2][rows] scratch, row minima then row maxima (DfqFold.scan_rows)     */
+  int32_t rext_rows;  /* DFQ_LAYER_ROWS_READY: 0 = the extrema of every row are in rext_off; n > 0 = only those of rows
+                         [0, min(n, rows)) are (DfqFold.row_prefix): dfq_cle_run completes the rest                   */
+  int32_t _pad;
 } DfqLayer;
 
 /* The flags are promises about the call that runs RIGHT AFTER dfq_bn_fold, on the same weights:
@@ -96,7 +99,11 @@ typedef struct DfqLayer {
  *                          layer to rext_off.  When every first layer of a k_cle_stack run carries it, the kernel may
  *                          derive the scales of the first two sweeps from these extrema and the column extrema alone and
  *                          apply both sweeps in one pass over the weights (DfqCleResult.fused_sweeps); the scratch is
- *                          consumed either way (its content after the call is unspecified). */
+ *                          consumed either way (its content after the call is unspecified).
+ *                          With rext_rows > 0 only a prefix of the rows was scanned.  The kernel's guard then decides from
+ *                          that prefix where it can (every metric term is >= 0, so a partial sum is a lower bound too) and
+ *                          derives the other rows' extrema while the fused pass holds them; where it cannot, it scans the
+ *                          remaining rows itself first and decides as with a full scan (DfqCleResult.rows_streamed). */
 #define DFQ_LAYER_COLS_READY 1
 #define DFQ_LAYER_FOLD_PENDING 2
 #define DFQ_LAYER_ROWS_READY 4
@@ -141,7 +148,19 @@ typedef struct DfqCleResult {
   int32_t bc_prepared;     /* 1: the attached bias correction (dfq_cle_run's bc tables) holds the results of the final
                               weights - the fused pass ran and every group stopped after sweep 2.  0: none attached, or
                               its scratch is stale (all or nothing).                                              */
+  int32_t rows_streamed;   /* first layers that arrived with a row prefix (DfqLayer.rext_rows): DFQ_ROWS_* below     */
+  int32_t _pad;
 } DfqCleResult;
+/* DfqCleResult.rows_streamed:
+ *   DFQ_ROWS_FULL       no first layer arrived with a prefix (or none was shorter than its rows)
+ *   DFQ_ROWS_STREAMED   the prefix decided the guard for every group; the fused pass derived the other rows' extrema
+ *   DFQ_ROWS_UNDECIDED  the prefix left some group undecided: the remaining rows were scanned, then the full guard ran
+ *   DFQ_ROWS_HOST_FULL  the prefix could not be used (no fused pass possible, or s_range with lo <= 0 or hi = inf):
+ *                       the remaining rows were scanned, then the full guard ran (where a fused pass is possible) */
+#define DFQ_ROWS_FULL 0
+#define DFQ_ROWS_STREAMED 1
+#define DFQ_ROWS_UNDECIDED 2
+#define DFQ_ROWS_HOST_FULL 3
 
 /* Cross-layer equalization to convergence.  Replaces dfq.py:78-117 (cross_layer_equalization) and,
  * with max_sweeps = 1 and a single relation, dfq.py:28-75 (_layer_equalization).
@@ -211,6 +230,9 @@ typedef struct DfqFold {
   int32_t scan_rows;          /* _DEFER only, 1: also write the row extrema of the FOLDED weights to the layer's rext_off
                                  ([0, rows) minima, [rows, 2 rows) maxima; layers[] must carry it).  0: no row scan.    */
   int64_t fac_off;            /* _DEFER, _APPLY: [rows] fold factors gamma/sqrt(var+eps)                              */
+  int32_t row_prefix;         /* with scan_rows: 0 = scan every row, n > 0 = only rows [0, min(n, rows)) (DfqLayer.rext_rows;
+                                 the layer must not also be column-scanned).  Ignored without scan_rows.             */
+  int32_t _pad;
 } DfqFold;
 /* DFQ_FOLD_FULL   the fold above: weights, bias, fake_weight / fake_bias.
  * DFQ_FOLD_DEFER  everything but the weights: bias, fake_weight / fake_bias, and each row's factor into fac_off.  With
