@@ -125,20 +125,23 @@ __device__ __forceinline__ void bc_expect(float* arena, const DfqBcLayer& b, con
   }
 }
 
-struct BcRing {
+// STAGES stages of kStageBytes: kBcStages for k_bc_stream and k_cle_stack (BcRing), kScanStages for the fold's scan.
+template <int STAGES>
+struct BcRingT {
+  static constexpr int kStages = STAGES;
   unsigned char* base;
   __device__ __forceinline__ float* stage(int s) const { return (float*)(base + (size_t)s * kStageBytes); }
-  uint64_t* full;      // [kBcStages]
-  uint64_t* empty;     // [kBcStages]
-  TileDesc* desc;      // [kBcStages]
+  uint64_t* full;      // [STAGES]
+  uint64_t* empty;     // [STAGES]
+  TileDesc* desc;      // [STAGES]
   __device__ void init(unsigned char* smem) {
     base = smem;
-    unsigned char* p = smem + (size_t)kBcStages * kStageBytes;
+    unsigned char* p = smem + (size_t)STAGES * kStageBytes;
     full = (uint64_t*)p;
-    empty = (uint64_t*)(p + 8 * kBcStages);
-    desc = (TileDesc*)(p + 16 * kBcStages + 16);
+    empty = (uint64_t*)(p + 8 * STAGES);
+    desc = (TileDesc*)(p + 16 * STAGES + 16);
     if (threadIdx.x == 0) {
-      for (int i = 0; i < kBcStages; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); desc[i].seq = -1; }
+      for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); desc[i].seq = -1; }
       mbar_fence_init();
     }
     __syncthreads();
@@ -147,14 +150,17 @@ struct BcRing {
   __device__ __forceinline__ float* ex_cache(int warp) const {
     return (float*)(base + ring_bytes()) + (size_t)warp * (kBcExCols + 4);
   }
-  __host__ __device__ static constexpr size_t ring_bytes() { return (((size_t)kBcStages * kStageBytes + 16 * kBcStages + 16 + kBcStages * sizeof(TileDesc)) + 127) & ~(size_t)127; }
+  __host__ __device__ static constexpr size_t ring_bytes() { return (((size_t)STAGES * kStageBytes + 16 * STAGES + 16 + STAGES * sizeof(TileDesc)) + 127) & ~(size_t)127; }
   static constexpr size_t smem_bytes() { return ring_bytes() + (size_t)kBcConsumers * (kBcExCols + 4) * 4 + 64; }
 };
+using BcRing = BcRingT<kBcStages>;
 
 // Producer lane: put item `d` at sequence number n.
-__device__ __forceinline__ void bc_produce(BcRing& ring, unsigned long long n, const TileDesc& d) {
-  const int s = (int)(n % kBcStages);
-  if (n >= kBcStages) mbar_wait(ring.empty + s, (uint32_t)(((n / kBcStages) - 1) & 1));
+template <class Ring>
+__device__ __forceinline__ void bc_produce(Ring& ring, unsigned long long n, const TileDesc& d) {
+  constexpr int S = Ring::kStages;
+  const int s = (int)(n % S);
+  if (n >= S) mbar_wait(ring.empty + s, (uint32_t)(((n / S) - 1) & 1));
   ring.desc[s] = d;
   ring.desc[s].seq = (int)n;            // before the arrive below: visible to whoever sees the phase complete
   if (d.kind == TK_BULK) {
@@ -177,10 +183,12 @@ __device__ __forceinline__ void bc_produce(BcRing& ring, unsigned long long n, c
 // runs of 1000+ blocks never hit it).  The producer therefore stamps every item with its sequence number before it arrives,
 // and the consumer re-checks the stamp after every wait (and waits once more after it matched: the stamp is written before
 // the producer's arrive, so by then the barrier is in the right phase).
-__device__ __forceinline__ int bc_take(BcRing& ring, unsigned long long n) {
-  const int s = (int)(n % kBcStages);
+template <class Ring>
+__device__ __forceinline__ int bc_take(Ring& ring, unsigned long long n) {
+  constexpr int S = Ring::kStages;
+  const int s = (int)(n % S);
   const volatile int* seq = &ring.desc[s].seq;
-  const uint32_t parity = (uint32_t)((n / kBcStages) & 1);
+  const uint32_t parity = (uint32_t)((n / S) & 1);
   for (;;) {                                   // common case: one hardware wait, one shared-memory compare
     mbar_wait(ring.full + s, parity);
     if (*seq == (int)n) break;                 // the stage holds MY item
@@ -189,7 +197,8 @@ __device__ __forceinline__ int bc_take(BcRing& ring, unsigned long long n) {
   mbar_wait(ring.full + s, parity);            // stamp seen => the barrier is in (or past) my phase: returns when the bytes have landed
   return s;
 }
-__device__ __forceinline__ void bc_give_back(BcRing& ring, int s, int lane) {
+template <class Ring>
+__device__ __forceinline__ void bc_give_back(Ring& ring, int s, int lane) {
   __syncwarp();
   if (lane == 0) mbar_arrive(ring.empty + s);
 }
@@ -197,6 +206,11 @@ __device__ __forceinline__ void bc_give_back(BcRing& ring, int s, int lane) {
 __device__ __forceinline__ float lds_f32(uint32_t saddr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ float4 lds_f4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
   return v;
 }
 

@@ -663,9 +663,10 @@ struct PassIter {
       break;
     }
   }
-  __device__ __forceinline__ void start(const long long* p, const int* sl, const DfqLayer* L_, const GroupState* G_, int qb, int qe) {
+  __device__ __forceinline__ void start(const long long* p, const int* sl, const DfqLayer* L_, const GroupState* G_, int qb, int qe,
+                                        long long max_block = kTileBlock) {
     ptr = p; step_layers = sl; L = L_; G = G_; q_end = qe; q_live = -1; g_seen = -1; g_done = 0; f_q = -1;
-    cur.init(p[qb], p[qe]);
+    cur.init(p[qb], p[qe], max_block);
     q = cur.valid() ? find_task(p, qb, qe, cur.t) : qb;
     q_lo = p[q]; q_hi = (q < qe) ? p[q + 1] : p[q];
     settle();
@@ -1131,7 +1132,8 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
 // k_cle_engine works on one tile per CTA at a time: every first-layer row pays a CTA-wide reduction barrier and its
 // bookkeeping goes through the producer warp's mailbox; with 3 stages per CTA only ~one 18 KB load per CTA is in flight
 // while a tile is consumed and another one stored (the warps of the plain pipe waited for data).  Here, like k_bc_stream:
-//   * one CTA per SM, kStackConsumers consumer WARPS + a producer warp, 11 stages; a warp owns whole tiles: no CTA barrier per tile;
+//   * one CTA per SM, kStackConsumers consumer WARPS + a producer warp, DFQ_STACK_STAGES stages; a warp owns whole tiles: no CTA
+//     barrier per tile;
 //   * first-layer rows: two passes over the row in shared memory (min/max, then rescale in place) by the warp alone, the
 //     per-channel bookkeeping of dfq.py:62-70 (publish_row) done lane-parallel - lane r retires row r - instead of by one
 //     producer lane;
@@ -1147,20 +1149,30 @@ k_cle_engine(float* arena, const DfqLayer* __restrict__ gL, int nL, const DfqRel
 // The first sweep also completes a BN fold deferred into it (DFQ_LAYER_FOLD_PENDING, RowCtx.fold): every row is multiplied by
 // its fold factor as it is read from the stage.
 // ------------------------------------------------------------------------------------------------------------
-// Consumer warps of k_cle_stack (of the kBcConsumers the CTA has): the pass is far from issue-bound (ncu, 7 consumers: issue
-// slots 19 % busy, 45 % of the warp samples waiting for data) - what matters is how many of the 11 stages are LOADING, i.e.
-// not held by a consumer.  Sequence numbers are dealt modulo this count; the other warps only join the grid barriers.
+// Consumer warps of k_cle_stack (of the kBcConsumers the CTA has): sequence numbers are dealt modulo this count; any other
+// warps only join the grid barriers.  Tuned on an H100 SXM at a 400 W limit (DESIGN.md, "k_cle_stack on H100"): every warp the CTA has consumes and the ring
+// keeps the stages their shared memory leaves.  One consumer warp per scheduler leaves each warp's load-use and shuffle
+// latencies exposed; more consumers hide them, while a stream whose consumers hand stages back at once reaches the
+// read + write ceiling with 4 stages (tools/microbench/hbm_ceiling.cu).
 #ifndef DFQ_STACK_CONSUMERS
-#define DFQ_STACK_CONSUMERS 4
+#define DFQ_STACK_CONSUMERS 7
+#endif
+#ifndef DFQ_STACK_STAGES
+#define DFQ_STACK_STAGES 10
 #endif
 constexpr int kStackConsumers = DFQ_STACK_CONSUMERS;
 static_assert(kStackConsumers >= 1 && kStackConsumers <= kBcConsumers, "k_cle_stack consumer count");
+using StackRing = BcRingT<DFQ_STACK_STAGES>;
+// Tiles per block of the block-cyclic walk (TileCursor) of k_cle_stack's passes, kTileBlock elsewhere.  A consumer warp that
+// meets a new layer stops on its stage for a chain of dependent global loads (the layer's context, the 1/s caches, the
+// correction's quantizer and E[x]), and all consumers of a CTA meet it within a few tiles of each other, so the CTA stops
+// pulling data for that long: at 64 tiles per block (an eighth of a [512,512,3,3] layer) that happened ~60 times per CTA and
+// pass on the synthetic stack.  512 (a whole such layer) measured 14.2-14.3 ms per pass against 15.2-15.3 ms (H100 SXM, 700 W).
+#ifndef DFQ_STACK_TILE_BLOCK
+#define DFQ_STACK_TILE_BLOCK 512
+#endif
+constexpr long long kStackTileBlock = DFQ_STACK_TILE_BLOCK;
 
-__device__ __forceinline__ float4 lds_f4(uint32_t a) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
-  return v;
-}
 __device__ __forceinline__ void sts_f4(uint32_t a, const float4& v) {
   asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
@@ -1393,7 +1405,7 @@ __device__ __forceinline__ void stack_fused_cols(uint32_t a0, int n4, const floa
 }
 
 // Producer lane: this CTA's tiles of one step (layers of converged groups skipped), SKIP padding, one END per consumer.
-__device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n, float* arena, PassIter it) {
+__device__ __noinline__ void cle_stack_feed(StackRing& ring, unsigned long long& n, float* arena, PassIter it) {
   TileDesc d;
   fence_proxy_async_all();          // rows written before the last grid barrier (bulk + plain stores) -> bulk loads
   while (it.valid()) { it.fill(d, arena); bc_produce(ring, n++, d); it.next(); }
@@ -1408,7 +1420,10 @@ __device__ __noinline__ void cle_stack_feed(BcRing& ring, unsigned long long& n,
 // more for the fused pass's second vector (ex_cache(kBcConsumers + warp)).  An attached correction caches E[x] per consumer
 // warp (stack_ex_slot): in the ring's caches no consumer uses (kStackConsumers .. kBcConsumers - 1), then behind the others.
 constexpr int kStackExExtra = 2 * kStackConsumers > kBcConsumers ? 2 * kStackConsumers - kBcConsumers : 0;
-constexpr size_t kStackSmemBytes = BcRing::smem_bytes() + (size_t)(kStackConsumers + kStackExExtra) * (kBcExCols + 4) * 4;
+constexpr size_t kStackSmemBytes = StackRing::smem_bytes() + (size_t)(kStackConsumers + kStackExExtra) * (kBcExCols + 4) * 4;
+// 18 KB per stage and three ~2 KB caches per consumer warp share the SM's 227 KB (the static RowCtx tables: < 3 KB): more
+// consumers, fewer stages
+static_assert(kStackSmemBytes + 3 * 1024 <= 227 * 1024, "k_cle_stack: stages + per-warp caches exceed an SM's shared memory");
 __device__ __forceinline__ int stack_ex_slot(int warp) {
   return warp < kBcConsumers - kStackConsumers ? kStackConsumers + warp : kBcConsumers + kStackConsumers + warp - (kBcConsumers - kStackConsumers);
 }
@@ -1434,7 +1449,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
   extern __shared__ __align__(128) unsigned char ring_smem[];
   __shared__ RowCtx wctx[kBcConsumers];
   __shared__ RowCtx wctx1[kStackConsumers];   // STREAM: the context of sweep 2 of the layer in hand
-  BcRing ring;
+  StackRing ring;
   ring.init(ring_smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool producer = (warp == kBcConsumers);
@@ -1516,7 +1531,7 @@ k_cle_stack(float* arena, const DfqLayer* __restrict__ L, int nL, const DfqRelat
       if (producer) {
         if (lane == 0) {
           PassIter it;
-          it.start(pass_ptr, step_layers, L, G, step_ptr[p], step_ptr[p + 1]);
+          it.start(pass_ptr, step_layers, L, G, step_ptr[p], step_ptr[p + 1], kStackTileBlock);
           cle_stack_feed(ring, n, arena, it);
         }
       } else if (warp < kStackConsumers) {

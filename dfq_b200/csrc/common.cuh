@@ -227,10 +227,11 @@ struct TileCursor {
     t = first + start_blk * B;
     blk_end = t + B;
   }
-  __device__ __forceinline__ void init(long long first_, long long end_) {
+  // max_block: the largest block (kTileBlock unless the kernel has its own, see kStackTileBlock)
+  __device__ __forceinline__ void init(long long first_, long long end_, long long max_block = kTileBlock) {
     first = first_; end = end_;
     const long long per_cta = (end_ - first_) / ((long long)gridDim.x * 4);
-    B = per_cta < 1 ? 1 : (per_cta > kTileBlock ? kTileBlock : per_cta);
+    B = per_cta < 1 ? 1 : (per_cta > max_block ? max_block : per_cta);
     seek(first_);
   }
   __device__ __forceinline__ bool valid() const { return t < end; }

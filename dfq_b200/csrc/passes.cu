@@ -82,6 +82,22 @@ __device__ __forceinline__ void fold_row(float* arena, const DfqLayer& l, const 
   if (lane == 0 && f.mode == DFQ_FOLD_FULL) bn_fold_vectors(arena, l, f, o, fac, den);
 }
 
+// Producer side of one ring phase: this CTA's tiles of tasks [q_begin, q_end) in block-cyclic order, then SKIP items up to
+// a multiple of NC (the consumer warps), then one END per consumer.  Called by lane 0 of the producer warp only.
+template <int NC, class Ring, class Geo>
+__device__ __forceinline__ void bc_feed(Ring& ring, unsigned long long& n, const long long* ptr, int q_begin, int q_end,
+                                        const Geo& geo) {
+  TileDesc d;
+  MatIter<Geo, true> it;
+  it.start(ptr, q_begin, q_end, geo);
+  while (it.valid()) { it.fill(d); bc_produce(ring, n++, d); it.next(); }
+  d.gptr = nullptr; d.task = -1; d.row0 = d.nrows = d.floats = 0;
+  d.kind = BTK_SKIP;
+  while (n % NC) bc_produce(ring, n++, d);
+  d.kind = BTK_END;
+  for (int i = 0; i < NC; ++i) bc_produce(ring, n++, d);
+}
+
 constexpr int kFoldScanCols = 1024;   // columns whose extrema a CTA accumulates in shared memory (more: global atomics)
 
 // The [rows]-vector work before the weight pass, a CTA per fold: buffer 0 of the column extrema of every fold that scans
@@ -210,6 +226,119 @@ k_bn_fold(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restric
   }
   flush();
   pipe.drain();
+}
+
+// The read-only scan of deferred folds, streaming variant (k_bn_fold<false>'s work on bc_stream.cuh's ring).  k_bn_fold's
+// RowPipe pays two or three CTA-wide barriers per 18 KB tile and writes every folded row back into its stage before the scans
+// read it again.  Here one CTA per SM runs a producer warp (bulk loads) and kScanConsumers consumer warps that each own
+// whole tiles: no CTA-wide barrier in the loop, fl(w * f) is formed in registers as the stage is read and never stored.
+//   * row extrema (DfqFold.scan_rows): per row, the minmax4 + warp_min / warp_max reduction of k_cle_stack's first sweep;
+//   * column extrema (DfqFold.scan_go > 0): every warp keeps its own [kFoldScanCols] min / max scratch, flushed into buffer 0
+//     with atomic_min_f / atomic_max_f when the warp moves to another fold.  Lane j mod 32 owns column j of every row it
+//     scans (scan_gi == cols: a group's columns are disjoint from every other group's).
+// Min and max are exact, and the scratch is updated as colscan_tile updates the RowPipe scan's: fminf / fmaxf for layers of
+// one row per tile and for ungrouped 1x1 layers, atomic_min_f / atomic_max_f (the integer order of the bit patterns) for the
+// others, so signed zeros and NaN fold the same way and the extrema are the same bits.  (One exception in the first kind of
+// layer: a column whose taps are NaN in every row one share of the rows holds - a RowPipe CTA's there, a warp's here - gives
+// a NaN maximum, and the shares differ between the two kernels.)
+#ifndef DFQ_SCAN_CONSUMERS
+#define DFQ_SCAN_CONSUMERS 4
+#endif
+#ifndef DFQ_SCAN_STAGES
+#define DFQ_SCAN_STAGES 9
+#endif
+constexpr int kScanConsumers = DFQ_SCAN_CONSUMERS;
+constexpr int kScanThreads = (kScanConsumers + 1) * 32;
+constexpr int kScanStages = DFQ_SCAN_STAGES;
+using ScanRing = BcRingT<kScanStages>;
+// the ring, then a [2][kFoldScanCols] column scratch per consumer warp
+constexpr size_t kScanSmemBytes = ScanRing::ring_bytes() + (size_t)kScanConsumers * 2 * kFoldScanCols * 4;
+static_assert(kScanSmemBytes <= 227 * 1024, "k_fold_scan: ring + column scratch exceed an SM's shared memory");
+static_assert(kPipeMaxRows <= 32, "a consumer warp holds one row's fold factor per lane");
+
+__global__ void __launch_bounds__(kScanThreads, 1)
+k_fold_scan(float* arena, const DfqLayer* __restrict__ L, const DfqFold* __restrict__ F, int nF, const long long* __restrict__ tptr) {
+  extern __shared__ __align__(128) unsigned char ring_smem[];
+  ScanRing ring;
+  ring.init(ring_smem);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == kScanConsumers) {
+    unsigned long long n = 0;
+    if (lane == 0) bc_feed<kScanConsumers>(ring, n, tptr, 0, nF, FoldGeo{arena, L, F});
+    return;
+  }
+  float* smin = (float*)(ring_smem + ScanRing::ring_bytes()) + (size_t)warp * 2 * kFoldScanCols;
+  float* smax = smin + kFoldScanCols;
+  for (int j = lane; j < kFoldScanCols; j += 32) { smin[j] = DFQ_INF; smax[j] = -DFQ_INF; }
+  int cur = -1, nch = 0, go = 1, J = 0, kk = 1, rows = 0;
+  bool scan_rows = false, single = true, own = true;
+  const float* fac = nullptr;
+  float *dmin = nullptr, *dmax = nullptr, *rext = nullptr;
+  auto flush = [&]() {
+    if (nch == 0) return;
+    __syncwarp();
+    colscan_flush<32>(lane, nch, smin, smax, dmin, dmax);
+    __syncwarp();
+  };
+  for (unsigned long long n = warp;; n += kScanConsumers) {
+    const int s = bc_take(ring, n);
+    const TileDesc d = ring.desc[s];
+    if (d.kind == BTK_END) { bc_give_back(ring, s, lane); break; }
+    if (d.kind == BTK_SKIP) { bc_give_back(ring, s, lane); continue; }
+    if (d.task != cur) {
+      flush();
+      cur = d.task;
+      const DfqFold& f = F[cur];
+      const DfqLayer l = L[f.layer];
+      J = l.cols; kk = l.kk; rows = l.rows;
+      fac = arena + f.fac_off;
+      scan_rows = f.scan_rows != 0;
+      rext = arena + l.rext_off;
+      nch = f.scan_go > 0 ? (l.rows / f.scan_go) * f.scan_gi : 0;
+      go = f.scan_go > 0 ? f.scan_go : 1;
+      single = f.scan_go == l.rows;
+      own = pipe_rows_per_tile(l.cols * l.kk) == 1 || (l.kk == 1 && single);
+      dmin = arena + l.cmin_off; dmax = arena + l.cmax_off;    // buffer 0
+    }
+    if (d.kind == TK_PLAIN) {       // a tile the TMA unit cannot move: the warp fetches it itself
+      for (int i = lane; i < d.floats; i += 32) ring.stage(s)[i] = ldg_stream1(d.gptr + i);
+      __syncwarp();
+    }
+    const int row_len = J * kk;
+    const uint32_t sbase = smem_u32(ring.stage(s));
+    const float fo_mine = lane < d.nrows ? fac[d.row0 + lane] : 1.f;
+    for (int r = 0; r < d.nrows; ++r) {
+      const float fo = __shfl_sync(0xffffffffu, fo_mine, r);
+      const uint32_t a0 = sbase + (uint32_t)r * (uint32_t)row_len * 4u;
+      if (scan_rows) {
+        float mn = DFQ_INF, mx = -DFQ_INF;
+        if ((row_len & 3) == 0) {
+          for (int i4 = lane; i4 < (row_len >> 2); i4 += 32) minmax4(mn, mx, mul4(lds_f4(a0 + 16u * i4), fo));
+        } else {
+          for (int i = lane; i < row_len; i += 32) { const float v = __fmul_rn(lds_f32(a0 + 4u * i), fo); mn = fminf(mn, v); mx = fmaxf(mx, v); }
+        }
+        mn = warp_min(mn); mx = warp_max(mx);
+        if (lane == 0) { rext[d.row0 + r] = mn; rext[rows + d.row0 + r] = mx; }
+      }
+      if (nch > 0) {
+        const int c0 = single ? 0 : ((d.row0 + r) / go) * J;
+        for (int j = lane; j < J; j += 32) {
+          const uint32_t a = a0 + 4u * (uint32_t)(j * kk);
+          float mn = __fmul_rn(lds_f32(a), fo), mx = mn;
+          if (kk == 9) {
+#pragma unroll
+            for (int k = 1; k < 9; ++k) { const float v = __fmul_rn(lds_f32(a + 4u * k), fo); mn = fminf(mn, v); mx = fmaxf(mx, v); }
+          } else {
+            for (int k = 1; k < kk; ++k) { const float v = __fmul_rn(lds_f32(a + 4u * k), fo); mn = fminf(mn, v); mx = fmaxf(mx, v); }
+          }
+          if (own) { smin[c0 + j] = fminf(smin[c0 + j], mn); smax[c0 + j] = fmaxf(smax[c0 + j], mx); }
+          else { atomic_min_f(smin + c0 + j, mn); atomic_max_f(smax + c0 + j, mx); }
+        }
+      }
+    }
+    bc_give_back(ring, s, lane);
+  }
+  flush();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -501,20 +630,6 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
 // ------------------------------------------------------------------------------------------------
 static_assert(kPipeMaxRows <= 32, "a consumer warp retires one row per lane");
 
-// Producer side of one ring phase: this CTA's tiles of tasks [q_begin, q_end) in block-cyclic order, then SKIP items up to
-// a multiple of kBcConsumers, then one END per consumer.  Called by lane 0 of the producer warp only.
-__device__ __forceinline__ void bc_feed(BcRing& ring, unsigned long long& n, const long long* ptr, int q_begin, int q_end,
-                                        const BcGeo& geo) {
-  TileDesc d;
-  MatIter<BcGeo, true> it;
-  it.start(ptr, q_begin, q_end, geo);
-  while (it.valid()) { it.fill(d); bc_produce(ring, n++, d); it.next(); }
-  d.gptr = nullptr; d.task = -1; d.row0 = d.nrows = d.floats = 0;
-  d.kind = BTK_SKIP;
-  while (n % kBcConsumers) bc_produce(ring, n++, d);
-  d.kind = BTK_END;
-  for (int i = 0; i < kBcConsumers; ++i) bc_produce(ring, n++, d);
-}
 
 __global__ void __launch_bounds__(kBcThreads, 1)
 k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __restrict__ B, int nB,
@@ -545,7 +660,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
   }
   if (mm_ptr[nB] > 0) {          // the others: streamed through the ring, one min/max pair per tile
     if (producer) {
-      if (lane == 0) bc_feed(ring, n, mm_ptr, 0, nB, geo);
+      if (lane == 0) bc_feed<kBcConsumers>(ring, n, mm_ptr, 0, nB, geo);
     } else {
       for (;; n += kBcConsumers) {
         const int s = bc_take(ring, n);
@@ -579,7 +694,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
     grid.sync();
     // ---- eps . E[x] per output row (dfq.py:216-219,281-293) ---------------------------------------------------
     if (producer) {
-      if (lane == 0) bc_feed(ring, n, row_ptr, level_ptr[lev], level_ptr[lev + 1], geo);
+      if (lane == 0) bc_feed<kBcConsumers>(ring, n, row_ptr, level_ptr[lev], level_ptr[lev + 1], geo);
     } else {
       int cur = -1, cur_group = -1, so = 1;
       DfqBcLayer b; DfqLayer l; BcFastQuant f;
@@ -730,10 +845,24 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
     }
   }
   const int n_rw = (int)rw.size(), n_ro = (int)ro.size();
+  // The read-only scan runs on the streaming kernel k_fold_scan unless some column-scanned layer has more columns than a
+  // consumer warp's scratch holds (k_bn_fold<false> then sends them to global atomics).  DFQ_FOLD_SCAN_STREAM=0/1 forces one.
+  bool scan_stream = true;
+  for (const DfqFold& f : ro)
+    if (f.scan_go > 0 && (int64_t)(layers[f.layer].rows / f.scan_go) * f.scan_gi > kFoldScanCols) scan_stream = false;
+  if (const char* e = getenv("DFQ_FOLD_SCAN_STREAM")) {
+    const bool want = atoi(e) != 0;
+    DFQ_REQUIRE(!want || scan_stream, "DFQ_FOLD_SCAN_STREAM=1: a column-scanned layer has more columns than k_fold_scan holds");
+    scan_stream = want;
+  }
   int grid_rw = 0, grid_ro = 0, rc;
   const size_t dyn = RowPipe::smem_bytes();
   if (n_rw && (rc = coop_grid((const void*)k_bn_fold<true>, "k_bn_fold", kThreads, dyn, rw_ptr.back(), &grid_rw))) return rc;
-  if (n_ro && (rc = coop_grid((const void*)k_bn_fold<false>, "k_bn_fold", kThreads, dyn, ro_ptr.back(), &grid_ro))) return rc;
+  if (n_ro && scan_stream) {
+    if ((rc = coop_grid((const void*)k_fold_scan, "k_fold_scan", kScanThreads, kScanSmemBytes, ro_ptr.back(), &grid_ro))) return rc;
+  } else if (n_ro && (rc = coop_grid((const void*)k_bn_fold<false>, "k_bn_fold", kThreads, dyn, ro_ptr.back(), &grid_ro))) {
+    return rc;
+  }
   TablePack tp;
   const int iL = tp.add(layers, n_layers), iF = tp.add(folds, n_folds);
   const int iRW = n_rw ? tp.add(rw.data(), n_rw) : -1, iRWP = n_rw ? tp.add(rw_ptr.data(), n_rw + 1) : -1;
@@ -742,7 +871,10 @@ extern "C" int dfq_bn_fold(float* arena, int64_t arena_floats, const DfqLayer* l
   const DfqLayer* dL = tp.ptr<DfqLayer>(iL);
   if (prologue) k_fold_prologue<<<std::min(n_folds, 4096), 128, 0, st>>>(arena, dL, tp.ptr<DfqFold>(iF), n_folds);
   if (n_rw) k_bn_fold<true><<<grid_rw, kThreads, dyn, st>>>(arena, dL, tp.ptr<DfqFold>(iRW), n_rw, tp.ptr<long long>(iRWP));
-  if (n_ro) k_bn_fold<false><<<grid_ro, kThreads, dyn, st>>>(arena, dL, tp.ptr<DfqFold>(iRO), n_ro, tp.ptr<long long>(iROP));
+  if (n_ro && scan_stream)
+    k_fold_scan<<<grid_ro, kScanThreads, kScanSmemBytes, st>>>(arena, dL, tp.ptr<DfqFold>(iRO), n_ro, tp.ptr<long long>(iROP));
+  else if (n_ro)
+    k_bn_fold<false><<<grid_ro, kThreads, dyn, st>>>(arena, dL, tp.ptr<DfqFold>(iRO), n_ro, tp.ptr<long long>(iROP));
   DFQ_CUDA(cudaGetLastError());
   tp.release(st);
   return 0;
