@@ -18,6 +18,17 @@
 // k_i8_upsample_bilinear resizes fp32 as torch does, to fp32 and / or codes in such a channel slice.
 // A fourth epilogue writes the fp32 output pixel-major into a slice of a detection head's [N, R, k] concatenation
 // (dfq_i8_conv_nhwc), so the permute / contiguous / cat of SSD's heads need no copies.
+//
+// A second integer scheme runs on the same main loops: the reference's asymmetric per-tensor min / max quantization
+// (QuantMeasure for activations, quantize_targ_layer for weights).  Codes q in [0, 2^b - 1] are stored shifted,
+// q' = q - 128, so the s8 x s8 tensor-core path and every layout stay as they are; the shift moves into the offsets.
+//   k_i8_quantize_affine   fp32 NCHW -> int8 NHWC q' (pad channels 0) and S[n, h, w] = sum of q' over the real channels
+//   k_i8_pack_affine       already fake-quantized fp32 weights -> their codes q' in the dense or depthwise layout, counting
+//                          the weights the round trip fp32(fp32(q fw) + mw) does not reproduce bit for bit
+//   k_i8_affine_table      dense: per output channel, the (kh+1) x (kw+1) prefix table of the tap sums of q'
+//   Out::AFFINE            y = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o] in double (dfq_i8_affine_conv): P the int32
+//                          sum, A the sum of q' over the in-image taps (dense: of S; depthwise: per channel in the main
+//                          loop), Wv the sum of q' of the weights over the same taps, Nv their count times C / groups
 #include <algorithm>
 #include <cmath>
 
@@ -41,7 +52,7 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED, ROWS };
+enum class Out { F32, I8, FUSED, ROWS, AFFINE };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -79,9 +90,43 @@ struct Rows {
   int64_t off, img_stride;
   float pre_lo, pre_hi, post_lo, post_hi;
 };
+// The affine epilogue (dfq_i8_affine_conv): S and table are the dense layer's per-pixel code sums and per-output-channel
+// prefix tables (unused by the depthwise kernel), k the constants of DfqI8Affine.
+struct Affine {
+  const int32_t* S;
+  const int32_t* table;
+  double kP, kA, kW, kN;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
 template <> struct EpiOf<Out::ROWS> { using type = Rows; };
+template <> struct EpiOf<Out::AFFINE> { using type = Affine; };
+
+// fp32(kP P + kA A + kW Wv + kN Nv) + b: each product and sum a separately rounded double op, in this order
+__device__ __forceinline__ float affine_value(int32_t P, int32_t A, int32_t Wv, int32_t Nv, float b, const Affine& e) {
+  double t = __dmul_rn(e.kP, (double)P);
+  t = __dadd_rn(t, __dmul_rn(e.kA, (double)A));
+  t = __dadd_rn(t, __dmul_rn(e.kW, (double)Wv));
+  t = __dadd_rn(t, __dmul_rn(e.kN, (double)Nv));
+  return __fadd_rn(__double2float_rn(t), b);
+}
+
+// The taps r in [lo, hi) of one axis whose input coordinate o * stride - pad + r * dil lies in [0, in): a range, since the
+// coordinate grows with r.  lo == hi when none does.
+__device__ __forceinline__ int2 tap_range(int o, int stride, int pad, int dil, int k, int in) {
+  const int base = o * stride - pad;
+  const int lo = base >= 0 ? 0 : min(k, (-base + dil - 1) / dil);
+  const int hi = base > in - 1 ? 0 : min(k, (in - 1 - base) / dil + 1);
+  return make_int2(lo, max(lo, hi));
+}
+
+// The activation code of the affine scheme, shifted: q = rint(clamp(fp32(fp32(v + neg_min) * inv_scale), 0, qmax)) - 128,
+// the ops of the fake quantization (common.cuh fake_quant<true>), so fp32(fp32((q' + 128) * scale) + min) is its output.
+// NaN has no code there; fmaxf turns it into 0 here (code -128).
+__device__ __forceinline__ int8_t affine_code(float v, float neg_min, float inv_scale, float qmax) {
+  const float t = fminf(fmaxf(__fmul_rn(__fadd_rn(v, neg_min), inv_scale), 0.f), qmax);
+  return (int8_t)((int)rintf(t) - 128);
+}
 
 // What the per-layer path computes from the convolution to the tensor after a residual block's add, in its order: the
 // pass-throughs before the add as one clamp, the fp32 add (rv = r[n, o, p], ignored without a residual), the ones after it.
@@ -136,6 +181,72 @@ __global__ void k_i8_pack_dw(const float* __restrict__ w, const float* __restric
   if (i >= taps * Cpad) return;
   const int c = i % Cpad, tap = i / Cpad;
   out[i] = c < C ? q8(w[c * taps + tap], ws[c]) : (int8_t)0;
+}
+
+// One thread per (n, pixel): its Cpad / 16 chunks of shifted codes and their sum over the real channels, S[n, h, w].
+__global__ void k_i8_quantize_affine(const float* __restrict__ x, int8_t* __restrict__ q, int32_t* __restrict__ S, int C,
+                                     int HW, int Cpad, int64_t total, float neg_min, float inv_scale, float qmax) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i % HW, n = i / HW;
+    int32_t sum = 0;
+    for (int ch = 0; ch < Cpad / 16; ++ch) {
+      alignas(16) int8_t v[16];
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        v[j] = c < C ? affine_code(x[(n * C + c) * HW + p], neg_min, inv_scale, qmax) : (int8_t)0;
+        sum += v[j];
+      }
+      *reinterpret_cast<int4*>(q + i * Cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+    }
+    S[i] = sum;
+  }
+}
+
+// Weight codes of an already fake-quantized tensor: q = clamp(rint(fp32(fp32(w - w_min) / w_scale)), 0, qmax), stored as
+// q - 128 in the layout of k_i8_pack_dense (dense) or k_i8_pack_dw (depthwise, element i = (tap, c)).  *n_bad counts the
+// weights with fp32(fp32(q * w_scale) + w_min) != w, bit for bit.
+__global__ void k_i8_pack_affine(const float* __restrict__ w, int8_t* __restrict__ out, int32_t* __restrict__ n_bad, int C,
+                                 int taps, int Cpad, bool dense, int64_t total, float w_min, float w_scale, float qmax) {
+  int32_t bad = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % Cpad);
+    const int64_t t = i / Cpad;
+    int8_t code = 0;
+    if (c < C) {
+      const float v = dense ? w[((t / taps) * C + c) * taps + t % taps] : w[(int64_t)c * taps + t];
+      const float q = fminf(fmaxf(rintf(__fdiv_rn(__fsub_rn(v, w_min), w_scale)), 0.f), qmax);
+      bad += __float_as_uint(__fadd_rn(__fmul_rn(q, w_scale), w_min)) != __float_as_uint(v);
+      code = (int8_t)((int)q - 128);
+    }
+    out[i] = code;
+  }
+  if (bad) atomicAdd(n_bad, bad);
+}
+
+// One thread per output channel o of a dense layer: T[r][s] = sum of its codes over taps (r' < r, s' < s) and all channels,
+// table + o * (kh + 1) * (kw + 1), row-major.  The in-image taps of any output pixel form a rectangle [r0, r1) x [s0, s1)
+// (tap_range), whose sum is T[r1][s1] - T[r0][s1] - T[r1][s0] + T[r0][s0].
+__global__ void k_i8_affine_table(const int8_t* __restrict__ wq, int32_t* __restrict__ table, int O, int kh, int kw,
+                                  int Cpad) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= O) return;
+  const int tw = kw + 1;
+  int32_t* T = table + (int64_t)o * (kh + 1) * tw;
+  for (int s = 0; s <= kw; ++s) T[s] = 0;
+  for (int r = 0; r < kh; ++r) {
+    T[(r + 1) * tw] = 0;
+    int32_t row = 0;
+    for (int s = 0; s < kw; ++s) {
+      const int4* src = reinterpret_cast<const int4*>(wq + ((int64_t)o * kh * kw + r * kw + s) * Cpad);
+      for (int ch = 0; ch < Cpad / 16; ++ch) {
+        const int4 v = src[ch];
+        row = __dp4a(v.x, 0x01010101, row), row = __dp4a(v.y, 0x01010101, row);
+        row = __dp4a(v.z, 0x01010101, row), row = __dp4a(v.w, 0x01010101, row);
+      }
+      T[(r + 1) * tw + s + 1] = T[r * tw + s + 1] + row;
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -268,6 +379,59 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
+  if constexpr (OUT == Out::AFFINE) {
+    // Past the [o][m] staging below: per pixel of the tile (THREADS == BM, one each) A = the sum of S over its in-image
+    // taps and the tap rectangle (r0 | r1 << 16, s0 | s1 << 16).
+    static_assert(THREADS == BM && BN * EPI_LD * 4 + BM * 12 <= STAGES * STAGE_BYTES, "affine epilogue staging");
+    int32_t* sA = reinterpret_cast<int32_t*>(smem + BN * EPI_LD * 4);
+    uint32_t* sR = reinterpret_cast<uint32_t*>(sA + BM);
+    {
+      const int64_t m = m0 + tid;
+      int32_t a = 0;
+      int2 rr = make_int2(0, 0), ss = make_int2(0, 0);
+      if (m < M) {
+        const int n = (int)(m / OHW), p = (int)(m % OHW), oh = p / g.OW, ow = p % g.OW;
+        rr = tap_range(oh, g.stride_h, g.pad_h, g.dil_h, g.kh, g.H);
+        ss = tap_range(ow, g.stride_w, g.pad_w, g.dil_w, g.kw, g.W);
+        const int32_t* img = rq.S + (int64_t)n * g.H * g.W;
+        for (int r = rr.x; r < rr.y; ++r) {
+          const int32_t* row = img + (int64_t)(oh * g.stride_h - g.pad_h + r * g.dil_h) * g.W;
+          for (int s = ss.x; s < ss.y; ++s) a += row[ow * g.stride_w - g.pad_w + s * g.dil_w];
+        }
+      }
+      sA[tid] = a;
+      sR[2 * tid] = (uint32_t)rr.x | ((uint32_t)rr.y << 16);
+      sR[2 * tid + 1] = (uint32_t)ss.x | ((uint32_t)ss.y << 16);
+    }
+    int32_t* st = reinterpret_cast<int32_t*>(smem);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int m = wm * 64 + i * 16 + (lane >> 2) + (r >> 1) * 8;
+          const int o = wn * 32 + j * 8 + (lane & 3) * 2 + (r & 1);
+          st[o * EPI_LD + m] = acc[i][j][r];
+        }
+    __syncthreads();
+    const int tw = g.kw + 1, tsize = (g.kh + 1) * tw;
+    for (int e = tid; e < BM * BN; e += THREADS) {
+      const int ml = e % BM, ol = e / BM;
+      const int64_t m = m0 + ml;
+      const int o = o0 + ol;
+      if (m >= M || o >= g.O) continue;
+      const int32_t P = st[ol * EPI_LD + ml];
+      const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
+      const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
+      const int32_t* T = rq.table + (int64_t)o * tsize;
+      const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
+      const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
+      y[idx] = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
+      if (acc_out) acc_out[idx] = P;
+    }
+    return;
+  }
   if constexpr (OUT == Out::ROWS) {
     // Straight from the accumulator layout: for one register pair (h = 0, 1), a warp holds 8 pixels x 8 consecutive
     // channels, so the stores run in 32-byte pieces along the channels of each pixel's row.  4-byte stores: off and O are
@@ -427,6 +591,11 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
     int32_t acc[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) acc[j] = 0;
+    int32_t xsum[16], wsum[16], ntaps = 0;                      // Out::AFFINE: A, Wv per channel, the in-image taps
+    if constexpr (OUT == Out::AFFINE) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) xsum[j] = wsum[j] = 0;
+    }
     const int8_t* img = xq + n * g.H * g.W * g.Cpad + ch * 16;
     for (int r = 0; r < g.kh; ++r) {
       const int ih = oh * g.stride_h - g.pad_h + r * g.dil_h;
@@ -440,7 +609,23 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         const int8_t* wb = reinterpret_cast<const int8_t*>(&wv);
 #pragma unroll
         for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
+        if constexpr (OUT == Out::AFFINE) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) xsum[j] += xb[j], wsum[j] += wb[j];
+          ++ntaps;
+        }
       }
+    }
+    if constexpr (OUT == Out::AFFINE) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        if (c >= g.C) break;
+        const int64_t idx = (n * g.C + c) * OHW + p;
+        y[idx] = affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq);
+        if (acc_out) acc_out[idx] = acc[j];
+      }
+      continue;
     }
     if constexpr (OUT == Out::FUSED) {                          // r and y along the pixels, as the F32 stores
       alignas(16) int8_t v[16];
@@ -913,6 +1098,108 @@ extern "C" int dfq_i8_upsample_bilinear(const float* x, float* y, int8_t* yq, co
   const bool ac = g->align_corners == 1;
   k_i8_upsample_bilinear<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
       x, y, yq, *g, bilinear_scale(g->H, g->OH, ac), bilinear_scale(g->W, g->OW, ac), total);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- the affine scheme -------------------------------------------------------------------------------------------------
+namespace dfq {
+namespace {
+
+// codes of 1..8 bits; K = kh * kw * C / groups below 2^17, so that |P| <= K * 128 * 128 < 2^31 (codes of -128 reach the
+// main loop)
+int check_affine(const DfqI8Conv* g, int num_bits, const char* who) {
+  if (int rc = check_geometry(g)) return rc;
+  if (num_bits > 8) {
+    set_error("%s: %d-bit codes do not fit in int8 (at most 8 bits)", who, num_bits);
+    return DFQ_E_UNSUPPORTED;
+  }
+  if (num_bits < 1) {
+    set_error("%s: num_bits must be at least 1, got %d", who, num_bits);
+    return DFQ_E_ARG;
+  }
+  const int64_t K = (int64_t)g->kh * g->kw * (g->C / g->groups);
+  if (K >= (1 << 17)) {
+    set_error("%s: K = kh * kw * C / groups = %lld reaches 131072, where K * 128 * 128 overflows the int32 sums", who,
+              (long long)K);
+    return DFQ_E_UNSUPPORTED;
+  }
+  return 0;
+}
+
+}  // namespace
+}  // namespace dfq
+
+extern "C" int dfq_i8_affine_quantize(const float* x, int8_t* q, int32_t* S, int32_t N, int32_t C, int32_t H, int32_t W,
+                                      int32_t Cpad, float act_min, float act_max, int32_t num_bits, void* stream) {
+  DFQ_REQUIRE(x && q && S && N > 0 && C > 0 && H > 0 && W > 0, "dfq_i8_affine_quantize: bad arguments");
+  DFQ_REQUIRE(Cpad >= C && Cpad % 16 == 0, "dfq_i8_affine_quantize: Cpad must be a multiple of 16 that holds C");
+  DFQ_REQUIRE(aligned16(q), "dfq_i8_affine_quantize: q must be 16-byte aligned");
+  if (num_bits < 1 || num_bits > 8) {
+    set_error("dfq_i8_affine_quantize: num_bits must be in [1, 8], got %d", num_bits);
+    return num_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
+  }
+  const QuantScalars qs = quant_scalars((double)act_min, (double)act_max, num_bits, 0);
+  if (!(std::isfinite(act_min) && std::isfinite(act_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
+    set_error("dfq_i8_affine_quantize: the range [%g, %g] is not finite or gives a scale that is not a finite fp32 number",
+              act_min, act_max);
+    return DFQ_E_ARG;
+  }
+  const int64_t total = (int64_t)N * H * W;
+  k_i8_quantize_affine<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x, q, S, C, H * W, Cpad, total, qs.neg_min,
+                                                                                qs.inv_scale, qs.qmax);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_affine_pack(const float* w, float w_min, float w_scale, int32_t num_bits, int8_t* packed,
+                                  int32_t* table, int32_t* n_bad, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_affine(g, num_bits, "dfq_i8_affine_pack")) return rc;
+  DFQ_REQUIRE(w && packed && n_bad, "dfq_i8_affine_pack: null pointer");
+  DFQ_REQUIRE(g->groups != 1 || table, "dfq_i8_affine_pack: a dense layer needs its prefix table");
+  DFQ_REQUIRE(aligned16(packed), "dfq_i8_affine_pack: packed must be 16-byte aligned");
+  if (!(std::isfinite(w_min) && std::isfinite(w_scale) && w_scale > 0.f)) {
+    set_error("dfq_i8_affine_pack: w_min must be finite and w_scale finite and positive, got %g and %g", w_min, w_scale);
+    return DFQ_E_ARG;
+  }
+  const int taps = g->kh * g->kw;
+  const bool dense = g->groups == 1;
+  const int64_t total = (dense ? (int64_t)g->O : 1) * taps * g->Cpad;
+  cudaStream_t st = (cudaStream_t)stream;
+  DFQ_CUDA(cudaMemsetAsync(n_bad, 0, sizeof(int32_t), st));
+  k_i8_pack_affine<<<grid_for(total, 256), 256, 0, st>>>(w, packed, n_bad, g->C, taps, g->Cpad, dense, total, w_min, w_scale,
+                                                         (float)(ldexp(1.0, num_bits) - 1.0));
+  DFQ_CUDA(cudaGetLastError());
+  if (dense) {
+    k_i8_affine_table<<<(g->O + 127) / 128, 128, 0, st>>>(packed, table, g->O, g->kh, g->kw, g->Cpad);
+    DFQ_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+extern "C" int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8_t* wq, const int32_t* table,
+                                  const DfqI8Affine* k, const float* bias, float* y, int32_t* acc_out, const DfqI8Conv* g,
+                                  void* stream) {
+  if (int rc = check_affine(g, 8, "dfq_i8_affine_conv")) return rc;
+  DFQ_REQUIRE(xq && wq && k && y, "dfq_i8_affine_conv: null pointer");
+  DFQ_REQUIRE(g->groups != 1 || (S && table), "dfq_i8_affine_conv: a dense layer needs S and its prefix table");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_affine_conv: codes must be 16-byte aligned");
+  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
+    set_error("dfq_i8_affine_conv: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", k->kP, k->kA, k->kW,
+              k->kN);
+    return DFQ_E_ARG;
+  }
+  const Affine ep{S, table, k->kP, k->kA, k->kW, k->kN};
+  cudaStream_t st = (cudaStream_t)stream;
+  if (g->groups == 1) {
+    const int64_t M = (int64_t)g->N * g->OH * g->OW;
+    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_affine_conv: too many output pixels");
+    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<Out::AFFINE><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, y, acc_out, *g, ep);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<Out::AFFINE><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, y, acc_out, *g, total, ep);
+  }
   DFQ_CUDA(cudaGetLastError());
   return 0;
 }

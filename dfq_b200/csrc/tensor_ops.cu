@@ -480,6 +480,7 @@ extern "C" int dfq_struct_size(int which) {
     case 9: return (int)sizeof(DfqI8Epilogue);
     case 10: return (int)sizeof(DfqI8Pool);
     case 11: return (int)sizeof(DfqI8Resize);
+    case 12: return (int)sizeof(DfqI8Affine);
     default: return -1;
   }
 }

@@ -16,6 +16,10 @@ Order of the calibration steps, as in convert_ncnn.py: BN fold, equalization (an
 ranges (set_quant_minmax or update_stat), then convert_to_int8 - BEFORE quantize_targ_layer, whose fake-quantized weights
 are not the fp32 weights the int8 codes are made from.  The observers replace_op() installs for functional ops are not used:
 tensors between converted layers stay fp32.
+
+convert_affine executes the reference's own quantization instead (asymmetric per-tensor min / max, dfq_i8_affine_*): called
+AFTER quantize_targ_layer and the activation ranges, it recovers the weight codes from the fake-quantized weights and
+computes each layer from integer sums, equal to the fake-quantized layer up to fp32 rounding.
 """
 import ctypes as C
 import operator
@@ -348,6 +352,190 @@ class Int8Linear(_Int8Layer):
         return "in_features=%d, out_features=%d, act_scale=%g" % (self.in_channels, self.out_channels, self.act_scale)
 
 
+# ---- the reference's own quantization: asymmetric per-tensor min / max -------------------------------------------------
+AFFINE_MAX_K = 1 << 17          # K = kh * kw * C / groups: codes of -128 reach the int32 sums, K * 128 * 128 < 2^31
+_GRID_ULPS = 8                  # weight-grid search: fp32 scales within this many ulps of (max - min) / (2^b - 1)
+
+
+def act_affine_scalars(running_min, running_max, num_bits):
+    """(ma, fa) of QuantMeasure's eval-mode fake quantization (utils/quantize.py, dfq_quant_dequant_dev with the range on the
+    device): ma = fp32(running_min), fa = fp32(max((running_max - running_min) / (2^b - 1), 1e-8)), the scale in double."""
+    mn, mx = float(_f32(running_min)), float(_f32(running_max))
+    s = max((mx - mn) / (2. ** int(num_bits) - 1.), 1e-8)
+    with np.errstate(over="ignore"):
+        return _f32(mn), _f32(s)
+
+
+def affine_constants(ma, fa, mw, fw):
+    """(kP, kA, kW, kN) of the affine epilogue (include/dfq_b200.h, DfqI8Affine) in double, in this order: the shifted offsets
+    ma' = ma + 128 fa and mw' = mw + 128 fw, then kP = fa fw, kA = fa mw', kW = ma' fw, kN = ma' mw'."""
+    ma, fa, mw, fw = float(ma), float(fa), float(mw), float(fw)
+    ma2 = ma + 128. * fa
+    mw2 = mw + 128. * fw
+    return fa * fw, fa * mw2, ma2 * fw, ma2 * mw2
+
+
+def weight_grid_candidates(w_min, w_max, num_bits):
+    """fp32 scales fw that may have produced fake-quantized weights with this min / max: fp32((max - min) / (2^b - 1)) in
+    double (at least fp32(1e-8), quantize_targ_layer's floor) and its neighbours within _GRID_ULPS ulps, those whose
+    top code reproduces max (fp32(fp32((2^b - 1) fw) + min) == max) first, then by distance."""
+    mn, mx = _f32(w_min), _f32(w_max)
+    qmax = _f32(2. ** int(num_bits) - 1.)
+    with np.errstate(over="ignore", invalid="ignore"):
+        base = _f32(max((float(mx) - float(mn)) / float(qmax), 1e-8))
+    if not (np.isfinite(base) and np.isfinite(mn) and np.isfinite(mx)):
+        return []
+    cands, up, down = [base], base, base
+    for _ in range(_GRID_ULPS):
+        up, down = np.nextafter(up, _f32(np.inf)), np.nextafter(down, _f32(0))
+        cands += [up, down]
+    cands = [c for c in cands if c > 0 and np.isfinite(c)]
+    with np.errstate(over="ignore"):
+        top = [bool(_f32(_f32(qmax * c) + mn) == mx) for c in cands]
+    return [c for t, c in sorted(zip(top, cands), key=lambda tc: not tc[0])]
+
+
+class _AffineInt8Layer(nn.Module):
+    """One layer of a fake-quantized model executed in integer arithmetic (dfq_i8_affine_*): the input is quantized with the
+    range its `quant` observer had at conversion, the weight codes are recovered from the fake-quantized weights, and the
+    output is fp32 NCHW.  The ranges are frozen: an observer whose update_stat is truthy would keep widening its range in
+    the fake-quantized model (set_layer_bits leaves update_stat = the bit width, quirk Q1), this layer does not."""
+
+    def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
+                 name=None):
+        super().__init__()
+        O, Cg, kh, kw = weight.shape
+        self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
+        self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
+        self.cpad = (self.in_channels + 15) // 16 * 16
+        self.layer_name = name
+        _affine_refusal(self._who(), self.in_channels, self.out_channels, self.groups, self.kernel_size, act_bits, w_bits)
+        self.act_bits, self.w_bits = int(act_bits), int(w_bits)
+        self.act_min, self.act_max = float(_f32(act_min)), float(_f32(act_max))
+        ma, fa = act_affine_scalars(act_min, act_max, act_bits)
+        if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(act_max))):
+            raise _lib.DfqError("layer %s: activation range [%g, %g] gives no finite fp32 scale" % (self._who(), ma, act_max))
+        dev = engine._default_device()
+        depthwise = self.groups > 1
+        taps = kh * kw
+        self.register_buffer("weight_codes", torch.zeros((taps * self.cpad,) if depthwise else (O * taps * self.cpad,),
+                                                         dtype=torch.int8, device=dev))
+        self.register_buffer("tap_table", torch.zeros((0,) if depthwise else (O * (kh + 1) * (kw + 1),), dtype=torch.int32,
+                                                      device=dev))
+        b = torch.zeros(O) if bias is None else bias.detach().float()
+        self.register_buffer("bias", b.to(dev).contiguous())
+        w = weight.detach().float().to(dev).contiguous()
+        mw, mx = _f32(w.min().item()), _f32(w.max().item())
+        fw = self._pack(w, mw, mx)
+        self.w_min, self.w_scale = float(mw), float(fw)
+        k = affine_constants(ma, fa, mw, fw)
+        if not all(np.isfinite(k)):
+            raise _lib.DfqError("layer %s: the affine constants %s are not finite" % (self._who(), k))
+        self.constants = np.zeros(1, _lib.I8_AFFINE_DT)
+        self.constants[0] = k
+
+    def _pack(self, w, mw, mx):
+        """Pack the codes at the first candidate scale whose round trip reproduces every weight; returns it."""
+        kh, kw = self.kernel_size
+        g = self._geometry(1, (kh - 1) * self.dilation[0] + 1, (kw - 1) * self.dilation[1] + 1, stride=(1, 1), padding=(0, 0))
+        lib, st = _lib.load(), _lib.stream_ptr()
+        n_bad = torch.zeros(1, dtype=torch.int32, device=w.device)
+        fewest = None
+        for fw in weight_grid_candidates(mw, mx, self.w_bits):
+            _lib.check(lib.dfq_i8_affine_pack(_ptr(w), C.c_float(mw), C.c_float(fw), self.w_bits, _ptr(self.weight_codes),
+                                              _ptr(self.tap_table) if self.tap_table.numel() else None, _ptr(n_bad),
+                                              _lib.table_ptr(g), st), "dfq_i8_affine_pack (layer %s)" % self._who())
+            bad = int(n_bad.item())
+            if bad == 0:
+                return fw
+            fewest = bad if fewest is None else min(fewest, bad)
+        raise _lib.DfqError("layer %s: its weights are not on a %d-bit min / max grid (min %g, max %g; %s of %d weights off "
+                            "the best candidate scale): run quantize_targ_layer first"
+                            % (self._who(), self.w_bits, mw, mx, "all" if fewest is None else fewest, w.numel()))
+
+    _geometry = _Int8Layer._geometry
+
+    def _who(self):
+        return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
+                                                                  self.kernel_size)
+
+    def run(self, x, with_acc=False):
+        """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes."""
+        if not x.is_cuda or not self.bias.is_cuda:
+            raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
+                                % (x.device, self.bias.device))
+        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
+            raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s %s" % (self.in_channels, x.dtype, tuple(x.shape)))
+        x = x.contiguous()
+        N, _, H, W = x.shape
+        g = self._geometry(N, H, W)
+        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
+        if OH <= 0 or OW <= 0:
+            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        lib, st = _lib.load(), _lib.stream_ptr()
+        xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
+        S = torch.empty(N * H * W, dtype=torch.int32, device=x.device)
+        _lib.check(lib.dfq_i8_affine_quantize(_ptr(x), _ptr(xq), _ptr(S), N, self.in_channels, H, W, self.cpad,
+                                              C.c_float(self.act_min), C.c_float(self.act_max), self.act_bits, st),
+                   "dfq_i8_affine_quantize (layer %s)" % self._who())
+        y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=x.device)
+        acc = torch.empty(y.shape, dtype=torch.int32, device=x.device) if with_acc else None
+        _lib.check(lib.dfq_i8_affine_conv(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                          _ptr(self.tap_table) if self.tap_table.numel() else None,
+                                          _lib.table_ptr(self.constants), _ptr(self.bias), _ptr(y), _ptr(acc),
+                                          _lib.table_ptr(g), st), "dfq_i8_affine_conv (layer %s)" % self._who())
+        return y, acc
+
+    def extra_repr(self):
+        return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act=[%g, %g] %d-bit, w_min=%g, " \
+               "w_scale=%g %d-bit" % (self.in_channels, self.out_channels, self.kernel_size, self.stride, self.padding,
+                                      self.dilation, self.groups, self.act_min, self.act_max, self.act_bits, self.w_min,
+                                      self.w_scale, self.w_bits)
+
+
+def _affine_refusal(who, C_in, C_out, groups, kernel_size, act_bits, w_bits):
+    """Raise DfqError naming the layer if dfq_i8_affine_* cannot run it."""
+    if groups != 1 and not (groups == C_in == C_out):
+        raise _lib.DfqError("layer %s cannot run in int8: needs groups == 1 or depthwise (groups == C_in == C_out), got "
+                            "groups=%d C_in=%d C_out=%d" % (who, groups, C_in, C_out))
+    for what, b in (("activation", act_bits), ("weight", w_bits)):
+        if not isinstance(b, (int, np.integer)) or isinstance(b, bool) or not 1 <= b <= 8:
+            raise _lib.DfqError("layer %s: %s codes of %r bits do not fit the int8 path (1 to 8 bits)" % (who, what, b))
+    K = kernel_size[0] * kernel_size[1] * (C_in // groups)
+    if K >= AFFINE_MAX_K:
+        raise _lib.DfqError("layer %s: K = kh * kw * C / groups = %d reaches %d, where the int32 sums can overflow"
+                            % (who, K, AFFINE_MAX_K))
+
+
+class AffineInt8Conv2d(_AffineInt8Layer):
+    """A fake-quantized nn.Conv2d (QuantNConv2d after quantize_targ_layer) executed in integer arithmetic."""
+
+    @classmethod
+    def from_conv(cls, conv: nn.Conv2d, act_min, act_max, act_bits=8, w_bits=8, name=None):
+        if isinstance(conv.padding, str) or conv.padding_mode != "zeros":
+            raise _lib.DfqError("layer %s: int8 execution supports numeric zero padding only (padding=%r, padding_mode=%r)"
+                                % (name, conv.padding, conv.padding_mode))
+        return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
+                   conv.groups, name=name)
+
+    def forward(self, x):
+        return self.run(x)[0]
+
+
+class AffineInt8Linear(_AffineInt8Layer):
+    """A fake-quantized nn.Linear executed in integer arithmetic: the 1x1 convolution of [B, I, 1, 1]."""
+
+    @classmethod
+    def from_linear(cls, lin: nn.Linear, act_min, act_max, act_bits=8, w_bits=8, name=None):
+        return cls(lin.weight.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias, act_min, act_max, act_bits, w_bits,
+                   name=name)
+
+    def forward(self, x):
+        lead = x.shape[:-1]
+        y, _ = self.run(x.reshape(-1, self.in_channels, 1, 1))
+        return y.reshape(*lead, self.out_channels)
+
+
 def _pool_extent(n, k, p, s, d, ceil_mode):
     """torch's pooling output size (floor division; in ceil mode the last window starts inside the input or its left pad)."""
     o = (n + 2 * p - d * (k - 1) - 1 + (s - 1 if ceil_mode else 0)) // s + 1
@@ -539,15 +727,66 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
     return done
 
 
+def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
+    """Replace every target layer of `graph` (types in targ_type, Conv2d or Linear with a `quant` observer) inside `model`,
+    in place, by an AffineInt8Conv2d / AffineInt8Linear that computes it in integer arithmetic under the reference's own
+    quantization (asymmetric per-tensor min / max, include/dfq_b200.h dfq_i8_affine_*); returns the names in graph order.
+
+    Call it in the reference's inference state: after quantize_targ_layer(graph, bits_weight, ...) and the activation ranges
+    (set_quant_minmax or update_quant_range).  Activation ranges and bits come from each layer's `quant` observer
+    (running_min, running_max, num_bits) and are frozen here: an observer left with a truthy update_stat keeps widening its
+    range in the fake-quantized model (set_layer_bits does this through quirk Q1), the converted layer does not.  The
+    weight codes are recovered from the fake-quantized weights: mw = min(weight), fw an fp32 scale near
+    (max - min) / (2^bits_weight - 1) whose round trip fp32(fp32(q fw) + mw) reproduces every weight bit for bit (checked on
+    the device).  The result agrees with the fake-quantized layer to fp32 rounding of its sum, not bit for bit.
+
+    Every layer is checked and packed before any is replaced: a layer that cannot run (grouping, padding mode, bits above 8,
+    K = kh * kw * C / groups >= 131072, no observer, a non-finite range) or whose weights are not on such a grid raises
+    DfqError naming it, and the model is left as it was."""
+    layers = [graph[k] for k in graph if type(graph[k]) in targ_type]
+    names = {id(m): n for n, m in model.named_modules()}
+    plan = []
+    for i, layer in enumerate(layers):
+        name = names.get(id(layer))
+        if name is None:
+            raise _lib.DfqError("target layer %d (%s) is not a submodule of the model" % (i, type(layer).__name__))
+        quant = getattr(layer, "quant", None)
+        if quant is None or not hasattr(quant, "running_min"):
+            raise _lib.DfqError("layer %s has no `quant` observer with an activation range" % name)
+        if isinstance(layer, nn.Conv2d):
+            if layer.padding_mode != "zeros" or isinstance(layer.padding, str):
+                raise _lib.DfqError("layer %s: int8 execution supports numeric zero padding only (padding=%r, "
+                                    "padding_mode=%r)" % (name, layer.padding, layer.padding_mode))
+            shape = (layer.in_channels, layer.out_channels, layer.groups, tuple(layer.kernel_size))
+        elif isinstance(layer, nn.Linear):
+            shape = (layer.in_features, layer.out_features, 1, (1, 1))
+        else:
+            raise _lib.DfqError("layer %s (%s) cannot run in int8: needs a Conv2d or a Linear" % (name, type(layer).__name__))
+        _affine_refusal(name, *shape, quant.num_bits, bits_weight)
+        plan.append((name, layer, float(quant.running_min.reshape(-1)[0]), float(quant.running_max.reshape(-1)[0]),
+                     quant.num_bits))
+    new = []
+    for name, layer, lo, hi, bits in plan:
+        if isinstance(layer, nn.Conv2d):
+            new.append(AffineInt8Conv2d.from_conv(layer, lo, hi, bits, bits_weight, name=name))
+        else:
+            new.append(AffineInt8Linear.from_linear(layer, lo, hi, bits, bits_weight, name=name))
+    for (name, *_), mod in zip(plan, new):
+        parent_name, _, attr = name.rpartition(".")
+        setattr(model.get_submodule(parent_name) if parent_name else model, attr, mod)
+    return [name for name, *_ in plan]
+
+
 # ---- chaining converted convolutions through int8 codes ---------------------------------------------------------------
 _INF = float("inf")
 
 
 class _Int8Tracer(fx.Tracer):
-    """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves"""
+    """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves.  The affine layers of
+    convert_affine are opaque leaves: they are no Int8Conv2d, so nothing is fused into or out of them."""
 
     def is_leaf_module(self, m, qualname):
-        return isinstance(m, _Int8Layer) or super().is_leaf_module(m, qualname)
+        return isinstance(m, (_Int8Layer, _AffineInt8Layer)) or super().is_leaf_module(m, qualname)
 
 
 def _arg(node, i, name, default):

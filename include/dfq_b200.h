@@ -44,7 +44,7 @@ int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
- * 11 DfqI8Resize): lets a binding verify
+ * 11 DfqI8Resize, 12 DfqI8Affine): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -536,6 +536,46 @@ typedef struct DfqI8Resize {
  * 4-byte aligned, an out_scale that is not finite and non-negative while yq is written, NaN or unordered bounds, x
  * overlapping y or the slice, y overlapping the slice. */
 int dfq_i8_upsample_bilinear(const float* x, float* y, int8_t* yq, const DfqI8Resize* g, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Int8 execution under the reference's own quantization: asymmetric per-tensor min / max, b <= 8 bits
+ *
+ * The state main_cls.py:196 runs: quantize_targ_layer has written w^ = fp32(fp32(qw * fw) + mw) into the weights (one
+ * (fw, mw) per tensor, codes qw in [0, 2^b - 1]) and QuantMeasure turns the input into x^ = fp32(fp32(qa * fa) + ma) with
+ *   ma = running_min,  s_a = max((running_max - running_min) / (2^b - 1), 1e-8) in double,  fa = fp32(s_a),
+ *   qa = rint(clamp(fp32(fp32(x + (-ma)) * fp32(1 / s_a)), 0, 2^b - 1))     (CUDA: the division is a reciprocal multiply)
+ * Codes are stored shifted, q' = q - 128, in the layouts of dfq_i8_quantize_nhwc / dfq_i8_pack_weights, and the shift goes
+ * into the offsets ma' = ma + 128 fa, mw' = mw + 128 fw.  Per output element, over the in-image taps only (padding is a
+ * dequantized 0.0 in the fake-quantized model, not a code):
+ *   y = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o]      each product and sum a double op, in this order, no FMA
+ *   P = sum qa' qw' (int32),  A = sum qa',  Wv = sum qw',  Nv = (in-image taps) * C / groups
+ *   kP = fa fw,  kA = fa mw',  kW = ma' fw,  kN = ma' mw'  (formed in double by the caller)
+ * This is the value of sum (qa fa + ma)(qw fw + mw) rounded to fp32 once; the fake-quantized model sums the rounded
+ * products x^ w^ in fp32, so the two agree to fp32 rounding, not bit for bit.  Grouping as dfq_i8_conv.  K = kh * kw * C /
+ * groups must stay below 131072 (codes of -128 reach the main loop and K * 128 * 128 must stay below 2^31): DFQ_E_UNSUPPORTED,
+ * as are codes of more than 8 bits.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct DfqI8Affine {
+  double kP, kA, kW, kN;
+} DfqI8Affine;
+/* fp32 NCHW x -> int8 NHWC q[N, H, W, Cpad] = qa - 128 (pad channels 0) and int32 S[N, H, W] = sum of q over the C real
+ * channels, with QuantMeasure's scalars of the range (act_min, act_max) at num_bits: fp32((q + 128) * fa) + ma is
+ * QuantMeasure's output bit for bit, +-inf included.  NaN has no code there (its output is NaN); here it gets qa = 0.
+ * q 16-byte aligned.  DFQ_E_ARG: a non-finite range or scale, num_bits < 1; DFQ_E_UNSUPPORTED: num_bits > 8. */
+int dfq_i8_affine_quantize(const float* x, int8_t* q, int32_t* S, int32_t N, int32_t C, int32_t H, int32_t W, int32_t Cpad,
+                           float act_min, float act_max, int32_t num_bits, void* stream);
+/* Weight codes of a fake-quantized tensor w^ (layout as dfq_i8_pack_weights): qw = clamp(rint(fp32(fp32(w^ - w_min) /
+ * w_scale)), 0, 2^b - 1), stored qw - 128; *n_bad (device int32, zeroed by the call) = the weights with
+ * fp32(fp32(qw * w_scale) + w_min) != w^ bit for bit.  Dense layers also get table[O][(kh + 1) * (kw + 1)], the prefix
+ * sums of their codes over the taps (T[r][s] = sum over taps r' < r, s' < s and all channels); depthwise layers take
+ * table = NULL.  DFQ_E_ARG: non-finite w_min, w_scale not finite and positive; refusals as dfq_i8_affine_conv. */
+int dfq_i8_affine_pack(const float* w, float w_min, float w_scale, int32_t num_bits, int8_t* packed, int32_t* table,
+                       int32_t* n_bad, const DfqI8Conv* g, void* stream);
+/* The convolution with the epilogue above: xq and S from dfq_i8_affine_quantize (S unused by depthwise layers), wq and
+ * table from dfq_i8_affine_pack, bias[O] (NULL: none), y fp32 NCHW [N, O, OH, OW]; acc_out (NULL: not written) receives P.
+ * DFQ_E_ARG: non-finite constants, a dense layer without S or table; DFQ_E_UNSUPPORTED: K >= 131072, other groupings. */
+int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8_t* wq, const int32_t* table, const DfqI8Affine* k,
+                       const float* bias, float* y, int32_t* acc_out, const DfqI8Conv* g, void* stream);
 
 #ifdef __cplusplus
 }

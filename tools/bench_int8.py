@@ -15,7 +15,9 @@ chain_int8(residual=True, pool_cat=True) (max pools and channel concatenations c
 network of tests/deeplab_v3plus_like.py and torchvision's DeepLab-v3 ResNet-50.  `layout`: per-layer against
 chain_int8(..., upsample=True) and chain_int8(..., layout=True) (zero pads folded into convolutions, detection heads written
 into their concatenation) on the networks of tests/deeplab_mobilenet_padded.py (8 x 513x513) and tests/ssd_lite_like.py
-(256 x 300x300).  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+(256 x 300x300).  `affine` (only when asked for: --sections affine): the reference's own asymmetric min / max quantization
+executed in integers (int8.convert_affine) against the fake-quantized model and the ncnn per-layer int8 model on
+MobileNetV2 and ResNet-18, with the logit errors against the fake-quantized model.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
 device; writes nothing.
 """
 import argparse
@@ -586,6 +588,64 @@ def layout_inference(dev, reps=10, rounds=5, seg_batch=8, ssd_batch=256):
     return out
 
 
+def affine_inference(dev, reps=10, batch=256, rounds=5):
+    """The reference's own quantization executed in integers (int8.convert_affine) on torchvision MobileNetV2 and ResNet-18 in
+    the reference's inference state (tests/affine_calibrated.py: BN fold, equalization, bias correction, quantize_targ_layer's
+    8-bit weights, observer ranges over synthetic images), timed alternately with the fake-quantized model it replaces
+    (QuantN* layers: only the inputs of the target layers are quantized, no functional-op observers) and with the ncnn
+    per-layer int8 model (convert_to_int8 on the same equalized fp32 weights, activation scales from the same observers),
+    `rounds` rounds of `reps` passes, median; and the relative logit error (2-norm over the batch) of each against the
+    fake-quantized model."""
+    import copy
+    import statistics
+    from collections import OrderedDict
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_calibrated
+    from dfq_b200 import int8
+    from dfq_b200.utils import quantize as Q
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds}
+    try:
+        x = torch.randn(batch, 3, 224, 224, device=dev, generator=torch.Generator(device=dev).manual_seed(3)).clamp_(-2.5, 2.5)
+        for net in ("mobilenet_v2", "resnet18"):
+            fq, _, qtarg, pre = affine_calibrated.calibrated(net, keep_unquantized=True)
+            aff = copy.deepcopy(fq)
+            int8.convert_affine(aff, OrderedDict((id(m), m) for m in aff.modules() if type(m) in qtarg), qtarg)
+            int8.convert_to_int8(pre, OrderedDict((id(m), m) for m in pre.modules() if type(m) in qtarg), qtarg)
+            arms = (("fake_quant", fq), ("affine_int8", aff), ("ncnn_int8_per_layer", pre))
+            with torch.no_grad():
+                ref = fq(x)
+                err = {k: float((m(x) - ref).norm() / ref.norm()) for k, m in arms[1:]}
+                for _ in range(2):
+                    for _, m in arms:
+                        m(x)
+                torch.cuda.synchronize(dev)
+                ms = {k: [] for k, _ in arms}
+                for _ in range(rounds):
+                    for k, m in arms:
+                        ms[k].append(timed(lambda m=m: m(x)))
+            med = {k: statistics.median(v) for k, v in ms.items()}
+            out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                        "ms_per_batch_rounds": ms, "rel_logit_error_vs_fake_quant": err,
+                        "layers": sum(1 for m in aff.modules() if isinstance(m, int8._AffineInt8Layer))}
+            del fq, aff, pre
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -607,7 +667,7 @@ def main():
     p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
-                   help="comma-separated sections to run (default: all)")
+                   help="comma-separated sections to run (default: all but affine)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -625,6 +685,8 @@ def main():
         res["upsample"] = upsample_inference(dev, reps=args.reps, batch=args.seg_batch)
     if "layout" in want:
         res["layout"] = layout_inference(dev, reps=args.reps, seg_batch=args.seg_batch, ssd_batch=args.ssd_batch)
+    if "affine" in want:
+        res["affine"] = affine_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
