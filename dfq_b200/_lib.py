@@ -99,13 +99,17 @@ I8_RESIZE_DT = np.dtype([(f, np.int32) for f in ("N", "C", "H", "W", "OH", "OW",
 
 I8_AFFINE_DT = np.dtype([(f, np.float64) for f in ("kP", "kA", "kW", "kN")], align=True)
 
+I8_AFFINE_EPILOGUE_DT = np.dtype([(f, np.uint64) for f in ("residual", "y", "yq", "S")] +
+                                 [("out_min", np.float32), ("out_max", np.float32), ("out_bits", np.int32)] +
+                                 [(f, np.float32) for f in ("pre_lo", "pre_hi", "post_lo", "post_hi")], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
     "DfqCleResult": (CLE_RESULT_DT, 544), "DfqFold": (FOLD_DT, 88), "DfqExpectTerm": (TERM_DT, 32),
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64), "DfqI8Resize": (I8_RESIZE_DT, 48),
-    "DfqI8Affine": (I8_AFFINE_DT, 32),
+    "DfqI8Affine": (I8_AFFINE_DT, 32), "DfqI8AffineEpilogue": (I8_AFFINE_EPILOGUE_DT, 64),
 }
 
 _PF = C.c_void_p   # device float*
@@ -165,6 +169,8 @@ SIGNATURES = {
     "dfq_i8_affine_pack": [_PF, C.c_float, C.c_float, _I32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_i8_affine_conv": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, C.c_void_p,
                            _ST],
+    "dfq_i8_affine_conv_fused": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p, C.c_void_p,
+                                 _ST],
 }
 
 _lib = None

@@ -29,6 +29,9 @@
 //   Out::AFFINE            y = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o] in double (dfq_i8_affine_conv): P the int32
 //                          sum, A the sum of q' over the in-image taps (dense: of S; depthwise: per channel in the main
 //                          loop), Wv the sum of q' of the weights over the same taps, Nv their count times C / groups
+//   Out::AFFINE_FUSED      the same value through the clamps and residual add of Out::FUSED, then fp32 NCHW and / or the
+//                          NEXT layer's shifted codes and their per-pixel sums S (dfq_i8_affine_conv_fused), which keeps
+//                          affine activations in int8 between chained layers
 #include <algorithm>
 #include <cmath>
 
@@ -52,7 +55,7 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED, ROWS, AFFINE };
+enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -97,10 +100,24 @@ struct Affine {
   const int32_t* table;
   double kP, kA, kW, kN;
 };
+// The affine residual epilogue (DfqI8AffineEpilogue): Affine's value, clamp(pre), + r (NULL: none), clamp(post), then y
+// (kernel argument, NULL: none) and / or yq = int8 NHWC [N, OH, OW, cpad] codes at the consumer's scalars (neg_min,
+// inv_scale, qmax) and S_out[n, p] = their sum over the real channels (NULL: none; atomicAdd into a zeroed S_out when
+// several launches' tiles or threads share a pixel, S_atomic).
+struct AffineFused : Affine {
+  const float* r;
+  int8_t* yq;
+  int32_t* S_out;
+  float neg_min, inv_scale, qmax;
+  float pre_lo, pre_hi, post_lo, post_hi;
+  int cpad;
+  bool S_atomic;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
 template <> struct EpiOf<Out::ROWS> { using type = Rows; };
 template <> struct EpiOf<Out::AFFINE> { using type = Affine; };
+template <> struct EpiOf<Out::AFFINE_FUSED> { using type = AffineFused; };
 
 // fp32(kP P + kA A + kW Wv + kN Nv) + b: each product and sum a separately rounded double op, in this order
 __device__ __forceinline__ float affine_value(int32_t P, int32_t A, int32_t Wv, int32_t Nv, float b, const Affine& e) {
@@ -379,7 +396,7 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
-  if constexpr (OUT == Out::AFFINE) {
+  if constexpr (OUT == Out::AFFINE || OUT == Out::AFFINE_FUSED) {
     // Past the [o][m] staging below: per pixel of the tile (THREADS == BM, one each) A = the sum of S over its in-image
     // taps and the tap rectangle (r0 | r1 << 16, s0 | s1 << 16).
     static_assert(THREADS == BM && BN * EPI_LD * 4 + BM * 12 <= STAGES * STAGE_BYTES, "affine epilogue staging");
@@ -416,21 +433,71 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
         }
     __syncthreads();
     const int tw = g.kw + 1, tsize = (g.kh + 1) * tw;
-    for (int e = tid; e < BM * BN; e += THREADS) {
-      const int ml = e % BM, ol = e / BM;
-      const int64_t m = m0 + ml;
-      const int o = o0 + ol;
-      if (m >= M || o >= g.O) continue;
-      const int32_t P = st[ol * EPI_LD + ml];
-      const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
-      const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
-      const int32_t* T = rq.table + (int64_t)o * tsize;
-      const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
-      const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
-      y[idx] = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
-      if (acc_out) acc_out[idx] = P;
+    if constexpr (OUT == Out::AFFINE) {
+      for (int e = tid; e < BM * BN; e += THREADS) {
+        const int ml = e % BM, ol = e / BM;
+        const int64_t m = m0 + ml;
+        const int o = o0 + ol;
+        if (m >= M || o >= g.O) continue;
+        const int32_t P = st[ol * EPI_LD + ml];
+        const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
+        const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
+        const int32_t* T = rq.table + (int64_t)o * tsize;
+        const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
+        const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
+        y[idx] = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
+        if (acc_out) acc_out[idx] = P;
+      }
+      return;
+    } else {
+      // Each element's code replaces its sum in the staging (the same thread reads and writes the word; channels O ..
+      // o0 + 63 stage code 0, the pad of yq); then one thread per pixel gathers its 64 codes, stores its chunks below
+      // cpad and sums them into S.  The residual reads and the y stores run along the pixels of one channel, as the F32
+      // epilogue's.
+      for (int e = tid; e < BM * BN; e += THREADS) {
+        const int ml = e % BM, ol = e / BM;
+        const int64_t m = m0 + ml;
+        const int o = o0 + ol;
+        if (m >= M) continue;
+        int32_t code = 0;
+        if (o < g.O) {
+          const int32_t P = st[ol * EPI_LD + ml];
+          const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
+          const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
+          const int32_t* T = rq.table + (int64_t)o * tsize;
+          const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
+          const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
+          float v = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
+          v = clamp_keep_nan(v, rq.pre_lo, rq.pre_hi);
+          if (rq.r) v = __fadd_rn(v, rq.r[idx]);
+          v = clamp_keep_nan(v, rq.post_lo, rq.post_hi);
+          if (y) y[idx] = v;
+          code = affine_code(v, rq.neg_min, rq.inv_scale, rq.qmax);
+        }
+        st[ol * EPI_LD + ml] = code;
+      }
+      if (!rq.yq) return;
+      __syncthreads();
+      const int64_t m = m0 + tid;
+      if (m >= M) return;
+      int32_t sum = 0;
+#pragma unroll
+      for (int c = 0; c < BN / 16; ++c) {
+        alignas(16) int8_t v[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          v[j] = (int8_t)st[(c * 16 + j) * EPI_LD + tid];
+          sum += v[j];
+        }
+        if (o0 + c * 16 < rq.cpad)
+          *reinterpret_cast<int4*>(rq.yq + m * rq.cpad + o0 + c * 16) = *reinterpret_cast<const int4*>(v);
+      }
+      if (rq.S_out) {
+        if (rq.S_atomic) atomicAdd(rq.S_out + m, sum);
+        else rq.S_out[m] = sum;
+      }
+      return;
     }
-    return;
   }
   if constexpr (OUT == Out::ROWS) {
     // Straight from the accumulator layout: for one register pair (h = 0, 1), a warp holds 8 pixels x 8 consecutive
@@ -582,7 +649,8 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
     const int64_t t = i / OHW;
     const int ch = (int)(t % chunks);
     const int64_t n = t / chunks;
-    if constexpr (OUT == Out::I8 || OUT == Out::FUSED) {
+    constexpr bool affine = OUT == Out::AFFINE || OUT == Out::AFFINE_FUSED;
+    if constexpr (OUT == Out::I8 || OUT == Out::FUSED || OUT == Out::AFFINE_FUSED) {
       // the input's Cpad may be wider than yq's cpad = round_up(O, 16): chunks past it hold only pad channels, and yq has
       // no room for them
       if (ch * 16 >= rq.cpad) continue;
@@ -591,8 +659,8 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
     int32_t acc[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) acc[j] = 0;
-    int32_t xsum[16], wsum[16], ntaps = 0;                      // Out::AFFINE: A, Wv per channel, the in-image taps
-    if constexpr (OUT == Out::AFFINE) {
+    int32_t xsum[16], wsum[16], ntaps = 0;                      // affine: A, Wv per channel, the in-image taps
+    if constexpr (affine) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) xsum[j] = wsum[j] = 0;
     }
@@ -609,7 +677,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         const int8_t* wb = reinterpret_cast<const int8_t*>(&wv);
 #pragma unroll
         for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
-        if constexpr (OUT == Out::AFFINE) {
+        if constexpr (affine) {
 #pragma unroll
           for (int j = 0; j < 16; ++j) xsum[j] += xb[j], wsum[j] += wb[j];
           ++ntaps;
@@ -624,6 +692,33 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         const int64_t idx = (n * g.C + c) * OHW + p;
         y[idx] = affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq);
         if (acc_out) acc_out[idx] = acc[j];
+      }
+      continue;
+    }
+    if constexpr (OUT == Out::AFFINE_FUSED) {                   // as Out::FUSED; the pixel's sum shared by its chunks
+      alignas(16) int8_t v[16];
+      int32_t sum = 0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        v[j] = 0;
+        if (c < g.C) {
+          const int64_t idx = (n * g.C + c) * OHW + p;
+          float f = affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq);
+          f = clamp_keep_nan(f, rq.pre_lo, rq.pre_hi);
+          if (rq.r) f = __fadd_rn(f, rq.r[idx]);
+          f = clamp_keep_nan(f, rq.post_lo, rq.post_hi);
+          if (y) y[idx] = f;
+          v[j] = affine_code(f, rq.neg_min, rq.inv_scale, rq.qmax);
+          sum += v[j];
+        }
+      }
+      if (rq.yq) {
+        *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+        if (rq.S_out) {
+          if (rq.S_atomic) atomicAdd(rq.S_out + n * OHW + p, sum);
+          else rq.S_out[n * OHW + p] = sum;
+        }
       }
       continue;
     }
@@ -1199,6 +1294,72 @@ extern "C" int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8
   } else {
     const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
     k_i8_conv_dw<Out::AFFINE><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, y, acc_out, *g, total, ep);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                        const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                                        const DfqI8Conv* g, void* stream) {
+  const char* who = "dfq_i8_affine_conv_fused";
+  if (int rc = check_affine(g, 8, who)) return rc;
+  DFQ_REQUIRE(xq && wq && k && e, "dfq_i8_affine_conv_fused: null pointer");
+  DFQ_REQUIRE(g->groups != 1 || (S_in && table), "dfq_i8_affine_conv_fused: a dense layer needs S and its prefix table");
+  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_affine_conv_fused: codes must be 16-byte aligned");
+  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
+    set_error("dfq_i8_affine_conv_fused: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", k->kP, k->kA,
+              k->kW, k->kN);
+    return DFQ_E_ARG;
+  }
+  DFQ_REQUIRE(e->y || e->yq, "dfq_i8_affine_conv_fused: no output requested (y and yq are both NULL)");
+  DFQ_REQUIRE(!e->S || e->yq, "dfq_i8_affine_conv_fused: S is the sum of the codes; it needs yq");
+  DFQ_REQUIRE(aligned16(e->yq), "dfq_i8_affine_conv_fused: yq must be 16-byte aligned");
+  DFQ_REQUIRE(((uintptr_t)e->residual & 3) == 0 && ((uintptr_t)e->y & 3) == 0 && ((uintptr_t)e->S & 3) == 0,
+              "dfq_i8_affine_conv_fused: residual, y and S must be 4-byte aligned");
+  DFQ_REQUIRE(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
+              "dfq_i8_affine_conv_fused: pre / post clamp bounds must be ordered and not NaN");
+  QuantScalars qs{};
+  if (e->yq) {                                                  // the consumer's quantizer, as dfq_i8_affine_quantize
+    if (e->out_bits < 1 || e->out_bits > 8) {
+      set_error("%s: out_bits must be in [1, 8], got %d", who, e->out_bits);
+      return e->out_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
+    }
+    qs = quant_scalars((double)e->out_min, (double)e->out_max, e->out_bits, 0);
+    if (!(std::isfinite(e->out_min) && std::isfinite(e->out_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
+      set_error("%s: the output range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
+                e->out_min, e->out_max);
+      return DFQ_E_ARG;
+    }
+  }
+  const int cpad = (g->O + 15) / 16 * 16;
+  const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
+  const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float), yq_bytes = pixels * cpad, s_bytes = pixels * 4;
+  DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes) &&
+                  !overlap(e->residual, y_bytes, e->S, s_bytes),
+              "dfq_i8_affine_conv_fused: residual overlaps y, yq or S");
+  DFQ_REQUIRE(!overlap(e->y, y_bytes, e->yq, yq_bytes) && !overlap(e->y, y_bytes, e->S, s_bytes) &&
+                  !overlap(e->yq, yq_bytes, e->S, s_bytes),
+              "dfq_i8_affine_conv_fused: y, yq and S overlap");
+  const bool dense = g->groups == 1;
+  DFQ_REQUIRE(!dense || (pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_affine_conv_fused: too many output pixels");
+  // one writer per pixel of S: a dense layer whose 64-channel tile covers O, a depthwise one with one 16-channel chunk
+  const bool atomic = e->S && (dense ? g->O > BN : cpad > 16);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (atomic) DFQ_CUDA(cudaMemsetAsync(e->S, 0, s_bytes, st));
+  AffineFused ep{};
+  static_cast<Affine&>(ep) = Affine{S_in, table, k->kP, k->kA, k->kW, k->kN};
+  ep.r = e->residual, ep.yq = e->yq, ep.S_out = e->S;
+  ep.neg_min = qs.neg_min, ep.inv_scale = qs.inv_scale, ep.qmax = qs.qmax;
+  ep.pre_lo = e->pre_lo, ep.pre_hi = e->pre_hi, ep.post_lo = e->post_lo, ep.post_hi = e->post_hi;
+  ep.cpad = cpad, ep.S_atomic = atomic;
+  if (dense) {
+    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<Out::AFFINE_FUSED><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, ep);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<Out::AFFINE_FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total,
+                                                                           ep);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;

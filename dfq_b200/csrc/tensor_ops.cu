@@ -481,6 +481,7 @@ extern "C" int dfq_struct_size(int which) {
     case 10: return (int)sizeof(DfqI8Pool);
     case 11: return (int)sizeof(DfqI8Resize);
     case 12: return (int)sizeof(DfqI8Affine);
+    case 13: return (int)sizeof(DfqI8AffineEpilogue);
     default: return -1;
   }
 }

@@ -399,7 +399,15 @@ class _AffineInt8Layer(nn.Module):
     """One layer of a fake-quantized model executed in integer arithmetic (dfq_i8_affine_*): the input is quantized with the
     range its `quant` observer had at conversion, the weight codes are recovered from the fake-quantized weights, and the
     output is fp32 NCHW.  The ranges are frozen: an observer whose update_stat is truthy would keep widening its range in
-    the fake-quantized model (set_layer_bits leaves update_stat = the bit width, quirk Q1), this layer does not."""
+    the fake-quantized model (set_layer_bits leaves update_stat = the bit width, quirk Q1), this layer does not.
+
+    Execution modes, set only on the copies chain_affine makes (`chained`): `codes_in` - the input is the pair (codes, S)
+    another layer's epilogue wrote at this layer's range (S None for a depthwise layer); `epilogue` - an Epilogue whose
+    out_scale is the consumer's (act_min, act_max, act_bits) (dfq_i8_affine_conv_fused), with `sums` - write S too."""
+
+    codes_in = False
+    epilogue = None
+    sums = False
 
     def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
                  name=None):
@@ -459,32 +467,127 @@ class _AffineInt8Layer(nn.Module):
         return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
                                                                   self.kernel_size)
 
-    def run(self, x, with_acc=False):
-        """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes."""
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False):
+        """A new module of the same class on the same buffers (weight_codes, tap_table, bias, constants), in the given
+        execution mode: codes_in - take (codes, S) from the previous layer's epilogue instead of quantizing fp32; requant =
+        ((act_min, act_max, act_bits), lo, hi) - return the consumer's codes after the clamp (lo, hi), the epilogue
+        Epilogue(out, (lo, hi)); epilogue - an Epilogue whose out_scale is the consumer's (act_min, act_max, act_bits) or
+        None (the residual epilogue, dfq_i8_affine_conv_fused); sums - the codes come with their per-pixel sums S (a dense
+        consumer reads them).  name: the layer's name in error messages.  self is not modified."""
+        new = type(self).__new__(type(self))
+        nn.Module.__init__(new)
+        for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad",
+                  "act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants"):
+            setattr(new, k, getattr(self, k))
+        for k, b in self._buffers.items():
+            new.register_buffer(k, b)
+        new.codes_in = bool(codes_in)
+        new.layer_name = name or self.layer_name
+        if requant is not None and epilogue is not None:
+            raise _lib.DfqError("layer %s: requant and epilogue are two output modes; give one" % new._who())
+        if requant is not None:
+            out, lo, hi = requant
+            epilogue = Epilogue(out, (lo, hi))
+        if epilogue is not None:
+            e = Epilogue(*epilogue)
+            if e.out_scale is None and not e.fp32:
+                raise _lib.DfqError("layer %s: the epilogue returns neither codes nor fp32" % new._who())
+            out = None
+            if e.out_scale is not None:
+                lo, hi, bits = e.out_scale
+                who = "%s -> next layer" % new._who()
+                _affine_refusal(who, 1, 1, 1, (1, 1), bits, 8)
+                ma, fa = act_affine_scalars(lo, hi, bits)
+                if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(hi))):
+                    raise _lib.DfqError("layer %s: output range [%g, %g] gives no finite fp32 scale" % (who, lo, hi))
+                out = (float(_f32(lo)), float(_f32(hi)), int(bits))
+            epilogue = Epilogue(out, _ordered(*e.pre, what="pre-add"), _ordered(*e.post, what="post-add"), bool(e.residual),
+                                bool(e.fp32))
+        new.epilogue = epilogue
+        new.sums = bool(sums) and epilogue is not None and epilogue.out_scale is not None
+        return new
+
+    def _input(self, x):
+        """(codes, S | None, N, H, W) of the input: quantized here from fp32, or the pair a codes_in layer takes."""
+        lib, st = _lib.load(), _lib.stream_ptr()
+        if self.codes_in:
+            xq, S = x if isinstance(x, tuple) and len(x) == 2 else (x, None)
+            if not isinstance(xq, torch.Tensor) or xq.dtype != torch.int8 or xq.dim() != 4 or xq.shape[3] != self.cpad:
+                raise _lib.DfqError("chained affine layer %s expects (int8 codes [N, H, W, %d], S), got %s" % (
+                    self._who(), self.cpad, "%s %s" % (xq.dtype, tuple(xq.shape)) if isinstance(xq, torch.Tensor)
+                    else type(x).__name__))
+            N, H, W, _ = xq.shape
+            if self.groups == 1 and (S is None or S.dtype != torch.int32 or S.numel() != N * H * W):
+                raise _lib.DfqError("chained affine layer %s is dense: it needs the codes' per-pixel sums S, int32 [%d, %d, %d]"
+                                    % (self._who(), N, H, W))
+            if not xq.is_cuda:
+                raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s" % xq.device)
+            return xq.contiguous(), None if S is None else S.contiguous(), N, H, W
+        if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
+            raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s" % (
+                self.in_channels, "%s %s" % (x.dtype, tuple(x.shape)) if isinstance(x, torch.Tensor) else type(x).__name__))
         if not x.is_cuda or not self.bias.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.bias.device))
-        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
-            raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s %s" % (self.in_channels, x.dtype, tuple(x.shape)))
         x = x.contiguous()
         N, _, H, W = x.shape
-        g = self._geometry(N, H, W)
-        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
-        if OH <= 0 or OW <= 0:
-            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
-        lib, st = _lib.load(), _lib.stream_ptr()
         xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
         S = torch.empty(N * H * W, dtype=torch.int32, device=x.device)
         _lib.check(lib.dfq_i8_affine_quantize(_ptr(x), _ptr(xq), _ptr(S), N, self.in_channels, H, W, self.cpad,
                                               C.c_float(self.act_min), C.c_float(self.act_max), self.act_bits, st),
                    "dfq_i8_affine_quantize (layer %s)" % self._who())
-        y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=x.device)
-        acc = torch.empty(y.shape, dtype=torch.int32, device=x.device) if with_acc else None
+        return xq, S, N, H, W
+
+    def run(self, x, with_acc=False, residual=None):
+        """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes.  In the chained modes
+        x is (codes [N, H, W, cpad], S [N, H, W] | None) (codes_in), and with an epilogue y is (codes, S | None), the fp32
+        output, or ((codes, S | None), fp32 output) when it returns both; `residual` is the fp32 tensor [N, C_out, OH, OW]
+        the epilogue adds (exactly that shape, no broadcasting, on the input's device)."""
+        if self.epilogue is not None and with_acc:
+            raise _lib.DfqError("a chained affine layer does not return its int32 sums")
+        if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
+            raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
+                                                    "takes no residual input"))
+        xq, S, N, H, W = self._input(x)
+        g = self._geometry(N, H, W)
+        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
+        if OH <= 0 or OW <= 0:
+            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        if self.epilogue is not None:
+            return self._run_fused(xq, S, residual, g, N, OH, OW), None
+        lib, st = _lib.load(), _lib.stream_ptr()
+        y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=xq.device)
+        acc = torch.empty(y.shape, dtype=torch.int32, device=xq.device) if with_acc else None
         _lib.check(lib.dfq_i8_affine_conv(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
                                           _ptr(self.tap_table) if self.tap_table.numel() else None,
                                           _lib.table_ptr(self.constants), _ptr(self.bias), _ptr(y), _ptr(acc),
                                           _lib.table_ptr(g), st), "dfq_i8_affine_conv (layer %s)" % self._who())
         return y, acc
+
+    def _run_fused(self, xq, S, r, g, N, OH, OW):
+        e = self.epilogue
+        shape = (N, self.out_channels, OH, OW)
+        if r is not None:
+            if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
+                    r.device != xq.device:
+                raise _lib.DfqError("layer %s: the residual must be fp32 %s on %s, got %s" % (
+                    self._who(), list(shape), xq.device, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
+                    if isinstance(r, torch.Tensor) else type(r).__name__))
+            r = r.contiguous()
+        yq = None if e.out_scale is None else \
+            torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=xq.device)
+        S_out = torch.empty((N, OH, OW), dtype=torch.int32, device=xq.device) if yq is not None and self.sums else None
+        y = torch.empty(shape, dtype=torch.float32, device=xq.device) if e.fp32 else None
+        d = np.zeros(1, _lib.I8_AFFINE_EPILOGUE_DT)
+        d[0] = tuple(0 if t is None else t.data_ptr() for t in (r, y, yq, S_out)) + (e.out_scale or (0.0, 0.0, 0)) + \
+            e.pre + e.post
+        _lib.check(_lib.load().dfq_i8_affine_conv_fused(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                                        _ptr(self.tap_table) if self.tap_table.numel() else None,
+                                                        _lib.table_ptr(self.constants), _ptr(self.bias), _lib.table_ptr(d),
+                                                        _lib.table_ptr(g), _lib.stream_ptr()),
+                   "dfq_i8_affine_conv_fused (layer %s)" % self._who())
+        codes = None if yq is None else (yq, S_out)
+        return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
 
     def extra_repr(self):
         return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act=[%g, %g] %d-bit, w_min=%g, " \
@@ -518,8 +621,8 @@ class AffineInt8Conv2d(_AffineInt8Layer):
         return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
                    conv.groups, name=name)
 
-    def forward(self, x):
-        return self.run(x)[0]
+    def forward(self, x, r=None):
+        return self.run(x, residual=r)[0]
 
 
 class AffineInt8Linear(_AffineInt8Layer):
@@ -782,8 +885,9 @@ _INF = float("inf")
 
 
 class _Int8Tracer(fx.Tracer):
-    """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves.  The affine layers of
-    convert_affine are opaque leaves: they are no Int8Conv2d, so nothing is fused into or out of them."""
+    """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves.  To chain_int8 the affine
+    layers of convert_affine are opaque leaves (they are no Int8Conv2d, so nothing is fused into or out of them), and to
+    chain_affine the ncnn layers are."""
 
     def is_leaf_module(self, m, qualname):
         return isinstance(m, (_Int8Layer, _AffineInt8Layer)) or super().is_leaf_module(m, qualname)
@@ -1174,18 +1278,7 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
         that tensor for its users, and the views, permutes, shape queries and pass-throughs are deleted.  If one operand
         does not qualify the cat stays in torch.  `fused_heads` records (cat node name, producer names, k).
     layout=True without upsample=True raises DfqError."""
-    tracer = _Int8Tracer()
-    graph = tracer.trace(model, concrete_args)
-    gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
-    mods = dict(gm.named_modules())
-    sites = {}
-    for node in gm.graph.nodes:
-        if node.op == "call_module":
-            sites[node.target] = sites.get(node.target, 0) + 1
-
-    def conv(node):
-        return node.op == "call_module" and isinstance(mods[node.target], Int8Conv2d) and sites[node.target] == 1
-
+    gm, mods, conv = _trace(model, concrete_args, _NCNN.layer)
     if pool_cat and not residual:
         raise _lib.DfqError("chain_int8: pool_cat=True builds on residual=True")
     if upsample and not pool_cat:
@@ -1199,7 +1292,87 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
             gm.folded_pads = folded
             gm.fused_heads = _fuse_heads(gm, conv, mods)
         return gm
+    return _chain_edges(gm, mods, conv, _NCNN)
 
+
+def chain_affine(model: nn.Module, concrete_args=None, residual=False) -> fx.GraphModule:
+    """A torch.fx GraphModule that computes what `model` (after convert_affine) computes, with activations kept as the
+    consumers' shifted affine codes between AffineInt8Conv2d layers, bit-identical to the per-layer path.
+
+    The rules are chain_int8's, with AffineInt8Conv2d (dense or depthwise, called at one site) in place of Int8Conv2d and a
+    consumer's (act_min, act_max, act_bits), compared bit for bit, in place of its act_scale - two consumers with equal
+    ranges and bits read identical codes:
+    - single-user edges: every node from P to Q has exactly one user and every node in between is one of chain_int8's
+      pass-throughs (exact-identity eval BatchNorm2d, ReLU / ReLU6 / Hardtanh in their module and functional forms,
+      nn.Identity, eval Dropout).  P's epilogue (dfq_i8_affine_conv_fused) applies them as one clamp and writes the codes
+      dfq_i8_affine_quantize would give Q's input, Q reads them and skips its quantizer, and the nodes in between are
+      deleted.
+    - residual=True adds chain_int8's fan-out and residual-add rules: from P forward through single-user pass-throughs to
+      a node with several users, the AffineInt8Conv2d users whose range key equals the first such user's (graph order)
+      take P's codes, every other user - a convolution at another range or bit width included - takes P's fp32 output of
+      the same launch; an add of two distinct nodes whose fused operand is P's single-user pass-through chain is computed
+      in P's epilogue (clamp before it, fp32 add of the residual, clamp after it), P moving to the add's position (ResNet's
+      downsample blocks compute the residual after the block's last convolution).  Adds whose operands differ in shape
+      raise DfqError naming the layer when the module runs.
+    A producer writes the codes' per-pixel sums S (which a dense consumer's epilogue reads) only when some code consumer is
+    dense, and its fp32 output only when a user other than those consumers remains.  Ncnn Int8Conv2d layers and
+    AffineInt8Linear stay opaque leaves, so no edge crosses the two schemes; pools, concatenations, upsampling, pads and
+    detection heads stay in torch, fp32.
+
+    The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
+    edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) the clamp
+    the consumer's codes were taken after; with residual=True the fused adds in `fused_adds`: (producer name, add node
+    name, residual node name, (lo, hi) before the add, (lo, hi) after it), as chain_int8 records them."""
+    gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer)
+    if residual:
+        return _chain_residual(gm, mods, conv, scheme=_AFFINE)
+    return _chain_edges(gm, mods, conv, _AFFINE)
+
+
+class _Scheme(NamedTuple):
+    """What the chaining rules need of one integer scheme: `layer`, the convolution class whose edges they fuse; key(m),
+    what decides the codes layer m reads, compared bit for bit by same(a, b) (consumers with equal keys read identical
+    codes); out(key), the producer's output argument for such a consumer (requant's first element, Epilogue.out_scale);
+    chained(m, codes_in, name, requant, epilogue, out_slice, sums), m's copy in its execution mode, sums True when a dense
+    consumer takes its codes."""
+    layer: type
+    key: object
+    same: object
+    out: object
+    chained: object
+
+
+_NCNN = _Scheme(Int8Conv2d, lambda m: _f32(m.act_scale), lambda a, b: a.view(np.int32) == b.view(np.int32), float,
+                lambda m, codes_in, name, requant, epilogue, out_slice, sums: m.chained(
+                    codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, out_slice=out_slice))
+_AFFINE = _Scheme(AffineInt8Conv2d, lambda m: (_f32(m.act_min), _f32(m.act_max), int(m.act_bits)),
+                  lambda a, b: a[0].view(np.int32) == b[0].view(np.int32) and a[1].view(np.int32) == b[1].view(np.int32)
+                  and a[2] == b[2],
+                  lambda k: (float(k[0]), float(k[1]), int(k[2])),
+                  lambda m, codes_in, name, requant, epilogue, out_slice, sums: m.chained(
+                      codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, sums=sums))
+
+
+def _trace(model, concrete_args, layer):
+    """(GraphModule of `model` traced with the int8 layers as leaves, its modules by name, conv(node): node calls a
+    `layer` module that is called at no other site)."""
+    tracer = _Int8Tracer()
+    graph = tracer.trace(model, concrete_args)
+    gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
+    mods = dict(gm.named_modules())
+    sites = {}
+    for node in gm.graph.nodes:
+        if node.op == "call_module":
+            sites[node.target] = sites.get(node.target, 0) + 1
+
+    def conv(node):
+        return node.op == "call_module" and isinstance(mods[node.target], layer) and sites[node.target] == 1
+
+    return gm, mods, conv
+
+
+def _chain_edges(gm, mods, conv, scheme):
+    """The single-user edge rule of chain_int8 / chain_affine (residual=False) on the traced `gm`."""
     edges, between = [], []
     for q in list(gm.graph.nodes):
         if not conv(q) or len(q.args) != 1 or q.kwargs or not isinstance(q.args[0], fx.Node):
@@ -1221,13 +1394,14 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     producers = {p: c for p, _, c in edges}
     consumers = {q for _, q, _ in edges}
     for target in producers.keys() | consumers:
-        requant = None
+        requant, sums = None, False
         if target in producers:
             nxt = mods[next(q for p, q, _ in edges if p == target)]
-            requant = (nxt.act_scale,) + tuple(producers[target])
+            requant = (scheme.out(scheme.key(nxt)),) + tuple(producers[target])
+            sums = nxt.groups == 1
         parent, _, attr = target.rpartition(".")
         setattr(gm.get_submodule(parent) if parent else gm, attr,
-                mods[target].chained(codes_in=target in consumers, requant=requant))
+                scheme.chained(mods[target], target in consumers, None, requant, None, None, sums))
     for p, q, path in between:
         q.args = (p,)
         for node in path:                                       # from the consumer side back: each has no user left
@@ -1238,8 +1412,10 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     return gm
 
 
-def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
-    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) on the traced `gm` (see chain_int8)."""
+def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None):
+    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True) on the traced
+    `gm` (see chain_int8); scheme: _NCNN (default) or _AFFINE."""
+    scheme = scheme or _NCNN
     full = (-_INF, _INF)
     order = {n: i for i, n in enumerate(gm.graph.nodes)}
 
@@ -1271,8 +1447,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
             node = node.args[0]
         return node if len(data_users(node, queries)) == 1 and producer(node) else None
 
-    def same(a, b):
-        return a.view(np.int32) == b.view(np.int32)
+    same = scheme.same
 
     # bilinear upsamples: the producer whose single-user pass-through chain ends at the upsample's input
     ends = {forward(p, full)[0]: p for p in gm.graph.nodes if producer(p)} if upsample else {}
@@ -1320,7 +1495,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
     def user_scale(u, tail, channels, pools=True):
         """The scale at which u takes the codes of `tail` (channels wide), or None when it takes fp32."""
         if producer(u) and u.args[0] is tail and mods[u.target].in_channels == channels:
-            return _f32(mods[u.target].act_scale)
+            return scheme.key(mods[u.target])
         if pools and pool_cat and _max_pool(u, mods) is not None and u.args[0] is tail:
             return pool_scale(u, channels)
         return None
@@ -1460,7 +1635,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
             add.prepend(p)
             p.args = (p.args[0], add.args[pl["ri"]])
         fp32 = any(u not in pl["codes"] for u in tail.users)
-        scale = float(pl["scale"]) if pl["codes"] else None
+        scale = scheme.out(pl["scale"]) if pl["codes"] else None
         clamp = pl["post"] if add is not None else pl["pre"]
         if add is None and not fp32:
             modes[p.target] = ("requant", (scale,) + tuple(clamp))
@@ -1570,14 +1745,14 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False):
         pools.append((u.name, pp["mode"], ("codes",) if codes_mode else ("fp32", "codes")))
 
     consumers = {q for _, q, _ in edges}
+    dense = {p for p, q, _ in edges if mods[q].groups == 1}          # producers whose codes a dense consumer reads
     for target in modes.keys() | consumers:
         kind, arg = modes.get(target, (None, None))
         parent, _, attr = target.rpartition(".")
         setattr(gm.get_submodule(parent) if parent else gm, attr,
-                mods[target].chained(codes_in=target in consumers, name=target,
-                                     requant=arg if kind == "requant" else (arg[0] if kind == "slice" else None),
-                                     epilogue=arg if kind == "epilogue" else None,
-                                     out_slice=arg[1] if kind == "slice" else None))
+                scheme.chained(mods[target], target in consumers, target,
+                               arg if kind == "requant" else (arg[0] if kind == "slice" else None),
+                               arg if kind == "epilogue" else None, arg[1] if kind == "slice" else None, target in dense))
     g.lint()
     gm.recompile()
     gm.requantized_edges = edges

@@ -44,7 +44,7 @@ int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
- * 11 DfqI8Resize, 12 DfqI8Affine): lets a binding verify
+ * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -576,6 +576,37 @@ int dfq_i8_affine_pack(const float* w, float w_min, float w_scale, int32_t num_b
  * DFQ_E_ARG: non-finite constants, a dense layer without S or table; DFQ_E_UNSUPPORTED: K >= 131072, other groupings. */
 int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8_t* wq, const int32_t* table, const DfqI8Affine* k,
                        const float* bias, float* y, int32_t* acc_out, const DfqI8Conv* g, void* stream);
+/* The affine residual epilogue of dfq_i8_affine_conv_fused, for layers chained through the next layer's codes.  Per output
+ * element (n, o, p), the ops of the per-layer path in its order:
+ *   v  = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o]          as dfq_i8_affine_conv
+ *   v  = v < pre_lo ? pre_lo : (v > pre_hi ? pre_hi : v)       NaN stays NaN
+ *   v  = fp32(v + residual[n, o, p])                           only when residual != NULL: fp32 NCHW [N, O, OH, OW]
+ *   v  = v < post_lo ? post_lo : (v > post_hi ? post_hi : v)
+ *   y[n, o, p]  = v                                            when y != NULL: fp32 NCHW [N, O, OH, OW]
+ *   yq[n, p, o] = the code dfq_i8_affine_quantize gives v at (out_min, out_max, out_bits), the CONSUMER's range: int8 NHWC
+ *                 [N, OH, OW, round_up(O, 16)] when yq != NULL, pad channels 0 (NaN -> -128, +-inf saturate)
+ *   S[n, p]     = the sum of yq[n, p, :] over the O real channels (int32 [N, OH, OW]) when S != NULL: what
+ *                 dfq_i8_affine_quantize writes, bit for bit, for a dense consumer
+ * No clamp is (-inf, +inf). */
+typedef struct DfqI8AffineEpilogue {
+  const float* residual;
+  float* y;
+  int8_t* yq;
+  int32_t* S;
+  float out_min, out_max;
+  int32_t out_bits;
+  float pre_lo, pre_hi, post_lo, post_hi;
+} DfqI8AffineEpilogue;
+/* The convolution of dfq_i8_affine_conv (inputs as there: xq and S_in, the layer's own input codes and sums) with the
+ * epilogue *e.  When S is written by more than one tile (O > 64 dense, O > 16 depthwise) the call zeroes it on `stream`
+ * first and the kernel adds into it.  DFQ_E_ARG, with a reason: y and yq both NULL, S without yq, yq not 16-byte aligned,
+ * residual, y or S not 4-byte aligned, NaN or unordered bounds in either clamp, and while yq is written an output range
+ * dfq_i8_affine_quantize refuses (non-finite, or a scale that is not a finite fp32 number) or out_bits < 1; outputs that
+ * overlap each other or the residual (extents from the geometry).  DFQ_E_UNSUPPORTED: out_bits > 8.  Refusals of
+ * dfq_i8_affine_conv as there. */
+int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                             const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e, const DfqI8Conv* g,
+                             void* stream);
 
 #ifdef __cplusplus
 }

@@ -17,7 +17,9 @@ chain_int8(..., upsample=True) and chain_int8(..., layout=True) (zero pads folde
 into their concatenation) on the networks of tests/deeplab_mobilenet_padded.py (8 x 513x513) and tests/ssd_lite_like.py
 (256 x 300x300).  `affine` (only when asked for: --sections affine): the reference's own asymmetric min / max quantization
 executed in integers (int8.convert_affine) against the fake-quantized model and the ncnn per-layer int8 model on
-MobileNetV2 and ResNet-18, with the logit errors against the fake-quantized model.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+MobileNetV2 and ResNet-18, with the logit errors against the fake-quantized model.  `affine_chained` (only when asked
+for): the fake-quantized model, convert_affine per layer, int8.chain_affine and chain_affine(residual=True) on the same
+networks, the three affine arms' logits asserted bit-identical.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
 device; writes nothing.
 """
 import argparse
@@ -646,6 +648,87 @@ def affine_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def affine_chained_inference(dev, reps=10, batch=256, rounds=5):
+    """The affine int8 path with activations carried as the consumers' shifted codes (int8.chain_affine) on the networks of
+    affine_inference, timed alternately with the fake-quantized model and the per-layer convert_affine model, `rounds`
+    rounds of `reps` passes, median: images/s, ms per batch, edges and fused adds, the fp32 traffic the residual arm avoids
+    per batch against the per-layer path (computed from shapes), and bit-identity of the three affine arms' logits
+    (asserted)."""
+    import copy
+    import statistics
+    from collections import OrderedDict
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_calibrated
+    from dfq_b200 import int8
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds,
+           "fp32_bytes_avoided_note": "fp32 bytes of the per-layer path that the residual arm does not move, per batch: per "
+                                      "element of every carried tensor, the quantizer's fp32 read (4 B) per carried consumer, "
+                                      "plus the producer's fp32 store (4 B) when no fp32 consumer is left; a read and a write "
+                                      "(8 B) per deleted pass-through; per fused add, its two reads and its write (12 B)"}
+    try:
+        x = torch.randn(batch, 3, 224, 224, device=dev, generator=torch.Generator(device=dev).manual_seed(3)).clamp_(-2.5, 2.5)
+        for net in ("mobilenet_v2", "resnet18"):
+            fq, _, qtarg = affine_calibrated.calibrated(net)
+            aff = copy.deepcopy(fq)
+            int8.convert_affine(aff, OrderedDict((id(m), m) for m in aff.modules() if type(m) in qtarg), qtarg)
+            chained = int8.chain_affine(aff)
+            gm = int8.chain_affine(aff, residual=True)
+            arms = (("fake_quant", fq), ("affine_per_layer", aff), ("affine_chained", chained), ("affine_residual", gm))
+            numel, mods = {}, dict(aff.named_modules())
+            hooks = [m.register_forward_hook(lambda m, i, o, n=n: numel.__setitem__(n, o.numel())) for n, m in mods.items()
+                     if isinstance(m, int8.AffineInt8Conv2d)]
+            with torch.no_grad():
+                ref = aff(x)
+                for h in hooks:
+                    h.remove()
+                logits = {k: m(x) for k, m in arms[2:]}
+                same = {k: bool(torch.equal(ref.view(torch.int32), v.view(torch.int32))) for k, v in logits.items()}
+                assert all(same.values()), same
+                traced, kept = int8._Int8Tracer().trace(aff), {n.name for n in gm.graph.nodes}
+                avoided = sum(4 * numel[p] for p, _, _ in gm.requantized_edges)
+                avoided += sum(4 * numel[n] for n, m in gm.named_modules() if isinstance(m, int8.AffineInt8Conv2d) and
+                               m.epilogue is not None and m.epilogue.out_scale is not None and not m.epilogue.fp32)
+                for n in traced.nodes:
+                    if n.name in kept or n.op not in ("call_module", "call_function", "call_method"):
+                        continue
+                    src = n.args[0] if n.args and isinstance(n.args[0], torch.fx.Node) else None
+                    while src is not None and not (src.op == "call_module" and src.target in numel):
+                        src = src.args[0] if src.args and isinstance(src.args[0], torch.fx.Node) else None
+                    if src is not None:
+                        avoided += numel[src.target] * (12 if int8._is_add(n) else 8)
+                for _ in range(2):
+                    for _, m in arms:
+                        m(x)
+                torch.cuda.synchronize(dev)
+                ms = {k: [] for k, _ in arms}
+                for _ in range(rounds):
+                    for k, m in arms:
+                        ms[k].append(timed(lambda m=m: m(x)))
+            med = {k: statistics.median(v) for k, v in ms.items()}
+            out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                        "ms_per_batch_rounds": ms, "edges": {"chained": len(chained.requantized_edges),
+                                                             "residual": len(gm.requantized_edges)},
+                        "fused_adds": len(gm.fused_adds), "fp32_bytes_avoided_per_batch": avoided,
+                        "logits_bit_identical_to_per_layer": same}
+            del fq, aff, chained, gm, logits
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -667,7 +750,7 @@ def main():
     p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
-                   help="comma-separated sections to run (default: all but affine)")
+                   help="comma-separated sections to run (default: all but affine and affine_chained)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -687,6 +770,8 @@ def main():
         res["layout"] = layout_inference(dev, reps=args.reps, seg_batch=args.seg_batch, ssd_batch=args.ssd_batch)
     if "affine" in want:
         res["affine"] = affine_inference(dev, reps=args.reps, batch=args.batch)
+    if "affine_chained" in want:
+        res["affine_chained"] = affine_chained_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
