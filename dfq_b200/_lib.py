@@ -103,6 +103,9 @@ I8_AFFINE_EPILOGUE_DT = np.dtype([(f, np.uint64) for f in ("residual", "y", "yq"
                                  [("out_min", np.float32), ("out_max", np.float32), ("out_bits", np.int32)] +
                                  [(f, np.float32) for f in ("pre_lo", "pre_hi", "post_lo", "post_hi")], align=True)
 
+I8_AFFINE_OBSERVE_DT = np.dtype([("obs_min", np.float32), ("obs_max", np.float32), ("obs_bits", np.int32),
+                                 ("res_min", np.float32), ("res_max", np.float32), ("res_bits", np.int32)], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -110,6 +113,7 @@ EXPECTED_SIZES = {
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64), "DfqI8Resize": (I8_RESIZE_DT, 48),
     "DfqI8Affine": (I8_AFFINE_DT, 32), "DfqI8AffineEpilogue": (I8_AFFINE_EPILOGUE_DT, 64),
+    "DfqI8AffineObserve": (I8_AFFINE_OBSERVE_DT, 24),
 }
 
 _PF = C.c_void_p   # device float*
@@ -171,6 +175,8 @@ SIGNATURES = {
                            _ST],
     "dfq_i8_affine_conv_fused": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p, C.c_void_p,
                                  _ST],
+    "dfq_i8_affine_conv_observed": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

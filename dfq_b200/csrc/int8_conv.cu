@@ -32,6 +32,9 @@
 //   Out::AFFINE_FUSED      the same value through the clamps and residual add of Out::FUSED, then fp32 NCHW and / or the
 //                          NEXT layer's shifted codes and their per-pixel sums S (dfq_i8_affine_conv_fused), which keeps
 //                          affine activations in int8 between chained layers
+//   Out::AFFINE_OBSERVED   Out::AFFINE_FUSED with QuantMeasure's fake quantization (fake_quant<true>) on the value after the
+//                          first clamp and / or on the residual, each when its observer is on (dfq_i8_affine_conv_observed):
+//                          the observers the reference's replace_op() puts on a residual add's operands run in the epilogue
 #include <algorithm>
 #include <cmath>
 
@@ -55,7 +58,7 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED };
+enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED, AFFINE_OBSERVED };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -113,11 +116,20 @@ struct AffineFused : Affine {
   int cpad;
   bool S_atomic;
 };
+// The observed affine epilogue (DfqI8AffineObserve): AffineFused's, with the fake quantization of `obs` on the value after
+// the pre clamp (obs_on) and of `res` on the residual (res_on).
+struct AffineObserved : AffineFused {
+  QuantScalars obs, res;
+  bool obs_on, res_on;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
 template <> struct EpiOf<Out::ROWS> { using type = Rows; };
 template <> struct EpiOf<Out::AFFINE> { using type = Affine; };
 template <> struct EpiOf<Out::AFFINE_FUSED> { using type = AffineFused; };
+template <> struct EpiOf<Out::AFFINE_OBSERVED> { using type = AffineObserved; };
+__host__ __device__ constexpr bool affine_out(Out o) { return o == Out::AFFINE || o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED; }
+__host__ __device__ constexpr bool affine_epilogue(Out o) { return o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED; }
 
 // fp32(kP P + kA A + kW Wv + kN Nv) + b: each product and sum a separately rounded double op, in this order
 __device__ __forceinline__ float affine_value(int32_t P, int32_t A, int32_t Wv, int32_t Nv, float b, const Affine& e) {
@@ -151,6 +163,18 @@ __device__ __forceinline__ float fused_value(int32_t acc, float dq, float b, flo
   float v = clamp_keep_nan(dequant(acc, dq, b), e.pre_lo, e.pre_hi);
   if (e.r) v = __fadd_rn(v, rv);
   return clamp_keep_nan(v, e.post_lo, e.post_hi);
+}
+
+// The observed add of Out::AFFINE_OBSERVED after the pre clamp: QuantMeasure's eval-mode output (common.cuh fake_quant, the
+// reciprocal multiply of CUDA tensors) of v and of the residual r[idx], each when its observer is on, then the fp32 add.
+__device__ __forceinline__ float observed_add(float v, int64_t idx, const AffineObserved& e) {
+  if (e.obs_on) v = fake_quant<true>(v, e.obs);
+  if (e.r) {
+    float rv = e.r[idx];
+    if (e.res_on) rv = fake_quant<true>(rv, e.res);
+    v = __fadd_rn(v, rv);
+  }
+  return v;
 }
 
 // fused_value without a residual, for the Rows epilogue
@@ -396,7 +420,7 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
   cp_async_wait<0>();
   __syncthreads();
 
-  if constexpr (OUT == Out::AFFINE || OUT == Out::AFFINE_FUSED) {
+  if constexpr (affine_out(OUT)) {
     // Past the [o][m] staging below: per pixel of the tile (THREADS == BM, one each) A = the sum of S over its in-image
     // taps and the tap rectangle (r0 | r1 << 16, s0 | s1 << 16).
     static_assert(THREADS == BM && BN * EPI_LD * 4 + BM * 12 <= STAGES * STAGE_BYTES, "affine epilogue staging");
@@ -469,7 +493,11 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
           const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
           float v = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
           v = clamp_keep_nan(v, rq.pre_lo, rq.pre_hi);
-          if (rq.r) v = __fadd_rn(v, rq.r[idx]);
+          if constexpr (OUT == Out::AFFINE_OBSERVED) {
+            v = observed_add(v, idx, rq);
+          } else {
+            if (rq.r) v = __fadd_rn(v, rq.r[idx]);
+          }
           v = clamp_keep_nan(v, rq.post_lo, rq.post_hi);
           if (y) y[idx] = v;
           code = affine_code(v, rq.neg_min, rq.inv_scale, rq.qmax);
@@ -649,8 +677,8 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
     const int64_t t = i / OHW;
     const int ch = (int)(t % chunks);
     const int64_t n = t / chunks;
-    constexpr bool affine = OUT == Out::AFFINE || OUT == Out::AFFINE_FUSED;
-    if constexpr (OUT == Out::I8 || OUT == Out::FUSED || OUT == Out::AFFINE_FUSED) {
+    constexpr bool affine = affine_out(OUT);
+    if constexpr (OUT == Out::I8 || OUT == Out::FUSED || affine_epilogue(OUT)) {
       // the input's Cpad may be wider than yq's cpad = round_up(O, 16): chunks past it hold only pad channels, and yq has
       // no room for them
       if (ch * 16 >= rq.cpad) continue;
@@ -695,7 +723,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
       }
       continue;
     }
-    if constexpr (OUT == Out::AFFINE_FUSED) {                   // as Out::FUSED; the pixel's sum shared by its chunks
+    if constexpr (affine_epilogue(OUT)) {                       // as Out::FUSED; the pixel's sum shared by its chunks
       alignas(16) int8_t v[16];
       int32_t sum = 0;
 #pragma unroll
@@ -706,7 +734,11 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
           const int64_t idx = (n * g.C + c) * OHW + p;
           float f = affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq);
           f = clamp_keep_nan(f, rq.pre_lo, rq.pre_hi);
-          if (rq.r) f = __fadd_rn(f, rq.r[idx]);
+          if constexpr (OUT == Out::AFFINE_OBSERVED) {
+            f = observed_add(f, idx, rq);
+          } else {
+            if (rq.r) f = __fadd_rn(f, rq.r[idx]);
+          }
           f = clamp_keep_nan(f, rq.post_lo, rq.post_hi);
           if (y) y[idx] = f;
           v[j] = affine_code(f, rq.neg_min, rq.inv_scale, rq.qmax);
@@ -1299,26 +1331,58 @@ extern "C" int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8
   return 0;
 }
 
-extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
-                                        const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
-                                        const DfqI8Conv* g, void* stream) {
-  const char* who = "dfq_i8_affine_conv_fused";
-  if (int rc = check_affine(g, 8, who)) return rc;
-  DFQ_REQUIRE(xq && wq && k && e, "dfq_i8_affine_conv_fused: null pointer");
-  DFQ_REQUIRE(g->groups != 1 || (S_in && table), "dfq_i8_affine_conv_fused: a dense layer needs S and its prefix table");
-  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_affine_conv_fused: codes must be 16-byte aligned");
-  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
-    set_error("dfq_i8_affine_conv_fused: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", k->kP, k->kA,
-              k->kW, k->kN);
+namespace dfq {
+namespace {
+
+#define DFQ_REQUIRE_WHO(cond, msg)                                         \
+  do {                                                                     \
+    if (!(cond)) {                                                         \
+      ::dfq::set_error("%s: %s (%s)", who, msg, #cond);                    \
+      return DFQ_E_ARG;                                                    \
+    }                                                                      \
+  } while (0)
+
+// An observer of DfqI8AffineObserve: off (bits 0), or QuantMeasure's scalars of a finite range with 1..8 bits.
+int observer_scalars(const char* who, const char* which, float lo, float hi, int32_t bits, QuantScalars* q, bool* on) {
+  *on = bits > 0;
+  if (bits < 0) {
+    set_error("%s: %s_bits must be 0 (off) or in [1, 8], got %d", who, which, bits);
     return DFQ_E_ARG;
   }
-  DFQ_REQUIRE(e->y || e->yq, "dfq_i8_affine_conv_fused: no output requested (y and yq are both NULL)");
-  DFQ_REQUIRE(!e->S || e->yq, "dfq_i8_affine_conv_fused: S is the sum of the codes; it needs yq");
-  DFQ_REQUIRE(aligned16(e->yq), "dfq_i8_affine_conv_fused: yq must be 16-byte aligned");
-  DFQ_REQUIRE(((uintptr_t)e->residual & 3) == 0 && ((uintptr_t)e->y & 3) == 0 && ((uintptr_t)e->S & 3) == 0,
-              "dfq_i8_affine_conv_fused: residual, y and S must be 4-byte aligned");
-  DFQ_REQUIRE(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
-              "dfq_i8_affine_conv_fused: pre / post clamp bounds must be ordered and not NaN");
+  if (bits > 8) {
+    set_error("%s: %s_bits = %d: the epilogue's observers have at most 8 bits", who, which, bits);
+    return DFQ_E_UNSUPPORTED;
+  }
+  if (!*on) return 0;
+  *q = quant_scalars((double)lo, (double)hi, bits, 0);
+  if (!(std::isfinite(lo) && std::isfinite(hi) && std::isfinite(q->scale) && std::isfinite(q->inv_scale))) {
+    set_error("%s: the %s observer's range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
+              which, lo, hi);
+    return DFQ_E_ARG;
+  }
+  return 0;
+}
+
+// dfq_i8_affine_conv_fused (o == NULL, Out::AFFINE_FUSED) and dfq_i8_affine_conv_observed (Out::AFFINE_OBSERVED)
+template <Out OUT>
+int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                         const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e, const DfqI8AffineObserve* o,
+                         const DfqI8Conv* g, void* stream) {
+  if (int rc = check_affine(g, 8, who)) return rc;
+  DFQ_REQUIRE_WHO(xq && wq && k && e, "null pointer");
+  DFQ_REQUIRE_WHO(g->groups != 1 || (S_in && table), "a dense layer needs S and its prefix table");
+  DFQ_REQUIRE_WHO(aligned16(xq) && aligned16(wq), "codes must be 16-byte aligned");
+  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
+    set_error("%s: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", who, k->kP, k->kA, k->kW, k->kN);
+    return DFQ_E_ARG;
+  }
+  DFQ_REQUIRE_WHO(e->y || e->yq, "no output requested (y and yq are both NULL)");
+  DFQ_REQUIRE_WHO(!e->S || e->yq, "S is the sum of the codes; it needs yq");
+  DFQ_REQUIRE_WHO(aligned16(e->yq), "yq must be 16-byte aligned");
+  DFQ_REQUIRE_WHO(((uintptr_t)e->residual & 3) == 0 && ((uintptr_t)e->y & 3) == 0 && ((uintptr_t)e->S & 3) == 0,
+                  "residual, y and S must be 4-byte aligned");
+  DFQ_REQUIRE_WHO(ordered(e->pre_lo, e->pre_hi) && ordered(e->post_lo, e->post_hi),
+                  "pre / post clamp bounds must be ordered and not NaN");
   QuantScalars qs{};
   if (e->yq) {                                                  // the consumer's quantizer, as dfq_i8_affine_quantize
     if (e->out_bits < 1 || e->out_bits > 8) {
@@ -1335,19 +1399,26 @@ extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, c
   const int cpad = (g->O + 15) / 16 * 16;
   const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
   const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float), yq_bytes = pixels * cpad, s_bytes = pixels * 4;
-  DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes) &&
-                  !overlap(e->residual, y_bytes, e->S, s_bytes),
-              "dfq_i8_affine_conv_fused: residual overlaps y, yq or S");
-  DFQ_REQUIRE(!overlap(e->y, y_bytes, e->yq, yq_bytes) && !overlap(e->y, y_bytes, e->S, s_bytes) &&
-                  !overlap(e->yq, yq_bytes, e->S, s_bytes),
-              "dfq_i8_affine_conv_fused: y, yq and S overlap");
+  DFQ_REQUIRE_WHO(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes) &&
+                      !overlap(e->residual, y_bytes, e->S, s_bytes),
+                  "residual overlaps y, yq or S");
+  DFQ_REQUIRE_WHO(!overlap(e->y, y_bytes, e->yq, yq_bytes) && !overlap(e->y, y_bytes, e->S, s_bytes) &&
+                      !overlap(e->yq, yq_bytes, e->S, s_bytes),
+                  "y, yq and S overlap");
   const bool dense = g->groups == 1;
-  DFQ_REQUIRE(!dense || (pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_affine_conv_fused: too many output pixels");
+  DFQ_REQUIRE_WHO(!dense || (pixels + BM - 1) / BM < (1LL << 31), "too many output pixels");
+  typename EpiOf<OUT>::type ep{};
+  if constexpr (OUT == Out::AFFINE_OBSERVED) {
+    DFQ_REQUIRE_WHO(o != nullptr, "null observer descriptor");
+    if (int rc = observer_scalars(who, "obs", o->obs_min, o->obs_max, o->obs_bits, &ep.obs, &ep.obs_on)) return rc;
+    if (int rc = observer_scalars(who, "res", o->res_min, o->res_max, o->res_bits, &ep.res, &ep.res_on)) return rc;
+    DFQ_REQUIRE_WHO(!ep.res_on || e->residual, "the residual's observer is on but there is no residual");
+    DFQ_REQUIRE_WHO(ep.obs_on || ep.res_on, "both observers are off (dfq_i8_affine_conv_fused computes that)");
+  }
   // one writer per pixel of S: a dense layer whose 64-channel tile covers O, a depthwise one with one 16-channel chunk
   const bool atomic = e->S && (dense ? g->O > BN : cpad > 16);
   cudaStream_t st = (cudaStream_t)stream;
   if (atomic) DFQ_CUDA(cudaMemsetAsync(e->S, 0, s_bytes, st));
-  AffineFused ep{};
   static_cast<Affine&>(ep) = Affine{S_in, table, k->kP, k->kA, k->kW, k->kN};
   ep.r = e->residual, ep.yq = e->yq, ep.S_out = e->S;
   ep.neg_min = qs.neg_min, ep.inv_scale = qs.inv_scale, ep.qmax = qs.qmax;
@@ -1355,12 +1426,30 @@ extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, c
   ep.cpad = cpad, ep.S_atomic = atomic;
   if (dense) {
     const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::AFFINE_FUSED><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, ep);
+    k_i8_conv_mma<OUT><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, ep);
   } else {
     const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::AFFINE_FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total,
-                                                                           ep);
+    k_i8_conv_dw<OUT><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total, ep);
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;
+}
+
+#undef DFQ_REQUIRE_WHO
+
+}  // namespace
+}  // namespace dfq
+
+extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                        const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                                        const DfqI8Conv* g, void* stream) {
+  return affine_conv_epilogue<Out::AFFINE_FUSED>("dfq_i8_affine_conv_fused", xq, S_in, wq, table, k, bias, e, nullptr, g,
+                                                 stream);
+}
+
+extern "C" int dfq_i8_affine_conv_observed(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                           const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                                           const DfqI8AffineObserve* o, const DfqI8Conv* g, void* stream) {
+  return affine_conv_epilogue<Out::AFFINE_OBSERVED>("dfq_i8_affine_conv_observed", xq, S_in, wq, table, k, bias, e, o, g,
+                                                    stream);
 }

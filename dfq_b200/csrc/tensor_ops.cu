@@ -482,6 +482,7 @@ extern "C" int dfq_struct_size(int which) {
     case 11: return (int)sizeof(DfqI8Resize);
     case 12: return (int)sizeof(DfqI8Affine);
     case 13: return (int)sizeof(DfqI8AffineEpilogue);
+    case 14: return (int)sizeof(DfqI8AffineObserve);
     default: return -1;
   }
 }

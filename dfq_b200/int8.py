@@ -19,10 +19,15 @@ tensors between converted layers stay fp32.
 
 convert_affine executes the reference's own quantization instead (asymmetric per-tensor min / max, dfq_i8_affine_*): called
 AFTER quantize_targ_layer and the activation ranges, it recovers the weight codes from the fake-quantized weights and
-computes each layer from integer sums, equal to the fake-quantized layer up to fp32 rounding.
+computes each layer from integer sums, equal to the fake-quantized layer up to fp32 rounding.  chain_affine carries its codes
+between layers; in the reference's evaluation state (replace_op() active with a CustomTensorOP) it replays the functional-op
+observers into its graph and runs those on a producer's path in that producer's epilogue (dfq_i8_affine_conv_observed), so it
+computes what the per-layer model computes under the patched ops.
 """
 import ctypes as C
 import operator
+import os
+import sys
 from typing import NamedTuple, Optional, Tuple
 
 import numpy as np
@@ -408,6 +413,7 @@ class _AffineInt8Layer(nn.Module):
     codes_in = False
     epilogue = None
     sums = False
+    observers = (None, None)
 
     def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
                  name=None):
@@ -507,6 +513,19 @@ class _AffineInt8Layer(nn.Module):
         new.sums = bool(sums) and epilogue is not None and epilogue.out_scale is not None
         return new
 
+    def observe(self, obs=None, res=None):
+        """Give this chained layer's epilogue the functional-op observers of the reference's evaluation state
+        (dfq_i8_affine_conv_observed): obs = (running_min, running_max, num_bits) of the QuantMeasure on v after the first
+        clamp (the fused operand of an observed add, or the producer's observed fp32 output), res = that of the one on
+        the residual; None: no observer.  Returns self."""
+        if self.epilogue is None:
+            raise _lib.DfqError("layer %s: observers run in a chained layer's epilogue" % self._who())
+        if res is not None and not self.epilogue.residual:
+            raise _lib.DfqError("layer %s: an observer on the residual needs a residual input" % self._who())
+        self.observers = tuple(None if o is None else _observer_range(o, "layer %s: %s observer" % (self._who(), w))
+                               for o, w in ((obs, "operand"), (res, "residual")))
+        return self
+
     def _input(self, x):
         """(codes, S | None, N, H, W) of the input: quantized here from fp32, or the pair a codes_in layer takes."""
         lib, st = _lib.load(), _lib.stream_ptr()
@@ -581,11 +600,18 @@ class _AffineInt8Layer(nn.Module):
         d = np.zeros(1, _lib.I8_AFFINE_EPILOGUE_DT)
         d[0] = tuple(0 if t is None else t.data_ptr() for t in (r, y, yq, S_out)) + (e.out_scale or (0.0, 0.0, 0)) + \
             e.pre + e.post
-        _lib.check(_lib.load().dfq_i8_affine_conv_fused(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
-                                                        _ptr(self.tap_table) if self.tap_table.numel() else None,
-                                                        _lib.table_ptr(self.constants), _ptr(self.bias), _lib.table_ptr(d),
-                                                        _lib.table_ptr(g), _lib.stream_ptr()),
-                   "dfq_i8_affine_conv_fused (layer %s)" % self._who())
+        lib, args = _lib.load(), (_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                  _ptr(self.tap_table) if self.tap_table.numel() else None, _lib.table_ptr(self.constants),
+                                  _ptr(self.bias), _lib.table_ptr(d))
+        obs, res = self.observers
+        if obs is None and res is None:
+            _lib.check(lib.dfq_i8_affine_conv_fused(*args, _lib.table_ptr(g), _lib.stream_ptr()),
+                       "dfq_i8_affine_conv_fused (layer %s)" % self._who())
+        else:
+            o = np.zeros(1, _lib.I8_AFFINE_OBSERVE_DT)
+            o[0] = (obs or (0.0, 0.0, 0)) + (res or (0.0, 0.0, 0))
+            _lib.check(lib.dfq_i8_affine_conv_observed(*args, _lib.table_ptr(o), _lib.table_ptr(g), _lib.stream_ptr()),
+                       "dfq_i8_affine_conv_observed (layer %s)" % self._who())
         codes = None if yq is None else (yq, S_out)
         return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
 
@@ -594,6 +620,18 @@ class _AffineInt8Layer(nn.Module):
                "w_scale=%g %d-bit" % (self.in_channels, self.out_channels, self.kernel_size, self.stride, self.padding,
                                       self.dilation, self.groups, self.act_min, self.act_max, self.act_bits, self.w_min,
                                       self.w_scale, self.w_bits)
+
+
+def _observer_range(o, who):
+    """(min, max, bits) of an epilogue observer as fp32 / int, or DfqError naming it: 1 to 8 bits and a range whose
+    QuantMeasure scale is a finite fp32 number."""
+    lo, hi, bits = o
+    if not isinstance(bits, (int, np.integer)) or isinstance(bits, bool) or not 1 <= bits <= 8:
+        raise _lib.DfqError("%s: %r bits do not fit the int8 epilogue (1 to 8 bits)" % (who, bits))
+    ma, fa = act_affine_scalars(lo, hi, bits)
+    if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(hi))):
+        raise _lib.DfqError("%s: range [%g, %g] gives no finite fp32 scale" % (who, lo, hi))
+    return float(_f32(lo)), float(_f32(hi)), int(bits)
 
 
 def _affine_refusal(who, C_in, C_out, groups, kernel_size, act_bits, w_bits):
@@ -884,13 +922,31 @@ def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
 _INF = float("inf")
 
 
+_TORCH_DIR = os.path.dirname(torch.__file__) + os.sep
+
+
 class _Int8Tracer(fx.Tracer):
     """symbolic tracing that keeps the int8 layers (whose forward calls the library) as leaves.  To chain_int8 the affine
     layers of convert_affine are opaque leaves (they are no Int8Conv2d, so nothing is fused into or out of them), and to
-    chain_affine the ncnn layers are."""
+    chain_affine the ncnn layers are.  callers=True records in node.meta["caller"] the (function name, line) of the first
+    frame outside torch that made each call node: the frame the reference's patched ops inspect."""
+
+    def __init__(self, callers=False):
+        super().__init__()
+        self.callers = callers
 
     def is_leaf_module(self, m, qualname):
         return isinstance(m, (_Int8Layer, _AffineInt8Layer)) or super().is_leaf_module(m, qualname)
+
+    def create_proxy(self, kind, target, args, kwargs, *rest, **kw):
+        proxy = super().create_proxy(kind, target, args, kwargs, *rest, **kw)
+        if self.callers and kind in ("call_function", "call_method"):
+            f = sys._getframe(1)
+            while f is not None and f.f_code.co_filename.startswith(_TORCH_DIR):
+                f = f.f_back
+            if f is not None:
+                proxy.node.meta["caller"] = (f.f_code.co_name, f.f_lineno)
+        return proxy
 
 
 def _arg(node, i, name, default):
@@ -1006,6 +1062,35 @@ def _bilinear_upsample(node, mods):
             isinstance(v, fx.Node) or (isinstance(v, int) and not isinstance(v, bool)) for v in size)):
         return None
     return size, ac
+
+
+def _observer_key(node, mods):
+    """(min, max, bits) of a call of a QuantMeasure whose fake quantization the affine epilogue runs bit for bit: eval
+    mode, update_stat falsy (its range is frozen), 1 to 8 bits, a range whose scale is a finite fp32 number; None for
+    any other node (such an observer stays in torch)."""
+    from .utils.quantize import QuantMeasure
+    if node.op != "call_module" or len(node.args) != 1 or node.kwargs or not isinstance(node.args[0], fx.Node):
+        return None
+    m = mods.get(node.target)
+    if type(m) is not QuantMeasure or m.training or m.update_stat:
+        return None
+    try:
+        return _observer_range((float(m.running_min.reshape(-1)[0]), float(m.running_max.reshape(-1)[0]), m.num_bits),
+                               node.target)
+    except _lib.DfqError:
+        return None
+
+
+def _is_view(node):
+    """view / reshape / flatten of one fx node by constant or shape-query arguments: the same elements, another shape."""
+    if not node.args or not isinstance(node.args[0], fx.Node) or node.kwargs.get("out") is not None:
+        return False
+    rest = list(node.args[1:]) + list(node.kwargs.values())
+    flat = [v for a in rest for v in (a if isinstance(a, (tuple, list)) else (a,))]
+    if not all(not isinstance(v, fx.Node) or _shape_only(v) for v in flat):
+        return False
+    return (node.op == "call_method" and node.target in ("view", "reshape", "flatten")) or \
+        (node.op == "call_function" and node.target in (torch.flatten, torch.reshape))
 
 
 def _shape_query(u, node):
@@ -1322,11 +1407,34 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False) -> fx.Gra
     The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
     edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) the clamp
     the consumer's codes were taken after; with residual=True the fused adds in `fused_adds`: (producer name, add node
-    name, residual node name, (lo, hi) before the add, (lo, hi) after it), as chain_int8 records them."""
-    gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer)
+    name, residual node name, (lo, hi) before the add, (lo, hi) after it), as chain_int8 records them.
+
+    In the reference's evaluation state - replace_op() active and utils.layer_transform.module_tensor_op a CustomTensorOP, as
+    main_*.py --quantize run - the functional ops fake-quantize their inputs with their own QuantMeasure.  chain_affine then
+    traces with the raw ops (the patched state is restored even when the trace raises), records each call's caller (the
+    first frame outside torch) and replays the cursor protocol of utils/layer_transform.py on the graph in node order: an
+    operator.add of two tensors matches add_<L>_2 or iadd_<L>_2, torch.cat of n tensors torch_cat_<L>_<n>, torch.mean /
+    F.interpolate / F.softmax ..._<L>_1, only when called from a function named `forward`; a match inserts call_module nodes
+    of the next observers on the op's operands (add: input, then the other; cat: in order).  DfqError when the live
+    cursors are not at 0 or the graph does not consume the records exactly once.  With residual=True:
+    - an add whose fused operand is observer(P's single-user pass-through chain) runs in P's epilogue with that observer
+      after the clamp before the add and the residual operand's observer on the fp32 residual (dfq_i8_affine_conv_observed);
+    - an observer on a producer's single-user pass-through chain, optionally followed by view / reshape / flatten (shape
+      queries do not count as users), is applied in that producer's epilogue to its fp32 output;
+    - observers with a truthy update_stat, in training mode, above 8 bits or with a non-finite range stay in torch.
+    Folded observers are deleted and recorded in `fused_observers`: (observer module, "operand" / "residual" / "output",
+    producer name).  The result's tensor adds are torch.add and its cat / mean / interpolate / softmax the raw ops, so its
+    forward can run while replace_op() stays active.  Outside that state nothing here changes."""
+    LT = _observed_state()
+    gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer, LT)
     if residual:
-        return _chain_residual(gm, mods, conv, scheme=_AFFINE)
-    return _chain_edges(gm, mods, conv, _AFFINE)
+        gm = _chain_residual(gm, mods, conv, scheme=_AFFINE)
+    else:
+        gm = _chain_edges(gm, mods, conv, _AFFINE)
+        gm.fused_observers = []
+    if LT is not None:
+        _unpatch_adds(gm, LT)
+    return gm
 
 
 class _Scheme(NamedTuple):
@@ -1353,12 +1461,157 @@ _AFFINE = _Scheme(AffineInt8Conv2d, lambda m: (_f32(m.act_min), _f32(m.act_max),
                       codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, sums=sums))
 
 
-def _trace(model, concrete_args, layer):
+def _observed_state():
+    """utils.layer_transform when the reference's evaluation state is active - replace_op() in place and a CustomTensorOP
+    as module_tensor_op (what main_*.py --quantize run, through dropin/) - else None."""
+    from .utils import layer_transform as LT
+    if LT.raw_torch_op.get("cat") is None or torch.cat is not LT.torch_cat or \
+            not isinstance(LT.module_tensor_op, LT.CustomTensorOP):
+        return None
+    return LT
+
+
+_OBSERVER_ROOT = "custom_tensor_op"
+
+
+_INT_ARITH = (operator.add, operator.sub, operator.mul, operator.floordiv, operator.truediv, operator.mod, operator.neg,
+              operator.pow)
+
+
+def _shape_only(n):
+    """n is an int or a shape - a size / dim / numel / .shape query, an item of one, or arithmetic on such nodes and
+    constants (x.size(2) * 2 + 1) - not a tensor."""
+    if n.op == "call_method" and n.target in ("size", "dim", "numel"):
+        return True
+    if n.op == "call_function" and n.target is getattr:
+        return True
+    if n.op == "call_function" and n.target is operator.getitem:
+        return isinstance(n.args[0], fx.Node) and _shape_only(n.args[0])
+    if n.op == "call_function" and n.target in _INT_ARITH and not n.kwargs:
+        nodes = [a for a in n.args if isinstance(a, fx.Node)]
+        return bool(nodes) and all(_shape_only(a) for a in nodes) and \
+            all(isinstance(a, fx.Node) or (isinstance(a, (int, float)) and not isinstance(a, bool)) for a in n.args)
+    return False
+
+
+def _replay_observers(gm, model, LT):
+    """Insert the observers of LT.module_tensor_op into the traced gm as call_module nodes, where the patched ops would
+    apply them: the cursor protocol of utils/layer_transform.py replayed on the graph in node order, on copies of the
+    cursors.  Returns nothing; raises DfqError when the cursors are not at 0 or the records are not consumed exactly once."""
+    ct = LT.module_tensor_op
+    recs = [r[1] for r in ct.name_tensor_op]
+    if ct.idx_name_tensor_op != 0 or ct.idx_tensor_op != 0:
+        raise _lib.DfqError("chain_affine: the functional-op observers' cursors are at record %d, observer %d, not 0: a "
+                            "forward was interrupted" % (ct.idx_name_tensor_op, ct.idx_tensor_op))
+    root = {id(m): n for n, m in model.named_modules()}.get(id(ct)) or _OBSERVER_ROOT
+    gm.add_submodule(root, ct)                                  # the observers are leaves: called, not traced
+    raw = {LT.raw_torch_op["cat"]: "torch_cat", LT.raw_torch_op["mean"]: "torch_mean",
+           LT.raw_func_op["interpolate"]: "F_interpolate", LT.raw_func_op["softmax"]: "F_softmax"}
+    i_rec, i_obs, consumed = 0, 0, 0
+    for node in list(gm.graph.nodes):
+        caller = node.meta.get("caller")
+        if node.op != "call_function" or caller is None or caller[0] != "forward" or not recs:
+            continue
+        line = caller[1]
+        if node.target is operator.add:
+            ops = node.args[:2]
+            if len(node.args) != 2 or node.kwargs or not all(isinstance(a, fx.Node) and not _shape_only(a) for a in ops):
+                continue
+            names_ok = ("add_%d_2" % line, "iadd_%d_2" % line)
+        elif node.target in raw and node.args:
+            if raw[node.target] == "torch_cat":
+                ts = node.args[0]
+                if not isinstance(ts, (list, tuple)) or not all(isinstance(t, fx.Node) for t in ts):
+                    continue
+                ops, names_ok = tuple(ts), ("torch_cat_%d_%d" % (line, len(ts)),)
+            else:
+                if not isinstance(node.args[0], fx.Node):
+                    continue
+                ops, names_ok = (node.args[0],), ("%s_%d_1" % (raw[node.target], line),)
+        else:
+            continue
+        if recs[i_rec] not in names_ok:
+            continue
+        obs = []
+        for t in ops:
+            with gm.graph.inserting_before(node):
+                obs.append(gm.graph.call_module("%s.%d" % (root, i_obs), (t,)))
+            i_obs = (i_obs + 1) % ct.len
+        if node.target is operator.add:
+            node.args = tuple(obs)
+        elif raw[node.target] == "torch_cat":
+            node.args = (type(node.args[0])(obs),) + tuple(node.args[1:])
+        else:
+            node.args = (obs[0],) + tuple(node.args[1:])
+        i_rec = (i_rec + 1) % len(recs)
+        consumed += 1
+    if consumed != len(recs):
+        raise _lib.DfqError("chain_affine: the traced graph %s the functional-op records: %s" % (
+            "consumes more than once" if consumed > len(recs) else "leaves unmatched",
+            "%d calls for %d records" % (consumed, len(recs)) if consumed > len(recs) else
+            "first unmatched record %r (record %d of %d)" % (recs[i_rec], i_rec, len(recs))))
+
+
+def _unpatch_adds(gm, LT):
+    """Make gm's generated forward immune to the patched ops: tensor operator.add -> torch.add (bit-identical, not
+    patched), and torch.cat / mean, F.interpolate / softmax -> the raw ops called through module-level functions (the
+    generated code would otherwise name the patched torch.cat etc.)."""
+    raw = {LT.raw_torch_op["cat"]: _raw_cat, LT.raw_torch_op["mean"]: _raw_mean,
+           LT.raw_func_op["interpolate"]: _raw_interpolate, LT.raw_func_op["softmax"]: _raw_softmax}
+    for node in gm.graph.nodes:
+        if node.op != "call_function":
+            continue
+        if node.target is operator.add and node.args and isinstance(node.args[0], fx.Node) and \
+                not _shape_only(node.args[0]):
+            node.target = torch.add
+        elif node.target in raw:
+            node.target = raw[node.target]
+    gm.recompile()
+
+
+def _raw(table, name):
+    from .utils import layer_transform as LT
+    return getattr(LT, table)[name]
+
+
+def _raw_cat(*a, **k):
+    return _raw("raw_torch_op", "cat")(*a, **k)
+
+
+def _raw_mean(*a, **k):
+    return _raw("raw_torch_op", "mean")(*a, **k)
+
+
+def _raw_interpolate(*a, **k):
+    return _raw("raw_func_op", "interpolate")(*a, **k)
+
+
+def _raw_softmax(*a, **k):
+    return _raw("raw_func_op", "softmax")(*a, **k)
+
+
+def _trace(model, concrete_args, layer, observed=None):
     """(GraphModule of `model` traced with the int8 layers as leaves, its modules by name, conv(node): node calls a
-    `layer` module that is called at no other site)."""
-    tracer = _Int8Tracer()
-    graph = tracer.trace(model, concrete_args)
+    `layer` module that is called at no other site).  observed: utils.layer_transform in the reference's evaluation state
+    (_observed_state): the model is traced with the raw ops in place (restored in every case) and the functional-op
+    observers are inserted as call_module nodes (_replay_observers)."""
+    tracer = _Int8Tracer(callers=observed is not None)
+    if observed is None:
+        graph = tracer.trace(model, concrete_args)
+    else:
+        LT = observed
+        patched = [(o, n, getattr(o, n)) for o, names in ((torch.Tensor, LT.tensor_magic_op_supported),
+                                                          (torch, LT.torch_op_supported), (F, LT.func_op_sopprted))
+                   for n in names]
+        try:
+            LT.restore_op()
+            graph = tracer.trace(model, concrete_args)
+        finally:
+            for o, n, f in patched:
+                setattr(o, n, f)
     gm = fx.GraphModule(tracer.root, graph, type(model).__name__ + "Int8Chained")
+    if observed is not None:
+        _replay_observers(gm, model, observed)
     mods = dict(gm.named_modules())
     sites = {}
     for node in gm.graph.nodes:
@@ -1437,6 +1690,13 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     def data_users(node, queries):
         """node's users, without those that only read its shape when `queries`."""
         return [u for u in node.users if not (queries and _shape_query(u, node))]
+
+    def observe(node):
+        """node calls a QuantMeasure the affine epilogue runs (_observer_key) and has one user."""
+        return scheme is _AFFINE and len(node.users) == 1 and _observer_key(node, mods) is not None
+
+    def unobserved(node):
+        return node.args[0] if observe(node) else node
 
     def back_to_producer(node, queries=False):
         """The producer whose single-user pass-through chain ends at `node`, or None.  queries: users that only read a
@@ -1526,13 +1786,19 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             continue
         end, pre, path = forward(p, full)
         add, ri, post, post_path, tail = None, None, full, [], end
+        fobs = robs = None
         if len(end.users) == 1:
             a = next(iter(end.users))
+            if observe(a):                                      # the observer on the fused operand (replace_op's add)
+                fobs, a = a, next(iter(a.users))
             if _is_add(a):
-                fused = next((i for i, v in enumerate(a.args) if back_to_producer(v) is not None), None)
-                if fused is not None and a.args[fused] is end:
+                fused = next((i for i, v in enumerate(a.args) if back_to_producer(unobserved(v)) is not None), None)
+                if fused is not None and unobserved(a.args[fused]) is end and (fobs is None or a.args[fused] is fobs):
                     add, ri = a, 1 - fused
                     tail, post, post_path = forward(a, full)
+                    robs = a.args[ri] if observe(a.args[ri]) else None
+            if add is None:
+                fobs = None
         out_c = mods[p.target].out_channels
         codes, scale = take_codes(tail, out_c)
         clamp = post if add is not None else pre
@@ -1548,10 +1814,32 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         if add is None and not codes:
             continue
         plans.append(dict(p=p, path=path, pre=pre, add=add, ri=ri, post=post, post_path=post_path, tail=tail, codes=codes,
-                          scale=scale))
+                          scale=scale, obs=fobs, robs=robs))
         for u in codes:
             if not producer(u):
                 codes_pool(u, out_c, clamp)
+
+    # observers on a producer's fp32 output: its single-user pass-through chain, then shape-only views, then the observer
+    # (shape queries not counted as users); the producer applies it in its epilogue and writes the observed fp32 output
+    taken = {n for pl in plans for n in (pl.get("obs"), pl.get("robs")) if n is not None}
+    planned = {pl["p"] for pl in plans}
+    for o in (list(gm.graph.nodes) if scheme is _AFFINE else []):
+        if o in taken or _observer_key(o, mods) is None:
+            continue
+        node = o.args[0]
+        while _is_view(node) and len(data_users(node, True)) == 1:
+            node = node.args[0]
+        q = back_to_producer(node, queries=True)
+        if q is None or q in planned:
+            continue
+        path, clamp, n = [], full, node
+        while n is not q:
+            clamp = _compose(_pass_through(n, mods), clamp)
+            path.append(n)
+            n = n.args[0]
+        plans.append(dict(p=q, path=path[::-1], pre=clamp, add=None, ri=None, post=full, post_path=[], tail=node, codes=[],
+                          scale=None, obs=o, robs=None, output=True))
+        planned.add(q)
 
     # concatenations whose operands come from their own producers and whose users all take codes at one scale
     cat_plans = []
@@ -1616,7 +1904,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         pl["skipped"] = []
         if pl["add"] is None:
             continue
-        r = pl["add"].args[pl["ri"]]
+        r = pl["robs"].args[0] if pl.get("robs") is not None else pl["add"].args[pl["ri"]]
         while r not in claimed and len(r.users) == 1 and _is_identity(r, mods) and isinstance(r.args[0], fx.Node):
             pl["skipped"].append(r)
             r = r.args[0]
@@ -1625,23 +1913,27 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     # rewrite in producer order: a producer's input may be the codes of an earlier one, and a residual its fp32 output
     g = gm.graph
     convs = {n for n in g.nodes if producer(n)}                 # before the rewrites give producers a second input
-    edges, adds, modes = [], [], {}
+    edges, adds, modes, observed, watched = [], [], {}, [], {}
     for pl in plans:
         p, add, tail = pl["p"], pl["add"], pl["tail"]
+        fobs, robs = pl.get("obs"), pl.get("robs")
         if add is not None:
             for node in pl["skipped"]:                          # from the add back: each loses its only user
                 node.replace_all_uses_with(node.args[0])
                 g.erase_node(node)
             add.prepend(p)
-            p.args = (p.args[0], add.args[pl["ri"]])
+            p.args = (p.args[0], robs.args[0] if robs is not None else add.args[pl["ri"]])
         fp32 = any(u not in pl["codes"] for u in tail.users)
         scale = scheme.out(pl["scale"]) if pl["codes"] else None
         clamp = pl["post"] if add is not None else pl["pre"]
+        keys = tuple(None if o is None else _observer_key(o, mods) for o in (fobs, robs))
         if add is None and not fp32:
             modes[p.target] = ("requant", (scale,) + tuple(clamp))
             codes_node = y_node = p
         else:
             modes[p.target] = ("epilogue", Epilogue(scale, pl["pre"], pl["post"], add is not None, fp32))
+            if keys != (None, None):
+                watched[p.target] = keys
             codes_node = y_node = p
             if scale is not None and fp32:
                 with g.inserting_after(p):
@@ -1652,12 +1944,22 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             u.replace_input_with(tail, codes_node)
             if u in convs:
                 edges.append((p.target, u.target, clamp))
+        for node in pl["path"]:                                 # shape queries inside the chain read p's output
+            for u in [u for u in node.users if _shape_query(u, node)]:
+                u.replace_input_with(node, y_node)
         if tail is not p:
             tail.replace_all_uses_with(y_node)
-            for node in reversed([*pl["path"], *([add] if add is not None else []), *pl["post_path"]]):
+            on_add = [o for o in (fobs, robs) if o is not None and add is not None]
+            for node in reversed([*pl["path"], *on_add, *([add] if add is not None else []), *pl["post_path"]]):
                 g.erase_node(node)
         else:
             p.replace_all_uses_with(y_node, delete_user_cb=lambda u: u not in (y_node, codes_node))
+        if pl.get("output"):                                    # the views now read the observed output
+            fobs.replace_all_uses_with(fobs.args[0])
+            g.erase_node(fobs)
+            observed.append((fobs.target, "output", p.target))
+        elif add is not None:
+            observed += [(o.target, what, p.target) for o, what in ((fobs, "operand"), (robs, "residual")) if o is not None]
         if add is not None:
             adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
 
@@ -1749,14 +2051,16 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     for target in modes.keys() | consumers:
         kind, arg = modes.get(target, (None, None))
         parent, _, attr = target.rpartition(".")
-        setattr(gm.get_submodule(parent) if parent else gm, attr,
-                scheme.chained(mods[target], target in consumers, target,
-                               arg if kind == "requant" else (arg[0] if kind == "slice" else None),
-                               arg if kind == "epilogue" else None, arg[1] if kind == "slice" else None, target in dense))
+        mod = scheme.chained(mods[target], target in consumers, target,
+                             arg if kind == "requant" else (arg[0] if kind == "slice" else None),
+                             arg if kind == "epilogue" else None, arg[1] if kind == "slice" else None, target in dense)
+        setattr(gm.get_submodule(parent) if parent else gm, attr, mod.observe(*watched[target]) if target in watched else mod)
     g.lint()
     gm.recompile()
     gm.requantized_edges = edges
     gm.fused_adds = adds
+    if scheme is _AFFINE:
+        gm.fused_observers = observed
     if pool_cat:
         gm.fused_cats = cats
         gm.fused_pools = pools

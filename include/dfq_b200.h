@@ -44,7 +44,7 @@ int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
- * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue): lets a binding verify
+ * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -607,6 +607,32 @@ typedef struct DfqI8AffineEpilogue {
 int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                              const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e, const DfqI8Conv* g,
                              void* stream);
+/* The observers the reference's replace_op() puts on functional ops (QuantMeasure in eval mode without update_stat), run in
+ * the affine epilogue.  With fq(t, lo, hi, b) = what QuantMeasure returns for t at running_min lo, running_max hi and
+ * num_bits b on a CUDA tensor (the double prologue of the fake quantization, a reciprocal multiply, rint, clamp to
+ * [0, 2^b - 1], fp32(fp32(q * scale) + min); NaN stays NaN, +-inf saturate), dfq_i8_affine_conv_observed computes per
+ * output element, in this order:
+ *   v  = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o]          as dfq_i8_affine_conv
+ *   v  = v < pre_lo ? pre_lo : (v > pre_hi ? pre_hi : v)
+ *   v  = fq(v, obs_min, obs_max, obs_bits)                     when obs_bits > 0: the observer on the fused operand
+ *   r  = fq(residual[n, o, p], res_min, res_max, res_bits)     when res_bits > 0 (residual[n, o, p] when 0)
+ *   v  = fp32(v + r)                                           only when residual != NULL
+ *   v  = v < post_lo ? post_lo : (v > post_hi ? post_hi : v)
+ *   y, yq and S as dfq_i8_affine_conv_fused.
+ * An observer with bits 0 is off. */
+typedef struct DfqI8AffineObserve {
+  float obs_min, obs_max;
+  int32_t obs_bits;
+  float res_min, res_max;
+  int32_t res_bits;
+} DfqI8AffineObserve;
+/* dfq_i8_affine_conv_fused with the observers *o.  Refusals of dfq_i8_affine_conv_fused as there, and DFQ_E_ARG with a
+ * reason: o NULL, an observer with bits < 0 or (when on) a non-finite range or a scale that is not a finite fp32 number,
+ * res_bits > 0 without a residual, both observers off (dfq_i8_affine_conv_fused computes that).  DFQ_E_UNSUPPORTED: an
+ * observer with bits > 8.  Nothing is written when a call is refused. */
+int dfq_i8_affine_conv_observed(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                                const DfqI8AffineObserve* o, const DfqI8Conv* g, void* stream);
 
 #ifdef __cplusplus
 }

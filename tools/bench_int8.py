@@ -19,7 +19,11 @@ into their concatenation) on the networks of tests/deeplab_mobilenet_padded.py (
 executed in integers (int8.convert_affine) against the fake-quantized model and the ncnn per-layer int8 model on
 MobileNetV2 and ResNet-18, with the logit errors against the fake-quantized model.  `affine_chained` (only when asked
 for): the fake-quantized model, convert_affine per layer, int8.chain_affine and chain_affine(residual=True) on the same
-networks, the three affine arms' logits asserted bit-identical.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+networks, the three affine arms' logits asserted bit-identical.  `affine_observed` (only when asked for): the same
+networks in the reference's evaluation state (tests/affine_observed_state.py: replace_op() active, the functional-op
+observers on every residual add and, for MobileNetV2 with the reference's head, on the mean's input), timing the
+fake-quantized model, the per-layer convert_affine model and chain_affine(residual=True), which runs the observers in its
+epilogues; the two affine arms' logits asserted bit-identical.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
 device; writes nothing.
 """
 import argparse
@@ -729,6 +733,63 @@ def affine_chained_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def affine_observed_inference(dev, reps=10, batch=256, rounds=5):
+    """MobileNetV2 (the reference's mean head) and ResNet-18 in the reference's evaluation state: the fake-quantized model,
+    convert_affine per layer and chain_affine(residual=True), all with replace_op() active, timed alternately, `rounds`
+    rounds of `reps` passes, median; the fused adds and observers, and bit-identity of the two affine arms' logits
+    (asserted)."""
+    import copy
+    import statistics
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_observed_state
+    from dfq_b200 import int8
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds}
+    try:
+        x = torch.randn(batch, 3, 224, 224, device=dev, generator=torch.Generator(device=dev).manual_seed(3)).clamp_(-2.5, 2.5)
+        for net in ("mobilenet_v2", "resnet18"):
+            with affine_observed_state.evaluation_state(net) as (model, qgraph, qtarg):
+                fq = copy.deepcopy(model)
+                int8.convert_affine(model, qgraph, qtarg)
+                gm = int8.chain_affine(model, residual=True)
+                arms = (("fake_quant", fq), ("affine_per_layer", model), ("affine_observed", gm))
+                with torch.no_grad():
+                    same = bool(torch.equal(model(x).view(torch.int32), gm(x).view(torch.int32)))
+                    assert same, net
+                    for _ in range(2):
+                        for _, m in arms:
+                            m(x)
+                    torch.cuda.synchronize(dev)
+                    ms = {k: [] for k, _ in arms}
+                    for _ in range(rounds):
+                        for k, m in arms:
+                            ms[k].append(timed(lambda m=m: m(x)))
+                med = {k: statistics.median(v) for k, v in ms.items()}
+                kinds = [w for _, w, _ in gm.fused_observers]
+                out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                            "ms_per_batch_rounds": ms, "observers": model.custom_tensor_op.len,
+                            "fused_observers": {k: kinds.count(k) for k in ("operand", "residual", "output")},
+                            "fused_adds": len(gm.fused_adds), "edges": len(gm.requantized_edges),
+                            "logits_bit_identical_to_per_layer": same}
+                del fq, gm
+            del model
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -750,7 +811,7 @@ def main():
     p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
-                   help="comma-separated sections to run (default: all but affine and affine_chained)")
+                   help="comma-separated sections to run (default: all but affine, affine_chained and affine_observed)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -772,6 +833,8 @@ def main():
         res["affine"] = affine_inference(dev, reps=args.reps, batch=args.batch)
     if "affine_chained" in want:
         res["affine_chained"] = affine_chained_inference(dev, reps=args.reps, batch=args.batch)
+    if "affine_observed" in want:
+        res["affine_observed"] = affine_observed_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
