@@ -7,12 +7,15 @@ import torch
 import torch.nn as nn
 
 
-def calibrated(net, batches=4, keep_unquantized=False):
+def calibrated(net, batches=4, keep_unquantized=False, bits_weight=8, bits_bias=16, quantize_on_cpu=False):
     """torchvision `net` (seeded, ReLU6 -> ReLU for MobileNetV2 as main_cls.py --relu does) through BN fold, equalization and
-    bias correction on its Conv2d / Linear layers, then QuantNConv2d / QuantNLinear layers with quantize_targ_layer's 8-bit
-    weights (16-bit biases) and observer ranges driven over `batches` batches of 16 synthetic images (update_quant_range's
-    way).  Returns (model, graph of its target layers, target types) and, with keep_unquantized, a copy of the model from
-    before quantize_targ_layer whose observers hold the same ranges (the input of int8.convert_to_int8)."""
+    bias correction on its Conv2d / Linear layers, then QuantNConv2d / QuantNLinear layers with quantize_targ_layer's
+    `bits_weight`-bit weights (`bits_bias`-bit biases) and observer ranges driven over `batches` batches of 16 synthetic
+    images (update_quant_range's way).  quantize_on_cpu: quantize_targ_layer runs before the model moves to the GPU, as in
+    the reference's main_cls.py / main_seg.py / main_ssd.py, so the parameters are fake-quantized with true division (the
+    CPU recipe) instead of the reciprocal multiply of CUDA tensors.  Returns (model, graph of its target layers, target
+    types) and, with keep_unquantized, a copy of the model from before quantize_targ_layer whose observers hold the same
+    ranges (the input of int8.convert_to_int8)."""
     import torchvision
     from dfq_b200 import dfq
     from dfq_b200.improve_dfq import set_update_stat
@@ -53,11 +56,14 @@ def calibrated(net, batches=4, keep_unquantized=False):
             q.load_state_dict(ch.state_dict(), strict=False)
             setattr(parent, name, q)
     swap(model)
-    model = model.cuda().eval()
+    model = model.eval() if quantize_on_cpu else model.cuda().eval()
     qtarg = [Q.QuantNConv2d, Q.QuantNLinear]
     qgraph = OrderedDict((id(m), m) for m in model.modules() if type(m) in qtarg)
     pre = copy.deepcopy(model) if keep_unquantized else None
-    LT.quantize_targ_layer(qgraph, 8, 16, qtarg)
+    LT.quantize_targ_layer(qgraph, bits_weight, bits_bias, qtarg)
+    if quantize_on_cpu:
+        model.cuda()
+        pre = None if pre is None else pre.cuda()
     set_update_stat(model, [Q.QuantMeasure], True)
     g = torch.Generator(device="cuda").manual_seed(1)
     with torch.no_grad():

@@ -1,5 +1,5 @@
-"""Models in the reference's evaluation state (main_cls.py / main_seg.py --quantize), for the affine observer tests and
-tools/bench_int8.py (needs a CUDA device; torchvision for the classifiers).
+"""Models in the reference's evaluation state (main_cls.py / main_seg.py / main_ssd.py --quantize), for the affine observer
+tests and tools/bench_int8.py (needs a CUDA device; torchvision for the classifiers and SSD-Lite).
 
 The state: BN fold, equalization and bias correction, QuantNConv2d / QuantNLinear layers with quantize_targ_layer's 8-bit
 weights, a CustomTensorOP of one QuantMeasure per functional-op operand installed as `custom_tensor_op` (switch_layers'
@@ -37,6 +37,9 @@ def build(net):
     if net == "deeplab":
         from deeplab_mobilenet_padded import DeepLabMobileNetPadded
         return DeepLabMobileNetPadded()
+    if net == "ssd":
+        from ssd_lite_like import SSDLiteLike
+        return SSDLiteLike(21, is_test=True)
     import torchvision
     return getattr(torchvision.models, net)(num_classes=1000)
 
