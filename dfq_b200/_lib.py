@@ -106,6 +106,15 @@ I8_AFFINE_EPILOGUE_DT = np.dtype([(f, np.uint64) for f in ("residual", "y", "yq"
 I8_AFFINE_OBSERVE_DT = np.dtype([("obs_min", np.float32), ("obs_max", np.float32), ("obs_bits", np.int32),
                                  ("res_min", np.float32), ("res_max", np.float32), ("res_bits", np.int32)], align=True)
 
+I8_AFFINE_LAYOUT_DT = np.dtype([(f, np.int32) for f in ("coff", "cstride", "S_accumulate", "pad_code_on", "pad_code")],
+                               align=True)
+
+I8_AFFINE_RESIZE_DT = np.dtype([(f, np.int32) for f in ("N", "C", "H", "W", "OH", "OW", "align_corners", "coff", "cstride")] +
+                               [("pre_lo", np.float32), ("pre_hi", np.float32), ("obs_min", np.float32),
+                                ("obs_max", np.float32), ("obs_bits", np.int32), ("post_lo", np.float32),
+                                ("post_hi", np.float32), ("out_min", np.float32), ("out_max", np.float32),
+                                ("out_bits", np.int32)], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -113,7 +122,8 @@ EXPECTED_SIZES = {
     "DfqBcLayer": (BC_LAYER_DT, 80), "DfqQuantTask": (QUANT_TASK_DT, 32), "DfqI8Conv": (I8_CONV_DT, 72),
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64), "DfqI8Resize": (I8_RESIZE_DT, 48),
     "DfqI8Affine": (I8_AFFINE_DT, 32), "DfqI8AffineEpilogue": (I8_AFFINE_EPILOGUE_DT, 64),
-    "DfqI8AffineObserve": (I8_AFFINE_OBSERVE_DT, 24),
+    "DfqI8AffineObserve": (I8_AFFINE_OBSERVE_DT, 24), "DfqI8AffineLayout": (I8_AFFINE_LAYOUT_DT, 20),
+    "DfqI8AffineResize": (I8_AFFINE_RESIZE_DT, 76),
 }
 
 _PF = C.c_void_p   # device float*
@@ -177,6 +187,9 @@ SIGNATURES = {
                                  _ST],
     "dfq_i8_affine_conv_observed": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p,
                                     C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_affine_conv_layout": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_affine_upsample_bilinear": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

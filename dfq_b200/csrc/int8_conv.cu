@@ -35,6 +35,13 @@
 //   Out::AFFINE_OBSERVED   Out::AFFINE_FUSED with QuantMeasure's fake quantization (fake_quant<true>) on the value after the
 //                          first clamp and / or on the residual, each when its observer is on (dfq_i8_affine_conv_observed):
 //                          the observers the reference's replace_op() puts on a residual add's operands run in the epilogue
+//   Out::AFFINE_LAYOUT     Out::AFFINE_OBSERVED (either observer optional) whose codes go to a channel slice of a wider
+//                          tensor and whose S adds into a sum the concatenation's writers share, and whose out-of-image taps
+//                          may read a pad code z' instead of being left out (dfq_i8_affine_conv_layout): a zero F.pad folded
+//                          into the convolution.  Dense layers correct P, A, Wv and Nv in the epilogue; the depthwise main
+//                          loop reads z' (k_i8_conv_dw<..., true>).
+//   k_i8_affine_upsample   torch's bilinear upsample (k_i8_upsample_bilinear's value) through clamp, observer, clamp to the
+//                          consumer's codes in a channel slice, S added (dfq_i8_affine_upsample_bilinear)
 #include <algorithm>
 #include <cmath>
 
@@ -58,7 +65,7 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED, AFFINE_OBSERVED };
+enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED, AFFINE_OBSERVED, AFFINE_LAYOUT };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -122,14 +129,33 @@ struct AffineObserved : AffineFused {
   QuantScalars obs, res;
   bool obs_on, res_on;
 };
+// The layout epilogue (DfqI8AffineLayout): AffineObserved's, the codes of pixel m at yq + m * cstride (yq at the slice's
+// first channel), and with pad_on every out-of-image tap reading the shifted code pad_code over the C real channels.
+struct AffineLayout : AffineObserved {
+  int cstride, pad_code;
+  bool pad_on;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
 template <> struct EpiOf<Out::ROWS> { using type = Rows; };
 template <> struct EpiOf<Out::AFFINE> { using type = Affine; };
 template <> struct EpiOf<Out::AFFINE_FUSED> { using type = AffineFused; };
 template <> struct EpiOf<Out::AFFINE_OBSERVED> { using type = AffineObserved; };
-__host__ __device__ constexpr bool affine_out(Out o) { return o == Out::AFFINE || o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED; }
-__host__ __device__ constexpr bool affine_epilogue(Out o) { return o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED; }
+template <> struct EpiOf<Out::AFFINE_LAYOUT> { using type = AffineLayout; };
+__host__ __device__ constexpr bool affine_out(Out o) {
+  return o == Out::AFFINE || o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT;
+}
+__host__ __device__ constexpr bool affine_epilogue(Out o) {
+  return o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT;
+}
+__host__ __device__ constexpr bool observed(Out o) { return o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT; }
+
+// the int8 elements between two pixels' codes in yq: a tensor of its own (cpad), or a concatenation's (cstride)
+template <Out OUT>
+__device__ __forceinline__ int64_t code_stride(const typename EpiOf<OUT>::type& e) {
+  if constexpr (OUT == Out::AFFINE_LAYOUT) return e.cstride;
+  else return e.cpad;
+}
 
 // fp32(kP P + kA A + kW Wv + kN Nv) + b: each product and sum a separately rounded double op, in this order
 __device__ __forceinline__ float affine_value(int32_t P, int32_t A, int32_t Wv, int32_t Nv, float b, const Affine& e) {
@@ -485,15 +511,26 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
         if (m >= M) continue;
         int32_t code = 0;
         if (o < g.O) {
-          const int32_t P = st[ol * EPI_LD + ml];
+          int32_t P = st[ol * EPI_LD + ml];
           const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
           const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
           const int32_t* T = rq.table + (int64_t)o * tsize;
-          const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
+          int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
           const int64_t idx = ((m / OHW) * g.O + o) * OHW + m % OHW;
-          float v = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
+          int32_t A = sA[ml], Nv = (r1 - r0) * (s1 - s0) * g.C;
+          if constexpr (OUT == Out::AFFINE_LAYOUT) {
+            // the out-of-image taps loaded 0; with a pad code they hold z' over the C real channels, which adds
+            // z' (Wtot - Win) to P and z' C (taps - in-image taps) to A; Wv and Nv then cover every tap
+            if (rq.pad_on) {
+              const int32_t Wt = T[g.kh * tw + g.kw];
+              P += rq.pad_code * (Wt - Wv);
+              A += rq.pad_code * (g.kh * g.kw * g.C - Nv);
+              Wv = Wt, Nv = g.kh * g.kw * g.C;
+            }
+          }
+          float v = affine_value(P, A, Wv, Nv, bias ? bias[o] : 0.f, rq);
           v = clamp_keep_nan(v, rq.pre_lo, rq.pre_hi);
-          if constexpr (OUT == Out::AFFINE_OBSERVED) {
+          if constexpr (observed(OUT)) {
             v = observed_add(v, idx, rq);
           } else {
             if (rq.r) v = __fadd_rn(v, rq.r[idx]);
@@ -518,7 +555,7 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
           sum += v[j];
         }
         if (o0 + c * 16 < rq.cpad)
-          *reinterpret_cast<int4*>(rq.yq + m * rq.cpad + o0 + c * 16) = *reinterpret_cast<const int4*>(v);
+          *reinterpret_cast<int4*>(rq.yq + m * code_stride<OUT>(rq) + o0 + c * 16) = *reinterpret_cast<const int4*>(v);
       }
       if (rq.S_out) {
         if (rq.S_atomic) atomicAdd(rq.S_out + m, sum);
@@ -667,10 +704,12 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
 // ------------------------------------------------------------------------------------------------------------------
 // depthwise on the CUDA cores: one thread per (n, 16 channels, output pixel), pixels fastest
 // ------------------------------------------------------------------------------------------------------------------
-template <Out OUT>
+// PAD (Out::AFFINE_LAYOUT with a pad code): every tap counts, the out-of-image ones reading the code rq.pad_code.
+template <Out OUT, bool PAD = false>
 __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __restrict__ wq, const float* __restrict__ dq,
                              const float* __restrict__ bias, float* __restrict__ y, int32_t* __restrict__ acc_out, DfqI8Conv g,
                              int64_t total, typename EpiOf<OUT>::type rq) {
+  static_assert(!PAD || OUT == Out::AFFINE_LAYOUT, "a pad code is the layout epilogue's");
   const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int p = (int)(i % OHW);
@@ -693,22 +732,38 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
       for (int j = 0; j < 16; ++j) xsum[j] = wsum[j] = 0;
     }
     const int8_t* img = xq + n * g.H * g.W * g.Cpad + ch * 16;
-    for (int r = 0; r < g.kh; ++r) {
-      const int ih = oh * g.stride_h - g.pad_h + r * g.dil_h;
-      if ((unsigned)ih >= (unsigned)g.H) continue;
-      for (int s = 0; s < g.kw; ++s) {
-        const int iw = ow * g.stride_w - g.pad_w + s * g.dil_w;
-        if ((unsigned)iw >= (unsigned)g.W) continue;
-        const int4 xv = __ldg(reinterpret_cast<const int4*>(img + ((int64_t)ih * g.W + iw) * g.Cpad));
-        const int4 wv = __ldg(reinterpret_cast<const int4*>(wq + (r * g.kw + s) * g.Cpad + ch * 16));
-        const int8_t* xb = reinterpret_cast<const int8_t*>(&xv);
-        const int8_t* wb = reinterpret_cast<const int8_t*>(&wv);
+    auto mac = [&](const int4& xv, int r, int s) {
+      const int4 wv = __ldg(reinterpret_cast<const int4*>(wq + (r * g.kw + s) * g.Cpad + ch * 16));
+      const int8_t* xb = reinterpret_cast<const int8_t*>(&xv);
+      const int8_t* wb = reinterpret_cast<const int8_t*>(&wv);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
-        if constexpr (affine) {
+      for (int j = 0; j < 16; ++j) acc[j] += (int32_t)xb[j] * (int32_t)wb[j];
+      if constexpr (affine) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) xsum[j] += xb[j], wsum[j] += wb[j];
-          ++ntaps;
+        for (int j = 0; j < 16; ++j) xsum[j] += xb[j], wsum[j] += wb[j];
+        ++ntaps;
+      }
+    };
+    if constexpr (PAD) {
+      const int z = (int)(uint8_t)rq.pad_code * 0x01010101;    // z' in every byte (pad channels: weights 0)
+      const int4 zv = make_int4(z, z, z, z);
+      for (int r = 0; r < g.kh; ++r) {
+        const int ih = oh * g.stride_h - g.pad_h + r * g.dil_h;
+        const bool row = (unsigned)ih < (unsigned)g.H;
+        for (int s = 0; s < g.kw; ++s) {
+          const int iw = ow * g.stride_w - g.pad_w + s * g.dil_w;
+          mac(row && (unsigned)iw < (unsigned)g.W
+                  ? __ldg(reinterpret_cast<const int4*>(img + ((int64_t)ih * g.W + iw) * g.Cpad)) : zv, r, s);
+        }
+      }
+    } else {
+      for (int r = 0; r < g.kh; ++r) {
+        const int ih = oh * g.stride_h - g.pad_h + r * g.dil_h;
+        if ((unsigned)ih >= (unsigned)g.H) continue;
+        for (int s = 0; s < g.kw; ++s) {
+          const int iw = ow * g.stride_w - g.pad_w + s * g.dil_w;
+          if ((unsigned)iw >= (unsigned)g.W) continue;
+          mac(__ldg(reinterpret_cast<const int4*>(img + ((int64_t)ih * g.W + iw) * g.Cpad)), r, s);
         }
       }
     }
@@ -734,7 +789,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
           const int64_t idx = (n * g.C + c) * OHW + p;
           float f = affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq);
           f = clamp_keep_nan(f, rq.pre_lo, rq.pre_hi);
-          if constexpr (OUT == Out::AFFINE_OBSERVED) {
+          if constexpr (observed(OUT)) {
             f = observed_add(f, idx, rq);
           } else {
             if (rq.r) f = __fadd_rn(f, rq.r[idx]);
@@ -746,7 +801,7 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         }
       }
       if (rq.yq) {
-        *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * rq.cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
+        *reinterpret_cast<int4*>(rq.yq + (n * OHW + p) * code_stride<OUT>(rq) + ch * 16) = *reinterpret_cast<const int4*>(v);
         if (rq.S_out) {
           if (rq.S_atomic) atomicAdd(rq.S_out + n * OHW + p, sum);
           else rq.S_out[n * OHW + p] = sum;
@@ -895,6 +950,17 @@ __device__ __forceinline__ BilinearTap bilinear_tap(int dst, float scale, bool a
   return t;
 }
 
+// torch's output at (oh, ow) of one channel plane img [H, W] (copy: the size does not change)
+__device__ __forceinline__ float bilinear_value(const float* img, int W, int oh, int ow, const BilinearTap& th,
+                                                const BilinearTap& tw, bool copy) {
+  if (copy) return __ldg(img + (int64_t)oh * W + ow);
+  const float* r0 = img + (int64_t)th.i0 * W;
+  const float* r1 = img + (int64_t)th.i1 * W;
+  const float a = __fmaf_rn(tw.l0, __ldg(r0 + tw.i0), __fmul_rn(tw.l1, __ldg(r0 + tw.i1)));
+  const float b = __fmaf_rn(tw.l0, __ldg(r1 + tw.i0), __fmul_rn(tw.l1, __ldg(r1 + tw.i1)));
+  return __fmaf_rn(th.l0, a, __fmul_rn(th.l1, b));
+}
+
 __global__ void k_i8_upsample_bilinear(const float* __restrict__ x, float* __restrict__ y, int8_t* __restrict__ yq,
                                        DfqI8Resize g, float scale_h, float scale_w, int64_t total) {
   const int chunks = (g.C + 15) / 16;
@@ -914,22 +980,53 @@ __global__ void k_i8_upsample_bilinear(const float* __restrict__ x, float* __res
       const int c = ch * 16 + j;
       v[j] = 0;
       if (c >= g.C) continue;
-      const float* img = x + (n * g.C + c) * HW;
-      float f;
-      if (copy) {
-        f = __ldg(img + (int64_t)oh * g.W + ow);
-      } else {
-        const float* r0 = img + (int64_t)th.i0 * g.W;
-        const float* r1 = img + (int64_t)th.i1 * g.W;
-        const float a = __fmaf_rn(tw.l0, __ldg(r0 + tw.i0), __fmul_rn(tw.l1, __ldg(r0 + tw.i1)));
-        const float b = __fmaf_rn(tw.l0, __ldg(r1 + tw.i0), __fmul_rn(tw.l1, __ldg(r1 + tw.i1)));
-        f = __fmaf_rn(th.l0, a, __fmul_rn(th.l1, b));
-      }
+      const float f = bilinear_value(x + (n * g.C + c) * HW, g.W, oh, ow, th, tw, copy);
       if (y) y[(n * g.C + c) * OHW + p] = f;
       v[j] = q8(clamp_keep_nan(f, g.lo, g.hi), g.out_scale);
     }
     if (yq)
       *reinterpret_cast<int4*>(yq + (n * OHW + p) * g.cstride + g.coff + ch * 16) = *reinterpret_cast<const int4*>(v);
+  }
+}
+
+// The affine scheme's scalars of dfq_i8_affine_upsample_bilinear: the observer (obs_on) and the consumer's quantizer.
+struct AffineResize {
+  QuantScalars obs;
+  float neg_min, inv_scale, qmax;
+  float pre_lo, pre_hi, post_lo, post_hi;
+  bool obs_on;
+};
+
+// k_i8_upsample_bilinear's thread layout and value v, then clamp(pre), the observer, clamp(post) and the consumer's shifted
+// code into channels [coff, coff + round_up(C, 16)) of yq [N, OH, OW, cstride], the 16 codes' sum added to S[n, p].
+__global__ void k_i8_affine_upsample(const float* __restrict__ x, int8_t* __restrict__ yq, int32_t* __restrict__ S,
+                                     DfqI8AffineResize g, AffineResize a, float scale_h, float scale_w, int64_t total) {
+  const int chunks = (g.C + 15) / 16;
+  const int64_t HW = (int64_t)g.H * g.W, OHW = (int64_t)g.OH * g.OW;
+  const bool copy = g.H == g.OH && g.W == g.OW;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i % OHW;
+    const int64_t t = i / OHW;
+    const int ch = (int)(t % chunks);
+    const int64_t n = t / chunks;
+    const int oh = (int)(p / g.OW), ow = (int)(p % g.OW);
+    const BilinearTap th = bilinear_tap(oh, scale_h, g.align_corners, g.H);
+    const BilinearTap tw = bilinear_tap(ow, scale_w, g.align_corners, g.W);
+    alignas(16) int8_t v[16];
+    int32_t sum = 0;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = ch * 16 + j;
+      v[j] = 0;
+      if (c >= g.C) continue;
+      float f = clamp_keep_nan(bilinear_value(x + (n * g.C + c) * HW, g.W, oh, ow, th, tw, copy), a.pre_lo, a.pre_hi);
+      if (a.obs_on) f = fake_quant<true>(f, a.obs);
+      f = clamp_keep_nan(f, a.post_lo, a.post_hi);
+      v[j] = affine_code(f, a.neg_min, a.inv_scale, a.qmax);
+      sum += v[j];
+    }
+    *reinterpret_cast<int4*>(yq + (n * OHW + p) * g.cstride + g.coff + ch * 16) = *reinterpret_cast<const int4*>(v);
+    if (S) atomicAdd(S + n * OHW + p, sum);
   }
 }
 
@@ -1363,11 +1460,12 @@ int observer_scalars(const char* who, const char* which, float lo, float hi, int
   return 0;
 }
 
-// dfq_i8_affine_conv_fused (o == NULL, Out::AFFINE_FUSED) and dfq_i8_affine_conv_observed (Out::AFFINE_OBSERVED)
+// dfq_i8_affine_conv_fused (o == NULL, Out::AFFINE_FUSED), dfq_i8_affine_conv_observed (Out::AFFINE_OBSERVED) and
+// dfq_i8_affine_conv_layout (Out::AFFINE_LAYOUT: o NULL or observed's, the layout l)
 template <Out OUT>
 int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                          const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e, const DfqI8AffineObserve* o,
-                         const DfqI8Conv* g, void* stream) {
+                         const DfqI8AffineLayout* l, const DfqI8Conv* g, void* stream) {
   if (int rc = check_affine(g, 8, who)) return rc;
   DFQ_REQUIRE_WHO(xq && wq && k && e, "null pointer");
   DFQ_REQUIRE_WHO(g->groups != 1 || (S_in && table), "a dense layer needs S and its prefix table");
@@ -1398,37 +1496,59 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
   }
   const int cpad = (g->O + 15) / 16 * 16;
   const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
-  const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float), yq_bytes = pixels * cpad, s_bytes = pixels * 4;
-  DFQ_REQUIRE_WHO(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, e->yq, yq_bytes) &&
+  int64_t coff = 0, cstride = cpad;
+  bool accumulate = false;
+  if constexpr (OUT == Out::AFFINE_LAYOUT) {
+    DFQ_REQUIRE_WHO(l != nullptr, "null layout descriptor");
+    DFQ_REQUIRE_WHO(l->coff >= 0 && l->cstride > 0 && l->coff % 16 == 0 && l->cstride % 16 == 0,
+                    "coff and cstride must be non-negative multiples of 16");
+    DFQ_REQUIRE_WHO((int64_t)l->coff + cpad <= l->cstride, "the slice coff + round_up(O, 16) exceeds cstride");
+    DFQ_REQUIRE_WHO((l->S_accumulate == 0 || l->S_accumulate == 1) && (l->pad_code_on == 0 || l->pad_code_on == 1),
+                    "S_accumulate and pad_code_on must be 0 or 1");
+    DFQ_REQUIRE_WHO(!l->pad_code_on || (l->pad_code >= -128 && l->pad_code <= 127), "the pad code must be in [-128, 127]");
+    coff = l->coff, cstride = l->cstride, accumulate = l->S_accumulate == 1;
+  }
+  int8_t* yq = e->yq ? e->yq + coff : nullptr;
+  const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float), yq_bytes = (pixels - 1) * cstride + cpad;
+  const int64_t s_bytes = pixels * 4;
+  DFQ_REQUIRE_WHO(!overlap(e->residual, y_bytes, e->y, y_bytes) && !overlap(e->residual, y_bytes, yq, yq_bytes) &&
                       !overlap(e->residual, y_bytes, e->S, s_bytes),
                   "residual overlaps y, yq or S");
-  DFQ_REQUIRE_WHO(!overlap(e->y, y_bytes, e->yq, yq_bytes) && !overlap(e->y, y_bytes, e->S, s_bytes) &&
-                      !overlap(e->yq, yq_bytes, e->S, s_bytes),
+  DFQ_REQUIRE_WHO(!overlap(e->y, y_bytes, yq, yq_bytes) && !overlap(e->y, y_bytes, e->S, s_bytes) &&
+                      !overlap(yq, yq_bytes, e->S, s_bytes),
                   "y, yq and S overlap");
   const bool dense = g->groups == 1;
   DFQ_REQUIRE_WHO(!dense || (pixels + BM - 1) / BM < (1LL << 31), "too many output pixels");
   typename EpiOf<OUT>::type ep{};
-  if constexpr (OUT == Out::AFFINE_OBSERVED) {
-    DFQ_REQUIRE_WHO(o != nullptr, "null observer descriptor");
-    if (int rc = observer_scalars(who, "obs", o->obs_min, o->obs_max, o->obs_bits, &ep.obs, &ep.obs_on)) return rc;
-    if (int rc = observer_scalars(who, "res", o->res_min, o->res_max, o->res_bits, &ep.res, &ep.res_on)) return rc;
-    DFQ_REQUIRE_WHO(!ep.res_on || e->residual, "the residual's observer is on but there is no residual");
-    DFQ_REQUIRE_WHO(ep.obs_on || ep.res_on, "both observers are off (dfq_i8_affine_conv_fused computes that)");
+  if constexpr (observed(OUT)) {
+    DFQ_REQUIRE_WHO(OUT == Out::AFFINE_LAYOUT || o != nullptr, "null observer descriptor");
+    if (o) {
+      if (int rc = observer_scalars(who, "obs", o->obs_min, o->obs_max, o->obs_bits, &ep.obs, &ep.obs_on)) return rc;
+      if (int rc = observer_scalars(who, "res", o->res_min, o->res_max, o->res_bits, &ep.res, &ep.res_on)) return rc;
+      DFQ_REQUIRE_WHO(!ep.res_on || e->residual, "the residual's observer is on but there is no residual");
+      DFQ_REQUIRE_WHO(ep.obs_on || ep.res_on, "both observers are off (dfq_i8_affine_conv_fused computes that)");
+    }
   }
-  // one writer per pixel of S: a dense layer whose 64-channel tile covers O, a depthwise one with one 16-channel chunk
-  const bool atomic = e->S && (dense ? g->O > BN : cpad > 16);
+  // one writer per pixel of S: a dense layer whose 64-channel tile covers O, a depthwise one with one 16-channel chunk;
+  // a concatenation's writers add into the S its caller zeroed
+  const bool atomic = e->S && (accumulate || (dense ? g->O > BN : cpad > 16));
   cudaStream_t st = (cudaStream_t)stream;
-  if (atomic) DFQ_CUDA(cudaMemsetAsync(e->S, 0, s_bytes, st));
+  if (atomic && !accumulate) DFQ_CUDA(cudaMemsetAsync(e->S, 0, s_bytes, st));
   static_cast<Affine&>(ep) = Affine{S_in, table, k->kP, k->kA, k->kW, k->kN};
-  ep.r = e->residual, ep.yq = e->yq, ep.S_out = e->S;
+  ep.r = e->residual, ep.yq = yq, ep.S_out = e->S;
   ep.neg_min = qs.neg_min, ep.inv_scale = qs.inv_scale, ep.qmax = qs.qmax;
   ep.pre_lo = e->pre_lo, ep.pre_hi = e->pre_hi, ep.post_lo = e->post_lo, ep.post_hi = e->post_hi;
   ep.cpad = cpad, ep.S_atomic = atomic;
+  bool pad = false;
+  if constexpr (OUT == Out::AFFINE_LAYOUT) ep.cstride = (int)cstride, ep.pad_code = l->pad_code, ep.pad_on = pad = l->pad_code_on;
+  const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
   if (dense) {
     const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
     k_i8_conv_mma<OUT><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, ep);
+  } else if (pad) {
+    if constexpr (OUT == Out::AFFINE_LAYOUT)
+      k_i8_conv_dw<OUT, true><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total, ep);
   } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
     k_i8_conv_dw<OUT><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total, ep);
   }
   DFQ_CUDA(cudaGetLastError());
@@ -1443,13 +1563,67 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
 extern "C" int dfq_i8_affine_conv_fused(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                                         const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
                                         const DfqI8Conv* g, void* stream) {
-  return affine_conv_epilogue<Out::AFFINE_FUSED>("dfq_i8_affine_conv_fused", xq, S_in, wq, table, k, bias, e, nullptr, g,
-                                                 stream);
+  return affine_conv_epilogue<Out::AFFINE_FUSED>("dfq_i8_affine_conv_fused", xq, S_in, wq, table, k, bias, e, nullptr,
+                                                 nullptr, g, stream);
 }
 
 extern "C" int dfq_i8_affine_conv_observed(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                                            const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
                                            const DfqI8AffineObserve* o, const DfqI8Conv* g, void* stream) {
-  return affine_conv_epilogue<Out::AFFINE_OBSERVED>("dfq_i8_affine_conv_observed", xq, S_in, wq, table, k, bias, e, o, g,
-                                                    stream);
+  return affine_conv_epilogue<Out::AFFINE_OBSERVED>("dfq_i8_affine_conv_observed", xq, S_in, wq, table, k, bias, e, o,
+                                                    nullptr, g, stream);
+}
+
+extern "C" int dfq_i8_affine_conv_layout(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                         const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                                         const DfqI8AffineObserve* o, const DfqI8AffineLayout* l, const DfqI8Conv* g,
+                                         void* stream) {
+  return affine_conv_epilogue<Out::AFFINE_LAYOUT>("dfq_i8_affine_conv_layout", xq, S_in, wq, table, k, bias, e, o, l, g,
+                                                  stream);
+}
+
+extern "C" int dfq_i8_affine_upsample_bilinear(const float* x, int8_t* yq, int32_t* S, const DfqI8AffineResize* g,
+                                               void* stream) {
+  const char* who = "dfq_i8_affine_upsample_bilinear";
+  DFQ_REQUIRE(g != nullptr, "dfq_i8_affine_upsample_bilinear: null geometry");
+  DFQ_REQUIRE(x != nullptr && yq != nullptr, "dfq_i8_affine_upsample_bilinear: null input or codes");
+  DFQ_REQUIRE(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->OH > 0 && g->OW > 0,
+              "dfq_i8_affine_upsample_bilinear: empty dimension (every size must be positive)");
+  DFQ_REQUIRE(g->align_corners == 0 || g->align_corners == 1,
+              "dfq_i8_affine_upsample_bilinear: align_corners must be 0 or 1");
+  const int cpad = (g->C + 15) / 16 * 16;
+  DFQ_REQUIRE(g->coff >= 0 && g->cstride > 0 && g->coff % 16 == 0 && g->cstride % 16 == 0,
+              "dfq_i8_affine_upsample_bilinear: coff and cstride must be non-negative multiples of 16");
+  DFQ_REQUIRE((int64_t)g->coff + cpad <= g->cstride,
+              "dfq_i8_affine_upsample_bilinear: the slice coff + round_up(C, 16) exceeds cstride");
+  DFQ_REQUIRE(aligned16(yq) && ((uintptr_t)x & 3) == 0 && ((uintptr_t)S & 3) == 0,
+              "dfq_i8_affine_upsample_bilinear: yq must be 16-byte aligned, x and S 4-byte aligned");
+  DFQ_REQUIRE(ordered(g->pre_lo, g->pre_hi) && ordered(g->post_lo, g->post_hi),
+              "dfq_i8_affine_upsample_bilinear: pre / post clamp bounds must be ordered and not NaN");
+  AffineResize a{};
+  if (int rc = observer_scalars(who, "obs", g->obs_min, g->obs_max, g->obs_bits, &a.obs, &a.obs_on)) return rc;
+  if (g->out_bits < 1 || g->out_bits > 8) {
+    set_error("%s: out_bits must be in [1, 8], got %d", who, g->out_bits);
+    return g->out_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
+  }
+  const QuantScalars qs = quant_scalars((double)g->out_min, (double)g->out_max, g->out_bits, 0);
+  if (!(std::isfinite(g->out_min) && std::isfinite(g->out_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
+    set_error("%s: the output range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
+              g->out_min, g->out_max);
+    return DFQ_E_ARG;
+  }
+  const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
+  const int8_t* slice = yq + g->coff;
+  const int64_t x_bytes = in_px * g->C * 4, slice_bytes = (out_px - 1) * g->cstride + cpad, s_bytes = out_px * 4;
+  DFQ_REQUIRE(!overlap(x, x_bytes, slice, slice_bytes) && !overlap(x, x_bytes, S, s_bytes) &&
+                  !overlap(slice, slice_bytes, S, s_bytes),
+              "dfq_i8_affine_upsample_bilinear: x, the slice and S overlap");
+  a.neg_min = qs.neg_min, a.inv_scale = qs.inv_scale, a.qmax = qs.qmax;
+  a.pre_lo = g->pre_lo, a.pre_hi = g->pre_hi, a.post_lo = g->post_lo, a.post_hi = g->post_hi;
+  const int64_t total = out_px * (cpad / 16);
+  const bool ac = g->align_corners == 1;
+  k_i8_affine_upsample<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      x, yq, S, *g, a, bilinear_scale(g->H, g->OH, ac), bilinear_scale(g->W, g->OW, ac), total);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
 }

@@ -483,6 +483,8 @@ extern "C" int dfq_struct_size(int which) {
     case 12: return (int)sizeof(DfqI8Affine);
     case 13: return (int)sizeof(DfqI8AffineEpilogue);
     case 14: return (int)sizeof(DfqI8AffineObserve);
+    case 15: return (int)sizeof(DfqI8AffineLayout);
+    case 16: return (int)sizeof(DfqI8AffineResize);
     default: return -1;
   }
 }

@@ -22,7 +22,9 @@ AFTER quantize_targ_layer and the activation ranges, it recovers the weight code
 computes each layer from integer sums, equal to the fake-quantized layer up to fp32 rounding.  chain_affine carries its codes
 between layers; in the reference's evaluation state (replace_op() active with a CustomTensorOP) it replays the functional-op
 observers into its graph and runs those on a producer's path in that producer's epilogue (dfq_i8_affine_conv_observed), so it
-computes what the per-layer model computes under the patched ops.
+computes what the per-layer model computes under the patched ops.  chain_affine(concat=True, fold_pads=True) also folds zero
+pads into the convolutions after them as pad codes and has the producers and bilinear upsamples of channel concatenations
+write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear).
 """
 import ctypes as C
 import operator
@@ -408,12 +410,16 @@ class _AffineInt8Layer(nn.Module):
 
     Execution modes, set only on the copies chain_affine makes (`chained`): `codes_in` - the input is the pair (codes, S)
     another layer's epilogue wrote at this layer's range (S None for a depthwise layer); `epilogue` - an Epilogue whose
-    out_scale is the consumer's (act_min, act_max, act_bits) (dfq_i8_affine_conv_fused), with `sums` - write S too."""
+    out_scale is the consumer's (act_min, act_max, act_bits) (dfq_i8_affine_conv_fused), with `sums` - write S too;
+    `out_slice` = (coff, cstride) - the codes go to a channel slice of a concatenation's codes and S adds into its sums;
+    `pad_code` - the shifted code every out-of-image tap reads (a folded F.pad; dfq_i8_affine_conv_layout)."""
 
     codes_in = False
     epilogue = None
     sums = False
     observers = (None, None)
+    out_slice = None
+    pad_code = None
 
     def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
                  name=None):
@@ -473,17 +479,20 @@ class _AffineInt8Layer(nn.Module):
         return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
                                                                   self.kernel_size)
 
-    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False, out_slice=None):
         """A new module of the same class on the same buffers (weight_codes, tap_table, bias, constants), in the given
         execution mode: codes_in - take (codes, S) from the previous layer's epilogue instead of quantizing fp32; requant =
         ((act_min, act_max, act_bits), lo, hi) - return the consumer's codes after the clamp (lo, hi), the epilogue
         Epilogue(out, (lo, hi)); epilogue - an Epilogue whose out_scale is the consumer's (act_min, act_max, act_bits) or
         None (the residual epilogue, dfq_i8_affine_conv_fused); sums - the codes come with their per-pixel sums S (a dense
-        consumer reads them).  name: the layer's name in error messages.  self is not modified."""
+        consumer reads them); out_slice = (coff, cstride), with codes and no fp32 output - write them into channels
+        [coff, coff + round_up(C_out, 16)) of a concatenation's codes [N, OH, OW, cstride] and add S into its sums,
+        given as forward(x, out=(codes, S | None)) or made (S zeroed) when out is None.  The pad code of a folded F.pad is
+        kept.  name: the layer's name in error messages.  self is not modified."""
         new = type(self).__new__(type(self))
         nn.Module.__init__(new)
         for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad",
-                  "act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants"):
+                  "act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants", "pad_code"):
             setattr(new, k, getattr(self, k))
         for k, b in self._buffers.items():
             new.register_buffer(k, b)
@@ -511,6 +520,28 @@ class _AffineInt8Layer(nn.Module):
                                 bool(e.fp32))
         new.epilogue = epilogue
         new.sums = bool(sums) and epilogue is not None and epilogue.out_scale is not None
+        if out_slice is not None:
+            coff, cstride = (int(v) for v in out_slice)
+            if epilogue is None or epilogue.out_scale is None or epilogue.fp32 or epilogue.residual:
+                raise _lib.DfqError("layer %s: a channel slice takes the codes only, without a residual" % new._who())
+            if coff < 0 or coff % 16 or cstride % 16 or coff + (self.out_channels + 15) // 16 * 16 > cstride:
+                raise _lib.DfqError("layer %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
+                                    % (new._who(), coff, cstride))
+            out_slice = (coff, cstride)
+        new.out_slice = out_slice
+        return new
+
+    def fold_pad(self, pad):
+        """This layer's copy (chained()) on the input F.pad(x, (l, l, t, t)) of constant zeros, pad = (t, l): padding (t, l)
+        and the shifted code of +0.0 at the input range on every out-of-image tap, as the per-layer path quantizes the
+        padded zeros.  Needs padding 0: a convolution's own padding is a dequantized 0.0, not a code."""
+        if self.padding != (0, 0) or self.pad_code is not None:
+            raise _lib.DfqError("layer %s: a pad folds only into a convolution with padding 0" % self._who())
+        if self.epilogue is not None or self.out_slice is not None:
+            raise _lib.DfqError("layer %s: fold a pad before the chained modes" % self._who())
+        new = self.chained(codes_in=self.codes_in, name=self.layer_name)
+        new.padding = (int(pad[0]), int(pad[1]))
+        new.pad_code = affine_code_of(0.0, self.act_min, self.act_max, self.act_bits)
         return new
 
     def observe(self, obs=None, res=None):
@@ -557,13 +588,16 @@ class _AffineInt8Layer(nn.Module):
                    "dfq_i8_affine_quantize (layer %s)" % self._who())
         return xq, S, N, H, W
 
-    def run(self, x, with_acc=False, residual=None):
+    def run(self, x, with_acc=False, residual=None, out=None):
         """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes.  In the chained modes
         x is (codes [N, H, W, cpad], S [N, H, W] | None) (codes_in), and with an epilogue y is (codes, S | None), the fp32
         output, or ((codes, S | None), fp32 output) when it returns both; `residual` is the fp32 tensor [N, C_out, OH, OW]
-        the epilogue adds (exactly that shape, no broadcasting, on the input's device)."""
-        if self.epilogue is not None and with_acc:
+        the epilogue adds (exactly that shape, no broadcasting, on the input's device).  With out_slice, y is `out` (the
+        concatenation's (codes, S | None)) or a new such pair, its slice written."""
+        if (self.epilogue is not None or self.pad_code is not None) and with_acc:
             raise _lib.DfqError("a chained affine layer does not return its int32 sums")
+        if out is not None and self.out_slice is None:
+            raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
         if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
             raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
                                                     "takes no residual input"))
@@ -572,8 +606,8 @@ class _AffineInt8Layer(nn.Module):
         OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
         if OH <= 0 or OW <= 0:
             raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
-        if self.epilogue is not None:
-            return self._run_fused(xq, S, residual, g, N, OH, OW), None
+        if self.epilogue is not None or self.pad_code is not None:
+            return self._run_fused(xq, S, residual, g, N, OH, OW, out), None
         lib, st = _lib.load(), _lib.stream_ptr()
         y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=xq.device)
         acc = torch.empty(y.shape, dtype=torch.int32, device=xq.device) if with_acc else None
@@ -583,8 +617,8 @@ class _AffineInt8Layer(nn.Module):
                                           _lib.table_ptr(g), st), "dfq_i8_affine_conv (layer %s)" % self._who())
         return y, acc
 
-    def _run_fused(self, xq, S, r, g, N, OH, OW):
-        e = self.epilogue
+    def _run_fused(self, xq, S, r, g, N, OH, OW, out=None):
+        e = self.epilogue or Epilogue(fp32=True)                # a folded pad alone: the fp32 output through the layout
         shape = (N, self.out_channels, OH, OW)
         if r is not None:
             if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
@@ -593,9 +627,12 @@ class _AffineInt8Layer(nn.Module):
                     self._who(), list(shape), xq.device, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
                     if isinstance(r, torch.Tensor) else type(r).__name__))
             r = r.contiguous()
-        yq = None if e.out_scale is None else \
-            torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=xq.device)
-        S_out = torch.empty((N, OH, OW), dtype=torch.int32, device=xq.device) if yq is not None and self.sums else None
+        if self.out_slice is not None:
+            yq, S_out = self._slice_buffers(out, N, OH, OW, xq.device)
+        else:
+            yq = None if e.out_scale is None else \
+                torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=xq.device)
+            S_out = torch.empty((N, OH, OW), dtype=torch.int32, device=xq.device) if yq is not None and self.sums else None
         y = torch.empty(shape, dtype=torch.float32, device=xq.device) if e.fp32 else None
         d = np.zeros(1, _lib.I8_AFFINE_EPILOGUE_DT)
         d[0] = tuple(0 if t is None else t.data_ptr() for t in (r, y, yq, S_out)) + (e.out_scale or (0.0, 0.0, 0)) + \
@@ -604,7 +641,20 @@ class _AffineInt8Layer(nn.Module):
                                   _ptr(self.tap_table) if self.tap_table.numel() else None, _lib.table_ptr(self.constants),
                                   _ptr(self.bias), _lib.table_ptr(d))
         obs, res = self.observers
-        if obs is None and res is None:
+        if self.out_slice is not None or self.pad_code is not None:
+            o = None
+            if obs is not None or res is not None:
+                o = np.zeros(1, _lib.I8_AFFINE_OBSERVE_DT)
+                o[0] = (obs or (0.0, 0.0, 0)) + (res or (0.0, 0.0, 0))
+            lay = np.zeros(1, _lib.I8_AFFINE_LAYOUT_DT)
+            lay[0] = (self.out_slice or (0, (self.out_channels + 15) // 16 * 16)) + (
+                int(self.out_slice is not None), int(self.pad_code is not None), self.pad_code or 0)
+            _lib.check(lib.dfq_i8_affine_conv_layout(*args, None if o is None else _lib.table_ptr(o), _lib.table_ptr(lay),
+                                                     _lib.table_ptr(g), _lib.stream_ptr()),
+                       "dfq_i8_affine_conv_layout (layer %s)" % self._who())
+            if self.out_slice is not None:
+                return yq, S_out
+        elif obs is None and res is None:
             _lib.check(lib.dfq_i8_affine_conv_fused(*args, _lib.table_ptr(g), _lib.stream_ptr()),
                        "dfq_i8_affine_conv_fused (layer %s)" % self._who())
         else:
@@ -614,6 +664,11 @@ class _AffineInt8Layer(nn.Module):
                        "dfq_i8_affine_conv_observed (layer %s)" % self._who())
         codes = None if yq is None else (yq, S_out)
         return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
+
+    def _slice_buffers(self, out, N, OH, OW, dev):
+        """(codes [N, OH, OW, cstride], S [N, OH, OW] | None) of this slice's concatenation: `out`, checked, or new ones
+        (S zeroed, when a dense consumer reads it) for the first writer."""
+        return _concat_buffers(out, (N, OH, OW, self.out_slice[1]), self.sums, dev, "layer %s" % self._who())
 
     def extra_repr(self):
         return "%d, %d, kernel_size=%s, stride=%s, padding=%s, dilation=%s, groups=%d, act=[%g, %g] %d-bit, w_min=%g, " \
@@ -632,6 +687,33 @@ def _observer_range(o, who):
     if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(hi))):
         raise _lib.DfqError("%s: range [%g, %g] gives no finite fp32 scale" % (who, lo, hi))
     return float(_f32(lo)), float(_f32(hi)), int(bits)
+
+
+def affine_code_of(v, act_min, act_max, num_bits):
+    """The shifted code dfq_i8_affine_quantize gives the fp32 value v at this range, with its fp32 ops:
+    rint(clamp(fp32(fp32(v + (-min)) * fp32(1 / scale)), 0, 2^b - 1)) - 128, the scale in double (QuantMeasure's)."""
+    mn, mx = float(_f32(act_min)), float(_f32(act_max))
+    qmax = 2. ** int(num_bits) - 1.
+    scale = max((mx - mn) / qmax, 1e-8)
+    with np.errstate(over="ignore", invalid="ignore"):
+        t = _f32(_f32(_f32(v) + _f32(-mn)) * _f32(1.0 / scale))
+    t = 0.0 if np.isnan(t) else min(max(float(t), 0.0), qmax)
+    return int(np.rint(t)) - 128
+
+
+def _concat_buffers(out, shape, sums, dev, who):
+    """(codes int8 `shape`, S int32 shape[:3] | None) of a concatenation's codes: `out` checked, or new ones for its first
+    writer, S zeroed (the writers add into it) when `sums`."""
+    if out is None:
+        return (torch.empty(shape, dtype=torch.int8, device=dev),
+                torch.zeros(shape[:3], dtype=torch.int32, device=dev) if sums else None)
+    codes, S = out if isinstance(out, tuple) and len(out) == 2 else (out, None)
+    if not isinstance(codes, torch.Tensor) or codes.dtype != torch.int8 or tuple(codes.shape) != shape or \
+            codes.device != dev or not codes.is_contiguous() or (S is None) == bool(sums) or (S is not None and (
+                S.dtype != torch.int32 or tuple(S.shape) != shape[:3] or S.device != dev or not S.is_contiguous())):
+        raise _lib.DfqError("%s: the concatenation's codes must be contiguous (int8 %s, %s) on %s" % (
+            who, list(shape), "int32 %s" % list(shape[:3]) if sums else "None", dev))
+    return codes, S
 
 
 def _affine_refusal(who, C_in, C_out, groups, kernel_size, act_bits, w_bits):
@@ -659,8 +741,8 @@ class AffineInt8Conv2d(_AffineInt8Layer):
         return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
                    conv.groups, name=name)
 
-    def forward(self, x, r=None):
-        return self.run(x, residual=r)[0]
+    def forward(self, x, r=None, out=None):
+        return self.run(x, residual=r, out=out)[0]
 
 
 class AffineInt8Linear(_AffineInt8Layer):
@@ -790,6 +872,54 @@ class Int8UpsampleBilinear(nn.Module):
     def extra_repr(self):
         return "channels=%d, align_corners=%s, out_scale=%g, clamp=%s, out_slice=%s" % (
             self.channels, self.align_corners, self.out_scale, self.clamp, self.out_slice)
+
+
+class AffineInt8UpsampleBilinear(nn.Module):
+    """A bilinear F.interpolate operand of a concatenation chained by chain_affine (dfq_i8_affine_upsample_bilinear): fp32
+    NCHW [N, channels, H, W] in; torch's bilinear output through clamp(pre), the operand's observer `obs` ((min, max, bits)
+    or None), clamp(post) and the consumer's quantizer out = (act_min, act_max, act_bits), written into channels
+    [coff, coff + round_up(channels, 16)) of the concatenation's (codes [N, OH, OW, cstride], S | None) - `out`, or new
+    ones (S zeroed when `sums`) - which it returns.  The size comes at run time and must be a pair of positive ints."""
+
+    def __init__(self, channels, align_corners, out, out_slice, pre=(-float("inf"), float("inf")), obs=None,
+                 post=(-float("inf"), float("inf")), sums=False, name=None):
+        super().__init__()
+        self.channels, self.align_corners, self.layer_name, self.sums = int(channels), bool(align_corners), name, bool(sums)
+        who = "bilinear upsample %s" % name
+        self.out = _observer_range(out, who + " output")
+        self.obs = None if obs is None else _observer_range(obs, who + " observer")
+        self.pre, self.post = _ordered(*pre, what=who + " pre"), _ordered(*post, what=who + " post")
+        coff, cstride = (int(v) for v in out_slice)
+        if coff < 0 or coff % 16 or cstride % 16 or coff + (self.channels + 15) // 16 * 16 > cstride:
+            raise _lib.DfqError("%s: channel slice (%d, %d) is not 16-aligned inside its tensor" % (who, coff, cstride))
+        self.out_slice = (coff, cstride)
+
+    def forward(self, x, size, out=None):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise _lib.DfqError("int8 bilinear upsample %s runs on the GPU only (no CPU fallback)" % self.layer_name)
+        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.channels:
+            raise _lib.DfqError("int8 bilinear upsample %s expects fp32 [N, %d, H, W], got %s %s"
+                                % (self.layer_name, self.channels, x.dtype, tuple(x.shape)))
+        if not isinstance(size, (tuple, list)) or len(size) != 2 or \
+                not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in size):
+            raise _lib.DfqError("int8 bilinear upsample %s: size must be a pair of positive ints, got %r"
+                                % (self.layer_name, size))
+        N, _, H, W = x.shape
+        OH, OW = int(size[0]), int(size[1])
+        coff, cstride = self.out_slice
+        codes, S = _concat_buffers(out, (N, OH, OW, cstride), self.sums, x.device, "bilinear upsample %s" % self.layer_name)
+        x = x.contiguous()
+        g = np.zeros(1, _lib.I8_AFFINE_RESIZE_DT)
+        g[0] = (N, self.channels, H, W, OH, OW, int(self.align_corners), coff, cstride) + self.pre + \
+            (self.obs or (0.0, 0.0, 0)) + self.post + self.out
+        _lib.check(_lib.load().dfq_i8_affine_upsample_bilinear(_ptr(x), _ptr(codes), _ptr(S), _lib.table_ptr(g),
+                                                               _lib.stream_ptr()),
+                   "dfq_i8_affine_upsample_bilinear (%s)" % self.layer_name)
+        return codes, S
+
+    def extra_repr(self):
+        return "channels=%d, align_corners=%s, pre=%s, obs=%s, post=%s, out=%s, out_slice=%s, sums=%s" % (
+            self.channels, self.align_corners, self.pre, self.obs, self.post, self.out, self.out_slice, self.sums)
 
 
 class Int8HeadConcat(nn.Module):
@@ -1039,10 +1169,17 @@ def _max_pool(node, mods):
     return None
 
 
-def _bilinear_upsample(node, mods):
+def _orig(name):
+    """The unpatched torch.cat / F.interpolate that utils/layer_transform.py saved when replace_op() patched it (what a
+    graph traced in the reference's evaluation state calls), or None."""
+    from .utils import layer_transform as LT
+    return LT.raw_torch_op.get(name) or LT.raw_func_op.get(name)
+
+
+def _bilinear_upsample(node, mods, raw=False):
     """(size, align_corners) of an F.interpolate / nn.Upsample node that resizes one fx node bilinearly to a given size:
     mode 'bilinear', size a pair of ints or a traced value, align_corners True or False, no scale_factor,
-    recompute_scale_factor or antialias; None otherwise."""
+    recompute_scale_factor or antialias; None otherwise.  raw: the unpatched F.interpolate counts too (_orig)."""
     if not node.args or not isinstance(node.args[0], fx.Node):
         return None
     if node.op == "call_module" and type(mods[node.target]) is nn.Upsample:
@@ -1050,7 +1187,7 @@ def _bilinear_upsample(node, mods):
         if len(node.args) != 1 or node.kwargs:
             return None
         size, sf, mode, ac, rsf, aa = m.size, m.scale_factor, m.mode, m.align_corners, m.recompute_scale_factor, False
-    elif node.op == "call_function" and node.target is F.interpolate:
+    elif node.op == "call_function" and (node.target is F.interpolate or (raw and node.target is _orig("interpolate"))):
         size, sf, mode, ac, rsf, aa = (_arg(node, i, k, d) for i, k, d in (
             (1, "size", None), (2, "scale_factor", None), (3, "mode", "nearest"), (4, "align_corners", None),
             (5, "recompute_scale_factor", None), (6, "antialias", False)))
@@ -1105,14 +1242,17 @@ def _shape_query(u, node):
 def _nchw_view(codes, channels):
     """A tensor of the shape [N, channels, H, W] of the fp32 tensor whose codes `codes` [N, H, W, *] carry, for the shape
     queries on a fused concatenation's operand (sizes taken as `x4.size()[2:]`): a zero-stride view, nothing allocated."""
+    if isinstance(codes, tuple):                                # the affine scheme's (codes, S)
+        codes = codes[0]
     N, H, W = codes.shape[:3]
     return codes.as_strided((N, channels, H, W), (0, 0, 0, 0))
 
 
-def _cat_operands(node):
+def _cat_operands(node, raw=False):
     """The operands of torch.cat / torch.concat along the channels (dim 1 or -3) of >= 2 distinct fx nodes, without out;
-    None otherwise."""
-    if node.op != "call_function" or node.target not in (torch.cat, torch.concat) or set(node.kwargs) - {"tensors", "dim"}:
+    None otherwise.  raw: the unpatched torch.cat counts too (_orig)."""
+    cats = (torch.cat, torch.concat) + ((_orig("cat"),) if raw else ())
+    if node.op != "call_function" or node.target not in cats or set(node.kwargs) - {"tensors", "dim"}:
         return None
     ops, dim = _arg(node, 0, "tensors", None), _arg(node, 1, "dim", 0)
     if dim not in (1, -3) or not isinstance(ops, (list, tuple)) or len(ops) < 2 or \
@@ -1138,8 +1278,10 @@ def _zero_pad(node):
     return t, l
 
 
-def _fold_pads(gm, mods, conv):
-    """Rule (a) of chain_int8(layout=True): fold each qualifying zero F.pad into its only user, an Int8Conv2d."""
+def _fold_pads(gm, mods, conv, affine=False):
+    """Rule (a) of chain_int8(layout=True): fold each qualifying zero F.pad into its only user, an Int8Conv2d.  affine
+    (chain_affine(fold_pads=True)): into an AffineInt8Conv2d with padding 0, whose out-of-image taps then read the code of
+    +0.0 at its input range (_AffineInt8Layer.fold_pad)."""
     folded = []
     for node in list(gm.graph.nodes):
         tl = _zero_pad(node)
@@ -1149,8 +1291,13 @@ def _fold_pads(gm, mods, conv):
         if not conv(q) or q.args != (node,) or q.kwargs:
             continue
         m = mods[q.target]
-        new = m.chained(name=q.target)
-        new.padding = (m.padding[0] + tl[0], m.padding[1] + tl[1])
+        if affine:
+            if m.padding != (0, 0):
+                continue
+            new = m.chained(name=q.target).fold_pad(tl)
+        else:
+            new = m.chained(name=q.target)
+            new.padding = (m.padding[0] + tl[0], m.padding[1] + tl[1])
         parent, _, attr = q.target.rpartition(".")
         setattr(gm.get_submodule(parent) if parent else gm, attr, new)
         mods[q.target] = new
@@ -1380,7 +1527,7 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     return _chain_edges(gm, mods, conv, _NCNN)
 
 
-def chain_affine(model: nn.Module, concrete_args=None, residual=False) -> fx.GraphModule:
+def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=False, fold_pads=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` (after convert_affine) computes, with activations kept as the
     consumers' shifted affine codes between AffineInt8Conv2d layers, bit-identical to the per-layer path.
 
@@ -1401,8 +1548,8 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False) -> fx.Gra
       raise DfqError naming the layer when the module runs.
     A producer writes the codes' per-pixel sums S (which a dense consumer's epilogue reads) only when some code consumer is
     dense, and its fp32 output only when a user other than those consumers remains.  Ncnn Int8Conv2d layers and
-    AffineInt8Linear stay opaque leaves, so no edge crosses the two schemes; pools, concatenations, upsampling, pads and
-    detection heads stay in torch, fp32.
+    AffineInt8Linear stay opaque leaves, so no edge crosses the two schemes; pools and detection heads stay in torch, fp32,
+    and so do concatenations, upsampling and pads unless concat / fold_pads (below) take them.
 
     The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
     edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) the clamp
@@ -1424,16 +1571,47 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False) -> fx.Gra
     - observers with a truthy update_stat, in training mode, above 8 bits or with a non-finite range stay in torch.
     Folded observers are deleted and recorded in `fused_observers`: (observer module, "operand" / "residual" / "output",
     producer name).  The result's tensor adds are torch.add and its cat / mean / interpolate / softmax the raw ops, so its
-    forward can run while replace_op() stays active.  Outside that state nothing here changes."""
+    forward can run while replace_op() stays active.  Outside that state nothing here changes.
+
+    fold_pads=True folds zero padding, as chain_int8(layout=True)'s rule (a) but for the affine scheme: an F.pad of one fx
+    node with constant arguments - pad (l, r) or (l, r, t, b), l == r >= 0, t == b >= 0, mode 'constant', value 0 or None -
+    whose only user is a single-site AffineInt8Conv2d with padding 0 taking it as its sole argument becomes that
+    convolution's padding (t, l), and the copy's out-of-image taps read the code of +0.0 at its input range
+    (affine_code_of; dfq_i8_affine_conv_layout's pad code), which is what the per-layer path quantizes the padded zeros to:
+    bit-identical (DeepLab-v3+'s fixed_padding).  A pad in front of a convolution with padding of its own stays in torch
+    (those taps are a dequantized 0.0, not codes), as does any pad chain_int8 leaves.  It runs before every other rule and
+    records `folded_pads`: (pad node name, conv name, (t, l)) in graph order.
+
+    concat=True (with residual=True) carries codes into channel concatenations, chain_int8(pool_cat=True, upsample=True)'s
+    concatenation rule and its upsample-as-operand rule under the affine scheme, bit-identical to the per-layer path:
+    - a torch.cat along dim 1 (or -3) of >= 2 distinct nodes, without out, every operand but the last with a multiple of 16
+      channels, each operand an AffineInt8Conv2d producer's single-user pass-through chain, optionally ending in a replayed
+      observer, or a bilinear upsample (F.interpolate to a size, no scale_factor; chain_int8's conditions) of such a chain -
+      its input observer folded into the producer's fp32 output - followed by single-user pass-throughs and an optional
+      observer; every user of the cat's tail (the cat and its single-user pass-throughs) an AffineInt8Conv2d at one range
+      key.
+    - Each producer (dfq_i8_affine_conv_layout) or upsample (AffineInt8UpsampleBilinear) writes its slice of the consumers'
+      codes, one buffer per forward, in graph order: the operand chain's clamp, the operand's observer, the tail's clamp,
+      then the consumers' code; the slice's channel sums add into one S zeroed by the first writer, only when a consumer
+      is dense.  Shape queries on the operands read a zero-stride view of the writer's codes (_nchw_view).
+    - max pools stay in torch, as does any cat not taken (SSD's head concatenations along dim 1 of [N, R, k] included).
+    `fused_cats` records (cat node name, writer names, channel offsets), `fused_upsamples` (node name, producer name,
+    "slice", align_corners), and the operands' observers enter `fused_observers` as (observer module, "cat", writer
+    name).  concat=True without residual=True raises DfqError."""
+    if concat and not residual:
+        raise _lib.DfqError("chain_affine: concat=True builds on residual=True")
     LT = _observed_state()
     gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer, LT)
+    folded = _fold_pads(gm, mods, conv, affine=True) if fold_pads else None
     if residual:
-        gm = _chain_residual(gm, mods, conv, scheme=_AFFINE)
+        gm = _chain_residual(gm, mods, conv, concat, concat, scheme=_AFFINE)
     else:
         gm = _chain_edges(gm, mods, conv, _AFFINE)
         gm.fused_observers = []
     if LT is not None:
         _unpatch_adds(gm, LT)
+    if fold_pads:
+        gm.folded_pads = folded
     return gm
 
 
@@ -1458,7 +1636,7 @@ _AFFINE = _Scheme(AffineInt8Conv2d, lambda m: (_f32(m.act_min), _f32(m.act_max),
                   and a[2] == b[2],
                   lambda k: (float(k[0]), float(k[1]), int(k[2])),
                   lambda m, codes_in, name, requant, epilogue, out_slice, sums: m.chained(
-                      codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, sums=sums))
+                      codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, sums=sums, out_slice=out_slice))
 
 
 def _observed_state():
@@ -1666,9 +1844,12 @@ def _chain_edges(gm, mods, conv, scheme):
 
 
 def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None):
-    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True) on the traced
-    `gm` (see chain_int8); scheme: _NCNN (default) or _AFFINE."""
+    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True[, concat=True],
+    which passes pool_cat = upsample = concat) on the traced `gm` (see chain_int8, chain_affine); scheme: _NCNN (default)
+    or _AFFINE.  Under _AFFINE, max pools and upsamples whose users take codes stay in torch."""
     scheme = scheme or _NCNN
+    affine = scheme is _AFFINE
+    pool = pool_cat and not affine
     full = (-_INF, _INF)
     order = {n: i for i, n in enumerate(gm.graph.nodes)}
 
@@ -1718,7 +1899,10 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         """The producer of a fusable bilinear upsample node, or None (as the traced graph has it: memoized before the
         rewrites)."""
         if node not in sources:
-            sources[node] = ends.get(node.args[0]) if ends and _bilinear_upsample(node, mods) is not None else None
+            src = node.args[0] if node.args else None
+            if affine and isinstance(src, fx.Node) and observe(src):   # its input observer goes into the producer
+                src = src.args[0]
+            sources[node] = ends.get(src) if ends and _bilinear_upsample(node, mods, affine) is not None else None
         return sources[node]
 
     def back_to_upsample(node):
@@ -1756,7 +1940,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         """The scale at which u takes the codes of `tail` (channels wide), or None when it takes fp32."""
         if producer(u) and u.args[0] is tail and mods[u.target].in_channels == channels:
             return scheme.key(mods[u.target])
-        if pools and pool_cat and _max_pool(u, mods) is not None and u.args[0] is tail:
+        if pools and pool and _max_pool(u, mods) is not None and u.args[0] is tail:
             return pool_scale(u, channels)
         return None
 
@@ -1802,7 +1986,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         out_c = mods[p.target].out_channels
         codes, scale = take_codes(tail, out_c)
         clamp = post if add is not None else pre
-        if add is None and not codes and pool_cat and len(tail.users) == 1:
+        if add is None and not codes and pool and len(tail.users) == 1:
             u = next(iter(tail.users))                          # fp32-mode pool: a user of the pool needs fp32
             if _max_pool(u, mods) is not None and u.args[0] is tail:
                 pc, ps = take_codes(u, out_c, pools=False)
@@ -1819,9 +2003,45 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             if not producer(u):
                 codes_pool(u, out_c, clamp)
 
+    # concatenations whose operands come from their own producers and whose users all take codes at one scale
+    cat_plans = []
+    for c in (list(gm.graph.nodes) if pool_cat else []):
+        ops = _cat_operands(c, affine)
+        if ops is None:
+            continue
+        # under the affine scheme an operand may end in its replayed observer, which the operand's writer applies
+        oobs = [o if affine and observe(o) else None for o in ops]
+        ops = [o.args[0] if ob is not None else o for o, ob in zip(ops, oobs)]
+        prods = [back_to_producer(o, upsample) or (back_to_upsample(o) if upsample else None) for o in ops]
+        if any(q is None for q in prods) or len(set(prods)) != len(prods):
+            continue
+        chans = [mods[(up_source(q) or q).target].out_channels for q in prods]
+        if any(k % 16 for k in chans[:-1]):
+            continue
+        tail, tclamp, tpath = forward(c, full)
+        codes, scale = take_codes(tail, sum(chans))
+        if not codes or len(codes) != len(tail.users):
+            continue
+        operands = []
+        for o, ob, q, k, off in zip(ops, oobs, prods, chans, np.cumsum([0] + chans[:-1]).tolist()):
+            node, clamp, opath = o, full, []
+            while node is not q:
+                clamp = _compose(_pass_through(node, mods), clamp)
+                opath.append(node)
+                node = node.args[0]
+            queries = [(u, n) for n in (q, *opath) for u in n.users if upsample and _shape_query(u, n)]
+            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), pre=clamp, obs=ob, coff=off, channels=k,
+                                 queries=queries))
+        cat_plans.append(dict(cat=c, operands=operands, tail=tail, path=tpath, codes=codes, scale=scale, clamp=tclamp,
+                              cstride=(sum(chans) + 15) // 16 * 16, sums=any(producer(u) and mods[u.target].groups == 1 for u in codes)))
+        for u in codes:
+            if not producer(u):
+                codes_pool(u, sum(chans), tclamp)
+
     # observers on a producer's fp32 output: its single-user pass-through chain, then shape-only views, then the observer
     # (shape queries not counted as users); the producer applies it in its epilogue and writes the observed fp32 output
     taken = {n for pl in plans for n in (pl.get("obs"), pl.get("robs")) if n is not None}
+    taken |= {o["obs"] for cp in cat_plans for o in cp["operands"] if o["obs"] is not None}
     planned = {pl["p"] for pl in plans}
     for o in (list(gm.graph.nodes) if scheme is _AFFINE else []):
         if o in taken or _observer_key(o, mods) is None:
@@ -1841,42 +2061,11 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
                           scale=None, obs=o, robs=None, output=True))
         planned.add(q)
 
-    # concatenations whose operands come from their own producers and whose users all take codes at one scale
-    cat_plans = []
-    for c in (list(gm.graph.nodes) if pool_cat else []):
-        ops = _cat_operands(c)
-        if ops is None:
-            continue
-        prods = [back_to_producer(o, upsample) or (back_to_upsample(o) if upsample else None) for o in ops]
-        if any(q is None for q in prods) or len(set(prods)) != len(prods):
-            continue
-        chans = [mods[(up_source(q) or q).target].out_channels for q in prods]
-        if any(k % 16 for k in chans[:-1]):
-            continue
-        tail, tclamp, tpath = forward(c, full)
-        codes, scale = take_codes(tail, sum(chans))
-        if not codes or len(codes) != len(tail.users):
-            continue
-        operands = []
-        for o, q, k, off in zip(ops, prods, chans, np.cumsum([0] + chans[:-1]).tolist()):
-            node, clamp, opath = o, full, []
-            while node is not q:
-                clamp = _compose(_pass_through(node, mods), clamp)
-                opath.append(node)
-                node = node.args[0]
-            queries = [(u, n) for n in (q, *opath) for u in n.users if upsample and _shape_query(u, n)]
-            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), coff=off, channels=k, queries=queries))
-        cat_plans.append(dict(cat=c, operands=operands, tail=tail, path=tpath, codes=codes, scale=scale, clamp=tclamp,
-                              cstride=(sum(chans) + 15) // 16 * 16))
-        for u in codes:
-            if not producer(u):
-                codes_pool(u, sum(chans), tclamp)
-
     # upsamples: slice mode through a fused concatenation above, codes mode when every user takes codes at one scale;
     # either way the producer writes its clamped fp32 output
     up_plans = [dict(node=o["p"], mode="slice") for cp in cat_plans for o in cp["operands"] if not producer(o["p"])]
     sliced = {up["node"] for up in up_plans}
-    for u in (list(gm.graph.nodes) if upsample else []):
+    for u in (list(gm.graph.nodes) if upsample and not affine else []):
         if u in sliced or up_source(u) is None:
             continue
         utail, uclamp, upath = forward(u, full)
@@ -1963,27 +2152,43 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         if add is not None:
             adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
 
-    def fuse_upsample(u, scale, clamp, out_slice=None, out=None):
-        """Turn the upsample node u into a call of its Int8UpsampleBilinear, on its (rewritten) input."""
-        (size, ac), p = _bilinear_upsample(u, mods), up_source(u)
-        mod = Int8UpsampleBilinear(mods[p.target].out_channels, ac, float(scale), clamp, out_slice, name=u.name)
+    def fuse_upsample(u, scale, clamp, out_slice=None, out=None, operand=None, sums=False):
+        """Turn the upsample node u into a call of its Int8UpsampleBilinear, on its (rewritten) input; under the affine
+        scheme of its AffineInt8UpsampleBilinear: the operand's clamp, its observer, then `clamp` (the cat tail's)."""
+        (size, ac), p = _bilinear_upsample(u, mods, affine), up_source(u)
+        if affine:
+            ob = None if operand["obs"] is None else _observer_key(operand["obs"], mods)
+            mod = AffineInt8UpsampleBilinear(mods[p.target].out_channels, ac, scheme.out(scale), out_slice, operand["pre"], ob,
+                                             clamp, sums, name=u.name)
+        else:
+            mod = Int8UpsampleBilinear(mods[p.target].out_channels, ac, float(scale), clamp, out_slice, name=u.name)
         name = "int8_up_" + u.name
         gm.add_submodule(name, mod)
         ups.append((order[u], (u.name, p.target, "slice" if out_slice else "codes", ac)))
         u.op, u.target, u.args, u.kwargs = "call_module", name, (u.args[0], size), ({} if out is None else {"out": out})
 
     # concatenations: the producers write their slices of one buffer in graph order, threaded through `out`
-    cats, ups = [], []
+    cats, ups, slice_sums = [], [], set()
     for cp in cat_plans:
         cstride, prev = cp["cstride"], None
         names = [o["p"].target if producer(o["p"]) else o["p"].name for o in cp["operands"]]
         for o in sorted(cp["operands"], key=lambda o: order[o["p"]]):
             q = o["p"]
             if not producer(q):
-                fuse_upsample(q, cp["scale"], o["clamp"], (o["coff"], cstride), prev)
+                if affine:
+                    fuse_upsample(q, cp["scale"], cp["clamp"], (o["coff"], cstride), prev, o, cp["sums"])
+                else:
+                    fuse_upsample(q, cp["scale"], o["clamp"], (o["coff"], cstride), prev)
                 prev = q
                 continue
-            modes[q.target] = ("slice", ((float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride)))
+            if affine:                                          # operand clamp, its observer, the tail's clamp
+                modes[q.target] = ("slice", (Epilogue(scheme.out(cp["scale"]), o["pre"], cp["clamp"]), (o["coff"], cstride)))
+                if o["obs"] is not None:
+                    watched[q.target] = (_observer_key(o["obs"], mods), None)
+                if cp["sums"]:
+                    slice_sums.add(q.target)
+            else:
+                modes[q.target] = ("slice", ((float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride)))
             if prev is not None:
                 q.kwargs = {"out": prev}
             prev = q
@@ -1994,7 +2199,10 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         for node in reversed(cp["path"]):
             g.erase_node(node)
         g.erase_node(cp["cat"])
-        for o in cp["operands"]:
+        for o, name in zip(cp["operands"], names):
+            if o["obs"] is not None:                            # the operand's observer, now in its writer
+                g.erase_node(o["obs"])
+                observed.append((o["obs"].target, "cat", name))
             for u, n in o["queries"]:                           # shape queries read the shape off the slice's writer
                 with g.inserting_before(u):
                     u.replace_input_with(n, g.call_function(_nchw_view, (o["p"], o["channels"])))
@@ -2051,9 +2259,11 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     for target in modes.keys() | consumers:
         kind, arg = modes.get(target, (None, None))
         parent, _, attr = target.rpartition(".")
+        sliced_epi = kind == "slice" and isinstance(arg[0], Epilogue)          # an affine slice: both clamps
         mod = scheme.chained(mods[target], target in consumers, target,
-                             arg if kind == "requant" else (arg[0] if kind == "slice" else None),
-                             arg if kind == "epilogue" else None, arg[1] if kind == "slice" else None, target in dense)
+                             arg if kind == "requant" else (arg[0] if kind == "slice" and not sliced_epi else None),
+                             arg if kind == "epilogue" else (arg[0] if sliced_epi else None),
+                             arg[1] if kind == "slice" else None, target in dense or target in slice_sums)
         setattr(gm.get_submodule(parent) if parent else gm, attr, mod.observe(*watched[target]) if target in watched else mod)
     g.lint()
     gm.recompile()

@@ -44,7 +44,8 @@ int dfq_abi_version(void);
 const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
- * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve): lets a binding verify
+ * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
+ * 16 DfqI8AffineResize): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -633,6 +634,48 @@ typedef struct DfqI8AffineObserve {
 int dfq_i8_affine_conv_observed(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                                 const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
                                 const DfqI8AffineObserve* o, const DfqI8Conv* g, void* stream);
+/* Where dfq_i8_affine_conv_layout puts its codes and S, and what its out-of-image taps read. */
+typedef struct DfqI8AffineLayout {
+  int32_t coff, cstride;       /* codes go to channels [coff, coff + round_up(O, 16)) of int8 NHWC [N, OH, OW, cstride]    */
+  int32_t S_accumulate;        /* 1: add the pixels' sums into S, which the caller zeroed (a concatenation's writers)       */
+  int32_t pad_code_on;         /* 1: every out-of-image tap reads the shifted code pad_code over the C real channels        */
+  int32_t pad_code;            /* in [-128, 127]                                                                           */
+} DfqI8AffineLayout;
+/* dfq_i8_affine_conv_observed (o != NULL) or dfq_i8_affine_conv_fused (o == NULL) with the layout *l:
+ *   yq[n, p, coff + o] = the code of v (pad channels O .. round_up(O, 16) written 0, nothing else of the row), pixel p's
+ *                 codes cstride bytes after pixel p - 1's: the producers of a channel concatenation write the consumer's
+ *                 input directly;
+ *   S[n, p]     += the sum of the slice's codes over its O real channels when S_accumulate (S zeroed by the caller once
+ *                 for all the concatenation's writers), else as dfq_i8_affine_conv_fused;
+ *   pad_code_on: y, yq and S equal, bit for bit, those of the same call with padding 0 on the input padded by pad_h rows
+ *                 and pad_w columns on each side whose padded pixels hold the code pad_code in every real channel (what
+ *                 the per-layer path computes on F.pad(x): its zeros become the code of +0.0 at the layer's input range).
+ *                 Dense layers correct P, A, Wv and Nv from the prefix table; depthwise layers read the code in the loop.
+ * Refusals of dfq_i8_affine_conv_observed / _fused as there (overlaps taken over the slice's extent), and DFQ_E_ARG with a
+ * reason: l NULL, coff or cstride not a multiple of 16, the slice past cstride, S_accumulate or pad_code_on not 0 / 1, a
+ * pad code outside [-128, 127].  Nothing is written when a call is refused. */
+int dfq_i8_affine_conv_layout(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                              const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e,
+                              const DfqI8AffineObserve* o, const DfqI8AffineLayout* l, const DfqI8Conv* g, void* stream);
+/* Bilinear resize into a concatenation's codes under the affine scheme. */
+typedef struct DfqI8AffineResize {
+  int32_t N, C, H, W, OH, OW, align_corners, coff, cstride;   /* as DfqI8Resize                                      */
+  float pre_lo, pre_hi;                                        /* clamp before the observer                           */
+  float obs_min, obs_max;                                      /* the observer on the concatenation operand           */
+  int32_t obs_bits;                                            /* 0: off                                              */
+  float post_lo, post_hi;                                      /* clamp after it                                      */
+  float out_min, out_max;                                      /* the consumer's range                                */
+  int32_t out_bits;
+} DfqI8AffineResize;
+/* x fp32 NCHW [N, C, H, W] -> per output value, in this order: v = dfq_i8_upsample_bilinear's y (torch's
+ * upsample_bilinear2d bit for bit), clamp(v, pre), fq(v, obs) when obs_bits > 0 (as dfq_i8_affine_conv_observed),
+ * clamp(v, post), then yq[n, p, coff + c] = the code dfq_i8_affine_quantize gives v at (out_min, out_max, out_bits), pad
+ * channels 0, nothing outside the slice; S[n, p] += the slice's sum over its C real channels (S NULL: not written; the
+ * caller zeroes S).  DFQ_E_ARG, with a reason: a non-positive size, align_corners not 0 / 1, coff or cstride not a multiple
+ * of 16 or the slice past cstride, x or yq NULL, yq not 16-byte aligned or x / S not 4-byte aligned, NaN or unordered
+ * bounds, an observer or output range as dfq_i8_affine_conv_observed refuses, x, the slice and S overlapping.
+ * DFQ_E_UNSUPPORTED: obs_bits or out_bits above 8.  Nothing is written when a call is refused. */
+int dfq_i8_affine_upsample_bilinear(const float* x, int8_t* yq, int32_t* S, const DfqI8AffineResize* g, void* stream);
 
 #ifdef __cplusplus
 }

@@ -790,6 +790,84 @@ def affine_observed_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def affine_layout_inference(dev, reps=10, batch=8, rounds=5, size=513):
+    """DeepLab-v3+ (tests/deeplab_mobilenet_padded.py) in the reference's evaluation state at batch x 3 x size x size:
+    convert_affine per layer, chain_affine(residual=True) and chain_affine(residual=True, concat=True, fold_pads=True),
+    timed alternately, `rounds` rounds of `reps` passes, median; the three outputs asserted bit-identical.  What the new
+    flags avoid is counted from the shapes of chain_affine(residual=True)'s graph (torch.fx ShapeProp): per folded pad,
+    fused concatenation or fused upsample, its fp32 input read, its fp32 output written and read again by the consumer's
+    quantizer, one launch for the node and one for that quantizer; per fused operand observer, its fp32 tensor read and
+    written and one launch."""
+    import statistics
+    import torch
+    from torch.fx.passes.shape_prop import ShapeProp
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_observed_state
+    from dfq_b200 import int8
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def nbytes(n):
+        m = n.meta.get("tensor_meta") if isinstance(n, torch.fx.Node) else None
+        return 4 * int(torch.Size(m.shape).numel()) if m is not None and hasattr(m, "shape") else 0
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x%dx%d" % (size, size), "unit": "images/s", "reps": reps, "rounds": rounds}
+    try:
+        x = torch.randn(batch, 3, size, size, device=dev, generator=torch.Generator(device=dev).manual_seed(3)).clamp_(-2.5,
+                                                                                                                   2.5)
+        with affine_observed_state.evaluation_state("deeplab", size=129) as (model, qgraph, qtarg):
+            int8.convert_affine(model, qgraph, qtarg)
+            base = int8.chain_affine(model, residual=True)
+            gm = int8.chain_affine(model, residual=True, concat=True, fold_pads=True)
+            arms = (("affine_per_layer", model), ("chain_affine_residual", base), ("chain_affine_concat_fold_pads", gm))
+            with torch.no_grad():
+                ys = [m(x) for _, m in arms]
+                same = all(torch.equal(ys[0].view(torch.int32), y.view(torch.int32)) for y in ys[1:])
+                assert same, "the three arms differ"
+                del ys
+                ShapeProp(base).propagate(x)
+                for _ in range(2):
+                    for _, m in arms:
+                        m(x)
+                torch.cuda.synchronize(dev)
+                ms = {k: [] for k, _ in arms}
+                for _ in range(rounds):
+                    for k, m in arms:
+                        ms[k].append(timed(lambda m=m: m(x)))
+            fused = {t[0] for t in gm.folded_pads} | {t[0] for t in gm.fused_cats} | {t[0] for t in gm.fused_upsamples}
+            avoided, launches = 0, 0
+            for n in base.graph.nodes:
+                if n.name in fused:
+                    ins = n.args[0] if n.args and isinstance(n.args[0], (list, tuple)) else n.args[:1]
+                    avoided += sum(nbytes(a) for a in ins) + 2 * nbytes(n)
+                    launches += 2
+            cat_obs = [o for o, w, _ in gm.fused_observers if w == "cat"]
+            for n in base.graph.nodes:
+                if n.op == "call_module" and n.target in cat_obs:
+                    avoided += 2 * nbytes(n)
+                    launches += 1
+            med = {k: statistics.median(v) for k, v in ms.items()}
+            out["deeplab"] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                              "ms_per_batch_rounds": ms, "folded_pads": len(gm.folded_pads),
+                              "fused_cats": len(gm.fused_cats), "fused_upsamples": len(gm.fused_upsamples),
+                              "fused_observers": len(gm.fused_observers), "edges": len(gm.requantized_edges),
+                              "edges_residual_only": len(base.requantized_edges),
+                              "fp32_bytes_avoided_per_batch": avoided, "launches_avoided_per_batch": launches,
+                              "outputs_bit_identical": same}
+            del base, gm
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -811,7 +889,8 @@ def main():
     p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
-                   help="comma-separated sections to run (default: all but affine, affine_chained and affine_observed)")
+                   help="comma-separated sections to run (default: all but affine, affine_chained, affine_observed and "
+                        "affine_layout)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -835,6 +914,8 @@ def main():
         res["affine_chained"] = affine_chained_inference(dev, reps=args.reps, batch=args.batch)
     if "affine_observed" in want:
         res["affine_observed"] = affine_observed_inference(dev, reps=args.reps, batch=args.batch)
+    if "affine_layout" in want:
+        res["affine_layout"] = affine_layout_inference(dev, reps=args.reps, batch=args.seg_batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
