@@ -1075,6 +1075,44 @@ int grid_for(int64_t total, int threads) {
   return (int)std::max<int64_t>(1, std::min<int64_t>((total + threads - 1) / threads, (int64_t)sm_count() * 32));
 }
 
+#define DFQ_REQUIRE_WHO(cond, msg)                                         \
+  do {                                                                     \
+    if (!(cond)) {                                                         \
+      ::dfq::set_error("%s: %s (%s)", who, msg, #cond);                    \
+      return DFQ_E_ARG;                                                    \
+    }                                                                      \
+  } while (0)
+
+// The convolution of output mode OUT on g with epilogue ep: the tensor-core main loop for groups == 1, else the depthwise
+// one (PAD: its variant that reads the pad code on out-of-image taps)
+template <Out OUT, bool PAD = false>
+int launch_conv(const char* who, const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, float* y,
+                int32_t* acc_out, const DfqI8Conv* g, const typename EpiOf<OUT>::type& ep, cudaStream_t st) {
+  if (g->groups == 1) {
+    const int64_t M = (int64_t)g->N * g->OH * g->OW;
+    DFQ_REQUIRE_WHO((M + BM - 1) / BM < (1LL << 31), "too many output pixels");
+    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
+    k_i8_conv_mma<OUT><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, ep);
+  } else {
+    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
+    k_i8_conv_dw<OUT, PAD><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, total, ep);
+  }
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// A slice of a concatenation's codes: channels [coff, coff + cpad) of rows of cstride codes, 16-aligned inside the row;
+// `channels` names the dimension cpad rounds up (O or C)
+int check_slice(const char* who, int64_t coff, int64_t cstride, int cpad, char channels) {
+  DFQ_REQUIRE_WHO(coff >= 0 && cstride > 0 && coff % 16 == 0 && cstride % 16 == 0,
+                  "coff and cstride must be non-negative multiples of 16");
+  if (coff + cpad > cstride) {
+    set_error("%s: the slice coff + round_up(%c, 16) exceeds cstride (coff + cpad <= cstride)", who, channels);
+    return DFQ_E_ARG;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace dfq
 
@@ -1111,18 +1149,7 @@ extern "C" int dfq_i8_conv(const int8_t* xq, const int8_t* wq, const float* dq, 
   if (int rc = check_geometry(g)) return rc;
   DFQ_REQUIRE(xq && wq && dq && y, "dfq_i8_conv: null pointer");
   DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_conv: codes must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (g->groups == 1) {
-    const int64_t M = (int64_t)g->N * g->OH * g->OW;
-    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_conv: too many output pixels");
-    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::F32><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, Requant{});
-  } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::F32><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, y, acc_out, *g, total, Requant{});
-  }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<Out::F32>("dfq_i8_conv", xq, wq, dq, bias, y, acc_out, g, Requant{}, (cudaStream_t)stream);
 }
 
 extern "C" int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, int8_t* yq,
@@ -1136,18 +1163,7 @@ extern "C" int dfq_i8_conv_requant(const int8_t* xq, const int8_t* wq, const flo
   DFQ_REQUIRE(std::isfinite(out_scale) && out_scale >= 0.f, "dfq_i8_conv_requant: out_scale must be finite and non-negative");
   const int cpad = (g->O + 15) / 16 * 16;
   const Requant rq{yq, out_scale, act_lo, act_hi, cpad, cpad};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (g->groups == 1) {
-    const int64_t M = (int64_t)g->N * g->OH * g->OW;
-    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_requant: too many output pixels");
-    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::I8><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, rq);
-  } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::I8><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, rq);
-  }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<Out::I8>("dfq_i8_conv_requant", xq, wq, dq, bias, nullptr, nullptr, g, rq, (cudaStream_t)stream);
 }
 
 extern "C" int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
@@ -1170,17 +1186,7 @@ extern "C" int dfq_i8_conv_fused(const int8_t* xq, const int8_t* wq, const float
               "dfq_i8_conv_fused: residual overlaps y or yq");
   DFQ_REQUIRE(!overlap(e->y, y_bytes, e->yq, yq_bytes), "dfq_i8_conv_fused: y overlaps yq");
   const Fused ep{e->yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cpad, e->residual, e->y, e->post_lo, e->post_hi};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (g->groups == 1) {
-    DFQ_REQUIRE((pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_fused: too many output pixels");
-    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::FUSED><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
-  } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
-  }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<Out::FUSED>("dfq_i8_conv_fused", xq, wq, dq, bias, nullptr, nullptr, g, ep, (cudaStream_t)stream);
 }
 
 extern "C" int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
@@ -1196,9 +1202,7 @@ extern "C" int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float
               "dfq_i8_conv_slice: pre / post clamp bounds must be ordered and not NaN");
   DFQ_REQUIRE(std::isfinite(e->out_scale) && e->out_scale >= 0.f, "dfq_i8_conv_slice: out_scale must be finite and non-negative");
   const int cpad = (g->O + 15) / 16 * 16;
-  DFQ_REQUIRE(coff >= 0 && cstride > 0 && coff % 16 == 0 && cstride % 16 == 0,
-              "dfq_i8_conv_slice: coff and cstride must be non-negative multiples of 16");
-  DFQ_REQUIRE((int64_t)coff + cpad <= cstride, "dfq_i8_conv_slice: the slice coff + round_up(O, 16) exceeds cstride");
+  if (int rc = check_slice("dfq_i8_conv_slice", coff, cstride, cpad, 'O')) return rc;
   const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
   const int64_t y_bytes = pixels * g->O * (int64_t)sizeof(float);
   int8_t* yq = e->yq + coff;
@@ -1207,22 +1211,13 @@ extern "C" int dfq_i8_conv_slice(const int8_t* xq, const int8_t* wq, const float
   DFQ_REQUIRE(!overlap(e->y, y_bytes, yq, slice_bytes), "dfq_i8_conv_slice: y overlaps the slice");
   DFQ_REQUIRE(!overlap(e->residual, y_bytes, e->y, y_bytes), "dfq_i8_conv_slice: residual overlaps y");
   cudaStream_t st = (cudaStream_t)stream;
-  const bool dense = g->groups == 1;
-  DFQ_REQUIRE(!dense || (pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_slice: too many output pixels");
-  const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-  const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
   if (!e->residual && !e->y && e->post_lo == -INFINITY && e->post_hi == INFINITY) {
     // codes only after one clamp: the requantizing epilogue
     const Requant rq{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride};
-    if (dense) k_i8_conv_mma<Out::I8><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, rq);
-    else k_i8_conv_dw<Out::I8><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, rq);
-  } else {
-    const Fused ep{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride, e->residual, e->y, e->post_lo, e->post_hi};
-    if (dense) k_i8_conv_mma<Out::FUSED><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
-    else k_i8_conv_dw<Out::FUSED><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
+    return launch_conv<Out::I8>("dfq_i8_conv_slice", xq, wq, dq, bias, nullptr, nullptr, g, rq, st);
   }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  const Fused ep{yq, e->out_scale, e->pre_lo, e->pre_hi, cpad, cstride, e->residual, e->y, e->post_lo, e->post_hi};
+  return launch_conv<Out::FUSED>("dfq_i8_conv_slice", xq, wq, dq, bias, nullptr, nullptr, g, ep, st);
 }
 
 extern "C" int dfq_i8_conv_nhwc(const int8_t* xq, const int8_t* wq, const float* dq, const float* bias, const DfqI8Epilogue* e,
@@ -1238,22 +1233,11 @@ extern "C" int dfq_i8_conv_nhwc(const int8_t* xq, const int8_t* wq, const float*
   const int64_t extent = (int64_t)g->OH * g->OW * g->O;              // floats of one image's rows
   DFQ_REQUIRE(off >= 0, "dfq_i8_conv_nhwc: off must be non-negative");
   DFQ_REQUIRE(img_stride >= off + extent, "dfq_i8_conv_nhwc: img_stride must be at least off + OH * OW * O");
-  const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
   const int64_t x_bytes = (int64_t)g->N * g->H * g->W * g->Cpad;
   const int64_t y_bytes = ((g->N - 1) * img_stride + extent) * (int64_t)sizeof(float);   // first to last row written
   DFQ_REQUIRE(!overlap(xq, x_bytes, e->y + off, y_bytes), "dfq_i8_conv_nhwc: y overlaps xq");
   const Rows ep{e->y, off, img_stride, e->pre_lo, e->pre_hi, e->post_lo, e->post_hi};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (g->groups == 1) {
-    DFQ_REQUIRE((pixels + BM - 1) / BM < (1LL << 31), "dfq_i8_conv_nhwc: too many output pixels");
-    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::ROWS><<<grid, THREADS, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, ep);
-  } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::ROWS><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, dq, bias, nullptr, nullptr, *g, total, ep);
-  }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<Out::ROWS>("dfq_i8_conv_nhwc", xq, wq, dq, bias, nullptr, nullptr, g, ep, (cudaStream_t)stream);
 }
 
 extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, float out_scale, const DfqI8Pool* g,
@@ -1301,10 +1285,7 @@ extern "C" int dfq_i8_upsample_bilinear(const float* x, float* y, int8_t* yq, co
               "dfq_i8_upsample_bilinear: empty dimension (every size must be positive)");
   DFQ_REQUIRE(g->align_corners == 0 || g->align_corners == 1, "dfq_i8_upsample_bilinear: align_corners must be 0 or 1");
   const int cpad = (g->C + 15) / 16 * 16;
-  DFQ_REQUIRE(g->coff >= 0 && g->cstride > 0 && g->coff % 16 == 0 && g->cstride % 16 == 0,
-              "dfq_i8_upsample_bilinear: coff and cstride must be non-negative multiples of 16");
-  DFQ_REQUIRE((int64_t)g->coff + cpad <= g->cstride,
-              "dfq_i8_upsample_bilinear: the slice coff + round_up(C, 16) exceeds cstride");
+  if (int rc = check_slice("dfq_i8_upsample_bilinear", g->coff, g->cstride, cpad, 'C')) return rc;
   DFQ_REQUIRE(y || yq, "dfq_i8_upsample_bilinear: no output requested (y and yq are both NULL)");
   DFQ_REQUIRE(aligned16(yq), "dfq_i8_upsample_bilinear: yq must be 16-byte aligned");
   DFQ_REQUIRE(((uintptr_t)x & 3) == 0 && ((uintptr_t)y & 3) == 0, "dfq_i8_upsample_bilinear: x and y must be 4-byte aligned");
@@ -1351,6 +1332,37 @@ int check_affine(const DfqI8Conv* g, int num_bits, const char* who) {
   return 0;
 }
 
+// QuantMeasure's scalars of a quantizer with 1..8 bits (`bits_name` in the error) and a finite range whose scale and
+// inverse are finite fp32 numbers (`range_name` in the error)
+int quantizer(const char* who, const char* bits_name, const char* range_name, float lo, float hi, int32_t bits,
+              QuantScalars* q) {
+  if (bits < 1 || bits > 8) {
+    set_error("%s: %s must be in [1, 8], got %d", who, bits_name, bits);
+    return bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
+  }
+  *q = quant_scalars((double)lo, (double)hi, bits, 0);
+  if (!(std::isfinite(lo) && std::isfinite(hi) && std::isfinite(q->scale) && std::isfinite(q->inv_scale))) {
+    set_error("%s: %s [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who, range_name, lo, hi);
+    return DFQ_E_ARG;
+  }
+  return 0;
+}
+
+// What every affine convolution entry checks of its geometry, codes, weights and constants; out: its output (y or the
+// epilogue)
+int check_affine_conv(const char* who, const DfqI8Conv* g, const int8_t* xq, const int32_t* S, const int8_t* wq,
+                      const int32_t* table, const DfqI8Affine* k, const void* out) {
+  if (int rc = check_affine(g, 8, who)) return rc;
+  DFQ_REQUIRE_WHO(xq && wq && k && out, "null pointer");
+  DFQ_REQUIRE_WHO(g->groups != 1 || (S && table), "a dense layer needs S and its prefix table");
+  DFQ_REQUIRE_WHO(aligned16(xq) && aligned16(wq), "codes must be 16-byte aligned");
+  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
+    set_error("%s: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", who, k->kP, k->kA, k->kW, k->kN);
+    return DFQ_E_ARG;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace dfq
 
@@ -1359,16 +1371,8 @@ extern "C" int dfq_i8_affine_quantize(const float* x, int8_t* q, int32_t* S, int
   DFQ_REQUIRE(x && q && S && N > 0 && C > 0 && H > 0 && W > 0, "dfq_i8_affine_quantize: bad arguments");
   DFQ_REQUIRE(Cpad >= C && Cpad % 16 == 0, "dfq_i8_affine_quantize: Cpad must be a multiple of 16 that holds C");
   DFQ_REQUIRE(aligned16(q), "dfq_i8_affine_quantize: q must be 16-byte aligned");
-  if (num_bits < 1 || num_bits > 8) {
-    set_error("dfq_i8_affine_quantize: num_bits must be in [1, 8], got %d", num_bits);
-    return num_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
-  }
-  const QuantScalars qs = quant_scalars((double)act_min, (double)act_max, num_bits, 0);
-  if (!(std::isfinite(act_min) && std::isfinite(act_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
-    set_error("dfq_i8_affine_quantize: the range [%g, %g] is not finite or gives a scale that is not a finite fp32 number",
-              act_min, act_max);
-    return DFQ_E_ARG;
-  }
+  QuantScalars qs;
+  if (int rc = quantizer("dfq_i8_affine_quantize", "num_bits", "the range", act_min, act_max, num_bits, &qs)) return rc;
   const int64_t total = (int64_t)N * H * W;
   k_i8_quantize_affine<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(x, q, S, C, H * W, Cpad, total, qs.neg_min,
                                                                                 qs.inv_scale, qs.qmax);
@@ -1404,40 +1408,14 @@ extern "C" int dfq_i8_affine_pack(const float* w, float w_min, float w_scale, in
 extern "C" int dfq_i8_affine_conv(const int8_t* xq, const int32_t* S, const int8_t* wq, const int32_t* table,
                                   const DfqI8Affine* k, const float* bias, float* y, int32_t* acc_out, const DfqI8Conv* g,
                                   void* stream) {
-  if (int rc = check_affine(g, 8, "dfq_i8_affine_conv")) return rc;
-  DFQ_REQUIRE(xq && wq && k && y, "dfq_i8_affine_conv: null pointer");
-  DFQ_REQUIRE(g->groups != 1 || (S && table), "dfq_i8_affine_conv: a dense layer needs S and its prefix table");
-  DFQ_REQUIRE(aligned16(xq) && aligned16(wq), "dfq_i8_affine_conv: codes must be 16-byte aligned");
-  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
-    set_error("dfq_i8_affine_conv: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", k->kP, k->kA, k->kW,
-              k->kN);
-    return DFQ_E_ARG;
-  }
+  const char* who = "dfq_i8_affine_conv";
+  if (int rc = check_affine_conv(who, g, xq, S, wq, table, k, y)) return rc;
   const Affine ep{S, table, k->kP, k->kA, k->kW, k->kN};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (g->groups == 1) {
-    const int64_t M = (int64_t)g->N * g->OH * g->OW;
-    DFQ_REQUIRE((M + BM - 1) / BM < (1LL << 31), "dfq_i8_affine_conv: too many output pixels");
-    const dim3 grid((unsigned)((M + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<Out::AFFINE><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, y, acc_out, *g, ep);
-  } else {
-    const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-    k_i8_conv_dw<Out::AFFINE><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, y, acc_out, *g, total, ep);
-  }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<Out::AFFINE>(who, xq, wq, nullptr, bias, y, acc_out, g, ep, (cudaStream_t)stream);
 }
 
 namespace dfq {
 namespace {
-
-#define DFQ_REQUIRE_WHO(cond, msg)                                         \
-  do {                                                                     \
-    if (!(cond)) {                                                         \
-      ::dfq::set_error("%s: %s (%s)", who, msg, #cond);                    \
-      return DFQ_E_ARG;                                                    \
-    }                                                                      \
-  } while (0)
 
 // An observer of DfqI8AffineObserve: off (bits 0), or QuantMeasure's scalars of a finite range with 1..8 bits.
 int observer_scalars(const char* who, const char* which, float lo, float hi, int32_t bits, QuantScalars* q, bool* on) {
@@ -1451,13 +1429,9 @@ int observer_scalars(const char* who, const char* which, float lo, float hi, int
     return DFQ_E_UNSUPPORTED;
   }
   if (!*on) return 0;
-  *q = quant_scalars((double)lo, (double)hi, bits, 0);
-  if (!(std::isfinite(lo) && std::isfinite(hi) && std::isfinite(q->scale) && std::isfinite(q->inv_scale))) {
-    set_error("%s: the %s observer's range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
-              which, lo, hi);
-    return DFQ_E_ARG;
-  }
-  return 0;
+  char range[32];
+  std::snprintf(range, sizeof range, "the %s observer's range", which);
+  return quantizer(who, which, range, lo, hi, bits, q);
 }
 
 // dfq_i8_affine_conv_fused (o == NULL, Out::AFFINE_FUSED), dfq_i8_affine_conv_observed (Out::AFFINE_OBSERVED) and
@@ -1466,14 +1440,7 @@ template <Out OUT>
 int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
                          const DfqI8Affine* k, const float* bias, const DfqI8AffineEpilogue* e, const DfqI8AffineObserve* o,
                          const DfqI8AffineLayout* l, const DfqI8Conv* g, void* stream) {
-  if (int rc = check_affine(g, 8, who)) return rc;
-  DFQ_REQUIRE_WHO(xq && wq && k && e, "null pointer");
-  DFQ_REQUIRE_WHO(g->groups != 1 || (S_in && table), "a dense layer needs S and its prefix table");
-  DFQ_REQUIRE_WHO(aligned16(xq) && aligned16(wq), "codes must be 16-byte aligned");
-  if (!(std::isfinite(k->kP) && std::isfinite(k->kA) && std::isfinite(k->kW) && std::isfinite(k->kN))) {
-    set_error("%s: the constants kP, kA, kW, kN must be finite, got %g, %g, %g, %g", who, k->kP, k->kA, k->kW, k->kN);
-    return DFQ_E_ARG;
-  }
+  if (int rc = check_affine_conv(who, g, xq, S_in, wq, table, k, e)) return rc;
   DFQ_REQUIRE_WHO(e->y || e->yq, "no output requested (y and yq are both NULL)");
   DFQ_REQUIRE_WHO(!e->S || e->yq, "S is the sum of the codes; it needs yq");
   DFQ_REQUIRE_WHO(aligned16(e->yq), "yq must be 16-byte aligned");
@@ -1483,16 +1450,7 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
                   "pre / post clamp bounds must be ordered and not NaN");
   QuantScalars qs{};
   if (e->yq) {                                                  // the consumer's quantizer, as dfq_i8_affine_quantize
-    if (e->out_bits < 1 || e->out_bits > 8) {
-      set_error("%s: out_bits must be in [1, 8], got %d", who, e->out_bits);
-      return e->out_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
-    }
-    qs = quant_scalars((double)e->out_min, (double)e->out_max, e->out_bits, 0);
-    if (!(std::isfinite(e->out_min) && std::isfinite(e->out_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
-      set_error("%s: the output range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
-                e->out_min, e->out_max);
-      return DFQ_E_ARG;
-    }
+    if (int rc = quantizer(who, "out_bits", "the output range", e->out_min, e->out_max, e->out_bits, &qs)) return rc;
   }
   const int cpad = (g->O + 15) / 16 * 16;
   const int64_t pixels = (int64_t)g->N * g->OH * g->OW;
@@ -1500,9 +1458,7 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
   bool accumulate = false;
   if constexpr (OUT == Out::AFFINE_LAYOUT) {
     DFQ_REQUIRE_WHO(l != nullptr, "null layout descriptor");
-    DFQ_REQUIRE_WHO(l->coff >= 0 && l->cstride > 0 && l->coff % 16 == 0 && l->cstride % 16 == 0,
-                    "coff and cstride must be non-negative multiples of 16");
-    DFQ_REQUIRE_WHO((int64_t)l->coff + cpad <= l->cstride, "the slice coff + round_up(O, 16) exceeds cstride");
+    if (int rc = check_slice(who, l->coff, l->cstride, cpad, 'O')) return rc;
     DFQ_REQUIRE_WHO((l->S_accumulate == 0 || l->S_accumulate == 1) && (l->pad_code_on == 0 || l->pad_code_on == 1),
                     "S_accumulate and pad_code_on must be 0 or 1");
     DFQ_REQUIRE_WHO(!l->pad_code_on || (l->pad_code >= -128 && l->pad_code <= 127), "the pad code must be in [-128, 127]");
@@ -1518,7 +1474,6 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
                       !overlap(yq, yq_bytes, e->S, s_bytes),
                   "y, yq and S overlap");
   const bool dense = g->groups == 1;
-  DFQ_REQUIRE_WHO(!dense || (pixels + BM - 1) / BM < (1LL << 31), "too many output pixels");
   typename EpiOf<OUT>::type ep{};
   if constexpr (observed(OUT)) {
     DFQ_REQUIRE_WHO(OUT == Out::AFFINE_LAYOUT || o != nullptr, "null observer descriptor");
@@ -1539,23 +1494,12 @@ int affine_conv_epilogue(const char* who, const int8_t* xq, const int32_t* S_in,
   ep.neg_min = qs.neg_min, ep.inv_scale = qs.inv_scale, ep.qmax = qs.qmax;
   ep.pre_lo = e->pre_lo, ep.pre_hi = e->pre_hi, ep.post_lo = e->post_lo, ep.post_hi = e->post_hi;
   ep.cpad = cpad, ep.S_atomic = atomic;
-  bool pad = false;
-  if constexpr (OUT == Out::AFFINE_LAYOUT) ep.cstride = (int)cstride, ep.pad_code = l->pad_code, ep.pad_on = pad = l->pad_code_on;
-  const int64_t total = (int64_t)g->N * (g->Cpad / 16) * g->OH * g->OW;
-  if (dense) {
-    const dim3 grid((unsigned)((pixels + BM - 1) / BM), (unsigned)((g->O + BN - 1) / BN));
-    k_i8_conv_mma<OUT><<<grid, THREADS, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, ep);
-  } else if (pad) {
-    if constexpr (OUT == Out::AFFINE_LAYOUT)
-      k_i8_conv_dw<OUT, true><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total, ep);
-  } else {
-    k_i8_conv_dw<OUT><<<grid_for(total, 256), 256, 0, st>>>(xq, wq, nullptr, bias, e->y, nullptr, *g, total, ep);
+  if constexpr (OUT == Out::AFFINE_LAYOUT) {
+    ep.cstride = (int)cstride, ep.pad_code = l->pad_code, ep.pad_on = l->pad_code_on;
+    if (ep.pad_on) return launch_conv<OUT, true>(who, xq, wq, nullptr, bias, e->y, nullptr, g, ep, st);
   }
-  DFQ_CUDA(cudaGetLastError());
-  return 0;
+  return launch_conv<OUT>(who, xq, wq, nullptr, bias, e->y, nullptr, g, ep, st);
 }
-
-#undef DFQ_REQUIRE_WHO
 
 }  // namespace
 }  // namespace dfq
@@ -1592,26 +1536,15 @@ extern "C" int dfq_i8_affine_upsample_bilinear(const float* x, int8_t* yq, int32
   DFQ_REQUIRE(g->align_corners == 0 || g->align_corners == 1,
               "dfq_i8_affine_upsample_bilinear: align_corners must be 0 or 1");
   const int cpad = (g->C + 15) / 16 * 16;
-  DFQ_REQUIRE(g->coff >= 0 && g->cstride > 0 && g->coff % 16 == 0 && g->cstride % 16 == 0,
-              "dfq_i8_affine_upsample_bilinear: coff and cstride must be non-negative multiples of 16");
-  DFQ_REQUIRE((int64_t)g->coff + cpad <= g->cstride,
-              "dfq_i8_affine_upsample_bilinear: the slice coff + round_up(C, 16) exceeds cstride");
+  if (int rc = check_slice(who, g->coff, g->cstride, cpad, 'C')) return rc;
   DFQ_REQUIRE(aligned16(yq) && ((uintptr_t)x & 3) == 0 && ((uintptr_t)S & 3) == 0,
               "dfq_i8_affine_upsample_bilinear: yq must be 16-byte aligned, x and S 4-byte aligned");
   DFQ_REQUIRE(ordered(g->pre_lo, g->pre_hi) && ordered(g->post_lo, g->post_hi),
               "dfq_i8_affine_upsample_bilinear: pre / post clamp bounds must be ordered and not NaN");
   AffineResize a{};
   if (int rc = observer_scalars(who, "obs", g->obs_min, g->obs_max, g->obs_bits, &a.obs, &a.obs_on)) return rc;
-  if (g->out_bits < 1 || g->out_bits > 8) {
-    set_error("%s: out_bits must be in [1, 8], got %d", who, g->out_bits);
-    return g->out_bits > 8 ? DFQ_E_UNSUPPORTED : DFQ_E_ARG;
-  }
-  const QuantScalars qs = quant_scalars((double)g->out_min, (double)g->out_max, g->out_bits, 0);
-  if (!(std::isfinite(g->out_min) && std::isfinite(g->out_max) && std::isfinite(qs.scale) && std::isfinite(qs.inv_scale))) {
-    set_error("%s: the output range [%g, %g] is not finite or gives a scale that is not a finite fp32 number", who,
-              g->out_min, g->out_max);
-    return DFQ_E_ARG;
-  }
+  QuantScalars qs;
+  if (int rc = quantizer(who, "out_bits", "the output range", g->out_min, g->out_max, g->out_bits, &qs)) return rc;
   const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
   const int8_t* slice = yq + g->coff;
   const int64_t x_bytes = in_px * g->C * 4, slice_bytes = (out_px - 1) * g->cstride + cpad, s_bytes = out_px * 4;

@@ -27,6 +27,7 @@ pads into the convolutions after them as pad codes and has the producers and bil
 write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear).
 """
 import ctypes as C
+import dataclasses
 import operator
 import os
 import sys
@@ -88,7 +89,110 @@ def _ordered(lo, hi, what="activation"):
     return float(lo), float(hi)
 
 
-class _Int8Layer(nn.Module):
+def _channel_slice(out_slice, channels, who):
+    """(coff, cstride) of channels [coff, coff + round_up(channels, 16)) of an int8 NHWC tensor of cstride channels (a
+    concatenation's codes), or DfqError naming `who` when the slice is not 16-aligned inside it."""
+    coff, cstride = (int(v) for v in out_slice)
+    if coff < 0 or coff % 16 or cstride % 16 or coff + (channels + 15) // 16 * 16 > cstride:
+        raise _lib.DfqError("%s: channel slice (%d, %d) is not 16-aligned inside its tensor" % (who, coff, cstride))
+    return coff, cstride
+
+
+def _zero_padding_refusal(conv, who=""):
+    """The DfqError refusing an nn.Conv2d whose padding is not numeric zero padding (all the int8 kernels compute), its
+    text prefixed by `who`; None when it is."""
+    if conv.padding_mode == "zeros" and not isinstance(conv.padding, str):
+        return None
+    return _lib.DfqError("%sint8 execution supports numeric zero padding only (padding=%r, padding_mode=%r)"
+                         % (who, conv.padding, conv.padding_mode))
+
+
+class _ConvLayer(nn.Module):
+    """What the two schemes' convolution layers share: the shape of the convolution, its geometry table, the copies
+    `chained` makes and the checks of `run`."""
+
+    codes_in = False
+    epilogue = None
+    out_slice = None
+    layer_name = None
+    _copied = ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad")
+
+    def __init__(self, weight, stride, padding, dilation, groups):
+        super().__init__()
+        O, Cg, kh, kw = weight.shape
+        self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
+        self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
+        self.cpad = (self.in_channels + 15) // 16 * 16
+
+    def _geometry(self, N, H, W, stride=None, padding=None):
+        (sh, sw), (ph, pw), (dh, dw) = stride or self.stride, padding or self.padding, self.dilation
+        kh, kw = self.kernel_size
+        g = np.zeros(1, _lib.I8_CONV_DT)
+        for k, v in dict(N=N, C=self.in_channels, H=H, W=W, O=self.out_channels, kh=kh, kw=kw, stride_h=sh, stride_w=sw,
+                         pad_h=ph, pad_w=pw, dil_h=dh, dil_w=dw, groups=self.groups,
+                         OH=(H + 2 * ph - dh * (kh - 1) - 1) // sh + 1, OW=(W + 2 * pw - dw * (kw - 1) - 1) // sw + 1,
+                         Cpad=self.cpad).items():
+            g[0][k] = v
+        return g
+
+    def _pack_geometry(self):
+        # geometry of a 1-pixel image: the packers only read O, C, kh, kw, groups and Cpad
+        kh, kw = self.kernel_size
+        return self._geometry(1, (kh - 1) * self.dilation[0] + 1, (kw - 1) * self.dilation[1] + 1, stride=(1, 1),
+                              padding=(0, 0))
+
+    def _who(self):
+        return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
+                                                                  self.kernel_size)
+
+    def _copy(self, codes_in, name):
+        """A new module of the same class on the same buffers, with the attributes in _copied, codes_in and name."""
+        new = type(self).__new__(type(self))
+        nn.Module.__init__(new)
+        for k in self._copied:
+            setattr(new, k, getattr(self, k))
+        for k, b in self._buffers.items():
+            new.register_buffer(k, b)
+        new.codes_in = bool(codes_in)
+        new.layer_name = name
+        return new
+
+    def _check_residual(self, residual):
+        if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
+            raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
+                                                    "takes no residual input"))
+
+    def _check_out(self, out):
+        if out is not None and self.out_slice is None:
+            raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
+
+    def _output_geometry(self, N, H, W):
+        """(geometry, OH, OW) of an input [N, *, H, W], or DfqError when it is smaller than the kernel."""
+        g = self._geometry(N, H, W)
+        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
+        if OH <= 0 or OW <= 0:
+            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        return g, OH, OW
+
+    def _residual(self, r, shape, dev):
+        """The residual r, checked to be fp32 `shape` on dev, contiguous; None when r is."""
+        if r is None:
+            return None
+        if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
+                r.device != dev:
+            raise _lib.DfqError("layer %s: the residual must be fp32 %s on %s, got %s" % (
+                self._who(), list(shape), dev, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
+                if isinstance(r, torch.Tensor) else type(r).__name__))
+        return r.contiguous()
+
+    def _linear_forward(self, x):
+        """forward of the Linear layers: x [..., in_features] as the 1x1 convolution of [B, I, 1, 1]."""
+        lead = x.shape[:-1]
+        y, _ = self.run(x.reshape(-1, self.in_channels, 1, 1))
+        return y.reshape(*lead, self.out_channels)
+
+
+class _Int8Layer(_ConvLayer):
     """Packed int8 weights, dq and bias of one layer on the device; forward quantizes the input and convolves.
 
     Execution modes, set only on the copies chain_int8 makes (`chained`): `codes_in` - the input is already int8 NHWC codes
@@ -97,22 +201,15 @@ class _Int8Layer(nn.Module):
     `rows` - the clamped fp32 output pixel-major, a detection head's rows of its concatenation (dfq_i8_conv_nhwc).
     A layer convert_to_int8 made takes and returns fp32 only."""
 
-    codes_in = False
     requant = None
-    epilogue = None
-    out_slice = None
     rows = False
-    layer_name = None
+    _copied = _ConvLayer._copied + ("act_scale",)
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
-        super().__init__()
-        O, Cg, kh, kw = weight.shape
-        self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
-        self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
-        self.cpad = (self.in_channels + 15) // 16 * 16
-        who = "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, int(O), self.kernel_size)
-        check_scale("activation", act_scale, who)
-        check_scale("weight", w_scale, who)
+        super().__init__(weight, stride, padding, dilation, groups)
+        O, _, kh, kw = weight.shape
+        check_scale("activation", act_scale, self._who())
+        check_scale("weight", w_scale, self._who())
         self.act_scale = float(_f32(act_scale))
         depthwise = self.groups == self.in_channels == self.out_channels and self.groups > 1
         if self.groups != 1 and not depthwise:
@@ -128,24 +225,11 @@ class _Int8Layer(nn.Module):
         b = torch.zeros(O) if bias is None else bias.detach().float()
         self.register_buffer("bias", b.to(dev).contiguous())
         w = weight.detach().float().to(dev).contiguous()
-        # geometry of a 1-pixel image: the packer only reads O, C, kh, kw, groups and Cpad
-        g = self._geometry(1, (kh - 1) * self.dilation[0] + 1, (kw - 1) * self.dilation[1] + 1, stride=(1, 1), padding=(0, 0))
         lib = _lib.load()
-        _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes), _lib.table_ptr(g),
-                                           _lib.stream_ptr()), "dfq_i8_pack_weights")
+        _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes),
+                                           _lib.table_ptr(self._pack_geometry()), _lib.stream_ptr()), "dfq_i8_pack_weights")
 
-    def _geometry(self, N, H, W, stride=None, padding=None):
-        (sh, sw), (ph, pw), (dh, dw) = stride or self.stride, padding or self.padding, self.dilation
-        kh, kw = self.kernel_size
-        g = np.zeros(1, _lib.I8_CONV_DT)
-        for k, v in dict(N=N, C=self.in_channels, H=H, W=W, O=self.out_channels, kh=kh, kw=kw, stride_h=sh, stride_w=sw,
-                         pad_h=ph, pad_w=pw, dil_h=dh, dil_w=dw, groups=self.groups,
-                         OH=(H + 2 * ph - dh * (kh - 1) - 1) // sh + 1, OW=(W + 2 * pw - dw * (kw - 1) - 1) // sw + 1,
-                         Cpad=self.cpad).items():
-            g[0][k] = v
-        return g
-
-    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None, rows=False):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None, rows=False, sums=False):
         """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
         mode: codes_in - take int8 NHWC codes; requant = (out_scale, lo, hi) - return the next layer's codes; epilogue - an
         Epilogue: the residual epilogue (not together with requant); out_slice = (coff, cstride), with requant - write the
@@ -154,16 +238,10 @@ class _Int8Layer(nn.Module):
         pixel-major (dfq_i8_conv_nhwc): forward(x, out=y, off=off) writes permute(0, 2, 3, 1) of it as OH * OW * C_out floats
         at y[n].view(-1)[off:] of a contiguous fp32 y [N, ...] (a detection head's slice of its [N, R, k] concatenation), or
         returns a new [N, OH * OW, C_out] tensor when out is None; the clamps come from an fp32-only epilogue without
-        residual (none: no clamp), and rows excludes requant.  name: the layer's name in error messages.  self is not
-        modified."""
-        new = type(self).__new__(type(self))
-        nn.Module.__init__(new)
-        for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad", "act_scale"):
-            setattr(new, k, getattr(self, k))
-        for k, b in self._buffers.items():
-            new.register_buffer(k, b)
-        new.codes_in = bool(codes_in)
-        new.layer_name = name
+        residual (none: no clamp), and rows excludes requant.  name: the layer's name in error messages.  sums: the affine
+        scheme's per-pixel code sums (_AffineInt8Layer.chained); ncnn codes have none, so it changes nothing here.  self
+        is not modified."""
+        new = self._copy(codes_in, name)
         if requant is not None and epilogue is not None:
             raise _lib.DfqError("layer %s: requant and epilogue are two output modes; give one" % new._who())
         if requant is not None:
@@ -182,13 +260,9 @@ class _Int8Layer(nn.Module):
                                 _ordered(*e.post, what="post-add"), bool(e.residual), bool(e.fp32))
         new.epilogue = epilogue
         if out_slice is not None:
-            coff, cstride = (int(v) for v in out_slice)
             if requant is None:
                 raise _lib.DfqError("layer %s: a channel slice needs requant" % new._who())
-            if coff < 0 or coff % 16 or cstride % 16 or coff + (self.out_channels + 15) // 16 * 16 > cstride:
-                raise _lib.DfqError("layer %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
-                                    % (new._who(), coff, cstride))
-            out_slice = (coff, cstride)
+            out_slice = _channel_slice(out_slice, self.out_channels, "layer %s" % new._who())
         new.out_slice = out_slice
         if rows:
             if requant is not None or out_slice is not None or \
@@ -197,10 +271,6 @@ class _Int8Layer(nn.Module):
             new.epilogue = epilogue or Epilogue(fp32=True)
         new.rows = bool(rows)
         return new
-
-    def _who(self):
-        return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
-                                                                  self.kernel_size)
 
     def run(self, x, with_acc=False, residual=None, out=None, off=0):
         """(y, acc | None) for x [N, C, H, W] fp32 on the GPU; acc = the int32 sums before the epilogue.  In the chained modes
@@ -223,14 +293,9 @@ class _Int8Layer(nn.Module):
             N, _, H, W = x.shape
         if (self.requant is not None or self.epilogue is not None) and with_acc:
             raise _lib.DfqError("a requantizing int8 layer does not return its int32 sums")
-        if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
-            raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
-                                                    "takes no residual input"))
+        self._check_residual(residual)
         x = x.contiguous()
-        g = self._geometry(N, H, W)
-        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
-        if OH <= 0 or OW <= 0:
-            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        g, OH, OW = self._output_geometry(N, H, W)
         lib, st = _lib.load(), _lib.stream_ptr()
         if self.codes_in:
             xq = x
@@ -242,8 +307,7 @@ class _Int8Layer(nn.Module):
             return self._run_rows(xq, out, off, g, N, OH, OW), None
         if self.epilogue is not None:
             return self._run_fused(xq, residual, g, N, OH, OW), None
-        if out is not None and self.out_slice is None:
-            raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
+        self._check_out(out)
         if self.out_slice is not None:
             return self._run_slice(xq, out, g, N, OH, OW), None
         if self.requant is not None:
@@ -304,13 +368,7 @@ class _Int8Layer(nn.Module):
     def _run_fused(self, xq, r, g, N, OH, OW):
         e = self.epilogue
         shape = (N, self.out_channels, OH, OW)
-        if r is not None:
-            if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
-                    r.device != xq.device:
-                raise _lib.DfqError("layer %s: the residual must be fp32 %s on %s, got %s" % (
-                    self._who(), list(shape), xq.device, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
-                    if isinstance(r, torch.Tensor) else type(r).__name__))
-            r = r.contiguous()
+        r = self._residual(r, shape, xq.device)
         yq = None if e.out_scale is None else \
             torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=xq.device)
         y = torch.empty(shape, dtype=torch.float32, device=xq.device) if e.fp32 else None
@@ -329,9 +387,9 @@ class Int8Conv2d(_Int8Layer):
 
     @classmethod
     def from_conv(cls, conv: nn.Conv2d, act_scale, w_scale):
-        if isinstance(conv.padding, str) or conv.padding_mode != "zeros":
-            raise _lib.DfqError("int8 execution supports numeric zero padding only (padding=%r, padding_mode=%r)"
-                                % (conv.padding, conv.padding_mode))
+        err = _zero_padding_refusal(conv)
+        if err is not None:
+            raise err
         return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
 
     def forward(self, x, r=None, out=None, off=0):
@@ -350,10 +408,7 @@ class Int8Linear(_Int8Layer):
     def from_linear(cls, lin: nn.Linear, act_scale, w_scale):
         return cls(lin.weight.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias, act_scale, w_scale)
 
-    def forward(self, x):
-        lead = x.shape[:-1]
-        y, _ = self.run(x.reshape(-1, self.in_channels, 1, 1))
-        return y.reshape(*lead, self.out_channels)
+    forward = _ConvLayer._linear_forward
 
     def extra_repr(self):
         return "in_features=%d, out_features=%d, act_scale=%g" % (self.in_channels, self.out_channels, self.act_scale)
@@ -402,7 +457,7 @@ def weight_grid_candidates(w_min, w_max, num_bits):
     return [c for t, c in sorted(zip(top, cands), key=lambda tc: not tc[0])]
 
 
-class _AffineInt8Layer(nn.Module):
+class _AffineInt8Layer(_ConvLayer):
     """One layer of a fake-quantized model executed in integer arithmetic (dfq_i8_affine_*): the input is quantized with the
     range its `quant` observer had at conversion, the weight codes are recovered from the fake-quantized weights, and the
     output is fp32 NCHW.  The ranges are frozen: an observer whose update_stat is truthy would keep widening its range in
@@ -414,27 +469,21 @@ class _AffineInt8Layer(nn.Module):
     `out_slice` = (coff, cstride) - the codes go to a channel slice of a concatenation's codes and S adds into its sums;
     `pad_code` - the shifted code every out-of-image tap reads (a folded F.pad; dfq_i8_affine_conv_layout)."""
 
-    codes_in = False
-    epilogue = None
     sums = False
     observers = (None, None)
-    out_slice = None
     pad_code = None
+    _copied = _ConvLayer._copied + ("act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants", "pad_code")
 
     def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
                  name=None):
-        super().__init__()
-        O, Cg, kh, kw = weight.shape
-        self.out_channels, self.in_channels, self.groups = int(O), int(Cg) * int(groups), int(groups)
-        self.kernel_size, self.stride, self.padding, self.dilation = (int(kh), int(kw)), _pair(stride), _pair(padding), _pair(dilation)
-        self.cpad = (self.in_channels + 15) // 16 * 16
+        super().__init__(weight, stride, padding, dilation, groups)
+        O, _, kh, kw = weight.shape
         self.layer_name = name
         _affine_refusal(self._who(), self.in_channels, self.out_channels, self.groups, self.kernel_size, act_bits, w_bits)
-        self.act_bits, self.w_bits = int(act_bits), int(w_bits)
-        self.act_min, self.act_max = float(_f32(act_min)), float(_f32(act_max))
+        self.w_bits = int(w_bits)
+        self.act_min, self.act_max, self.act_bits = _affine_range(_f32(act_min), act_max, act_bits, "layer %s" % self._who(),
+                                                                  "activation range")
         ma, fa = act_affine_scalars(act_min, act_max, act_bits)
-        if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(act_max))):
-            raise _lib.DfqError("layer %s: activation range [%g, %g] gives no finite fp32 scale" % (self._who(), ma, act_max))
         dev = engine._default_device()
         depthwise = self.groups > 1
         taps = kh * kw
@@ -456,8 +505,7 @@ class _AffineInt8Layer(nn.Module):
 
     def _pack(self, w, mw, mx):
         """Pack the codes at the first candidate scale whose round trip reproduces every weight; returns it."""
-        kh, kw = self.kernel_size
-        g = self._geometry(1, (kh - 1) * self.dilation[0] + 1, (kw - 1) * self.dilation[1] + 1, stride=(1, 1), padding=(0, 0))
+        g = self._pack_geometry()
         lib, st = _lib.load(), _lib.stream_ptr()
         n_bad = torch.zeros(1, dtype=torch.int32, device=w.device)
         fewest = None
@@ -473,12 +521,6 @@ class _AffineInt8Layer(nn.Module):
                             "the best candidate scale): run quantize_targ_layer first"
                             % (self._who(), self.w_bits, mw, mx, "all" if fewest is None else fewest, w.numel()))
 
-    _geometry = _Int8Layer._geometry
-
-    def _who(self):
-        return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
-                                                                  self.kernel_size)
-
     def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False, out_slice=None):
         """A new module of the same class on the same buffers (weight_codes, tap_table, bias, constants), in the given
         execution mode: codes_in - take (codes, S) from the previous layer's epilogue instead of quantizing fp32; requant =
@@ -489,15 +531,7 @@ class _AffineInt8Layer(nn.Module):
         [coff, coff + round_up(C_out, 16)) of a concatenation's codes [N, OH, OW, cstride] and add S into its sums,
         given as forward(x, out=(codes, S | None)) or made (S zeroed) when out is None.  The pad code of a folded F.pad is
         kept.  name: the layer's name in error messages.  self is not modified."""
-        new = type(self).__new__(type(self))
-        nn.Module.__init__(new)
-        for k in ("out_channels", "in_channels", "groups", "kernel_size", "stride", "padding", "dilation", "cpad",
-                  "act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants", "pad_code"):
-            setattr(new, k, getattr(self, k))
-        for k, b in self._buffers.items():
-            new.register_buffer(k, b)
-        new.codes_in = bool(codes_in)
-        new.layer_name = name or self.layer_name
+        new = self._copy(codes_in, name or self.layer_name)
         if requant is not None and epilogue is not None:
             raise _lib.DfqError("layer %s: requant and epilogue are two output modes; give one" % new._who())
         if requant is not None:
@@ -512,22 +546,15 @@ class _AffineInt8Layer(nn.Module):
                 lo, hi, bits = e.out_scale
                 who = "%s -> next layer" % new._who()
                 _affine_refusal(who, 1, 1, 1, (1, 1), bits, 8)
-                ma, fa = act_affine_scalars(lo, hi, bits)
-                if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(hi))):
-                    raise _lib.DfqError("layer %s: output range [%g, %g] gives no finite fp32 scale" % (who, lo, hi))
-                out = (float(_f32(lo)), float(_f32(hi)), int(bits))
+                out = _affine_range(lo, hi, bits, "layer %s" % who, "output range")
             epilogue = Epilogue(out, _ordered(*e.pre, what="pre-add"), _ordered(*e.post, what="post-add"), bool(e.residual),
                                 bool(e.fp32))
         new.epilogue = epilogue
         new.sums = bool(sums) and epilogue is not None and epilogue.out_scale is not None
         if out_slice is not None:
-            coff, cstride = (int(v) for v in out_slice)
             if epilogue is None or epilogue.out_scale is None or epilogue.fp32 or epilogue.residual:
                 raise _lib.DfqError("layer %s: a channel slice takes the codes only, without a residual" % new._who())
-            if coff < 0 or coff % 16 or cstride % 16 or coff + (self.out_channels + 15) // 16 * 16 > cstride:
-                raise _lib.DfqError("layer %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
-                                    % (new._who(), coff, cstride))
-            out_slice = (coff, cstride)
+            out_slice = _channel_slice(out_slice, self.out_channels, "layer %s" % new._who())
         new.out_slice = out_slice
         return new
 
@@ -596,16 +623,10 @@ class _AffineInt8Layer(nn.Module):
         concatenation's (codes, S | None)) or a new such pair, its slice written."""
         if (self.epilogue is not None or self.pad_code is not None) and with_acc:
             raise _lib.DfqError("a chained affine layer does not return its int32 sums")
-        if out is not None and self.out_slice is None:
-            raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
-        if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
-            raise _lib.DfqError("layer %s: %s" % (self._who(), "takes a residual input" if residual is None else
-                                                    "takes no residual input"))
+        self._check_out(out)
+        self._check_residual(residual)
         xq, S, N, H, W = self._input(x)
-        g = self._geometry(N, H, W)
-        OH, OW = int(g[0]["OH"]), int(g[0]["OW"])
-        if OH <= 0 or OW <= 0:
-            raise _lib.DfqError("int8 layer: input %dx%d is smaller than the kernel" % (H, W))
+        g, OH, OW = self._output_geometry(N, H, W)
         if self.epilogue is not None or self.pad_code is not None:
             return self._run_fused(xq, S, residual, g, N, OH, OW, out), None
         lib, st = _lib.load(), _lib.stream_ptr()
@@ -620,13 +641,7 @@ class _AffineInt8Layer(nn.Module):
     def _run_fused(self, xq, S, r, g, N, OH, OW, out=None):
         e = self.epilogue or Epilogue(fp32=True)                # a folded pad alone: the fp32 output through the layout
         shape = (N, self.out_channels, OH, OW)
-        if r is not None:
-            if not isinstance(r, torch.Tensor) or r.dtype != torch.float32 or not r.is_cuda or tuple(r.shape) != shape or \
-                    r.device != xq.device:
-                raise _lib.DfqError("layer %s: the residual must be fp32 %s on %s, got %s" % (
-                    self._who(), list(shape), xq.device, "%s %s on %s" % (r.dtype, list(r.shape), r.device)
-                    if isinstance(r, torch.Tensor) else type(r).__name__))
-            r = r.contiguous()
+        r = self._residual(r, shape, xq.device)
         if self.out_slice is not None:
             yq, S_out = self._slice_buffers(out, N, OH, OW, xq.device)
         else:
@@ -683,9 +698,15 @@ def _observer_range(o, who):
     lo, hi, bits = o
     if not isinstance(bits, (int, np.integer)) or isinstance(bits, bool) or not 1 <= bits <= 8:
         raise _lib.DfqError("%s: %r bits do not fit the int8 epilogue (1 to 8 bits)" % (who, bits))
+    return _affine_range(lo, hi, bits, who, "range")
+
+
+def _affine_range(lo, hi, bits, who, what):
+    """(fp32 lo, fp32 hi, bits) of a quantizer's range and bits (1 to 8, checked by the caller), or DfqError
+    "<who>: <what> [lo, hi] gives no finite fp32 scale" when its QuantMeasure scale is not a finite fp32 number."""
     ma, fa = act_affine_scalars(lo, hi, bits)
     if not (np.isfinite(ma) and np.isfinite(fa) and np.isfinite(_f32(hi))):
-        raise _lib.DfqError("%s: range [%g, %g] gives no finite fp32 scale" % (who, lo, hi))
+        raise _lib.DfqError("%s: %s [%g, %g] gives no finite fp32 scale" % (who, what, lo, hi))
     return float(_f32(lo)), float(_f32(hi)), int(bits)
 
 
@@ -735,9 +756,9 @@ class AffineInt8Conv2d(_AffineInt8Layer):
 
     @classmethod
     def from_conv(cls, conv: nn.Conv2d, act_min, act_max, act_bits=8, w_bits=8, name=None):
-        if isinstance(conv.padding, str) or conv.padding_mode != "zeros":
-            raise _lib.DfqError("layer %s: int8 execution supports numeric zero padding only (padding=%r, padding_mode=%r)"
-                                % (name, conv.padding, conv.padding_mode))
+        err = _zero_padding_refusal(conv, "layer %s: " % name)
+        if err is not None:
+            raise err
         return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
                    conv.groups, name=name)
 
@@ -753,10 +774,7 @@ class AffineInt8Linear(_AffineInt8Layer):
         return cls(lin.weight.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias, act_min, act_max, act_bits, w_bits,
                    name=name)
 
-    def forward(self, x):
-        lead = x.shape[:-1]
-        y, _ = self.run(x.reshape(-1, self.in_channels, 1, 1))
-        return y.reshape(*lead, self.out_channels)
+    forward = _ConvLayer._linear_forward
 
 
 def _pool_extent(n, k, p, s, d, ceil_mode):
@@ -817,6 +835,21 @@ class Int8MaxPool2d(nn.Module):
             "codes" if self.codes_in else "fp32 in, out_scale=%s, fp32=%s" % (self.out_scale, self.fp32))
 
 
+def _upsample_input(x, size, channels, name):
+    """(N, H, W, OH, OW) of an int8 bilinear upsample's input x, fp32 [N, channels, H, W] on the GPU, to its run-time size,
+    a pair of positive ints; DfqError otherwise."""
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise _lib.DfqError("int8 bilinear upsample %s runs on the GPU only (no CPU fallback)" % name)
+    if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != channels:
+        raise _lib.DfqError("int8 bilinear upsample %s expects fp32 [N, %d, H, W], got %s %s"
+                            % (name, channels, x.dtype, tuple(x.shape)))
+    if not isinstance(size, (tuple, list)) or len(size) != 2 or \
+            not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in size):
+        raise _lib.DfqError("int8 bilinear upsample %s: size must be a pair of positive ints, got %r" % (name, size))
+    N, _, H, W = x.shape
+    return N, H, W, int(size[0]), int(size[1])
+
+
 class Int8UpsampleBilinear(nn.Module):
     """F.interpolate(x, size, mode='bilinear', align_corners=...) of a chained model (dfq_i8_upsample_bilinear): fp32 NCHW
     [N, channels, H, W] in, the codes q(clamp(y, *clamp), out_scale) of torch's bilinear output y out - int8 NHWC
@@ -831,26 +864,10 @@ class Int8UpsampleBilinear(nn.Module):
         check_scale("output", out_scale, "bilinear upsample %s" % name)
         self.out_scale = float(_f32(out_scale))
         self.clamp = _ordered(*clamp, what="upsample %s clamp" % name)
-        if out_slice is not None:
-            coff, cstride = (int(v) for v in out_slice)
-            if coff < 0 or coff % 16 or cstride % 16 or coff + self.cpad > cstride:
-                raise _lib.DfqError("bilinear upsample %s: channel slice (%d, %d) is not 16-aligned inside its tensor"
-                                    % (name, coff, cstride))
-            out_slice = (coff, cstride)
-        self.out_slice = out_slice
+        self.out_slice = None if out_slice is None else _channel_slice(out_slice, self.channels, "bilinear upsample %s" % name)
 
     def forward(self, x, size, out=None):
-        if not isinstance(x, torch.Tensor) or not x.is_cuda:
-            raise _lib.DfqError("int8 bilinear upsample %s runs on the GPU only (no CPU fallback)" % self.layer_name)
-        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.channels:
-            raise _lib.DfqError("int8 bilinear upsample %s expects fp32 [N, %d, H, W], got %s %s"
-                                % (self.layer_name, self.channels, x.dtype, tuple(x.shape)))
-        if not isinstance(size, (tuple, list)) or len(size) != 2 or \
-                not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in size):
-            raise _lib.DfqError("int8 bilinear upsample %s: size must be a pair of positive ints, got %r"
-                                % (self.layer_name, size))
-        N, _, H, W = x.shape
-        OH, OW = int(size[0]), int(size[1])
+        N, H, W, OH, OW = _upsample_input(x, size, self.channels, self.layer_name)
         coff, cstride = self.out_slice or (0, self.cpad)
         shape = (N, OH, OW, cstride)
         if out is not None and self.out_slice is None:
@@ -889,23 +906,10 @@ class AffineInt8UpsampleBilinear(nn.Module):
         self.out = _observer_range(out, who + " output")
         self.obs = None if obs is None else _observer_range(obs, who + " observer")
         self.pre, self.post = _ordered(*pre, what=who + " pre"), _ordered(*post, what=who + " post")
-        coff, cstride = (int(v) for v in out_slice)
-        if coff < 0 or coff % 16 or cstride % 16 or coff + (self.channels + 15) // 16 * 16 > cstride:
-            raise _lib.DfqError("%s: channel slice (%d, %d) is not 16-aligned inside its tensor" % (who, coff, cstride))
-        self.out_slice = (coff, cstride)
+        self.out_slice = _channel_slice(out_slice, self.channels, who)
 
     def forward(self, x, size, out=None):
-        if not isinstance(x, torch.Tensor) or not x.is_cuda:
-            raise _lib.DfqError("int8 bilinear upsample %s runs on the GPU only (no CPU fallback)" % self.layer_name)
-        if x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.channels:
-            raise _lib.DfqError("int8 bilinear upsample %s expects fp32 [N, %d, H, W], got %s %s"
-                                % (self.layer_name, self.channels, x.dtype, tuple(x.shape)))
-        if not isinstance(size, (tuple, list)) or len(size) != 2 or \
-                not all(isinstance(v, int) and not isinstance(v, bool) and v > 0 for v in size):
-            raise _lib.DfqError("int8 bilinear upsample %s: size must be a pair of positive ints, got %r"
-                                % (self.layer_name, size))
-        N, _, H, W = x.shape
-        OH, OW = int(size[0]), int(size[1])
+        N, H, W, OH, OW = _upsample_input(x, size, self.channels, self.layer_name)
         coff, cstride = self.out_slice
         codes, S = _concat_buffers(out, (N, OH, OW, cstride), self.sums, x.device, "bilinear upsample %s" % self.layer_name)
         x = x.contiguous()
@@ -982,7 +986,7 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
         check_scale("weight", w_scale, name)
         if isinstance(layer, nn.Conv2d):
             ok = (layer.groups == 1 or layer.groups == layer.in_channels == layer.out_channels) and \
-                layer.padding_mode == "zeros" and not isinstance(layer.padding, str)
+                _zero_padding_refusal(layer) is None
         else:
             ok = isinstance(layer, nn.Linear)
         if not ok:
@@ -991,9 +995,8 @@ def convert_to_int8(model: nn.Module, graph, targ_type, act_scales=None):
         plan.append((name, layer, a, w_scale))
     done = []
     for name, layer, a, w_scale in plan:
-        new = (Int8Conv2d.from_conv if isinstance(layer, nn.Conv2d) else Int8Linear.from_linear)(layer, a, w_scale)
-        parent_name, _, attr = name.rpartition(".")
-        setattr(model.get_submodule(parent_name) if parent_name else model, attr, new)
+        _set_module(model, name, (Int8Conv2d.from_conv if isinstance(layer, nn.Conv2d) else Int8Linear.from_linear)(
+            layer, a, w_scale))
         done.append(name)
     return done
 
@@ -1025,9 +1028,9 @@ def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
         if quant is None or not hasattr(quant, "running_min"):
             raise _lib.DfqError("layer %s has no `quant` observer with an activation range" % name)
         if isinstance(layer, nn.Conv2d):
-            if layer.padding_mode != "zeros" or isinstance(layer.padding, str):
-                raise _lib.DfqError("layer %s: int8 execution supports numeric zero padding only (padding=%r, "
-                                    "padding_mode=%r)" % (name, layer.padding, layer.padding_mode))
+            err = _zero_padding_refusal(layer, "layer %s: " % name)
+            if err is not None:
+                raise err
             shape = (layer.in_channels, layer.out_channels, layer.groups, tuple(layer.kernel_size))
         elif isinstance(layer, nn.Linear):
             shape = (layer.in_features, layer.out_features, 1, (1, 1))
@@ -1043,9 +1046,14 @@ def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
         else:
             new.append(AffineInt8Linear.from_linear(layer, lo, hi, bits, bits_weight, name=name))
     for (name, *_), mod in zip(plan, new):
-        parent_name, _, attr = name.rpartition(".")
-        setattr(model.get_submodule(parent_name) if parent_name else model, attr, mod)
+        _set_module(model, name, mod)
     return [name for name, *_ in plan]
+
+
+def _set_module(root, name, mod):
+    """Replace the submodule of root at the dotted `name` by mod."""
+    parent, _, attr = name.rpartition(".")
+    setattr(root.get_submodule(parent) if parent else root, attr, mod)
 
 
 # ---- chaining converted convolutions through int8 codes ---------------------------------------------------------------
@@ -1066,7 +1074,7 @@ class _Int8Tracer(fx.Tracer):
         self.callers = callers
 
     def is_leaf_module(self, m, qualname):
-        return isinstance(m, (_Int8Layer, _AffineInt8Layer)) or super().is_leaf_module(m, qualname)
+        return isinstance(m, _ConvLayer) or super().is_leaf_module(m, qualname)
 
     def create_proxy(self, kind, target, args, kwargs, *rest, **kw):
         proxy = super().create_proxy(kind, target, args, kwargs, *rest, **kw)
@@ -1130,6 +1138,30 @@ def _compose(first, then):
     """The one clamp equal to clamp(clamp(v, *first), *then); both keep NaN."""
     (a, b), (c, d) = first, then
     return (min(max(a, c), d), max(min(b, d), c))
+
+
+def _data_users(node, queries):
+    """node's users, without those that only read its shape when `queries`."""
+    return [u for u in node.users if not (queries and _shape_query(u, node))]
+
+
+def _walk_back(node, mods, stop, queries=False):
+    """(source, clamp, path) of the single-user pass-through chain that ends at `node`: from node back through
+    pass-throughs of one fx node to the first node for which stop(n) holds, every node on the way, the source included,
+    with exactly one user (users that only read its shape not counted when `queries`); clamp composes the pass-throughs'
+    (the first in graph order runs first), path lists them from node back.  None when the chain ends elsewhere."""
+    clamp, path = (-_INF, _INF), []
+    while True:
+        if len(_data_users(node, queries)) != 1:
+            return None
+        if stop(node):
+            return node, clamp, path
+        c = _pass_through(node, mods)
+        if c is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
+            return None
+        clamp = _compose(c, clamp)                              # walking backwards: this clamp runs first
+        path.append(node)
+        node = node.args[0]
 
 
 def _is_identity(node, mods):
@@ -1298,8 +1330,7 @@ def _fold_pads(gm, mods, conv, affine=False):
         else:
             new = m.chained(name=q.target)
             new.padding = (m.padding[0] + tl[0], m.padding[1] + tl[1])
-        parent, _, attr = q.target.rpartition(".")
-        setattr(gm.get_submodule(parent) if parent else gm, attr, new)
+        _set_module(gm, q.target, new)
         mods[q.target] = new
         q.args = (node.args[0],)
         gm.graph.erase_node(node)
@@ -1326,17 +1357,13 @@ def _head_operand(view, conv, mods):
             and tuple(node.args[1:] if len(node.args) == 5 else (node.args[1] if len(node.args) == 2 else ())) == (0, 2, 3, 1)):
         return None
     path.append(node)
-    node, clamp = node.args[0], (-_INF, _INF)
-    while not conv(node):
-        c = _pass_through(node, mods)
-        if c is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
-            return None
-        clamp = _compose(c, clamp)
-        path.append(node)
-        node = node.args[0]
+    back = _walk_back(node.args[0], mods, conv, queries=True)
+    if back is None:
+        return None
+    node, clamp, between = back
     if len(node.args) != 1 or node.kwargs or not isinstance(node.args[0], fx.Node):
         return None
-    path.append(node)
+    path += between + [node]
 
     def query_nodes(u, n):
         """[u, ...] when u reads a shape of n and everything it feeds ends at the view; None otherwise."""
@@ -1398,8 +1425,7 @@ def _fuse_heads(gm, conv, mods):
             p = h["p"]
             layer = gm.get_submodule(p.target).chained(codes_in=gm.get_submodule(p.target).codes_in, name=p.target,
                                                       epilogue=Epilogue(None, h["clamp"], fp32=True), rows=True)
-            parent, _, attr = p.target.rpartition(".")
-            setattr(gm.get_submodule(parent) if parent else gm, attr, layer)
+            _set_module(gm, p.target, layer)
             layers.append(layer)
         name = "int8_heads_" + c.name
         gm.add_submodule(name, Int8HeadConcat(layers, heads[0]["k"], batch, name=c.name))
@@ -1618,25 +1644,20 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=Fa
 class _Scheme(NamedTuple):
     """What the chaining rules need of one integer scheme: `layer`, the convolution class whose edges they fuse; key(m),
     what decides the codes layer m reads, compared bit for bit by same(a, b) (consumers with equal keys read identical
-    codes); out(key), the producer's output argument for such a consumer (requant's first element, Epilogue.out_scale);
-    chained(m, codes_in, name, requant, epilogue, out_slice, sums), m's copy in its execution mode, sums True when a dense
-    consumer takes its codes."""
+    codes); out(key), the producer's output argument for such a consumer (requant's first element, Epilogue.out_scale).
+    Both schemes' layers take a mode as the same chained() arguments (codes_in, name, requant or epilogue, out_slice,
+    sums)."""
     layer: type
     key: object
     same: object
     out: object
-    chained: object
 
 
-_NCNN = _Scheme(Int8Conv2d, lambda m: _f32(m.act_scale), lambda a, b: a.view(np.int32) == b.view(np.int32), float,
-                lambda m, codes_in, name, requant, epilogue, out_slice, sums: m.chained(
-                    codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, out_slice=out_slice))
+_NCNN = _Scheme(Int8Conv2d, lambda m: _f32(m.act_scale), lambda a, b: a.view(np.int32) == b.view(np.int32), float)
 _AFFINE = _Scheme(AffineInt8Conv2d, lambda m: (_f32(m.act_min), _f32(m.act_max), int(m.act_bits)),
                   lambda a, b: a[0].view(np.int32) == b[0].view(np.int32) and a[1].view(np.int32) == b[1].view(np.int32)
                   and a[2] == b[2],
-                  lambda k: (float(k[0]), float(k[1]), int(k[2])),
-                  lambda m, codes_in, name, requant, epilogue, out_slice, sums: m.chained(
-                      codes_in=codes_in, name=name, requant=requant, epilogue=epilogue, sums=sums, out_slice=out_slice))
+                  lambda k: (float(k[0]), float(k[1]), int(k[2])))
 
 
 def _observed_state():
@@ -1808,18 +1829,10 @@ def _chain_edges(gm, mods, conv, scheme):
     for q in list(gm.graph.nodes):
         if not conv(q) or len(q.args) != 1 or q.kwargs or not isinstance(q.args[0], fx.Node):
             continue
-        node, clamp, path = q.args[0], (-_INF, _INF), []
-        while len(node.users) == 1:
-            if conv(node):
-                break
-            c = _pass_through(node, mods)
-            if c is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
-                break
-            clamp = _compose(c, clamp)                          # walking backwards: this clamp runs first
-            path.append(node)
-            node = node.args[0]
-        if len(node.users) != 1 or not conv(node) or mods[node.target].out_channels != mods[q.target].in_channels:
+        back = _walk_back(q.args[0], mods, conv)
+        if back is None or mods[back[0].target].out_channels != mods[q.target].in_channels:
             continue
+        node, clamp, path = back
         edges.append((node.target, q.target, clamp))
         between.append((node, q, path))
     producers = {p: c for p, _, c in edges}
@@ -1830,9 +1843,7 @@ def _chain_edges(gm, mods, conv, scheme):
             nxt = mods[next(q for p, q, _ in edges if p == target)]
             requant = (scheme.out(scheme.key(nxt)),) + tuple(producers[target])
             sums = nxt.groups == 1
-        parent, _, attr = target.rpartition(".")
-        setattr(gm.get_submodule(parent) if parent else gm, attr,
-                scheme.chained(mods[target], target in consumers, None, requant, None, None, sums))
+        _set_module(gm, target, mods[target].chained(codes_in=target in consumers, requant=requant, sums=sums))
     for p, q, path in between:
         q.args = (p,)
         for node in path:                                       # from the consumer side back: each has no user left
@@ -1841,6 +1852,38 @@ def _chain_edges(gm, mods, conv, scheme):
     gm.recompile()
     gm.requantized_edges = edges
     return gm
+
+
+@dataclasses.dataclass
+class _Plan:
+    """One producer's rewrite in _chain_residual: producer p, its single-user pass-throughs `path` (clamp `pre`) to the
+    node `tail` whose users `codes` take its codes at key `scale`; with a fused add `add`, residual argument index ri, the
+    pass-throughs after the add `post_path` (clamp `post`); the fused operand's and the residual's observers obs / robs
+    (`output`: obs is on the fp32 output instead); the residual's skipped identities and its node's name r_name."""
+    p: fx.Node
+    path: list
+    pre: tuple
+    tail: fx.Node
+    codes: list = dataclasses.field(default_factory=list)
+    scale: object = None
+    add: Optional[fx.Node] = None
+    ri: Optional[int] = None
+    post: tuple = (-_INF, _INF)
+    post_path: list = dataclasses.field(default_factory=list)
+    obs: Optional[fx.Node] = None
+    robs: Optional[fx.Node] = None
+    output: bool = False
+    skipped: list = dataclasses.field(default_factory=list)
+    r_name: Optional[str] = None
+
+
+def _split(g, node):
+    """(codes, fp32): getitem nodes inserted after `node`, a call that returns both."""
+    with g.inserting_after(node):
+        y = g.call_function(operator.getitem, (node, 1))
+    with g.inserting_after(node):
+        codes = g.call_function(operator.getitem, (node, 0))
+    return codes, y
 
 
 def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None):
@@ -1856,21 +1899,22 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     def producer(node):
         return conv(node) and len(node.args) == 1 and not node.kwargs and isinstance(node.args[0], fx.Node)
 
-    def forward(node, clamp):
-        """Walk from node through single-user pass-throughs: (last node, composed clamp, the pass-throughs)."""
-        path = []
+    def forward(node, step=lambda u: _pass_through(u, mods)):
+        """Walk from node through its single users u of one fx input for which step(u) is a clamp (by default the
+        pass-throughs): (last node, composed clamp, the nodes walked)."""
+        clamp, path = full, []
         while len(node.users) == 1:
             u = next(iter(node.users))
-            c = _pass_through(u, mods)
+            c = step(u)
             if c is None or len(u.all_input_nodes) != 1 or u.args[0] is not node:
                 break
             clamp, node = _compose(clamp, c), u
             path.append(u)
         return node, clamp, path
 
-    def data_users(node, queries):
-        """node's users, without those that only read its shape when `queries`."""
-        return [u for u in node.users if not (queries and _shape_query(u, node))]
+    def identity(u):
+        """The step of the walk after a pool: exact identities, no clamp."""
+        return full if _is_identity(u, mods) else None
 
     def observe(node):
         """node calls a QuantMeasure the affine epilogue runs (_observer_key) and has one user."""
@@ -1879,19 +1923,10 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     def unobserved(node):
         return node.args[0] if observe(node) else node
 
-    def back_to_producer(node, queries=False):
-        """The producer whose single-user pass-through chain ends at `node`, or None.  queries: users that only read a
-        node's shape do not count."""
-        while len(data_users(node, queries)) == 1 and not producer(node):
-            if _pass_through(node, mods) is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
-                return None
-            node = node.args[0]
-        return node if len(data_users(node, queries)) == 1 and producer(node) else None
-
     same = scheme.same
 
     # bilinear upsamples: the producer whose single-user pass-through chain ends at the upsample's input
-    ends = {forward(p, full)[0]: p for p in gm.graph.nodes if producer(p)} if upsample else {}
+    ends = {forward(p)[0]: p for p in gm.graph.nodes if producer(p)} if upsample else {}
 
     sources = {}
 
@@ -1905,32 +1940,13 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             sources[node] = ends.get(src) if ends and _bilinear_upsample(node, mods, affine) is not None else None
         return sources[node]
 
-    def back_to_upsample(node):
-        """The fusable upsample whose single-user pass-through chain ends at `node` (shape queries not counted), or None."""
-        while len(data_users(node, True)) == 1 and up_source(node) is None:
-            if _pass_through(node, mods) is None or len(node.all_input_nodes) != 1 or not isinstance(node.args[0], fx.Node):
-                return None
-            node = node.args[0]
-        return node if len(data_users(node, True)) == 1 and up_source(node) is not None else None
-
-    def after_pool(node):
-        """Walk from a pool through single-user exact identities: (last node, the identities)."""
-        path = []
-        while len(node.users) == 1:
-            u = next(iter(node.users))
-            if not _is_identity(u, mods) or len(u.all_input_nodes) != 1 or u.args[0] is not node:
-                break
-            node = u
-            path.append(u)
-        return node, path
-
     pool_memo = {}
 
     def pool_scale(pool, channels):
         """The scale at which every user of a pool (past exact identities) takes codes, or None."""
         if pool not in pool_memo:
             pool_memo[pool] = None
-            tail, _ = after_pool(pool)
+            tail = forward(pool, identity)[0]
             scales = [user_scale(u, tail, channels) for u in tail.users]
             if scales and all(s is not None and same(s, scales[0]) for s in scales):
                 pool_memo[pool] = scales[0]
@@ -1957,7 +1973,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     pool_plans = []
 
     def codes_pool(u, channels, clamp):
-        tail, ids = after_pool(u)
+        tail, _, ids = forward(u, identity)
         pool_plans.append(dict(node=u, mode="codes", tail=tail, path=ids, codes=sorted(tail.users, key=order.get),
                                scale=pool_scale(u, channels), clamp=clamp, channels=channels))
         for v in tail.users:
@@ -1968,7 +1984,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     for p in list(gm.graph.nodes):
         if not producer(p):
             continue
-        end, pre, path = forward(p, full)
+        end, pre, path = forward(p)
         add, ri, post, post_path, tail = None, None, full, [], end
         fobs = robs = None
         if len(end.users) == 1:
@@ -1976,10 +1992,11 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             if observe(a):                                      # the observer on the fused operand (replace_op's add)
                 fobs, a = a, next(iter(a.users))
             if _is_add(a):
-                fused = next((i for i, v in enumerate(a.args) if back_to_producer(unobserved(v)) is not None), None)
+                fused = next((i for i, v in enumerate(a.args) if _walk_back(unobserved(v), mods, producer) is not None),
+                             None)
                 if fused is not None and unobserved(a.args[fused]) is end and (fobs is None or a.args[fused] is fobs):
                     add, ri = a, 1 - fused
-                    tail, post, post_path = forward(a, full)
+                    tail, post, post_path = forward(a)
                     robs = a.args[ri] if observe(a.args[ri]) else None
             if add is None:
                 fobs = None
@@ -1991,14 +2008,13 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             if _max_pool(u, mods) is not None and u.args[0] is tail:
                 pc, ps = take_codes(u, out_c, pools=False)
                 if pc:
-                    pool_plans.append(dict(node=u, mode="fp32", codes=pc, scale=ps, clamp=clamp, channels=out_c))
-                    plans.append(dict(p=p, path=path, pre=pre, add=None, ri=None, post=full, post_path=[], tail=tail,
-                                      codes=[], scale=None))
+                    pool_plans.append(dict(node=u, mode="fp32", path=[], codes=pc, scale=ps, clamp=clamp, channels=out_c))
+                    plans.append(_Plan(p, path, pre, tail))
             continue
         if add is None and not codes:
             continue
-        plans.append(dict(p=p, path=path, pre=pre, add=add, ri=ri, post=post, post_path=post_path, tail=tail, codes=codes,
-                          scale=scale, obs=fobs, robs=robs))
+        plans.append(_Plan(p, path, pre, tail, codes, scale, add=add, ri=ri, post=post, post_path=post_path, obs=fobs,
+                           robs=robs))
         for u in codes:
             if not producer(u):
                 codes_pool(u, out_c, clamp)
@@ -2012,23 +2028,19 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         # under the affine scheme an operand may end in its replayed observer, which the operand's writer applies
         oobs = [o if affine and observe(o) else None for o in ops]
         ops = [o.args[0] if ob is not None else o for o, ob in zip(ops, oobs)]
-        prods = [back_to_producer(o, upsample) or (back_to_upsample(o) if upsample else None) for o in ops]
-        if any(q is None for q in prods) or len(set(prods)) != len(prods):
+        backs = [_walk_back(o, mods, producer, upsample) or
+                 (_walk_back(o, mods, lambda n: up_source(n) is not None, True) if upsample else None) for o in ops]
+        if any(b is None for b in backs) or len({b[0] for b in backs}) != len(backs):
             continue
-        chans = [mods[(up_source(q) or q).target].out_channels for q in prods]
+        chans = [mods[(up_source(q) or q).target].out_channels for q, _, _ in backs]
         if any(k % 16 for k in chans[:-1]):
             continue
-        tail, tclamp, tpath = forward(c, full)
+        tail, tclamp, tpath = forward(c)
         codes, scale = take_codes(tail, sum(chans))
         if not codes or len(codes) != len(tail.users):
             continue
         operands = []
-        for o, ob, q, k, off in zip(ops, oobs, prods, chans, np.cumsum([0] + chans[:-1]).tolist()):
-            node, clamp, opath = o, full, []
-            while node is not q:
-                clamp = _compose(_pass_through(node, mods), clamp)
-                opath.append(node)
-                node = node.args[0]
+        for ob, (q, clamp, opath), k, off in zip(oobs, backs, chans, np.cumsum([0] + chans[:-1]).tolist()):
             queries = [(u, n) for n in (q, *opath) for u in n.users if upsample and _shape_query(u, n)]
             operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), pre=clamp, obs=ob, coff=off, channels=k,
                                  queries=queries))
@@ -2040,117 +2052,105 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
 
     # observers on a producer's fp32 output: its single-user pass-through chain, then shape-only views, then the observer
     # (shape queries not counted as users); the producer applies it in its epilogue and writes the observed fp32 output
-    taken = {n for pl in plans for n in (pl.get("obs"), pl.get("robs")) if n is not None}
+    taken = {n for pl in plans for n in (pl.obs, pl.robs) if n is not None}
     taken |= {o["obs"] for cp in cat_plans for o in cp["operands"] if o["obs"] is not None}
-    planned = {pl["p"] for pl in plans}
+    planned = {pl.p for pl in plans}
     for o in (list(gm.graph.nodes) if scheme is _AFFINE else []):
         if o in taken or _observer_key(o, mods) is None:
             continue
         node = o.args[0]
-        while _is_view(node) and len(data_users(node, True)) == 1:
+        while _is_view(node) and len(_data_users(node, True)) == 1:
             node = node.args[0]
-        q = back_to_producer(node, queries=True)
-        if q is None or q in planned:
+        back = _walk_back(node, mods, producer, queries=True)
+        if back is None or back[0] in planned:
             continue
-        path, clamp, n = [], full, node
-        while n is not q:
-            clamp = _compose(_pass_through(n, mods), clamp)
-            path.append(n)
-            n = n.args[0]
-        plans.append(dict(p=q, path=path[::-1], pre=clamp, add=None, ri=None, post=full, post_path=[], tail=node, codes=[],
-                          scale=None, obs=o, robs=None, output=True))
+        q, clamp, path = back
+        plans.append(_Plan(q, path[::-1], clamp, node, obs=o, output=True))
         planned.add(q)
 
     # upsamples: slice mode through a fused concatenation above, codes mode when every user takes codes at one scale;
     # either way the producer writes its clamped fp32 output
-    up_plans = [dict(node=o["p"], mode="slice") for cp in cat_plans for o in cp["operands"] if not producer(o["p"])]
+    up_plans = [dict(node=o["p"], mode="slice", path=[]) for cp in cat_plans for o in cp["operands"] if not producer(o["p"])]
     sliced = {up["node"] for up in up_plans}
     for u in (list(gm.graph.nodes) if upsample and not affine else []):
         if u in sliced or up_source(u) is None:
             continue
-        utail, uclamp, upath = forward(u, full)
+        utail, uclamp, upath = forward(u)
         codes, scale = take_codes(utail, mods[up_source(u).target].out_channels, pools=False)
         if codes and len(codes) == len(utail.users):
             up_plans.append(dict(node=u, mode="codes", tail=utail, clamp=uclamp, path=upath, codes=codes, scale=scale))
-    planned = {pl["p"] for pl in plans}
+    planned = {pl.p for pl in plans}
     for up in up_plans:
         p = up_source(up["node"])
         if p not in planned:
-            end, pre, path = forward(p, full)
-            plans.append(dict(p=p, path=path, pre=pre, add=None, ri=None, post=full, post_path=[], tail=end, codes=[],
-                              scale=None))
+            end, pre, path = forward(p)
+            plans.append(_Plan(p, path, pre, end))
             planned.add(p)
-    plans.sort(key=lambda pl: order[pl["p"]])
+    plans.sort(key=lambda pl: order[pl.p])
 
     # the residual's exact identities, skipped once every plan's own nodes are known: a node another plan deletes (an
     # identity at the end of its post-add chain, say) stays the residual, and that plan replaces it by its fp32 output
-    claimed = {n for pl in plans for n in (pl["p"], *pl["path"], *([pl["add"]] if pl["add"] is not None else []),
-                                            *pl["post_path"])}
+    claimed = {n for pl in plans for n in (pl.p, *pl.path, *([pl.add] if pl.add is not None else []), *pl.post_path)}
     claimed |= {n for cp in cat_plans for n in (cp["cat"], *cp["path"], *(n for o in cp["operands"] for n in (o["p"], *o["path"])))}
-    claimed |= {n for pp in pool_plans for n in (pp["node"], *pp.get("path", []))}
-    claimed |= {n for up in up_plans for n in (up["node"], *up.get("path", []))}
+    claimed |= {n for pp in pool_plans for n in (pp["node"], *pp["path"])}
+    claimed |= {n for up in up_plans for n in (up["node"], *up["path"])}
     for pl in plans:
-        pl["skipped"] = []
-        if pl["add"] is None:
+        if pl.add is None:
             continue
-        r = pl["robs"].args[0] if pl.get("robs") is not None else pl["add"].args[pl["ri"]]
+        r = pl.robs.args[0] if pl.robs is not None else pl.add.args[pl.ri]
         while r not in claimed and len(r.users) == 1 and _is_identity(r, mods) and isinstance(r.args[0], fx.Node):
-            pl["skipped"].append(r)
+            pl.skipped.append(r)
             r = r.args[0]
-        pl["r_name"] = r.name
+        pl.r_name = r.name
 
     # rewrite in producer order: a producer's input may be the codes of an earlier one, and a residual its fp32 output
     g = gm.graph
     convs = {n for n in g.nodes if producer(n)}                 # before the rewrites give producers a second input
     edges, adds, modes, observed, watched = [], [], {}, [], {}
     for pl in plans:
-        p, add, tail = pl["p"], pl["add"], pl["tail"]
-        fobs, robs = pl.get("obs"), pl.get("robs")
+        p, add, tail, fobs, robs = pl.p, pl.add, pl.tail, pl.obs, pl.robs
         if add is not None:
-            for node in pl["skipped"]:                          # from the add back: each loses its only user
+            for node in pl.skipped:                             # from the add back: each loses its only user
                 node.replace_all_uses_with(node.args[0])
                 g.erase_node(node)
             add.prepend(p)
-            p.args = (p.args[0], robs.args[0] if robs is not None else add.args[pl["ri"]])
-        fp32 = any(u not in pl["codes"] for u in tail.users)
-        scale = scheme.out(pl["scale"]) if pl["codes"] else None
-        clamp = pl["post"] if add is not None else pl["pre"]
+            p.args = (p.args[0], robs.args[0] if robs is not None else add.args[pl.ri])
+        fp32 = any(u not in pl.codes for u in tail.users)
+        scale = scheme.out(pl.scale) if pl.codes else None
+        clamp = pl.post if add is not None else pl.pre
         keys = tuple(None if o is None else _observer_key(o, mods) for o in (fobs, robs))
         if add is None and not fp32:
-            modes[p.target] = ("requant", (scale,) + tuple(clamp))
+            modes[p.target] = ("requant", (scale,) + tuple(clamp), None)
             codes_node = y_node = p
         else:
-            modes[p.target] = ("epilogue", Epilogue(scale, pl["pre"], pl["post"], add is not None, fp32))
+            modes[p.target] = ("epilogue", Epilogue(scale, pl.pre, pl.post, add is not None, fp32), None)
             if keys != (None, None):
                 watched[p.target] = keys
             codes_node = y_node = p
             if scale is not None and fp32:
-                with g.inserting_after(p):
-                    y_node = g.call_function(operator.getitem, (p, 1))
-                with g.inserting_after(p):
-                    codes_node = g.call_function(operator.getitem, (p, 0))
-        for u in pl["codes"]:
+                codes_node, y_node = _split(g, p)
+        for u in pl.codes:
             u.replace_input_with(tail, codes_node)
             if u in convs:
                 edges.append((p.target, u.target, clamp))
-        for node in pl["path"]:                                 # shape queries inside the chain read p's output
+        for node in pl.path:                                    # shape queries inside the chain read p's output
             for u in [u for u in node.users if _shape_query(u, node)]:
                 u.replace_input_with(node, y_node)
         if tail is not p:
             tail.replace_all_uses_with(y_node)
             on_add = [o for o in (fobs, robs) if o is not None and add is not None]
-            for node in reversed([*pl["path"], *on_add, *([add] if add is not None else []), *pl["post_path"]]):
+            for node in reversed([*pl.path, *on_add, *([add] if add is not None else []), *pl.post_path]):
                 g.erase_node(node)
         else:
             p.replace_all_uses_with(y_node, delete_user_cb=lambda u: u not in (y_node, codes_node))
-        if pl.get("output"):                                    # the views now read the observed output
+        if pl.output:                                           # the views now read the observed output
             fobs.replace_all_uses_with(fobs.args[0])
             g.erase_node(fobs)
             observed.append((fobs.target, "output", p.target))
         elif add is not None:
             observed += [(o.target, what, p.target) for o, what in ((fobs, "operand"), (robs, "residual")) if o is not None]
         if add is not None:
-            adds.append((p.target, add.name, pl["r_name"], pl["pre"], pl["post"]))
+            adds.append((p.target, add.name, pl.r_name, pl.pre, pl.post))
 
     def fuse_upsample(u, scale, clamp, out_slice=None, out=None, operand=None, sums=False):
         """Turn the upsample node u into a call of its Int8UpsampleBilinear, on its (rewritten) input; under the affine
@@ -2182,13 +2182,13 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
                 prev = q
                 continue
             if affine:                                          # operand clamp, its observer, the tail's clamp
-                modes[q.target] = ("slice", (Epilogue(scheme.out(cp["scale"]), o["pre"], cp["clamp"]), (o["coff"], cstride)))
+                modes[q.target] = ("epilogue", Epilogue(scheme.out(cp["scale"]), o["pre"], cp["clamp"]), (o["coff"], cstride))
                 if o["obs"] is not None:
                     watched[q.target] = (_observer_key(o["obs"], mods), None)
                 if cp["sums"]:
                     slice_sums.add(q.target)
             else:
-                modes[q.target] = ("slice", ((float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride)))
+                modes[q.target] = ("requant", (float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride))
             if prev is not None:
                 q.kwargs = {"out": prev}
             prev = q
@@ -2242,10 +2242,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
             for node in reversed(pp["path"]):
                 g.erase_node(node)
         else:
-            with g.inserting_after(u):
-                y_node = g.call_function(operator.getitem, (u, 1))
-            with g.inserting_after(u):
-                codes_node = g.call_function(operator.getitem, (u, 0))
+            codes_node, y_node = _split(g, u)
             for v in pp["codes"]:
                 v.replace_input_with(u, codes_node)
             u.replace_all_uses_with(y_node, delete_user_cb=lambda x: x not in (y_node, codes_node))
@@ -2257,14 +2254,11 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
     consumers = {q for _, q, _ in edges}
     dense = {p for p, q, _ in edges if mods[q].groups == 1}          # producers whose codes a dense consumer reads
     for target in modes.keys() | consumers:
-        kind, arg = modes.get(target, (None, None))
-        parent, _, attr = target.rpartition(".")
-        sliced_epi = kind == "slice" and isinstance(arg[0], Epilogue)          # an affine slice: both clamps
-        mod = scheme.chained(mods[target], target in consumers, target,
-                             arg if kind == "requant" else (arg[0] if kind == "slice" and not sliced_epi else None),
-                             arg if kind == "epilogue" else (arg[0] if sliced_epi else None),
-                             arg[1] if kind == "slice" else None, target in dense or target in slice_sums)
-        setattr(gm.get_submodule(parent) if parent else gm, attr, mod.observe(*watched[target]) if target in watched else mod)
+        kind, arg, out_slice = modes.get(target, (None, None, None))
+        mod = mods[target].chained(codes_in=target in consumers, name=target, requant=arg if kind == "requant" else None,
+                                   epilogue=arg if kind == "epilogue" else None, out_slice=out_slice,
+                                   sums=target in dense or target in slice_sums)
+        _set_module(gm, target, mod.observe(*watched[target]) if target in watched else mod)
     g.lint()
     gm.recompile()
     gm.requantized_edges = edges
