@@ -115,6 +115,11 @@ I8_AFFINE_RESIZE_DT = np.dtype([(f, np.int32) for f in ("N", "C", "H", "W", "OH"
                                 ("post_hi", np.float32), ("out_min", np.float32), ("out_max", np.float32),
                                 ("out_bits", np.int32)], align=True)
 
+I8_AFFINE_ROWS_DT = np.dtype([("y", np.uint64), ("off", np.int64), ("img_stride", np.int64)] +
+                             [(f, np.float32) for f in ("pre_lo", "pre_hi", "post_lo", "post_hi", "obs_min", "obs_max")] +
+                             [("obs_bits", np.int32), ("tail_min", np.float32), ("tail_max", np.float32),
+                              ("tail_bits", np.int32)], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -123,7 +128,7 @@ EXPECTED_SIZES = {
     "DfqI8Epilogue": (I8_EPILOGUE_DT, 48), "DfqI8Pool": (I8_POOL_DT, 64), "DfqI8Resize": (I8_RESIZE_DT, 48),
     "DfqI8Affine": (I8_AFFINE_DT, 32), "DfqI8AffineEpilogue": (I8_AFFINE_EPILOGUE_DT, 64),
     "DfqI8AffineObserve": (I8_AFFINE_OBSERVE_DT, 24), "DfqI8AffineLayout": (I8_AFFINE_LAYOUT_DT, 20),
-    "DfqI8AffineResize": (I8_AFFINE_RESIZE_DT, 76),
+    "DfqI8AffineResize": (I8_AFFINE_RESIZE_DT, 76), "DfqI8AffineRows": (I8_AFFINE_ROWS_DT, 64),
 }
 
 _PF = C.c_void_p   # device float*
@@ -190,6 +195,9 @@ SIGNATURES = {
     "dfq_i8_affine_conv_layout": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_i8_affine_upsample_bilinear": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_affine_conv_rows": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p, C.c_void_p,
+                                _ST],
+    "dfq_i8_affine_maxpool": [C.c_void_p, _PF, _PF, C.c_void_p, C.c_void_p, C.c_float, C.c_float, _I32, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -42,6 +42,11 @@
 //                          loop reads z' (k_i8_conv_dw<..., true>).
 //   k_i8_affine_upsample   torch's bilinear upsample (k_i8_upsample_bilinear's value) through clamp, observer, clamp to the
 //                          consumer's codes in a channel slice, S added (dfq_i8_affine_upsample_bilinear)
+//   Out::AFFINE_ROWS       Out::AFFINE's value through clamp, QuantMeasure's fake quantization (either optional), clamp and a
+//                          second fake quantization, written pixel-major into a slice of a detection head's [N, R, k]
+//                          concatenation (dfq_i8_affine_conv_rows), as Out::ROWS
+//   k_i8_maxpool<., true>  k_i8_maxpool on shifted codes, or fp32 to fp32 and / or the consumer's shifted codes, with their
+//                          per-pixel sums S (dfq_i8_affine_maxpool)
 #include <algorithm>
 #include <cmath>
 
@@ -65,7 +70,7 @@ __device__ __forceinline__ float dequant(int32_t acc, float dq, float b) {
 // FUSED: Fused below.  ROWS: Rows below.
 // Both code-writing epilogues store pixel m's chunks [0, cpad) at yq + m * cstride: cstride = cpad for a tensor of its own,
 // wider for a channel slice of a concatenation (yq then points at the slice's first channel, dfq_i8_conv_slice).
-enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED, AFFINE_OBSERVED, AFFINE_LAYOUT };
+enum class Out { F32, I8, FUSED, ROWS, AFFINE, AFFINE_FUSED, AFFINE_OBSERVED, AFFINE_LAYOUT, AFFINE_ROWS };
 struct Requant {
   int8_t* yq;
   float scale, lo, hi;
@@ -135,6 +140,15 @@ struct AffineLayout : AffineObserved {
   int cstride, pad_code;
   bool pad_on;
 };
+// The affine rows epilogue (DfqI8AffineRows): Affine's value, clamp(pre), fq(obs) (obs_on), clamp(post), fq(tail)
+// (tail_on), stored as Rows stores it.
+struct AffineRows : Affine {
+  float* y;
+  int64_t off, img_stride;
+  float pre_lo, pre_hi, post_lo, post_hi;
+  QuantScalars obs, tail;
+  bool obs_on, tail_on;
+};
 template <Out OUT> struct EpiOf { using type = Requant; };
 template <> struct EpiOf<Out::FUSED> { using type = Fused; };
 template <> struct EpiOf<Out::ROWS> { using type = Rows; };
@@ -142,8 +156,10 @@ template <> struct EpiOf<Out::AFFINE> { using type = Affine; };
 template <> struct EpiOf<Out::AFFINE_FUSED> { using type = AffineFused; };
 template <> struct EpiOf<Out::AFFINE_OBSERVED> { using type = AffineObserved; };
 template <> struct EpiOf<Out::AFFINE_LAYOUT> { using type = AffineLayout; };
+template <> struct EpiOf<Out::AFFINE_ROWS> { using type = AffineRows; };
 __host__ __device__ constexpr bool affine_out(Out o) {
-  return o == Out::AFFINE || o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT;
+  return o == Out::AFFINE || o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT ||
+         o == Out::AFFINE_ROWS;
 }
 __host__ __device__ constexpr bool affine_epilogue(Out o) {
   return o == Out::AFFINE_FUSED || o == Out::AFFINE_OBSERVED || o == Out::AFFINE_LAYOUT;
@@ -206,6 +222,17 @@ __device__ __forceinline__ float observed_add(float v, int64_t idx, const Affine
 // fused_value without a residual, for the Rows epilogue
 __device__ __forceinline__ float rows_value(int32_t acc, float dq, float b, const Rows& e) {
   return clamp_keep_nan(clamp_keep_nan(dequant(acc, dq, b), e.pre_lo, e.pre_hi), e.post_lo, e.post_hi);
+}
+
+// What the per-layer path computes from the affine layer's value to a detection head's concatenation, in its order: the
+// pass-throughs, the cat operand's observer, the cat tail's pass-throughs, the observer of the cat's single user (an
+// elementwise op, so per slice)
+__device__ __forceinline__ float affine_rows_value(float v, const AffineRows& e) {
+  v = clamp_keep_nan(v, e.pre_lo, e.pre_hi);
+  if (e.obs_on) v = fake_quant<true>(v, e.obs);
+  v = clamp_keep_nan(v, e.post_lo, e.post_hi);
+  if (e.tail_on) v = fake_quant<true>(v, e.tail);
+  return v;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -483,7 +510,23 @@ __global__ void __launch_bounds__(THREADS) k_i8_conv_mma(const int8_t* __restric
         }
     __syncthreads();
     const int tw = g.kw + 1, tsize = (g.kh + 1) * tw;
-    if constexpr (OUT == Out::AFFINE) {
+    if constexpr (OUT == Out::AFFINE_ROWS) {
+      // channels fastest, so the stores run along each pixel's row of the pixel-major output
+      for (int e = tid; e < BM * BN; e += THREADS) {
+        const int ol = e % BN, ml = e / BN;
+        const int64_t m = m0 + ml;
+        const int o = o0 + ol;
+        if (m >= M || o >= g.O) continue;
+        const int32_t P = st[ol * EPI_LD + ml];
+        const uint32_t rh = sR[2 * ml], rw = sR[2 * ml + 1];
+        const int r0 = rh & 0xffff, r1 = rh >> 16, s0 = rw & 0xffff, s1 = rw >> 16;
+        const int32_t* T = rq.table + (int64_t)o * tsize;
+        const int32_t Wv = T[r1 * tw + s1] - T[r0 * tw + s1] - T[r1 * tw + s0] + T[r0 * tw + s0];
+        const float v = affine_value(P, sA[ml], Wv, (r1 - r0) * (s1 - s0) * g.C, bias ? bias[o] : 0.f, rq);
+        rq.y[(m / OHW) * rq.img_stride + rq.off + (m % OHW) * g.O + o] = affine_rows_value(v, rq);
+      }
+      return;
+    } else if constexpr (OUT == Out::AFFINE) {
       for (int e = tid; e < BM * BN; e += THREADS) {
         const int ml = e % BM, ol = e / BM;
         const int64_t m = m0 + ml;
@@ -767,6 +810,15 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
         }
       }
     }
+    if constexpr (OUT == Out::AFFINE_ROWS) {                    // this pixel's 16 channels of its row
+      float* row = rq.y + n * rq.img_stride + rq.off + (int64_t)p * g.C + ch * 16;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = ch * 16 + j;
+        if (c < g.C) row[j] = affine_rows_value(affine_value(acc[j], xsum[j], wsum[j], ntaps, bias ? bias[c] : 0.f, rq), rq);
+      }
+      continue;
+    }
     if constexpr (OUT == Out::AFFINE) {
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -860,12 +912,22 @@ __global__ void k_i8_conv_dw(const int8_t* __restrict__ xq, const int8_t* __rest
 // ------------------------------------------------------------------------------------------------------------------
 // CODES: xq int8 NHWC [N, H, W, Cpad] -> yq int8 NHWC [N, OH, OW, Cpad], a byte-wise signed max of 16-byte taps.  q8() is
 // monotone non-decreasing for a scale >= 0, so the max of the codes is the code of the max for any window without NaN.
-// A window with no tap inside the input (possible with dilation) is -inf in torch, whose code is -127; pad channels 0.
+// A window with no tap inside the input (possible with dilation) is -inf in torch, whose code is -127 (AFFINE: -128, below);
+// pad channels 0.
 // !CODES: x fp32 NCHW [N, C, H, W] -> y fp32 NCHW [N, C, OH, OW] and / or yq int8 NHWC at `scale`, with torch's CUDA rule:
 // from -inf, taps row-major, the running max replaced when v > m or v is NaN (so the first of tied values is kept).
-template <bool CODES>
+// AFFINE (dfq_i8_affine_maxpool): the codes are the affine scheme's shifted codes, in [-128, 127].  affine_code is monotone
+// non-decreasing too (a positive inv_scale), the empty window's -inf has code -128, the !CODES codes are the consumer's
+// (a.neg_min, a.inv_scale, a.qmax) and, with a.S, S[n, p] += the sum of the pooled codes over the real channels.
+struct AffinePool {
+  int32_t* S;
+  float neg_min, inv_scale, qmax;
+};
+
+template <bool CODES, bool AFFINE = false>
 __global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restrict__ x, float* __restrict__ y,
-                             int8_t* __restrict__ yq, float scale, DfqI8Pool g, int64_t total) {
+                             int8_t* __restrict__ yq, float scale, DfqI8Pool g, int64_t total, AffinePool a) {
+  constexpr int lowest = AFFINE ? (int)0x80808080 : (int)0x81818181;   // the smallest code in every byte
   const int chunks = g.Cpad / 16, OHW = g.OH * g.OW;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int p = (int)(i % OHW);
@@ -876,7 +938,7 @@ __global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restr
     alignas(16) int8_t v[16];
     if constexpr (CODES) {
       const int8_t* img = xq + n * g.H * g.W * g.Cpad + ch * 16;
-      int m[4] = {(int)0x81818181, (int)0x81818181, (int)0x81818181, (int)0x81818181};
+      int m[4] = {lowest, lowest, lowest, lowest};
       bool any = false;
       for (int r = 0; r < g.kh; ++r) {
         const int ih = h0 + r * g.dil_h;
@@ -892,7 +954,7 @@ __global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restr
       *reinterpret_cast<int4*>(v) = make_int4(m[0], m[1], m[2], m[3]);
       if (!any) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = ch * 16 + j < g.C ? (int8_t)-127 : (int8_t)0;
+        for (int j = 0; j < 16; ++j) v[j] = ch * 16 + j < g.C ? (int8_t)lowest : (int8_t)0;
       }
     } else {
 #pragma unroll 1
@@ -913,9 +975,21 @@ __global__ void k_i8_maxpool(const int8_t* __restrict__ xq, const float* __restr
           }
         }
         if (y) y[(n * g.C + c) * OHW + p] = mx;
-        v[j] = q8(mx, scale);
+        if constexpr (AFFINE) {
+          if (yq) v[j] = affine_code(mx, a.neg_min, a.inv_scale, a.qmax);
+        } else {
+          v[j] = q8(mx, scale);
+        }
       }
       if (!yq) continue;
+    }
+    if constexpr (AFFINE) {
+      if (a.S) {
+        int32_t sum = 0;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) sum += ch * 16 + j < g.C ? v[j] : 0;
+        atomicAdd(a.S + n * OHW + p, sum);
+      }
     }
     *reinterpret_cast<int4*>(yq + (n * OHW + p) * g.Cpad + ch * 16) = *reinterpret_cast<const int4*>(v);
   }
@@ -1113,6 +1187,26 @@ int check_slice(const char* who, int64_t coff, int64_t cstride, int cpad, char c
   return 0;
 }
 
+// A max pool's geometry: torch's max_pool2d (padding at most half the kernel, OH / OW as torch forms them) on codes of
+// Cpad channels; exactly one input, codes xq or fp32 x
+int check_pool(const char* who, const DfqI8Pool* g, const void* xq, const void* x) {
+  DFQ_REQUIRE_WHO(g != nullptr, "null geometry");
+  DFQ_REQUIRE_WHO(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->kh > 0 && g->kw > 0, "empty dimension");
+  DFQ_REQUIRE_WHO(g->stride_h > 0 && g->stride_w > 0 && g->dil_h > 0 && g->dil_w > 0 && g->pad_h >= 0 && g->pad_w >= 0 &&
+                      (g->ceil_mode == 0 || g->ceil_mode == 1),
+                  "bad stride / padding / dilation / ceil_mode");
+  DFQ_REQUIRE_WHO(g->pad_h <= g->kh / 2 && g->pad_w <= g->kw / 2 && g->pad_h <= (g->dil_h * (g->kh - 1) + 1) / 2 &&
+                      g->pad_w <= (g->dil_w * (g->kw - 1) + 1) / 2,
+                  "padding must be at most half of the kernel and of the effective kernel");
+  DFQ_REQUIRE_WHO(g->Cpad >= g->C && g->Cpad % 16 == 0, "Cpad must be a multiple of 16 that holds C");
+  DFQ_REQUIRE_WHO(g->OH == pool_extent(g->H, g->kh, g->pad_h, g->stride_h, g->dil_h, g->ceil_mode) &&
+                      g->OW == pool_extent(g->W, g->kw, g->pad_w, g->stride_w, g->dil_w, g->ceil_mode) && g->OH > 0 &&
+                      g->OW > 0,
+                  "OH / OW do not follow from the geometry");
+  DFQ_REQUIRE_WHO((xq != nullptr) != (x != nullptr), "give exactly one input, codes xq or fp32 x");
+  return 0;
+}
+
 }  // namespace
 }  // namespace dfq
 
@@ -1242,19 +1336,7 @@ extern "C" int dfq_i8_conv_nhwc(const int8_t* xq, const int8_t* wq, const float*
 
 extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, float out_scale, const DfqI8Pool* g,
                               void* stream) {
-  DFQ_REQUIRE(g != nullptr, "dfq_i8_maxpool: null geometry");
-  DFQ_REQUIRE(g->N > 0 && g->C > 0 && g->H > 0 && g->W > 0 && g->kh > 0 && g->kw > 0, "dfq_i8_maxpool: empty dimension");
-  DFQ_REQUIRE(g->stride_h > 0 && g->stride_w > 0 && g->dil_h > 0 && g->dil_w > 0 && g->pad_h >= 0 && g->pad_w >= 0 &&
-                  (g->ceil_mode == 0 || g->ceil_mode == 1),
-              "dfq_i8_maxpool: bad stride / padding / dilation / ceil_mode");
-  DFQ_REQUIRE(g->pad_h <= g->kh / 2 && g->pad_w <= g->kw / 2 && g->pad_h <= (g->dil_h * (g->kh - 1) + 1) / 2 &&
-                  g->pad_w <= (g->dil_w * (g->kw - 1) + 1) / 2,
-              "dfq_i8_maxpool: padding must be at most half of the kernel and of the effective kernel");
-  DFQ_REQUIRE(g->Cpad >= g->C && g->Cpad % 16 == 0, "dfq_i8_maxpool: Cpad must be a multiple of 16 that holds C");
-  DFQ_REQUIRE(g->OH == pool_extent(g->H, g->kh, g->pad_h, g->stride_h, g->dil_h, g->ceil_mode) &&
-                  g->OW == pool_extent(g->W, g->kw, g->pad_w, g->stride_w, g->dil_w, g->ceil_mode) && g->OH > 0 && g->OW > 0,
-              "dfq_i8_maxpool: OH / OW do not follow from the geometry");
-  DFQ_REQUIRE((xq != nullptr) != (x != nullptr), "dfq_i8_maxpool: give exactly one input, codes xq or fp32 x");
+  if (int rc = check_pool("dfq_i8_maxpool", g, xq, x)) return rc;
   const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
   const int64_t total = out_px * (g->Cpad / 16);
   cudaStream_t st = (cudaStream_t)stream;
@@ -1262,7 +1344,7 @@ extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t
     DFQ_REQUIRE(yq && !y, "dfq_i8_maxpool: codes in give codes out only (yq, no y)");
     DFQ_REQUIRE(aligned16(xq) && aligned16(yq), "dfq_i8_maxpool: xq and yq must be 16-byte aligned");
     DFQ_REQUIRE(!overlap(xq, in_px * g->Cpad, yq, out_px * g->Cpad), "dfq_i8_maxpool: yq overlaps xq");
-    k_i8_maxpool<true><<<grid_for(total, 256), 256, 0, st>>>(xq, nullptr, nullptr, yq, 0.f, *g, total);
+    k_i8_maxpool<true><<<grid_for(total, 256), 256, 0, st>>>(xq, nullptr, nullptr, yq, 0.f, *g, total, AffinePool{});
   } else {
     DFQ_REQUIRE(y || yq, "dfq_i8_maxpool: no output requested (y and yq are both NULL)");
     DFQ_REQUIRE(aligned16(yq), "dfq_i8_maxpool: yq must be 16-byte aligned");
@@ -1272,7 +1354,7 @@ extern "C" int dfq_i8_maxpool(const int8_t* xq, const float* x, float* y, int8_t
     const int64_t x_bytes = in_px * g->C * 4, y_bytes = out_px * g->C * 4, yq_bytes = out_px * g->Cpad;
     DFQ_REQUIRE(!overlap(x, x_bytes, y, y_bytes) && !overlap(x, x_bytes, yq, yq_bytes) && !overlap(y, y_bytes, yq, yq_bytes),
                 "dfq_i8_maxpool: x, y and yq overlap");
-    k_i8_maxpool<false><<<grid_for(total, 256), 256, 0, st>>>(nullptr, x, y, yq, out_scale, *g, total);
+    k_i8_maxpool<false><<<grid_for(total, 256), 256, 0, st>>>(nullptr, x, y, yq, out_scale, *g, total, AffinePool{});
   }
   DFQ_CUDA(cudaGetLastError());
   return 0;
@@ -1559,4 +1641,69 @@ extern "C" int dfq_i8_affine_upsample_bilinear(const float* x, int8_t* yq, int32
       x, yq, S, *g, a, bilinear_scale(g->H, g->OH, ac), bilinear_scale(g->W, g->OW, ac), total);
   DFQ_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int dfq_i8_affine_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, int32_t* S, float out_min,
+                                     float out_max, int32_t out_bits, const DfqI8Pool* g, void* stream) {
+  const char* who = "dfq_i8_affine_maxpool";
+  if (int rc = check_pool(who, g, xq, x)) return rc;
+  DFQ_REQUIRE_WHO(!S || yq, "S is the sum of the codes; it needs yq");
+  DFQ_REQUIRE_WHO(((uintptr_t)S & 3) == 0, "S must be 4-byte aligned");
+  const int64_t in_px = (int64_t)g->N * g->H * g->W, out_px = (int64_t)g->N * g->OH * g->OW;
+  const int64_t yq_bytes = out_px * g->Cpad, s_bytes = out_px * 4;
+  AffinePool a{S, 0.f, 0.f, 0.f};
+  if (xq) {
+    DFQ_REQUIRE_WHO(yq && !y, "codes in give codes out only (yq, no y)");
+    DFQ_REQUIRE_WHO(aligned16(xq) && aligned16(yq), "xq and yq must be 16-byte aligned");
+    const int64_t xq_bytes = in_px * g->Cpad;
+    DFQ_REQUIRE_WHO(!overlap(xq, xq_bytes, yq, yq_bytes) && !overlap(xq, xq_bytes, S, s_bytes) &&
+                        !overlap(yq, yq_bytes, S, s_bytes),
+                    "xq, yq and S overlap");
+  } else {
+    DFQ_REQUIRE_WHO(y || yq, "no output requested (y and yq are both NULL)");
+    DFQ_REQUIRE_WHO(aligned16(yq), "yq must be 16-byte aligned");
+    DFQ_REQUIRE_WHO(((uintptr_t)x & 3) == 0 && ((uintptr_t)y & 3) == 0, "x and y must be 4-byte aligned");
+    if (yq) {                                                   // the consumer's quantizer, as dfq_i8_affine_quantize
+      QuantScalars qs;
+      if (int rc = quantizer(who, "out_bits", "the output range", out_min, out_max, out_bits, &qs)) return rc;
+      a.neg_min = qs.neg_min, a.inv_scale = qs.inv_scale, a.qmax = qs.qmax;
+    }
+    const int64_t x_bytes = in_px * g->C * 4, y_bytes = out_px * g->C * 4;
+    DFQ_REQUIRE_WHO(!overlap(x, x_bytes, y, y_bytes) && !overlap(x, x_bytes, yq, yq_bytes) &&
+                        !overlap(x, x_bytes, S, s_bytes) && !overlap(y, y_bytes, yq, yq_bytes) &&
+                        !overlap(y, y_bytes, S, s_bytes) && !overlap(yq, yq_bytes, S, s_bytes),
+                    "x, y, yq and S overlap");
+  }
+  const int64_t total = out_px * (g->Cpad / 16);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (S) DFQ_CUDA(cudaMemsetAsync(S, 0, s_bytes, st));       // the chunks of a pixel add their sums
+  if (xq) k_i8_maxpool<true, true><<<grid_for(total, 256), 256, 0, st>>>(xq, nullptr, nullptr, yq, 0.f, *g, total, a);
+  else k_i8_maxpool<false, true><<<grid_for(total, 256), 256, 0, st>>>(nullptr, x, y, yq, 0.f, *g, total, a);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_affine_conv_rows(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                                       const DfqI8Affine* k, const float* bias, const DfqI8AffineRows* r, const DfqI8Conv* g,
+                                       void* stream) {
+  const char* who = "dfq_i8_affine_conv_rows";
+  if (int rc = check_affine_conv(who, g, xq, S_in, wq, table, k, r)) return rc;
+  DFQ_REQUIRE_WHO(r->y, "no output (y is NULL)");
+  DFQ_REQUIRE_WHO(((uintptr_t)r->y & 3) == 0, "y must be 4-byte aligned");
+  DFQ_REQUIRE_WHO(ordered(r->pre_lo, r->pre_hi) && ordered(r->post_lo, r->post_hi),
+                  "pre / post clamp bounds must be ordered and not NaN");
+  const int64_t extent = (int64_t)g->OH * g->OW * g->O;                // floats of one image's rows
+  DFQ_REQUIRE_WHO(r->off >= 0, "off must be non-negative");
+  DFQ_REQUIRE_WHO(r->img_stride >= r->off + extent, "img_stride must be at least off + OH * OW * O");
+  const int64_t x_bytes = (int64_t)g->N * g->H * g->W * g->Cpad, s_bytes = (int64_t)g->N * g->H * g->W * 4;
+  const int64_t y_bytes = ((g->N - 1) * r->img_stride + extent) * (int64_t)sizeof(float);   // first to last row written
+  DFQ_REQUIRE_WHO(!overlap(xq, x_bytes, r->y + r->off, y_bytes) && !overlap(S_in, s_bytes, r->y + r->off, y_bytes),
+                  "y overlaps xq or S");
+  AffineRows ep{};
+  if (int rc = observer_scalars(who, "obs", r->obs_min, r->obs_max, r->obs_bits, &ep.obs, &ep.obs_on)) return rc;
+  if (int rc = observer_scalars(who, "tail", r->tail_min, r->tail_max, r->tail_bits, &ep.tail, &ep.tail_on)) return rc;
+  static_cast<Affine&>(ep) = Affine{S_in, table, k->kP, k->kA, k->kW, k->kN};
+  ep.y = r->y, ep.off = r->off, ep.img_stride = r->img_stride;
+  ep.pre_lo = r->pre_lo, ep.pre_hi = r->pre_hi, ep.post_lo = r->post_lo, ep.post_hi = r->post_hi;
+  return launch_conv<Out::AFFINE_ROWS>(who, xq, wq, nullptr, bias, nullptr, nullptr, g, ep, (cudaStream_t)stream);
 }

@@ -485,6 +485,7 @@ extern "C" int dfq_struct_size(int which) {
     case 14: return (int)sizeof(DfqI8AffineObserve);
     case 15: return (int)sizeof(DfqI8AffineLayout);
     case 16: return (int)sizeof(DfqI8AffineResize);
+    case 17: return (int)sizeof(DfqI8AffineRows);
     default: return -1;
   }
 }

@@ -24,7 +24,8 @@ between layers; in the reference's evaluation state (replace_op() active with a 
 observers into its graph and runs those on a producer's path in that producer's epilogue (dfq_i8_affine_conv_observed), so it
 computes what the per-layer model computes under the patched ops.  chain_affine(concat=True, fold_pads=True) also folds zero
 pads into the convolutions after them as pad codes and has the producers and bilinear upsamples of channel concatenations
-write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear).
+write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear), and
+chain_affine(pools=True) carries the codes through max pools (dfq_i8_affine_maxpool).
 """
 import ctypes as C
 import dataclasses
@@ -165,6 +166,31 @@ class _ConvLayer(nn.Module):
     def _check_out(self, out):
         if out is not None and self.out_slice is None:
             raise _lib.DfqError("layer %s: takes no output tensor" % self._who())
+
+    def out_extent(self, x):
+        """OH * OW * C_out: the floats one image of input x (fp32 NCHW, or the codes of a codes_in layer - the affine
+        scheme's (codes, S) pair) gives."""
+        if isinstance(x, tuple):
+            x = x[0]
+        H, W = (x.shape[1], x.shape[2]) if self.codes_in else (x.shape[2], x.shape[3])
+        g = self._geometry(1, int(H), int(W))
+        return int(g[0]["OH"]) * int(g[0]["OW"]) * self.out_channels
+
+    def _rows_out(self, out, off, N, OH, OW, dev):
+        """(out, off) of a rows-mode layer: `out` checked to hold this layer's rows at `off` of each image, or a new
+        [N, OH * OW, C_out] tensor and 0."""
+        n = OH * OW * self.out_channels
+        if out is None:
+            return torch.empty((N, OH * OW, self.out_channels), dtype=torch.float32, device=dev), 0
+        if not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.dim() < 2 or out.shape[0] != N or \
+                out.device != dev or not out.is_contiguous():
+            raise _lib.DfqError("layer %s: the rows' tensor must be contiguous fp32 [%d, ...] on %s, got %s" % (
+                self._who(), N, dev, "%s %s on %s" % (out.dtype, list(out.shape), out.device)
+                if isinstance(out, torch.Tensor) else type(out).__name__))
+        if not 0 <= off <= out[0].numel() - n:
+            raise _lib.DfqError("layer %s: rows [%d, %d) do not fit in the %d floats of an image"
+                                % (self._who(), off, off + n, out[0].numel()))
+        return out, off
 
     def _output_geometry(self, N, H, W):
         """(geometry, OH, OW) of an input [N, *, H, W], or DfqError when it is smaller than the kernel."""
@@ -340,24 +366,9 @@ class _Int8Layer(_ConvLayer):
                    "dfq_i8_conv_slice (layer %s)" % self._who())
         return out
 
-    def out_extent(self, x):
-        """OH * OW * C_out: the floats one image of input x (fp32 NCHW, or the codes of a codes_in layer) gives."""
-        H, W = (x.shape[1], x.shape[2]) if self.codes_in else (x.shape[2], x.shape[3])
-        g = self._geometry(1, int(H), int(W))
-        return int(g[0]["OH"]) * int(g[0]["OW"]) * self.out_channels
-
     def _run_rows(self, xq, out, off, g, N, OH, OW):
-        e, n = self.epilogue, OH * OW * self.out_channels
-        if out is None:
-            out, off = torch.empty((N, OH * OW, self.out_channels), dtype=torch.float32, device=xq.device), 0
-        elif not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.dim() < 2 or out.shape[0] != N or \
-                out.device != xq.device or not out.is_contiguous():
-            raise _lib.DfqError("layer %s: the rows' tensor must be contiguous fp32 [%d, ...] on %s, got %s" % (
-                self._who(), N, xq.device, "%s %s on %s" % (out.dtype, list(out.shape), out.device)
-                if isinstance(out, torch.Tensor) else type(out).__name__))
-        if not 0 <= off <= out[0].numel() - n:
-            raise _lib.DfqError("layer %s: rows [%d, %d) do not fit in the %d floats of an image"
-                                % (self._who(), off, off + n, out[0].numel()))
+        e = self.epilogue
+        out, off = self._rows_out(out, off, N, OH, OW, xq.device)
         d = np.zeros(1, _lib.I8_EPILOGUE_DT)
         d[0] = (0, out.data_ptr(), 0, 0.0) + e.pre + e.post
         _lib.check(_lib.load().dfq_i8_conv_nhwc(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
@@ -471,6 +482,8 @@ class _AffineInt8Layer(_ConvLayer):
 
     sums = False
     observers = (None, None)
+    tail_observer = None
+    rows = False
     pad_code = None
     _copied = _ConvLayer._copied + ("act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants", "pad_code")
 
@@ -521,7 +534,7 @@ class _AffineInt8Layer(_ConvLayer):
                             "the best candidate scale): run quantize_targ_layer first"
                             % (self._who(), self.w_bits, mw, mx, "all" if fewest is None else fewest, w.numel()))
 
-    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False, out_slice=None):
+    def chained(self, codes_in=False, requant=None, epilogue=None, name=None, sums=False, out_slice=None, rows=False):
         """A new module of the same class on the same buffers (weight_codes, tap_table, bias, constants), in the given
         execution mode: codes_in - take (codes, S) from the previous layer's epilogue instead of quantizing fp32; requant =
         ((act_min, act_max, act_bits), lo, hi) - return the consumer's codes after the clamp (lo, hi), the epilogue
@@ -529,8 +542,10 @@ class _AffineInt8Layer(_ConvLayer):
         None (the residual epilogue, dfq_i8_affine_conv_fused); sums - the codes come with their per-pixel sums S (a dense
         consumer reads them); out_slice = (coff, cstride), with codes and no fp32 output - write them into channels
         [coff, coff + round_up(C_out, 16)) of a concatenation's codes [N, OH, OW, cstride] and add S into its sums,
-        given as forward(x, out=(codes, S | None)) or made (S zeroed) when out is None.  The pad code of a folded F.pad is
-        kept.  name: the layer's name in error messages.  self is not modified."""
+        given as forward(x, out=(codes, S | None)) or made (S zeroed) when out is None; rows - the fp32 output
+        pixel-major into a detection head's concatenation (dfq_i8_affine_conv_rows), as _Int8Layer.chained(rows=True),
+        the clamps from an fp32-only epilogue without residual.  The pad code of a folded F.pad is kept.  name: the layer's
+        name in error messages.  self is not modified."""
         new = self._copy(codes_in, name or self.layer_name)
         if requant is not None and epilogue is not None:
             raise _lib.DfqError("layer %s: requant and epilogue are two output modes; give one" % new._who())
@@ -556,6 +571,12 @@ class _AffineInt8Layer(_ConvLayer):
                 raise _lib.DfqError("layer %s: a channel slice takes the codes only, without a residual" % new._who())
             out_slice = _channel_slice(out_slice, self.out_channels, "layer %s" % new._who())
         new.out_slice = out_slice
+        if rows:
+            if out_slice is not None or self.pad_code is not None or \
+                    (epilogue is not None and (epilogue.out_scale is not None or epilogue.residual)):
+                raise _lib.DfqError("layer %s: pixel-major fp32 rows exclude codes, a residual and a pad code" % new._who())
+            new.epilogue = epilogue or Epilogue(fp32=True)
+        new.rows = bool(rows)
         return new
 
     def fold_pad(self, pad):
@@ -571,17 +592,21 @@ class _AffineInt8Layer(_ConvLayer):
         new.pad_code = affine_code_of(0.0, self.act_min, self.act_max, self.act_bits)
         return new
 
-    def observe(self, obs=None, res=None):
+    def observe(self, obs=None, res=None, tail=None):
         """Give this chained layer's epilogue the functional-op observers of the reference's evaluation state
         (dfq_i8_affine_conv_observed): obs = (running_min, running_max, num_bits) of the QuantMeasure on v after the first
-        clamp (the fused operand of an observed add, or the producer's observed fp32 output), res = that of the one on
-        the residual; None: no observer.  Returns self."""
+        clamp (the fused operand of an observed add, the producer's observed fp32 output, or a head's concatenation
+        operand), res = that of the one on the residual, tail = (rows mode) that of the one on the head concatenation's
+        output, after the second clamp; None: no observer.  Returns self."""
         if self.epilogue is None:
             raise _lib.DfqError("layer %s: observers run in a chained layer's epilogue" % self._who())
         if res is not None and not self.epilogue.residual:
             raise _lib.DfqError("layer %s: an observer on the residual needs a residual input" % self._who())
+        if tail is not None and not self.rows:
+            raise _lib.DfqError("layer %s: an observer on a head concatenation's output needs rows mode" % self._who())
         self.observers = tuple(None if o is None else _observer_range(o, "layer %s: %s observer" % (self._who(), w))
                                for o, w in ((obs, "operand"), (res, "residual")))
+        self.tail_observer = None if tail is None else _observer_range(tail, "layer %s: tail observer" % self._who())
         return self
 
     def _input(self, x):
@@ -615,18 +640,22 @@ class _AffineInt8Layer(_ConvLayer):
                    "dfq_i8_affine_quantize (layer %s)" % self._who())
         return xq, S, N, H, W
 
-    def run(self, x, with_acc=False, residual=None, out=None):
+    def run(self, x, with_acc=False, residual=None, out=None, off=0):
         """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes.  In the chained modes
         x is (codes [N, H, W, cpad], S [N, H, W] | None) (codes_in), and with an epilogue y is (codes, S | None), the fp32
         output, or ((codes, S | None), fp32 output) when it returns both; `residual` is the fp32 tensor [N, C_out, OH, OW]
         the epilogue adds (exactly that shape, no broadcasting, on the input's device).  With out_slice, y is `out` (the
-        concatenation's (codes, S | None)) or a new such pair, its slice written."""
+        concatenation's (codes, S | None)) or a new such pair, its slice written.  With rows, y is `out` with this layer's
+        rows written at `off` of each image, or a new [N, OH * OW, C_out] tensor (see _Int8Layer.chained)."""
         if (self.epilogue is not None or self.pad_code is not None) and with_acc:
             raise _lib.DfqError("a chained affine layer does not return its int32 sums")
-        self._check_out(out)
+        if not self.rows:
+            self._check_out(out)
         self._check_residual(residual)
         xq, S, N, H, W = self._input(x)
         g, OH, OW = self._output_geometry(N, H, W)
+        if self.rows:
+            return self._run_rows(xq, S, out, off, g, N, OH, OW), None
         if self.epilogue is not None or self.pad_code is not None:
             return self._run_fused(xq, S, residual, g, N, OH, OW, out), None
         lib, st = _lib.load(), _lib.stream_ptr()
@@ -679,6 +708,18 @@ class _AffineInt8Layer(_ConvLayer):
                        "dfq_i8_affine_conv_observed (layer %s)" % self._who())
         codes = None if yq is None else (yq, S_out)
         return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
+
+    def _run_rows(self, xq, S, out, off, g, N, OH, OW):
+        out, off = self._rows_out(out, off, N, OH, OW, xq.device)
+        e, (obs, _), tail = self.epilogue, self.observers, self.tail_observer
+        r = np.zeros(1, _lib.I8_AFFINE_ROWS_DT)
+        r[0] = (out.data_ptr(), int(off), out[0].numel()) + e.pre + e.post + (obs or (0.0, 0.0, 0)) + (tail or (0.0, 0.0, 0))
+        _lib.check(_lib.load().dfq_i8_affine_conv_rows(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                                       _ptr(self.tap_table) if self.tap_table.numel() else None,
+                                                       _lib.table_ptr(self.constants), _ptr(self.bias), _lib.table_ptr(r),
+                                                       _lib.table_ptr(g), _lib.stream_ptr()),
+                   "dfq_i8_affine_conv_rows (layer %s)" % self._who())
+        return out
 
     def _slice_buffers(self, out, N, OH, OW, dev):
         """(codes [N, OH, OW, cstride], S [N, OH, OW] | None) of this slice's concatenation: `out`, checked, or new ones
@@ -762,8 +803,8 @@ class AffineInt8Conv2d(_AffineInt8Layer):
         return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
                    conv.groups, name=name)
 
-    def forward(self, x, r=None, out=None):
-        return self.run(x, residual=r, out=out)[0]
+    def forward(self, x, r=None, out=None, off=0):
+        return self.run(x, residual=r, out=out, off=off)[0]
 
 
 class AffineInt8Linear(_AffineInt8Layer):
@@ -795,14 +836,27 @@ class Int8MaxPool2d(nn.Module):
         self.stride = self.kernel_size if stride is None or stride == [] or stride == () else _pair(stride)
         self.ceil_mode, self.channels, self.codes_in = bool(ceil_mode), int(channels), bool(codes_in)
         self.cpad = (self.channels + 15) // 16 * 16
-        self.out_scale = None if out_scale is None else float(_f32(out_scale))
         self.fp32, self.layer_name = bool(fp32), name
-        if self.out_scale is not None:
-            check_scale("output", self.out_scale, "max pool %s" % name)
+        self.out_scale = None if out_scale is None else self._out(out_scale)
         if not codes_in and self.out_scale is None and not self.fp32:
             raise _lib.DfqError("max pool %s returns neither codes nor fp32" % name)
 
+    def _out(self, out_scale):
+        """out_scale as the pool keeps it (fp32 mode's codes are at it), checked."""
+        s = float(_f32(out_scale))
+        check_scale("output", s, "max pool %s" % self.layer_name)
+        return s
+
     def forward(self, x):
+        x, g, y, yq = self._launch_args(x)
+        _lib.check(_lib.load().dfq_i8_maxpool(_ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y),
+                                              _ptr(yq), C.c_float(self.out_scale or 0.0), _lib.table_ptr(g),
+                                              _lib.stream_ptr()), "dfq_i8_maxpool (%s)" % self.layer_name)
+        return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
+
+    def _launch_args(self, x):
+        """(x contiguous, DfqI8Pool table, y | None, yq | None) of the pool on its input x (codes or fp32, as codes_in
+        says), checked: the outputs allocated, fp32 y in fp32 mode when `fp32`, the codes yq when codes_in or out_scale."""
         if not isinstance(x, torch.Tensor) or not x.is_cuda:
             raise _lib.DfqError("int8 max pool %s runs on the GPU only (no CPU fallback)" % self.layer_name)
         if self.codes_in:
@@ -824,15 +878,43 @@ class Int8MaxPool2d(nn.Module):
             if self.codes_in or self.out_scale is not None else None
         y = torch.empty((N, self.channels, OH, OW), dtype=torch.float32, device=x.device) \
             if not self.codes_in and self.fp32 else None
-        _lib.check(_lib.load().dfq_i8_maxpool(_ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y),
-                                              _ptr(yq), C.c_float(self.out_scale or 0.0), _lib.table_ptr(g),
-                                              _lib.stream_ptr()), "dfq_i8_maxpool (%s)" % self.layer_name)
-        return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
+        return x, g, y, yq
 
     def extra_repr(self):
         return "kernel_size=%s, stride=%s, padding=%s, dilation=%s, ceil_mode=%s, channels=%d, %s" % (
             self.kernel_size, self.stride, self.padding, self.dilation, self.ceil_mode, self.channels,
             "codes" if self.codes_in else "fp32 in, out_scale=%s, fp32=%s" % (self.out_scale, self.fp32))
+
+
+class AffineInt8MaxPool2d(Int8MaxPool2d):
+    """F.max_pool2d of a model chained by chain_affine(pools=True) (dfq_i8_affine_maxpool): Int8MaxPool2d's geometry and
+    modes on the affine scheme's shifted codes.  codes_in: (codes [N, H, W, round_up(channels, 16)], S | None) in - S is
+    not read - and the pooled codes out.  Otherwise fp32 NCHW in, torch's max_pool2d out (`fp32`) and / or its codes at
+    out_scale = the consumers' (act_min, act_max, act_bits).  The codes come as (codes, S | None), S their per-pixel sums
+    when `sums` (a dense consumer reads them); ((codes, S | None), fp32) when both."""
+
+    def __init__(self, kernel_size, stride, padding, dilation, ceil_mode, channels, codes_in, out_scale=None, fp32=False,
+                 sums=False, name=None):
+        super().__init__(kernel_size, stride, padding, dilation, ceil_mode, channels, codes_in, out_scale, fp32, name)
+        self.sums = bool(sums)
+
+    def _out(self, out_scale):
+        return _observer_range(out_scale, "max pool %s: output" % self.layer_name)
+
+    def forward(self, x):
+        if self.codes_in and isinstance(x, tuple) and len(x) == 2:
+            x = x[0]                                            # the pool sums its own codes
+        x, g, y, yq = self._launch_args(x)
+        S = torch.empty(yq.shape[:3], dtype=torch.int32, device=x.device) if yq is not None and self.sums else None
+        lo, hi, bits = self.out_scale or (0.0, 0.0, 0)
+        _lib.check(_lib.load().dfq_i8_affine_maxpool(
+            _ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y), _ptr(yq), _ptr(S), C.c_float(lo),
+            C.c_float(hi), bits, _lib.table_ptr(g), _lib.stream_ptr()), "dfq_i8_affine_maxpool (%s)" % self.layer_name)
+        codes = None if yq is None else (yq, S)
+        return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
+
+    def extra_repr(self):
+        return super().extra_repr() + ", sums=%s" % self.sums
 
 
 def _upsample_input(x, size, channels, name):
@@ -928,8 +1010,9 @@ class AffineInt8UpsampleBilinear(nn.Module):
 
 class Int8HeadConcat(nn.Module):
     """torch.cat(..., 1) of detection heads laid out as `conv(x_i).permute(0, 2, 3, 1).contiguous().view(N, -1, k)` in a
-    chained model: each head (a rows-mode Int8Conv2d, _Int8Layer.chained(rows=True)) writes its pixel-major fp32 output
-    straight into its slice of one [N, R, k] tensor (dfq_i8_conv_nhwc), in order.  R and the offsets follow from the inputs'
+    chained model: each head (a rows-mode Int8Conv2d or AffineInt8Conv2d, chained(rows=True)) writes its pixel-major fp32
+    output straight into its slice of one [N, R, k] tensor (dfq_i8_conv_nhwc, dfq_i8_affine_conv_rows), in order; an
+    affine head's input may be the pair (codes, S).  R and the offsets follow from the inputs'
     sizes when the module runs.  batch: the view's constant N (None: the input's batch), checked."""
 
     def __init__(self, heads, k, batch=None, name=None):
@@ -940,15 +1023,16 @@ class Int8HeadConcat(nn.Module):
     def forward(self, *xs):
         if len(xs) != len(self.heads):
             raise _lib.DfqError("head concatenation %s takes %d inputs, got %d" % (self.layer_name, len(self.heads), len(xs)))
-        N = int(xs[0].shape[0])
-        if any(int(x.shape[0]) != N for x in xs) or (self.batch is not None and self.batch != N):
+        ts = [x[0] if isinstance(x, tuple) else x for x in xs]  # an affine head's (codes, S)
+        N = int(ts[0].shape[0])
+        if any(int(t.shape[0]) != N for t in ts) or (self.batch is not None and self.batch != N):
             raise _lib.DfqError("head concatenation %s: inputs of batch %s do not match the view's batch %s"
-                                % (self.layer_name, [int(x.shape[0]) for x in xs], self.batch or N))
+                                % (self.layer_name, [int(t.shape[0]) for t in ts], self.batch or N))
         ext = [h.out_extent(x) for h, x in zip(self.heads, xs)]
         if any(e % self.k for e in ext):
             raise _lib.DfqError("head concatenation %s: head outputs of %s floats per image do not view as rows of %d"
                                 % (self.layer_name, ext, self.k))
-        out = torch.empty((N, sum(ext) // self.k, self.k), dtype=torch.float32, device=xs[0].device)
+        out = torch.empty((N, sum(ext) // self.k, self.k), dtype=torch.float32, device=ts[0].device)
         off = 0
         for h, x, e in zip(self.heads, xs, ext):
             h(x, out=out, off=off)
@@ -1403,28 +1487,43 @@ def _head_operand(view, conv, mods):
     return dict(p=node, clamp=clamp, path=path + queries, k=k, batch=n)
 
 
-def _fuse_heads(gm, conv, mods):
-    """Rule (b) of chain_int8(layout=True): detection-head concatenations written in place by their producers."""
+def _fuse_heads(gm, conv, mods, affine=False):
+    """Rule (b) of chain_int8(layout=True): detection-head concatenations written in place by their producers.  affine
+    (chain_affine(heads=True)): AffineInt8Conv2d producers without a pad code, each operand optionally ending in its
+    replayed observer (after the view) and the cat's single user optionally a replayed observer, both applied by every
+    producer; returns (fused heads, fused observers as (observer module, "head" / "tail", producer name))."""
+    cats = (torch.cat, torch.concat) + ((_orig("cat"),) if affine else ())
     plans = []
+
+    def observer(node):
+        return node if affine and len(node.users) == 1 and _observer_key(node, mods) is not None else None
+
     for c in gm.graph.nodes:
-        if c.op != "call_function" or c.target not in (torch.cat, torch.concat) or set(c.kwargs) - {"tensors", "dim"}:
+        if c.op != "call_function" or c.target not in cats or set(c.kwargs) - {"tensors", "dim"}:
             continue
         ops, dim = _arg(c, 0, "tensors", None), _arg(c, 1, "dim", 0)
         if dim != 1 or not isinstance(ops, (list, tuple)) or len(ops) < 2 or not all(isinstance(o, fx.Node) for o in ops) \
                 or len(set(ops)) != len(ops):
             continue
-        heads = [_head_operand(o, conv, mods) for o in ops]
+        obs = [observer(o) for o in ops]
+        heads = [_head_operand(o if ob is None else o.args[0], conv, mods) for o, ob in zip(ops, obs)]
         if any(h is None for h in heads) or len({h["k"] for h in heads}) != 1 or len({h["p"] for h in heads}) != len(heads) \
-                or len({h["batch"] for h in heads} - {None}) > 1:
+                or len({h["batch"] for h in heads} - {None}) > 1 or \
+                any(getattr(gm.get_submodule(h["p"].target), "pad_code", None) is not None for h in heads):
             continue
-        plans.append((c, heads, next((h["batch"] for h in heads if h["batch"] is not None), None)))
-    g, fused = gm.graph, []
-    for c, heads, batch in plans:
+        tail = observer(next(iter(c.users))) if len(c.users) == 1 else None
+        plans.append((c, heads, next((h["batch"] for h in heads if h["batch"] is not None), None), obs, tail))
+    g, fused, observed = gm.graph, [], []
+    for c, heads, batch, obs, tail in plans:
         layers = []
-        for h in heads:
+        tkey = None if tail is None else _observer_key(tail, mods)
+        for h, ob in zip(heads, obs):
             p = h["p"]
             layer = gm.get_submodule(p.target).chained(codes_in=gm.get_submodule(p.target).codes_in, name=p.target,
                                                       epilogue=Epilogue(None, h["clamp"], fp32=True), rows=True)
+            if ob is not None or tail is not None:
+                layer = layer.observe(obs=None if ob is None else _observer_key(ob, mods), tail=tkey)
+                observed += [(o.target, what, p.target) for o, what in ((ob, "head"), (tail, "tail")) if o is not None]
             _set_module(gm, p.target, layer)
             layers.append(layer)
         name = "int8_heads_" + c.name
@@ -1433,7 +1532,10 @@ def _fuse_heads(gm, conv, mods):
             node = g.call_module(name, tuple(h["p"].args[0] for h in heads))
         c.replace_all_uses_with(node)
         g.erase_node(c)
-        dead = {n for h in heads for n in h["path"]}
+        if tail is not None:
+            tail.replace_all_uses_with(node)
+            g.erase_node(tail)
+        dead = {n for h in heads for n in h["path"]} | {ob for ob in obs if ob is not None}
         while dead:                                             # each node goes once nothing uses it
             for n in [n for n in dead if not n.users]:
                 g.erase_node(n)
@@ -1441,7 +1543,7 @@ def _fuse_heads(gm, conv, mods):
         fused.append((c.name, [h["p"].target for h in heads], heads[0]["k"]))
     g.lint()
     gm.recompile()
-    return fused
+    return (fused, observed) if affine else fused
 
 
 def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False, upsample=False,
@@ -1553,7 +1655,8 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
     return _chain_edges(gm, mods, conv, _NCNN)
 
 
-def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=False, fold_pads=False) -> fx.GraphModule:
+def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=False, fold_pads=False,
+                 pools=False, heads=False) -> fx.GraphModule:
     """A torch.fx GraphModule that computes what `model` (after convert_affine) computes, with activations kept as the
     consumers' shifted affine codes between AffineInt8Conv2d layers, bit-identical to the per-layer path.
 
@@ -1574,8 +1677,8 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=Fa
       raise DfqError naming the layer when the module runs.
     A producer writes the codes' per-pixel sums S (which a dense consumer's epilogue reads) only when some code consumer is
     dense, and its fp32 output only when a user other than those consumers remains.  Ncnn Int8Conv2d layers and
-    AffineInt8Linear stay opaque leaves, so no edge crosses the two schemes; pools and detection heads stay in torch, fp32,
-    and so do concatenations, upsampling and pads unless concat / fold_pads (below) take them.
+    AffineInt8Linear stay opaque leaves, so no edge crosses the two schemes; detection heads, max pools, concatenations,
+    upsampling and pads stay in torch, fp32, unless heads / pools / concat / fold_pads (below) take them.
 
     The layers of the result are new modules sharing the packed buffers of `model`'s; `model` is not modified.  The fused
     edges are recorded in `requantized_edges`: (producer name, consumer name, (lo, hi)) in graph order, (lo, hi) the clamp
@@ -1620,17 +1723,46 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=Fa
       codes, one buffer per forward, in graph order: the operand chain's clamp, the operand's observer, the tail's clamp,
       then the consumers' code; the slice's channel sums add into one S zeroed by the first writer, only when a consumer
       is dense.  Shape queries on the operands read a zero-stride view of the writer's codes (_nchw_view).
-    - max pools stay in torch, as does any cat not taken (SSD's head concatenations along dim 1 of [N, R, k] included).
+    - any cat not taken stays in torch (SSD's head concatenations along dim 1 of [N, R, k] included).
     `fused_cats` records (cat node name, writer names, channel offsets), `fused_upsamples` (node name, producer name,
     "slice", align_corners), and the operands' observers enter `fused_observers` as (observer module, "cat", writer
-    name).  concat=True without residual=True raises DfqError."""
+    name).  concat=True without residual=True raises DfqError.
+
+    pools=True (with residual=True) carries the codes through max pools, chain_int8(pool_cat=True)'s pool rule under the
+    affine scheme (AffineInt8MaxPool2d, dfq_i8_affine_maxpool), with the consumers' range key in place of their scale:
+    codes mode pools the codes of a producer's tail, a fused concatenation's (with concat=True) or another fused pool's,
+    every user of the pool past exact identities taking codes at one key; fp32 mode pools a producer's clamped fp32 output
+    when some user of the pool needs fp32 (ResNet's stem, whose pooled tensor is a residual) and writes the codes of the
+    users at the first key too.  The pool writes S only when one of its code consumers is dense.  replace_op() puts no
+    observer on max pools; one on a pool's input or output is an fp32 user.  Bit-identical to the per-layer path except for
+    a window holding a NaN, which gives the max of the other codes where the per-layer path gives code -128.  `fused_pools`
+    records (pool node name, "codes" or "fp32", the outputs it writes), as chain_int8 records it.  pools=True without
+    residual=True raises DfqError.
+
+    heads=True (with residual=True) writes detection-head concatenations in place, chain_int8(layout=True)'s rule (b)
+    under the affine scheme: a torch.cat along dim 1 of >= 2 operands, each `view(N, -1, k)` / `reshape` of [`.contiguous()`
+    of] `.permute(0, 2, 3, 1)` of a distinct single-site AffineInt8Conv2d's single-user pass-through chain (no folded pad),
+    optionally followed by the operand's replayed observer, one k and one N.  Each producer becomes a rows-mode copy
+    (_AffineInt8Layer.chained(rows=True), dfq_i8_affine_conv_rows) that writes its slice of one [N, R, k] tensor
+    (Int8HeadConcat): the clamp, the operand's observer, and - when the cat's only user is a replayed observer (SSD's
+    softmax input, an elementwise op, so per slice) - that observer too, which is deleted.  Any operand that does not
+    qualify leaves the cat in torch.  `fused_heads` records (cat node name, producer names, k), and the observers enter
+    `fused_observers` as (observer module, "head", producer name) and, once per producer, (observer module, "tail",
+    producer name).  heads=True without residual=True raises DfqError."""
     if concat and not residual:
         raise _lib.DfqError("chain_affine: concat=True builds on residual=True")
+    if pools and not residual:
+        raise _lib.DfqError("chain_affine: pools=True builds on residual=True")
+    if heads and not residual:
+        raise _lib.DfqError("chain_affine: heads=True builds on residual=True")
     LT = _observed_state()
     gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer, LT)
     folded = _fold_pads(gm, mods, conv, affine=True) if fold_pads else None
     if residual:
-        gm = _chain_residual(gm, mods, conv, concat, concat, scheme=_AFFINE)
+        gm = _chain_residual(gm, mods, conv, concat, concat, scheme=_AFFINE, pool_rule=pools)
+        if heads:
+            gm.fused_heads, observed = _fuse_heads(gm, conv, mods, affine=True)
+            gm.fused_observers = gm.fused_observers + observed
     else:
         gm = _chain_edges(gm, mods, conv, _AFFINE)
         gm.fused_observers = []
@@ -1886,13 +2018,14 @@ def _split(g, node):
     return codes, y
 
 
-def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None):
-    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True[, concat=True],
-    which passes pool_cat = upsample = concat) on the traced `gm` (see chain_int8, chain_affine); scheme: _NCNN (default)
-    or _AFFINE.  Under _AFFINE, max pools and upsamples whose users take codes stay in torch."""
+def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None, pool_rule=None):
+    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True[, concat=True]
+    [, pools=True]), which passes pool_cat = upsample = concat, on the traced `gm` (see chain_int8, chain_affine); scheme:
+    _NCNN (default) or _AFFINE.  pool_rule: apply the max pool rule (None: when pool_cat).  Under _AFFINE, upsamples
+    whose users take codes stay in torch."""
     scheme = scheme or _NCNN
     affine = scheme is _AFFINE
-    pool = pool_cat and not affine
+    pool = pool_cat if pool_rule is None else pool_rule
     full = (-_INF, _INF)
     order = {n: i for i, n in enumerate(gm.graph.nodes)}
 
@@ -2230,8 +2363,12 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         k, s, pad, dil, ceil = _max_pool(u, mods)
         codes_mode = pp["mode"] == "codes"
         fp32 = not codes_mode
-        mod = Int8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, None if codes_mode else float(pp["scale"]),
-                            fp32, name=u.name)
+        out = None if codes_mode else scheme.out(pp["scale"])
+        if affine:                                              # S only for a dense consumer
+            sums = any(v in convs and mods[v.target].groups == 1 for v in pp["codes"])
+            mod = AffineInt8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, out, fp32, sums, name=u.name)
+        else:
+            mod = Int8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, out, fp32, name=u.name)
         name = "int8_pool_" + u.name
         gm.add_submodule(name, mod)
         inp = u.args[0]
@@ -2267,6 +2404,7 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None)
         gm.fused_observers = observed
     if pool_cat:
         gm.fused_cats = cats
+    if pool_cat or pool:
         gm.fused_pools = pools
     if upsample:
         gm.fused_upsamples = ups

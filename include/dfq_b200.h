@@ -45,7 +45,7 @@ const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
- * 16 DfqI8AffineResize): lets a binding verify
+ * 16 DfqI8AffineResize, 17 DfqI8AffineRows): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -676,6 +676,47 @@ typedef struct DfqI8AffineResize {
  * bounds, an observer or output range as dfq_i8_affine_conv_observed refuses, x, the slice and S overlapping.
  * DFQ_E_UNSUPPORTED: obs_bits or out_bits above 8.  Nothing is written when a call is refused. */
 int dfq_i8_affine_upsample_bilinear(const float* x, int8_t* yq, int32_t* S, const DfqI8AffineResize* g, void* stream);
+/* A detection head's rows under the affine scheme (dfq_i8_conv_nhwc's layout): the convolution of dfq_i8_affine_conv
+ * (inputs as there) with, per output element (n, o, p), in this order:
+ *   v = fp32(kP P + kA A + kW Wv + kN Nv) + bias[o]           as dfq_i8_affine_conv
+ *   v = clamp(v, pre_lo, pre_hi)                               NaN stays NaN; (-inf, +inf): no clamp
+ *   v = fq(v, obs_min, obs_max, obs_bits)                      when obs_bits > 0: the concatenation operand's observer
+ *   v = clamp(v, post_lo, post_hi)
+ *   v = fq(v, tail_min, tail_max, tail_bits)                   when tail_bits > 0: the observer of the concatenation's
+ *                                                              single user (elementwise, so per slice)
+ *   y[n * img_stride + off + p * O + o] = v
+ * fq as dfq_i8_affine_conv_observed.  Nothing else of y is written. */
+typedef struct DfqI8AffineRows {
+  float* y;
+  int64_t off, img_stride;     /* the slice of each image's img_stride floats; img_stride >= off + OH * OW * O      */
+  float pre_lo, pre_hi, post_lo, post_hi;
+  float obs_min, obs_max;
+  int32_t obs_bits;            /* 0: off                                                                          */
+  float tail_min, tail_max;
+  int32_t tail_bits;           /* 0: off                                                                          */
+} DfqI8AffineRows;
+/* Refusals of dfq_i8_affine_conv as there, and DFQ_E_ARG with a reason: r or y NULL, y not 4-byte aligned, NaN or
+ * unordered bounds, off < 0, img_stride < off + OH * OW * O, the rows overlapping xq or S_in, an observer with bits < 0
+ * or (when on) a non-finite range or a scale that is not a finite fp32 number.  DFQ_E_UNSUPPORTED: an observer with bits
+ * > 8.  Nothing is written when a call is refused. */
+int dfq_i8_affine_conv_rows(const int8_t* xq, const int32_t* S_in, const int8_t* wq, const int32_t* table,
+                            const DfqI8Affine* k, const float* bias, const DfqI8AffineRows* r, const DfqI8Conv* g,
+                            void* stream);
+/* dfq_i8_maxpool under the affine scheme; the geometry and the two modes as there (exactly one input):
+ *   xq (codes): shifted codes int8 NHWC [N, H, W, Cpad] -> yq, the byte-wise signed max of the taps inside the input.  The
+ *      shifted code of dfq_i8_affine_quantize is monotone non-decreasing (its scale is at least 1e-8), so this is the code
+ *      of max_pool2d(v) for any window without NaN.  A window with no tap in the input gives -128, the code of torch's
+ *      -inf; pad channels 0.  The exception of the per-layer path: a window holding a NaN gives -128 there (NaN quantizes
+ *      to code 0) and the max of the other codes here.  y must be NULL; out_min, out_max and out_bits are not read.
+ *   x (fp32): NCHW -> y (NULL: not written) bit for bit torch's CUDA max_pool2d, as dfq_i8_maxpool, and / or yq = the codes
+ *      dfq_i8_affine_quantize gives y at (out_min, out_max, out_bits), the consumer's range (NULL: not written).
+ * Both: S[n, p] = the sum of yq[n, p, :] over the C real channels (int32 [N, OH, OW]; NULL: not written), what
+ * dfq_i8_affine_quantize writes bit for bit; the call zeroes it on `stream` and the kernel adds into it.
+ * Refusals of dfq_i8_maxpool as there, and DFQ_E_ARG with a reason: S without yq or not 4-byte aligned, inputs and outputs
+ * S included overlapping, and while yq is written in fp32 mode an output range dfq_i8_affine_quantize refuses or
+ * out_bits < 1.  DFQ_E_UNSUPPORTED: out_bits > 8 in that case.  Nothing is written when a call is refused. */
+int dfq_i8_affine_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, int32_t* S, float out_min, float out_max,
+                          int32_t out_bits, const DfqI8Pool* g, void* stream);
 
 #ifdef __cplusplus
 }

@@ -23,7 +23,11 @@ networks, the three affine arms' logits asserted bit-identical.  `affine_observe
 networks in the reference's evaluation state (tests/affine_observed_state.py: replace_op() active, the functional-op
 observers on every residual add and, for MobileNetV2 with the reference's head, on the mean's input), timing the
 fake-quantized model, the per-layer convert_affine model and chain_affine(residual=True), which runs the observers in its
-epilogues; the two affine arms' logits asserted bit-identical.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+epilogues; the two affine arms' logits asserted bit-identical.  `affine_pool_heads` (only when asked for):
+ResNet-18 and GoogLeNet in that state, per-layer against chain_affine(residual=True[, concat=True]) and the same with
+pools=True (max pools carried as affine codes), and SSD-Lite at 300x300 against chain_affine(residual=True, concat=True,
+fold_pads=True) and the same with heads=True (detection heads written in place), outputs asserted bit-identical, with
+the fp32 bytes the flags avoid.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
 device; writes nothing.
 """
 import argparse
@@ -868,6 +872,114 @@ def affine_layout_inference(dev, reps=10, batch=8, rounds=5, size=513):
     return out
 
 
+def affine_pool_heads_inference(dev, reps=10, batch=256, rounds=5, ssd_batch=256):
+    """Networks in the reference's evaluation state, replace_op() active, each timed alternately in three arms (per-layer
+    convert_affine, chain_affine without the new flag, the same call with it), `rounds` rounds of `reps` passes, median,
+    the arms' outputs asserted bit-identical: ResNet-18 (residual=True, then pools=True) and GoogLeNet (residual=True,
+    concat=True, then pools=True) at batch x 3 x 224 x 224, SSD-Lite (tests/ssd_lite_like.py, is_test; residual=True,
+    concat=True, fold_pads=True, then heads=True) at ssd_batch x 3 x 300 x 300.  The fp32 bytes the flag avoids are counted
+    from the shapes of the arm without it (torch.fx ShapeProp): per fused pool its fp32 output written and read by its
+    consumers' quantizer, and in codes mode its fp32 input written and read; per fused head its NCHW output written and
+    read by the permute copy, that copy written and read by the cat (and by the operand's observer, written and read
+    again, when it has one); per fused tail observer the concatenation read and written."""
+    import statistics
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_observed_state
+    from dfq_b200 import int8
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    def same(a, b):
+        if isinstance(a, (tuple, list)):
+            return all(same(u, v) for u, v in zip(a, b))
+        return bool(torch.equal(a.view(torch.int32), b.view(torch.int32)))
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"unit": "images/s", "reps": reps, "rounds": rounds}
+    nets = (("resnet18", 224, batch, {}, "pools"), ("googlenet", 224, batch, {"concat": True}, "pools"),
+            ("ssd", 300, ssd_batch, {"concat": True, "fold_pads": True}, "heads"))
+    try:
+        for net, size, n, kw, flag in nets:
+            x = torch.randn(n, 3, size, size, device=dev, generator=torch.Generator(device=dev).manual_seed(3))
+            x.clamp_(-2.5, 2.5)
+            with affine_observed_state.evaluation_state(net, size=size) as (model, qgraph, qtarg):
+                int8.convert_affine(model, qgraph, qtarg)
+                base = int8.chain_affine(model, residual=True, **kw)
+                gm = int8.chain_affine(model, residual=True, **kw, **{flag: True})
+                arms = (("affine_per_layer", model), ("affine_chained", base), ("affine_chained_" + flag, gm))
+                with torch.no_grad():
+                    ref = model(x)
+                    ok = all(same(ref, m(x)) for _, m in arms[1:])
+                    assert ok, net
+                    for _, m in arms:
+                        m(x)
+                    torch.cuda.synchronize(dev)
+                    ms = {k: [] for k, _ in arms}
+                    for _ in range(rounds):
+                        for k, m in arms:
+                            ms[k].append(timed(lambda m=m: m(x)))
+                    size_of = _fp32_bytes(base, x)
+                med = {k: statistics.median(v) for k, v in ms.items()}
+                avoided = 0
+                for name, mode, _ in getattr(gm, "fused_pools", []):
+                    i_bytes, o_bytes = size_of[name]
+                    avoided += 2 * o_bytes + (2 * i_bytes if mode == "codes" else 0)
+                heads = getattr(gm, "fused_heads", [])
+                observed = {(what, p) for _, what, p in gm.fused_observers}
+                for _, producers, _ in heads:
+                    for p in producers:
+                        e = size_of[p][1]
+                        avoided += 4 * e + (2 * e if ("head", p) in observed else 0) + \
+                            (2 * e if ("tail", p) in observed else 0)
+                rec = {"batch": n, "image": "3x%dx%d" % (size, size),
+                       "images_per_s": {k: n / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                       "ms_per_batch_rounds": ms, "fused_observers": len(gm.fused_observers),
+                       "observers": model.custom_tensor_op.len,
+                       "edges": [len(base.requantized_edges), len(gm.requantized_edges)],
+                       "fp32_bytes_avoided_per_batch": avoided, "outputs_bit_identical": ok}
+                if flag == "pools":
+                    rec["fused_pools"] = [p[:2] for p in gm.fused_pools]
+                    rec["fused_cats"] = len(getattr(gm, "fused_cats", []))
+                else:
+                    rec["fused_heads"] = [(c, len(ps), k) for c, ps, k in heads]
+                    rec["fused_observers_by_kind"] = {w: sum(1 for _, v, _ in gm.fused_observers if v == w)
+                                                      for w in ("residual", "operand", "output", "cat", "head", "tail")}
+                out[net] = rec
+                del base, gm
+            del model, x
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
+def _fp32_bytes(gm, x):
+    """{node name and call_module target: (bytes of its first tensor argument, of its output)} of gm's nodes with a
+    single tensor output, from torch.fx ShapeProp on x."""
+    from torch.fx.passes.shape_prop import ShapeProp
+    ShapeProp(gm).propagate(x)
+    out = {}
+    for n in gm.graph.nodes:
+        meta = n.meta.get("tensor_meta")
+        if not hasattr(meta, "shape"):
+            continue
+        a = n.args[0] if n.args and hasattr(n.args[0], "meta") else None
+        am = a.meta.get("tensor_meta") if a is not None else None
+        nbytes = (am.shape.numel() * am.dtype.itemsize if hasattr(am, "shape") else 0, meta.shape.numel() * meta.dtype.itemsize)
+        out[n.name] = nbytes
+        if n.op == "call_module":
+            out[n.target] = nbytes
+    return out
+
+
 def card():
     """Name and power limit of the GPU (read only)."""
     import torch
@@ -889,8 +1001,8 @@ def main():
     p.add_argument("--seg-batch", type=int, default=8, help="batch of the 513x513 segmentation networks (upsample, layout)")
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
-                   help="comma-separated sections to run (default: all but affine, affine_chained, affine_observed and "
-                        "affine_layout)")
+                   help="comma-separated sections to run (default: all but affine, affine_chained, affine_observed, "
+                        "affine_layout and affine_pool_heads)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -916,6 +1028,9 @@ def main():
         res["affine_observed"] = affine_observed_inference(dev, reps=args.reps, batch=args.batch)
     if "affine_layout" in want:
         res["affine_layout"] = affine_layout_inference(dev, reps=args.reps, batch=args.seg_batch)
+    if "affine_pool_heads" in want:
+        res["affine_pool_heads"] = affine_pool_heads_inference(dev, reps=args.reps, batch=args.batch,
+                                                               ssd_batch=args.ssd_batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
