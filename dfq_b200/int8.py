@@ -27,6 +27,7 @@ pads into the convolutions after them as pad codes and has the producers and bil
 write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear), and
 chain_affine(pools=True) carries the codes through max pools (dfq_i8_affine_maxpool).
 """
+import collections
 import ctypes as C
 import dataclasses
 import operator
@@ -827,10 +828,11 @@ def _pool_extent(n, k, p, s, d, ceil_mode):
 class Int8MaxPool2d(nn.Module):
     """F.max_pool2d of a chained model (dfq_i8_maxpool).  codes_in: int8 NHWC codes [N, H, W, round_up(channels, 16)] in,
     the pooled codes out (the max of codes is the code of the max, q being monotone).  Otherwise fp32 NCHW in, bit for bit
-    torch's max_pool2d out (`fp32`) and / or its codes at out_scale: (codes, fp32) when both."""
+    torch's max_pool2d out (`fp32`) and / or its codes at out_scale: (codes, fp32) when both.  sums: ignored (ncnn codes
+    have no per-pixel sums), so that AffineInt8MaxPool2d's arguments fit both."""
 
     def __init__(self, kernel_size, stride, padding, dilation, ceil_mode, channels, codes_in, out_scale=None, fp32=False,
-                 name=None):
+                 name=None, sums=False):
         super().__init__()
         self.kernel_size, self.padding, self.dilation = _pair(kernel_size), _pair(padding), _pair(dilation)
         self.stride = self.kernel_size if stride is None or stride == [] or stride == () else _pair(stride)
@@ -937,10 +939,15 @@ class Int8UpsampleBilinear(nn.Module):
     [N, channels, H, W] in, the codes q(clamp(y, *clamp), out_scale) of torch's bilinear output y out - int8 NHWC
     [N, OH, OW, round_up(channels, 16)], or with out_slice = (coff, cstride) channels [coff, coff + round_up(channels, 16))
     of `out` (int8 [N, OH, OW, cstride], made when None).  The size comes at run time (often a traced value such as
-    x.shape[-2:]) and must be a pair of positive ints."""
+    x.shape[-2:]) and must be a pair of positive ints.  pre, obs, post, sums: as AffineInt8UpsampleBilinear's (a given
+    pre makes the clamp pre then post; ncnn has no observers or sums)."""
 
-    def __init__(self, channels, align_corners, out_scale, clamp=(-float("inf"), float("inf")), out_slice=None, name=None):
+    def __init__(self, channels, align_corners, out_scale, clamp=(-float("inf"), float("inf")), out_slice=None, name=None,
+                 pre=None, obs=None, post=(-float("inf"), float("inf")), sums=False):
         super().__init__()
+        if obs is not None:
+            raise _lib.DfqError("bilinear upsample %s: the ncnn scheme runs no observer" % name)
+        clamp = clamp if pre is None else _compose(pre, post)
         self.channels, self.align_corners, self.layer_name = int(channels), bool(align_corners), name
         self.cpad = (self.channels + 15) // 16 * 16
         check_scale("output", out_scale, "bilinear upsample %s" % name)
@@ -1142,6 +1149,7 @@ def _set_module(root, name, mod):
 
 # ---- chaining converted convolutions through int8 codes ---------------------------------------------------------------
 _INF = float("inf")
+_FULL = (-_INF, _INF)                                           # no clamp
 
 
 _TORCH_DIR = os.path.dirname(torch.__file__) + os.sep
@@ -1200,9 +1208,7 @@ def _pass_through(node, mods):
             return (0.0, _INF)
         if type(m) in (nn.ReLU6, nn.Hardtanh):                  # ReLU6 is Hardtanh(0, 6)
             return (float(m.min_val), float(m.max_val))
-        if type(m) is nn.Identity:
-            return (-_INF, _INF)
-        if type(m) is nn.Dropout and not m.training:
+        if type(m) is nn.Identity or (type(m) is nn.Dropout and not m.training):
             return (-_INF, _INF)
         return None
     if node.op == "call_function":
@@ -1364,14 +1370,14 @@ def _nchw_view(codes, channels):
     return codes.as_strided((N, channels, H, W), (0, 0, 0, 0))
 
 
-def _cat_operands(node, raw=False):
-    """The operands of torch.cat / torch.concat along the channels (dim 1 or -3) of >= 2 distinct fx nodes, without out;
-    None otherwise.  raw: the unpatched torch.cat counts too (_orig)."""
+def _cat_operands(node, raw=False, dims=(1, -3)):
+    """The operands of torch.cat / torch.concat along the channels (a dim in `dims`) of >= 2 distinct fx nodes, without
+    out; None otherwise.  raw: the unpatched torch.cat counts too (_orig)."""
     cats = (torch.cat, torch.concat) + ((_orig("cat"),) if raw else ())
     if node.op != "call_function" or node.target not in cats or set(node.kwargs) - {"tensors", "dim"}:
         return None
     ops, dim = _arg(node, 0, "tensors", None), _arg(node, 1, "dim", 0)
-    if dim not in (1, -3) or not isinstance(ops, (list, tuple)) or len(ops) < 2 or \
+    if dim not in dims or not isinstance(ops, (list, tuple)) or len(ops) < 2 or \
             not all(isinstance(o, fx.Node) for o in ops) or len(set(ops)) != len(ops):
         return None
     return list(ops)
@@ -1394,10 +1400,9 @@ def _zero_pad(node):
     return t, l
 
 
-def _fold_pads(gm, mods, conv, affine=False):
-    """Rule (a) of chain_int8(layout=True): fold each qualifying zero F.pad into its only user, an Int8Conv2d.  affine
-    (chain_affine(fold_pads=True)): into an AffineInt8Conv2d with padding 0, whose out-of-image taps then read the code of
-    +0.0 at its input range (_AffineInt8Layer.fold_pad)."""
+def _fold_pads(gm, mods, conv, scheme):
+    """Rule (a) of chain_int8(layout=True) and chain_affine(fold_pads=True): fold each qualifying zero F.pad into its only
+    user, a `scheme` convolution that takes it (_Scheme.fold_pad); recorded in gm.folded_pads."""
     folded = []
     for node in list(gm.graph.nodes):
         tl = _zero_pad(node)
@@ -1406,26 +1411,31 @@ def _fold_pads(gm, mods, conv, affine=False):
         q = next(iter(node.users))
         if not conv(q) or q.args != (node,) or q.kwargs:
             continue
-        m = mods[q.target]
-        if affine:
-            if m.padding != (0, 0):
-                continue
-            new = m.chained(name=q.target).fold_pad(tl)
-        else:
-            new = m.chained(name=q.target)
-            new.padding = (m.padding[0] + tl[0], m.padding[1] + tl[1])
+        new = scheme.fold_pad(mods[q.target], q.target, tl)
+        if new is None:
+            continue
         _set_module(gm, q.target, new)
         mods[q.target] = new
         q.args = (node.args[0],)
         gm.graph.erase_node(node)
         folded.append((node.name, q.target, tl))
-    return folded
+    gm.folded_pads = folded
+
+
+@dataclasses.dataclass
+class _Head:
+    """A detection-head operand: producer p, its clamp, the nodes deleted with it, the view's k and constant N or None."""
+    p: fx.Node
+    clamp: tuple
+    path: list
+    k: int
+    batch: Optional[int]
 
 
 def _head_operand(view, conv, mods):
-    """(producer, clamp, nodes to delete, k, constant N or None) of a cat operand `view(N, -1, k)` / `reshape` of
-    [`.contiguous()` of] `.permute(0, 2, 3, 1)` of an Int8Conv2d producer's single-user pass-through chain; None otherwise.
-    N is a constant or a dim-0 shape query (.size(0), .shape[0], .size()[0]) of a node on that path, used only by the view."""
+    """The _Head of a cat operand `view(N, -1, k)` / `reshape` of [`.contiguous()` of] `.permute(0, 2, 3, 1)` of a `conv`
+    producer's single-user pass-through chain; None otherwise.  N is a constant or a dim-0 shape query (.size(0),
+    .shape[0], .size()[0]) of a node on that path, used only by the view."""
     if view.op != "call_method" or view.target not in ("view", "reshape") or view.kwargs or len(view.args) < 2 or \
             not isinstance(view.args[0], fx.Node) or len(view.users) != 1:
         return None
@@ -1451,11 +1461,8 @@ def _head_operand(view, conv, mods):
 
     def query_nodes(u, n):
         """[u, ...] when u reads a shape of n and everything it feeds ends at the view; None otherwise."""
-        if u.op == "call_method" and u.target == "size" and u.args[0] is n and not u.kwargs and len(u.args) <= 2:
-            pass
-        elif u.op == "call_function" and u.target is getattr and u.args == (n, "shape"):
-            pass
-        else:
+        if not (u.op == "call_method" and u.target == "size" and u.args[0] is n and not u.kwargs and len(u.args) <= 2) \
+                and not (u.op == "call_function" and u.target is getattr and u.args == (n, "shape")):
             return None
         if u.users.keys() == {view}:
             return [u]
@@ -1466,9 +1473,7 @@ def _head_operand(view, conv, mods):
     queries = []
     for a, b in zip(path[1:], path):                            # every node but the view: the next node and shape queries
         for u in a.users:
-            if u is b:
-                continue
-            qn = query_nodes(u, a)
+            qn = [] if u is b else query_nodes(u, a)
             if qn is None:
                 return None
             queries += qn
@@ -1484,66 +1489,57 @@ def _head_operand(view, conv, mods):
         return None
     if any(q.users.keys() - {view} - set(queries) for q in queries):
         return None
-    return dict(p=node, clamp=clamp, path=path + queries, k=k, batch=n)
+    return _Head(node, clamp, path + queries, k, n)
 
 
-def _fuse_heads(gm, conv, mods, affine=False):
-    """Rule (b) of chain_int8(layout=True): detection-head concatenations written in place by their producers.  affine
-    (chain_affine(heads=True)): AffineInt8Conv2d producers without a pad code, each operand optionally ending in its
-    replayed observer (after the view) and the cat's single user optionally a replayed observer, both applied by every
-    producer; returns (fused heads, fused observers as (observer module, "head" / "tail", producer name))."""
-    cats = (torch.cat, torch.concat) + ((_orig("cat"),) if affine else ())
-    plans = []
+def _replayed_observer(node, mods, scheme):
+    """node, when it calls a replayed observer an epilogue of `scheme` runs (_observer_key) and has one user; else None."""
+    return node if scheme.observers and len(node.users) == 1 and _observer_key(node, mods) is not None else None
 
-    def observer(node):
-        return node if affine and len(node.users) == 1 and _observer_key(node, mods) is not None else None
 
-    for c in gm.graph.nodes:
-        if c.op != "call_function" or c.target not in cats or set(c.kwargs) - {"tensors", "dim"}:
-            continue
-        ops, dim = _arg(c, 0, "tensors", None), _arg(c, 1, "dim", 0)
-        if dim != 1 or not isinstance(ops, (list, tuple)) or len(ops) < 2 or not all(isinstance(o, fx.Node) for o in ops) \
-                or len(set(ops)) != len(ops):
-            continue
-        obs = [observer(o) for o in ops]
-        heads = [_head_operand(o if ob is None else o.args[0], conv, mods) for o, ob in zip(ops, obs)]
-        if any(h is None for h in heads) or len({h["k"] for h in heads}) != 1 or len({h["p"] for h in heads}) != len(heads) \
-                or len({h["batch"] for h in heads} - {None}) > 1 or \
-                any(getattr(gm.get_submodule(h["p"].target), "pad_code", None) is not None for h in heads):
-            continue
-        tail = observer(next(iter(c.users))) if len(c.users) == 1 else None
-        plans.append((c, heads, next((h["batch"] for h in heads if h["batch"] is not None), None), obs, tail))
+def _fuse_heads(gm, conv, mods, scheme):
+    """Rule (b) of chain_int8(layout=True) and chain_affine(heads=True): detection-head concatenations written in place by
+    their producers (no pad code), each applying its operand's replayed observer and one on the cat's single user, if
+    any; returns (fused heads, fused observers as (observer module, "head" / "tail", producer name))."""
     g, fused, observed = gm.graph, [], []
-    for c, heads, batch, obs, tail in plans:
-        layers = []
-        tkey = None if tail is None else _observer_key(tail, mods)
+    for c in list(g.nodes):                                     # a cat's rewrite touches only its own operands' nodes
+        ops = _cat_operands(c, scheme.observers, dims=(1,))
+        if ops is None:
+            continue
+        obs = [_replayed_observer(o, mods, scheme) for o in ops]
+        heads = [_head_operand(o if ob is None else o.args[0], conv, mods) for o, ob in zip(ops, obs)]
+        if any(h is None for h in heads) or len({h.k for h in heads}) != 1 or len({h.p for h in heads}) != len(heads) \
+                or len({h.batch for h in heads} - {None}) > 1 or \
+                any(getattr(gm.get_submodule(h.p.target), "pad_code", None) is not None for h in heads):
+            continue
+        tail = _replayed_observer(next(iter(c.users)), mods, scheme) if len(c.users) == 1 else None
+        tkey, layers = None if tail is None else _observer_key(tail, mods), []
         for h, ob in zip(heads, obs):
-            p = h["p"]
+            p = h.p
             layer = gm.get_submodule(p.target).chained(codes_in=gm.get_submodule(p.target).codes_in, name=p.target,
-                                                      epilogue=Epilogue(None, h["clamp"], fp32=True), rows=True)
+                                                      epilogue=Epilogue(None, h.clamp, fp32=True), rows=True)
             if ob is not None or tail is not None:
                 layer = layer.observe(obs=None if ob is None else _observer_key(ob, mods), tail=tkey)
                 observed += [(o.target, what, p.target) for o, what in ((ob, "head"), (tail, "tail")) if o is not None]
             _set_module(gm, p.target, layer)
             layers.append(layer)
         name = "int8_heads_" + c.name
-        gm.add_submodule(name, Int8HeadConcat(layers, heads[0]["k"], batch, name=c.name))
+        batch = next((h.batch for h in heads if h.batch is not None), None)
+        gm.add_submodule(name, Int8HeadConcat(layers, heads[0].k, batch, name=c.name))
         with g.inserting_before(c):
-            node = g.call_module(name, tuple(h["p"].args[0] for h in heads))
-        c.replace_all_uses_with(node)
-        g.erase_node(c)
-        if tail is not None:
-            tail.replace_all_uses_with(node)
-            g.erase_node(tail)
-        dead = {n for h in heads for n in h["path"]} | {ob for ob in obs if ob is not None}
+            node = g.call_module(name, tuple(h.p.args[0] for h in heads))
+        for old in [c] + ([tail] if tail is not None else []):
+            old.replace_all_uses_with(node)
+            g.erase_node(old)
+        dead = {n for h in heads for n in h.path} | {o for o in obs if o is not None}
         while dead:                                             # each node goes once nothing uses it
             for n in [n for n in dead if not n.users]:
                 g.erase_node(n)
                 dead.discard(n)
-        fused.append((c.name, [h["p"].target for h in heads], heads[0]["k"]))
+        fused.append((c.name, [h.p.target for h in heads], heads[0].k))
     g.lint()
     gm.recompile()
-    return (fused, observed) if affine else fused
+    return fused, observed
 
 
 def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=False, upsample=False,
@@ -1639,20 +1635,14 @@ def chain_int8(model: nn.Module, concrete_args=None, residual=False, pool_cat=Fa
         does not qualify the cat stays in torch.  `fused_heads` records (cat node name, producer names, k).
     layout=True without upsample=True raises DfqError."""
     gm, mods, conv = _trace(model, concrete_args, _NCNN.layer)
-    if pool_cat and not residual:
-        raise _lib.DfqError("chain_int8: pool_cat=True builds on residual=True")
-    if upsample and not pool_cat:
-        raise _lib.DfqError("chain_int8: upsample=True builds on pool_cat=True")
-    if layout and not upsample:
-        raise _lib.DfqError("chain_int8: layout=True builds on upsample=True")
-    folded = _fold_pads(gm, mods, conv) if layout else None
-    if residual:
-        gm = _chain_residual(gm, mods, conv, pool_cat, upsample)
-        if layout:
-            gm.folded_pads = folded
-            gm.fused_heads = _fuse_heads(gm, conv, mods)
-        return gm
-    return _chain_edges(gm, mods, conv, _NCNN)
+    for flag, on, base, has in (("pool_cat", pool_cat, "residual", residual), ("upsample", upsample, "pool_cat", pool_cat),
+                                ("layout", layout, "upsample", upsample)):
+        if on and not has:
+            raise _lib.DfqError("chain_int8: %s=True builds on %s=True" % (flag, base))
+    if layout:
+        _fold_pads(gm, mods, conv, _NCNN)
+    rules = _Rules(cats=pool_cat, pools=pool_cat, up_slices=upsample, up_codes=upsample, heads=layout)
+    return _Rewriter(gm, mods, conv, _NCNN, rules).run() if residual else _chain_edges(gm, mods, conv, _NCNN)
 
 
 def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=False, fold_pads=False,
@@ -1749,27 +1739,17 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=Fa
     qualify leaves the cat in torch.  `fused_heads` records (cat node name, producer names, k), and the observers enter
     `fused_observers` as (observer module, "head", producer name) and, once per producer, (observer module, "tail",
     producer name).  heads=True without residual=True raises DfqError."""
-    if concat and not residual:
-        raise _lib.DfqError("chain_affine: concat=True builds on residual=True")
-    if pools and not residual:
-        raise _lib.DfqError("chain_affine: pools=True builds on residual=True")
-    if heads and not residual:
-        raise _lib.DfqError("chain_affine: heads=True builds on residual=True")
+    for flag, on in (("concat", concat), ("pools", pools), ("heads", heads)):
+        if on and not residual:
+            raise _lib.DfqError("chain_affine: %s=True builds on residual=True" % flag)
     LT = _observed_state()
     gm, mods, conv = _trace(model, concrete_args, _AFFINE.layer, LT)
-    folded = _fold_pads(gm, mods, conv, affine=True) if fold_pads else None
-    if residual:
-        gm = _chain_residual(gm, mods, conv, concat, concat, scheme=_AFFINE, pool_rule=pools)
-        if heads:
-            gm.fused_heads, observed = _fuse_heads(gm, conv, mods, affine=True)
-            gm.fused_observers = gm.fused_observers + observed
-    else:
-        gm = _chain_edges(gm, mods, conv, _AFFINE)
-        gm.fused_observers = []
+    if fold_pads:
+        _fold_pads(gm, mods, conv, _AFFINE)
+    rules = _Rules(cats=concat, pools=pools, up_slices=concat, up_codes=False, heads=heads)
+    gm = _Rewriter(gm, mods, conv, _AFFINE, rules).run() if residual else _chain_edges(gm, mods, conv, _AFFINE)
     if LT is not None:
         _unpatch_adds(gm, LT)
-    if fold_pads:
-        gm.folded_pads = folded
     return gm
 
 
@@ -1777,19 +1757,45 @@ class _Scheme(NamedTuple):
     """What the chaining rules need of one integer scheme: `layer`, the convolution class whose edges they fuse; key(m),
     what decides the codes layer m reads, compared bit for bit by same(a, b) (consumers with equal keys read identical
     codes); out(key), the producer's output argument for such a consumer (requant's first element, Epilogue.out_scale).
-    Both schemes' layers take a mode as the same chained() arguments (codes_in, name, requant or epilogue, out_slice,
-    sums)."""
+    observers: replayed observers exist and the evaluation state's raw ops count (_orig).  pool, upsample: the fused
+    modules' classes (one argument list).  slice(out, pre, post): a cat writer's chained() mode (clamp pre, observer,
+    clamp post).  fold_pad(m, name, (t, l)): m's copy reading through a zero pad, or None."""
     layer: type
     key: object
     same: object
     out: object
+    observers: bool
+    pool: type
+    upsample: type
+    slice: object
+    fold_pad: object
 
 
-_NCNN = _Scheme(Int8Conv2d, lambda m: _f32(m.act_scale), lambda a, b: a.view(np.int32) == b.view(np.int32), float)
+def _fold_ncnn_pad(m, name, pad):
+    new = m.chained(name=name)
+    new.padding = (m.padding[0] + pad[0], m.padding[1] + pad[1])
+    return new
+
+
+_NCNN = _Scheme(Int8Conv2d, lambda m: _f32(m.act_scale), lambda a, b: a.view(np.int32) == b.view(np.int32), float,
+                observers=False, pool=Int8MaxPool2d, upsample=Int8UpsampleBilinear,
+                slice=lambda out, pre, post: dict(requant=(out,) + _compose(pre, post)), fold_pad=_fold_ncnn_pad)
 _AFFINE = _Scheme(AffineInt8Conv2d, lambda m: (_f32(m.act_min), _f32(m.act_max), int(m.act_bits)),
                   lambda a, b: a[0].view(np.int32) == b[0].view(np.int32) and a[1].view(np.int32) == b[1].view(np.int32)
                   and a[2] == b[2],
-                  lambda k: (float(k[0]), float(k[1]), int(k[2])))
+                  lambda k: (float(k[0]), float(k[1]), int(k[2])),
+                  observers=True, pool=AffineInt8MaxPool2d, upsample=AffineInt8UpsampleBilinear,
+                  slice=lambda out, pre, post: dict(epilogue=Epilogue(out, pre, post)),
+                  fold_pad=lambda m, name, pad: m.chained(name=name).fold_pad(pad) if m.padding == (0, 0) else None)
+
+
+class _Rules(NamedTuple):
+    """_Rewriter's rules besides fan-out and adds: cats, pools, upsamples into cats or to codes users, detection heads."""
+    cats: bool
+    pools: bool
+    up_slices: bool
+    up_codes: bool
+    heads: bool
 
 
 def _observed_state():
@@ -1855,9 +1861,9 @@ def _replay_observers(gm, model, LT):
                 if not isinstance(ts, (list, tuple)) or not all(isinstance(t, fx.Node) for t in ts):
                     continue
                 ops, names_ok = tuple(ts), ("torch_cat_%d_%d" % (line, len(ts)),)
+            elif not isinstance(node.args[0], fx.Node):
+                continue
             else:
-                if not isinstance(node.args[0], fx.Node):
-                    continue
                 ops, names_ok = (node.args[0],), ("%s_%d_1" % (raw[node.target], line),)
         else:
             continue
@@ -1944,10 +1950,7 @@ def _trace(model, concrete_args, layer, observed=None):
     if observed is not None:
         _replay_observers(gm, model, observed)
     mods = dict(gm.named_modules())
-    sites = {}
-    for node in gm.graph.nodes:
-        if node.op == "call_module":
-            sites[node.target] = sites.get(node.target, 0) + 1
+    sites = collections.Counter(node.target for node in gm.graph.nodes if node.op == "call_module")
 
     def conv(node):
         return node.op == "call_module" and isinstance(mods[node.target], layer) and sites[node.target] == 1
@@ -1956,7 +1959,7 @@ def _trace(model, concrete_args, layer, observed=None):
 
 
 def _chain_edges(gm, mods, conv, scheme):
-    """The single-user edge rule of chain_int8 / chain_affine (residual=False) on the traced `gm`."""
+    """The single-user edge rule of chain_int8 / chain_affine (residual=False) on the traced `gm`; no observer fused."""
     edges, between = [], []
     for q in list(gm.graph.nodes):
         if not conv(q) or len(q.args) != 1 or q.kwargs or not isinstance(q.args[0], fx.Node):
@@ -1983,15 +1986,16 @@ def _chain_edges(gm, mods, conv, scheme):
     gm.graph.lint()
     gm.recompile()
     gm.requantized_edges = edges
+    if scheme.observers:
+        gm.fused_observers = []
     return gm
 
 
 @dataclasses.dataclass
 class _Plan:
-    """One producer's rewrite in _chain_residual: producer p, its single-user pass-throughs `path` (clamp `pre`) to the
-    node `tail` whose users `codes` take its codes at key `scale`; with a fused add `add`, residual argument index ri, the
-    pass-throughs after the add `post_path` (clamp `post`); the fused operand's and the residual's observers obs / robs
-    (`output`: obs is on the fp32 output instead); the residual's skipped identities and its node's name r_name."""
+    """A producer's plan: p, its pass-throughs `path` (clamp `pre`) to `tail`, whose users `codes` take codes at `scale`;
+    a fused `add`, its residual argument ri and the pass-throughs `post_path` after it (clamp `post`); the observers obs
+    (without an add: on the fp32 output) and robs (residual); the residual's skipped identities and its name r_name."""
     p: fx.Node
     path: list
     pre: tuple
@@ -2000,13 +2004,53 @@ class _Plan:
     scale: object = None
     add: Optional[fx.Node] = None
     ri: Optional[int] = None
-    post: tuple = (-_INF, _INF)
+    post: tuple = _FULL
     post_path: list = dataclasses.field(default_factory=list)
     obs: Optional[fx.Node] = None
     robs: Optional[fx.Node] = None
-    output: bool = False
     skipped: list = dataclasses.field(default_factory=list)
     r_name: Optional[str] = None
+
+    def nodes(self):
+        return (self.p, *self.path, *([self.add] if self.add is not None else []), *self.post_path)
+
+
+@dataclasses.dataclass
+class _Codes:
+    """A node whose users `codes` take its codes, `channels` wide, at key `scale` after the clamp `clamp`, past the
+    pass-throughs `path` to `tail`: a codes-mode upsample's plan, or a max pool's (exact identities; no tail: fp32 mode)."""
+    node: fx.Node
+    path: list
+    tail: Optional[fx.Node]
+    clamp: tuple
+    codes: list
+    scale: object
+    channels: int
+
+    def nodes(self):
+        return (self.node, *self.path)
+
+
+@dataclasses.dataclass
+class _Operand:
+    """A fused cat's operand: writer p, the nodes `path` back to it (clamp `pre`), observer, slice and shape queries."""
+    p: fx.Node
+    path: list
+    pre: tuple
+    obs: Optional[fx.Node]
+    coff: int
+    channels: int
+    queries: list
+
+
+@dataclasses.dataclass
+class _CatPlan(_Codes):
+    """A concatenation's plan: its _Operands write one buffer, with sums when a consumer is dense."""
+    operands: list
+    sums: bool
+
+    def nodes(self):
+        return (*super().nodes(), *(n for o in self.operands for n in (o.p, *o.path)))
 
 
 def _split(g, node):
@@ -2018,230 +2062,212 @@ def _split(g, node):
     return codes, y
 
 
-def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None, pool_rule=None):
-    """chain_int8(..., residual=True[, pool_cat=True[, upsample=True]]) or chain_affine(..., residual=True[, concat=True]
-    [, pools=True]), which passes pool_cat = upsample = concat, on the traced `gm` (see chain_int8, chain_affine); scheme:
-    _NCNN (default) or _AFFINE.  pool_rule: apply the max pool rule (None: when pool_cat).  Under _AFFINE, upsamples
-    whose users take codes stay in torch."""
-    scheme = scheme or _NCNN
-    affine = scheme is _AFFINE
-    pool = pool_cat if pool_rule is None else pool_rule
-    full = (-_INF, _INF)
-    order = {n: i for i, n in enumerate(gm.graph.nodes)}
+class _Rewriter:
+    """chain_int8(residual=True, ...) / chain_affine(residual=True, ...) on the traced gm: fan-out, adds and `rules` under
+    `scheme`.  The plan_* steps read the graph as traced, as do the memos; run() then rewrites it."""
 
-    def producer(node):
-        return conv(node) and len(node.args) == 1 and not node.kwargs and isinstance(node.args[0], fx.Node)
+    def __init__(self, gm, mods, conv, scheme, rules):
+        self.gm, self.mods, self.conv, self.scheme, self.rules = gm, mods, conv, scheme, rules
+        self.order = {n: i for i, n in enumerate(gm.graph.nodes)}
+        self.convs = {n for n in gm.graph.nodes if self.producer(n)}   # before the rewrites give producers a second input
+        # bilinear upsamples: the producer whose single-user pass-through chain ends at the upsample's input
+        self.ends = {self.forward(p)[0]: p for p in self.convs} if rules.up_slices or rules.up_codes else {}
+        self.sources, self.pool_scales, self.pools = {}, {}, []
+        self.edges, self.adds, self.modes, self.watched, self.observed, self.cats, self.ups = [], [], {}, {}, [], [], []
 
-    def forward(node, step=lambda u: _pass_through(u, mods)):
-        """Walk from node through its single users u of one fx input for which step(u) is a clamp (by default the
-        pass-throughs): (last node, composed clamp, the nodes walked)."""
-        clamp, path = full, []
+    def producer(self, node):
+        return self.conv(node) and len(node.args) == 1 and not node.kwargs and isinstance(node.args[0], fx.Node)
+
+    def forward(self, node, identities=False):
+        """(last node, composed clamp, nodes walked) from node through single users of one fx input that are
+        pass-throughs (exact identities, as after a pool, with `identities`)."""
+        clamp, path = _FULL, []
         while len(node.users) == 1:
             u = next(iter(node.users))
-            c = step(u)
+            c = (_FULL if _is_identity(u, self.mods) else None) if identities else _pass_through(u, self.mods)
             if c is None or len(u.all_input_nodes) != 1 or u.args[0] is not node:
                 break
             clamp, node = _compose(clamp, c), u
             path.append(u)
         return node, clamp, path
 
-    def identity(u):
-        """The step of the walk after a pool: exact identities, no clamp."""
-        return full if _is_identity(u, mods) else None
+    def observer(self, node):
+        return _replayed_observer(node, self.mods, self.scheme) is not None
 
-    def observe(node):
-        """node calls a QuantMeasure the affine epilogue runs (_observer_key) and has one user."""
-        return scheme is _AFFINE and len(node.users) == 1 and _observer_key(node, mods) is not None
-
-    def unobserved(node):
-        return node.args[0] if observe(node) else node
-
-    same = scheme.same
-
-    # bilinear upsamples: the producer whose single-user pass-through chain ends at the upsample's input
-    ends = {forward(p)[0]: p for p in gm.graph.nodes if producer(p)} if upsample else {}
-
-    sources = {}
-
-    def up_source(node):
-        """The producer of a fusable bilinear upsample node, or None (as the traced graph has it: memoized before the
-        rewrites)."""
-        if node not in sources:
+    def up_source(self, node):
+        """The producer of a fusable bilinear upsample node, or None."""
+        if node not in self.sources:
             src = node.args[0] if node.args else None
-            if affine and isinstance(src, fx.Node) and observe(src):   # its input observer goes into the producer
+            if isinstance(src, fx.Node) and self.observer(src):    # its input observer goes into the producer
                 src = src.args[0]
-            sources[node] = ends.get(src) if ends and _bilinear_upsample(node, mods, affine) is not None else None
-        return sources[node]
+            self.sources[node] = self.ends.get(src) if self.ends and \
+                _bilinear_upsample(node, self.mods, self.scheme.observers) is not None else None
+        return self.sources[node]
 
-    pool_memo = {}
+    def pool_scale(self, pool, channels):
+        """The key at which every user of a pool (past exact identities) takes codes, or None."""
+        if pool not in self.pool_scales:
+            self.pool_scales[pool] = None
+            tail = self.forward(pool, True)[0]
+            scales = [self.user_scale(u, tail, channels) for u in tail.users]
+            self.pool_scales[pool] = scales[0] if scales and all(
+                s is not None and self.scheme.same(s, scales[0]) for s in scales) else None
+        return self.pool_scales[pool]
 
-    def pool_scale(pool, channels):
-        """The scale at which every user of a pool (past exact identities) takes codes, or None."""
-        if pool not in pool_memo:
-            pool_memo[pool] = None
-            tail = forward(pool, identity)[0]
-            scales = [user_scale(u, tail, channels) for u in tail.users]
-            if scales and all(s is not None and same(s, scales[0]) for s in scales):
-                pool_memo[pool] = scales[0]
-        return pool_memo[pool]
-
-    def user_scale(u, tail, channels, pools=True):
-        """The scale at which u takes the codes of `tail` (channels wide), or None when it takes fp32."""
-        if producer(u) and u.args[0] is tail and mods[u.target].in_channels == channels:
-            return scheme.key(mods[u.target])
-        if pools and pool and _max_pool(u, mods) is not None and u.args[0] is tail:
-            return pool_scale(u, channels)
+    def user_scale(self, u, tail, channels, pools=True):
+        """The key at which u takes the codes of `tail` (channels wide), or None when it takes fp32."""
+        if self.producer(u) and u.args[0] is tail and self.mods[u.target].in_channels == channels:
+            return self.scheme.key(self.mods[u.target])
+        if pools and self.rules.pools and _max_pool(u, self.mods) is not None and u.args[0] is tail:
+            return self.pool_scale(u, channels)
         return None
 
-    def take_codes(tail, channels, pools=True):
-        """The fan-out rule: the users of tail that take codes at the first such user's scale (graph order), and it."""
+    def take_codes(self, tail, channels, pools=True):
+        """The fan-out rule: the users of tail that take codes at the first such user's key (graph order), and it."""
         codes, scale = [], None
-        for u in sorted(tail.users, key=order.get):
-            s = user_scale(u, tail, channels, pools)
-            if s is not None and (scale is None or same(s, scale)):
+        for u in sorted(tail.users, key=self.order.get):
+            s = self.user_scale(u, tail, channels, pools)
+            if s is not None and (scale is None or self.scheme.same(s, scale)):
                 scale = s
                 codes.append(u)
         return codes, scale
 
-    pool_plans = []
-
-    def codes_pool(u, channels, clamp):
-        tail, _, ids = forward(u, identity)
-        pool_plans.append(dict(node=u, mode="codes", tail=tail, path=ids, codes=sorted(tail.users, key=order.get),
-                               scale=pool_scale(u, channels), clamp=clamp, channels=channels))
-        for v in tail.users:
-            if not producer(v):
-                codes_pool(v, channels, clamp)
-
-    plans = []
-    for p in list(gm.graph.nodes):
-        if not producer(p):
-            continue
-        end, pre, path = forward(p)
-        add, ri, post, post_path, tail = None, None, full, [], end
-        fobs = robs = None
-        if len(end.users) == 1:
-            a = next(iter(end.users))
-            if observe(a):                                      # the observer on the fused operand (replace_op's add)
-                fobs, a = a, next(iter(a.users))
-            if _is_add(a):
-                fused = next((i for i, v in enumerate(a.args) if _walk_back(unobserved(v), mods, producer) is not None),
-                             None)
-                if fused is not None and unobserved(a.args[fused]) is end and (fobs is None or a.args[fused] is fobs):
-                    add, ri = a, 1 - fused
-                    tail, post, post_path = forward(a)
-                    robs = a.args[ri] if observe(a.args[ri]) else None
-            if add is None:
-                fobs = None
-        out_c = mods[p.target].out_channels
-        codes, scale = take_codes(tail, out_c)
-        clamp = post if add is not None else pre
-        if add is None and not codes and pool and len(tail.users) == 1:
-            u = next(iter(tail.users))                          # fp32-mode pool: a user of the pool needs fp32
-            if _max_pool(u, mods) is not None and u.args[0] is tail:
-                pc, ps = take_codes(u, out_c, pools=False)
-                if pc:
-                    pool_plans.append(dict(node=u, mode="fp32", path=[], codes=pc, scale=ps, clamp=clamp, channels=out_c))
-                    plans.append(_Plan(p, path, pre, tail))
-            continue
-        if add is None and not codes:
-            continue
-        plans.append(_Plan(p, path, pre, tail, codes, scale, add=add, ri=ri, post=post, post_path=post_path, obs=fobs,
-                           robs=robs))
+    def plan_pools(self, codes, channels, clamp):
+        """The codes-mode pools among `codes` (users that take a tail's codes) and among the users after them."""
         for u in codes:
-            if not producer(u):
-                codes_pool(u, out_c, clamp)
+            if not self.producer(u):
+                tail, _, ids = self.forward(u, True)
+                self.pools.append(_Codes(u, ids, tail, clamp, sorted(tail.users, key=self.order.get),
+                                         self.pool_scale(u, channels), channels))
+                self.plan_pools(tail.users, channels, clamp)
 
-    # concatenations whose operands come from their own producers and whose users all take codes at one scale
-    cat_plans = []
-    for c in (list(gm.graph.nodes) if pool_cat else []):
-        ops = _cat_operands(c, affine)
-        if ops is None:
-            continue
-        # under the affine scheme an operand may end in its replayed observer, which the operand's writer applies
-        oobs = [o if affine and observe(o) else None for o in ops]
-        ops = [o.args[0] if ob is not None else o for o, ob in zip(ops, oobs)]
-        backs = [_walk_back(o, mods, producer, upsample) or
-                 (_walk_back(o, mods, lambda n: up_source(n) is not None, True) if upsample else None) for o in ops]
-        if any(b is None for b in backs) or len({b[0] for b in backs}) != len(backs):
-            continue
-        chans = [mods[(up_source(q) or q).target].out_channels for q, _, _ in backs]
-        if any(k % 16 for k in chans[:-1]):
-            continue
-        tail, tclamp, tpath = forward(c)
-        codes, scale = take_codes(tail, sum(chans))
-        if not codes or len(codes) != len(tail.users):
-            continue
-        operands = []
-        for ob, (q, clamp, opath), k, off in zip(oobs, backs, chans, np.cumsum([0] + chans[:-1]).tolist()):
-            queries = [(u, n) for n in (q, *opath) for u in n.users if upsample and _shape_query(u, n)]
-            operands.append(dict(p=q, path=opath, clamp=_compose(clamp, tclamp), pre=clamp, obs=ob, coff=off, channels=k,
-                                 queries=queries))
-        cat_plans.append(dict(cat=c, operands=operands, tail=tail, path=tpath, codes=codes, scale=scale, clamp=tclamp,
-                              cstride=(sum(chans) + 15) // 16 * 16, sums=any(producer(u) and mods[u.target].groups == 1 for u in codes)))
-        for u in codes:
-            if not producer(u):
-                codes_pool(u, sum(chans), tclamp)
+    def plan_producers(self):
+        """Single-user edges, fan-out and residual adds, and fp32-mode pools: the producers' _Plans."""
+        plans, mods = [], self.mods
+        for p in list(self.gm.graph.nodes):
+            if not self.producer(p):
+                continue
+            end, pre, path = self.forward(p)
+            add, ri, post, post_path, tail = None, None, _FULL, [], end
+            fobs = robs = None
+            if len(end.users) == 1:
+                a = next(iter(end.users))
+                if self.observer(a):                            # the observer on the fused operand (replace_op's add)
+                    fobs, a = a, next(iter(a.users))
+                if _is_add(a):
+                    ops = [v.args[0] if self.observer(v) else v for v in a.args]
+                    fused = next((i for i, v in enumerate(ops) if _walk_back(v, mods, self.producer) is not None), None)
+                    if fused is not None and ops[fused] is end and (fobs is None or a.args[fused] is fobs):
+                        add, ri = a, 1 - fused
+                        tail, post, post_path = self.forward(a)
+                        robs = a.args[ri] if self.observer(a.args[ri]) else None
+                if add is None:
+                    fobs = None
+            out_c = mods[p.target].out_channels
+            codes, scale = self.take_codes(tail, out_c)
+            clamp = post if add is not None else pre
+            if add is None and not codes and self.rules.pools and len(tail.users) == 1:
+                u = next(iter(tail.users))                      # fp32-mode pool: a user of the pool needs fp32
+                if _max_pool(u, mods) is not None and u.args[0] is tail:
+                    pc, ps = self.take_codes(u, out_c, pools=False)
+                    if pc:
+                        self.pools.append(_Codes(u, [], None, clamp, pc, ps, out_c))
+                        plans.append(_Plan(p, path, pre, tail))
+                continue
+            if add is None and not codes:
+                continue
+            plans.append(_Plan(p, path, pre, tail, codes, scale, add=add, ri=ri, post=post, post_path=post_path, obs=fobs,
+                               robs=robs))
+            self.plan_pools(codes, out_c, clamp)
+        return plans
 
-    # observers on a producer's fp32 output: its single-user pass-through chain, then shape-only views, then the observer
-    # (shape queries not counted as users); the producer applies it in its epilogue and writes the observed fp32 output
-    taken = {n for pl in plans for n in (pl.obs, pl.robs) if n is not None}
-    taken |= {o["obs"] for cp in cat_plans for o in cp["operands"] if o["obs"] is not None}
-    planned = {pl.p for pl in plans}
-    for o in (list(gm.graph.nodes) if scheme is _AFFINE else []):
-        if o in taken or _observer_key(o, mods) is None:
-            continue
-        node = o.args[0]
-        while _is_view(node) and len(_data_users(node, True)) == 1:
-            node = node.args[0]
-        back = _walk_back(node, mods, producer, queries=True)
-        if back is None or back[0] in planned:
-            continue
-        q, clamp, path = back
-        plans.append(_Plan(q, path[::-1], clamp, node, obs=o, output=True))
-        planned.add(q)
+    def plan_cats(self):
+        """Concatenations whose operands come from their own writers and whose users all take codes at one key."""
+        plans, up, mods = [], self.rules.up_slices, self.mods
+        for c in (list(self.gm.graph.nodes) if self.rules.cats else []):
+            ops = _cat_operands(c, self.scheme.observers)
+            if ops is None:
+                continue
+            oobs = [o if self.observer(o) else None for o in ops]   # the operand's writer applies its observer
+            ops = [o.args[0] if ob is not None else o for o, ob in zip(ops, oobs)]
+            backs = [_walk_back(o, mods, self.producer, up) or
+                     (_walk_back(o, mods, lambda n: self.up_source(n) is not None, True) if up else None) for o in ops]
+            if any(b is None for b in backs) or len({b[0] for b in backs}) != len(backs):
+                continue
+            chans = [mods[(self.up_source(q) or q).target].out_channels for q, _, _ in backs]
+            if any(k % 16 for k in chans[:-1]):
+                continue
+            tail, tclamp, tpath = self.forward(c)
+            codes, scale = self.take_codes(tail, sum(chans))
+            if not codes or len(codes) != len(tail.users):
+                continue
+            operands = [_Operand(q, opath, clamp, ob, off, k,
+                                 [(u, n) for n in (q, *opath) for u in n.users if up and _shape_query(u, n)])
+                        for ob, (q, clamp, opath), k, off in zip(oobs, backs, chans, np.cumsum([0] + chans[:-1]).tolist())]
+            plans.append(_CatPlan(c, tpath, tail, tclamp, codes, scale, sum(chans), operands,
+                                  any(self.producer(u) and mods[u.target].groups == 1 for u in codes)))
+            self.plan_pools(codes, sum(chans), tclamp)
+        return plans
 
-    # upsamples: slice mode through a fused concatenation above, codes mode when every user takes codes at one scale;
-    # either way the producer writes its clamped fp32 output
-    up_plans = [dict(node=o["p"], mode="slice", path=[]) for cp in cat_plans for o in cp["operands"] if not producer(o["p"])]
-    sliced = {up["node"] for up in up_plans}
-    for u in (list(gm.graph.nodes) if upsample and not affine else []):
-        if u in sliced or up_source(u) is None:
-            continue
-        utail, uclamp, upath = forward(u)
-        codes, scale = take_codes(utail, mods[up_source(u).target].out_channels, pools=False)
-        if codes and len(codes) == len(utail.users):
-            up_plans.append(dict(node=u, mode="codes", tail=utail, clamp=uclamp, path=upath, codes=codes, scale=scale))
-    planned = {pl.p for pl in plans}
-    for up in up_plans:
-        p = up_source(up["node"])
-        if p not in planned:
-            end, pre, path = forward(p)
-            plans.append(_Plan(p, path, pre, end))
-            planned.add(p)
-    plans.sort(key=lambda pl: order[pl.p])
+    def plan_observers(self, plans, cats):
+        """Add to `plans` the observers after a producer's pass-throughs and shape-only views, run in its epilogue."""
+        taken = {n for pl in plans for n in (pl.obs, pl.robs)} | {o.obs for cp in cats for o in cp.operands}
+        planned = {pl.p for pl in plans}
+        for o in (list(self.gm.graph.nodes) if self.scheme.observers else []):
+            if o in taken or _observer_key(o, self.mods) is None:
+                continue
+            node = o.args[0]
+            while _is_view(node) and len(_data_users(node, True)) == 1:
+                node = node.args[0]
+            back = _walk_back(node, self.mods, self.producer, queries=True)
+            if back is None or back[0] in planned:
+                continue
+            q, clamp, path = back
+            plans.append(_Plan(q, path[::-1], clamp, node, obs=o))
+            planned.add(q)
 
-    # the residual's exact identities, skipped once every plan's own nodes are known: a node another plan deletes (an
-    # identity at the end of its post-add chain, say) stays the residual, and that plan replaces it by its fp32 output
-    claimed = {n for pl in plans for n in (pl.p, *pl.path, *([pl.add] if pl.add is not None else []), *pl.post_path)}
-    claimed |= {n for cp in cat_plans for n in (cp["cat"], *cp["path"], *(n for o in cp["operands"] for n in (o["p"], *o["path"])))}
-    claimed |= {n for pp in pool_plans for n in (pp["node"], *pp["path"])}
-    claimed |= {n for up in up_plans for n in (up["node"], *up["path"])}
-    for pl in plans:
-        if pl.add is None:
-            continue
-        r = pl.robs.args[0] if pl.robs is not None else pl.add.args[pl.ri]
-        while r not in claimed and len(r.users) == 1 and _is_identity(r, mods) and isinstance(r.args[0], fx.Node):
-            pl.skipped.append(r)
-            r = r.args[0]
-        pl.r_name = r.name
+    def plan_upsamples(self, plans, cats):
+        """Codes-mode upsamples; their and the fused cats' upsamples' producers write fp32 (a _Plan added if none)."""
+        sliced, ups = [o.p for cp in cats for o in cp.operands if not self.producer(o.p)], []
+        for u in (list(self.gm.graph.nodes) if self.rules.up_codes else []):
+            if u in sliced or self.up_source(u) is None:
+                continue
+            tail, clamp, path = self.forward(u)
+            channels = self.mods[self.up_source(u).target].out_channels
+            codes, scale = self.take_codes(tail, channels, pools=False)
+            if codes and len(codes) == len(tail.users):
+                ups.append(_Codes(u, path, tail, clamp, codes, scale, channels))
+        planned = {pl.p for pl in plans}
+        for u in sliced + [up.node for up in ups]:
+            p = self.up_source(u)
+            if p not in planned:
+                plans.append(_Plan(p, *self.forward(p)[::-1]))   # (path, pre, tail)
+                planned.add(p)
+        return ups
 
-    # rewrite in producer order: a producer's input may be the codes of an earlier one, and a residual its fp32 output
-    g = gm.graph
-    convs = {n for n in g.nodes if producer(n)}                 # before the rewrites give producers a second input
-    edges, adds, modes, observed, watched = [], [], {}, [], {}
-    for pl in plans:
-        p, add, tail, fobs, robs = pl.p, pl.add, pl.tail, pl.obs, pl.robs
+    def skip_identities(self, plans, claimed):
+        """Skip the residual's exact identities once every plan's nodes are `claimed`: a node another plan deletes (say an
+        identity ending its post-add chain) stays the residual, which that plan replaces by its fp32 output."""
+        for pl in plans:
+            if pl.add is None:
+                continue
+            r = pl.robs.args[0] if pl.robs is not None else pl.add.args[pl.ri]
+            while r not in claimed and len(r.users) == 1 and _is_identity(r, self.mods) and isinstance(r.args[0], fx.Node):
+                pl.skipped.append(r)
+                r = r.args[0]
+            pl.r_name = r.name
+
+    def hand_over(self, plan, src, name):
+        """plan's code users read src instead of its tail, its path goes, and its edges are recorded as from `name`."""
+        for v in plan.codes:
+            v.replace_input_with(plan.tail, src)
+            if v in self.convs:
+                self.edges.append((name, v.target, plan.clamp))
+        for node in reversed(plan.path):
+            self.gm.graph.erase_node(node)
+
+    def rewrite_producer(self, pl):
+        g, p, add, tail, fobs, robs = self.gm.graph, pl.p, pl.add, pl.tail, pl.obs, pl.robs
         if add is not None:
             for node in pl.skipped:                             # from the add back: each loses its only user
                 node.replace_all_uses_with(node.args[0])
@@ -2249,23 +2275,22 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None,
             add.prepend(p)
             p.args = (p.args[0], robs.args[0] if robs is not None else add.args[pl.ri])
         fp32 = any(u not in pl.codes for u in tail.users)
-        scale = scheme.out(pl.scale) if pl.codes else None
+        scale = self.scheme.out(pl.scale) if pl.codes else None
         clamp = pl.post if add is not None else pl.pre
-        keys = tuple(None if o is None else _observer_key(o, mods) for o in (fobs, robs))
+        codes_node = y_node = p
         if add is None and not fp32:
-            modes[p.target] = ("requant", (scale,) + tuple(clamp), None)
-            codes_node = y_node = p
+            self.modes[p.target] = dict(requant=(scale,) + tuple(clamp))
         else:
-            modes[p.target] = ("epilogue", Epilogue(scale, pl.pre, pl.post, add is not None, fp32), None)
+            self.modes[p.target] = dict(epilogue=Epilogue(scale, pl.pre, pl.post, add is not None, fp32))
+            keys = tuple(None if o is None else _observer_key(o, self.mods) for o in (fobs, robs))
             if keys != (None, None):
-                watched[p.target] = keys
-            codes_node = y_node = p
+                self.watched[p.target] = keys
             if scale is not None and fp32:
                 codes_node, y_node = _split(g, p)
         for u in pl.codes:
             u.replace_input_with(tail, codes_node)
-            if u in convs:
-                edges.append((p.target, u.target, clamp))
+            if u in self.convs:
+                self.edges.append((p.target, u.target, clamp))
         for node in pl.path:                                    # shape queries inside the chain read p's output
             for u in [u for u in node.users if _shape_query(u, node)]:
                 u.replace_input_with(node, y_node)
@@ -2276,136 +2301,110 @@ def _chain_residual(gm, mods, conv, pool_cat=False, upsample=False, scheme=None,
                 g.erase_node(node)
         else:
             p.replace_all_uses_with(y_node, delete_user_cb=lambda u: u not in (y_node, codes_node))
-        if pl.output:                                           # the views now read the observed output
+        if add is None and fobs is not None:                    # the views now read the observed output
             fobs.replace_all_uses_with(fobs.args[0])
             g.erase_node(fobs)
-            observed.append((fobs.target, "output", p.target))
+            self.observed.append((fobs.target, "output", p.target))
         elif add is not None:
-            observed += [(o.target, what, p.target) for o, what in ((fobs, "operand"), (robs, "residual")) if o is not None]
-        if add is not None:
-            adds.append((p.target, add.name, pl.r_name, pl.pre, pl.post))
+            self.observed += [(o.target, w, p.target) for o, w in ((fobs, "operand"), (robs, "residual")) if o is not None]
+            self.adds.append((p.target, add.name, pl.r_name, pl.pre, pl.post))
 
-    def fuse_upsample(u, scale, clamp, out_slice=None, out=None, operand=None, sums=False):
-        """Turn the upsample node u into a call of its Int8UpsampleBilinear, on its (rewritten) input; under the affine
-        scheme of its AffineInt8UpsampleBilinear: the operand's clamp, its observer, then `clamp` (the cat tail's)."""
-        (size, ac), p = _bilinear_upsample(u, mods, affine), up_source(u)
-        if affine:
-            ob = None if operand["obs"] is None else _observer_key(operand["obs"], mods)
-            mod = AffineInt8UpsampleBilinear(mods[p.target].out_channels, ac, scheme.out(scale), out_slice, operand["pre"], ob,
-                                             clamp, sums, name=u.name)
-        else:
-            mod = Int8UpsampleBilinear(mods[p.target].out_channels, ac, float(scale), clamp, out_slice, name=u.name)
+    def fuse_upsample(self, u, scale, pre, post, out_slice=None, out=None, obs=None, sums=False):
+        """Make u call the scheme's upsample module: clamp pre, observer obs, clamp post, codes at `scale` [into `out`]."""
+        (size, ac), p = _bilinear_upsample(u, self.mods, self.scheme.observers), self.up_source(u)
+        mod = self.scheme.upsample(self.mods[p.target].out_channels, ac, self.scheme.out(scale), out_slice=out_slice,
+                                   pre=pre, obs=None if obs is None else _observer_key(obs, self.mods), post=post,
+                                   sums=sums, name=u.name)
         name = "int8_up_" + u.name
-        gm.add_submodule(name, mod)
-        ups.append((order[u], (u.name, p.target, "slice" if out_slice else "codes", ac)))
+        self.gm.add_submodule(name, mod)
+        self.ups.append((self.order[u], (u.name, p.target, "slice" if out_slice else "codes", ac)))
         u.op, u.target, u.args, u.kwargs = "call_module", name, (u.args[0], size), ({} if out is None else {"out": out})
 
-    # concatenations: the producers write their slices of one buffer in graph order, threaded through `out`
-    cats, ups, slice_sums = [], [], set()
-    for cp in cat_plans:
-        cstride, prev = cp["cstride"], None
-        names = [o["p"].target if producer(o["p"]) else o["p"].name for o in cp["operands"]]
-        for o in sorted(cp["operands"], key=lambda o: order[o["p"]]):
-            q = o["p"]
-            if not producer(q):
-                if affine:
-                    fuse_upsample(q, cp["scale"], cp["clamp"], (o["coff"], cstride), prev, o, cp["sums"])
-                else:
-                    fuse_upsample(q, cp["scale"], o["clamp"], (o["coff"], cstride), prev)
-                prev = q
-                continue
-            if affine:                                          # operand clamp, its observer, the tail's clamp
-                modes[q.target] = ("epilogue", Epilogue(scheme.out(cp["scale"]), o["pre"], cp["clamp"]), (o["coff"], cstride))
-                if o["obs"] is not None:
-                    watched[q.target] = (_observer_key(o["obs"], mods), None)
-                if cp["sums"]:
-                    slice_sums.add(q.target)
+    def rewrite_cat(self, cp):
+        """The writers fill their slices of one buffer in graph order, threaded through `out`."""
+        g, prev = self.gm.graph, None
+        names = [o.p.target if self.producer(o.p) else o.p.name for o in cp.operands]
+        for o in sorted(cp.operands, key=lambda o: self.order[o.p]):
+            q, out_slice = o.p, (o.coff, (cp.channels + 15) // 16 * 16)
+            if not self.producer(q):
+                self.fuse_upsample(q, cp.scale, o.pre, cp.clamp, out_slice, prev, o.obs, cp.sums)
             else:
-                modes[q.target] = ("requant", (float(cp["scale"]),) + tuple(o["clamp"]), (o["coff"], cstride))
-            if prev is not None:
-                q.kwargs = {"out": prev}
+                self.modes[q.target] = dict(self.scheme.slice(self.scheme.out(cp.scale), o.pre, cp.clamp),
+                                            out_slice=out_slice, sums=cp.sums)
+                if o.obs is not None:
+                    self.watched[q.target] = (_observer_key(o.obs, self.mods), None)
+                if prev is not None:
+                    q.kwargs = {"out": prev}
             prev = q
-        for u in cp["codes"]:
-            u.replace_input_with(cp["tail"], prev)
-            if u in convs:
-                edges.append((cp["cat"].name, u.target, cp["clamp"]))
-        for node in reversed(cp["path"]):
-            g.erase_node(node)
-        g.erase_node(cp["cat"])
-        for o, name in zip(cp["operands"], names):
-            if o["obs"] is not None:                            # the operand's observer, now in its writer
-                g.erase_node(o["obs"])
-                observed.append((o["obs"].target, "cat", name))
-            for u, n in o["queries"]:                           # shape queries read the shape off the slice's writer
+        self.hand_over(cp, prev, cp.node.name)
+        g.erase_node(cp.node)
+        for o, name in zip(cp.operands, names):
+            if o.obs is not None:                               # the operand's observer, now in its writer
+                g.erase_node(o.obs)
+                self.observed.append((o.obs.target, "cat", name))
+            for u, n in o.queries:                              # shape queries read the shape off the slice's writer
                 with g.inserting_before(u):
-                    u.replace_input_with(n, g.call_function(_nchw_view, (o["p"], o["channels"])))
-            for node in o["path"]:                              # from the cat back to the producer
+                    u.replace_input_with(n, g.call_function(_nchw_view, (o.p, o.channels)))
+            for node in o.path:                                 # from the cat back to the producer
                 g.erase_node(node)
-        cats.append((cp["cat"].name, names, [o["coff"] for o in cp["operands"]]))
+        self.cats.append((cp.node.name, names, [o.coff for o in cp.operands]))
 
-    # upsamples whose users all take their codes
-    for up in up_plans:
-        if up["mode"] != "codes":
-            continue
-        u = up["node"]
-        fuse_upsample(u, up["scale"], up["clamp"])
-        for v in up["codes"]:
-            v.replace_input_with(up["tail"], u)
-            edges.append((u.name, v.target, up["clamp"]))
-        for node in reversed(up["path"]):
-            g.erase_node(node)
-    ups = [t for _, t in sorted(ups)]
-
-    # pools, last: each reads its input as the rewrites above left it
-    pools = []
-    for pp in sorted(pool_plans, key=lambda pp: order[pp["node"]]):
-        u = pp["node"]
-        k, s, pad, dil, ceil = _max_pool(u, mods)
-        codes_mode = pp["mode"] == "codes"
-        fp32 = not codes_mode
-        out = None if codes_mode else scheme.out(pp["scale"])
-        if affine:                                              # S only for a dense consumer
-            sums = any(v in convs and mods[v.target].groups == 1 for v in pp["codes"])
-            mod = AffineInt8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, out, fp32, sums, name=u.name)
-        else:
-            mod = Int8MaxPool2d(k, s, pad, dil, ceil, pp["channels"], codes_mode, out, fp32, name=u.name)
+    def rewrite_pool(self, pp):
+        """The pool reads its input as the rewrites before it left it; returns its fused_pools record."""
+        g, u = self.gm.graph, pp.node
+        codes_mode = pp.tail is not None
+        sums = any(v in self.convs and self.mods[v.target].groups == 1 for v in pp.codes)   # S only for a dense consumer
+        mod = self.scheme.pool(*_max_pool(u, self.mods), pp.channels, codes_mode,
+                               None if codes_mode else self.scheme.out(pp.scale), not codes_mode, sums=sums, name=u.name)
         name = "int8_pool_" + u.name
-        gm.add_submodule(name, mod)
-        inp = u.args[0]
-        u.op, u.target, u.args, u.kwargs = "call_module", name, (inp,), {}
+        self.gm.add_submodule(name, mod)
+        u.op, u.target, u.args, u.kwargs = "call_module", name, (u.args[0],), {}
         if codes_mode:
-            for v in pp["codes"]:
-                v.replace_input_with(pp["tail"], u)
-            for node in reversed(pp["path"]):
-                g.erase_node(node)
-        else:
-            codes_node, y_node = _split(g, u)
-            for v in pp["codes"]:
-                v.replace_input_with(u, codes_node)
-            u.replace_all_uses_with(y_node, delete_user_cb=lambda x: x not in (y_node, codes_node))
-        for v in pp["codes"]:
-            if v in convs:
-                edges.append((u.name, v.target, pp["clamp"]))
-        pools.append((u.name, pp["mode"], ("codes",) if codes_mode else ("fp32", "codes")))
+            self.hand_over(pp, u, u.name)
+            return u.name, "codes", ("codes",)
+        codes_node, y_node = _split(g, u)
+        for v in pp.codes:
+            v.replace_input_with(u, codes_node)
+        u.replace_all_uses_with(y_node, delete_user_cb=lambda x: x not in (y_node, codes_node))
+        self.edges += [(u.name, v.target, pp.clamp) for v in pp.codes if v in self.convs]
+        return u.name, "fp32", ("fp32", "codes")
 
-    consumers = {q for _, q, _ in edges}
-    dense = {p for p, q, _ in edges if mods[q].groups == 1}          # producers whose codes a dense consumer reads
-    for target in modes.keys() | consumers:
-        kind, arg, out_slice = modes.get(target, (None, None, None))
-        mod = mods[target].chained(codes_in=target in consumers, name=target, requant=arg if kind == "requant" else None,
-                                   epilogue=arg if kind == "epilogue" else None, out_slice=out_slice,
-                                   sums=target in dense or target in slice_sums)
-        _set_module(gm, target, mod.observe(*watched[target]) if target in watched else mod)
-    g.lint()
-    gm.recompile()
-    gm.requantized_edges = edges
-    gm.fused_adds = adds
-    if scheme is _AFFINE:
-        gm.fused_observers = observed
-    if pool_cat:
-        gm.fused_cats = cats
-    if pool_cat or pool:
-        gm.fused_pools = pools
-    if upsample:
-        gm.fused_upsamples = ups
-    return gm
+    def run(self):
+        plans, cats = self.plan_producers(), self.plan_cats()
+        self.plan_observers(plans, cats)
+        ups = self.plan_upsamples(plans, cats)
+        plans.sort(key=lambda pl: self.order[pl.p])
+        self.skip_identities(plans, {n for plan in (*plans, *cats, *self.pools, *ups) for n in plan.nodes()})
+        # rewrite in producer order (a producer's input may be the codes of an earlier one, and a residual its fp32
+        # output), then the concatenations, the codes-mode upsamples and, last, the pools
+        gm, g, mods = self.gm, self.gm.graph, self.mods
+        for pl in plans:
+            self.rewrite_producer(pl)
+        for cp in cats:
+            self.rewrite_cat(cp)
+        for up in ups:
+            self.fuse_upsample(up.node, up.scale, up.clamp, _FULL)
+            self.hand_over(up, up.node, up.node.name)
+        pools = [self.rewrite_pool(pp) for pp in sorted(self.pools, key=lambda pp: self.order[pp.node])]
+        consumers = {q for _, q, _ in self.edges}
+        dense = {p for p, q, _ in self.edges if mods[q].groups == 1}   # producers whose codes a dense consumer reads
+        for target in self.modes.keys() | consumers:
+            kw = self.modes.get(target, {})
+            mod = mods[target].chained(codes_in=target in consumers, name=target,
+                                       **dict(kw, sums=target in dense or kw.get("sums", False)))
+            _set_module(gm, target, mod.observe(*self.watched[target]) if target in self.watched else mod)
+        g.lint()
+        gm.recompile()
+        if self.rules.heads:
+            gm.fused_heads, observed = _fuse_heads(gm, self.conv, mods, self.scheme)
+            self.observed += observed
+        gm.requantized_edges, gm.fused_adds = self.edges, self.adds
+        if self.scheme.observers:
+            gm.fused_observers = self.observed
+        if self.rules.cats:
+            gm.fused_cats = self.cats
+        if self.rules.cats or self.rules.pools:
+            gm.fused_pools = pools
+        if self.rules.up_slices:
+            gm.fused_upsamples = [t for _, t in sorted(self.ups)]
+        return gm
