@@ -18,7 +18,8 @@ are not the fp32 weights the int8 codes are made from.  The observers replace_op
 tensors between converted layers stay fp32.
 
 convert_affine executes the reference's own quantization instead (asymmetric per-tensor min / max, dfq_i8_affine_*): called
-AFTER quantize_targ_layer and the activation ranges, it recovers the weight codes from the fake-quantized weights and
+AFTER quantize_targ_layer and the activation ranges, it recovers the weight codes from the fake-quantized weights (of a
+QConv2d / QuantConv2d layer: the weights its forward quantizes on the GPU, the --distill_range and --trainable states) and
 computes each layer from integer sums, equal to the fake-quantized layer up to fp32 rounding.  chain_affine carries its codes
 between layers; in the reference's evaluation state (replace_op() active with a CustomTensorOP) it replays the functional-op
 observers into its graph and runs those on a producer's path in that producer's epilogue (dfq_i8_affine_conv_observed), so it
@@ -794,15 +795,18 @@ def _affine_refusal(who, C_in, C_out, groups, kernel_size, act_bits, w_bits):
 
 
 class AffineInt8Conv2d(_AffineInt8Layer):
-    """A fake-quantized nn.Conv2d (QuantNConv2d after quantize_targ_layer) executed in integer arithmetic."""
+    """A fake-quantized nn.Conv2d (QuantNConv2d after quantize_targ_layer, or a QConv2d / QuantConv2d) executed in integer
+    arithmetic."""
 
     @classmethod
-    def from_conv(cls, conv: nn.Conv2d, act_min, act_max, act_bits=8, w_bits=8, name=None):
+    def from_conv(cls, conv: nn.Conv2d, act_min, act_max, act_bits=8, w_bits=8, name=None, weight=None, bias=None):
+        """weight / bias: the fake-quantized tensors to run in place of conv's own (those a per-forward layer convolves
+        with); None: conv.weight, conv.bias."""
         err = _zero_padding_refusal(conv, "layer %s: " % name)
         if err is not None:
             raise err
-        return cls(conv.weight, conv.bias, act_min, act_max, act_bits, w_bits, conv.stride, conv.padding, conv.dilation,
-                   conv.groups, name=name)
+        return cls(conv.weight if weight is None else weight, conv.bias if bias is None else bias, act_min, act_max,
+                   act_bits, w_bits, conv.stride, conv.padding, conv.dilation, conv.groups, name=name)
 
     def forward(self, x, r=None, out=None, off=0):
         return self.run(x, residual=r, out=out, off=off)[0]
@@ -812,9 +816,11 @@ class AffineInt8Linear(_AffineInt8Layer):
     """A fake-quantized nn.Linear executed in integer arithmetic: the 1x1 convolution of [B, I, 1, 1]."""
 
     @classmethod
-    def from_linear(cls, lin: nn.Linear, act_min, act_max, act_bits=8, w_bits=8, name=None):
-        return cls(lin.weight.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias, act_min, act_max, act_bits, w_bits,
-                   name=name)
+    def from_linear(cls, lin: nn.Linear, act_min, act_max, act_bits=8, w_bits=8, name=None, weight=None, bias=None):
+        """weight / bias: as AffineInt8Conv2d.from_conv."""
+        w = lin.weight if weight is None else weight
+        return cls(w.reshape(lin.out_features, lin.in_features, 1, 1), lin.bias if bias is None else bias, act_min, act_max,
+                   act_bits, w_bits, name=name)
 
     forward = _ConvLayer._linear_forward
 
@@ -1097,17 +1103,26 @@ def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
     in place, by an AffineInt8Conv2d / AffineInt8Linear that computes it in integer arithmetic under the reference's own
     quantization (asymmetric per-tensor min / max, include/dfq_b200.h dfq_i8_affine_*); returns the names in graph order.
 
-    Call it in the reference's inference state: after quantize_targ_layer(graph, bits_weight, ...) and the activation ranges
-    (set_quant_minmax or update_quant_range).  Activation ranges and bits come from each layer's `quant` observer
-    (running_min, running_max, num_bits) and are frozen here: an observer left with a truthy update_stat keeps widening its
-    range in the fake-quantized model (set_layer_bits does this through quirk Q1), the converted layer does not.  The
-    weight codes are recovered from the fake-quantized weights: mw = min(weight), fw an fp32 scale near
-    (max - min) / (2^bits_weight - 1) whose round trip fp32(fp32(q fw) + mw) reproduces every weight bit for bit (checked on
-    the device).  The result agrees with the fake-quantized layer to fp32 rounding of its sum, not bit for bit.
+    Call it in one of the reference's inference states, after the activation ranges (set_quant_minmax or
+    update_quant_range):
+      - QuantNConv2d / QuantNLinear (the default --quantize state), after quantize_targ_layer(graph, bits_weight, ...): the
+        weights and biases are the layers' own, fake-quantized offline;
+      - QConv2d / QLinear (--distill_range) or QuantConv2d / QuantLinear (--trainable), which quantize their weights and
+        bias on every forward: the weights are _quant_param_per_forward(weight, layer.num_bits) and the bias
+        quantize(bias, num_bits=layer.num_bits_bias) (the implicit-range path, at 32 bits too), both computed on the GPU
+        as the forward computes them there.  The layer states its weight bits: layer.num_bits must equal bits_weight.  A
+        layer carrying learned scales (scale / scale_prev of set_scale) is refused; merge_scale_to_weight merges them.
+    Activation ranges and bits come from each layer's `quant` observer (running_min, running_max, num_bits) and are frozen
+    here: an observer left with a truthy update_stat keeps widening its range in the fake-quantized model (set_layer_bits
+    does this through quirk Q1), the converted layer does not.  The weight codes are recovered from the fake-quantized
+    weights: mw = min(weight), fw an fp32 scale near (max - min) / (2^bits_weight - 1) whose round trip
+    fp32(fp32(q fw) + mw) reproduces every weight bit for bit (checked on the device).  The result agrees with the
+    fake-quantized layer to fp32 rounding of its sum, not bit for bit.  The original layers' parameters are not modified.
 
     Every layer is checked and packed before any is replaced: a layer that cannot run (grouping, padding mode, bits above 8,
-    K = kh * kw * C / groups >= 131072, no observer, a non-finite range) or whose weights are not on such a grid raises
-    DfqError naming it, and the model is left as it was."""
+    K = kh * kw * C / groups >= 131072, no observer, a non-finite range, a per-forward layer's bits other than bits_weight
+    or learned scales) or whose weights are not on such a grid raises DfqError naming it, and the model is left as it
+    was."""
     layers = [graph[k] for k in graph if type(graph[k]) in targ_type]
     names = {id(m): n for n, m in model.named_modules()}
     plan = []
@@ -1128,17 +1143,42 @@ def convert_affine(model: nn.Module, graph, targ_type, bits_weight=8):
         else:
             raise _lib.DfqError("layer %s (%s) cannot run in int8: needs a Conv2d or a Linear" % (name, type(layer).__name__))
         _affine_refusal(name, *shape, quant.num_bits, bits_weight)
+        weight, bias = _per_forward_params(layer, name, bits_weight)
         plan.append((name, layer, float(quant.running_min.reshape(-1)[0]), float(quant.running_max.reshape(-1)[0]),
-                     quant.num_bits))
+                     quant.num_bits, weight, bias))
     new = []
-    for name, layer, lo, hi, bits in plan:
+    for name, layer, lo, hi, bits, weight, bias in plan:
         if isinstance(layer, nn.Conv2d):
-            new.append(AffineInt8Conv2d.from_conv(layer, lo, hi, bits, bits_weight, name=name))
+            new.append(AffineInt8Conv2d.from_conv(layer, lo, hi, bits, bits_weight, name=name, weight=weight, bias=bias))
         else:
-            new.append(AffineInt8Linear.from_linear(layer, lo, hi, bits, bits_weight, name=name))
+            new.append(AffineInt8Linear.from_linear(layer, lo, hi, bits, bits_weight, name=name, weight=weight, bias=bias))
     for (name, *_), mod in zip(plan, new):
         _set_module(model, name, mod)
     return [name for name, *_ in plan]
+
+
+def _per_forward_params(layer, name, bits_weight):
+    """(weight, bias) a QConv2d / QLinear / QuantConv2d / QuantLinear convolves with, on the GPU: its forward's
+    _quant_param_per_forward(weight, num_bits) and quantize(bias, num_bits=num_bits_bias) (None without a bias), computed
+    from copies of its parameters; (None, None) for any other layer (a QuantN* layer runs its own weight and bias).
+    DfqError naming the layer when its num_bits is not bits_weight or it carries learned scales that its forward merges
+    into the weights first (a QConv2d / QLinear after set_scale)."""
+    from .utils import quantize as Q
+    if not isinstance(layer, (Q.QConv2d, Q.QLinear, Q.QuantConv2d, Q.QuantLinear)):
+        return None, None
+    if isinstance(layer, (Q.QConv2d, Q.QLinear)) and (getattr(layer, "scale", None) is not None or
+                                                      getattr(layer, "scale_prev", None) is not None):
+        raise _lib.DfqError("layer %s carries learned scales (scale / scale_prev of set_scale): merge them into its weights "
+                            "first (merge_scale_to_weight)" % name)
+    if layer.num_bits != bits_weight:
+        raise _lib.DfqError("layer %s quantizes its weights to %r bits on every forward, not bits_weight = %r"
+                            % (name, layer.num_bits, bits_weight))
+    dev = engine._default_device()
+    with torch.no_grad():
+        weight = Q._quant_param_per_forward(layer.weight.detach().to(dev, copy=True), layer.num_bits)
+        bias = None if layer.bias is None else Q.quantize(layer.bias.detach().to(dev, copy=True),
+                                                          num_bits=layer.num_bits_bias)
+    return weight, bias
 
 
 def _set_module(root, name, mod):

@@ -27,7 +27,10 @@ epilogues; the two affine arms' logits asserted bit-identical.  `affine_pool_hea
 ResNet-18 and GoogLeNet in that state, per-layer against chain_affine(residual=True[, concat=True]) and the same with
 pools=True (max pools carried as affine codes), and SSD-Lite at 300x300 against chain_affine(residual=True, concat=True,
 fold_pads=True) and the same with heads=True (detection heads written in place), outputs asserted bit-identical, with
-the fp32 bytes the flags avoid.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
+the fp32 bytes the flags avoid.  `affine_distilled` (only when asked for): MobileNetV2 and ResNet-18 in the reference's
+--distill_range state (tests/affine_distilled_state.py: QConv2d / QLinear, which re-quantize every weight and bias on each
+forward), timing the fake-quantized model, the per-layer convert_affine model and chain_affine(residual=True), the two
+affine arms' logits asserted bit-identical.  The card's name and power limit are read in the same run and reported beside the numbers.  Needs a CUDA
 device; writes nothing.
 """
 import argparse
@@ -794,6 +797,62 @@ def affine_observed_inference(dev, reps=10, batch=256, rounds=5):
     return out
 
 
+def affine_distilled_inference(dev, reps=10, batch=256, rounds=5):
+    """MobileNetV2 (the reference's mean head) and ResNet-18 in the reference's --distill_range state
+    (tests/affine_distilled_state.py: QConv2d / QLinear, which quantize their weights and bias on every forward, ranges from
+    update_quant_range, replace_op() active): the fake-quantized model, convert_affine per layer and
+    chain_affine(residual=True), timed alternately, `rounds` rounds of `reps` passes, median; bit-identity of the two
+    affine arms' logits (asserted)."""
+    import copy
+    import statistics
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import affine_distilled_state
+    from dfq_b200 import int8
+
+    def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            fn()
+        e1.record(); e1.synchronize()
+        return e0.elapsed_time(e1) / reps
+
+    prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    out = {"batch": batch, "image": "3x224x224", "unit": "images/s", "reps": reps, "rounds": rounds}
+    try:
+        for net in ("mobilenet_v2", "resnet18"):
+            x = affine_distilled_state.inputs(net, batch, 224, torch.Generator(device=dev).manual_seed(3))
+            with affine_distilled_state.distilled_state(net) as (model, qgraph, qtarg):
+                fq = copy.deepcopy(model)
+                int8.convert_affine(model, qgraph, qtarg)
+                gm = int8.chain_affine(model, residual=True)
+                arms = (("fake_quant", fq), ("affine_per_layer", model), ("affine_chained", gm))
+                with torch.no_grad():
+                    same = bool(torch.equal(model(x).view(torch.int32), gm(x).view(torch.int32)))
+                    assert same, net
+                    for _ in range(2):
+                        for _, m in arms:
+                            m(x)
+                    torch.cuda.synchronize(dev)
+                    ms = {k: [] for k, _ in arms}
+                    for _ in range(rounds):
+                        for k, m in arms:
+                            ms[k].append(timed(lambda m=m: m(x)))
+                med = {k: statistics.median(v) for k, v in ms.items()}
+                out[net] = {"images_per_s": {k: batch / (v * 1e-3) for k, v in med.items()}, "ms_per_batch": med,
+                            "ms_per_batch_rounds": ms, "observers": model.custom_tensor_op.len,
+                            "fused_observers": len(gm.fused_observers), "fused_adds": len(gm.fused_adds),
+                            "logits_bit_identical_to_per_layer": same}
+                del fq, gm
+            del model
+            torch.cuda.empty_cache()
+    finally:
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = prev
+    return out
+
+
 def affine_layout_inference(dev, reps=10, batch=8, rounds=5, size=513):
     """DeepLab-v3+ (tests/deeplab_mobilenet_padded.py) in the reference's evaluation state at batch x 3 x size x size:
     convert_affine per layer, chain_affine(residual=True) and chain_affine(residual=True, concat=True, fold_pads=True),
@@ -1002,7 +1061,7 @@ def main():
     p.add_argument("--ssd-batch", type=int, default=256, help="batch of the 300x300 SSD-Lite (layout)")
     p.add_argument("--sections", default="int8,chained,residual,pool_cat,upsample,layout",
                    help="comma-separated sections to run (default: all but affine, affine_chained, affine_observed, "
-                        "affine_layout and affine_pool_heads)")
+                        "affine_layout, affine_pool_heads and affine_distilled)")
     args = p.parse_args()
     want = set(args.sections.split(","))
     import torch
@@ -1031,6 +1090,8 @@ def main():
     if "affine_pool_heads" in want:
         res["affine_pool_heads"] = affine_pool_heads_inference(dev, reps=args.reps, batch=args.batch,
                                                                ssd_batch=args.ssd_batch)
+    if "affine_distilled" in want:
+        res["affine_distilled"] = affine_distilled_inference(dev, reps=args.reps, batch=args.batch)
     res["gpu"] = card()
     print(json.dumps({"int8": res}))
 
