@@ -27,6 +27,9 @@ computes what the per-layer model computes under the patched ops.  chain_affine(
 pads into the convolutions after them as pad codes and has the producers and bilinear upsamples of channel concatenations
 write the consumer's codes directly (dfq_i8_affine_conv_layout, dfq_i8_affine_upsample_bilinear), and
 chain_affine(pools=True) carries the codes through max pools (dfq_i8_affine_maxpool).
+
+save / load write a chained model of either scheme to one file and rebuild it, in any process, from dfq_b200 alone
+(dfq_b200/int8_io.py).
 """
 import collections
 import ctypes as C
@@ -148,17 +151,22 @@ class _ConvLayer(nn.Module):
         return self.layer_name or "%s(%d, %d, kernel_size=%s)" % (type(self).__name__, self.in_channels, self.out_channels,
                                                                   self.kernel_size)
 
+    @classmethod
+    def _build(cls, attrs, buffers):
+        """A module of this class with the given attributes on the given buffers, nothing packed: the one route by which
+        chained copies (_copy) and loaded layers (int8.load) are made."""
+        new = cls.__new__(cls)
+        nn.Module.__init__(new)
+        for k, v in attrs.items():
+            setattr(new, k, v)
+        for k, b in buffers.items():
+            new.register_buffer(k, b)
+        return new
+
     def _copy(self, codes_in, name):
         """A new module of the same class on the same buffers, with the attributes in _copied, codes_in and name."""
-        new = type(self).__new__(type(self))
-        nn.Module.__init__(new)
-        for k in self._copied:
-            setattr(new, k, getattr(self, k))
-        for k, b in self._buffers.items():
-            new.register_buffer(k, b)
-        new.codes_in = bool(codes_in)
-        new.layer_name = name
-        return new
+        return self._build(dict({k: getattr(self, k) for k in self._copied}, codes_in=bool(codes_in), layer_name=name),
+                           self._buffers)
 
     def _check_residual(self, residual):
         if (residual is not None) != bool(self.epilogue and self.epilogue.residual):
@@ -232,6 +240,7 @@ class _Int8Layer(_ConvLayer):
     requant = None
     rows = False
     _copied = _ConvLayer._copied + ("act_scale",)
+    _modes = ("codes_in", "layer_name", "requant", "epilogue", "out_slice", "rows")     # what chained() sets
 
     def __init__(self, weight, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
         super().__init__(weight, stride, padding, dilation, groups)
@@ -488,6 +497,8 @@ class _AffineInt8Layer(_ConvLayer):
     rows = False
     pad_code = None
     _copied = _ConvLayer._copied + ("act_bits", "w_bits", "act_min", "act_max", "w_min", "w_scale", "constants", "pad_code")
+    # what chained() and observe() set
+    _modes = ("codes_in", "layer_name", "epilogue", "sums", "out_slice", "rows", "observers", "tail_observer")
 
     def __init__(self, weight, bias, act_min, act_max, act_bits=8, w_bits=8, stride=1, padding=0, dilation=1, groups=1,
                  name=None):
@@ -1793,6 +1804,33 @@ def chain_affine(model: nn.Module, concrete_args=None, residual=False, concat=Fa
     return gm
 
 
+def save(gm: fx.GraphModule, path):
+    """Write a chained int8 model - the GraphModule chain_int8 / chain_affine returned, with any flags - to the file `path`,
+    for load() in another process: the graph as a node list, each layer's packed codes, tables, ranges and execution modes,
+    each shared buffer once, and the chain's records (requantized_edges, fused_*, folded_pads).  One torch.save of plain
+    containers and CPU tensors (dfq_b200/int8_io.py has the format).  A per-layer model is not taken: save
+    chain_int8(model) / chain_affine(model) with no flags, which computes the same bit for bit.  A graph calling a function,
+    tensor method or module type outside the allowlist of what the chains emit (a user function, a module class of the
+    model's own) raises DfqError naming it, before anything is written; the file appears whole or not at all, and gm is
+    not modified."""
+    from . import int8_io
+    int8_io.save(gm, path)
+
+
+def load(path, device=None) -> fx.GraphModule:
+    """The chained model save() wrote, rebuilt on the current CUDA device from its stored state, computing what the saved
+    model computed, bit for bit, with its records; nothing is repacked.  No code from the file runs: it is read with
+    torch.load(weights_only=True), every target and module type is checked against save()'s allowlist, and every name the
+    generated forward spells as code (node names, parameters, module paths, keywords, dict keys) must be an identifier (or
+    an index in a path).  Each layer's buffers must fit its stored geometry.  It needs dfq_b200 alone: not the model's
+    classes, the reference's layers or replace_op().  device: None or the current CUDA device - the layers launch on the
+    current device's stream, so load and run a model for another GPU inside `with torch.cuda.device(...)`; any other
+    device is refused.  A file of another format or version, with a missing key or failing a check raises DfqError, as
+    does a machine without a CUDA device."""
+    from . import int8_io
+    return int8_io.load(path, device)
+
+
 class _Scheme(NamedTuple):
     """What the chaining rules need of one integer scheme: `layer`, the convolution class whose edges they fuse; key(m),
     what decides the codes layer m reads, compared bit for bit by same(a, b) (consumers with equal keys read identical
@@ -1947,8 +1985,11 @@ def _unpatch_adds(gm, LT):
 
 
 def _raw(table, name):
+    """The unpatched op: the one replace_op() saved, or the live one when replace_op() never ran in this process (a
+    chained model loaded by int8.load)."""
     from .utils import layer_transform as LT
-    return getattr(LT, table)[name]
+    op = getattr(LT, table).get(name)
+    return op if op is not None else getattr(torch if table == "raw_torch_op" else F, name)
 
 
 def _raw_cat(*a, **k):
