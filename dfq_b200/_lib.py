@@ -120,6 +120,10 @@ I8_AFFINE_ROWS_DT = np.dtype([("y", np.uint64), ("off", np.int64), ("img_stride"
                              [("obs_bits", np.int32), ("tail_min", np.float32), ("tail_max", np.float32),
                               ("tail_bits", np.int32)], align=True)
 
+SSD_NMS_DT = np.dtype([(f, np.int32) for f in ("N", "P", "C", "prior_batch")] +
+                      [(f, np.float32) for f in ("center_variance", "size_variance", "prob_threshold", "iou_threshold")] +
+                      [("candidate_size", np.int32), ("top_k", np.int32)], align=True)
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -129,6 +133,7 @@ EXPECTED_SIZES = {
     "DfqI8Affine": (I8_AFFINE_DT, 32), "DfqI8AffineEpilogue": (I8_AFFINE_EPILOGUE_DT, 64),
     "DfqI8AffineObserve": (I8_AFFINE_OBSERVE_DT, 24), "DfqI8AffineLayout": (I8_AFFINE_LAYOUT_DT, 20),
     "DfqI8AffineResize": (I8_AFFINE_RESIZE_DT, 76), "DfqI8AffineRows": (I8_AFFINE_ROWS_DT, 64),
+    "DfqSsdNms": (SSD_NMS_DT, 40),
 }
 
 _PF = C.c_void_p   # device float*
@@ -198,6 +203,9 @@ SIGNATURES = {
     "dfq_i8_affine_conv_rows": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p, C.c_void_p,
                                 _ST],
     "dfq_i8_affine_maxpool": [C.c_void_p, _PF, _PF, C.c_void_p, C.c_void_p, C.c_float, C.c_float, _I32, C.c_void_p, _ST],
+    "dfq_ssd_decode": [_PF, _PF, _PF, C.c_void_p, _ST],
+    "dfq_ssd_nms": [_PF, _PF, _PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_ssd_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -486,6 +486,7 @@ extern "C" int dfq_struct_size(int which) {
     case 15: return (int)sizeof(DfqI8AffineLayout);
     case 16: return (int)sizeof(DfqI8AffineResize);
     case 17: return (int)sizeof(DfqI8AffineRows);
+    case 18: return (int)sizeof(DfqSsdNms);
     default: return -1;
   }
 }

@@ -45,7 +45,7 @@ const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
- * 16 DfqI8AffineResize, 17 DfqI8AffineRows): lets a binding verify
+ * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -717,6 +717,46 @@ int dfq_i8_affine_conv_rows(const int8_t* xq, const int32_t* S_in, const int8_t*
  * out_bits < 1.  DFQ_E_UNSUPPORTED: out_bits > 8 in that case.  Nothing is written when a call is refused. */
 int dfq_i8_affine_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq, int32_t* S, float out_min, float out_max,
                           int32_t out_bits, const DfqI8Pool* g, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * SSD post-processing (modeling/detection/predictor.py Predictor.predict, utils/detection/box_utils.py) for a batch
+ * ------------------------------------------------------------------------------------------- */
+typedef struct DfqSsdNms {
+  int32_t N, P, C;               /* images, priors, classes (class 0 is the background)                               */
+  int32_t prior_batch;           /* priors [prior_batch, P, 4]: 1 (shared by every image) or N                        */
+  float center_variance, size_variance;
+  float prob_threshold;          /* candidates: score > prob_threshold (strict: NaN never is one)                     */
+  float iou_threshold;           /* a remaining box is kept while iou_of(box, picked) <= iou_threshold                */
+  int32_t candidate_size;        /* the best candidate_size candidates of a class enter NMS, 1 .. 1024                */
+  int32_t top_k;                 /* > 0: at most top_k picks per class; <= 0: no limit                                */
+} DfqSsdNms;
+/* convert_locations_to_boxes + center_form_to_corner_form, bit for bit torch's CUDA ops: per (image n, prior p), with
+ * l = locations[n, p], q = priors[prior_batch == 1 ? 0 : n, p] (centre form), every op rounded to fp32 in this order:
+ *   cx = (l0 * cv) * q2 + q0,  cy = (l1 * cv) * q3 + q1,  w = expf(l2 * sv) * q2,  h = expf(l3 * sv) * q3
+ *   boxes[n, p] = (cx - w / 2, cy - h / 2, cx + w / 2, cy + h / 2)
+ * locations and boxes fp32 [N, P, 4].  Reads N, P, prior_batch and the variances of *d.  DFQ_E_ARG, with a reason: d
+ * NULL, N or P < 1, prior_batch neither 1 nor N, a NULL or not 16-byte aligned pointer. */
+int dfq_ssd_decode(const float* locations, const float* priors, float* boxes, const DfqSsdNms* d, void* stream);
+/* Per (image n, class c = 1 .. C-1) of scores fp32 [N, P, C] and the decoded boxes fp32 [N, P, 4]: the candidates
+ * (score > prob_threshold) ordered by score descending, -0.0 equal to +0.0, ties broken by the lower prior index (the
+ * reference's CPU sort is not stable; this is the one place the result may differ from it); the first candidate_size of
+ * them; then box_utils.hard_nms: pick the first remaining, stop once top_k > 0 picks are made, drop every remaining box r
+ * with !(iou_of(r, picked) <= iou_threshold), iou_of in the reference's fp32 op order with NaN-propagating max, min and
+ * clamp.  Writes, for segment s = n * (C - 1) + c - 1, its picks in pick order to slot_boxes fp32 [N * (C - 1),
+ * candidate_size, 4] and slot_probs [N * (C - 1), candidate_size] (the candidates' scores), their number to counts[s]
+ * (int32 [N * (C - 1)]), and the exclusive scan of counts to offsets (int64 [N * (C - 1) + 1]; offsets[n * (C - 1)] is
+ * where image n starts in the flat output, the last entry the total).  DFQ_E_ARG, with a reason: the refusals of
+ * dfq_ssd_decode, C < 2, candidate_size < 1, boxes or slot_boxes not 16-byte aligned.  DFQ_E_UNSUPPORTED: candidate_size
+ * above 1024, N * (C - 1) above INT32_MAX. */
+int dfq_ssd_nms(const float* scores, const float* boxes, float* slot_boxes, float* slot_probs, int32_t* counts,
+                int64_t* offsets, const DfqSsdNms* d, void* stream);
+/* The flat output of the picks dfq_ssd_nms left in the slots, what Predictor.predict returns for each image in turn:
+ * out_boxes fp32 [T, 4] (times (w, h, w, h) of image_sizes fp32 [N, 2] = (width, height) per image, unscaled when
+ * image_sizes is NULL), out_labels int64 [T] = c, out_probs fp32 [T]; T = offsets[N * (C - 1)].  Classes ascending, picks
+ * in pick order.  Refusals of dfq_ssd_nms, and DFQ_E_ARG for a NULL output or out_boxes not 16-byte aligned. */
+int dfq_ssd_compact(const float* slot_boxes, const float* slot_probs, const int32_t* counts, const int64_t* offsets,
+                    const float* image_sizes, float* out_boxes, int64_t* out_labels, float* out_probs, const DfqSsdNms* d,
+                    void* stream);
 
 #ifdef __cplusplus
 }

@@ -19,7 +19,10 @@ build container.  Committed next to its outputs so every fixture can be regenera
   ref_live_pins.npz       the reference's _layer_equalization, replace_op forward and getDistilData on the inputs of the
                           pin tests (tests/test_oracle_pins.py, test_op_patching.py, test_distill.py)
 
+  ref_ssd_postprocess.npz the reference's Predictor.predict post-processing on seeded SSD-Lite-shaped outputs
+
 usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
+       [ssd_post]
 """
 import hashlib
 import json
@@ -372,3 +375,60 @@ def live_pins():
 
 if __name__ == "__main__" and "live" in sys.argv[1:]:
     live_pins()
+
+
+# ---------------------------------------------------------------------------------------------------------
+SSD_POST_CONFIGS = [(-1, 200), (1, 200), (5, 200), (-1, 1)]     # (top_k, candidate_size)
+
+
+def ssd_postprocess():
+    """The reference's Predictor.predict post-processing (box_utils decode, threshold, sort, hard_nms, scaling) run on
+    seeded SSD-Lite-shaped outputs with the priors of mobilenetv1_ssd_config (3,000 x 4), for each (top_k, candidate_size)
+    of SSD_POST_CONFIGS.  Image 0 has a class without candidates, image 2 no detection at all; no class has tied scores,
+    so the unstable sort does not decide anything."""
+    from modeling.detection.config import mobilenetv1_ssd_config as cfg
+    from modeling.detection.predictor import Predictor
+    priors = cfg.priors.float().contiguous()
+    P, C = priors.shape[0], 21
+    g = torch.Generator().manual_seed(7)
+    logits = torch.randn(3, P, C, generator=g) * 2.5
+    logits[..., 0] += 5.0
+    logits[0, :, 5] -= 30.0                       # no candidate of class 5 in image 0
+    logits[1, :, 1:] *= 1.6                       # a peakier image
+    logits[2, :, 0] += 40.0                       # nothing above the threshold
+    scores = torch.softmax(logits, dim=2)
+    locations = torch.randn(3, P, 4, generator=g) * 0.7
+    sizes = np.array([[300, 300], [640, 480], [333, 500]], np.int64)
+    for n in range(3):
+        for c in range(1, C):
+            s = scores[n, :, c]
+            assert torch.unique(s[s > 0.01]).numel() == int((s > 0.01).sum()), "tied scores"
+
+    class Outputs(nn.Module):
+        def forward(self, x):
+            return self.scores, (self.locations, priors, cfg.center_variance, cfg.size_variance)
+
+    net = Outputs()
+    out = dict(scores=scores.numpy(), locations=locations.numpy(), priors=priors.numpy(), image_sizes=sizes,
+               variances=np.array([cfg.center_variance, cfg.size_variance]), prob_threshold=np.array(0.01),
+               iou_threshold=np.array(cfg.iou_threshold), configs=np.array(SSD_POST_CONFIGS))
+    for k, (top_k, cand) in enumerate(SSD_POST_CONFIGS):
+        pred = Predictor(net, cfg.image_size, cfg.image_mean, cfg.image_std, iou_threshold=cfg.iou_threshold,
+                         candidate_size=cand, device=torch.device("cpu"))
+        boxes, labels, probs, offs = [], [], [], [0]
+        for n in range(3):
+            net.scores, net.locations = scores[n:n + 1], locations[n:n + 1]
+            w, h = (int(v) for v in sizes[n])
+            b, l, p = pred.predict(np.zeros((h, w, 3), np.uint8), top_k=top_k, prob_threshold=0.01)
+            boxes.append(b.reshape(-1, 4)); labels.append(l.reshape(-1).long()); probs.append(p.reshape(-1))
+            offs.append(offs[-1] + b.shape[0])
+        out["boxes_%d" % k] = torch.cat(boxes).numpy()
+        out["labels_%d" % k] = torch.cat(labels).numpy()
+        out["probs_%d" % k] = torch.cat(probs).numpy()
+        out["offsets_%d" % k] = np.array(offs)
+        print("ssd postprocess top_k %d candidate_size %d: kept per image %s" % (top_k, cand, np.diff(offs).tolist()))
+    np.savez_compressed(os.path.join(GOLD, "ref_ssd_postprocess.npz"), **out)
+
+
+if __name__ == "__main__" and "ssd_post" in sys.argv[1:]:
+    ssd_postprocess()
