@@ -124,6 +124,12 @@ SSD_NMS_DT = np.dtype([(f, np.int32) for f in ("N", "P", "C", "prior_batch")] +
                       [(f, np.float32) for f in ("center_variance", "size_variance", "prob_threshold", "iou_threshold")] +
                       [("candidate_size", np.int32), ("top_k", np.int32)], align=True)
 
+SEG_ARGMAX_DT = np.dtype([(f, np.int32) for f in ("N", "C", "H", "W", "OH", "OW", "align_corners", "label_type")],
+                         align=True)
+SEG_LABEL_U8, SEG_LABEL_I64, SEG_LABEL_F32 = 0, 1, 2
+# DfqSegArgmax is struct-size index 19, checked on its own: EXPECTED_SIZES stays the table of indices 0 .. 18
+SEG_ARGMAX_INDEX, SEG_ARGMAX_SIZE = 19, 32
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -206,6 +212,7 @@ SIGNATURES = {
     "dfq_ssd_decode": [_PF, _PF, _PF, C.c_void_p, _ST],
     "dfq_ssd_nms": [_PF, _PF, _PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_ssd_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, _ST],
+    "dfq_seg_argmax": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -487,6 +487,7 @@ extern "C" int dfq_struct_size(int which) {
     case 16: return (int)sizeof(DfqI8AffineResize);
     case 17: return (int)sizeof(DfqI8AffineRows);
     case 18: return (int)sizeof(DfqSsdNms);
+    case 19: return (int)sizeof(DfqSegArgmax);
     default: return -1;
   }
 }

@@ -1349,10 +1349,11 @@ def _orig(name):
     return LT.raw_torch_op.get(name) or LT.raw_func_op.get(name)
 
 
-def _bilinear_upsample(node, mods, raw=False):
+def _bilinear_upsample(node, mods, raw=False, wrapped=False):
     """(size, align_corners) of an F.interpolate / nn.Upsample node that resizes one fx node bilinearly to a given size:
     mode 'bilinear', size a pair of ints or a traced value, align_corners True or False, no scale_factor,
-    recompute_scale_factor or antialias; None otherwise.  raw: the unpatched F.interpolate counts too (_orig)."""
+    recompute_scale_factor or antialias; None otherwise.  raw: the unpatched F.interpolate counts too (_orig).  wrapped:
+    _raw_interpolate counts too (what chain_affine and load leave in a graph; the chaining rules never see it)."""
     if not node.args or not isinstance(node.args[0], fx.Node):
         return None
     if node.op == "call_module" and type(mods[node.target]) is nn.Upsample:
@@ -1360,7 +1361,8 @@ def _bilinear_upsample(node, mods, raw=False):
         if len(node.args) != 1 or node.kwargs:
             return None
         size, sf, mode, ac, rsf, aa = m.size, m.scale_factor, m.mode, m.align_corners, m.recompute_scale_factor, False
-    elif node.op == "call_function" and (node.target is F.interpolate or (raw and node.target is _orig("interpolate"))):
+    elif node.op == "call_function" and (node.target is F.interpolate or (raw and node.target is _orig("interpolate")) or
+                                         (wrapped and node.target is _raw_interpolate)):
         size, sf, mode, ac, rsf, aa = (_arg(node, i, k, d) for i, k, d in (
             (1, "size", None), (2, "scale_factor", None), (3, "mode", "nearest"), (4, "align_corners", None),
             (5, "recompute_scale_factor", None), (6, "antialias", False)))

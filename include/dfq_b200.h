@@ -45,7 +45,7 @@ const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
- * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms): lets a binding verify
+ * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -757,6 +757,33 @@ int dfq_ssd_nms(const float* scores, const float* boxes, float* slot_boxes, floa
 int dfq_ssd_compact(const float* slot_boxes, const float* slot_probs, const int32_t* counts, const int64_t* offsets,
                     const float* image_sizes, float* out_boxes, int64_t* out_labels, float* out_probs, const DfqSsdNms* d,
                     void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Segmentation evaluation (utils/segmentation/utils.py forward_all, utils/metrics.py Evaluator) for a batch
+ * ------------------------------------------------------------------------------------------- */
+#define DFQ_SEG_LABEL_U8 0
+#define DFQ_SEG_LABEL_I64 1
+#define DFQ_SEG_LABEL_F32 2
+typedef struct DfqSegArgmax {
+  int32_t N, C, H, W;            /* logits fp32 NCHW [N, C, H, W], contiguous                                          */
+  int32_t OH, OW;                /* output size: pred and labels are [N, OH, OW]                                       */
+  int32_t align_corners;         /* 0 or 1; ignored when (OH, OW) == (H, W) (torch's plain copy)                       */
+  int32_t label_type;            /* DFQ_SEG_LABEL_U8 (uint8), _I64 (int64) or _F32 (float32)                           */
+} DfqSegArgmax;
+/* Per output pixel (n, oh, ow): the C values of F.interpolate(logits, (OH, OW), mode="bilinear", align_corners) at that
+ * pixel, bit for bit torch's CUDA upsample_bilinear2d (the plain copy when the size does not change), and their argmax
+ * under torch's CUDA max(dim) rule: the first NaN wins over every number, otherwise the larger value, and on equal values
+ * (-0.0 equal to +0.0) the lower index.  pred (int64 [N, OH, OW], optional) receives the argmax.  count (uint64 [C, C],
+ * optional, accumulated: the caller clears it) receives, per pixel whose label gt passes the Evaluator's mask
+ * 0 <= gt < C, one count at [gt][argmax].  The label of labels [N, OH, OW] is the value itself for uint8 and int64; for
+ * float32 it is the value truncated toward zero (numpy's astype(np.uint8)) when -1 < v < 256, and NaN or any other value
+ * is dropped.  labels and count are both given or both NULL; at least one of pred and count is given.
+ * DFQ_E_ARG, with a reason and before any write: d NULL, a size below 1, align_corners not 0 or 1, an unknown label_type,
+ * logits NULL, labels without count or count without labels, neither pred nor count, a pointer not aligned to its element
+ * (labels to its label type), count or pred overlapping another buffer.  DFQ_E_UNSUPPORTED: C above 160, 2^62 elements
+ * or more. */
+int dfq_seg_argmax(const float* logits, const void* labels, int64_t* pred, uint64_t* count, const DfqSegArgmax* d,
+                   void* stream);
 
 #ifdef __cplusplus
 }

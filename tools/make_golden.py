@@ -20,9 +20,10 @@ build container.  Committed next to its outputs so every fixture can be regenera
                           pin tests (tests/test_oracle_pins.py, test_op_patching.py, test_distill.py)
 
   ref_ssd_postprocess.npz the reference's Predictor.predict post-processing on seeded SSD-Lite-shaped outputs
+  ref_seg_eval.npz        the reference's forward_all predictions and Evaluator matrices and metrics on seeded batches
 
 usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
-       [ssd_post]
+       [ssd_post] [seg_eval]
 """
 import hashlib
 import json
@@ -432,3 +433,53 @@ def ssd_postprocess():
 
 if __name__ == "__main__" and "ssd_post" in sys.argv[1:]:
     ssd_postprocess()
+
+
+# ---------------------------------------------------------------------------------------------------------
+def seg_eval():
+    """forward_all's per-batch steps (utils/segmentation/utils.py) on three seeded batches of full-resolution logits
+    [2, 21, 20, 28] and float32 labels, as the reference's dataset yields them: torch.max(logits, 1)[1] as uint8, the
+    labels through astype(np.uint8), then the reference's own Evaluator.add_batch.  Batch 0 has logits rounded to a coarse
+    grid (many tied maxima) and labels with 255 borders and fractional values (-0.5 .. 20.9); batch 1 has no pixel of class
+    7 in its labels; batch 2 is all 255.  Stores the matrix after each add_batch and the four metrics of each, and those of
+    a fresh Evaluator given the all-255 batch alone (an empty matrix: NaN metrics)."""
+    from utils.metrics import Evaluator
+    g = torch.Generator().manual_seed(5)
+    N, C, H, W = 2, 21, 20, 28
+    out = {}
+    ev = Evaluator(C)
+
+    def metrics(e):
+        with np.errstate(all="ignore"):
+            return np.array([e.Pixel_Accuracy(), e.Pixel_Accuracy_Class(), e.Mean_Intersection_over_Union(),
+                             e.Frequency_Weighted_Intersection_over_Union()])
+    for b in range(3):
+        logits = torch.randn(N, C, H, W, generator=g)
+        logits[:, 0] += 0.8                                       # background most likely, as in VOC
+        if b == 0:
+            logits = torch.round(logits * 2) / 2
+        labels = torch.randint(0, C, (N, H, W), generator=g).float()
+        labels[torch.rand(N, H, W, generator=g) < 0.5] = 0.
+        if b == 0:
+            labels += torch.rand(N, H, W, generator=g).mul(0.9)    # fractional values truncate toward zero
+            labels[0, 5, :5] = -0.5
+        if b == 1:
+            labels[labels == 7] = 3.
+        labels[:, :2] = 255.
+        labels[:, :, -1] = 255.
+        if b == 2:
+            labels[:] = 255.
+        pred = torch.max(logits, 1)[1].numpy().astype(np.uint8)
+        lab = labels.numpy().astype(np.uint8)
+        ev.add_batch(lab, pred)
+        out.update({"logits_%d" % b: logits.numpy(), "labels_%d" % b: labels.numpy(), "pred_%d" % b: pred,
+                    "matrix_%d" % b: ev.confusion_matrix.copy(), "metrics_%d" % b: metrics(ev)})
+        print("seg eval batch %d: %d pixels counted, metrics %s" % (b, int(ev.confusion_matrix.sum()), metrics(ev)))
+    empty = Evaluator(C)
+    empty.add_batch(out["labels_2"].astype(np.uint8), out["pred_2"])
+    out["matrix_empty"], out["metrics_empty"] = empty.confusion_matrix.copy(), metrics(empty)
+    np.savez_compressed(os.path.join(GOLD, "ref_seg_eval.npz"), **out)
+
+
+if __name__ == "__main__" and "seg_eval" in sys.argv[1:]:
+    seg_eval()
