@@ -130,6 +130,9 @@ SEG_LABEL_U8, SEG_LABEL_I64, SEG_LABEL_F32 = 0, 1, 2
 # DfqSegArgmax is struct-size index 19, checked on its own: EXPECTED_SIZES stays the table of indices 0 .. 18
 SEG_ARGMAX_INDEX, SEG_ARGMAX_SIZE = 19, 32
 
+MAP_IGNORED, MAP_TP, MAP_FP = 0, 1, 2                  # verdicts of dfq_map_match
+MAP_ERR_DET_LABEL, MAP_ERR_GT_LABEL, MAP_ERR_DET_OFFSETS, MAP_ERR_GT_OFFSETS = 1, 2, 4, 8   # its device error bits
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -213,6 +216,9 @@ SIGNATURES = {
     "dfq_ssd_nms": [_PF, _PF, _PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_ssd_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, _ST],
     "dfq_seg_argmax": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_map_match": [_PF, C.c_void_p, _PF, C.c_void_p, _I64, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _I64, _I32, _I32,
+                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_map_curve": [C.c_void_p, C.c_void_p, _I64, _I32, C.c_void_p, _I32, C.c_void_p, _I64, C.c_void_p, _ST],
 }
 
 _lib = None

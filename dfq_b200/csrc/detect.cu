@@ -12,6 +12,7 @@
 
 #include <cub/block/block_scan.cuh>
 
+#include "box_iou.cuh"
 #include "common.cuh"
 
 namespace dfq {
@@ -35,21 +36,6 @@ __global__ void __launch_bounds__(256) k_ssd_decode(const float4* __restrict__ l
     const float hw = w * 0.5f, hh = h * 0.5f;   // torch divides by a CPU scalar as a multiply by its reciprocal
     boxes[i] = make_float4(cx - hw, cy - hh, cx + hw, cy + hh);
   }
-}
-
-// torch.maximum / torch.minimum / clamp(min=0): NaN in, NaN out
-__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
-__device__ __forceinline__ float nan_min(float a, float b) { return (a < b || a != a) ? a : b; }
-__device__ __forceinline__ float clamp0(float a) { return a < 0.f ? 0.f : a; }
-
-// box_utils.iou_of(r, cur) for one pair, in the reference's op order
-__device__ __forceinline__ float iou_of(const float4 r, const float4 c) {
-  const float ow = clamp0(nan_min(r.z, c.z) - nan_max(r.x, c.x));
-  const float oh = clamp0(nan_min(r.w, c.w) - nan_max(r.y, c.y));
-  const float ov = ow * oh;
-  const float a0 = clamp0(r.z - r.x) * clamp0(r.w - r.y);
-  const float a1 = clamp0(c.z - c.x) * clamp0(c.w - c.y);
-  return ov / (((a0 + a1) - ov) + 1e-5f);
 }
 
 // Order key of a candidate: the score's bits made unsigned-orderable (-0.0 folded onto +0.0), then P-1-index so that among

@@ -1,4 +1,5 @@
-"""SSD post-processing for whole batches on the GPU: box decoding and the reference's per-class hard NMS.
+"""SSD post-processing and evaluation for whole batches on the GPU: box decoding, the reference's per-class hard NMS and
+its VOC average precision.
 
 `postprocess` returns, for every image of a batch, what the reference's `Predictor.predict`
 (modeling/detection/predictor.py) returns for that image alone - the decode of utils/detection/box_utils.py bit for bit
@@ -10,6 +11,15 @@ order among equal scores is arbitrary).  Soft NMS is not offered (DESIGN.md sect
     det = detect.postprocess(scores, boxes, image_sizes=sizes)
     for boxes, labels, probs in det.per_image():
         ...
+
+`Evaluator` computes from those detections, batch by batch and without a host synchronisation until the end, the
+per-class average precision main_ssd.py computes (compute_average_precision_per_class, DESIGN.md section 3.11):
+
+    ev = detect.Evaluator(num_classes=21)
+    for images, sizes, annotations in loader:
+        ev.add_batch(detect.postprocess(*net(images), image_sizes=sizes), detect.ground_truth(annotations, "cuda"))
+    aps = ev.average_precision()           # classes 1 .. C-1
+    print(ev.mean_average_precision())
 """
 from __future__ import annotations
 
@@ -21,7 +31,11 @@ import torch
 
 from . import _lib
 
-__all__ = ["Detections", "decode_boxes", "postprocess"]
+__all__ = ["Detections", "Evaluator", "GroundTruth", "decode_boxes", "ground_truth", "postprocess"]
+
+MAX_MAP_CLASSES = 4096
+MAX_MAP_DETECTIONS = 2 ** 31 - 1
+MATCH_IGNORED, MATCH_TP, MATCH_FP = _lib.MAP_IGNORED, _lib.MAP_TP, _lib.MAP_FP
 
 
 def _ptr(t):
@@ -155,3 +169,232 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
                                        _ptr(image_sizes), _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, st),
                    "dfq_ssd_compact")
     return Detections(out_boxes, labels, probs, seg_offsets[::C_ - 1])
+
+
+# ---- VOC average precision -------------------------------------------------------------------------------------------
+
+@dataclass
+class GroundTruth:
+    """The ground truth of a batch of N images, on the device: image n's boxes are rows offsets[n] .. offsets[n + 1] of
+    boxes fp32 [G, 4] (0-based corner form, pixels, as VOCDataset.get_annotation returns them), labels int64 [G] and
+    difficult uint8 [G] (non-zero: difficult), in annotation order.  offsets is int64 [N + 1]."""
+    boxes: torch.Tensor
+    labels: torch.Tensor
+    difficult: torch.Tensor
+    offsets: torch.Tensor
+
+
+def ground_truth(annotations, device) -> GroundTruth:
+    """A GroundTruth from the (boxes, labels, is_difficult) triples VOCDataset.get_annotation returns, one per image (numpy
+    arrays or CPU tensors; an image may have no boxes), packed on the host and moved to `device` in one copy.  Boxes must be
+    float32, as the dataset yields them; labels and difficult flags may be of any integer or bool type."""
+    boxes, labels, difficult, offsets = [], [], [], [0]
+    for n, ann in enumerate(annotations):
+        if not isinstance(ann, (tuple, list)) or len(ann) != 3:
+            raise _lib.DfqError("annotation %d must be a (boxes, labels, is_difficult) triple, got %s" % (n, type(ann).__name__))
+        b, l, d = (np.asarray(v.cpu() if isinstance(v, torch.Tensor) else v) for v in ann)
+        if b.dtype != np.float32:
+            raise _lib.DfqError("annotation %d: boxes must be float32, got %s" % (n, b.dtype))
+        if b.size == 0:
+            b = b.reshape(0, 4)
+        if b.ndim != 2 or b.shape[1] != 4:
+            raise _lib.DfqError("annotation %d: boxes must have shape [k, 4], got %s" % (n, b.shape))
+        k = b.shape[0]
+        if l.shape != (k,) or d.shape != (k,):
+            raise _lib.DfqError("annotation %d: %d boxes, but labels of shape %s and is_difficult of shape %s"
+                                % (n, k, l.shape, d.shape))
+        if not (np.issubdtype(l.dtype, np.integer) or k == 0):
+            raise _lib.DfqError("annotation %d: labels must be integers, got %s" % (n, l.dtype))
+        if not (np.issubdtype(d.dtype, np.integer) or d.dtype == np.bool_ or k == 0):
+            raise _lib.DfqError("annotation %d: is_difficult must be integers or bools, got %s" % (n, d.dtype))
+        boxes.append(b); labels.append(l.astype(np.int64)); difficult.append((d != 0).astype(np.uint8))
+        offsets.append(offsets[-1] + k)
+    N, G = len(offsets) - 1, offsets[-1]
+    if N < 1:
+        raise _lib.DfqError("ground_truth needs at least one image")
+    # one byte buffer: boxes at 0 (16-byte aligned), labels at 16 G, offsets at 24 G, difficult at 24 G + 8 (N + 1)
+    o_lab, o_off, o_dif = 16 * G, 24 * G, 24 * G + 8 * (N + 1)
+    host = np.empty(o_dif + G, np.uint8)
+    host[:o_lab].view(np.float32)[:] = np.concatenate(boxes).reshape(-1) if G else []
+    host[o_lab:o_off].view(np.int64)[:] = np.concatenate(labels) if G else []
+    host[o_off:o_dif].view(np.int64)[:] = offsets
+    host[o_dif:] = np.concatenate(difficult) if G else []
+    buf = torch.from_numpy(host).to(device)
+    return GroundTruth(buf[:o_lab].view(torch.float32).view(G, 4), buf[o_lab:o_off].view(torch.int64),
+                       buf[o_dif:], buf[o_off:o_dif].view(torch.int64))
+
+
+def _field(t, name, dtype, shape, device):
+    """t, contiguous, when it is a tensor of `dtype` and `shape` on `device`, else DfqError."""
+    if not isinstance(t, torch.Tensor):
+        raise _lib.DfqError("%s must be a torch.Tensor, got %s" % (name, type(t).__name__))
+    if not t.is_cuda:
+        raise _lib.DfqError("%s must be on the GPU (no CPU fallback), got %s" % (name, t.device))
+    if t.dtype != dtype:
+        raise _lib.DfqError("%s must be %s, got %s" % (name, dtype, t.dtype))
+    if tuple(t.shape) != shape:
+        raise _lib.DfqError("%s must have shape %s, got %s" % (name, shape, tuple(t.shape)))
+    if t.device != device:
+        raise _lib.DfqError("%s is on %s, expected %s" % (name, t.device, device))
+    return t.contiguous()
+
+
+_ERRORS = [(_lib.MAP_ERR_DET_LABEL, "a detection label outside 1 .. num_classes - 1"),
+           (_lib.MAP_ERR_GT_LABEL, "a ground-truth label outside 0 .. num_classes - 1"),
+           (_lib.MAP_ERR_DET_OFFSETS, "detection offsets that do not run from 0 to the detection count without decreasing"),
+           (_lib.MAP_ERR_GT_OFFSETS, "ground-truth offsets that do not run from 0 to the box count without decreasing")]
+
+
+class Evaluator:
+    """main_ssd.py's per-class VOC average precision (compute_average_precision_per_class, DESIGN.md section 3.11) over the
+    batches added, computed on the GPU.  The defaults are main_ssd.py's.
+
+    add_batch matches each batch's detections against its ground truth as soon as they exist and appends them to buffers on
+    the device, without synchronising with the host.  average_precision() sorts everything added and reads back the
+    compact per-class results once.  The one intended difference from the reference: detections of equal score are taken
+    in the order they were added (images in order, then row order within an image), where the reference's sort is not
+    stable.  The accumulators live on the device of the first batch."""
+
+    def __init__(self, num_classes=21, iou_threshold=0.5, use_2007_metric=True):
+        if not isinstance(num_classes, int) or isinstance(num_classes, bool) or not 2 <= num_classes <= MAX_MAP_CLASSES:
+            raise _lib.DfqError("num_classes must be an int in 2 .. %d, got %r" % (MAX_MAP_CLASSES, num_classes))
+        if isinstance(iou_threshold, bool) or not isinstance(iou_threshold, (int, float)):
+            raise _lib.DfqError("iou_threshold must be a real number, got %r" % (iou_threshold,))
+        if not isinstance(use_2007_metric, bool):
+            raise _lib.DfqError("use_2007_metric must be a bool, got %r" % (use_2007_metric,))
+        self.num_classes = num_classes
+        self.iou_threshold = float(iou_threshold)
+        self.use_2007_metric = use_2007_metric
+        self.device = None
+        self._keys = self._flags = self._gt_count = self._error = None
+        self.reset()
+
+    def reset(self):
+        """Forget every batch added."""
+        self._count = 0          # detections added
+        self._gt_total = 0       # ground-truth boxes added
+        if self._gt_count is not None:
+            self._gt_count.zero_()
+            self._error.zero_()
+
+    @property
+    def match_flags(self):
+        """The verdict of every detection added, uint8 on the device in the order added: MATCH_TP, MATCH_FP or MATCH_IGNORED
+        (the best box was difficult)."""
+        if self._flags is None:
+            return torch.empty(0, dtype=torch.uint8)
+        return self._flags[:self._count]
+
+    def add_batch(self, det, gt):
+        """Match a batch: det the Detections of N images with boxes in pixels (postprocess(..., image_sizes=...)), gt the
+        GroundTruth of the same N images.  Shapes, dtypes and devices are checked here; labels and offsets are checked on
+        the device, and average_precision() raises if they were wrong.  Does not synchronise with the host."""
+        if not isinstance(det, Detections):
+            raise _lib.DfqError("det must be a detect.Detections, got %s" % type(det).__name__)
+        if not isinstance(gt, GroundTruth):
+            raise _lib.DfqError("gt must be a detect.GroundTruth, got %s" % type(gt).__name__)
+        if not isinstance(det.offsets, torch.Tensor) or det.offsets.dim() != 1 or det.offsets.shape[0] < 2:
+            raise _lib.DfqError("det.offsets must be a tensor [N + 1] with N >= 1")
+        if not isinstance(det.probs, torch.Tensor) or det.probs.dim() != 1:
+            raise _lib.DfqError("det.probs must be a tensor [T]")
+        if not isinstance(gt.labels, torch.Tensor) or gt.labels.dim() != 1:
+            raise _lib.DfqError("gt.labels must be a tensor [G]")
+        N, T, G = det.offsets.shape[0] - 1, det.probs.shape[0], gt.labels.shape[0]
+        dev = self.device if self.device is not None else det.probs.device
+        if not det.probs.is_cuda:
+            raise _lib.DfqError("det.probs must be on the GPU (no CPU fallback), got %s" % det.probs.device)
+        d_boxes = _field(det.boxes, "det.boxes", torch.float32, (T, 4), dev)
+        d_labels = _field(det.labels, "det.labels", torch.int64, (T,), dev)
+        d_probs = _field(det.probs, "det.probs", torch.float32, (T,), dev)
+        d_offs = _field(det.offsets, "det.offsets", torch.int64, (N + 1,), dev)
+        g_boxes = _field(gt.boxes, "gt.boxes", torch.float32, (G, 4), dev)
+        g_labels = _field(gt.labels, "gt.labels", torch.int64, (G,), dev)
+        g_diff = _field(gt.difficult, "gt.difficult", torch.uint8, (G,), dev)
+        g_offs = _field(gt.offsets, "gt.offsets", torch.int64, (N + 1,), dev)
+        for t, name in ((d_boxes, "det.boxes"), (g_boxes, "gt.boxes")):
+            if t.numel() and t.data_ptr() % 16:
+                raise _lib.DfqError("%s must be 16-byte aligned" % name)
+        if self._count + T > MAX_MAP_DETECTIONS:
+            raise _lib.DfqError("%d detections added in all, above the limit %d" % (self._count + T, MAX_MAP_DETECTIONS))
+        if self._gt_count is None:
+            self.device = dev
+            self._gt_count = torch.zeros(self.num_classes, dtype=torch.int64, device=dev)
+            self._error = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._reserve(self._count + T)
+        lib = _lib.load()
+        _lib.check(lib.dfq_map_match(
+            _ptr(d_boxes), _ptr(d_labels), _ptr(d_probs), _ptr(d_offs), T, _ptr(g_boxes), _ptr(g_labels), _ptr(g_diff),
+            _ptr(g_offs), G, N, self.num_classes, self.iou_threshold,
+            C.c_void_p(self._keys.data_ptr() + 8 * self._count), C.c_void_p(self._flags.data_ptr() + self._count),
+            _ptr(self._gt_count), _ptr(self._error), _lib.stream_ptr()), "dfq_map_match")
+        self._count += T
+        self._gt_total += G
+
+    def _reserve(self, n):
+        """Room for n detections in the accumulation buffers, grown on the device (no synchronisation)."""
+        cap = 0 if self._keys is None else self._keys.shape[0]
+        if n <= cap:
+            return
+        cap = max(n, 2 * cap, 1 << 16)
+        keys = torch.empty(cap, dtype=torch.int64, device=self.device)
+        flags = torch.empty(cap, dtype=torch.uint8, device=self.device)
+        if self._count:
+            keys[:self._count].copy_(self._keys[:self._count])
+            flags[:self._count].copy_(self._flags[:self._count])
+        self._keys, self._flags = keys, flags
+
+    def _curve(self):
+        """(gt_count, counts, out) on the host: dfq_map_curve's results, read back in one copy."""
+        Cn = self.num_classes
+        if self._gt_count is None:
+            return np.zeros(Cn, np.int64), np.zeros(Cn, np.int64), np.zeros(11 * (Cn - 1))
+        n_out = 11 * (Cn - 1) if self.use_2007_metric else self._gt_total + Cn
+        # error (padded to 8 bytes), gt_count [C], counts [C], out [n_out]
+        buf = torch.zeros(8 + 16 * Cn + 8 * n_out, dtype=torch.uint8, device=self.device)
+        counts = buf[8 + 8 * Cn:8 + 16 * Cn].view(torch.int64)
+        out = buf[8 + 16 * Cn:].view(torch.float64)
+        D = self._count
+        _lib.check(_lib.load().dfq_map_curve(
+            _ptr(self._keys) if D else None, _ptr(self._flags) if D else None, D, Cn, _ptr(self._gt_count),
+            int(self.use_2007_metric), _ptr(out), n_out, _ptr(counts), _lib.stream_ptr()), "dfq_map_curve")
+        buf[:4].copy_(self._error.view(torch.uint8))
+        buf[8:8 + 8 * Cn].copy_(self._gt_count.view(torch.uint8))
+        host = buf.cpu().numpy()
+        error = int(host[:4].view(np.int32)[0])
+        if error:
+            raise _lib.DfqError("detect.Evaluator: the batches added had %s"
+                                % "; ".join(msg for bit, msg in _ERRORS if error & bit))
+        return (host[8:8 + 8 * Cn].view(np.int64), host[8 + 8 * Cn:8 + 16 * Cn].view(np.int64),
+                host[8 + 16 * Cn:].view(np.float64))
+
+    def _aps(self):
+        """(aps as the reference's own list, with its Python float / numpy float64 types, gt_count)."""
+        gt_count, counts, out = self._curve()
+        aps = []
+        for c in range(1, self.num_classes):
+            if gt_count[c] == 0:
+                aps.append(float("nan"))                 # the reference raises KeyError for this class
+            elif self.use_2007_metric:
+                ap = 0.
+                for p in out[11 * (c - 1):11 * c].tolist():
+                    ap = ap + p / 11.
+                aps.append(np.float64(ap) if counts[c] else ap)   # a class without detections never meets numpy
+            else:
+                base = c - 1 + int(gt_count[1:c].sum())
+                aps.append(out[base:base + counts[c]].copy().sum())
+        return aps, gt_count
+
+    def average_precision(self):
+        """float64 numpy [num_classes - 1]: compute_average_precision_per_class for classes 1 .. num_classes - 1, bit for
+        bit, NaN included.  A class with no non-difficult ground truth, for which the reference raises KeyError, is NaN.
+        Raises DfqError when a batch added had labels or offsets out of range."""
+        return np.array(self._aps()[0], dtype=np.float64)
+
+    def mean_average_precision(self):
+        """sum(aps) / len(aps) as main_ssd.py prints it.  DfqError when a class has no non-difficult ground truth."""
+        aps, gt_count = self._aps()
+        missing = [c for c in range(1, self.num_classes) if gt_count[c] == 0]
+        if missing:
+            raise _lib.DfqError("class %d has no non-difficult ground truth (main_ssd.py raises KeyError for it)%s"
+                                % (missing[0], "" if len(missing) == 1 else "; so do %d more" % (len(missing) - 1)))
+        return sum(aps) / len(aps)

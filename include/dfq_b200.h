@@ -785,6 +785,50 @@ typedef struct DfqSegArgmax {
 int dfq_seg_argmax(const float* logits, const void* labels, int64_t* pred, uint64_t* count, const DfqSegArgmax* d,
                    void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * VOC average precision of SSD detections (main_ssd.py compute_average_precision_per_class,
+ * utils/detection/measurements.py), accumulated batch by batch
+ * ------------------------------------------------------------------------------------------- */
+#define DFQ_MAP_IGNORED 0              /* verdict of a detection: neither true nor false positive (a difficult box) */
+#define DFQ_MAP_TP 1
+#define DFQ_MAP_FP 2
+#define DFQ_MAP_ERR_DET_LABEL 1        /* bits of the device error word */
+#define DFQ_MAP_ERR_GT_LABEL 2
+#define DFQ_MAP_ERR_DET_OFFSETS 4
+#define DFQ_MAP_ERR_GT_OFFSETS 8
+/* One batch of N images: detections det_boxes fp32 [T, 4] (corner form, pixels), det_labels int64 [T], det_probs fp32 [T],
+ * image n's rows det_offsets[n] .. det_offsets[n + 1] (int64 [N + 1]); ground truth gt_boxes fp32 [G, 4] (0-based corner
+ * form, pixels), gt_labels int64 [G], gt_difficult uint8 [G] (non-zero: difficult), image n's rows gt_offsets[n] ..
+ * gt_offsets[n + 1].  Adds each non-difficult box to gt_count[label] (uint64 [C], accumulated).  Per detection t of class
+ * c: box = fl32(fl32(b + 1) - 1) per coordinate (the text round trip of main_ssd.py); no box of class c in the image:
+ * false positive; else m = max and g = argmax of iou_of(box, gt) over the image's boxes of class c in annotation order
+ * (box_utils' fp32 op order; the first NaN, else the first maximum); unless (double)m > iou_threshold: false positive;
+ * box g difficult: ignored; else box g goes to the first detection claiming it in score-descending order (equal scores:
+ * the lower row), a true positive, and every later claim is a false positive.  Writes keys[t] = (c << 32) | the score's
+ * descending rank bits (-0.0 equal to +0.0, NaN last) and flags[t] = DFQ_MAP_IGNORED / _TP / _FP; pass keys and flags
+ * offset to where the batch is appended.  Checks needing device data set bits of *error (atomicOr) instead of failing:
+ * a detection label outside 1 .. C-1, a ground-truth label outside 0 .. C-1, offsets that do not run from 0 up to T
+ * (resp. G) without decreasing; an image with bad offsets is skipped.  Does not synchronise.  DFQ_E_ARG, with a reason
+ * and before any write: C < 2, N < 1, T or G < 0, a NULL pointer that is needed (the detection buffers when T > 0, the
+ * ground-truth buffers when G > 0), boxes not 16-byte aligned.  DFQ_E_UNSUPPORTED: C above 4096, T above INT32_MAX. */
+int dfq_map_match(const float* det_boxes, const int64_t* det_labels, const float* det_probs, const int64_t* det_offsets,
+                  int64_t T, const float* gt_boxes, const int64_t* gt_labels, const uint8_t* gt_difficult,
+                  const int64_t* gt_offsets, int64_t G, int32_t N, int32_t C, double iou_threshold, uint64_t* keys,
+                  uint8_t* flags, uint64_t* gt_count, int32_t* error, void* stream);
+/* The precision/recall curve of every class c = 1 .. C-1 over the D accumulated detections (keys, flags of
+ * dfq_map_match), ordered by a stable sort on (class ascending, score descending): equal scores keep the order they were
+ * appended in.  tp, fp the cumulative counts, precision = tp / (tp + fp), recall = tp / gt_count[c], float64.
+ * use_2007 = 1: out[(c - 1) * 11 + k] = max(precision[recall >= k * 0.1]) (NaN-propagating), 0.0 when nothing is
+ * selected, and term_count[c] (int64 [C]) = the class's number of detections; out_len >= 11 * (C - 1).  use_2007 = 0: the area terms (recall[j + 1] - recall[j]) * precision'[j + 1] of
+ * compute_average_precision at each j where the padded recall changes, precision' the running maximum from the end
+ * (NaN-propagating) of the padded precision; class c's terms, term_count[c] of them (int64 [C]), start at
+ * (c - 1) + the sum of gt_count[1 .. c-1]; out_len >= G + C for G ground-truth boxes in all.  A class without non-difficult
+ * ground truth (gt_count 0) yields values without meaning.  Does not synchronise.  DFQ_E_ARG, with a reason and before any
+ * write: C < 2, D < 0, use_2007 not 0 or 1, a needed NULL pointer, out_len too small.  DFQ_E_UNSUPPORTED: C above 4096,
+ * D above INT32_MAX. */
+int dfq_map_curve(const uint64_t* keys, const uint8_t* flags, int64_t D, int32_t C, const uint64_t* gt_count,
+                  int32_t use_2007, double* out, int64_t out_len, int64_t* term_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

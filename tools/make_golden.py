@@ -21,9 +21,10 @@ build container.  Committed next to its outputs so every fixture can be regenera
 
   ref_ssd_postprocess.npz the reference's Predictor.predict post-processing on seeded SSD-Lite-shaped outputs
   ref_seg_eval.npz        the reference's forward_all predictions and Evaluator matrices and metrics on seeded batches
+  ref_ssd_map.npz         main_ssd.py's per-class VOC average precision on a seeded set of detections and annotations
 
 usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
-       [ssd_post] [seg_eval]
+       [ssd_post] [seg_eval] [ssd_map]
 """
 import hashlib
 import json
@@ -483,3 +484,174 @@ def seg_eval():
 
 if __name__ == "__main__" and "seg_eval" in sys.argv[1:]:
     seg_eval()
+
+
+# ---------------------------------------------------------------------------------------------------------
+SSD_MAP_CONFIGS = [(0.5, True), (0.5, False), (0.55, True), (0.55, False)]     # (iou_threshold, use_2007_metric)
+
+
+def _ulp_search(x0, f, want, n=20000):
+    """The fp32 x nearest to x0, within n ulps either side, with want(f(x)) true."""
+    k = np.arange(-n, n, dtype=np.float32)
+    k = k[np.argsort(np.abs(k), kind="stable")]
+    xs = torch.from_numpy(np.float32(x0) + k * np.spacing(np.float32(x0)))
+    hit = torch.nonzero(want(f(xs))).reshape(-1)
+    assert hit.numel(), "no seeded box found"
+    return np.float32(xs[hit[0]])
+
+
+def ssd_map_scene():
+    """Seeded detections and annotations for 9 classes (class 8 has no ground truth) in which each rule of DESIGN.md
+    section 3.11 decides an AP: a random scene of jittered copies of the annotations plus clutter, and constructed images
+    for the +1/-1 rounding, an IoU equal to float32(0.55), a second detection on one box, a difficult argmax next to a
+    passing non-difficult box, equal IoUs, a class whose best detection hits a difficult box, detections on images
+    without boxes of their class, a class without detections (6) and NaN boxes.  No class has tied scores."""
+    g = np.random.default_rng(11)
+    C = 9
+    gts, dets = [], []
+
+    def add(gt, det):                     # gt [(box, label, difficult)], det [(box, label, score)]
+        gts.append((np.array([b for b, _, _ in gt], np.float32).reshape(-1, 4) if gt else np.array([], np.float32),
+                    np.array([l for _, l, _ in gt], np.int64), np.array([d for _, _, d in gt], np.uint8)))
+        dets.append(det)
+    # random scene: 24 images, classes 1 .. 5 and 7
+    for n in range(24):
+        gt, det = [], []
+        for _ in range(int(g.integers(0, 6))):
+            x1, y1 = g.uniform(0, 400, 2)
+            w, h = g.uniform(20, 200, 2)
+            gt.append(([x1, y1, min(x1 + w, 500), min(y1 + h, 500)], int(g.choice([1, 2, 3, 4, 5, 7])),
+                       int(g.random() < 0.2)))
+        for b, l, _ in gt:
+            for _ in range(int(g.integers(0, 4))):
+                det.append((np.float32(np.array(b) + g.normal(0, 12, 4)), l, None))
+        for _ in range(int(g.integers(0, 6))):
+            x1, y1 = g.uniform(0, 400, 2)
+            det.append((np.float32([x1, y1, x1 + g.uniform(10, 100), y1 + g.uniform(10, 100)]),
+                        int(g.choice([1, 2, 3, 4, 5, 7])), None))
+        add(gt, det)
+    # the +1/-1 rounding moves an IoU across the threshold: box x2 in [255, 256), where b + 1 loses a bit
+    for thr in (0.5, 0.55):
+        gx1 = np.float32(255.0 - thr * 400.0)
+        for y2 in range(300, 400):                   # the first box height with a crossing near x2 = 255
+            gt = [gx1, 40.0, gx1 + 400.0, float(y2)]
+
+            def iou_x2(xs, plus_one):
+                b = torch.stack([torch.full_like(xs, gx1), torch.full_like(xs, 40.0), xs, torch.full_like(xs, float(y2))], 1)
+                if plus_one:
+                    b = (b + 1.0) - 1.0
+                return _ref_iou_of(b, torch.tensor([gt], dtype=torch.float32))
+            try:
+                x2 = _ulp_search(255.0, lambda xs: torch.stack([iou_x2(xs, False), iou_x2(xs, True)]),
+                                 lambda v: (v[0].double() > thr) != (v[1].double() > thr))
+                break
+            except AssertionError:
+                continue
+        add([(gt, 1, 0)], [(np.float32([gx1, 40.0, x2, y2]), 1, None)])
+    # an fp32 IoU equal to float32(0.55): above 0.55 in float64, not in fp32
+    gt = [55.0, 40.0, 455.0, 300.0]
+
+    def iou_55(xs):
+        b = torch.stack([torch.full_like(xs, 55.0), torch.full_like(xs, 40.0), xs, torch.full_like(xs, 300.0)], 1)
+        return _ref_iou_of((b + 1.0) - 1.0, torch.tensor([gt], dtype=torch.float32))
+    x2 = _ulp_search(274.99, iou_55, lambda v: v == np.float32(0.55))
+    add([(gt, 2, 0)], [(np.float32([55.0, 40.0, x2, 300.0]), 2, None)])
+    # two detections on one box: the second is a false positive
+    add([([100., 100., 200., 200.], 1, 0)], [(np.float32([101, 100, 200, 201]), 1, None),
+                                            (np.float32([100, 99, 199, 200]), 1, None)])
+    # the argmax is a difficult box while a non-difficult one also passes: ignored
+    add([([50., 50., 150., 150.], 2, 1), ([56., 52., 150., 152.], 2, 0)], [(np.float32([50, 50, 150, 150]), 2, None)])
+    # equal IoU against two boxes (difficult first): the first wins, so the detection is ignored
+    add([([90., 100., 190., 200.], 3, 1), ([110., 100., 210., 200.], 3, 0)], [(np.float32([100, 100, 200, 200]), 3, None)])
+    # class 4's best detection hits a difficult box: NaN under the 2007 metric, finite under the area metric
+    add([([300., 300., 400., 420.], 4, 1), ([20., 30., 120., 90.], 4, 0)],
+        [(np.float32([300, 300, 400, 420]), 4, 0.9999), (np.float32([20, 30, 120, 90]), 4, 0.9998)])
+    # detections of class 5 on images without boxes of class 5 (one without any box)
+    add([([10., 10., 60., 60.], 1, 0)], [(np.float32([10, 10, 60, 60]), 5, 0.9997)])
+    add([], [(np.float32([200, 200, 260, 280]), 5, 0.9996), (np.float32([5, 5, 50, 50]), 7, None)])
+    # class 6 has boxes but no detection
+    add([([30., 40., 230., 240.], 6, 0), ([40., 40., 90., 90.], 6, 1)], [])
+    # NaN boxes: a ground-truth box with a NaN first (every IoU against it NaN wins), and a NaN detection
+    add([([np.nan, 300., 400., 400.], 7, 0), ([10., 10., 110., 110.], 7, 0)], [(np.float32([10, 10, 110, 110]), 7, 0.9995)])
+    add([([10., 10., 110., 110.], 7, 0)], [(np.float32([10, np.nan, 110, 110]), 7, 0.9994)])
+    # class 8 has detections but no ground truth: the reference raises KeyError
+    add([], [(np.float32([0, 0, 30, 30]), 8, 0.5)])
+    # scores: the given ones, the rest random, unique within each class
+    out = []
+    for det in dets:
+        rows = [(b, l, np.float32(s) if s is not None else np.float32(g.uniform(0.011, 0.99))) for b, l, s in det]
+        rows.sort(key=lambda r: (r[1], -r[2]))            # classes ascending, score descending, as postprocess returns
+        out.append((torch.tensor(np.array([r[0] for r in rows], np.float32).reshape(-1, 4)),
+                    torch.tensor([r[1] for r in rows], dtype=torch.int64), torch.tensor([r[2] for r in rows])))
+    for c in range(1, C):
+        s = torch.cat([p[l == c] for _, l, p in out])
+        assert torch.unique(s).numel() == s.numel(), "tied scores in class %d" % c
+    return C, gts, out
+
+
+def _ref_iou_of(boxes, gt):
+    """box_utils.iou_of(boxes, gt) for the searches above (the reference's own function)."""
+    from utils.detection import box_utils
+    return box_utils.iou_of(boxes, gt)
+
+
+def ssd_map():
+    """main_ssd.py's evaluation on ssd_map_scene(): the per-class files written exactly as the main's loop writes them,
+    group_annotation_by_class on a stand-in dataset and compute_average_precision_per_class per class, for each
+    (iou_threshold, use_2007_metric) of SSD_MAP_CONFIGS.  A KeyError (class 8) is stored as NaN."""
+    import tempfile
+    saved = sys.argv
+    sys.argv = ["main_ssd.py"]
+    import main_ssd
+    sys.argv = saved
+    C, gts, dets = ssd_map_scene()
+
+    class Dataset:
+        ids = ["%06d" % n for n in range(len(gts))]
+
+        def __len__(self):
+            return len(self.ids)
+
+        def get_annotation(self, i):
+            return self.ids[i], gts[i]
+    dataset = Dataset()
+    true_case_stat, all_gb_boxes, all_difficult_cases = main_ssd.group_annotation_by_class(dataset)
+    results = []
+    for i, (boxes, labels, probs) in enumerate(dets):
+        indexes = torch.ones(labels.size(0), 1, dtype=torch.float32) * i
+        results.append(torch.cat([indexes.reshape(-1, 1), labels.reshape(-1, 1).float(), probs.reshape(-1, 1),
+                                  boxes + 1.0], dim=1))
+    results = torch.cat(results)
+    out = dict(num_classes=np.array(C), configs=np.array(SSD_MAP_CONFIGS, np.float64))
+    with tempfile.TemporaryDirectory() as tmp:
+        for c in range(1, C):
+            with open(os.path.join(tmp, "det_test_%d.txt" % c), "w") as f:
+                sub = results[results[:, 1] == c, :]
+                for i in range(sub.size(0)):
+                    prob_box = sub[i, 2:].numpy()
+                    print(dataset.ids[int(sub[i, 0])] + " " + " ".join([str(v) for v in prob_box]), file=f)
+        for k, (thr, use_2007) in enumerate(SSD_MAP_CONFIGS):
+            aps = []
+            for c in range(1, C):
+                try:
+                    with np.errstate(all="ignore"):
+                        aps.append(main_ssd.compute_average_precision_per_class(
+                            true_case_stat[c], all_gb_boxes[c], all_difficult_cases[c],
+                            os.path.join(tmp, "det_test_%d.txt" % c), thr, use_2007))
+                except KeyError:
+                    aps.append(np.nan)
+            out["aps_%d" % k] = np.array(aps, np.float64)
+            print("ssd map iou %.2f 2007 %s: %s" % (thr, use_2007, out["aps_%d" % k]))
+    out["gt_boxes"] = np.concatenate([b.reshape(-1, 4) for b, _, _ in gts])
+    out["gt_labels"] = np.concatenate([l for _, l, _ in gts])
+    out["gt_difficult"] = np.concatenate([d for _, _, d in gts])
+    out["gt_offsets"] = np.cumsum([0] + [len(l) for _, l, _ in gts])
+    out["det_boxes"] = torch.cat([b for b, _, _ in dets]).numpy()
+    out["det_labels"] = torch.cat([l for _, l, _ in dets]).numpy()
+    out["det_probs"] = torch.cat([p for _, _, p in dets]).numpy()
+    out["det_offsets"] = np.cumsum([0] + [l.numel() for _, l, _ in dets])
+    np.savez_compressed(os.path.join(GOLD, "ref_ssd_map.npz"), **out)
+
+
+if __name__ == "__main__" and "ssd_map" in sys.argv[1:]:
+    ssd_map()
