@@ -130,6 +130,16 @@ SEG_LABEL_U8, SEG_LABEL_I64, SEG_LABEL_F32 = 0, 1, 2
 # DfqSegArgmax is struct-size index 19, checked on its own: EXPECTED_SIZES stays the table of indices 0 .. 18
 SEG_ARGMAX_INDEX, SEG_ARGMAX_SIZE = 19, 32
 
+PRE_IMAGE_DT = np.dtype([(f, np.int64) for f in ("src", "label", "xtap", "ytap", "xnear", "ynear")] +
+                        [(f, np.int32) for f in ("H", "W", "xk", "yk")], align=True)
+PRE_RESAMPLE_DT = np.dtype([(f, np.int32) for f in ("n", "out_h", "out_w", "filter", "norm", "_pad")] +
+                           [("blob_bytes", np.int64), ("mean", np.float32, (3,)), ("std", np.float32, (3,)),
+                            ("mean64", np.float64, (3,)), ("std64", np.float64, (3,))], align=True)
+PRE_PIL_BILINEAR, PRE_CV_LINEAR = 0, 1
+PRE_NORM_F32, PRE_NORM_F64, PRE_NORM_SUB_DIV = 0, 1, 2
+# struct-size indices of DfqPreImage and DfqPreResample, checked on their own like DfqSegArgmax's; index 20 stays -1
+PRE_SIZES = {21: (PRE_IMAGE_DT, 64), 22: (PRE_RESAMPLE_DT, 104)}
+
 MAP_IGNORED, MAP_TP, MAP_FP = 0, 1, 2                  # verdicts of dfq_map_match
 MAP_ERR_DET_LABEL, MAP_ERR_GT_LABEL, MAP_ERR_DET_OFFSETS, MAP_ERR_GT_OFFSETS = 1, 2, 4, 8   # its device error bits
 
@@ -219,6 +229,7 @@ SIGNATURES = {
     "dfq_map_match": [_PF, C.c_void_p, _PF, C.c_void_p, _I64, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _I64, _I32, _I32,
                       C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_map_curve": [C.c_void_p, C.c_void_p, _I64, _I32, C.c_void_p, _I32, C.c_void_p, _I64, C.c_void_p, _ST],
+    "dfq_pre_resample": [C.c_void_p, C.c_void_p, C.c_void_p, _PF, _PF, _ST],
 }
 
 _lib = None

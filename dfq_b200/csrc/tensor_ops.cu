@@ -488,6 +488,8 @@ extern "C" int dfq_struct_size(int which) {
     case 17: return (int)sizeof(DfqI8AffineRows);
     case 18: return (int)sizeof(DfqSsdNms);
     case 19: return (int)sizeof(DfqSegArgmax);
+    case 21: return (int)sizeof(DfqPreImage);
+    case 22: return (int)sizeof(DfqPreResample);
     default: return -1;
   }
 }

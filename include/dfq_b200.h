@@ -45,7 +45,8 @@ const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
- * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax): lets a binding verify
+ * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax, 21 DfqPreImage, 22 DfqPreResample; 20 is
+ * unassigned and returns -1, as ABI 11 released it): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
 /* number of SMs and max co-resident CTAs of the persistent kernels on the current device */
@@ -828,6 +829,50 @@ int dfq_map_match(const float* det_boxes, const int64_t* det_labels, const float
  * D above INT32_MAX. */
 int dfq_map_curve(const uint64_t* keys, const uint8_t* flags, int64_t D, int32_t C, const uint64_t* gt_count,
                   int32_t use_2007, double* out, int64_t out_len, int64_t* term_count, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Evaluation preprocessing: the reference's resize, crop and normalisation of decoded uint8 images
+ * (torchvision Resize + CenterCrop + ToTensor + Normalize, custom_transforms FixScaleCrop + Normalize,
+ * SSD PredictionTransform), a batch of images of mixed sizes in one launch
+ * ------------------------------------------------------------------------------------------- */
+#define DFQ_PRE_PIL_BILINEAR 0   /* Pillow BILINEAR: 22-bit taps, both passes rounded and clipped to uint8          */
+#define DFQ_PRE_CV_LINEAR 1      /* OpenCV INTER_LINEAR on uint8: 11-bit taps, int32 rows, the vectorised vertical step */
+#define DFQ_PRE_NORM_F32 0       /* (float(u) / 255 - mean) / std, each step in fp32 (torchvision)                    */
+#define DFQ_PRE_NORM_F64 1       /* float(u) / 255 in fp32; - mean and / std in fp64, each rounded to fp32 (numpy)     */
+#define DFQ_PRE_NORM_SUB_DIV 2   /* (float(u) - mean) / std, each step in fp32 (SubtractMeans, / std)                 */
+/* One image of the batch.  Offsets are bytes into the batch blob (one device buffer).  A tap table of an axis holds, per
+ * output coordinate after the crop, K int32 pairs {source index, weight}; the source indices of each coordinate are
+ * ascending, and so is the first and the last index from one coordinate to the next.  Pairs past a coordinate's own taps
+ * repeat its last index with weight 0. */
+typedef struct DfqPreImage {
+  int64_t src;                   /* uint8 HWC RGB [H, W, 3], contiguous                                               */
+  int64_t label;                 /* uint8 [H, W] label, or -1                                                         */
+  int64_t xtap, ytap;            /* column and row tap tables: out_w * xk and out_h * yk pairs                        */
+  int64_t xnear, ynear;          /* int32 source column / row of each label output, or -1 (with label -1)             */
+  int32_t H, W;
+  int32_t xk, yk;                /* taps per output column / row, 1 .. 4096                                           */
+} DfqPreImage;
+typedef struct DfqPreResample {
+  int32_t n;                     /* images; out is float32 [n, 3, out_h, out_w], labels float32 [n, out_h, out_w]      */
+  int32_t out_h, out_w;
+  int32_t filter;                /* DFQ_PRE_PIL_BILINEAR or DFQ_PRE_CV_LINEAR                                         */
+  int32_t norm;                  /* DFQ_PRE_NORM_*                                                                    */
+  int32_t _pad;
+  int64_t blob_bytes;            /* size of the blob: every table and image must lie inside it                        */
+  float mean[3], std[3];         /* DFQ_PRE_NORM_F32 and _SUB_DIV                                                     */
+  double mean64[3], std64[3];    /* DFQ_PRE_NORM_F64                                                                  */
+} DfqPreResample;
+/* Per output pixel (n, y, x) and channel c: the resized value through the taps of row y and column x (horizontal pass
+ * first: Pillow rounds and clips it to uint8, OpenCV keeps the int32 sum), then the normalisation, written to out
+ * [n, c, y, x].  With image n's label given, labels[n, y, x] = float(label[ynear[y], xnear[x]]).  images: host array of
+ * d->n descriptors, uploaded by the call; blob: device pointer.  labels is NULL exactly when no image has a label.
+ * DFQ_E_ARG, with a reason and before any launch: d, images, blob or out NULL, n, out_h or out_w below 1, an unknown
+ * filter or norm, a std of zero, an image below 1 x 1, taps outside 1 .. 4096, a table or image outside the blob or
+ * misaligned, labels given for some images only or without the labels pointer.  The tables' contents live on the device
+ * and are not read by the call: every source index must lie in its image (columns below W, rows below H) and follow the
+ * order stated above, or the kernel reads outside the image.  dfq_b200.preprocess builds them so. */
+int dfq_pre_resample(const DfqPreResample* d, const DfqPreImage* images, const void* blob, float* out, float* labels,
+                     void* stream);
 
 #ifdef __cplusplus
 }

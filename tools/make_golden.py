@@ -655,3 +655,42 @@ def ssd_map():
 
 if __name__ == "__main__" and "ssd_map" in sys.argv[1:]:
     ssd_map()
+
+
+# ---------------------------------------------------------------------------------------------------------
+def preprocess():
+    """The reference's evaluation transforms on the seeded images of tests/preprocess_cases.py: torchvision's
+    Resize(256) / CenterCrop(224) / ToTensor / Normalize (main_cls.py), VOCSegmentation.transform_val's FixScaleCrop(513) /
+    Normalize / ToTensor (custom_transforms), and PredictionTransform(300, 127, 128) (main_ssd.py).  Stores the sha256 of
+    each float32 output's bytes: the tests compare bit for bit, and the outputs themselves are megabytes each."""
+    import hashlib
+    from PIL import Image
+    from torchvision import transforms
+    import dataset.segmentation.custom_transforms as tr
+    from modeling.detection.data_preprocessing import PredictionTransform
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import preprocess_cases as PC
+    cls = transforms.Compose([transforms.Resize(256), transforms.CenterCrop(224), transforms.ToTensor(),
+                              transforms.Normalize((0.485, 0.456, 0.406), (0.229, 0.224, 0.225))])
+    seg = transforms.Compose([tr.FixScaleCrop(crop_size=513), tr.Normalize(mean=(0.485, 0.456, 0.406),
+                                                                              std=(0.229, 0.224, 0.225)), tr.ToTensor()])
+    ssd = PredictionTransform(300, np.array([127, 127, 127]), 128.0)
+
+    def sha(t):
+        return hashlib.sha256(np.ascontiguousarray(t.numpy(), np.float32).tobytes()).hexdigest()
+    out = {"names": np.array([c[0] for c in PC.cases()])}
+    for name, img, lab in PC.cases():
+        h, w = img.shape[:2]
+        c = cls(Image.fromarray(img))
+        out["cls_" + name] = sha(c)
+        s = seg({"image": Image.fromarray(img), "label": Image.fromarray(lab)})
+        out["seg_" + name], out["seglab_" + name] = sha(s["image"]), sha(s["label"])
+        d = ssd(img)
+        out["ssd_" + name] = sha(d)
+        print("preprocess %s: cls %s seg %s ssd %s" % (name, out["cls_" + name][:8], out["seg_" + name][:8],
+                                                     out["ssd_" + name][:8]))
+    np.savez_compressed(os.path.join(GOLD, "ref_preprocess.npz"), **out)
+
+
+if __name__ == "__main__" and "preprocess" in sys.argv[1:]:
+    preprocess()
