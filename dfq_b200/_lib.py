@@ -140,6 +140,19 @@ PRE_NORM_F32, PRE_NORM_F64, PRE_NORM_SUB_DIV = 0, 1, 2
 # struct-size indices of DfqPreImage and DfqPreResample, checked on their own like DfqSegArgmax's; index 20 stays -1
 PRE_SIZES = {21: (PRE_IMAGE_DT, 64), 22: (PRE_RESAMPLE_DT, 104)}
 
+JPEG_IMAGE_DT = np.dtype([("dst", np.int64), ("tables", np.int64)] +
+                         [(f, np.int32) for f in ("H", "W", "ncomp", "hs", "vs", "mcux", "mcuy", "_pad")], align=True)
+JPEG_SEGMENT_DT = np.dtype([("begin", np.int64), ("end", np.int64)] +
+                           [(f, np.int32) for f in ("image", "mcu0", "mcus", "_pad")], align=True)
+JPEG_DECODE_DT = np.dtype([("n", np.int32), ("nseg", np.int32), ("blob_bytes", np.int64), ("call", np.uint64)], align=True)
+JPEG_HUFF_DT = np.dtype([("maxcode", np.int32, (18,)), ("valoff", np.int32, (18,)), ("look", np.uint16, (512,)),
+                         ("vals", np.uint8, (256,))], align=True)
+JPEG_TABLES_DT = np.dtype([("q", np.int32, (3, 64)), ("dc", JPEG_HUFF_DT, (3,)), ("ac", JPEG_HUFF_DT, (3,))], align=True)
+JPEG_BAD_CODE, JPEG_BAD_RUN, JPEG_SHORT_SCAN = 1, 2, 4    # reason bits of dfq_jpeg_decode's error word
+# struct-size indices of the JPEG decoder's structs, checked on their own like PRE_SIZES
+JPEG_SIZES = {23: (JPEG_IMAGE_DT, 48), 24: (JPEG_SEGMENT_DT, 32), 25: (JPEG_DECODE_DT, 24), 26: (JPEG_HUFF_DT, 1424),
+              27: (JPEG_TABLES_DT, 9312)}
+
 MAP_IGNORED, MAP_TP, MAP_FP = 0, 1, 2                  # verdicts of dfq_map_match
 MAP_ERR_DET_LABEL, MAP_ERR_GT_LABEL, MAP_ERR_DET_OFFSETS, MAP_ERR_GT_OFFSETS = 1, 2, 4, 8   # its device error bits
 
@@ -230,6 +243,7 @@ SIGNATURES = {
                       C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_map_curve": [C.c_void_p, C.c_void_p, _I64, _I32, C.c_void_p, _I32, C.c_void_p, _I64, C.c_void_p, _ST],
     "dfq_pre_resample": [C.c_void_p, C.c_void_p, C.c_void_p, _PF, _PF, _ST],
+    "dfq_jpeg_decode": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

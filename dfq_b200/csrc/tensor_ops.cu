@@ -490,6 +490,11 @@ extern "C" int dfq_struct_size(int which) {
     case 19: return (int)sizeof(DfqSegArgmax);
     case 21: return (int)sizeof(DfqPreImage);
     case 22: return (int)sizeof(DfqPreResample);
+    case 23: return (int)sizeof(DfqJpegImage);
+    case 24: return (int)sizeof(DfqJpegSegment);
+    case 25: return (int)sizeof(DfqJpegDecode);
+    case 26: return (int)sizeof(DfqJpegHuff);
+    case 27: return (int)sizeof(DfqJpegTables);
     default: return -1;
   }
 }

@@ -3,7 +3,8 @@
 The reference's three evaluation loops transform every decoded image on the CPU before the network sees it:
 main_cls.py with torchvision Resize(256) -> CenterCrop(224) -> ToTensor -> Normalize (Pillow bilinear), main_seg.py with
 custom_transforms FixScaleCrop(513) -> Normalize -> ToTensor (Pillow bilinear image, Pillow nearest label), and
-main_ssd.py with PredictionTransform (cv2.resize INTER_LINEAR -> - mean -> / std).  Here the loader only decodes: the batch's
+main_ssd.py with PredictionTransform (cv2.resize INTER_LINEAR -> - mean -> / std).  Here the loader only decodes (or, with
+dfq_b200.jpeg, only reads the file: JPEG bytes are decoded on the device into the same blob): the batch's
 images, of any sizes, are gathered into one page-locked buffer, moved by one host-to-device copy, and one kernel launch
 resizes, crops and normalises them into the NCHW float32 batch.  The resize coefficients are the libraries' own, formed on
 the host by their rules; the arithmetic on the device is theirs step for step, so the output equals the CPU transform's.
@@ -21,7 +22,7 @@ import numbers
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, jpeg
 
 __all__ = ["imagenet", "voc_segmentation", "ssd"]
 
@@ -83,12 +84,15 @@ def _pairs(idx, w):
 
 # ---- argument checks ---------------------------------------------------------------------------------------------------
 def _images(images, what="images", planes=3):
-    if isinstance(images, (np.ndarray, torch.Tensor)) or not hasattr(images, "__len__"):
+    if isinstance(images, (np.ndarray, torch.Tensor, bytes, bytearray, memoryview)) or not hasattr(images, "__len__"):
         raise _lib.DfqError("%s must be a list of uint8 arrays, got %s" % (what, type(images).__name__))
     if len(images) == 0:
         raise _lib.DfqError("%s: the batch is empty" % what)
     out = []
-    for i, a in enumerate(images):
+    for i, a in enumerate(jpeg.parse(images, what) if planes else images):
+        if isinstance(a, jpeg._Jpeg):
+            out.append(a)
+            continue
         if isinstance(a, torch.Tensor):
             if a.device.type != "cpu":
                 raise _lib.DfqError("%s[%d] is on %s: decoded images come from the host" % (what, i, a.device))
@@ -96,7 +100,8 @@ def _images(images, what="images", planes=3):
                 raise _lib.DfqError("%s[%d] must be uint8, got %s" % (what, i, a.dtype))
             a = a.numpy()
         elif not isinstance(a, np.ndarray):
-            raise _lib.DfqError("%s[%d] must be a numpy array or a CPU tensor, got %s" % (what, i, type(a).__name__))
+            raise _lib.DfqError("%s[%d] must be a numpy array, a CPU tensor%s, got %s"
+                                % (what, i, " or JPEG bytes" if planes else "", type(a).__name__))
         if a.dtype != np.uint8:
             raise _lib.DfqError("%s[%d] must be uint8, got %s" % (what, i, a.dtype))
         if planes and (a.ndim != 3 or a.shape[2] != planes):
@@ -148,53 +153,78 @@ def _device():
     return torch.device("cuda", torch.cuda.current_device())
 
 
+class _Stage:
+    """A batch gathered into one page-locked block: segments placed 64-byte aligned, tables shared by identity (images of
+    one size share their tap tables, JPEGs of one encoder their Huffman and quantisation tables)."""
+
+    def __init__(self):
+        self.segs, self.offs, self.total, self.tables = [], [], 0, {}
+
+    def place(self, a):
+        self.segs.append(a)
+        self.offs.append(self.total)
+        self.total += (a.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
+        return self.offs[-1]
+
+    def table(self, t):
+        key = id(t)
+        if key not in self.tables:
+            self.tables[key] = (self.place(t), t)
+        return self.tables[key][0]
+
+    def upload(self, extra=0):
+        """Gather into the staging block and move it with one host-to-device copy into a device block `extra` bytes longer
+        (room that only the device writes)."""
+        lib = _lib.load()
+        # A page-locked block of torch's caching host allocator: the non-blocking copy below records its stream on the
+        # block, so the block is handed out again (to a later batch of the same or a smaller size) only once that copy has
+        # completed, and the host never waits for it.
+        buf = _pinned(self.total)
+        ptrs = np.array([a.ctypes.data for a in self.segs], np.uintp)
+        nbytes = np.array([a.nbytes for a in self.segs], np.uintp)
+        offsets = np.array(self.offs, np.uintp)
+        _lib.check(lib.dfq_host_copy_segments(C.c_void_p(buf.data_ptr()), _lib.table_ptr(ptrs), _lib.table_ptr(nbytes),
+                                              _lib.table_ptr(offsets), len(self.segs), 0, 0), "dfq_host_copy_segments")
+        dev = _device()
+        if not extra:
+            return buf.to(dev, non_blocking=True)
+        blob = torch.empty(self.total + extra, dtype=torch.uint8, device=dev)
+        blob[:self.total].copy_(buf, non_blocking=True)
+        return blob
+
+
 def _launch(images, labels, xtaps, ytaps, near, filt, norm, out_h, out_w, mean, std):
-    """Gather the batch into the staging buffer, one H2D copy, one dfq_pre_resample launch."""
+    """Gather the batch into the staging buffer, one H2D copy, dfq_jpeg_decode when the batch holds JPEG bytes, one
+    dfq_pre_resample launch."""
     _lib.require_cuda()
     lib = _lib.load()
-    segs, offs, total = [], [], 0
-
-    def place(a):
-        nonlocal total
-        segs.append(a)
-        offs.append(total)
-        total += (a.nbytes + _ALIGN - 1) // _ALIGN * _ALIGN
-        return offs[-1]
-
-    tables = {}
-
-    def table(t):                                      # images of one size share their tables
-        key = id(t)
-        if key not in tables:
-            tables[key] = (place(t), t)
-        return tables[key][0]
-
+    stage = _Stage()
+    jpegs = jpeg._Batch(stage)
     n = len(images)
     desc = np.zeros(n, _lib.PRE_IMAGE_DT)
+    coded = {}
     for i, a in enumerate(images):
         d = desc[i]
         d["H"], d["W"] = a.shape[:2]
-        d["src"] = place(a)
-        d["xtap"], d["ytap"] = table(xtaps[i]), table(ytaps[i])
+        if isinstance(a, jpeg._Jpeg):
+            coded[i] = jpegs.add(a)
+        else:
+            d["src"] = stage.place(a)
+        d["xtap"], d["ytap"] = stage.table(xtaps[i]), stage.table(ytaps[i])
         d["xk"], d["yk"] = xtaps[i].shape[1], ytaps[i].shape[1]
         if labels is None:
             d["label"] = d["xnear"] = d["ynear"] = -1
         else:
-            d["label"] = place(labels[i])
-            d["xnear"], d["ynear"] = table(near[i][0]), table(near[i][1])
-    # A page-locked block of torch's caching host allocator: the non-blocking copy below records its stream on the block, so
-    # the block is handed out again (to a later batch of the same or a smaller size) only once that copy has completed,
-    # and the host never waits for it.
-    buf = _pinned(total)
-    ptrs = np.array([a.ctypes.data for a in segs], np.uintp)
-    nbytes = np.array([a.nbytes for a in segs], np.uintp)
-    offsets = np.array(offs, np.uintp)
-    _lib.check(lib.dfq_host_copy_segments(C.c_void_p(buf.data_ptr()), _lib.table_ptr(ptrs), _lib.table_ptr(nbytes),
-                                          _lib.table_ptr(offsets), len(segs), 0, 0), "dfq_host_copy_segments")
-    dev = _device()
-    blob = buf.to(dev, non_blocking=True)
+            d["label"] = stage.place(labels[i])
+            d["xnear"], d["ynear"] = stage.table(near[i][0]), stage.table(near[i][1])
+    for i, k in coded.items():                         # the decoded pixels go past every copied byte
+        desc[i]["src"] = jpegs.dst(k)
+    blob = stage.upload(jpegs.extra)
+    if coded:
+        jpegs.launch(blob)
+    dev = blob.device
     p = np.zeros(1, _lib.PRE_RESAMPLE_DT)
-    p["n"], p["out_h"], p["out_w"], p["filter"], p["norm"], p["blob_bytes"] = n, out_h, out_w, filt, norm, total
+    p["n"], p["out_h"], p["out_w"], p["filter"], p["norm"], p["blob_bytes"] = n, out_h, out_w, filt, norm, blob.numel()
     p["mean"], p["std"], p["mean64"], p["std64"] = mean, std, mean, std
     out = torch.empty(n, 3, out_h, out_w, dtype=torch.float32, device=dev)
     lab = torch.empty(n, out_h, out_w, dtype=torch.float32, device=dev) if labels is not None else None
@@ -210,8 +240,9 @@ def imagenet(images, resize=256, crop=224, mean=_IMAGENET_MEAN, std=_IMAGENET_ST
     Normalize(mean, std)]) of Image.fromarray(img) for each image, bit for bit (Pillow's antialiased bilinear; x / 255,
     - mean, / std each in fp32).  images: a list of uint8 HWC RGB numpy arrays or CPU tensors, each of its own size.
     mean, std: a number or 3 numbers (a tuple, list or numpy array).
-    An image whose resize is smaller than the crop (CenterCrop would pad) is refused.  Does not synchronise with the
-    host."""
+    Items may also be JPEG bytes (jpeg.probe says which are taken), decoded on the device as Pillow decodes them; a
+    batch may mix them with arrays.  An image whose resize is smaller than the crop (CenterCrop would pad) is refused.
+    Does not synchronise with the host."""
     imgs = _images(images)
     resize, crop = _positive("resize", resize), _positive("crop", crop)
     mean, std = _triple("mean", mean), _stds(std)
@@ -233,9 +264,9 @@ def voc_segmentation(images, labels=None, crop_size=513, mean=_IMAGENET_MEAN, st
     """(image float32 [N, 3, crop_size, crop_size], label float32 [N, crop_size, crop_size] or None) on the current device:
     VOCSegmentation.transform_val's sample['image'] and sample['label'], bit for bit.  FixScaleCrop(crop_size) resizes the
     short side to crop_size (Pillow bilinear for the image, nearest for the label) and center-crops; Normalize divides by
-    255 in fp32 and applies mean and std in fp64, each rounded back to fp32.  images as for imagenet(); labels: None or a
-    list of uint8 HW arrays of the images' sizes.  The label output is what segment.Evaluator.add_logits takes.  Does
-    not synchronise with the host."""
+    255 in fp32 and applies mean and std in fp64, each rounded back to fp32.  images as for imagenet() (JPEG bytes
+    included, EXIF orientation ignored as Pillow ignores it); labels: None or a list of uint8 HW arrays of the images'
+    sizes.  The label output is what segment.Evaluator.add_logits takes.  Does not synchronise with the host."""
     imgs = _images(images)
     labs = None
     if labels is not None:
@@ -272,8 +303,13 @@ def ssd(images, size=300, mean=127.0, std=128.0):
     PredictionTransform(size, mean, std)(img) bit for bit (cv2.resize INTER_LINEAR, float32(x) - float32(mean), / std in
     fp32); the sizes go to detect.postprocess(image_sizes=...).  mean: a number or 3 numbers (a tuple, list or numpy
     array, e.g. the configs' image_mean); std: a Python number (the configs' image_std).  images as for imagenet().
-    Does not synchronise with the host."""
+    Given JPEG bytes, decoded as cv2.imread decodes them; bytes with an EXIF orientation other than 1, which cv2.imread
+    would rotate, are refused.  Does not synchronise with the host."""
     imgs = _images(images)
+    for i, a in enumerate(imgs):
+        if isinstance(a, jpeg._Jpeg) and a.orientation != 1:
+            raise _lib.DfqError("images[%d] has EXIF orientation %d, which cv2.imread applies and the device decode does not: "
+                                "decode it with cv2.imread on the host" % (i, a.orientation))
     size = _positive("size", size)
     if type(std) not in (int, float):
         # a numpy scalar or array would make numpy divide the float32 image in float64 (NEP 50), a Python number in float32

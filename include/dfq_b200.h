@@ -45,7 +45,8 @@ const char* dfq_last_error(void);
 /* sizeof() of the descriptor structs as compiled (0 DfqLayer, 1 DfqRelation, 2 DfqCleParams,
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
- * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax, 21 DfqPreImage, 22 DfqPreResample; 20 is
+ * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax, 21 DfqPreImage, 22 DfqPreResample,
+ * 23 DfqJpegImage, 24 DfqJpegSegment, 25 DfqJpegDecode, 26 DfqJpegHuff, 27 DfqJpegTables; 20 is
  * unassigned and returns -1, as ABI 11 released it): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
@@ -873,6 +874,63 @@ typedef struct DfqPreResample {
  * order stated above, or the kernel reads outside the image.  dfq_b200.preprocess builds them so. */
 int dfq_pre_resample(const DfqPreResample* d, const DfqPreImage* images, const void* blob, float* out, float* labels,
                      void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * JPEG decoding: baseline sequential Huffman streams (SOF0 / SOF1, 8-bit, 1 component or 3 YCbCr components with luma
+ * sampling 1x1, 2x1 or 2x2 and chroma 1x1, one interleaved scan, any restart interval) decoded as libjpeg-turbo decodes
+ * them with its defaults (jpeg_idct_islow, fancy upsampling, ycc_rgb_convert), into uint8 HWC RGB
+ * ------------------------------------------------------------------------------------------- */
+/* One Huffman table as libjpeg's jpeg_make_d_derived_tbl derives it: maxcode[l] the largest code of length l (-1 when
+ * none, maxcode[17] 0xFFFFF), valoff[l] the index into vals of that length's first code minus the code, look[] the next
+ * 9 bits -> (length << 8 | symbol) for codes of up to 9 bits, 0 otherwise. */
+typedef struct DfqJpegHuff {
+  int32_t maxcode[18];
+  int32_t valoff[18];
+  uint16_t look[512];
+  uint8_t vals[256];
+} DfqJpegHuff;
+/* The tables of one stream, per component in frame order: the quantisation table in natural order and the scan's DC and
+ * AC Huffman tables.  Gray streams use entry 0 only. */
+typedef struct DfqJpegTables {
+  int32_t q[3][64];
+  DfqJpegHuff dc[3], ac[3];
+} DfqJpegTables;
+typedef struct DfqJpegImage {
+  int64_t dst;                   /* uint8 HWC RGB [H, W, 3] output: byte offset in the blob                           */
+  int64_t tables;                /* its DfqJpegTables: byte offset in the blob, 8-byte aligned                         */
+  int32_t H, W;
+  int32_t ncomp;                 /* 1 (gray, written as R = G = B) or 3 (YCbCr)                                        */
+  int32_t hs, vs;                /* luma sampling: 1x1, 2x1 or 2x2 (1x1 for gray); chroma is 1x1                       */
+  int32_t mcux, mcuy;            /* MCUs per row and per column: ceil(W / (8 hs)), ceil(H / (8 vs))                    */
+  int32_t _pad;
+} DfqJpegImage;
+/* One restart interval of one image: its entropy-coded bytes (byte stuffing included, the RSTn marker and fill bytes
+ * not), which decode MCUs mcu0 .. mcu0 + mcus - 1 with the DC predictors starting at zero. */
+typedef struct DfqJpegSegment {
+  int64_t begin, end;            /* byte offsets in the blob                                                           */
+  int32_t image;
+  int32_t mcu0, mcus;
+  int32_t _pad;
+} DfqJpegSegment;
+typedef struct DfqJpegDecode {
+  int32_t n, nseg;               /* images, segments: 1 .. 65535 images, 1 .. 2^31 - 1 segments                         */
+  int64_t blob_bytes;            /* size of the blob: every segment, table block and output must lie inside it          */
+  uint64_t call;                 /* tag of this call in the error word, below 2^31                                      */
+} DfqJpegDecode;
+#define DFQ_JPEG_BAD_CODE 1      /* error reasons, OR-ed into error[1]                                                 */
+#define DFQ_JPEG_BAD_RUN 2
+#define DFQ_JPEG_SHORT_SCAN 4
+/* Decodes every image of the batch into its dst.  images, segs: host arrays, uploaded by the call; blob: device pointer.
+ * error: device uint64 [2].  A segment found corrupt on the device (an invalid Huffman code, a run past coefficient 63,
+ * data that ends before its last MCU) stops that segment's decode, atomicMin's (call << 32 | image) into error[0] and
+ * OR's its reason into error[1]; that image's pixels are then unspecified, and no read or write leaves its segment, its
+ * tables or its output.  Workspace (int16 coefficients and the component planes) is allocated stream-ordered and freed
+ * by the call.  Does not synchronise.  DFQ_E_ARG, with a reason and before any launch: a NULL pointer, n or nseg out of
+ * range, an image of unsupported geometry or whose MCU counts disagree with its size, a table block, output or segment
+ * outside the blob, a segment whose image or MCUs are out of range, or segments that do not cover each image's MCUs
+ * exactly once in order. */
+int dfq_jpeg_decode(const DfqJpegDecode* d, const DfqJpegImage* images, const DfqJpegSegment* segs, void* blob,
+                    uint64_t* error, void* stream);
 
 #ifdef __cplusplus
 }

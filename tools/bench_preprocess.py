@@ -1,5 +1,6 @@
 """Evaluation preprocessing throughput on the H100: the reference's CPU transforms in DataLoader workers against workers
-that only decode, followed by dfq_b200.preprocess; prints one JSON line.
+that only decode, followed by dfq_b200.preprocess, and workers that only read the file, followed by the device decode of
+dfq_b200.jpeg and dfq_b200.preprocess; prints one JSON line.
 
     python tools/bench_preprocess.py [--batch 64] [--batches 12] [--workers 1,2,4,8]
 
@@ -10,14 +11,17 @@ synchronise).  Arms:
   reference   workers decode with PIL and run the reference's transform (torchvision Compose, FixScaleCrop + Normalize,
               cv2.resize + SubtractMeans + / std), the batch is copied to the device
   gpu         workers decode only; dfq_b200.preprocess forms the batch on the device
-Both arms' outputs are asserted equal on every timed batch.  Without a network behind the loop the rate is the ceiling the
+  bytes       workers return the file's bytes; dfq_b200.preprocess decodes them on the device and forms the batch
+All arms' outputs are asserted equal on every timed batch.  Without a network behind the loop the rate is the ceiling the
 input pipeline puts on an evaluation.  With --network, each main's loop is also timed at its own worker count with the
 chained affine int8 network (tests/affine_observed_state.py: MobileNetV2 at 224, DeepLab-v3+ at 513, SSD-Lite at 300,
 TF32 off) and the matching evaluation step behind it: the logits, segment.Evaluator.add_logits, detect.postprocess.
 Per main also: the whole preprocessing call per batch (CUDA events around calls on batches decoded beforehand, so the
 gather and the copy are in it) and the kernel alone (torch.profiler's device time of k_pre_resample, in a run of its own:
 events cannot bracket a kernel that the call enqueues behind its copy).  The card's name and power limit are read in the
-same run.  Needs a CUDA device; writes nothing.
+same run.  For the bytes arm also: the corpus's compressed / decoded byte ratio, the call time at batch 64 and 256, the
+device time of each decode phase (k_jpeg_huff, k_jpeg_idct, k_jpeg_color) and of k_pre_resample, and Pillow's decode
+rate on one core of this host for scale.  Needs a CUDA device; writes nothing.
 """
 import argparse
 import io
@@ -61,16 +65,18 @@ def _jpegs(sizes, n, seed):
 
 
 class _Set(torch.utils.data.Dataset):
-    def __init__(self, items, main, transform):
-        self.items, self.main, self.transform = items, main, transform
+    def __init__(self, items, main, mode):
+        self.items, self.main, self.mode = items, main, mode
 
     def __len__(self):
         return len(self.items)
 
     def __getitem__(self, i):
         jpg, lab = self.items[i]
+        if self.mode == "bytes":
+            return jpg, lab
         img = Image.open(io.BytesIO(jpg)).convert("RGB")
-        if not self.transform:                          # tensors: they leave the worker through shared memory
+        if self.mode == "gpu":                          # tensors: they leave the worker through shared memory
             return torch.from_numpy(np.asarray(img)), torch.from_numpy(lab)
         if self.main == "cls":
             return _cls()(img), lab
@@ -122,8 +128,9 @@ def _gpu(main, imgs, labs):
     return P.ssd(imgs, mean=(127, 127, 127))[0], None
 
 
-def _loop(main, items, batch, workers, transform, consume=None):
-    dl = torch.utils.data.DataLoader(_Set(items, main, transform), batch_size=batch, num_workers=workers,
+def _loop(main, items, batch, workers, mode, consume=None):
+    transform = mode == "reference"
+    dl = torch.utils.data.DataLoader(_Set(items, main, mode), batch_size=batch, num_workers=workers,
                                      collate_fn=_collate_ref if transform else _collate_list,
                                      persistent_workers=False, prefetch_factor=2)
     outs = []
@@ -181,14 +188,51 @@ def _with_network(main, items, batch, workers):
                     return detect.postprocess(*gm(x), priors=pri, center_variance=cv, size_variance=sv).boxes
         out = {}
         rates = []
-        for transform in (True, False):
-            rate, outs = _loop(main, items, batch, workers, transform, consume)
+        for mode in ("reference", "gpu", "bytes"):
+            rate, outs = _loop(main, items, batch, workers, mode, consume)
             rates.append(outs)
-            out["reference_img_s" if transform else "gpu_img_s"] = round(rate, 1)
-        for o0, o1 in zip(*rates):
-            assert torch.equal(o0, o1), main
+            out[mode + "_img_s"] = round(rate, 1)
+        for o0, o1, o2 in zip(*rates):
+            assert torch.equal(o0, o1) and torch.equal(o0, o2), main
         out["workers"] = workers
         return out
+
+
+def _bytes_arm(main, items, labs, batch):
+    """The device decode: byte ratio, call time at batch 64 and 256 (and `batch`), per-phase kernel times, Pillow's rate."""
+    from torch.profiler import ProfilerActivity, profile
+    from dfq_b200 import jpeg
+    dec = [np.asarray(Image.open(io.BytesIO(j)).convert("RGB")) for j, _ in items]
+    out = {"compressed_over_decoded": round(sum(len(j) for j, _ in items) / sum(d.nbytes for d in dec), 4)}
+    t0 = time.perf_counter()
+    for j, _ in items[:64]:
+        np.asarray(Image.open(io.BytesIO(j)).convert("RGB"))
+    out["pillow_decode_img_s_one_core"] = round(64 / (time.perf_counter() - t0), 1)
+    for n in sorted({64, 256, batch}):
+        js = [items[i % len(items)][0] for i in range(n)]
+        ls = [items[i % len(items)][1] for i in range(n)]
+        ds = [dec[i % len(items)] for i in range(n)]
+        want = _gpu(main, ds, ls)
+        got = _gpu(main, js, ls)
+        assert torch.equal(want[0], got[0]) and (want[1] is None or torch.equal(want[1], got[1])), (main, n)
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+        torch.cuda.synchronize()
+        ev[0].record()
+        for _ in range(10):
+            _gpu(main, js, ls)
+        ev[1].record()
+        torch.cuda.synchronize()
+        row = {"call_ms": round(ev[0].elapsed_time(ev[1]) / 10, 3)}
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(3):
+                _gpu(main, js, ls)
+            torch.cuda.synchronize()
+        for k in ("k_jpeg_huff", "k_jpeg_idct", "k_jpeg_color", "k_pre_resample"):
+            t = [e.device_time for e in prof.events() if k in e.name]
+            row[k + "_ms"] = round(sum(t) / max(len(t), 1) / 1e3, 3)
+        out["batch_%d" % n] = row
+    jpeg.check()
+    return out
 
 
 def main():
@@ -204,11 +248,14 @@ def main():
         items = _jpegs(sizes, a.batch * a.batches, seed=len(main))
         r = {"main_workers": own}
         for w in sorted(set(workers + [own])):
-            ref_rate, ref_out = _loop(main, items, a.batch, w, True)
-            gpu_rate, gpu_out = _loop(main, items, a.batch, w, False)
-            for (x0, y0), (x1, y1) in zip(ref_out, gpu_out):
+            ref_rate, ref_out = _loop(main, items, a.batch, w, "reference")
+            gpu_rate, gpu_out = _loop(main, items, a.batch, w, "gpu")
+            byte_rate, byte_out = _loop(main, items, a.batch, w, "bytes")
+            for (x0, y0), (x1, y1), (x2, y2) in zip(ref_out, gpu_out, byte_out):
                 assert torch.equal(x0, x1) and (y0 is None or torch.equal(y0, y1)), (main, w)
-            r["workers_%d" % w] = {"reference_img_s": round(ref_rate, 1), "gpu_img_s": round(gpu_rate, 1)}
+                assert torch.equal(x0, x2) and (y0 is None or torch.equal(y0, y2)), (main, w)
+            r["workers_%d" % w] = {"reference_img_s": round(ref_rate, 1), "gpu_img_s": round(gpu_rate, 1),
+                                   "bytes_img_s": round(byte_rate, 1)}
         dec = [np.asarray(Image.open(io.BytesIO(j)).convert("RGB")) for j, _ in items[:a.batch]]
         labs = [l for _, l in items[:a.batch]]
         for _ in range(3):
@@ -228,6 +275,7 @@ def main():
             torch.cuda.synchronize()
         k = [e.device_time for e in prof.events() if "k_pre_resample" in e.name]
         r["kernel_ms_per_batch"] = round(sum(k) / max(len(k), 1) / 1e3, 3)
+        r["bytes"] = _bytes_arm(main, items, labs, a.batch)
         if a.network:
             r["with_network"] = _with_network(main, items, a.batch, own)
         res["mains"][main] = r
