@@ -330,6 +330,58 @@ class Evaluator:
         self._count += T
         self._gt_total += G
 
+    def all_reduce(self, group=None) -> "Evaluator":
+        """A new Evaluator holding the batches of every rank of `group` (the default group when None), on every rank; this
+        one is left as it is.  Every rank must call it, with the same num_classes, also a rank that added no batch.
+
+        The match records (sort key and verdict of every detection) are concatenated in rank order, so with the dataset
+        split by dist.shard they stand in dataset order, the order one process would have added them in.  dfq_map_curve's
+        sort is stable, so detections of equal score then come out in the one-process order and average_precision() is
+        bit for bit the one-process value.  The ground-truth counts are summed and the device error words OR-ed, so a bad
+        label or offset on any rank raises in average_precision() on every rank.  Two all-gathers: the per-rank sizes with
+        the counts and error word (one host synchronisation), then the records, padded to the longest rank's.  A union of
+        more than MAX_MAP_DETECTIONS detections is refused on every rank."""
+        from . import dist as ddist
+        Cn = self.num_classes
+        dev = self.device if self.device is not None else ddist._idle_device()
+        head = torch.zeros(3 + Cn, dtype=torch.int64, device=dev)       # count, gt_total, error, gt_count [C]
+        head[0], head[1] = self._count, self._gt_total
+        if self._gt_count is not None:
+            head[2:3].copy_(self._error)
+            head[3:].copy_(self._gt_count)
+        heads = ddist._gather_rows(head, group)
+        sizes = heads[:, :2].cpu().tolist()
+        counts = [c for c, _ in sizes]
+        total = sum(counts)
+        if total > MAX_MAP_DETECTIONS:
+            raise _lib.DfqError("detect.Evaluator.all_reduce: the ranks hold %d detections in all (%s), above "
+                                "MAX_MAP_DETECTIONS = %d" % (total, " + ".join(map(str, counts)), MAX_MAP_DETECTIONS))
+        out = Evaluator(Cn, self.iou_threshold, self.use_2007_metric)
+        out.device = dev
+        out._gt_count = heads[:, 3:].sum(0)
+        error = heads[0, 2]
+        for r in range(1, heads.shape[0]):
+            error = error | heads[r, 2]
+        out._error = error.to(torch.int32).reshape(1)
+        out._gt_total = sum(g for _, g in sizes)
+        cap = max(counts)
+        if cap:
+            # one uint8 row per rank: keys (8 bytes each) then verdicts, padded to the longest rank's count and to 8 bytes
+            send = torch.zeros(8 * cap + (cap + 7) // 8 * 8, dtype=torch.uint8, device=dev)
+            if self._count:
+                send[:8 * self._count].copy_(self._keys[:self._count].view(torch.uint8))
+                send[8 * cap:8 * cap + self._count].copy_(self._flags[:self._count])
+            recs = ddist._gather_rows(send, group)
+            out._reserve(total)
+            o = 0
+            for r, c in enumerate(counts):
+                if c:
+                    out._keys[o:o + c].copy_(recs[r, :8 * c].view(torch.int64))
+                    out._flags[o:o + c].copy_(recs[r, 8 * cap:8 * cap + c])
+                    o += c
+            out._count = total
+        return out
+
     def _reserve(self, n):
         """Room for n detections in the accumulation buffers, grown on the device (no synchronisation)."""
         cap = 0 if self._keys is None else self._keys.shape[0]

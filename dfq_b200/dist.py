@@ -21,6 +21,10 @@ Convergence (dfq.py:81-115 is a GLOBAL rule: sum over all layers):
 
 Replaying S (step 4) applies the accumulated product in one multiplication instead of one per sweep: owner ranks hold
 bit-exact values, replicas agree to ~3e-6 relative (SURVEY 8e).
+
+Sharded evaluation (DESIGN.md section 3.14): `shard` gives each rank a contiguous block of the dataset, and the
+classify, segment and detect evaluators' `all_reduce` merge the ranks' evaluators into the one-process result through
+`_gather_rows` below.
 """
 from __future__ import annotations
 
@@ -42,6 +46,44 @@ def _all_gather_flat(recv: torch.Tensor, send: torch.Tensor, group=None):
         recv.copy_(r)
     else:
         dist.all_gather_into_tensor(recv, send, group=group)
+
+
+def _world_rank(group=None) -> Tuple[int, int]:
+    if not dist.is_initialized():
+        return 1, 0
+    return dist.get_world_size(group), dist.get_rank(group)
+
+
+def shard(n: int, group=None) -> range:
+    """This rank's share of a dataset of n items for sharded evaluation: one contiguous block per rank, in rank order, the
+    first n % world ranks taking one item more.  A rank may get an empty range.  Without a process group, or with one
+    rank, range(n).
+
+    torch.utils.data.DistributedSampler is not a substitute: it deals items to the ranks in turn and pads the last round
+    by repeating items, so repeated images are counted twice, and the detection evaluator's order among equal scores (the
+    order images were added, DESIGN.md section 4) is no longer the dataset's order.  With shard(), the ranks' blocks
+    concatenated in rank order are range(n), which is what the evaluators' all_reduce() relies on."""
+    if isinstance(n, bool) or not isinstance(n, int) or n < 0:
+        raise ValueError("shard: n must be a non-negative int, got %r" % (n,))
+    world, rank = _world_rank(group)
+    base, extra = divmod(n, world)
+    start = rank * base + min(rank, extra)
+    return range(start, start + base + (rank < extra))
+
+
+def _idle_device() -> torch.device:
+    """Where an evaluator that never received a batch stages its (zero) share of a reduction: the current CUDA device."""
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _gather_rows(send: torch.Tensor, group=None) -> torch.Tensor:
+    """[world, n]: every rank's 1-D `send` (n elements on every rank), in rank order.  One process: send as one row."""
+    world, _ = _world_rank(group)
+    if world == 1:
+        return send.reshape(1, -1).clone()
+    recv = torch.empty(world * send.numel(), dtype=send.dtype, device=send.device)
+    _all_gather_flat(recv, send.contiguous(), group)
+    return recv.view(world, -1)
 
 
 def build_chains(relations) -> List[List[int]]:

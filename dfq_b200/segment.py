@@ -126,6 +126,18 @@ class Evaluator:
         if self.counts is not None:
             self.counts.zero_()
 
+    def all_reduce(self, group=None) -> "Evaluator":
+        """A new Evaluator whose matrix is the sum of every rank's in `group` (the default group when None), on every rank;
+        this one is left as it is.  Every rank must call it, also a rank that added no batch.  The matrix is int64, so the
+        sum is exact: the result is what one process adding every rank's batches holds.  See dist.shard for the split."""
+        from . import dist as ddist
+        dev = self.counts.device if self.counts is not None else ddist._idle_device()
+        send = self.counts if self.counts is not None else \
+            torch.zeros(self.num_class, self.num_class, dtype=torch.int64, device=dev)
+        out = Evaluator(self.num_class)
+        out.counts = ddist._gather_rows(send.reshape(-1), group).sum(0).view(self.num_class, self.num_class)
+        return out
+
     @property
     def confusion_matrix(self):
         """float64 numpy [num_class, num_class], rows the labels and columns the predictions, as the reference keeps it."""

@@ -788,6 +788,20 @@ int dfq_seg_argmax(const float* logits, const void* labels, int64_t* pred, uint6
                    void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Classification accuracy (main_cls.py inference_all), counted on the device
+ * ------------------------------------------------------------------------------------------- */
+/* Per row n of logits fp32 [N, C] (contiguous): the argmax of the row under torch's CUDA max(dim) rule (as
+ * dfq_seg_argmax: the first NaN wins over every number, otherwise the larger value, and on equal values, -0.0 equal to
+ * +0.0, the lower index).  pred (int64 [N], optional) receives it.  correct (uint64 [1], optional, accumulated: the caller
+ * clears it) receives the number of rows whose label (labels int64 [N]) equals the argmax; a label outside 0 .. C-1
+ * never does.  labels and correct are both given or both NULL; at least one of pred and correct is given.  Does not
+ * synchronise.  DFQ_E_ARG, with a reason and before any write: N or C below 1, logits NULL, labels without correct or
+ * correct without labels, neither pred nor correct, a pointer not aligned to its element, correct or pred overlapping
+ * another buffer.  DFQ_E_UNSUPPORTED: 2^60 logits or more. */
+int dfq_cls_count(const float* logits, const int64_t* labels, int64_t* pred, uint64_t* correct, int64_t N, int32_t C,
+                  void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * VOC average precision of SSD detections (main_ssd.py compute_average_precision_per_class,
  * utils/detection/measurements.py), accumulated batch by batch
  * ------------------------------------------------------------------------------------------- */
