@@ -156,6 +156,11 @@ JPEG_SIZES = {23: (JPEG_IMAGE_DT, 48), 24: (JPEG_SEGMENT_DT, 32), 25: (JPEG_DECO
 MAP_IGNORED, MAP_TP, MAP_FP = 0, 1, 2                  # verdicts of dfq_map_match
 MAP_ERR_DET_LABEL, MAP_ERR_GT_LABEL, MAP_ERR_DET_OFFSETS, MAP_ERR_GT_OFFSETS = 1, 2, 4, 8   # its device error bits
 
+# dfq_bias_correct_absorb_clip's relation table (include/dfq_b200.h), struct-size index 28
+ABSORB_DT = np.dtype([("first", np.int32), ("second", np.int32), ("n", np.int32), ("_pad", np.int32),
+                      ("bn_w_off", np.int64), ("bn_b_off", np.int64), ("c_off", np.int64)], align=True)
+ABSORB_SIZES = {28: (ABSORB_DT, 40)}
+
 # sizes the C side uses (checked in tests against sizeof via the header's layout rules)
 EXPECTED_SIZES = {
     "DfqLayer": (LAYER_DT, 88), "DfqRelation": (RELATION_DT, 64), "DfqCleParams": (CLE_PARAMS_DT, 48),
@@ -196,6 +201,8 @@ SIGNATURES = {
     "dfq_cle_takes_stack": [C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, C.c_void_p, _I32, _I32, C.c_void_p],
     "dfq_bn_fold": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, _ST],
     "dfq_bias_correct": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, _I32, _ST],
+    "dfq_bias_correct_absorb_clip": [_PF, _I64, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, C.c_void_p, _I32, _I32,
+                                     C.c_void_p, _I32, C.c_float, _I32, C.c_float, C.c_float, _ST],
     "dfq_quantize_tensors": [_PF, _I64, C.c_void_p, _I32, C.c_int, _ST],
     "dfq_minmax": [_PF, _I64, _PF, _ST],
     "dfq_quant_dequant": [_PF, _PF, _I64, C.c_float, C.c_double, C.c_float, C.c_float, C.c_int, _PF, _ST],

@@ -9,18 +9,27 @@ graph once, stages the model ONCE (one pinned H2D copy), runs 3-4 kernel launche
     cal.run(equalize=True, correction=True, quantize_bits=(8, 16))      # same results as the four separate calls
     cal.relations                                                        # utils.relation.Relation objects with .S set
 
-Semantics are those of the separate calls in the reference's order (fold -> equalize -> [absorb/clip not included] ->
-correct -> quantize); it is exercised against them in tests/test_gpu_pipeline.py.
+Semantics are those of the separate calls in the reference's order (fold -> equalize -> absorb -> clip -> correct ->
+quantize, main_cls.py:149-181); it is exercised against them in tests/test_gpu_pipeline.py and
+tests/test_gpu_calibrate_absorb_clip.py.  The mains' --absorption and --clip_weight flags:
+
+    cal.run(equalize=True, absorption=True, clip_weight=(-15, 15), correction=True, quantize_bits=(8, 16))
+
+run inside the same residency: the absorption vectors are formed on the device, and the correction reads each weight row
+once to add its absorption dot, clamp it and take its quantization error (dfq_bias_correct_absorb_clip).
 """
 from __future__ import annotations
 
+import math
 from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 
+from ._lib import DfqError
 from .engine import CleResult, Session
-from .graphwalk import bias_correction_recipe
+from .graphwalk import bias_correction_recipe, relu_between
 from .utils.layer_transform import _identity_bn_eps
 from .utils.relation import create_relation
 
@@ -102,14 +111,63 @@ class GraphCalibration:
             self._bc_plan = sess.plan_bias_correct(items) if items else None
             self._quant_plan = None
             self._quant_bits = None
+            self._absorb = None       # plan_absorb's table, planned on the first run that absorbs
+            self._absorb_raw = None   # the absorption alone as raw-sum correction entries (runs without the correction)
         self.last_cle: Optional[CleResult] = None
+
+    @staticmethod
+    def _check_flags(absorption_n, clip_weight):
+        """The refusals of absorption_n and clip_weight, before anything is planned or launched."""
+        try:
+            n = float(absorption_n)
+        except (TypeError, ValueError):
+            raise DfqError("absorption_n must be a number, got %r" % (absorption_n,)) from None
+        with np.errstate(over="ignore"):             # the library takes N as a float32: beyond its range it is inf
+            if not (math.isfinite(n) and np.isfinite(np.float32(n))):
+                raise DfqError("absorption_n must be finite in float32, got %r" % (absorption_n,))
+        if clip_weight is not None:
+            try:
+                lo, hi = (float(v) for v in clip_weight)
+            except (TypeError, ValueError):
+                raise DfqError("clip_weight must be a (lo, hi) pair of numbers, got %r" % (clip_weight,)) from None
+            with np.errstate(over="ignore"):         # a bound beyond float32 becomes inf: refused like inf itself
+                lo, hi = np.float32(lo), np.float32(hi)
+            if not (np.isfinite(lo) and np.isfinite(hi) and lo <= hi):
+                raise DfqError("clip_weight must be two finite numbers with lo <= hi, got %r" % (clip_weight,))
+
+    def plan_absorption(self):
+        """Plan the absorption: which relations absorb (a torch.nn.ReLU between the layers, dfq.py:123-130) and their c
+        vectors.  run() does it before its upload.  A caller that drives upload() / run_device() / download() itself calls it
+        before upload(): planned later, the first run_device(absorption=True) grows the arena on the device."""
+        if self._absorb is not None:
+            return
+        table, items = [], []
+        for rr in self.relations:
+            a, b, bn_key = rr.get_idxs()
+            if relu_between(self.graph, self.bottoms, b, a):
+                v = self._bn[bn_key]
+                table.append((self._layer[a], self._layer[b], v["fake_w"], v["fake_b"]))
+        self._absorb = self.sess.plan_absorb(table)
+        for t in self._absorb:        # without the correction: (sum_k W) . c added to the bias (dfq.py:150-153,164)
+            c = int(t["c_off"])
+            items.append(dict(layer=int(t["second"]), signed=False, level=0, next_bn_b_off=-1, raw_sum=True, add=True,
+                              terms=[dict(bn_w_off=c, bn_b_off=c, n=int(t["n"]), relu=False, op="set")]))
+        self._absorb_raw = self.sess.plan_bias_correct(items) if items else None
 
     # -- device-resident pieces (bench: time them separately) -----------------------------------------------------------
     def upload(self):
+        """Stage the model in the arena (one H2D copy).  To absorb in the runs that follow, plan_absorption() first."""
         self.sess.upload()
 
     def run_device(self, equalize=True, correction=True, quantize_bits: Optional[Tuple[int, int]] = None, signed=False,
-                   s_range=(1e-8, 1e8), converge_thres=2e-7, converge_count=20, eps=0):
+                   s_range=(1e-8, 1e8), converge_thres=2e-7, converge_count=20, eps=0, absorption=False, absorption_n=3,
+                   clip_weight: Optional[Tuple[float, float]] = None):
+        """absorption: bias_absorption(relations, bottoms, absorption_n) after the equalization (dfq.py:121-164);
+        clip_weight: (lo, hi), clip_weight(graph, [lo, hi], targ) after it (dfq.py:167-170).  Both run inside the
+        correction's pass over the weights; neither adds a transfer or a host synchronisation."""
+        self._check_flags(absorption_n, clip_weight)
+        if absorption:
+            self.plan_absorption()
         sess = self.sess
         run_cle = equalize and self._cle_plan is not None
         scan = run_cle and self._fold_plan_scan is not None
@@ -120,12 +178,21 @@ class GraphCalibration:
             self.last_cle = sess.run_cle_plan(self._cle_plan, s_range, converge_thres, converge_count, signed, eps,
                                               cols_ready=self._fold_plan_scan["scanned"] if scan else None)
             hints = sess.cle_col_hints(self._cle_plan, self.last_cle)   # weights stay untouched until the correction
+        absorb = self._absorb if absorption and len(self._absorb) else None
+        clip = tuple(clip_weight) if clip_weight is not None else None
         if correction and self._bc_plan is not None:
             if signed:
                 for it in self._bc_items:
                     it["signed"] = True
                 self._bc_plan = sess.plan_bias_correct(self._bc_items)
-            sess.run_bias_correct_plan(self._bc_plan, 8, col_hints=hints)          # quirk Q2: always 8 bits (dfq.py:218)
+            if absorb is not None or clip is not None:
+                sess.run_bias_correct_absorb_clip(self._bc_plan, 8, col_hints=hints, absorb=absorb, absorb_n=absorption_n,
+                                                  clip=clip)
+            else:
+                sess.run_bias_correct_plan(self._bc_plan, 8, col_hints=hints)      # quirk Q2: always 8 bits (dfq.py:218)
+        elif absorb is not None or clip is not None:
+            sess.run_bias_correct_absorb_clip(self._absorb_raw if absorb is not None else None, 8, absorb=absorb,
+                                              absorb_n=absorption_n, clip=clip)
         if quantize_bits is not None:
             if self._quant_plan is None or self._quant_bits != tuple(quantize_bits):
                 bw, bb = quantize_bits
@@ -159,7 +226,11 @@ class GraphCalibration:
                     rr.set_scale_vec(s.clone())
 
     def run(self, **kw):
-        """upload -> fold/equalize/correct/quantize on the device -> download (results in place in the modules)."""
+        """upload -> fold/equalize/[absorb/clip]/correct/quantize on the device -> download (results in place in the modules).
+        Keywords: those of run_device."""
+        self._check_flags(kw.get("absorption_n", 3), kw.get("clip_weight"))
+        if kw.get("absorption"):
+            self.plan_absorption()
         self.upload()
         self.run_device(**kw)
         self.download()

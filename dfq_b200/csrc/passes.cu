@@ -2,13 +2,16 @@
 //
 //   dfq_bn_fold           utils/layer_transform.py:231-276  (merge_batchnorm)
 //   dfq_bias_correct      dfq.py:173-293                    (bias_correction)
+//   dfq_bias_correct_absorb_clip  dfq.py:121-170 + 173-293  (bias_absorption, clip_weight, bias_correction)
 //   dfq_quantize_tensors  utils/layer_transform.py:279-296  (quantize_targ_layer)
 #include <cooperative_groups.h>
 
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
+#include <functional>
 #include <vector>
 
 #include "common.cuh"
@@ -478,10 +481,118 @@ __device__ __forceinline__ double bc_row(const float* __restrict__ row, int cols
   return warp_sum(acc);
 }
 
+// ---- bias absorption and weight clipping inside the correction (dfq_bias_correct_absorb_clip) ----------------------
+// Per correction entry: the absorption vector c whose dot (sum_k W) . c the row adds to its bias before the clip (the entry's
+// layer is the `second` of an absorbing relation, dfq.py:150-153,164), and the c it then subtracts (the layer is that
+// relation's `first`, dfq.py:162).  -1: none.
+struct AcSlot { int64_t wc_c_off, sub_c_off; int32_t wc_so, _pad; };   // wc_so: rows per group of c
+struct AcArgs { const AcSlot* slot; float lo, hi; int clip; };
+
+// The per-tensor range of a clipped weight: clamping is monotonic, so min/max of the clamped tensor are the clamped min/max.
+__device__ __forceinline__ QuantScalars bc_scalars(const float* arena, const DfqBcLayer& b, int num_bits, const AcArgs* ac) {
+  float mn = __ldcg(arena + b.minmax_off), mx = __ldcg(arena + b.minmax_off + 1);
+  if (ac && ac->clip) { mn = clamp_nan(mn, ac->lo, ac->hi); mx = clamp_nan(mx, ac->lo, ac->hi); }
+  return quant_scalars((double)mn, (double)mx, num_bits, b.signed_mode);
+}
+
+// One output row with absorption and clipping, in ONE sweep over its taps (`row`: shared or global memory; `grow`: the row in
+// the arena).  Per column: the raw tap sum before the clip, the clamped taps written back to the arena where they changed,
+// and the quantization error QE on the clamped taps (raw entries: the raw sum).  acc: eps . E[x] (raw: sum_k W . E[x]);
+// wacc: sum_k W . cv (cv = nullptr: none).  Same per-lane order and arithmetic as bc_row / bc_stream_row_*: bc_row's
+// `acc += (double)E * (double)ex` (a separate mul.rn.f64 + add.rn.f64 under --fmad=false) and the __fma_rn here give the same
+// double, because the product of two floats is exact in double (24 + 24 significant bits <= 53, exponents far inside the
+// double range), so the multiply never rounds and both forms round once, at the add (tests/test_calibrate_absorb_clip_host.py
+// ::test_float_products_are_exact_in_double).
+template <int TPR, class QE>
+__device__ __forceinline__ void bc_row_ac(const float* row, float* grow, int cols, int kk, const float* __restrict__ ex,
+                                          const float* __restrict__ cv, bool raw, const AcArgs& ac, const QE& qe, int lane,
+                                          double& acc, double& wacc) {
+  acc = 0.0; wacc = 0.0;
+  for (int j = lane; j < cols; j += TPR) {
+    const float* p = row + (size_t)j * kk;
+    float* gp = grow + (size_t)j * kk;
+    float R = 0.f, E = 0.f;
+    for (int k = 0; k < kk; ++k) {
+      const float w0 = p[k];
+      R = __fadd_rn(R, w0);
+      float w = w0;
+      if (ac.clip) {
+        w = clamp_nan(w0, ac.lo, ac.hi);
+        if (__float_as_uint(w) != __float_as_uint(w0)) gp[k] = w;
+      }
+      if (!raw) E = __fadd_rn(E, qe(w));
+    }
+    acc = __fma_rn((double)(raw ? R : E), (double)ex[j], acc);
+    if (cv) wacc = __fma_rn((double)R, (double)__ldcg(cv + j), wacc);
+  }
+  acc = warp_sum(acc);
+  wacc = warp_sum(wacc);
+}
+
+__device__ __forceinline__ void bc_fetch_row_ac(const float* arena, const DfqLayer& l, const DfqBcLayer& b, const AcSlot& a, int o,
+                                                float& old_bias, float& old_next, float& csub) {
+  bc_fetch_row(arena, l, b, o, old_bias, old_next);
+  if (a.sub_c_off >= 0) csub = __ldcg(arena + a.sub_c_off + o);
+}
+// The bias rounds in the order of the separate calls: fl(fl(fl(b + wc) - c) - delta) (dfq.py:164, :162, :292); a raw entry
+// is the absorption itself: fl(fl(b + wc) - c).
+__device__ __forceinline__ void bc_retire_row_ac(float* arena, const DfqLayer& l, const DfqBcLayer& b, const AcSlot& a, int o,
+                                                 float dl, float wc, float old_bias, float old_next, float csub) {
+  const bool raw = (b.flags & 1) != 0;
+  const float d = (b.flags & 2) ? dl : -dl;
+  float nb = old_bias;
+  if (raw) nb = __fadd_rn(nb, d);
+  else if (a.wc_c_off >= 0) nb = __fadd_rn(nb, wc);
+  if (a.sub_c_off >= 0) nb = __fsub_rn(nb, csub);
+  if (!raw) nb = __fadd_rn(nb, d);
+  __stcg(arena + b.delta_off + o, dl);
+  __stcg(arena + l.bias_off + o, nb);
+  if (b.next_bn_b_off >= 0) __stcg(arena + b.next_bn_b_off + o, __fadd_rn(old_next, -dl));
+}
+
+// c = clamp(fake_bias - N * fake_weight, 0) of every absorbing relation (dfq.py:143-144), fake_bias -= c (:163), and
+// first.bias -= c (:162) where no correction entry of `first` does it after its own absorption.  A CTA per relation.
+__global__ void k_absorb_vectors(float* arena, const DfqAbsorb* __restrict__ A, int nA, const int64_t* __restrict__ first_bias,
+                                 float N) {
+  for (int i = blockIdx.x; i < nA; i += gridDim.x) {
+    const DfqAbsorb a = A[i];
+    const int64_t fb_off = first_bias[i];
+    for (int o = threadIdx.x; o < a.n; o += blockDim.x) {
+      const float fb = __ldcg(arena + a.bn_b_off + o);
+      float c = __fsub_rn(fb, __fmul_rn(N, __ldcg(arena + a.bn_w_off + o)));
+      c = c < 0.f ? 0.f : c;                   // clamp_(0): NaN stays NaN
+      __stcg(arena + a.c_off + o, c);
+      __stcg(arena + a.bn_b_off + o, __fsub_rn(fb, c));
+      if (fb_off >= 0) __stcg(arena + fb_off + o, __fsub_rn(__ldcg(arena + fb_off + o), c));
+    }
+  }
+}
+
+// Weights that no correction entry reads, clamped to [lo, hi] (dfq.py:167-170): one launch for all of them.
+struct ClipTask { int64_t off, n; };
+__global__ void __launch_bounds__(kThreads) k_clip_tensors(float* arena, const ClipTask* __restrict__ T, int nT, float lo, float hi) {
+  for (int t = 0; t < nT; ++t) {
+    float* x = arena + T[t].off;
+    const int64_t n = T[t].n;
+    for (int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
+      const float w0 = ldg_stream1(x + i), w = clamp_nan(w0, lo, hi);
+      if (__float_as_uint(w) != __float_as_uint(w0)) x[i] = w;
+    }
+  }
+}
+
+struct EngineQE {            // k_bc_engine's quantization error of one weight
+  QuantScalars q;
+  __device__ __forceinline__ float operator()(float w) const { return __fsub_rn(fake_quant<false>(w, q), w); }
+};
+
+// AC: absorption and clipping (dfq_bias_correct_absorb_clip); false: dfq_bias_correct, unchanged.
+template <bool AC>
 __global__ void __launch_bounds__(kThreads, kPipeCtas)
 k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __restrict__ B, int nB,
             const DfqExpectTerm* __restrict__ T, const int* __restrict__ level_ptr, int n_levels, int num_bits,
-            const long long* __restrict__ row_ptr, const long long* __restrict__ mm_ptr, const int* __restrict__ level_local) {
+            const long long* __restrict__ row_ptr, const long long* __restrict__ mm_ptr, const int* __restrict__ level_local,
+            AcArgs ac) {
   cg::grid_group grid = cg::this_grid();
   __shared__ float red[2 * kWarps];
   __shared__ double dred[kWarps];
@@ -558,13 +669,19 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
       for (int i = 0; i < kPipeStages - 1 && ahead.valid(); ++i) { ahead.fill(nd); pipe.issue(nd); ahead.next(); }
     int cur = -1;
     DfqBcLayer b; DfqLayer l; QuantScalars q; int so = 1, ex_cached = 0;
+    AcSlot a;
     while (it.valid()) {
       const int sidx = pipe.acquire();
       const TileDesc d = pipe.desc[sidx];
       if (d.task != cur) {
         cur = d.task;
         b = B[cur]; l = L[b.layer];
-        q = quant_scalars((double)__ldcg(arena + b.minmax_off), (double)__ldcg(arena + b.minmax_off + 1), num_bits, b.signed_mode);
+        if constexpr (AC) {
+          q = bc_scalars(arena, b, num_bits, &ac);
+          a = ac.slot[cur];
+        } else {
+          q = quant_scalars((double)__ldcg(arena + b.minmax_off), (double)__ldcg(arena + b.minmax_off + 1), num_bits, b.signed_mode);
+        }
         so = l.rows / (b.expect_len / l.cols);
         ex_cached = (b.expect_len <= kExpectCache);
         __syncthreads();
@@ -577,7 +694,48 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
       }
       const int row_len = l.cols * l.kk;
       const bool raw = (b.flags & 1) != 0;
-      if (d.nrows == 1) {
+      if constexpr (AC) {
+        __shared__ double wred[kWarps];
+        const EngineQE qe{q};
+        if (d.nrows == 1) {
+          const int o = d.row0;
+          const float* row = (d.kind == TK_DIRECT) ? d.gptr : pipe.stage[sidx];
+          const float* ex = (ex_cached ? s_ex : arena + b.expect_off) + (size_t)(o / so) * l.cols;
+          const float* cv = a.wc_c_off >= 0 ? arena + a.wc_c_off + (size_t)(o / a.wc_so) * l.cols : nullptr;
+          float old_bias = 0.f, old_next = 0.f, csub = 0.f;
+          if (threadIdx.x == 0) bc_fetch_row_ac(arena, l, b, a, o, old_bias, old_next, csub);
+          double acc, wacc;
+          bc_row_ac<kThreads>(row, d.gptr, l.cols, l.kk, ex, cv, raw, ac, qe, threadIdx.x, acc, wacc);
+          if (lane == 0) { dred[warp] = acc; wred[warp] = wacc; }
+          __syncthreads();
+          if (threadIdx.x == 0) {
+            acc = 0.0; wacc = 0.0;
+#pragma unroll
+            for (int i = 0; i < kWarps; ++i) { acc += dred[i]; wacc += wred[i]; }
+            bc_retire_row_ac(arena, l, b, a, o, (float)acc, (float)wacc, old_bias, old_next, csub);
+          }
+        } else {
+          const int mine = (d.nrows - warp + kWarps - 1) / kWarps;
+          for (int base = 0; base < mine; base += 32) {
+            const int il = base + lane;
+            const int ol = d.row0 + warp + il * kWarps;
+            float old_bias = 0.f, old_next = 0.f, csub = 0.f, dl = 0.f, wl = 0.f;
+            if (il < mine) bc_fetch_row_ac(arena, l, b, a, ol, old_bias, old_next, csub);
+            const int nb = min(32, mine - base);
+            for (int j = 0; j < nb; ++j) {
+              const int r = warp + (base + j) * kWarps;
+              const int o = d.row0 + r;
+              const float* ex = (ex_cached ? s_ex : arena + b.expect_off) + (size_t)(o / so) * l.cols;
+              const float* cv = a.wc_c_off >= 0 ? arena + a.wc_c_off + (size_t)(o / a.wc_so) * l.cols : nullptr;
+              double acc, wacc;
+              bc_row_ac<32>(pipe.stage[sidx] + (size_t)r * row_len, d.gptr + (size_t)r * row_len, l.cols, l.kk, ex, cv, raw, ac,
+                            qe, lane, acc, wacc);
+              if (lane == j) { dl = (float)acc; wl = (float)wacc; }
+            }
+            if (il < mine) bc_retire_row_ac(arena, l, b, a, ol, dl, wl, old_bias, old_next, csub);
+          }
+        }
+      } else if (d.nrows == 1) {
         const int o = d.row0;
         const float* row = (d.kind == TK_DIRECT) ? d.gptr : pipe.stage[sidx];
         const float* ex = (ex_cached ? s_ex : arena + b.expect_off) + (size_t)(o / so) * l.cols;
@@ -631,10 +789,17 @@ k_bc_engine(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
 static_assert(kPipeMaxRows <= 32, "a consumer warp retires one row per lane");
 
 
+struct StreamQE {            // k_bc_stream's quantization error of one weight (mode 0: XU-free, 1: IEEE chain)
+  BcFastQuant f; int mode;
+  __device__ __forceinline__ float operator()(float w) const { return mode == 0 ? bc_qerr_own_range(w, f) : bc_qerr<false>(w, f); }
+};
+
+// AC: absorption and clipping (dfq_bias_correct_absorb_clip); false: dfq_bias_correct, unchanged.
+template <bool AC>
 __global__ void __launch_bounds__(kBcThreads, 1)
 k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __restrict__ B, int nB,
             const DfqExpectTerm* __restrict__ T, const int* __restrict__ level_ptr, int n_levels, int num_bits,
-            const long long* __restrict__ row_ptr, const long long* __restrict__ mm_ptr) {
+            const long long* __restrict__ row_ptr, const long long* __restrict__ mm_ptr, AcArgs ac) {
   cg::grid_group grid = cg::this_grid();
   extern __shared__ __align__(128) unsigned char ring_smem[];
   BcRing ring;
@@ -698,6 +863,7 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
     } else {
       int cur = -1, cur_group = -1, so = 1;
       DfqBcLayer b; DfqLayer l; BcFastQuant f;
+      AcSlot a;
       int mode = 1;                                  // 0: XU-free arithmetic, 1: IEEE chain, 2: raw sums (bias absorption)
       bool excached = false;
       float* exs = ring.ex_cache(warp);
@@ -709,8 +875,13 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         if (d.task != cur) {
           cur = d.task; cur_group = -1;
           b = B[cur]; l = L[b.layer];
-          f = bc_fast_quant(quant_scalars((double)__ldcg(arena + b.minmax_off), (double)__ldcg(arena + b.minmax_off + 1),
-                                          num_bits, b.signed_mode), num_bits);
+          if constexpr (AC) {
+            f = bc_fast_quant(bc_scalars(arena, b, num_bits, &ac), num_bits);
+            a = ac.slot[cur];
+          } else {
+            f = bc_fast_quant(quant_scalars((double)__ldcg(arena + b.minmax_off), (double)__ldcg(arena + b.minmax_off + 1),
+                                            num_bits, b.signed_mode), num_bits);
+          }
           so = l.rows / (b.expect_len / l.cols);
           mode = (b.flags & 1) ? 2 : (f.ok ? 0 : 1);
           excached = l.cols <= kBcExCols;
@@ -719,6 +890,31 @@ k_bc_stream(float* arena, const DfqLayer* __restrict__ L, const DfqBcLayer* __re
         if (d.kind == TK_PLAIN) {       // a tile the TMA unit cannot move: the warp fetches it itself
           for (int i = lane; i < d.floats; i += 32) ring.stage(s)[i] = ldg_stream1(d.gptr + i);
           __syncwarp();
+        }
+        if constexpr (AC) {
+          float old_bias = 0.f, old_next = 0.f, csub = 0.f, dl = 0.f, wl = 0.f;
+          if (lane < d.nrows) bc_fetch_row_ac(arena, l, b, a, d.row0 + lane, old_bias, old_next, csub);
+          const StreamQE qe{f, mode};
+          for (int r = 0; r < d.nrows; ++r) {
+            const int o = d.row0 + r;
+            const int g = o / so;
+            const float* ex = arena + b.expect_off + (size_t)g * l.cols;
+            if (excached && g != cur_group) {
+              cur_group = g;
+              __syncwarp();
+              for (int j = lane; j < l.cols; j += 32) exs[j] = __ldcg(ex + j);
+              __syncwarp();
+            }
+            const float* cv = a.wc_c_off >= 0 ? arena + a.wc_c_off + (size_t)(o / a.wc_so) * l.cols : nullptr;
+            float* grow = d.gptr + (size_t)r * row_len;
+            double acc, wacc;
+            bc_row_ac<32>(d.kind == TK_DIRECT ? grow : ring.stage(s) + (size_t)r * row_len, grow, l.cols, l.kk,
+                          excached ? exs : ex, cv, mode == 2, ac, qe, lane, acc, wacc);
+            if (lane == r) { dl = (float)acc; wl = (float)wacc; }
+          }
+          if (lane < d.nrows) bc_retire_row_ac(arena, l, b, a, d.row0 + lane, dl, wl, old_bias, old_next, csub);
+          bc_give_back(ring, s, lane);
+          continue;
         }
         // lane r requests row r's read-modify-write operands before the tile and retires them after it
         float old_bias = 0.f, old_next = 0.f, dl = 0.f;
@@ -909,15 +1105,58 @@ extern "C" int dfq_quantize_tensors(float* arena, int64_t arena_floats, const Df
   return 0;
 }
 
-extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
-                                const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
-                                const int32_t* level_ptr, int32_t n_levels, int32_t num_bits, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  DFQ_REQUIRE(arena && layers && bc && terms && level_ptr, "null argument");
-  if (n_bc <= 0 || n_levels <= 0) return 0;
+// The correction's launch; `ac` (absorption and clipping, dfq_bias_correct_absorb_clip) selects the AC instantiations and
+// must then hold the per-entry slots, already in device memory.  `before` (optional) enqueues the work that must precede
+// the correction; it runs only once everything that can refuse the launch (grid size, table upload) has succeeded, so a
+// refused call leaves the arena untouched.
+static int bc_launch(float* arena, const DfqLayer* layers, int32_t n_layers, const DfqBcLayer* bc, int32_t n_bc,
+                     const DfqExpectTerm* terms, int32_t n_terms, const int32_t* level_ptr, int32_t n_levels, int32_t num_bits,
+                     const std::vector<long long>& row_ptr, const std::vector<long long>& mm_ptr, const AcArgs* ac,
+                     const std::function<int()>* before, cudaStream_t st) {
+  const int64_t max_tiles = std::max<int64_t>(1, row_ptr[n_bc]);
+  std::vector<int32_t> level_local(n_levels, 0);
+  for (int lv = 0; lv < n_levels; ++lv) {
+    bool ok = (level_ptr[lv + 1] - level_ptr[lv]) <= 4;
+    for (int i = level_ptr[lv]; ok && i < level_ptr[lv + 1]; ++i) ok = bc[i].expect_len <= kExpectCache;
+    level_local[lv] = ok ? 1 : 0;
+  }
+  int grid, rc;
+  // Large phases (bandwidth-bound: many tiles per CTA and level) take the streaming kernel, small models (latency-bound:
+  // a few tiles per level, level_local shortcuts) the per-CTA engine.  DFQ_BC_STREAM=0/1 forces one of them.
+  const int sms = std::max(1, sm_count());
+  bool stream_variant = row_ptr[n_bc] >= (long long)16 * sms * n_levels;
+  if (const char* e = getenv("DFQ_BC_STREAM")) stream_variant = atoi(e) != 0;
+  const void* kfn = stream_variant ? (ac ? (const void*)k_bc_stream<true> : (const void*)k_bc_stream<false>)
+                                   : (ac ? (const void*)k_bc_engine<true> : (const void*)k_bc_engine<false>);
+  TablePack tp;
+  const int iL = tp.add(layers, n_layers), iB = tp.add(bc, n_bc), iT = tp.add(terms, n_terms);
+  const int iLP = tp.add(level_ptr, n_levels + 1), iRP = tp.add(row_ptr.data(), n_bc + 1), iMP = tp.add(mm_ptr.data(), n_bc + 1);
+  const int iLL = stream_variant ? -1 : tp.add(level_local.data(), n_levels);
+  const size_t dyn = stream_variant ? BcRing::smem_bytes() : RowPipe::smem_bytes();
+  if (stream_variant) rc = coop_grid(kfn, "k_bc_stream", kBcThreads, dyn, max_tiles, &grid);
+  else                rc = coop_grid(kfn, "k_bc_engine", kThreads, dyn, max_tiles, &grid);
+  if (rc) return rc;
+  if ((rc = tp.upload(st))) return rc;
+  if (before && (rc = (*before)())) { tp.release(st); return rc; }
+  DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqBcLayer* dB = tp.ptr<DfqBcLayer>(iB); DfqExpectTerm* dT = tp.ptr<DfqExpectTerm>(iT);
+  int32_t* dLP = tp.ptr<int32_t>(iLP); long long* dRP = tp.ptr<long long>(iRP); long long* dMP = tp.ptr<long long>(iMP);
+  int32_t* dLL = stream_variant ? nullptr : tp.ptr<int32_t>(iLL);
+  AcArgs a = ac ? *ac : AcArgs{nullptr, 0.f, 0.f, 0};
+  void* stream_args[] = {&arena, &dL, &dB, (void*)&n_bc, &dT, &dLP, (void*)&n_levels, (void*)&num_bits, &dRP, &dMP, &a};
+  void* engine_args[] = {&arena, &dL, &dB, (void*)&n_bc, &dT, &dLP, (void*)&n_levels, (void*)&num_bits, &dRP, &dMP, &dLL, &a};
+  const cudaError_t e = stream_variant ? cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(kBcThreads), stream_args, dyn, st)
+                                       : cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(kThreads), engine_args, dyn, st);
+  tp.release(st);
+  DFQ_CUDA(e);
+  return 0;
+}
+
+// Checks of a correction table shared by both entries; fills the tile prefixes of its two weight phases.
+static int bc_check(int64_t arena_floats, const DfqLayer* layers, int32_t n_layers, const DfqBcLayer* bc, int32_t n_bc,
+                    const DfqExpectTerm* terms, int32_t n_terms, const int32_t* level_ptr, int32_t n_levels,
+                    std::vector<long long>& row_ptr, std::vector<long long>& mm_ptr) {
   DFQ_REQUIRE(level_ptr[0] == 0 && level_ptr[n_levels] == n_bc, "levels must partition the layer list");
-  int64_t max_tiles = 1;
-  std::vector<long long> row_ptr(n_bc + 1, 0), mm_ptr(n_bc + 1, 0);
+  row_ptr.assign(n_bc + 1, 0); mm_ptr.assign(n_bc + 1, 0);
   for (int i = 0; i < n_bc; ++i) {
     const DfqBcLayer& b = bc[i];
     DFQ_REQUIRE(b.layer >= 0 && b.layer < n_layers, "bc layer index");
@@ -934,7 +1173,18 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
                   "column-extrema hint outside arena");
     mm_ptr[i + 1] = mm_ptr[i] + (b.n_col > 0 ? 0 : pipe_tiles(l.rows, l.cols * l.kk));
   }
-  max_tiles = std::max<int64_t>(max_tiles, row_ptr[n_bc]);
+  return 0;
+}
+
+extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
+                                const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
+                                const int32_t* level_ptr, int32_t n_levels, int32_t num_bits, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  DFQ_REQUIRE(arena && layers && bc && terms && level_ptr, "null argument");
+  if (n_bc <= 0 || n_levels <= 0) return 0;
+  std::vector<long long> row_ptr, mm_ptr;
+  int rc;
+  if ((rc = bc_check(arena_floats, layers, n_layers, bc, n_bc, terms, n_terms, level_ptr, n_levels, row_ptr, mm_ptr))) return rc;
   std::vector<BcRetire> retire;
   int max_rows = 1;
   for (int i = 0; i < n_bc; ++i) {
@@ -949,7 +1199,6 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
     DFQ_REQUIRE((int)retire.size() == n_bc, "a table that mixes DFQ_BC_PREPARED and unprepared entries");
     TablePack tp;
     const int iE = tp.add(retire.data(), n_bc);
-    int rc;
     if ((rc = tp.upload(st))) return rc;
     const int threads = std::min(512, (max_rows + 31) / 32 * 32);
     k_bc_retire<<<std::min(n_bc, std::max(1, sm_count()) * 8), threads, 0, st>>>(arena, tp.ptr<BcRetire>(iE), n_bc);
@@ -957,36 +1206,89 @@ extern "C" int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLay
     tp.release(st);
     return 0;
   }
-  std::vector<int32_t> level_local(n_levels, 0);
-  for (int lv = 0; lv < n_levels; ++lv) {
-    bool ok = (level_ptr[lv + 1] - level_ptr[lv]) <= 4;
-    for (int i = level_ptr[lv]; ok && i < level_ptr[lv + 1]; ++i) ok = bc[i].expect_len <= kExpectCache;
-    level_local[lv] = ok ? 1 : 0;
+  return bc_launch(arena, layers, n_layers, bc, n_bc, terms, n_terms, level_ptr, n_levels, num_bits, row_ptr, mm_ptr, nullptr,
+                   nullptr, st);
+}
+
+extern "C" int dfq_bias_correct_absorb_clip(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
+                                            const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
+                                            const int32_t* level_ptr, int32_t n_levels, int32_t num_bits,
+                                            const DfqAbsorb* absorb, int32_t n_absorb, float absorb_n,
+                                            int32_t clip, float clip_lo, float clip_hi, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  DFQ_REQUIRE(arena && layers, "null argument");
+  DFQ_REQUIRE(n_bc <= 0 || (bc && terms && level_ptr && n_levels > 0), "null argument");
+  DFQ_REQUIRE(n_absorb <= 0 || absorb, "null argument");
+  if (n_bc < 0) n_bc = 0;
+  if (n_absorb < 0) n_absorb = 0;
+  if (n_absorb > 0) DFQ_REQUIRE(std::isfinite(absorb_n), "absorption N must be finite");
+  if (clip) DFQ_REQUIRE(std::isfinite(clip_lo) && std::isfinite(clip_hi) && clip_lo <= clip_hi, "clip range must be finite with lo <= hi");
+  std::vector<long long> row_ptr, mm_ptr;
+  int rc;
+  if (n_bc > 0 && (rc = bc_check(arena_floats, layers, n_layers, bc, n_bc, terms, n_terms, level_ptr, n_levels, row_ptr, mm_ptr)))
+    return rc;
+  std::vector<int> slot_of(n_layers, -1);
+  for (int i = 0; i < n_bc; ++i) {
+    DFQ_REQUIRE(!(bc[i].flags & DFQ_BC_PREPARED), "DFQ_BC_PREPARED entries are not absorbed or clipped");
+    DFQ_REQUIRE(slot_of[bc[i].layer] < 0, "a layer with two correction entries");
+    DFQ_REQUIRE(bc[i].delta_off >= 0 && bc[i].delta_off + layers[bc[i].layer].rows <= arena_floats, "delta scratch outside arena");
+    slot_of[bc[i].layer] = i;
   }
-  int grid, rc;
-  // Large phases (bandwidth-bound: many tiles per CTA and level) take the streaming kernel, small models (latency-bound:
-  // a few tiles per level, level_local shortcuts) the per-CTA engine.  DFQ_BC_STREAM=0/1 forces one of them.
-  const int sms = std::max(1, sm_count());
-  bool stream_variant = row_ptr[n_bc] >= (long long)16 * sms * n_levels;
-  if (const char* e = getenv("DFQ_BC_STREAM")) stream_variant = atoi(e) != 0;
+  std::vector<AcSlot> slots(std::max(1, (int)n_bc), AcSlot{-1, -1, 1, 0});
+  std::vector<int64_t> first_bias(std::max(1, (int)n_absorb), -1);
+  std::vector<char> is_first(n_layers, 0), is_second(n_layers, 0);
+  for (int i = 0; i < n_absorb; ++i) {
+    const DfqAbsorb& a = absorb[i];
+    DFQ_REQUIRE(a.first >= 0 && a.first < n_layers && a.second >= 0 && a.second < n_layers && a.first != a.second, "absorption layer index");
+    DFQ_REQUIRE(!is_first[a.first] && !is_second[a.second], "a layer is `first` of one absorbing relation and `second` of one only");
+    is_first[a.first] = is_second[a.second] = 1;
+    const DfqLayer& l1 = layers[a.first];
+    const DfqLayer& l2 = layers[a.second];
+    DFQ_REQUIRE(a.n == l1.rows && a.n > 0 && a.n % l2.cols == 0 && l2.rows % (a.n / l2.cols) == 0, "absorption relation shapes");
+    DFQ_REQUIRE(a.c_off >= 0 && a.c_off + a.n <= arena_floats && a.bn_w_off >= 0 && a.bn_w_off + a.n <= arena_floats &&
+                a.bn_b_off >= 0 && a.bn_b_off + a.n <= arena_floats, "absorption vectors outside arena");
+    const int s2 = slot_of[a.second];
+    DFQ_REQUIRE(s2 >= 0, "the `second` layer of an absorbing relation needs a correction entry");
+    if (!(bc[s2].flags & 1)) {              // a raw-sum entry is this absorption itself (its terms hold c)
+      slots[s2].wc_c_off = a.c_off;
+      slots[s2].wc_so = l2.rows / (a.n / l2.cols);
+    }
+    const int s1 = slot_of[a.first];
+    if (s1 >= 0) slots[s1].sub_c_off = a.c_off;
+    else first_bias[i] = l1.bias_off;
+  }
+  std::vector<ClipTask> clips;
+  if (clip)
+    for (int li = 0; li < n_layers; ++li) {
+      const DfqLayer& l = layers[li];
+      const int64_t n = (int64_t)l.rows * l.cols * l.kk;
+      DFQ_REQUIRE(l.w_off >= 0 && l.w_off + n <= arena_floats, "weight outside arena");
+      if (slot_of[li] < 0 && n > 0) clips.push_back(ClipTask{l.w_off, n});
+    }
   TablePack tp;
-  const int iL = tp.add(layers, n_layers), iB = tp.add(bc, n_bc), iT = tp.add(terms, n_terms);
-  const int iLP = tp.add(level_ptr, n_levels + 1), iRP = tp.add(row_ptr.data(), n_bc + 1), iMP = tp.add(mm_ptr.data(), n_bc + 1);
-  const int iLL = stream_variant ? -1 : tp.add(level_local.data(), n_levels);
-  const size_t dyn = stream_variant ? BcRing::smem_bytes() : RowPipe::smem_bytes();
-  if (stream_variant) rc = coop_grid((const void*)k_bc_stream, "k_bc_stream", kBcThreads, dyn, max_tiles, &grid);
-  else                rc = coop_grid((const void*)k_bc_engine, "k_bc_engine", kThreads, dyn, max_tiles, &grid);
-  if (rc) return rc;
+  const int iA = n_absorb ? tp.add(absorb, n_absorb) : -1, iF = n_absorb ? tp.add(first_bias.data(), n_absorb) : -1;
+  const int iC = clips.empty() ? -1 : tp.add(clips.data(), (int)clips.size());
+  const int iS = n_bc ? tp.add(slots.data(), n_bc) : -1;
   if ((rc = tp.upload(st))) return rc;
-  DfqLayer* dL = tp.ptr<DfqLayer>(iL); DfqBcLayer* dB = tp.ptr<DfqBcLayer>(iB); DfqExpectTerm* dT = tp.ptr<DfqExpectTerm>(iT);
-  int32_t* dLP = tp.ptr<int32_t>(iLP); long long* dRP = tp.ptr<long long>(iRP); long long* dMP = tp.ptr<long long>(iMP);
-  int32_t* dLL = stream_variant ? nullptr : tp.ptr<int32_t>(iLL);
-  // k_bc_engine's parameter list is k_bc_stream's plus level_local; a launch reads as many entries as its kernel has
-  void* args[] = {&arena, &dL, &dB, (void*)&n_bc, &dT, &dLP, (void*)&n_levels, (void*)&num_bits, &dRP, &dMP, &dLL};
-  if (stream_variant) DFQ_CUDA(cudaLaunchCooperativeKernel((void*)k_bc_stream, dim3(grid), dim3(kBcThreads), args, dyn, st));
-  else DFQ_CUDA(cudaLaunchCooperativeKernel((void*)k_bc_engine, dim3(grid), dim3(kThreads), args, dyn, st));
+  // the absorption vectors and the clip-only layers: enqueued only once the correction's launch cannot be refused any more
+  const std::function<int()> before = [&]() -> int {
+    if (n_absorb)
+      k_absorb_vectors<<<std::min(n_absorb, 1024), 256, 0, st>>>(arena, tp.ptr<DfqAbsorb>(iA), n_absorb, tp.ptr<int64_t>(iF),
+                                                                 absorb_n);
+    if (!clips.empty())
+      k_clip_tensors<<<std::max(1, sm_count()) * 4, kThreads, 0, st>>>(arena, tp.ptr<ClipTask>(iC), (int)clips.size(), clip_lo,
+                                                                       clip_hi);
+    DFQ_CUDA(cudaGetLastError());
+    return 0;
+  };
+  if (n_bc) {
+    const AcArgs ac{tp.ptr<AcSlot>(iS), clip_lo, clip_hi, clip ? 1 : 0};
+    rc = bc_launch(arena, layers, n_layers, bc, n_bc, terms, n_terms, level_ptr, n_levels, num_bits, row_ptr, mm_ptr, &ac, &before, st);
+  } else {
+    rc = before();
+  }
   tp.release(st);
-  return 0;
+  return rc;
 }
 
 extern "C" int dfq_selftest_bc_arithmetic(const float* w, float* eps_fast, float* eps_div, int64_t n, const float* minmax2,

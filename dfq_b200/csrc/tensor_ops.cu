@@ -495,6 +495,7 @@ extern "C" int dfq_struct_size(int which) {
     case 25: return (int)sizeof(DfqJpegDecode);
     case 26: return (int)sizeof(DfqJpegHuff);
     case 27: return (int)sizeof(DfqJpegTables);
+    case 28: return (int)sizeof(DfqAbsorb);
     default: return -1;
   }
 }

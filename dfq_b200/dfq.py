@@ -19,7 +19,7 @@ import torch.nn as nn
 
 from . import _lib
 from .engine import Session
-from .graphwalk import bias_correction_recipe
+from .graphwalk import bias_correction_recipe, relu_between
 from .utils import visualize_per_layer   # noqa: F401  (dfq.py:5 imports it; kept for API parity)
 from .utils import quantize as _Q
 from .utils.quantize import UniformQuantize, tensor_minmax, _ptr  # noqa: F401
@@ -173,21 +173,11 @@ def _equalize_any_order(sess, table, s_range, converge_thres, converge_count, si
 
 def bias_absorption(graph, relations, bottoms, N=3):
     print("Absorbing bias")
-
-    def relu_between(second, first):
-        key = second
-        while key != first:
-            assert len(bottoms[key]) == 1, 'graph in equalization relations should be 1-to-1 input-output'
-            if type(graph[bottoms[key][0]]) == torch.nn.ReLU:
-                return True
-            key = bottoms[key][0]
-        return False
-
     with torch.no_grad():
         todo = []
         for rr in relations:
             first, second, bn_idx = rr.get_idxs()
-            if not relu_between(second, first):
+            if not relu_between(graph, bottoms, second, first):
                 continue
             bn = graph[bn_idx]
             # c = clamp(beta - N*gamma, 0)   (dfq.py:143-144), a [C] vector

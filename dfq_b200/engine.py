@@ -651,19 +651,60 @@ class Session:
         if ready is not None and ready[0] is plan and ready[1] == int(num_bits) and col_hints is not None:
             bt = bt.copy()
             bt["flags"] |= _lib.BC_PREPARED
-        elif col_hints is not None and len(col_hints["layer"]):
-            bt = bt.copy()
-            lut = np.full(len(lt), -1, dtype=np.int64)
-            lut[col_hints["layer"]] = np.arange(len(col_hints["layer"]))
-            k = lut[bt["layer"]]
-            m = (k >= 0) & ((bt["flags"] & 1) == 0)          # bias absorption (raw sums) needs no range at all
-            for name in ("colmin_off", "colmax_off", "n_col"):
-                col = bt[name]
-                col[m] = col_hints[name][k[m]]
+        else:
+            bt = self._with_col_hints(lt, bt, col_hints)
         _lib.check(self.lib.dfq_bias_correct(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
                                              _lib.table_ptr(bt), len(bt), _lib.table_ptr(tt), plan["n_terms"],
                                              _lib.table_ptr(plan["level_ptr"]), plan["n_levels"], int(num_bits),
                                              _lib.stream_ptr()), "dfq_bias_correct")
+
+    @staticmethod
+    def _with_col_hints(lt: np.ndarray, bt: np.ndarray, col_hints: Optional[Dict[str, np.ndarray]]) -> np.ndarray:
+        if col_hints is None or not len(col_hints["layer"]):
+            return bt
+        bt = bt.copy()
+        lut = np.full(len(lt), -1, dtype=np.int64)
+        lut[col_hints["layer"]] = np.arange(len(col_hints["layer"]))
+        k = lut[bt["layer"]]
+        m = (k >= 0) & ((bt["flags"] & 1) == 0)          # bias absorption (raw sums) needs no range at all
+        for name in ("colmin_off", "colmax_off", "n_col"):
+            col = bt[name]
+            col[m] = col_hints[name][k[m]]
+        return bt
+
+    # ---- bias absorption and weight clipping inside the correction --------------------------------------------------
+    def plan_absorb(self, relations: Sequence[Tuple[int, int, int, int]]) -> np.ndarray:
+        """relations: (first_layer, second_layer, bn_w_off, bn_b_off) of every relation that absorbs (dfq.py:121-164), in
+        the order of the relation list.  Reserves each one's c vector; returns the DfqAbsorb table."""
+        at = np.zeros(len(relations), dtype=_lib.ABSORB_DT)
+        for i, (a, b, bnw, bnb) in enumerate(relations):
+            n = self._layers[a]["rows"]
+            at[i]["first"] = a; at[i]["second"] = b; at[i]["n"] = n
+            at[i]["bn_w_off"] = bnw; at[i]["bn_b_off"] = bnb; at[i]["c_off"] = self.alloc(n)
+        return at
+
+    def run_bias_correct_absorb_clip(self, plan: Optional[dict], num_bits: int = 8,
+                                     col_hints: Optional[Dict[str, np.ndarray]] = None, absorb: Optional[np.ndarray] = None,
+                                     absorb_n: float = 3, clip: Optional[Tuple[float, float]] = None):
+        """dfq_bias_correct_absorb_clip: bias absorption (absorb: plan_absorb's table, factor absorb_n) and weight clipping
+        (clip: (lo, hi), every layer of the session) inside the correction `plan` (plan_bias_correct; None: no correction -
+        the clip alone, or a plan of raw-sum entries that is the absorption itself).  The weights of `plan` are read once."""
+        self._ensure_room()
+        self.finish_fold()
+        lt = plan["lt"] if plan is not None else self._layer_table()
+        at = absorb if absorb is not None and len(absorb) else np.zeros(1, dtype=_lib.ABSORB_DT)
+        n_abs = len(absorb) if absorb is not None else 0
+        if plan is not None:
+            bt, tt, n_terms, lp, n_levels = self._with_col_hints(lt, plan["bt"], col_hints), plan["tt"], plan["n_terms"], \
+                plan["level_ptr"], plan["n_levels"]
+        else:
+            bt, tt, n_terms = np.zeros(1, dtype=_lib.BC_LAYER_DT), np.zeros(1, dtype=_lib.TERM_DT), 0
+            lp, n_levels = np.zeros(1, dtype=np.int32), 0
+        lo, hi = (float(clip[0]), float(clip[1])) if clip is not None else (0.0, 0.0)
+        _lib.check(self.lib.dfq_bias_correct_absorb_clip(
+            self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt), _lib.table_ptr(bt), len(plan["bt"]) if plan else 0,
+            _lib.table_ptr(tt), n_terms, _lib.table_ptr(lp), n_levels, int(num_bits), _lib.table_ptr(at), n_abs,
+            float(absorb_n), 1 if clip is not None else 0, lo, hi, _lib.stream_ptr()), "dfq_bias_correct_absorb_clip")
 
     def run_bias_correct(self, items: Sequence[dict], num_bits: int = 8):
         """plan + run; returns the list of delta offsets ([rows] each), in the order of `items`."""

@@ -61,6 +61,18 @@ def find_prev_bn(bn_module, relu_attached, graph, bottoms, bot):
     return bn_list, relu_attach_list, connect_type_list, targ_without_bn
 
 
+def relu_between(graph, bottoms, second, first) -> bool:
+    """dfq.py:123-130: whether the walk from `second` back to `first` meets a torch.nn.ReLU (ReLU6 does not count); the
+    path must be 1-to-1."""
+    key = second
+    while key != first:
+        assert len(bottoms[key]) == 1, 'graph in equalization relations should be 1-to-1 input-output'
+        if type(graph[bottoms[key][0]]) == torch.nn.ReLU:
+            return True
+        key = bottoms[key][0]
+    return False
+
+
 def merge_order(entries):
     """The order in which dfq.py:228-275 (and layer_transform.py:490-567) folds the BNs of one branch:
     deepest path first, then ties of equal depth, cutting the depth when none is left at the current one.

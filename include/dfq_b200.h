@@ -46,7 +46,7 @@ const char* dfq_last_error(void);
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
  * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax, 21 DfqPreImage, 22 DfqPreResample,
- * 23 DfqJpegImage, 24 DfqJpegSegment, 25 DfqJpegDecode, 26 DfqJpegHuff, 27 DfqJpegTables; 20 is
+ * 23 DfqJpegImage, 24 DfqJpegSegment, 25 DfqJpegDecode, 26 DfqJpegHuff, 27 DfqJpegTables, 28 DfqAbsorb; 20 is
  * unassigned and returns -1, as ABI 11 released it): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
@@ -290,6 +290,33 @@ typedef struct DfqBcLayer {
 int dfq_bias_correct(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
                      const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
                      const int32_t* level_ptr, int32_t n_levels, int32_t num_bits, void* stream);
+
+/* Bias absorption and weight clipping inside the bias correction: what the separate calls
+ *   bias_absorption(graph, relations, bottoms, N)   dfq.py:121-164
+ *   clip_weight(graph, [lo, hi], targ)              dfq.py:167-170
+ *   bias_correction(graph, bottoms, targ)           dfq.py:173-293
+ * compute one after the other, with each corrected weight row read once.  One DfqAbsorb per absorbing relation (the
+ * caller decides which relations absorb: a torch.nn.ReLU between the layers, dfq.py:123-130): */
+typedef struct DfqAbsorb {
+  int32_t first, second;     /* layer indices of the relation */
+  int32_t n;                 /* channels = first.rows = groups * second.cols */
+  int32_t _pad;
+  int64_t bn_w_off, bn_b_off;  /* the relation's BN fake_weight / fake_bias (after equalization) */
+  int64_t c_off;             /* scratch/out [n]: c = clamp(fake_bias - N * fake_weight, 0) (dfq.py:143-144) */
+} DfqAbsorb;
+/* Before the correction: c of every relation, fake_bias -= c, and first.bias -= c when `first` has no correction entry.
+ * The `second` layer of every relation needs an entry: a raw-sum entry (flags bit 0, its terms holding c) is the
+ * absorption alone; any other entry adds (sum_k W) . c of the UNCLIPPED row to the bias, per group as dfq.py:150-153.
+ * clip != 0: every weight of `layers` is clamped to [clip_lo, clip_hi] in the arena - those of the entries while their rows
+ * are read (the correction's quantization error and per-tensor range are those of the clamped weights), the others in one
+ * more launch.  Biases are never clipped.  The bias of an entry rounds as the separate calls do:
+ * fl(fl(fl(b + wc) - c) - delta).  n_bc = 0: the clip alone.
+ * Refused: a non-finite absorb_n, a clip range that is not finite with lo <= hi, DFQ_BC_PREPARED entries. */
+int dfq_bias_correct_absorb_clip(float* arena, int64_t arena_floats, const DfqLayer* layers, int32_t n_layers,
+                                 const DfqBcLayer* bc, int32_t n_bc, const DfqExpectTerm* terms, int32_t n_terms,
+                                 const int32_t* level_ptr, int32_t n_levels, int32_t num_bits,
+                                 const DfqAbsorb* absorb, int32_t n_absorb, float absorb_n,
+                                 int32_t clip, float clip_lo, float clip_hi, void* stream);
 
 /* Per-tensor min/max + in-place fake quantization of arena tensors, batched
  * (utils/layer_transform.py:279-296 quantize_targ_layer; CPU semantics: true division). */

@@ -22,9 +22,14 @@ build container.  Committed next to its outputs so every fixture can be regenera
   ref_ssd_postprocess.npz the reference's Predictor.predict post-processing on seeded SSD-Lite-shaped outputs
   ref_seg_eval.npz        the reference's forward_all predictions and Evaluator matrices and metrics on seeded batches
   ref_ssd_map.npz         main_ssd.py's per-class VOC average precision on a seeded set of detections and annotations
+  ref_absorb_clip.npz     the reference's merge_batchnorm -> cross_layer_equalization -> bias_absorption -> clip_weight ->
+                          bias_correction (main_cls.py:149-181 with --relu --equalize --absorption --clip_weight
+                          --correction) on the seeded models of tests/absorb_clip_case.py: every weight, bias,
+                          fake_bias after equalization, after absorption, after the clip and at the end (weights: after
+                          equalization and after the clip)
 
 usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
-       [ssd_post] [seg_eval] [ssd_map]
+       [ssd_post] [seg_eval] [ssd_map] [absorb_clip]
 """
 import hashlib
 import json
@@ -694,3 +699,46 @@ def preprocess():
 
 if __name__ == "__main__" and "preprocess" in sys.argv[1:]:
     preprocess()
+
+
+# ---------------------------------------------------------------------------------------------------------
+def absorb_clip_fixture():
+    """dfq.py:121-170 between the equalization and the correction, in the mains' order, on tests/absorb_clip_case.py."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import absorb_clip_case as case
+    targ = [nn.Conv2d, nn.Linear]
+    out = {}
+    for name, seed, n, clip in case.FIXTURE_CASES:
+        graph, bottoms, _ = workload.build_graph(case.topology(name), seed=seed)
+        keys = list(graph.keys())
+        pos = {k: i for i, k in enumerate(keys)}
+
+        def stage(tag):
+            for k in keys:
+                m = graph[k]
+                if type(m) in targ:
+                    if tag in ("cle", "clip"):      # absorption and correction leave the weights alone
+                        out["%s_%s_w_%d" % (name, tag, pos[k])] = m.weight.detach().numpy().copy()
+                    if m.bias is not None:
+                        out["%s_%s_b_%d" % (name, tag, pos[k])] = m.bias.detach().numpy().copy()
+                elif hasattr(m, "fake_bias") and not isinstance(m, str):
+                    out["%s_%s_fw_%d" % (name, tag, pos[k])] = m.fake_weight.numpy().copy()
+                    out["%s_%s_fb_%d" % (name, tag, pos[k])] = m.fake_bias.numpy().copy()
+        ref.layer_transform.merge_batchnorm(None, graph, bottoms, targ)
+        rels = ref.relation.create_relation(graph, bottoms, targ)
+        out[name + "_relations"] = np.array([[pos[a], pos[b], pos[c]] for a, b, c in (r.get_idxs() for r in rels)], np.int64)
+        ref.dfq.cross_layer_equalization(graph, rels, targ)
+        stage("cle")
+        ref.dfq.bias_absorption(graph, rels, bottoms, n)
+        stage("absorb")
+        ref.dfq.clip_weight(graph, list(clip), targ)
+        stage("clip")
+        ref.dfq.bias_correction(graph, bottoms, targ)
+        stage("bc")
+        out[name + "_meta"] = np.array(json.dumps(dict(seed=seed, N=n, clip=list(clip), torch=torch.__version__)))
+    np.savez_compressed(os.path.join(GOLD, "ref_absorb_clip.npz"), **out)
+    print("absorb_clip", len(out), "arrays")
+
+
+if __name__ == "__main__" and "absorb_clip" in sys.argv[1:]:
+    absorb_clip_fixture()
