@@ -181,9 +181,9 @@ class GraphCalibration:
         absorb = self._absorb if absorption and len(self._absorb) else None
         clip = tuple(clip_weight) if clip_weight is not None else None
         if correction and self._bc_plan is not None:
-            if signed:
+            if any(it["signed"] != bool(signed) for it in self._bc_items):    # every run sets the mode: replan on a change
                 for it in self._bc_items:
-                    it["signed"] = True
+                    it["signed"] = bool(signed)
                 self._bc_plan = sess.plan_bias_correct(self._bc_items)
             if absorb is not None or clip is not None:
                 sess.run_bias_correct_absorb_clip(self._bc_plan, 8, col_hints=hints, absorb=absorb, absorb_n=absorption_n,

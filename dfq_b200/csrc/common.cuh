@@ -297,6 +297,10 @@ __device__ __forceinline__ float clamp_nan(float t, float lo, float hi) {
   asm("min.NaN.f32 %0, %0, %1;" : "+f"(r) : "f"(hi));
   return r;
 }
+// torch.clamp_(w, lo, hi) of one weight (clip_weight, dfq.py:167-170): only a value below lo or above hi changes.  One inside
+// the range keeps its bits - a NaN its payload, a zero its sign at a zero bound - where max.NaN / min.NaN (clamp_nan) give
+// the canonical NaN and turn -0.0 into +0.0 at lo = 0.
+__device__ __forceinline__ float clamp_keep(float w, float lo, float hi) { return w < lo ? lo : (w > hi ? hi : w); }
 
 // quantize.py:70-74, one element.  Every op is individually rounded (no FMA contraction).
 template <bool RECIP>

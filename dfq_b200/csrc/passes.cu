@@ -517,7 +517,7 @@ __device__ __forceinline__ void bc_row_ac(const float* row, float* grow, int col
       R = __fadd_rn(R, w0);
       float w = w0;
       if (ac.clip) {
-        w = clamp_nan(w0, ac.lo, ac.hi);
+        w = clamp_keep(w0, ac.lo, ac.hi);
         if (__float_as_uint(w) != __float_as_uint(w0)) gp[k] = w;
       }
       if (!raw) E = __fadd_rn(E, qe(w));
@@ -575,7 +575,7 @@ __global__ void __launch_bounds__(kThreads) k_clip_tensors(float* arena, const C
     float* x = arena + T[t].off;
     const int64_t n = T[t].n;
     for (int64_t i = blockIdx.x * (int64_t)kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
-      const float w0 = ldg_stream1(x + i), w = clamp_nan(w0, lo, hi);
+      const float w0 = ldg_stream1(x + i), w = clamp_keep(w0, lo, hi);
       if (__float_as_uint(w) != __float_as_uint(w0)) x[i] = w;
     }
   }

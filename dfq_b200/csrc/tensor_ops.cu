@@ -441,7 +441,7 @@ __global__ void k_fill(float* p, int64_t n, float v) {
 
 __global__ void __launch_bounds__(kThreads) k_clamp(float* x, int64_t n, float lo, float hi) {
   const int64_t start = blockIdx.x * (int64_t)kThreads + threadIdx.x, stride = (int64_t)gridDim.x * kThreads;
-  for (int64_t i = start; i < n; i += stride) x[i] = clamp_nan(x[i], lo, hi);
+  for (int64_t i = start; i < n; i += stride) x[i] = clamp_keep(x[i], lo, hi);
 }
 
 static int flat_grid(int64_t n, int per_thread) {

@@ -123,10 +123,13 @@ def quantize_tensor_range(x: np.ndarray, num_bits: int, min_value, max_value, sy
         return (np.rint(np.minimum(np.maximum(t, qmin), qmax)) * scale + mn).astype(f32)
 
 
-def quantize_error(w: np.ndarray, num_bits: int = 8, signed: bool = False) -> np.ndarray:
-    """dfq.py:8-25 with ``reduction=None``: Q(W) - W using the tensor's own min/max."""
+def quantize_error(w: np.ndarray, num_bits: int = 8, signed: bool = False, value_range=None) -> np.ndarray:
+    """dfq.py:8-25 with ``reduction=None``: Q(W) - W using the tensor's own min/max (``value_range``: that (min, max) given,
+    e.g. ``flat_minmax``'s, which skips NaN as the library's reductions do)."""
     w = np.ascontiguousarray(w, dtype=f32)
-    q = quantize(w, num_bits, float(w.min()), float(w.max()), symmetric=signed)
+    mn, mx = value_range if value_range is not None else (w.min(), w.max())
+    with np.errstate(invalid="ignore", over="ignore"):
+        q = quantize(w, num_bits, float(mn), float(mx), symmetric=signed)
     return (q - w).astype(f32)
 
 
@@ -362,7 +365,8 @@ def bias_delta(w: np.ndarray, expect: np.ndarray, signed: bool = False, num_bits
     return out
 
 
-def bias_delta_bound(w: np.ndarray, expect: np.ndarray, signed: bool = False, num_bits: int = 8, raw: bool = False):
+def bias_delta_bound(w: np.ndarray, expect: np.ndarray, signed: bool = False, num_bits: int = 8, raw: bool = False,
+                     value_range=None):
     """Per-row acceptance bound for a bias-correction kernel: returns (exact, bound), both float64 [O].
 
     ``exact[o]`` = sum over (c, t) of eps[o, c, t] * E[c] in float64 from the bit-exact per-element errors
@@ -371,12 +375,14 @@ def bias_delta_bound(w: np.ndarray, expect: np.ndarray, signed: bool = False, nu
 
         (kk - 1) * 2^-24 * sum_c |E_c| * sum_t |eps_oct|      fp32 sum of the taps, any order
       + n * 2^-53 * sum_c |E_c * sum_t eps_oct|               float64 dot over the n = cols columns
-      + 2^-24 * |exact[o]|                                     final rounding to fp32
+      + 2^-24 * |exact[o]| + 2^-150                            final rounding to fp32 (2^-150: half the spacing of the
+                                                               subnormals, where a relative bound does not hold)
 
-    of ``exact[o]``.  Unlike a normwise gate over the whole layer this sees an error confined to one row, column or tap.
+    of ``exact[o]``.  (The fp32 sums need no such term: a sum that lands among the subnormals is exact.)  Unlike a normwise gate over the whole layer this sees an error confined to one row, column or tap.
+    ``value_range``: the per-tensor (min, max) of the quantization, as in ``quantize_error``.
     """
     w = np.ascontiguousarray(w, f32)
-    eps = w if raw else quantize_error(w, num_bits, signed)
+    eps = w if raw else quantize_error(w, num_bits, signed, value_range)
     O, J = w.shape[0], w.shape[1]
     e3 = eps.reshape(O, J, -1).astype(np.float64)
     kk = e3.shape[2]
@@ -388,7 +394,7 @@ def bias_delta_bound(w: np.ndarray, expect: np.ndarray, signed: bool = False, nu
     exact = (colsum * ex).sum(axis=1)
     bound = ((kk - 1) * 2.0 ** -24 * (np.abs(ex) * np.abs(e3).sum(axis=2)).sum(axis=1)
              + J * 2.0 ** -53 * np.abs(colsum * ex).sum(axis=1)
-             + 2.0 ** -24 * np.abs(exact))
+             + 2.0 ** -24 * np.abs(exact) + 2.0 ** -150)
     return exact, bound
 
 
