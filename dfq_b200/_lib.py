@@ -245,6 +245,8 @@ SIGNATURES = {
     "dfq_ssd_decode": [_PF, _PF, _PF, C.c_void_p, _ST],
     "dfq_ssd_nms": [_PF, _PF, _PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_ssd_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, _ST],
+    "dfq_ssd_soft_nms": [_PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, _ST],
+    "dfq_ssd_soft_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, C.c_float, _ST],
     "dfq_seg_argmax": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_cls_count": [_PF, C.c_void_p, C.c_void_p, C.c_void_p, _I64, _I32, _ST],
     "dfq_map_match": [_PF, C.c_void_p, _PF, C.c_void_p, _I64, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _I64, _I32, _I32,

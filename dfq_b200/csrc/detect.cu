@@ -8,6 +8,8 @@
 //                   sort, the suppression bitmask from the decoded boxes, then the greedy scan in one warp.
 //   k_ssd_scan      one CTA: exclusive scan of the per-(image, class) pick counts.
 //   k_ssd_compact   one CTA per (image, class): the picks into the flat outputs, scaled by the image sizes, with labels.
+//   k_ssd_soft      box_utils.soft_nms per (image, class), in three launches by candidate count; run once for the pick
+//                   counts and once more to write the picks to the flat outputs.
 #include <algorithm>
 
 #include <cub/block/block_scan.cuh>
@@ -222,6 +224,180 @@ __global__ void __launch_bounds__(128) k_ssd_compact(const float4* __restrict__ 
   }
 }
 
+// ---- soft NMS ----------------------------------------------------------------------------------------------------------
+// box_utils.soft_nms per (image, foreground class) segment on rows (box, score) that live either in shared memory or in a
+// global slab of the CTA.  Every step keeps the reference's row order: the candidates are gathered in prior order, the
+// picked row is overwritten by the last one, and the rows that survive the rescoring are compacted stably.  Each step is
+// one pass over the rows that rescores, compacts and finds the next argmax together.
+//
+// Work per segment grows with the square of its candidate count, which differs a lot between classes, so three launches
+// share the segments by count m: kSoftSmallRows or fewer on a small CTA (many per SM), up to kSoftLargeRows on a CTA that
+// holds them all in shared memory, and beyond that on a CTA of a grid-wide persistent launch with a slab of P rows each.
+constexpr int kSoftSmallThreads = 128;
+constexpr int kSoftSmallRows = 1024;
+constexpr int kSoftLargeThreads = 512;
+constexpr int kSoftLargeRows = 11264;     // 20 bytes a row: 225,280 bytes of the 227 KB an sm_90 CTA may hold
+constexpr int kSoftMaxWarps = kSoftLargeThreads / 32;
+
+inline size_t soft_smem(int rows) { return (sizeof(float4) + sizeof(float)) * (size_t)rows; }
+
+// torch.argmax's order: a beats b when a is NaN and b is not, or a > b, or they tie and a comes first
+__device__ __forceinline__ bool soft_better(float a, int ai, float b, int bi) {
+  if (a != a) return b == b || ai < bi;
+  if (b != b) return false;
+  return a > b || (a == b && ai < bi);
+}
+
+// Exclusive prefix of `flag` over the CTA (thread order) and the total.  The first barrier separates every thread's reads
+// before the call from every write after it; the second keeps `warp_tot` until all threads have read it.
+template <int kThreads>
+__device__ __forceinline__ int soft_scan(bool flag, int* warp_tot, int* total) {
+  constexpr int kWarps = kThreads / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t ballot = __ballot_sync(0xffffffffu, flag);
+  if (lane == 0) warp_tot[warp] = __popc(ballot);
+  __syncthreads();
+  int before = __popc(ballot & ((1u << lane) - 1u)), all = 0;
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) {
+    const int t = warp_tot[w];
+    before += w < warp ? t : 0;
+    all += t;
+  }
+  __syncthreads();
+  *total = all;
+  return before;
+}
+
+// The CTA's best (value, index) under soft_better.  Ends with a barrier, so the slots can be reused at once.
+template <int kThreads>
+__device__ __forceinline__ int soft_argmax(float v, int i, float* best_v, int* best_i) {
+  constexpr int kWarps = kThreads / 32;
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_down_sync(0xffffffffu, v, o);
+    const int oi = __shfl_down_sync(0xffffffffu, i, o);
+    if (soft_better(ov, oi, v, i)) { v = ov; i = oi; }
+  }
+  if ((threadIdx.x & 31) == 0) { best_v[threadIdx.x >> 5] = v; best_i[threadIdx.x >> 5] = i; }
+  __syncthreads();
+  v = best_v[0];
+  i = best_i[0];
+#pragma unroll
+  for (int w = 1; w < kWarps; ++w)
+    if (soft_better(best_v[w], best_i[w], v, i)) { v = best_v[w]; i = best_i[w]; }
+  __syncthreads();
+  return i;
+}
+
+// One launch of the soft NMS over the segments whose candidate count m lies in (lo, hi].  kCount: this launch counts the
+// candidates of every segment (writing cand[s]) and gathers on the fly while they fit; the others read cand.  Without
+// `out_boxes` the launch writes each segment's pick count to counts[s]; with it, the picks themselves to the flat output
+// at offs[s], scaled by `sizes` and labelled.  kGlobal: the rows live in slab blockIdx.x of g_box / g_sc (P rows each).
+template <int kThreads, bool kCount, bool kGlobal>
+__global__ void __launch_bounds__(kThreads) k_ssd_soft(const float* __restrict__ scores, const float4* __restrict__ boxes,
+                                                      int32_t* __restrict__ cand, int32_t* __restrict__ counts,
+                                                      const int64_t* __restrict__ offs, const float* __restrict__ sizes,
+                                                      float4* __restrict__ out_boxes, int64_t* __restrict__ out_labels,
+                                                      float* __restrict__ out_probs, float4* __restrict__ g_box,
+                                                      float* __restrict__ g_sc, int64_t P, int C, float thr, float sigma,
+                                                      int top_k, int lo, int hi, int S) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  __shared__ int warp_tot[kSoftMaxWarps];
+  __shared__ float best_v[kSoftMaxWarps];
+  __shared__ int best_i[kSoftMaxWarps];
+  float4* bx = kGlobal ? g_box + (int64_t)blockIdx.x * P : (float4*)smem;
+  float* sc = kGlobal ? g_sc + (int64_t)blockIdx.x * P : (float*)(bx + hi);
+  const int tid = threadIdx.x;
+
+  for (int seg = blockIdx.x; seg < S; seg += gridDim.x) {
+    const int64_t n = seg / (C - 1);
+    const int c = seg % (C - 1) + 1;
+    const float* s = scores + n * P * C + c;
+    const float4* b = boxes + n * P;
+
+    // the candidates, score > thr, in prior order
+    if (!kCount && (cand[seg] <= lo || cand[seg] > hi)) continue;
+    int m = 0;
+    for (int64_t i0 = 0; i0 < P; i0 += kThreads) {
+      const int64_t i = i0 + tid;
+      const float v = i < P ? s[i * C] : 0.f;
+      const bool f = i < P && v > thr;
+      int tot;
+      const int at = m + soft_scan<kThreads>(f, warp_tot, &tot);
+      if (f && at < hi) { bx[at] = b[i]; sc[at] = v; }
+      m += tot;
+    }
+    __syncthreads();
+    if (kCount) {
+      if (tid == 0) cand[seg] = m;
+      if (m <= lo || m > hi) continue;
+    }
+    if (m == 0) {
+      if (!out_boxes && tid == 0) counts[seg] = 0;
+      continue;
+    }
+
+    int j;
+    {
+      float v = -INFINITY;
+      int vi = INT_MAX;
+      for (int i = tid; i < m; i += kThreads)
+        if (soft_better(sc[i], i, v, vi)) { v = sc[i]; vi = i; }
+      j = soft_argmax<kThreads>(v, vi, best_v, best_i);
+    }
+    const int64_t dst = out_boxes ? offs[seg] : 0;
+    int picks = 0;
+    while (true) {
+      const float4 cur = bx[j];
+      if (out_boxes && tid == 0) {
+        float4 o = cur;
+        if (sizes) {
+          const float w = sizes[2 * n], h = sizes[2 * n + 1];
+          o = make_float4(o.x * w, o.y * h, o.z * w, o.w * h);
+        }
+        out_boxes[dst + picks] = o;
+        out_labels[dst + picks] = c;
+        out_probs[dst + picks] = sc[j];
+      }
+      ++picks;
+      if ((top_k > 0 && picks == top_k) || m == 1) break;
+      // row j takes the last row's place and the last row goes; then s = s * exp(-(iou * iou) / sigma) and the rows with
+      // s > thr are kept in order.  Writes go to positions at or below the rows read in the same chunk, and the scan's
+      // first barrier orders them after those reads (cur and the last row among them).
+      const float4 last_b = bx[m - 1];
+      const float last_s = sc[m - 1];
+      float v = -INFINITY;
+      int vi = INT_MAX, kept = 0;
+      for (int i0 = 0; i0 < m - 1; i0 += kThreads) {
+        const int i = i0 + tid;
+        float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
+        float rs = 0.f;
+        bool keep = false;
+        if (i < m - 1) {
+          r = i == j ? last_b : bx[i];
+          rs = i == j ? last_s : sc[i];
+          const float iou = iou_of(cur, r);
+          rs = rs * expf(-(iou * iou) / sigma);
+          keep = rs > thr;
+        }
+        int tot;
+        const int at = kept + soft_scan<kThreads>(keep, warp_tot, &tot);
+        if (keep) {
+          bx[at] = r;
+          sc[at] = rs;
+          if (soft_better(rs, at, v, vi)) { v = rs; vi = at; }
+        }
+        kept += tot;
+      }
+      m = kept;
+      if (m == 0) break;
+      j = soft_argmax<kThreads>(v, vi, best_v, best_i);
+    }
+    if (!out_boxes && tid == 0) counts[seg] = picks;
+    __syncthreads();   // the rows are rewritten by the next segment's gather
+  }
+}
+
 int check_desc(const DfqSsdNms* d, const char* who) {
   if (!d) { set_error("%s: descriptor is NULL", who); return DFQ_E_ARG; }
   if (d->N < 1 || d->P < 1) { set_error("%s: N and P must be positive, got %d and %d", who, d->N, d->P); return DFQ_E_ARG; }
@@ -241,6 +417,57 @@ int check_nms(const DfqSsdNms* d, const char* who) {
     return DFQ_E_UNSUPPORTED;
   }
   if ((int64_t)d->N * (d->C - 1) > INT32_MAX) { set_error("%s: N * (C - 1) does not fit in int32", who); return DFQ_E_UNSUPPORTED; }
+  return 0;
+}
+
+int check_soft(const DfqSsdNms* d, float sigma, const char* who) {
+  if (int rc = check_desc(d, who)) return rc;
+  if (d->C < 2) { set_error("%s: C must be at least 2 (background and one class), got %d", who, d->C); return DFQ_E_ARG; }
+  if (!(sigma > 0.f) || sigma == INFINITY) {
+    set_error("%s: sigma must be a finite positive number, got %g", who, (double)sigma);
+    return DFQ_E_ARG;
+  }
+  if ((int64_t)d->N * (d->C - 1) > INT32_MAX) { set_error("%s: N * (C - 1) does not fit in int32", who); return DFQ_E_UNSUPPORTED; }
+  return 0;
+}
+
+// The soft NMS over every segment, in up to three launches by candidate count (k_ssd_soft).  Without out_boxes it writes
+// the pick counts; with them, the picks.  Both runs take the same steps, so they agree on every count.
+int soft_run(const float* scores, const float* boxes, int32_t* cand, int32_t* counts, const int64_t* offs,
+             const float* sizes, float* out_boxes, int64_t* out_labels, float* out_probs, const DfqSsdNms* d, float sigma,
+             cudaStream_t st) {
+  const int S = d->N * (d->C - 1);
+  const float4* bx = (const float4*)boxes;
+  float4* ob = (float4*)out_boxes;
+  k_ssd_soft<kSoftSmallThreads, true, false><<<S, kSoftSmallThreads, soft_smem(kSoftSmallRows), st>>>(
+      scores, bx, cand, counts, offs, sizes, ob, out_labels, out_probs, nullptr, nullptr, d->P, d->C, d->prob_threshold,
+      sigma, d->top_k, -1, kSoftSmallRows, S);
+  DFQ_CUDA(cudaGetLastError());
+  if (d->P > kSoftSmallRows) {
+    const int rows = std::min(d->P, kSoftLargeRows);
+    auto k = k_ssd_soft<kSoftLargeThreads, false, false>;
+    DFQ_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)soft_smem(rows)));
+    k<<<std::min(S, sm_count()), kSoftLargeThreads, soft_smem(rows), st>>>(
+        scores, bx, cand, counts, offs, sizes, ob, out_labels, out_probs, nullptr, nullptr, d->P, d->C, d->prob_threshold,
+        sigma, d->top_k, kSoftSmallRows, rows, S);
+    DFQ_CUDA(cudaGetLastError());
+  }
+  if (d->P > kSoftLargeRows) {
+    const int grid = std::min(S, sm_count());
+    float4* g_box = nullptr;
+    float* g_sc = nullptr;
+    DFQ_CUDA(cudaMallocAsync((void**)&g_box, sizeof(float4) * grid * (size_t)d->P, st));
+    cudaError_t e = cudaMallocAsync((void**)&g_sc, sizeof(float) * grid * (size_t)d->P, st);
+    if (e == cudaSuccess) {
+      k_ssd_soft<kSoftLargeThreads, false, true><<<grid, kSoftLargeThreads, 0, st>>>(
+          scores, bx, cand, counts, offs, sizes, ob, out_labels, out_probs, g_box, g_sc, d->P, d->C, d->prob_threshold,
+          sigma, d->top_k, kSoftLargeRows, INT_MAX, S);
+      e = cudaGetLastError();
+    }
+    free_async(g_sc, st);
+    free_async(g_box, st);
+    DFQ_CUDA(e);
+  }
   return 0;
 }
 
@@ -299,4 +526,34 @@ extern "C" int dfq_ssd_compact(const float* slot_boxes, const float* slot_probs,
       d->candidate_size);
   DFQ_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int dfq_ssd_soft_nms(const float* scores, const float* boxes, int32_t* candidates, int32_t* counts,
+                                int64_t* offsets, const DfqSsdNms* d, float sigma, void* stream) {
+  const char* who = "dfq_ssd_soft_nms";
+  if (int rc = check_soft(d, sigma, who)) return rc;
+  if (!scores || !boxes || !candidates || !counts || !offsets || !aligned16(boxes)) {
+    set_error("%s: every pointer must be non-NULL, boxes 16-byte aligned", who);
+    return DFQ_E_ARG;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = soft_run(scores, boxes, candidates, counts, nullptr, nullptr, nullptr, nullptr, nullptr, d, sigma, st))
+    return rc;
+  k_ssd_scan<<<1, kScanThreads, 0, st>>>(counts, offsets, d->N * (d->C - 1));
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_ssd_soft_compact(const float* scores, const float* boxes, int32_t* candidates, const int64_t* offsets,
+                                    const float* image_sizes, float* out_boxes, int64_t* out_labels, float* out_probs,
+                                    const DfqSsdNms* d, float sigma, void* stream) {
+  const char* who = "dfq_ssd_soft_compact";
+  if (int rc = check_soft(d, sigma, who)) return rc;
+  if (!scores || !boxes || !candidates || !offsets || !out_boxes || !out_labels || !out_probs || !aligned16(boxes) ||
+      !aligned16(out_boxes)) {
+    set_error("%s: every pointer but image_sizes must be non-NULL, boxes and out_boxes 16-byte aligned", who);
+    return DFQ_E_ARG;
+  }
+  return soft_run(scores, boxes, candidates, nullptr, offsets, image_sizes, out_boxes, out_labels, out_probs, d, sigma,
+                  (cudaStream_t)stream);
 }

@@ -1,11 +1,15 @@
-"""SSD post-processing and evaluation for whole batches on the GPU: box decoding, the reference's per-class hard NMS and
-its VOC average precision.
+"""SSD post-processing and evaluation for whole batches on the GPU: box decoding, the reference's per-class hard or soft
+NMS and its VOC average precision.
 
 `postprocess` returns, for every image of a batch, what the reference's `Predictor.predict`
 (modeling/detection/predictor.py) returns for that image alone - the decode of utils/detection/box_utils.py bit for bit
 with torch's CUDA ops, then per foreground class the threshold, the sort, the `candidate_size` cut and `hard_nms` - with
 one difference: candidates of equal score are ordered by prior index (the reference's CPU sort is not stable, so its
-order among equal scores is arbitrary).  Soft NMS is not offered (DESIGN.md section 8).
+order among equal scores is arbitrary).  With nms_method="soft" it runs `soft_nms` instead, every op the reference's
+bit for bit except the rescoring's exp, which is torch's CUDA exp where the reference uses its CPU exp (DESIGN.md
+section 4 gives the measured difference):
+
+    det = detect.postprocess(scores, boxes, image_sizes=sizes, nms_method="soft", sigma=0.5)
 
     scores, boxes = model(images)          # the reference's is_test form: boxes = (locations, priors, cv, sv)
     det = detect.postprocess(scores, boxes, image_sizes=sizes)
@@ -109,8 +113,9 @@ class Detections:
 
 
 def postprocess(scores, locations, priors=None, center_variance=None, size_variance=None, image_sizes=None,
-                prob_threshold=0.01, iou_threshold=0.45, candidate_size=200, top_k=-1) -> Detections:
-    """Predictor.predict's post-processing (hard NMS) for a batch, on the GPU, with one host synchronisation.
+                prob_threshold=0.01, iou_threshold=0.45, candidate_size=200, top_k=-1, nms_method=None,
+                sigma=0.5) -> Detections:
+    """Predictor.predict's post-processing for a batch, on the GPU, with one host synchronisation.
 
     scores: softmax output fp32 [N, P, C], class 0 the background.  locations: fp32 [N, P, 4], or the tuple
     (locations, priors, center_variance, size_variance) that an SSD in the reference's is_test form returns next to the
@@ -122,7 +127,22 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
     by prior index), box_utils.hard_nms at iou_threshold stopping at top_k picks when top_k > 0.  Thresholds are taken as
     fp32, as torch compares an fp32 tensor with a Python float.  Predictor.predict(image, top_k, prob_threshold) falls back
     to its filter_threshold when prob_threshold is None or 0; pass that value here.  candidate_size is 1 .. 1024.
+
+    nms_method: None or "hard" as above; "soft" is box_utils.soft_nms, as Predictor(nms_method="soft", sigma=sigma) runs
+    it: per class, every candidate (no candidate_size cut, iou_threshold unused) in prior order, then repeatedly the
+    first row of the largest current score is picked with that score, the last row takes its place, every remaining row
+    is rescored by exp(-(iou * iou) / sigma) and dropped unless its score stays above prob_threshold; at most top_k picks
+    when top_k > 0.  Every op is the reference's bit for bit except exp, which is torch's exp on a CUDA tensor (CUDA's
+    expf) where the reference runs torch's CPU exp; DESIGN.md section 4 states the difference.  sigma is a finite
+    positive number, taken as fp32.
     """
+    if nms_method not in (None, "hard", "soft"):
+        raise _lib.DfqError("nms_method must be None, 'hard' or 'soft', got %r" % (nms_method,))
+    if nms_method == "soft":
+        with np.errstate(over="ignore"):
+            sigma32 = np.float32(sigma) if isinstance(sigma, (int, float)) and not isinstance(sigma, bool) else None
+        if sigma32 is None or not np.isfinite(sigma32) or not sigma32 > 0:
+            raise _lib.DfqError("sigma must be a finite positive number, got %r" % (sigma,))
     if isinstance(locations, (tuple, list)):
         if priors is not None or center_variance is not None or size_variance is not None:
             raise _lib.DfqError("locations is the (locations, priors, center_variance, size_variance) tuple: pass the "
@@ -153,6 +173,8 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
     dev = scores.device
     boxes = torch.empty_like(locations)
     _lib.check(lib.dfq_ssd_decode(_ptr(locations), _ptr(priors), _ptr(boxes), dp, st), "dfq_ssd_decode")
+    if nms_method == "soft":
+        return _soft(lib, st, dp, scores, boxes, image_sizes, N, C_, float(sigma))
     S, K = N * (C_ - 1), candidate_size
     slot_boxes = torch.empty(S, K, 4, dtype=torch.float32, device=dev)
     slot_probs = torch.empty(S, K, dtype=torch.float32, device=dev)
@@ -168,6 +190,27 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
         _lib.check(lib.dfq_ssd_compact(_ptr(slot_boxes), _ptr(slot_probs), _ptr(counts), _ptr(seg_offsets),
                                        _ptr(image_sizes), _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, st),
                    "dfq_ssd_compact")
+    return Detections(out_boxes, labels, probs, seg_offsets[::C_ - 1])
+
+
+def _soft(lib, st, dp, scores, boxes, image_sizes, N, C_, sigma):
+    """The soft NMS half of postprocess: pick counts and their scan, the one synchronisation for the total, then the
+    picks written straight to their rows (the kernel runs the same steps twice, so nothing is kept per candidate)."""
+    dev = scores.device
+    S = N * (C_ - 1)
+    work = torch.empty(2 * S, dtype=torch.int32, device=dev)          # candidate counts, pick counts
+    cands, counts = work[:S], work[S:]
+    seg_offsets = torch.empty(S + 1, dtype=torch.int64, device=dev)
+    _lib.check(lib.dfq_ssd_soft_nms(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(counts), _ptr(seg_offsets), dp, sigma,
+                                    st), "dfq_ssd_soft_nms")
+    T = int(seg_offsets[-1])
+    out_boxes = torch.empty(T, 4, dtype=torch.float32, device=dev)
+    labels = torch.empty(T, dtype=torch.int64, device=dev)
+    probs = torch.empty(T, dtype=torch.float32, device=dev)
+    if T:
+        _lib.check(lib.dfq_ssd_soft_compact(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(seg_offsets), _ptr(image_sizes),
+                                            _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, sigma, st),
+                   "dfq_ssd_soft_compact")
     return Detections(out_boxes, labels, probs, seg_offsets[::C_ - 1])
 
 

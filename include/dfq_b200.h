@@ -786,6 +786,27 @@ int dfq_ssd_nms(const float* scores, const float* boxes, float* slot_boxes, floa
 int dfq_ssd_compact(const float* slot_boxes, const float* slot_probs, const int32_t* counts, const int64_t* offsets,
                     const float* image_sizes, float* out_boxes, int64_t* out_labels, float* out_probs, const DfqSsdNms* d,
                     void* stream);
+/* box_utils.soft_nms per (image n, class c = 1 .. C-1), as Predictor.predict calls it with nms_method "soft": of scores
+ * fp32 [N, P, C] and the decoded boxes fp32 [N, P, 4], the candidates (score > prob_threshold) in prior order; then, until
+ * no row remains: pick the first row of the largest score (NaN the largest), emit its box and current score, stop once
+ * top_k > 0 picks are made or it was the only row, move the last row into its place and drop the last row, rescore every
+ * row s = fl(s * expf(fl(fl(-fl(iou * iou)) / sigma))) with iou = iou_of(picked, row) in the reference's op order, and
+ * keep the rows with s > prob_threshold in order.  expf is CUDA's precise expf (torch's exp on a CUDA tensor); every
+ * other op is the reference's, bit for bit.  candidate_size and iou_threshold are not read.
+ * Writes the candidate count of segment s = n * (C - 1) + c - 1 to candidates[s] and its pick count to counts[s] (both
+ * int32 [N * (C - 1)]), and the exclusive scan of counts to offsets (int64 [N * (C - 1) + 1], as dfq_ssd_nms).  Segments
+ * of more than 11,264 candidates hold their rows in global memory: the call then allocates 20 * P bytes per SM on
+ * `stream` and frees them there.  DFQ_E_ARG, with a reason: the refusals of dfq_ssd_decode, C < 2, sigma not finite and
+ * positive, a NULL pointer, boxes not 16-byte aligned.  DFQ_E_UNSUPPORTED: N * (C - 1) above INT32_MAX. */
+int dfq_ssd_soft_nms(const float* scores, const float* boxes, int32_t* candidates, int32_t* counts, int64_t* offsets,
+                     const DfqSsdNms* d, float sigma, void* stream);
+/* The flat output of dfq_ssd_soft_nms's picks, laid out as dfq_ssd_compact lays out the hard picks (out_probs the picks'
+ * decayed scores).  It runs the same soft NMS again on the same inputs, d and sigma, with candidates and offsets as
+ * dfq_ssd_soft_nms left them, and writes each pick straight to its row.  Refusals of dfq_ssd_soft_nms, and DFQ_E_ARG for
+ * a NULL output or out_boxes not 16-byte aligned. */
+int dfq_ssd_soft_compact(const float* scores, const float* boxes, int32_t* candidates, const int64_t* offsets,
+                         const float* image_sizes, float* out_boxes, int64_t* out_labels, float* out_probs,
+                         const DfqSsdNms* d, float sigma, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Segmentation evaluation (utils/segmentation/utils.py forward_all, utils/metrics.py Evaluator) for a batch

@@ -20,6 +20,7 @@ build container.  Committed next to its outputs so every fixture can be regenera
                           pin tests (tests/test_oracle_pins.py, test_op_patching.py, test_distill.py)
 
   ref_ssd_postprocess.npz the reference's Predictor.predict post-processing on seeded SSD-Lite-shaped outputs
+  ref_ssd_soft_nms.npz    the same with Predictor(nms_method="soft"): soft_nms on the CPU, sigma 0.3, top_k -1 / 1 / 5
   ref_seg_eval.npz        the reference's forward_all predictions and Evaluator matrices and metrics on seeded batches
   ref_ssd_map.npz         main_ssd.py's per-class VOC average precision on a seeded set of detections and annotations
   ref_absorb_clip.npz     the reference's merge_batchnorm -> cross_layer_equalization -> bias_absorption -> clip_weight ->
@@ -29,7 +30,7 @@ build container.  Committed next to its outputs so every fixture can be regenera
                           equalization and after the clip)
 
 usage: python tools/make_golden.py [topology] [mobilenetv2] [resnet18] [deeplab] [ssd] [ops] [bc] [minmax] [table] [live]
-       [ssd_post] [seg_eval] [ssd_map] [absorb_clip]
+       [ssd_post] [ssd_soft] [seg_eval] [ssd_map] [absorb_clip]
 """
 import hashlib
 import json
@@ -439,6 +440,57 @@ def ssd_postprocess():
 
 if __name__ == "__main__" and "ssd_post" in sys.argv[1:]:
     ssd_postprocess()
+
+
+SSD_SOFT_TOP_K = [-1, 1, 5]
+SSD_SOFT_SIGMA = 0.3
+
+
+def ssd_soft_nms():
+    """The reference's Predictor(nms_method="soft", sigma=SSD_SOFT_SIGMA).predict (box_utils decode, threshold,
+    soft_nms, scaling) on the CPU, run on two seeded SSD-Lite-shaped images with the priors of mobilenetv1_ssd_config
+    (3,000 x 4), for each top_k of SSD_SOFT_TOP_K.  Image 1 is peakier and has a class without candidates."""
+    from modeling.detection.config import mobilenetv1_ssd_config as cfg
+    from modeling.detection.predictor import Predictor
+    priors = cfg.priors.float().contiguous()
+    P, C = priors.shape[0], 21
+    g = torch.Generator().manual_seed(11)
+    logits = torch.randn(2, P, C, generator=g) * 2.5
+    logits[..., 0] += 5.0
+    logits[1, :, 1:] *= 1.6
+    logits[1, :, 7] -= 40.0                       # no candidate of class 7 in image 1
+    scores = torch.softmax(logits, dim=2)
+    locations = torch.randn(2, P, 4, generator=g) * 0.7
+    sizes = np.array([[500, 375], [300, 300]], np.int64)
+
+    class Outputs(nn.Module):
+        def forward(self, x):
+            return self.scores, (self.locations, priors, cfg.center_variance, cfg.size_variance)
+
+    net = Outputs()
+    out = dict(scores=scores.numpy(), locations=locations.numpy(), priors=priors.numpy(), image_sizes=sizes,
+               variances=np.array([cfg.center_variance, cfg.size_variance]), prob_threshold=np.array(0.01),
+               sigma=np.array(SSD_SOFT_SIGMA), top_ks=np.array(SSD_SOFT_TOP_K))
+    pred = Predictor(net, cfg.image_size, cfg.image_mean, cfg.image_std, nms_method="soft", sigma=SSD_SOFT_SIGMA,
+                     device=torch.device("cpu"))
+    for k, top_k in enumerate(SSD_SOFT_TOP_K):
+        boxes, labels, probs, offs = [], [], [], [0]
+        for n in range(2):
+            net.scores, net.locations = scores[n:n + 1], locations[n:n + 1]
+            w, h = (int(v) for v in sizes[n])
+            b, l, p = pred.predict(np.zeros((h, w, 3), np.uint8), top_k=top_k, prob_threshold=0.01)
+            boxes.append(b.reshape(-1, 4)); labels.append(l.reshape(-1).long()); probs.append(p.reshape(-1))
+            offs.append(offs[-1] + b.shape[0])
+        out["boxes_%d" % k] = torch.cat(boxes).numpy()
+        out["labels_%d" % k] = torch.cat(labels).numpy()
+        out["probs_%d" % k] = torch.cat(probs).numpy()
+        out["offsets_%d" % k] = np.array(offs)
+        print("ssd soft nms top_k %d: kept per image %s" % (top_k, np.diff(offs).tolist()))
+    np.savez_compressed(os.path.join(GOLD, "ref_ssd_soft_nms.npz"), **out)
+
+
+if __name__ == "__main__" and "ssd_soft" in sys.argv[1:]:
+    ssd_soft_nms()
 
 
 # ---------------------------------------------------------------------------------------------------------
