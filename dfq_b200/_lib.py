@@ -242,6 +242,9 @@ SIGNATURES = {
     "dfq_i8_affine_conv_rows": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _PF, C.c_void_p, C.c_void_p,
                                 _ST],
     "dfq_i8_affine_maxpool": [C.c_void_p, _PF, _PF, C.c_void_p, C.c_void_p, C.c_float, C.c_float, _I32, C.c_void_p, _ST],
+    "dfq_i8_pack_codes": [C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_unpack_codes": [C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_i8_plane_mean": [_PF, _PF, C.c_void_p, _I64, _I32, _I64, _I32, C.c_float, _ST],
     "dfq_ssd_decode": [_PF, _PF, _PF, C.c_void_p, _ST],
     "dfq_ssd_nms": [_PF, _PF, _PF, _PF, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
     "dfq_ssd_compact": [_PF, _PF, C.c_void_p, C.c_void_p, _PF, _PF, C.c_void_p, _PF, C.c_void_p, _ST],

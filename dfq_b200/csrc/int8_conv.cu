@@ -1168,6 +1168,82 @@ int check_pool(const char* who, const DfqI8Pool* g, const void* xq, const void* 
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// ncnn model files: weight codes verbatim, and ncnn's plane mean
+// ------------------------------------------------------------------------------------------------------------------
+
+// Element (o, c, tap) of ncnn's codes [O][C/g][kh][kw] -> its index in the packed layout of k_i8_pack_dense (groups == 1:
+// [O][taps][Cpad]) or k_i8_pack_dw (depthwise, c == 0: [taps][Cpad] with channel o)
+__device__ __forceinline__ int64_t packed_index(int64_t o, int c, int tap, int taps, int Cpad, bool dense) {
+  return dense ? (o * taps + tap) * Cpad + c : (int64_t)tap * Cpad + o;
+}
+
+// One thread per packed byte: the code it holds, or 0 in a pad channel
+__global__ void k_i8_pack_codes(const int8_t* __restrict__ codes, int8_t* __restrict__ out, int C, int taps, int Cpad,
+                                bool dense, int64_t total) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % Cpad);
+    const int64_t t = i / Cpad;
+    if (dense) {
+      const int tap = (int)(t % taps);
+      const int64_t o = t / taps;
+      out[i] = c < C ? codes[(o * C + c) * taps + tap] : (int8_t)0;
+    } else {
+      out[i] = c < C ? codes[(int64_t)c * taps + t] : (int8_t)0;
+    }
+  }
+}
+
+// One thread per code of ncnn's layout, read back from the packed layout
+__global__ void k_i8_unpack_codes(const int8_t* __restrict__ packed, int8_t* __restrict__ codes, int Cg, int taps, int Cpad,
+                                  bool dense, int64_t total) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int tap = (int)(i % taps);
+    const int64_t t = i / taps;
+    codes[i] = packed[packed_index(t / Cg, (int)(t % Cg), tap, taps, Cpad, dense)];
+  }
+}
+
+// ncnn's mean of each (image, channel) plane of x [N, C, P]: sum = 0.f, then sum += x[p] for p = 0 .. P - 1 in order (fp32,
+// each add rounded), then sum * k (Reduction MEAN: k = fp32(1 / P)) or sum / P (Pooling global average, divide).  Row r
+// of the output walks [N, cols): cols = Cpad when the codes are written (r past C: a pad channel, code 0), else C.
+// Each warp owns 32 consecutive rows.  It stages them 32 columns at a time through shared memory - one coalesced 128-byte
+// load per plane - and lane i then adds row i's 32 values in plane order, so the order is the sequential one.
+constexpr int PM_WARPS = 8;
+
+__global__ void __launch_bounds__(PM_WARPS * 32) k_i8_plane_mean(const float* __restrict__ x, float* __restrict__ y,
+                                                                 int8_t* __restrict__ yq, int C, int cols, int64_t P,
+                                                                 int64_t rows, bool divide, float k, float out_scale) {
+  __shared__ float tile[PM_WARPS][32][33];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float(*s)[33] = tile[warp];
+  for (int64_t base = ((int64_t)blockIdx.x * PM_WARPS + warp) * 32; base < rows;
+       base += (int64_t)gridDim.x * PM_WARPS * 32) {
+    const int64_t r = base + lane;
+    const int64_t n = r / cols;
+    const int c = (int)(r - n * cols);
+    const bool real = r < rows && c < C;
+    const int64_t off = real ? (n * C + c) * P : -1;        // this lane's plane, broadcast to the warp below
+    float sum = 0.f;
+    for (int64_t j0 = 0; j0 < P; j0 += 32) {
+      const bool col = j0 + lane < P;
+#pragma unroll 8
+      for (int i = 0; i < 32; ++i) {
+        const int64_t o = __shfl_sync(0xffffffffu, off, i);
+        if (o >= 0 && col) s[i][lane] = __ldg(x + o + j0 + lane);
+      }
+      __syncwarp();
+      const int m = P - j0 < 32 ? (int)(P - j0) : 32;
+      for (int j = 0; j < m; ++j) sum = __fadd_rn(sum, s[lane][j]);
+      __syncwarp();
+    }
+    if (r >= rows) continue;
+    const float v = divide ? __fdiv_rn(sum, (float)P) : __fmul_rn(sum, k);
+    if (real && y) y[n * C + c] = v;
+    if (yq) yq[r] = real ? q8(v, out_scale) : (int8_t)0;
+  }
+}
+
 }  // namespace
 }  // namespace dfq
 
@@ -1667,4 +1743,61 @@ extern "C" int dfq_i8_affine_conv_rows(const int8_t* xq, const int32_t* S_in, co
   ep.y = r->y, ep.off = r->off, ep.img_stride = r->img_stride;
   ep.pre_lo = r->pre_lo, ep.pre_hi = r->pre_hi, ep.post_lo = r->post_lo, ep.post_hi = r->post_hi;
   return launch_conv<Out::AFFINE_ROWS>(who, xq, wq, nullptr, bias, nullptr, nullptr, g, ep, (cudaStream_t)stream);
+}
+
+// The packed layout's geometry: a dense or depthwise layer of g (the packers read O, C, kh, kw, groups and Cpad)
+static int check_codes(const char* who, const DfqI8Conv* g, const int8_t* a, const int8_t* b) {
+  if (int rc = check_geometry(g)) return rc;
+  DFQ_REQUIRE_WHO(a && b, "null pointer");
+  const int64_t n_codes = (int64_t)g->O * (g->C / g->groups) * g->kh * g->kw;
+  const int64_t n_packed = (int64_t)(g->groups == 1 ? g->O : 1) * g->kh * g->kw * g->Cpad;
+  DFQ_REQUIRE_WHO(!overlap(a, n_codes, b, n_packed), "codes and packed overlap");
+  return 0;
+}
+
+extern "C" int dfq_i8_pack_codes(const int8_t* codes, int8_t* packed, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_codes("dfq_i8_pack_codes", g, codes, packed)) return rc;
+  const int taps = g->kh * g->kw;
+  const bool dense = g->groups == 1;
+  const int64_t total = (int64_t)(dense ? g->O : 1) * taps * g->Cpad;
+  k_i8_pack_codes<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(codes, packed, g->C, taps, g->Cpad, dense, total);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_unpack_codes(const int8_t* packed, int8_t* codes, const DfqI8Conv* g, void* stream) {
+  if (int rc = check_codes("dfq_i8_unpack_codes", g, codes, packed)) return rc;
+  const int taps = g->kh * g->kw;
+  const bool dense = g->groups == 1;
+  const int64_t total = (int64_t)g->O * (g->C / g->groups) * taps;
+  k_i8_unpack_codes<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(packed, codes, g->C / g->groups, taps, g->Cpad,
+                                                                            dense, total);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dfq_i8_plane_mean(const float* x, float* y, int8_t* yq, int64_t N, int32_t C, int64_t P, int32_t divide,
+                                 float out_scale, void* stream) {
+  const char* who = "dfq_i8_plane_mean";
+  DFQ_REQUIRE_WHO(x != nullptr, "null input");
+  DFQ_REQUIRE_WHO(y || yq, "no output requested (y and yq are both NULL)");
+  DFQ_REQUIRE_WHO(N > 0 && C > 0 && P > 0, "empty dimension");
+  DFQ_REQUIRE_WHO(divide == 0 || divide == 1, "divide must be 0 (multiply by fp32(1 / P)) or 1 (divide by P)");
+  DFQ_REQUIRE_WHO(((uintptr_t)x & 3) == 0 && ((uintptr_t)y & 3) == 0, "x and y must be 4-byte aligned");
+  DFQ_REQUIRE_WHO(aligned16(yq), "yq must be 16-byte aligned");
+  DFQ_REQUIRE_WHO(!yq || (std::isfinite(out_scale) && out_scale >= 0.f),
+                  "out_scale must be finite and non-negative when yq is written");
+  DFQ_REQUIRE_WHO(N <= INT64_MAX / C / P / 4, "x is too large");
+  const int cpad = (C + 15) / 16 * 16;
+  const int64_t x_bytes = N * C * P * 4, y_bytes = N * C * 4, yq_bytes = N * cpad;
+  DFQ_REQUIRE_WHO(!overlap(x, x_bytes, y, y_bytes) && !overlap(x, x_bytes, yq, yq_bytes) && !overlap(y, y_bytes, yq, yq_bytes),
+                  "x, y and yq overlap");
+  const int cols = yq ? cpad : C;
+  const int64_t rows = N * cols;
+  const int64_t blocks = std::max<int64_t>(1, std::min<int64_t>((rows + PM_WARPS * 32 - 1) / (PM_WARPS * 32),
+                                                                (int64_t)sm_count() * 8));
+  k_i8_plane_mean<<<(unsigned)blocks, PM_WARPS * 32, 0, (cudaStream_t)stream>>>(x, y, yq, C, cols, P, rows, divide != 0,
+                                                                                1.f / (float)P, out_scale);
+  DFQ_CUDA(cudaGetLastError());
+  return 0;
 }

@@ -261,10 +261,25 @@ class _Int8Layer(_ConvLayer):
         self.register_buffer("dq", torch.from_numpy(dequant_scales(self.act_scale, w_scale)).to(dev))
         b = torch.zeros(O) if bias is None else bias.detach().float()
         self.register_buffer("bias", b.to(dev).contiguous())
-        w = weight.detach().float().to(dev).contiguous()
         lib = _lib.load()
+        if weight.dtype == torch.int8:                          # codes, packed verbatim (Int8Conv2d.from_codes)
+            w = weight.detach().to(dev).contiguous()
+            _lib.check(lib.dfq_i8_pack_codes(_ptr(w), _ptr(self.weight_codes), _lib.table_ptr(self._pack_geometry()),
+                                             _lib.stream_ptr()), "dfq_i8_pack_codes")
+            return
+        w = weight.detach().float().to(dev).contiguous()
         _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes),
                                            _lib.table_ptr(self._pack_geometry()), _lib.stream_ptr()), "dfq_i8_pack_weights")
+
+    def unpack_codes(self):
+        """The int8 weight codes [O, C/groups, kh, kw] of the packed layer (dfq_i8_unpack_codes), on its device."""
+        kh, kw = self.kernel_size
+        codes = torch.empty((self.out_channels, self.in_channels // self.groups, kh, kw), dtype=torch.int8,
+                            device=self.weight_codes.device)
+        _lib.check(_lib.load().dfq_i8_unpack_codes(_ptr(self.weight_codes), _ptr(codes),
+                                                   _lib.table_ptr(self._pack_geometry()), _lib.stream_ptr()),
+                   "dfq_i8_unpack_codes (layer %s)" % self._who())
+        return codes
 
     def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None, rows=False, sums=False):
         """A new module of the same class on the same packed buffers (weight_codes, dq, bias, w_scale), in the given execution
@@ -413,6 +428,16 @@ class Int8Conv2d(_Int8Layer):
         if err is not None:
             raise err
         return cls(conv.weight, conv.bias, act_scale, w_scale, conv.stride, conv.padding, conv.dilation, conv.groups)
+
+    @classmethod
+    def from_codes(cls, codes, bias, act_scale, w_scale, stride=1, padding=0, dilation=1, groups=1):
+        """The layer of int8 weight codes [O, C/groups, kh, kw] (an ncnn model file's, ncnn.load), packed verbatim
+        (dfq_i8_pack_codes) rather than re-derived from fp32 weights; bias [O] or None, w_scale a scalar or [O]."""
+        codes = torch.as_tensor(np.ascontiguousarray(codes, np.int8))
+        if codes.dim() != 4:
+            raise _lib.DfqError("int8 weight codes must be [O, C/groups, kh, kw], got %s" % list(codes.shape))
+        return cls(codes, None if bias is None else torch.as_tensor(np.asarray(bias, _f32)), act_scale, w_scale, stride,
+                   padding, dilation, groups)
 
     def forward(self, x, r=None, out=None, off=0):
         return self.run(x, residual=r, out=out, off=off)[0]
@@ -1217,7 +1242,8 @@ class _Int8Tracer(fx.Tracer):
         self.callers = callers
 
     def is_leaf_module(self, m, qualname):
-        return isinstance(m, _ConvLayer) or super().is_leaf_module(m, qualname)
+        from .ncnn import PlaneMean                             # an ncnn model's means (ncnn.load) call the library
+        return isinstance(m, (_ConvLayer, PlaneMean)) or super().is_leaf_module(m, qualname)
 
     def create_proxy(self, kind, target, args, kwargs, *rest, **kw):
         proxy = super().create_proxy(kind, target, args, kwargs, *rest, **kw)
@@ -2452,10 +2478,56 @@ class _Rewriter:
         self.edges += [(u.name, v.target, pp.clamp) for v in pp.codes if v in self.convs]
         return u.name, "fp32", ("fp32", "codes")
 
+    def plan_means(self, planned):
+        """The tail rule of an ncnn model (ncnn.load): a producer's single-user pass-through chain, an optional flatten,
+        a PlaneMean and, past an optional reshape, a dense 1 x 1 Int8Conv2d of its channels.  Returns [(producer, its
+        pass-throughs, clamp, flatten | None, mean node, reshape | None, consumer)]."""
+        from .ncnn import PlaneMean
+        means = []
+        for m in (list(self.gm.graph.nodes) if self.scheme is _NCNN else []):
+            if m.op != "call_module" or type(self.mods[m.target]) is not PlaneMean or \
+                    self.mods[m.target].out_scale is not None or len(m.users) != 1 or len(m.args) != 1 or m.kwargs:
+                continue
+            x, view = m.args[0], None
+            if isinstance(x, fx.Node) and x.op == "call_method" and x.target == "flatten" and len(x.users) == 1:
+                x, view = x.args[0], x
+            back = _walk_back(x, self.mods, self.producer) if isinstance(x, fx.Node) else None
+            if back is None or back[0] in planned:
+                continue
+            q, reshape = next(iter(m.users)), None
+            if q.op == "call_method" and q.target in ("reshape", "view") and len(q.users) == 1 and len(q.all_input_nodes) == 1:
+                q, reshape = next(iter(q.users)), q
+            if not self.producer(q) or q.args[0] is not (reshape or m):
+                continue
+            c, mod = self.mods[back[0].target].out_channels, self.mods[q.target]
+            if mod.groups != 1 or mod.kernel_size != (1, 1) or mod.in_channels != c:
+                continue
+            means.append((back[0], back[2], back[1], view, m, reshape, q))
+        return means
+
+    def rewrite_mean(self, p, path, clamp, view, m, reshape, q):
+        """p writes its clamped fp32 output, the mean writes q's codes [N, 1, 1, Cpad] and q reads them."""
+        g = self.gm.graph
+        self.modes[p.target] = dict(epilogue=Epilogue(None, clamp, _FULL, False, True))
+        first = path[0] if path else p
+        first.replace_all_uses_with(p)
+        for node in path:                                       # from the flatten back: each has no user left
+            g.erase_node(node)
+        mean = self.mods[m.target]
+        name = "int8_mean_" + m.name
+        self.gm.add_submodule(name, type(mean)(mean.divide, self.scheme.out(self.scheme.key(self.mods[q.target])),
+                                               name=mean.layer_name))
+        m.target = name
+        if reshape is not None:
+            q.replace_input_with(reshape, m)
+            g.erase_node(reshape)
+        self.edges.append((m.name, q.target, clamp))
+
     def run(self):
         plans, cats = self.plan_producers(), self.plan_cats()
         self.plan_observers(plans, cats)
         ups = self.plan_upsamples(plans, cats)
+        means = self.plan_means({pl.p for pl in plans})
         plans.sort(key=lambda pl: self.order[pl.p])
         self.skip_identities(plans, {n for plan in (*plans, *cats, *self.pools, *ups) for n in plan.nodes()})
         # rewrite in producer order (a producer's input may be the codes of an earlier one, and a residual its fp32
@@ -2469,6 +2541,8 @@ class _Rewriter:
             self.fuse_upsample(up.node, up.scale, up.clamp, _FULL)
             self.hand_over(up, up.node, up.node.name)
         pools = [self.rewrite_pool(pp) for pp in sorted(self.pools, key=lambda pp: self.order[pp.node])]
+        for mp in means:
+            self.rewrite_mean(*mp)
         consumers = {q for _, q, _ in self.edges}
         dense = {p for p, q, _ in self.edges if mods[q].groups == 1}   # producers whose codes a dense consumer reads
         for target in self.modes.keys() | consumers:

@@ -29,6 +29,7 @@ import torch.nn.functional as F
 
 from . import _lib, engine
 from . import int8 as I
+from . import ncnn as N
 from .utils.quantize import QuantMeasure
 
 FORMAT = "dfq_b200.int8.chained"
@@ -47,6 +48,7 @@ _CONSTRUCTED = {
     I.AffineInt8UpsampleBilinear: ("channels", "align_corners", "out", "out_slice", "pre", "obs", "post", "sums",
                                    "layer_name"),
     I.Int8HeadConcat: ("k", "batch", "layer_name"),
+    N.PlaneMean: ("divide", "out_scale", "layer_name"),
 }
 _LAYERS = (I.Int8Conv2d, I.Int8Linear, I.AffineInt8Conv2d, I.AffineInt8Linear)
 # modules rebuilt from their plain attributes, parameters and buffers

@@ -748,6 +748,29 @@ int dfq_i8_affine_maxpool(const int8_t* xq, const float* x, float* y, int8_t* yq
                           int32_t out_bits, const DfqI8Pool* g, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * ncnn int8 model files (dfq_b200/ncnn.py): the weight codes as the file holds them, and ncnn's mean of a plane
+ * ------------------------------------------------------------------------------------------- */
+/* int8 codes in ncnn's weight layout [O][C/groups][kh][kw] -> the packed layout of dfq_i8_pack_weights (groups == 1:
+ * [O][kh][kw][Cpad]; depthwise: [kh*kw][Cpad]; pad channels 0), copied verbatim: no scale, no rounding.  Uses g's O, C,
+ * kh, kw, groups and Cpad; refusals of dfq_i8_pack_weights, and DFQ_E_ARG with a reason: a NULL pointer, codes and packed
+ * overlapping. */
+int dfq_i8_pack_codes(const int8_t* codes, int8_t* packed, const DfqI8Conv* g, void* stream);
+/* The inverse: the codes [O][C/groups][kh][kw] of a packed layer (pad channels are not read).  Refusals as
+ * dfq_i8_pack_codes. */
+int dfq_i8_unpack_codes(const int8_t* packed, int8_t* codes, const DfqI8Conv* g, void* stream);
+/* ncnn's mean of each (image, channel) plane of x fp32 [N, C, P] (contiguous), in ncnn's order:
+ *   sum = 0.f;  for p in 0 .. P - 1: sum = fp32(sum + x[n, c, p])         sequential, every add rounded
+ *   v   = divide ? fp32(sum / P) : fp32(sum * fp32(1 / P))                   Pooling global average : Reduction MEAN
+ * (a reading of ncnn's pooling.cpp and reduction.cpp, coeff 1).  y fp32 [N, C] receives v (NULL: not written), and / or
+ * yq int8 [N, round_up(C, 16)] the consumer's codes q8(v, out_scale) as dfq_i8_quantize_nhwc forms them (roundf, clamp
+ * +-127, NaN -> -127), pad channels 0 (NULL: not written) - the codes a chained 1 x 1 layer reads as [N, 1, 1, Cpad].
+ * No host synchronisation.  DFQ_E_ARG with a reason: x NULL, y and yq both NULL, N, C or P not positive, divide not 0 or
+ * 1, x or y not 4-byte aligned, yq not 16-byte aligned, out_scale not finite and non-negative while yq is written, x
+ * past 2^63 bytes, x, y and yq overlapping. */
+int dfq_i8_plane_mean(const float* x, float* y, int8_t* yq, int64_t N, int32_t C, int64_t P, int32_t divide, float out_scale,
+                      void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * SSD post-processing (modeling/detection/predictor.py Predictor.predict, utils/detection/box_utils.py) for a batch
  * ------------------------------------------------------------------------------------------- */
 typedef struct DfqSsdNms {
