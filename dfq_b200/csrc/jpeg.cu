@@ -8,9 +8,11 @@
 //                  zeroed workspace.  Reads stay inside the segment (past its end the reader shifts in zeros, as libjpeg
 //                  does, and counts them); an invalid code, a run past coefficient 63 or bits taken past the end stop
 //                  the segment and are recorded in the error word.  A warp thus holds up to 32 independent walkers.
-//   k_jpeg_idct    8 threads per block: dequantisation and jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2, pass 1 down
-//                  the columns into shared memory, pass 2 along the rows, the masked post-IDCT range-limit table), one
-//                  uint8 plane per component, padded to whole MCUs.
+//   k_jpeg_idct    8 threads per block: dequantisation and the islow IDCT (CONST_BITS 13, PASS1_BITS 2, pass 1 down the
+//                  columns into shared memory, pass 2 along the rows) with the arithmetic of libjpeg-turbo's SIMD
+//                  jsimd_idct_islow: 16-bit dequantisation and lane sums, pass 1 saturated to int16 (or its 16-bit
+//                  DC-only shortcut), the output saturated to 0 .. 255; one uint8 plane per component, padded to whole
+//                  MCUs.
 //   k_jpeg_color   one thread per output pixel: h2v1 / h2v2 "fancy" upsampling (the triangle filter, edges replicated
 //                  at the downsampled width and height; plain replication when the chroma plane is at most 2 wide, as
 //                  jinit_upsampler chooses), then ycc_rgb_convert's 16-bit fixed-point tables, written HWC RGB into
@@ -153,33 +155,38 @@ __global__ void __launch_bounds__(kSegThreads) k_jpeg_huff(const DfqJpegSegment*
   }
 }
 
-// ---- jpeg_idct_islow -------------------------------------------------------------------------------------------------------
-constexpr long long F0_298 = 2446, F0_390 = 3196, F0_541 = 4433, F0_765 = 6270, F0_899 = 7373, F1_175 = 9633,
-                    F1_501 = 12299, F1_847 = 15137, F1_961 = 16069, F2_053 = 16819, F2_562 = 20995, F3_072 = 25172;
+// ---- jsimd_idct_islow -------------------------------------------------------------------------------------------------------
+// libjpeg-turbo's SIMD islow IDCT (what Pillow and OpenCV run on x86), not the C jidctint.c: the arithmetic of its 16-bit
+// lanes is part of the output once a block reconstructs outside 0 .. 255.
+constexpr int F0_298 = 2446, F0_390 = 3196, F0_541 = 4433, F0_765 = 6270, F0_899 = 7373, F1_175 = 9633, F1_501 = 12299,
+              F1_847 = 15137, F1_961 = 16069, F2_053 = 16819, F2_562 = 20995, F3_072 = 25172;
 
-// One 1-D pass on x[0..7] (index = frequency), results before the descale in o[0..7] (index = position).
-__device__ __forceinline__ void idct_1d(const long long* x, long long* o) {
-  long long z1 = (x[2] + x[6]) * F0_541;
-  const long long tmp2 = z1 + x[6] * -F1_847, tmp3 = z1 + x[2] * F0_765;
-  const long long tmp0 = (x[0] + x[4]) * 8192, tmp1 = (x[0] - x[4]) * 8192;   // LEFT_SHIFT(, CONST_BITS)
-  const long long t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
-  long long a0 = x[7], a1 = x[5], a2 = x[3], a3 = x[1];
-  z1 = a0 + a3;
-  long long z2 = a1 + a2, z3 = a0 + a2, z4 = a1 + a3;
-  const long long z5 = (z3 + z4) * F1_175;
-  a0 *= F0_298; a1 *= F2_053; a2 *= F3_072; a3 *= F1_501;
-  z1 *= -F0_899; z2 *= -F2_562; z3 *= -F1_961; z4 *= -F0_390;
-  z3 += z5; z4 += z5;
-  a0 += z1 + z3; a1 += z2 + z4; a2 += z2 + z3; a3 += z1 + z4;
+__device__ __forceinline__ int lo16(int v) { return (int)(int16_t)(uint16_t)(unsigned)v; }     // a 16-bit lane's wrap
+__device__ __forceinline__ unsigned mul(int a, int c) { return (unsigned)a * (unsigned)c; }
+
+// One 1-D pass on the int16 values x[0..7] (index = frequency), results before the descale in o[0..7] (index = position),
+// modulo 2^32 as the lanes form them: x0 + x4, x0 - x4, x7 + x3 and x5 + x1 wrap in 16 bits (paddw / psubw), every other
+// sum is taken in 32 bits from pmaddwd products with the constant pairs below.
+__device__ __forceinline__ void idct_1d(const int* x, unsigned* o) {
+  const unsigned tmp3 = mul(x[2], F0_541 + F0_765) + mul(x[6], F0_541);
+  const unsigned tmp2 = mul(x[2], F0_541) + mul(x[6], F0_541 - F1_847);
+  const unsigned tmp0 = mul(lo16(x[0] + x[4]), 8192), tmp1 = mul(lo16(x[0] - x[4]), 8192);   // << CONST_BITS
+  const unsigned t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  const int z3 = lo16(x[7] + x[3]), z4 = lo16(x[5] + x[1]);
+  const unsigned y3 = mul(z3, F1_175 - F1_961) + mul(z4, F1_175), y4 = mul(z3, F1_175) + mul(z4, F1_175 - F0_390);
+  const unsigned a0 = mul(x[7], F0_298 - F0_899) + mul(x[1], -F0_899) + y3;
+  const unsigned a3 = mul(x[7], -F0_899) + mul(x[1], F1_501 - F0_899) + y4;
+  const unsigned a1 = mul(x[5], F2_053 - F2_562) + mul(x[3], -F2_562) + y4;
+  const unsigned a2 = mul(x[5], -F2_562) + mul(x[3], F3_072 - F2_562) + y3;
   o[0] = t10 + a3; o[7] = t10 - a3; o[1] = t11 + a2; o[6] = t11 - a2;
   o[2] = t12 + a1; o[5] = t12 - a1; o[3] = t13 + a0; o[4] = t13 - a0;
 }
 
-// range_limit[x & RANGE_MASK] of the post-IDCT table: x + 128 for -128 .. 127, 255 up to 383, 0 from -512, wrapping.
-__device__ __forceinline__ uint8_t idct_limit(long long x) {
-  const int m = (int)(x & 1023);
-  return (uint8_t)(m < 128 ? m + 128 : m < 512 ? 255 : m < 896 ? 0 : m - 896);
-}
+// DESCALE(, n) as paddd + psrad: the rounding constant added modulo 2^32, then an arithmetic shift.
+__device__ __forceinline__ int descale(unsigned v, int n) { return (int)(v + (1u << (n - 1))) >> n; }
+
+// The output limit: packssdw + packsswb saturate to -128 .. 127, then paddb adds CENTERJSAMPLE.
+__device__ __forceinline__ uint32_t idct_limit(int v) { return (uint32_t)(min(max(v, -128), 127) + 128); }
 
 __global__ void __launch_bounds__(kIdctThreads) k_jpeg_idct(const DfqJpegImage* __restrict__ ims,
                                                             const JpegWork* __restrict__ work, int n, int64_t nblocks,
@@ -191,7 +198,9 @@ __global__ void __launch_bounds__(kIdctThreads) k_jpeg_idct(const DfqJpegImage* 
   const bool live = blk < nblocks;
   int i = 0, comp = 0;
   int64_t b = 0, bx = 0, by = 0;
-  long long x[8], o[8];
+  int x[8];
+  unsigned o[8];
+  bool ac = false;
   if (live) {
     i = owner(n, blk, [&](int k) { return work[k].block0; });
     const DfqJpegImage& im = ims[i];
@@ -211,10 +220,22 @@ __global__ void __launch_bounds__(kIdctThreads) k_jpeg_idct(const DfqJpegImage* 
     const int32_t* q = ((const DfqJpegTables*)(blob + im.tables))->q[comp];
     const int16_t* cb = coef + work[i].coef + b * 64;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) x[k] = (long long)((int)cb[k * 8 + t] * q[k * 8 + t]);    // DEQUANTIZE
-    idct_1d(x, o);
+    for (int k = 0; k < 8; ++k) {
+      x[k] = lo16((int)cb[k * 8 + t] * q[k * 8 + t]);              // DEQUANTIZE: pmullw keeps the low 16 bits
+      ac |= k > 0 && cb[k * 8 + t] != 0;
+    }
+  }
+  // Pass 1's shortcut is taken per block, when the coefficients of rows 1 .. 7 are all zero (its 8 threads' votes).
+  const bool dc_only = ((__ballot_sync(0xffffffffu, ac) >> (threadIdx.x & 24)) & 0xFF) == 0;
+  if (live) {
+    if (dc_only) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) ws[lb][k * 8 + t] = (int)((o[k] + (1 << 10)) >> 11);   // DESCALE(, CONST_BITS - PASS1_BITS)
+      for (int k = 0; k < 8; ++k) ws[lb][k * 8 + t] = lo16(x[0] * 4);                 // psllw by PASS1_BITS
+    } else {
+      idct_1d(x, o);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) ws[lb][k * 8 + t] = min(max(descale(o[k], 11), -32768), 32767);   // packssdw
+    }
   }
   __syncwarp();                                                   // a block's 8 threads share a warp
   if (!live) return;
@@ -224,8 +245,8 @@ __global__ void __launch_bounds__(kIdctThreads) k_jpeg_idct(const DfqJpegImage* 
   uint32_t lo = 0, hi = 0;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    lo |= (uint32_t)idct_limit((o[k] + (1 << 17)) >> 18) << (8 * k);         // DESCALE(, CONST_BITS + PASS1_BITS + 3)
-    hi |= (uint32_t)idct_limit((o[k + 4] + (1 << 17)) >> 18) << (8 * k);
+    lo |= idct_limit(descale(o[k], 18)) << (8 * k);               // DESCALE(, CONST_BITS + PASS1_BITS + 3)
+    hi |= idct_limit(descale(o[k + 4], 18)) << (8 * k);
   }
   uint8_t* dst = planes + work[i].plane[comp] + (by * 8 + t) * work[i].pw[comp] + bx * 8;
   *(uint2*)dst = make_uint2(lo, hi);

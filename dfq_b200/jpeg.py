@@ -267,8 +267,8 @@ def _huff(counts, vals, dc):
             code += counts[l - 1]
             k += counts[l - 1]
             t["maxcode"][l] = code - 1
-            if code > (1 << l):
-                raise Refused("bad Huffman table (overfull at length %d)" % l)
+            if code >= (1 << l):                      # libjpeg: no code may be all ones, so the last must stay below
+                raise Refused("bad Huffman table (full at length %d: a code of all ones)" % l)
         code <<= 1
     t["maxcode"][17] = 0xFFFFF
     t["vals"][:len(vals)] = np.frombuffer(vals, np.uint8)

@@ -1,5 +1,6 @@
 """A numpy / Python restatement of libjpeg-turbo's baseline decode, as Pillow and OpenCV run it: Huffman decoding with
-restart markers, dequantisation, jpeg_idct_islow (CONST_BITS 13, PASS1_BITS 2, the masked range-limit table), "fancy"
+restart markers, dequantisation and the islow IDCT as the x86 SIMD jsimd_idct_islow computes it (16-bit dequantisation
+and lane sums, pass 1 saturated to int16, the output saturated; not the C jidctint.c's masked range-limit table), "fancy"
 h2v1 / h2v2 chroma upsampling (plain replication when the chroma plane is 2 samples wide or less) and ycc_rgb_convert's
 16-bit fixed-point tables.  Independent of dfq_b200.jpeg: it parses the markers itself.  Test infrastructure only.
 
@@ -51,7 +52,7 @@ def _segments(data):
         elif m in (0xC0, 0xC1):
             H, W, nc = int.from_bytes(body[1:3], "big"), int.from_bytes(body[3:5], "big"), body[5]
             comps = [(body[6 + 3 * k], body[7 + 3 * k] >> 4, body[7 + 3 * k] & 15, body[8 + 3 * k]) for k in range(nc)]
-            frame = (H, W, comps, dict(q))
+            frame = (H, W, comps, q)       # the tables as SOS finds them: libjpeg latches them per scan
         elif m == 0xDD:
             ri = int.from_bytes(body[:2], "big")
         elif m == 0xDA:
@@ -154,8 +155,9 @@ def _decode_interval(buf, mcus, layout, tables, coef, blk0):
         raise Corrupt("scan ends before its last MCU")
 
 
-def coefficients(data):
-    """(frame, int64 coefficient planes per component [by, bx, 64] in natural order, padded to whole MCUs)."""
+def coefficients(data, dequantise=True):
+    """(frame, int64 coefficient planes per component [by, bx, 64] in natural order, padded to whole MCUs): the int16
+    block values times the quantisation table, or as the scan codes them with dequantise=False."""
     (H, W, comps, q), sel, h, ri, ent = _segments(data)
     nc = len(comps)
     if nc == 1:
@@ -181,52 +183,70 @@ def coefficients(data):
     for c in comps:
         hv = c[1] * c[2]
         b = cm[:, :, j:j + hv].reshape(my, mx, c[2], c[1], 64).transpose(0, 2, 1, 3, 4).reshape(my * c[2], mx * c[1], 64)
-        planes.append(b * q[c[3]][None, None, :])
+        planes.append(b * q[c[3]][None, None, :] if dequantise else b.copy())
         j += hv
     return (H, W, comps, hm, vm), planes
 
 
-# ---- jpeg_idct_islow ---------------------------------------------------------------------------------------------------
+# ---- jsimd_idct_islow ---------------------------------------------------------------------------------------------------
 F = dict(c0_298=2446, c0_390=3196, c0_541=4433, c0_765=6270, c0_899=7373, c1_175=9633, c1_501=12299, c1_847=15137,
          c1_961=16069, c2_053=16819, c2_562=20995, c3_072=25172)
 
 
+def wrap16(x):
+    return ((x + (1 << 15)) & 0xFFFF) - (1 << 15)
+
+
+def wrap32(x):
+    return ((x + (1 << 31)) & 0xFFFFFFFF) - (1 << 31)
+
+
 def _idct_1d(x0, x1, x2, x3, x4, x5, x6, x7):
-    z2, z3 = x2, x6
-    z1 = (z2 + z3) * F["c0_541"]
-    tmp2 = z1 + z3 * -F["c1_847"]
-    tmp3 = z1 + z2 * F["c0_765"]
-    tmp0 = (x0 + x4) << 13
-    tmp1 = (x0 - x4) << 13
+    """One pass of jsimd_idct_islow on int16 inputs, before the descale: the 16-bit lane sums x0 + x4, x0 - x4,
+    x7 + x3 and x5 + x1 wrap (paddw / psubw), every other sum is formed in 32 bits (pmaddwd, paddd), modulo 2^32."""
+    tmp3 = x2 * (F["c0_541"] + F["c0_765"]) + x6 * F["c0_541"]
+    tmp2 = x2 * F["c0_541"] + x6 * (F["c0_541"] - F["c1_847"])
+    tmp0 = wrap16(x0 + x4) << 13
+    tmp1 = wrap16(x0 - x4) << 13
     t10, t13, t11, t12 = tmp0 + tmp3, tmp0 - tmp3, tmp1 + tmp2, tmp1 - tmp2
-    tmp0, tmp1, tmp2, tmp3 = x7, x5, x3, x1
-    z1, z2, z3, z4 = tmp0 + tmp3, tmp1 + tmp2, tmp0 + tmp2, tmp1 + tmp3
-    z5 = (z3 + z4) * F["c1_175"]
-    tmp0, tmp1, tmp2, tmp3 = tmp0 * F["c0_298"], tmp1 * F["c2_053"], tmp2 * F["c3_072"], tmp3 * F["c1_501"]
-    z1, z2, z3, z4 = z1 * -F["c0_899"], z2 * -F["c2_562"], z3 * -F["c1_961"], z4 * -F["c0_390"]
-    z3 += z5
-    z4 += z5
-    tmp0 += z1 + z3
-    tmp1 += z2 + z4
-    tmp2 += z2 + z3
-    tmp3 += z1 + z4
+    z3, z4 = wrap16(x7 + x3), wrap16(x5 + x1)
+    z3, z4 = (z3 * (F["c1_175"] - F["c1_961"]) + z4 * F["c1_175"],
+              z3 * F["c1_175"] + z4 * (F["c1_175"] - F["c0_390"]))
+    tmp0 = x7 * (F["c0_298"] - F["c0_899"]) + x1 * -F["c0_899"] + z3
+    tmp3 = x7 * -F["c0_899"] + x1 * (F["c1_501"] - F["c0_899"]) + z4
+    tmp1 = x5 * (F["c2_053"] - F["c2_562"]) + x3 * -F["c2_562"] + z4
+    tmp2 = x5 * -F["c2_562"] + x3 * (F["c3_072"] - F["c2_562"]) + z3
     return [t10 + tmp3, t11 + tmp2, t12 + tmp1, t13 + tmp0, t13 - tmp0, t12 - tmp1, t11 - tmp2, t10 - tmp3]
 
 
-def _range_limit(v):
-    """range_limit[v & RANGE_MASK] of the post-IDCT table (CENTERJSAMPLE already in the table)."""
-    m = v & 1023
-    return np.where(m < 128, m + 128, np.where(m < 512, 255, np.where(m < 896, 0, m - 896))).astype(np.uint8)
+def _descale(v, n):
+    """paddd of the rounding constant and psrad: in 32 bits, wrapping."""
+    return wrap32(v + (1 << (n - 1))) >> n
 
 
-def idct_islow(blocks):
-    """blocks: int64 [..., 64] dequantised, natural order -> uint8 [..., 8, 8]."""
+def idct_islow(blocks, trace=None):
+    """blocks: int64 [..., 64] dequantised (exact products), natural order -> uint8 [..., 8, 8].  A trace dict receives
+    the per-block facts the crafted streams assert: "shortcut" (pass 1's DC-only path taken), "pass1" (pass 1 before its
+    saturation, [n, 8, 8]) and "out" (pass 2 before the output limit, [n, 8, 8]).
+
+    libjpeg-turbo's SIMD jsimd_idct_islow (the SSE2 and AVX2 kernels compute the same): the dequantised value is the
+    low 16 bits of coefficient x quantiser (pmullw); a block whose rows 1 .. 7 are all zero takes pass 1's shortcut,
+    (dc << PASS1_BITS) in 16 bits (psllw, wrapping); otherwise pass 1 saturates its results to int16 (packssdw);
+    pass 2 saturates to int8 (packssdw, packsswb) and adds CENTERJSAMPLE.  Within the range of well-behaved streams
+    this equals jidctint.c; outside it, jidctint.c's masked range-limit table wraps where this saturates."""
+    shape = blocks.shape[:-1]
     b = blocks.reshape(-1, 8, 8)                     # [n, row(u), col]
-    cols = _idct_1d(*[b[:, k, :] for k in range(8)])          # pass 1 over columns: each [n, col]
-    ws = np.stack([(c + (1 << 10)) >> 11 for c in cols], 1)         # DESCALE(x, CONST_BITS - PASS1_BITS): [n, row, col]
+    d = wrap16(b)
+    cols = _idct_1d(*[d[:, k, :] for k in range(8)])          # pass 1 over columns: each [n, col]
+    p1 = np.stack([_descale(c, 11) for c in cols], 1)         # DESCALE(, CONST_BITS - PASS1_BITS): [n, row, col]
+    ws = np.clip(p1, -32768, 32767)
+    dc_only = ~b[:, 1:, :].any(axis=(1, 2))
+    ws[dc_only] = wrap16(d[dc_only, :1, :] << 2)
     rows = _idct_1d(*[ws[:, :, k] for k in range(8)])        # pass 2 over rows: each [n, row]
-    out = np.stack([_range_limit((r + (1 << 17)) >> 18) for r in rows], 2)   # DESCALE(x, CONST_BITS + PASS1_BITS + 3)
-    return out.reshape(blocks.shape[:-1] + (8, 8))
+    out = np.stack([_descale(r, 18) for r in rows], 2)        # DESCALE(, CONST_BITS + PASS1_BITS + 3)
+    if trace is not None:
+        trace.update(shortcut=dc_only, pass1=p1, out=out)
+    return (np.clip(out, -128, 127) + 128).astype(np.uint8).reshape(shape + (8, 8))
 
 
 def _plane(blocks):
