@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.environ.get("DFQ_LIB_OUT") or os.path.join(HERE, "libdfq_sm90.so")
 SOURCES = ["tensor_ops.cu", "cle_engine.cu", "passes.cu", "distill.cu", "host_copy.cu", "int8_conv.cu", "detect.cu",
-           "segment.cu", "detect_map.cu", "preprocess.cu", "jpeg.cu", "classify.cu"]
+           "segment.cu", "detect_map.cu", "preprocess.cu", "jpeg.cu", "classify.cu",
+           "png.cu"]
 HEADERS = [os.path.join(CSRC, h) for h in ("common.cuh", "rowpipe.cuh", "colscan.cuh", "bc_stream.cuh", "bilinear.cuh",
                                            "box_iou.cuh")] + \
     [os.path.join(HERE, "..", "include", "dfq_b200.h")]

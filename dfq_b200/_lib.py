@@ -153,6 +153,15 @@ JPEG_BAD_CODE, JPEG_BAD_RUN, JPEG_SHORT_SCAN = 1, 2, 4    # reason bits of dfq_j
 JPEG_SIZES = {23: (JPEG_IMAGE_DT, 48), 24: (JPEG_SEGMENT_DT, 32), 25: (JPEG_DECODE_DT, 24), 26: (JPEG_HUFF_DT, 1424),
               27: (JPEG_TABLES_DT, 9312)}
 
+PNG_IMAGE_DT = np.dtype([(f, np.int64) for f in ("src", "src_end", "work", "dst")] + [("H", np.int32), ("W", np.int32)],
+                        align=True)
+PNG_DECODE_DT = np.dtype([("n", np.int32), ("_pad", np.int32), ("blob_bytes", np.int64), ("call", np.uint64)], align=True)
+# reason bits of dfq_png_decode's error word
+PNG_BAD_BLOCK, PNG_BAD_CODESET, PNG_BAD_CODE, PNG_FAR, PNG_STORED_LEN, PNG_SHORT, PNG_BAD_FILTER, PNG_ADLER = \
+    1, 2, 4, 8, 16, 32, 64, 128
+# struct-size indices of the PNG decoder's structs, checked on their own like JPEG_SIZES
+PNG_SIZES = {29: (PNG_IMAGE_DT, 40), 30: (PNG_DECODE_DT, 24)}
+
 MAP_IGNORED, MAP_TP, MAP_FP = 0, 1, 2                  # verdicts of dfq_map_match
 MAP_ERR_DET_LABEL, MAP_ERR_GT_LABEL, MAP_ERR_DET_OFFSETS, MAP_ERR_GT_OFFSETS = 1, 2, 4, 8   # its device error bits
 
@@ -257,6 +266,7 @@ SIGNATURES = {
     "dfq_map_curve": [C.c_void_p, C.c_void_p, _I64, _I32, C.c_void_p, _I32, C.c_void_p, _I64, C.c_void_p, _ST],
     "dfq_pre_resample": [C.c_void_p, C.c_void_p, C.c_void_p, _PF, _PF, _ST],
     "dfq_jpeg_decode": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
+    "dfq_png_decode": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, _ST],
 }
 
 _lib = None

@@ -496,6 +496,8 @@ extern "C" int dfq_struct_size(int which) {
     case 26: return (int)sizeof(DfqJpegHuff);
     case 27: return (int)sizeof(DfqJpegTables);
     case 28: return (int)sizeof(DfqAbsorb);
+    case 29: return (int)sizeof(DfqPngImage);
+    case 30: return (int)sizeof(DfqPngDecode);
     default: return -1;
   }
 }

@@ -22,7 +22,7 @@ import numbers
 import numpy as np
 import torch
 
-from . import _lib, jpeg
+from . import _lib, jpeg, png
 
 __all__ = ["imagenet", "voc_segmentation", "ssd"]
 
@@ -89,8 +89,8 @@ def _images(images, what="images", planes=3):
     if len(images) == 0:
         raise _lib.DfqError("%s: the batch is empty" % what)
     out = []
-    for i, a in enumerate(jpeg.parse(images, what) if planes else images):
-        if isinstance(a, jpeg._Jpeg):
+    for i, a in enumerate(jpeg.parse(images, what) if planes else png.parse(images, what)):
+        if isinstance(a, (jpeg._Jpeg, png._Png)):
             out.append(a)
             continue
         if isinstance(a, torch.Tensor):
@@ -101,7 +101,7 @@ def _images(images, what="images", planes=3):
             a = a.numpy()
         elif not isinstance(a, np.ndarray):
             raise _lib.DfqError("%s[%d] must be a numpy array, a CPU tensor%s, got %s"
-                                % (what, i, " or JPEG bytes" if planes else "", type(a).__name__))
+                                % (what, i, " or JPEG bytes" if planes else " or PNG bytes", type(a).__name__))
         if a.dtype != np.uint8:
             raise _lib.DfqError("%s[%d] must be uint8, got %s" % (what, i, a.dtype))
         if planes and (a.ndim != 3 or a.shape[2] != planes):
@@ -194,15 +194,15 @@ class _Stage:
 
 
 def _launch(images, labels, xtaps, ytaps, near, filt, norm, out_h, out_w, mean, std):
-    """Gather the batch into the staging buffer, one H2D copy, dfq_jpeg_decode when the batch holds JPEG bytes, one
-    dfq_pre_resample launch."""
+    """Gather the batch into the staging buffer, one H2D copy, dfq_jpeg_decode when the batch holds JPEG bytes,
+    dfq_png_decode when its labels hold PNG bytes, one dfq_pre_resample launch."""
     _lib.require_cuda()
     lib = _lib.load()
     stage = _Stage()
-    jpegs = jpeg._Batch(stage)
+    jpegs, pngs = jpeg._Batch(stage), png._Batch(stage)
     n = len(images)
     desc = np.zeros(n, _lib.PRE_IMAGE_DT)
-    coded = {}
+    coded, coded_labels = {}, {}
     for i, a in enumerate(images):
         d = desc[i]
         d["H"], d["W"] = a.shape[:2]
@@ -215,13 +215,21 @@ def _launch(images, labels, xtaps, ytaps, near, filt, norm, out_h, out_w, mean, 
         if labels is None:
             d["label"] = d["xnear"] = d["ynear"] = -1
         else:
-            d["label"] = stage.place(labels[i])
+            if isinstance(labels[i], png._Png):
+                coded_labels[i] = pngs.add(labels[i])
+            else:
+                d["label"] = stage.place(labels[i])
             d["xnear"], d["ynear"] = stage.table(near[i][0]), stage.table(near[i][1])
-    for i, k in coded.items():                         # the decoded pixels go past every copied byte
+    pngs.base = jpegs.extra                            # the decoded pixels and labels go past every copied byte
+    for i, k in coded.items():
         desc[i]["src"] = jpegs.dst(k)
-    blob = stage.upload(jpegs.extra)
+    for i, k in coded_labels.items():
+        desc[i]["label"] = pngs.dst(k)
+    blob = stage.upload(jpegs.extra + pngs.extra)
     if coded:
         jpegs.launch(blob)
+    if coded_labels:
+        pngs.launch(blob)
     dev = blob.device
     p = np.zeros(1, _lib.PRE_RESAMPLE_DT)
     p["n"], p["out_h"], p["out_w"], p["filter"], p["norm"], p["blob_bytes"] = n, out_h, out_w, filt, norm, blob.numel()
@@ -266,7 +274,8 @@ def voc_segmentation(images, labels=None, crop_size=513, mean=_IMAGENET_MEAN, st
     short side to crop_size (Pillow bilinear for the image, nearest for the label) and center-crops; Normalize divides by
     255 in fp32 and applies mean and std in fp64, each rounded back to fp32.  images as for imagenet() (JPEG bytes
     included, EXIF orientation ignored as Pillow ignores it); labels: None or a list of uint8 HW arrays of the images'
-    sizes.  The label output is what segment.Evaluator.add_logits takes.  Does not synchronise with the host."""
+    sizes, or of PNG bytes (png.probe says which are taken) decoded on the device as Image.open reads them, mixed with
+    arrays if need be; a PNG's size is checked from its header, before any copy.  The label output is what segment.Evaluator.add_logits takes.  Does not synchronise with the host."""
     imgs = _images(images)
     labs = None
     if labels is not None:

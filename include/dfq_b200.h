@@ -46,7 +46,8 @@ const char* dfq_last_error(void);
  * 3 DfqCleResult, 4 DfqFold, 5 DfqExpectTerm, 6 DfqBcLayer, 7 DfqQuantTask, 8 DfqI8Conv, 9 DfqI8Epilogue, 10 DfqI8Pool,
  * 11 DfqI8Resize, 12 DfqI8Affine, 13 DfqI8AffineEpilogue, 14 DfqI8AffineObserve, 15 DfqI8AffineLayout,
  * 16 DfqI8AffineResize, 17 DfqI8AffineRows, 18 DfqSsdNms, 19 DfqSegArgmax, 21 DfqPreImage, 22 DfqPreResample,
- * 23 DfqJpegImage, 24 DfqJpegSegment, 25 DfqJpegDecode, 26 DfqJpegHuff, 27 DfqJpegTables, 28 DfqAbsorb; 20 is
+ * 23 DfqJpegImage, 24 DfqJpegSegment, 25 DfqJpegDecode, 26 DfqJpegHuff, 27 DfqJpegTables, 28 DfqAbsorb,
+ * 29 DfqPngImage, 30 DfqPngDecode; 20 is
  * unassigned and returns -1, as ABI 11 released it): lets a binding verify
  * its struct mirrors without a GPU. */
 int dfq_struct_size(int which);
@@ -1016,6 +1017,43 @@ typedef struct DfqJpegDecode {
  * exactly once in order. */
 int dfq_jpeg_decode(const DfqJpegDecode* d, const DfqJpegImage* images, const DfqJpegSegment* segs, void* blob,
                     uint64_t* error, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * PNG label decoding: non-interlaced 8-bit palette (indices, the palette never applied) or 8-bit gray streams, decoded
+ * as Pillow's Image.open reads them (zlib inflate fed one row at a time, then the five scanline filters), into uint8 HW
+ * ------------------------------------------------------------------------------------------- */
+typedef struct DfqPngImage {
+  int64_t src, src_end;          /* the zlib stream (its 2-byte header, the IDAT payloads joined): byte offsets in the blob */
+  int64_t work;                  /* H * (W + 1) bytes of room for the filtered scanlines: byte offset in the blob          */
+  int64_t dst;                   /* uint8 [H, W] output: byte offset in the blob                                           */
+  int32_t H, W;
+} DfqPngImage;
+typedef struct DfqPngDecode {
+  int32_t n;                     /* images, 1 .. 65535                                                                    */
+  int32_t _pad;
+  int64_t blob_bytes;            /* size of the blob: every stream, workspace and output must lie inside it               */
+  uint64_t call;                 /* tag of this call in the error word, below 2^31                                        */
+} DfqPngDecode;
+#define DFQ_PNG_BAD_BLOCK 1      /* error reasons, OR-ed into error[1]: block type 3                                      */
+#define DFQ_PNG_BAD_CODESET 2    /* an invalid code-length, literal/length or distance code set                           */
+#define DFQ_PNG_BAD_CODE 4       /* an invalid literal/length or distance code                                            */
+#define DFQ_PNG_FAR 8            /* a distance past the start of the output                                               */
+#define DFQ_PNG_STORED_LEN 16    /* a stored block whose LEN and NLEN disagree                                            */
+#define DFQ_PNG_SHORT 32         /* the stream ends before the last row, not at a row's end with its whole trailer       */
+#define DFQ_PNG_BAD_FILTER 64    /* a scanline filter type above 4                                                        */
+#define DFQ_PNG_ADLER 128        /* the Adler-32 after the last row's final block differs                                 */
+/* Inflates each image's stream into its work room and unfilters the scanlines into its dst.  images: host array of d->n
+ * descriptors, uploaded by the call; blob: device pointer; error: device uint64 [2].  Past the image's last byte the
+ * stream is still decoded up to the first symbol that would write (block headers, code sets, end-of-block codes, a
+ * distance code after a length, the Adler-32 after the final block), as zlib does for Pillow.  A final block that ends
+ * at the end of an earlier row, followed by its whole and right Adler-32, leaves the rows not reached zero, as Pillow
+ * does.  A stream found corrupt
+ * stops that image, atomicMin's (call << 32 | image) into error[0] and OR's its reasons into error[1]; that image's
+ * output is then unspecified, and no read or write leaves its stream, its work room or its output.  The zlib header is
+ * not read: the caller checks it.  Does not synchronise.  DFQ_E_ARG, with a reason and before any launch: a NULL
+ * pointer, n out of range, an image below 1 x 1 or above 2^31 - 1 pixels, a stream shorter than its header, or a
+ * stream, work room or output outside the blob or overlapping one another. */
+int dfq_png_decode(const DfqPngDecode* d, const DfqPngImage* images, void* blob, uint64_t* error, void* stream);
 
 #ifdef __cplusplus
 }
