@@ -6,6 +6,7 @@ with C alignment, so whole tables are passed as one pointer).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -317,5 +318,42 @@ def require_cuda():
 
 
 def stream_ptr():
+    """The current device's current stream.  The package launches through launch(), which makes its tensors' device
+    current first; this raw form is for direct ABI calls made on the current device."""
     import torch
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _device_index(o) -> int:
+    """CUDA device index of a tensor or device; -1 for the CPU."""
+    import torch
+    if isinstance(o, torch.Tensor):
+        return o.get_device()
+    d = torch.device(o)
+    if d.type != "cuda":
+        return -1
+    return torch.cuda.current_device() if d.index is None else d.index
+
+
+@contextlib.contextmanager
+def launch(*on):
+    """The launch context of library calls: `with launch(x, y) as st:` makes the one CUDA device of `on` (tensors,
+    torch.devices or None, which are skipped) the current device and yields that device's current stream.  Every library
+    call of the package is made inside one, so a call follows its tensors as torch's own ops do: tensors on cuda:1 run on
+    cuda:1's current stream even when cuda:0 is current, the library's stream-ordered allocations come from cuda:1, and
+    its per-device host state (DESIGN.md, "Launch context") is cuda:1's.  Tensors on two devices raise DfqError naming
+    both, before anything is entered or launched.  CPU tensors enter no device: the entry points refuse them before their
+    library calls, except under the host-side twins the tests run them through."""
+    import torch
+    idx = []
+    for o in on:
+        if o is not None and _device_index(o) not in idx:
+            idx.append(_device_index(o))
+    if len(idx) != 1:
+        raise DfqError("a library call takes its tensors on one device, got %s"
+                       % (" and ".join("cpu" if i < 0 else "cuda:%d" % i for i in idx) if idx else "none"))
+    if idx[0] < 0:
+        yield stream_ptr()
+        return
+    with torch.cuda.device(idx[0]):
+        yield stream_ptr()

@@ -44,13 +44,15 @@ def _logits(x):
 
 def _run(logits, labels, pred, correct):
     N, C_ = logits.shape
-    _lib.check(_lib.load().dfq_cls_count(_ptr(logits), _ptr(labels), _ptr(pred), _ptr(correct), N, C_,
-                                         _lib.stream_ptr()), "dfq_cls_count")
+    with _lib.launch(logits, labels, pred, correct) as st:
+        _lib.check(_lib.load().dfq_cls_count(_ptr(logits), _ptr(labels), _ptr(pred), _ptr(correct), N, C_, st),
+                   "dfq_cls_count")
 
 
 def predict(logits) -> torch.Tensor:
     """int64 [N]: torch.max(logits, 1)[1] bit for bit (DESIGN.md section 4 has the rule for ties, NaN and -0.0).  logits:
-    contiguous fp32 [N, C] on the GPU.  Does not synchronise with the host."""
+    contiguous fp32 [N, C] on the GPU.  Runs on logits' device and its current stream, the result on that device, whichever
+    device is current.  Does not synchronise with the host."""
     logits = _logits(logits)
     pred = torch.empty(logits.shape[0], dtype=torch.int64, device=logits.device)
     _run(logits, None, pred, None)
@@ -60,7 +62,8 @@ def predict(logits) -> torch.Tensor:
 class Evaluator:
     """main_cls.py inference_all's count with the counting on the GPU.  add_logits counts a batch; num_correct, num_total
     and accuracy() are what the main's num_correct, num_total and acc hold after the same batches, with the same types.
-    The correct count is kept as int64 on the device of the first batch and never leaves it between batches."""
+    The correct count is kept as int64 on the device of the first batch and never leaves it between batches; add_logits
+    counts on that device's current stream, whichever device is current, and a batch on another device raises DfqError."""
 
     def __init__(self, num_classes):
         if not isinstance(num_classes, int) or isinstance(num_classes, bool) or not 1 <= num_classes <= MAX_CLASSES:

@@ -63,13 +63,21 @@ __global__ void __launch_bounds__(kMatchThreads) k_map_match(
     int64_t G, int N, int C, double iou_threshold, unsigned long long* __restrict__ claims, uint64_t* __restrict__ keys,
     uint8_t* __restrict__ flags, unsigned long long* __restrict__ gt_count, int* __restrict__ error) {
   const int n = blockIdx.x, tid = threadIdx.x;
-  const int64_t d0 = det_off[n], d1 = det_off[n + 1], g0 = gt_off[n], g1 = gt_off[n + 1];
-  const bool det_ok = 0 <= d0 && d0 <= d1 && d1 <= T && (n > 0 || d0 == 0) && (n < N - 1 || d1 == T);
-  const bool gt_ok = 0 <= g0 && g0 <= g1 && g1 <= G && (n > 0 || g0 == 0) && (n < N - 1 || g1 == G);
-  if (!det_ok || !gt_ok) {
-    if (tid == 0) atomicOr(error, (det_ok ? 0 : DFQ_MAP_ERR_DET_OFFSETS) | (gt_ok ? 0 : DFQ_MAP_ERR_GT_OFFSETS));
+  // Every CTA checks both offset arrays whole: from 0, non-decreasing, to T (G).  A CTA whose own pair looked right while
+  // an offset further on was out of order would take rows of other images, and two CTAs would race on the same rows (the
+  // second pass would then find another CTA's pending verdict without a box of its class).  Any fault stops the batch.
+  int bad = 0;
+  for (int i = tid; i <= N; i += blockDim.x) {
+    const int64_t d = det_off[i], g = gt_off[i];
+    if ((i == 0 && d != 0) || (i == N && d != T) || (i < N && d > det_off[i + 1])) bad |= DFQ_MAP_ERR_DET_OFFSETS;
+    if ((i == 0 && g != 0) || (i == N && g != G) || (i < N && g > gt_off[i + 1])) bad |= DFQ_MAP_ERR_GT_OFFSETS;
+  }
+  const int det_bad = __syncthreads_or(bad & DFQ_MAP_ERR_DET_OFFSETS), gt_bad = __syncthreads_or(bad & DFQ_MAP_ERR_GT_OFFSETS);
+  if (det_bad || gt_bad) {
+    if (tid == 0 && n == 0) atomicOr(error, (det_bad ? DFQ_MAP_ERR_DET_OFFSETS : 0) | (gt_bad ? DFQ_MAP_ERR_GT_OFFSETS : 0));
     return;
   }
+  const int64_t d0 = det_off[n], d1 = det_off[n + 1], g0 = gt_off[n], g1 = gt_off[n + 1];
   for (int64_t g = g0 + tid; g < g1; g += blockDim.x) {
     const int64_t l = gt_labels[g];
     if (l < 0 || l >= C) atomicOr(error, DFQ_MAP_ERR_GT_LABEL);
@@ -112,7 +120,7 @@ __global__ void __launch_bounds__(kMatchThreads) k_map_match(
     float m;
     const int64_t arg = best_gt(box, det_labels[t], gt_boxes, gt_labels, g0, g1, &m);
     const unsigned long long mine = ((unsigned long long)(keys[t] & 0xffffffffu) << 32) | (uint32_t)(t - d0);
-    flags[t] = claims[arg] == mine ? DFQ_MAP_TP : DFQ_MAP_FP;
+    flags[t] = arg >= 0 && claims[arg] == mine ? DFQ_MAP_TP : DFQ_MAP_FP;
   }
 }
 

@@ -5,6 +5,7 @@
 #include <cstring>
 #include <algorithm>
 #include <mutex>
+#include <unordered_map>
 
 #include <cooperative_groups.h>
 
@@ -43,10 +44,11 @@ int coop_grid(const void* kernel, const char* kernel_name, int threads, size_t d
 
 namespace {
 struct Slot { unsigned char* host = nullptr; unsigned char* dev = nullptr; size_t cap = 0; cudaEvent_t ev = nullptr; bool used = false; };
-Slot g_slots[4];
-int g_next_slot = 0;
+// One ring per device: a slot's event belongs to the device it was created on and is recorded on that device's streams
+// only, and each device's default pool is tuned once.
+struct SlotRing { Slot slots[4]; int next = 0; bool pool_tuned = false; };
+std::unordered_map<int, SlotRing> g_rings;
 std::mutex g_slot_mu;
-bool g_pool_tuned = false;
 }  // namespace
 
 // word-wise copy between device memory and mapped page-locked host memory (either direction), a few KB to a few hundred KB
@@ -112,32 +114,44 @@ void ReadBack::abandon() {
 int TablePack::upload(cudaStream_t st) {
   dev = nullptr;
   if (total == 0) return 0;
+  int d = 0;
+  DFQ_CUDA(cudaGetDevice(&d));
   std::lock_guard<std::mutex> lk(g_slot_mu);
-  if (!g_pool_tuned) {   // keep freed descriptor blocks in the default pool instead of returning them to the OS at every sync
-    int d = 0; cudaMemPool_t pool;
-    if (cudaGetDevice(&d) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, d) == cudaSuccess) {
+  SlotRing& ring = g_rings[d];
+  if (!ring.pool_tuned) {   // keep freed descriptor blocks in the default pool instead of returning them to the OS at every sync
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, d) == cudaSuccess) {
       unsigned long long thr = ~0ull;
       cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
     }
-    g_pool_tuned = true;
+    ring.pool_tuned = true;
   }
-  Slot& sl = g_slots[g_next_slot];
-  g_next_slot = (g_next_slot + 1) % 4;
+  Slot& sl = ring.slots[ring.next];
+  ring.next = (ring.next + 1) % 4;
   if (sl.used) DFQ_CUDA(cudaEventSynchronize(sl.ev));
+  sl.used = false;
   if (sl.cap < total) {
     if (sl.host) cudaFreeHost(sl.host);
-    sl.cap = std::max<size_t>(total, 1 << 20);
-    DFQ_CUDA(cudaHostAlloc((void**)&sl.host, sl.cap, cudaHostAllocMapped));
+    sl.host = nullptr; sl.cap = 0;
+    const size_t cap = std::max<size_t>(total, 1 << 20);
+    DFQ_CUDA(cudaHostAlloc((void**)&sl.host, cap, cudaHostAllocMapped));
     DFQ_CUDA(cudaHostGetDevicePointer((void**)&sl.dev, sl.host, 0));
+    sl.cap = cap;
   }
   if (!sl.ev) DFQ_CUDA(cudaEventCreateWithFlags(&sl.ev, cudaEventDisableTiming));
   for (int i = 0; i < n; ++i)
     if (items[i].bytes) memcpy(sl.host + items[i].off, items[i].src, items[i].bytes);
   DFQ_CUDA(cudaMallocAsync((void**)&dev, total, st));
-  { const int rc = launch_copy_words(dev, sl.dev, total, st); if (rc) return rc; }
-  DFQ_CUDA(cudaEventRecord(sl.ev, st));
-  sl.used = true;
-  return 0;
+  int rc = launch_copy_words(dev, sl.dev, total, st);
+  if (rc == 0) {
+    const cudaError_t e = cudaEventRecord(sl.ev, st);
+    if (e == cudaSuccess) { sl.used = true; return 0; }
+    rc = cuda_fail(e, "cudaEventRecord(sl.ev, st)");
+  }
+  // the copy may be in flight without an event to wait on: let it finish before the slot is reused, then free the block
+  cudaStreamSynchronize(st);
+  release(st);
+  return rc;
 }
 
 constexpr int kThreads = 256;

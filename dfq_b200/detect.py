@@ -80,11 +80,13 @@ def _descriptor(locations, priors, center_variance, size_variance, C_=2, prob_th
 def decode_boxes(locations, priors, center_variance, size_variance):
     """Corner-form boxes fp32 [N, P, 4] of SSD regression outputs: box_utils.center_form_to_corner_form(
     box_utils.convert_locations_to_boxes(locations, priors, center_variance, size_variance)) bit for bit with torch on CUDA.
-    locations fp32 [N, P, 4]; priors fp32 in centre form, [P, 4], [1, P, 4] or [N, P, 4]; the variances Python floats."""
+    locations fp32 [N, P, 4]; priors fp32 in centre form, [P, 4], [1, P, 4] or [N, P, 4]; the variances Python floats.
+    Runs on locations' device and its current stream, the boxes on that device, whichever device is current."""
     d, priors = _descriptor(locations, priors, center_variance, size_variance)
     boxes = torch.empty_like(locations)
-    _lib.check(_lib.load().dfq_ssd_decode(_ptr(locations), _ptr(priors), _ptr(boxes), _lib.table_ptr(d), _lib.stream_ptr()),
-               "dfq_ssd_decode")
+    with _lib.launch(locations) as st:
+        _lib.check(_lib.load().dfq_ssd_decode(_ptr(locations), _ptr(priors), _ptr(boxes), _lib.table_ptr(d), st),
+                   "dfq_ssd_decode")
     return boxes
 
 
@@ -135,6 +137,9 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
     when top_k > 0.  Every op is the reference's bit for bit except exp, which is torch's exp on a CUDA tensor (CUDA's
     expf) where the reference runs torch's CPU exp; DESIGN.md section 4 states the difference.  sigma is a finite
     positive number, taken as fp32.
+
+    Runs on scores' device and its current stream, the detections on that device, whichever device is current; the one
+    synchronisation waits for that stream only.
     """
     if nms_method not in (None, "hard", "soft"):
         raise _lib.DfqError("nms_method must be None, 'hard' or 'soft', got %r" % (nms_method,))
@@ -169,31 +174,34 @@ def postprocess(scores, locations, priors=None, center_variance=None, size_varia
             raise _lib.DfqError("image_sizes must be a real tensor [%d, 2] of (width, height) on the GPU, got %s"
                                 % (N, tuple(image_sizes.shape) if isinstance(image_sizes, torch.Tensor) else image_sizes))
         image_sizes = image_sizes.to(device=scores.device, dtype=torch.float32).contiguous()
-    lib, st, dp = _lib.load(), _lib.stream_ptr(), _lib.table_ptr(d)
-    dev = scores.device
+    lib, dp = _lib.load(), _lib.table_ptr(d)
     boxes = torch.empty_like(locations)
-    _lib.check(lib.dfq_ssd_decode(_ptr(locations), _ptr(priors), _ptr(boxes), dp, st), "dfq_ssd_decode")
+    with _lib.launch(scores) as st:
+        _lib.check(lib.dfq_ssd_decode(_ptr(locations), _ptr(priors), _ptr(boxes), dp, st), "dfq_ssd_decode")
     if nms_method == "soft":
-        return _soft(lib, st, dp, scores, boxes, image_sizes, N, C_, float(sigma))
+        return _soft(lib, dp, scores, boxes, image_sizes, N, C_, float(sigma))
+    dev = scores.device
     S, K = N * (C_ - 1), candidate_size
     slot_boxes = torch.empty(S, K, 4, dtype=torch.float32, device=dev)
     slot_probs = torch.empty(S, K, dtype=torch.float32, device=dev)
     counts = torch.empty(S, dtype=torch.int32, device=dev)
     seg_offsets = torch.empty(S + 1, dtype=torch.int64, device=dev)
-    _lib.check(lib.dfq_ssd_nms(_ptr(scores), _ptr(boxes), _ptr(slot_boxes), _ptr(slot_probs), _ptr(counts),
-                               _ptr(seg_offsets), dp, st), "dfq_ssd_nms")
+    with _lib.launch(dev) as st:
+        _lib.check(lib.dfq_ssd_nms(_ptr(scores), _ptr(boxes), _ptr(slot_boxes), _ptr(slot_probs), _ptr(counts),
+                                   _ptr(seg_offsets), dp, st), "dfq_ssd_nms")
     T = int(seg_offsets[-1])
     out_boxes = torch.empty(T, 4, dtype=torch.float32, device=dev)
     labels = torch.empty(T, dtype=torch.int64, device=dev)
     probs = torch.empty(T, dtype=torch.float32, device=dev)
     if T:
-        _lib.check(lib.dfq_ssd_compact(_ptr(slot_boxes), _ptr(slot_probs), _ptr(counts), _ptr(seg_offsets),
-                                       _ptr(image_sizes), _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, st),
-                   "dfq_ssd_compact")
+        with _lib.launch(dev) as st:
+            _lib.check(lib.dfq_ssd_compact(_ptr(slot_boxes), _ptr(slot_probs), _ptr(counts), _ptr(seg_offsets),
+                                           _ptr(image_sizes), _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, st),
+                       "dfq_ssd_compact")
     return Detections(out_boxes, labels, probs, seg_offsets[::C_ - 1])
 
 
-def _soft(lib, st, dp, scores, boxes, image_sizes, N, C_, sigma):
+def _soft(lib, dp, scores, boxes, image_sizes, N, C_, sigma):
     """The soft NMS half of postprocess: pick counts and their scan, the one synchronisation for the total, then the
     picks written straight to their rows (the kernel runs the same steps twice, so nothing is kept per candidate)."""
     dev = scores.device
@@ -201,16 +209,18 @@ def _soft(lib, st, dp, scores, boxes, image_sizes, N, C_, sigma):
     work = torch.empty(2 * S, dtype=torch.int32, device=dev)          # candidate counts, pick counts
     cands, counts = work[:S], work[S:]
     seg_offsets = torch.empty(S + 1, dtype=torch.int64, device=dev)
-    _lib.check(lib.dfq_ssd_soft_nms(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(counts), _ptr(seg_offsets), dp, sigma,
-                                    st), "dfq_ssd_soft_nms")
+    with _lib.launch(dev) as st:
+        _lib.check(lib.dfq_ssd_soft_nms(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(counts), _ptr(seg_offsets), dp, sigma,
+                                        st), "dfq_ssd_soft_nms")
     T = int(seg_offsets[-1])
     out_boxes = torch.empty(T, 4, dtype=torch.float32, device=dev)
     labels = torch.empty(T, dtype=torch.int64, device=dev)
     probs = torch.empty(T, dtype=torch.float32, device=dev)
     if T:
-        _lib.check(lib.dfq_ssd_soft_compact(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(seg_offsets), _ptr(image_sizes),
-                                            _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, sigma, st),
-                   "dfq_ssd_soft_compact")
+        with _lib.launch(dev) as st:
+            _lib.check(lib.dfq_ssd_soft_compact(_ptr(scores), _ptr(boxes), _ptr(cands), _ptr(seg_offsets),
+                                                _ptr(image_sizes), _ptr(out_boxes), _ptr(labels), _ptr(probs), dp, sigma,
+                                                st), "dfq_ssd_soft_compact")
     return Detections(out_boxes, labels, probs, seg_offsets[::C_ - 1])
 
 
@@ -296,7 +306,8 @@ class Evaluator:
     the device, without synchronising with the host.  average_precision() sorts everything added and reads back the
     compact per-class results once.  The one intended difference from the reference: detections of equal score are taken
     in the order they were added (images in order, then row order within an image), where the reference's sort is not
-    stable.  The accumulators live on the device of the first batch."""
+    stable.  The accumulators live on the device of the first batch; add_batch and average_precision() run on that
+    device's current stream, whichever device is current, and a batch on another device raises DfqError."""
 
     def __init__(self, num_classes=21, iou_threshold=0.5, use_2007_metric=True):
         if not isinstance(num_classes, int) or isinstance(num_classes, bool) or not 2 <= num_classes <= MAX_MAP_CLASSES:
@@ -365,11 +376,12 @@ class Evaluator:
             self._error = torch.zeros(1, dtype=torch.int32, device=dev)
         self._reserve(self._count + T)
         lib = _lib.load()
-        _lib.check(lib.dfq_map_match(
-            _ptr(d_boxes), _ptr(d_labels), _ptr(d_probs), _ptr(d_offs), T, _ptr(g_boxes), _ptr(g_labels), _ptr(g_diff),
-            _ptr(g_offs), G, N, self.num_classes, self.iou_threshold,
-            C.c_void_p(self._keys.data_ptr() + 8 * self._count), C.c_void_p(self._flags.data_ptr() + self._count),
-            _ptr(self._gt_count), _ptr(self._error), _lib.stream_ptr()), "dfq_map_match")
+        with _lib.launch(dev) as st:
+            _lib.check(lib.dfq_map_match(
+                _ptr(d_boxes), _ptr(d_labels), _ptr(d_probs), _ptr(d_offs), T, _ptr(g_boxes), _ptr(g_labels), _ptr(g_diff),
+                _ptr(g_offs), G, N, self.num_classes, self.iou_threshold,
+                C.c_void_p(self._keys.data_ptr() + 8 * self._count), C.c_void_p(self._flags.data_ptr() + self._count),
+                _ptr(self._gt_count), _ptr(self._error), st), "dfq_map_match")
         self._count += T
         self._gt_total += G
 
@@ -449,9 +461,10 @@ class Evaluator:
         counts = buf[8 + 8 * Cn:8 + 16 * Cn].view(torch.int64)
         out = buf[8 + 16 * Cn:].view(torch.float64)
         D = self._count
-        _lib.check(_lib.load().dfq_map_curve(
-            _ptr(self._keys) if D else None, _ptr(self._flags) if D else None, D, Cn, _ptr(self._gt_count),
-            int(self.use_2007_metric), _ptr(out), n_out, _ptr(counts), _lib.stream_ptr()), "dfq_map_curve")
+        with _lib.launch(self.device) as st:
+            _lib.check(_lib.load().dfq_map_curve(
+                _ptr(self._keys) if D else None, _ptr(self._flags) if D else None, D, Cn, _ptr(self._gt_count),
+                int(self.use_2007_metric), _ptr(out), n_out, _ptr(counts), st), "dfq_map_curve")
         buf[:4].copy_(self._error.view(torch.uint8))
         buf[8:8 + 8 * Cn].copy_(self._gt_count.view(torch.uint8))
         host = buf.cpu().numpy()

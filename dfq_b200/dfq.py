@@ -47,8 +47,9 @@ def _quantize_error(param, num_bits=8, reduction='sum', signed=False):
         if src.is_cuda:
             eps = _Q.fake_quant_device_range(dev, num_bits, mm[0:1], mm[1:2], signed, prologue=0, div_mode=1) - dev
         else:
-            _lib.check(lib.dfq_quant_error(_ptr(dev), _ptr(eps), dev.numel(), _ptr(mm), int(num_bits), 1 if signed else 0,
-                                           _lib.stream_ptr()), "dfq_quant_error")
+            with _lib.launch(dev) as st:
+                _lib.check(lib.dfq_quant_error(_ptr(dev), _ptr(eps), dev.numel(), _ptr(mm), int(num_bits), 1 if signed else 0,
+                                               st), "dfq_quant_error")
         if reduction == 'sum':
             eps = torch.sum(torch.abs(eps))
         elif reduction == 'mean':
@@ -159,8 +160,9 @@ def _equalize_any_order(sess, table, s_range, converge_thres, converge_count, si
         diff_tmp = 0.0
         for l in layers:
             cur = sess.view(sess.layer(l)["w_off"], prev[l].numel())
-            _lib.check(lib.dfq_mean_abs_diff(_ptr(cur), _ptr(prev[l]), prev[l].numel(), C.c_void_p(out.data_ptr()),
-                                             _lib.stream_ptr()), "dfq_mean_abs_diff")
+            with _lib.launch(cur) as st:
+                _lib.check(lib.dfq_mean_abs_diff(_ptr(cur), _ptr(prev[l]), prev[l].numel(), C.c_void_p(out.data_ptr()),
+                                                 st), "dfq_mean_abs_diff")
             diff_tmp += float(out.item())
         diffs.append(diff_tmp)
         n += 1
@@ -223,8 +225,9 @@ def clip_weight(graph, range_clip=[-15, 15], targ_type=[nn.Conv2d, nn.Linear]):
             dev, _ = _Q._dev_f32(w)
             if dev.data_ptr() == w.data_ptr():
                 dev = dev.clone()
-            _lib.check(lib.dfq_clamp(_ptr(dev), dev.numel(), float(range_clip[0]), float(range_clip[1]), _lib.stream_ptr()),
-                       "dfq_clamp")
+            with _lib.launch(dev) as st:
+                _lib.check(lib.dfq_clamp(_ptr(dev), dev.numel(), float(range_clip[0]), float(range_clip[1]), st),
+                           "dfq_clamp")
             w.copy_(dev.view(w.shape))
 
 

@@ -52,8 +52,9 @@ class _BNStatLoss(torch.autograd.Function):
         hw = xc.numel() // (n * c)
         m = xc.new_empty((n * c,)); s = xc.new_empty((n * c,))
         loss = xc.new_empty((2,), dtype=torch.float64)
-        _lib.check(lib.dfq_bnstat_loss_fwd(_ptr(xc), n, c, hw, _ptr(bn_mean), _ptr(bn_std), C.c_float(eps), _ptr(m), _ptr(s),
-                                           _ptr(loss), _lib.stream_ptr()), "dfq_bnstat_loss_fwd")
+        with _lib.launch(xc) as st:
+            _lib.check(lib.dfq_bnstat_loss_fwd(_ptr(xc), n, c, hw, _ptr(bn_mean), _ptr(bn_std), C.c_float(eps), _ptr(m), _ptr(s),
+                                               _ptr(loss), st), "dfq_bnstat_loss_fwd")
         ctx.save_for_backward(xc, bn_mean, bn_std, m, s)
         ctx.eps = eps
         return loss.float()
@@ -66,8 +67,9 @@ class _BNStatLoss(torch.autograd.Function):
         hw = xc.numel() // (n * c)
         gx = torch.empty_like(xc)
         g2 = grad.detach().float().contiguous()
-        _lib.check(lib.dfq_bnstat_loss_bwd(_ptr(xc), _ptr(gx), n, c, hw, _ptr(bn_mean), _ptr(bn_std), C.c_float(ctx.eps), _ptr(m),
-                                           _ptr(s), _ptr(g2), 0, _lib.stream_ptr()), "dfq_bnstat_loss_bwd")
+        with _lib.launch(xc) as st:
+            _lib.check(lib.dfq_bnstat_loss_bwd(_ptr(xc), _ptr(gx), n, c, hw, _ptr(bn_mean), _ptr(bn_std), C.c_float(ctx.eps), _ptr(m),
+                                               _ptr(s), _ptr(g2), 0, st), "dfq_bnstat_loss_bwd")
         return gx, None, None, None
 
 

@@ -261,7 +261,7 @@ class Session:
         with torch.no_grad():
             if x["d2h_runs"]:
                 if self.arena.is_cuda:
-                    torch.cuda.current_stream().synchronize()
+                    torch.cuda.current_stream(self.arena.device).synchronize()
                 dst, src = [], []
                 for b, v in (() if self._host_copy(x, "d2h", 1) else zip(x["d2h_bounds"], x["d2h_src"])):
                     t = b.tensor.detach()
@@ -381,8 +381,9 @@ class Session:
         self._ensure_room()
         self.finish_fold()
         ft, lt = plan["ft"], plan["lt"]
-        _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
-                                        _lib.table_ptr(ft), len(ft), _lib.stream_ptr()), "dfq_bn_fold")
+        with _lib.launch(self.arena) as st:
+            _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
+                                            _lib.table_ptr(ft), len(ft), st), "dfq_bn_fold")
         if plan.get("deferred"):
             self._pending = plan
 
@@ -403,8 +404,9 @@ class Session:
         for k, (li, fac_off) in enumerate(plan["deferred"]):
             ft[k]["layer"] = li; ft[k]["mode"] = _lib.FOLD_APPLY; ft[k]["fac_off"] = fac_off
         lt = plan["lt"]
-        _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
-                                        _lib.table_ptr(ft), len(ft), _lib.stream_ptr()), "dfq_bn_fold")
+        with _lib.launch(self.arena) as st:
+            _lib.check(self.lib.dfq_bn_fold(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
+                                            _lib.table_ptr(ft), len(ft), st), "dfq_bn_fold")
 
     # ---- cross-layer equalization -----------------------------------------------------------------
     def plan_cle(self, relations: Sequence[Tuple[int, int, int, int]], groups: Optional[Sequence[int]] = None) -> dict:
@@ -533,10 +535,12 @@ class Session:
                 _lib.table_ptr(plan["step_ptr"]), _lib.table_ptr(plan["step_layers"]), plan["n_steps"], _lib.table_ptr(P),
                 _lib.table_ptr(R), plan["n_groups"], _lib.table_ptr(gs))
         if att is not None:
-            _lib.check(run_bc(*args, _lib.table_ptr(att["plan"]["bt"]), len(att["plan"]["bt"]), _lib.table_ptr(att["plan"]["tt"]),
-                              att["plan"]["n_terms"], int(att["num_bits"]), _lib.stream_ptr()), "dfq_cle_run_bc")
+            with _lib.launch(self.arena) as st:
+                _lib.check(run_bc(*args, _lib.table_ptr(att["plan"]["bt"]), len(att["plan"]["bt"]), _lib.table_ptr(att["plan"]["tt"]),
+                                  att["plan"]["n_terms"], int(att["num_bits"]), st), "dfq_cle_run_bc")
         else:
-            _lib.check(self.lib.dfq_cle_run(*args, _lib.stream_ptr()), "dfq_cle_run")
+            with _lib.launch(self.arena) as st:
+                _lib.check(self.lib.dfq_cle_run(*args, st), "dfq_cle_run")
         if pending is not None:
             self._pending = None
         n = int(R[0]["n_sweeps"])
@@ -653,10 +657,11 @@ class Session:
             bt["flags"] |= _lib.BC_PREPARED
         else:
             bt = self._with_col_hints(lt, bt, col_hints)
-        _lib.check(self.lib.dfq_bias_correct(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
-                                             _lib.table_ptr(bt), len(bt), _lib.table_ptr(tt), plan["n_terms"],
-                                             _lib.table_ptr(plan["level_ptr"]), plan["n_levels"], int(num_bits),
-                                             _lib.stream_ptr()), "dfq_bias_correct")
+        with _lib.launch(self.arena) as st:
+            _lib.check(self.lib.dfq_bias_correct(self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt),
+                                                 _lib.table_ptr(bt), len(bt), _lib.table_ptr(tt), plan["n_terms"],
+                                                 _lib.table_ptr(plan["level_ptr"]), plan["n_levels"], int(num_bits),
+                                                 st), "dfq_bias_correct")
 
     @staticmethod
     def _with_col_hints(lt: np.ndarray, bt: np.ndarray, col_hints: Optional[Dict[str, np.ndarray]]) -> np.ndarray:
@@ -701,10 +706,11 @@ class Session:
             bt, tt, n_terms = np.zeros(1, dtype=_lib.BC_LAYER_DT), np.zeros(1, dtype=_lib.TERM_DT), 0
             lp, n_levels = np.zeros(1, dtype=np.int32), 0
         lo, hi = (float(clip[0]), float(clip[1])) if clip is not None else (0.0, 0.0)
-        _lib.check(self.lib.dfq_bias_correct_absorb_clip(
-            self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt), _lib.table_ptr(bt), len(plan["bt"]) if plan else 0,
-            _lib.table_ptr(tt), n_terms, _lib.table_ptr(lp), n_levels, int(num_bits), _lib.table_ptr(at), n_abs,
-            float(absorb_n), 1 if clip is not None else 0, lo, hi, _lib.stream_ptr()), "dfq_bias_correct_absorb_clip")
+        with _lib.launch(self.arena) as st:
+            _lib.check(self.lib.dfq_bias_correct_absorb_clip(
+                self._ptr(), self.arena.numel(), _lib.table_ptr(lt), len(lt), _lib.table_ptr(bt), len(plan["bt"]) if plan else 0,
+                _lib.table_ptr(tt), n_terms, _lib.table_ptr(lp), n_levels, int(num_bits), _lib.table_ptr(at), n_abs,
+                float(absorb_n), 1 if clip is not None else 0, lo, hi, st), "dfq_bias_correct_absorb_clip")
 
     def run_bias_correct(self, items: Sequence[dict], num_bits: int = 8):
         """plan + run; returns the list of delta offsets ([rows] each), in the order of `items`."""
@@ -734,5 +740,6 @@ class Session:
             qt = self.plan_quantize(tasks)["qt"]
         self._ensure_room()
         self.finish_fold()
-        _lib.check(self.lib.dfq_quantize_tensors(self._ptr(), self.arena.numel(), _lib.table_ptr(qt), len(qt),
-                                                 int(div_mode), _lib.stream_ptr()), "dfq_quantize_tensors")
+        with _lib.launch(self.arena) as st:
+            _lib.check(self.lib.dfq_quantize_tensors(self._ptr(), self.arena.numel(), _lib.table_ptr(qt), len(qt),
+                                                     int(div_mode), st), "dfq_quantize_tensors")

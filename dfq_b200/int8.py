@@ -264,21 +264,24 @@ class _Int8Layer(_ConvLayer):
         lib = _lib.load()
         if weight.dtype == torch.int8:                          # codes, packed verbatim (Int8Conv2d.from_codes)
             w = weight.detach().to(dev).contiguous()
-            _lib.check(lib.dfq_i8_pack_codes(_ptr(w), _ptr(self.weight_codes), _lib.table_ptr(self._pack_geometry()),
-                                             _lib.stream_ptr()), "dfq_i8_pack_codes")
+            with _lib.launch(w, self.weight_codes) as st:
+                _lib.check(lib.dfq_i8_pack_codes(_ptr(w), _ptr(self.weight_codes), _lib.table_ptr(self._pack_geometry()),
+                                                 st), "dfq_i8_pack_codes")
             return
         w = weight.detach().float().to(dev).contiguous()
-        _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes),
-                                           _lib.table_ptr(self._pack_geometry()), _lib.stream_ptr()), "dfq_i8_pack_weights")
+        with _lib.launch(w, self.weight_codes) as st:
+            _lib.check(lib.dfq_i8_pack_weights(_ptr(w), _ptr(self.w_scale), _ptr(self.weight_codes),
+                                               _lib.table_ptr(self._pack_geometry()), st), "dfq_i8_pack_weights")
 
     def unpack_codes(self):
         """The int8 weight codes [O, C/groups, kh, kw] of the packed layer (dfq_i8_unpack_codes), on its device."""
         kh, kw = self.kernel_size
         codes = torch.empty((self.out_channels, self.in_channels // self.groups, kh, kw), dtype=torch.int8,
                             device=self.weight_codes.device)
-        _lib.check(_lib.load().dfq_i8_unpack_codes(_ptr(self.weight_codes), _ptr(codes),
-                                                   _lib.table_ptr(self._pack_geometry()), _lib.stream_ptr()),
-                   "dfq_i8_unpack_codes (layer %s)" % self._who())
+        with _lib.launch(self.weight_codes, codes) as st:
+            _lib.check(_lib.load().dfq_i8_unpack_codes(_ptr(self.weight_codes), _ptr(codes),
+                                                       _lib.table_ptr(self._pack_geometry()), st),
+                       "dfq_i8_unpack_codes (layer %s)" % self._who())
         return codes
 
     def chained(self, codes_in=False, requant=None, epilogue=None, name=None, out_slice=None, rows=False, sums=False):
@@ -334,6 +337,9 @@ class _Int8Layer(_ConvLayer):
         if not x.is_cuda or not self.dq.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.dq.device))
+        if x.device != self.dq.device:
+            raise _lib.DfqError("layer %s is on %s, its input on %s: an int8 layer runs on its own device"
+                                % (self._who(), self.dq.device, x.device))
         if self.codes_in:
             if x.dtype != torch.int8 or x.dim() != 4 or x.shape[3] != self.cpad:
                 raise _lib.DfqError("chained int8 layer expects int8 codes [N, H, W, %d], got %s %s"
@@ -348,13 +354,14 @@ class _Int8Layer(_ConvLayer):
         self._check_residual(residual)
         x = x.contiguous()
         g, OH, OW = self._output_geometry(N, H, W)
-        lib, st = _lib.load(), _lib.stream_ptr()
+        lib = _lib.load()
         if self.codes_in:
             xq = x
         else:
             xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
-            _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, self.in_channels, H, W, self.cpad,
-                                                C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
+            with _lib.launch(x, self.dq) as st:
+                _lib.check(lib.dfq_i8_quantize_nhwc(_ptr(x), _ptr(xq), N, self.in_channels, H, W, self.cpad,
+                                                    C.c_float(self.act_scale), st), "dfq_i8_quantize_nhwc")
         if self.rows:
             return self._run_rows(xq, out, off, g, N, OH, OW), None
         if self.epilogue is not None:
@@ -365,14 +372,16 @@ class _Int8Layer(_ConvLayer):
         if self.requant is not None:
             s, lo, hi = self.requant
             yq = torch.empty((N, OH, OW, (self.out_channels + 15) // 16 * 16), dtype=torch.int8, device=x.device)
-            _lib.check(lib.dfq_i8_conv_requant(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(yq),
-                                               C.c_float(s), C.c_float(lo), C.c_float(hi), _lib.table_ptr(g), st),
-                       "dfq_i8_conv_requant")
+            with _lib.launch(xq, self.weight_codes) as st:
+                _lib.check(lib.dfq_i8_conv_requant(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(yq),
+                                                   C.c_float(s), C.c_float(lo), C.c_float(hi), _lib.table_ptr(g), st),
+                           "dfq_i8_conv_requant")
             return yq, None
         y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=x.device)
         acc = torch.empty(y.shape, dtype=torch.int32, device=x.device) if with_acc else None
-        _lib.check(lib.dfq_i8_conv(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(y), _ptr(acc),
-                                   _lib.table_ptr(g), st), "dfq_i8_conv")
+        with _lib.launch(xq, self.weight_codes) as st:
+            _lib.check(lib.dfq_i8_conv(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias), _ptr(y), _ptr(acc),
+                                       _lib.table_ptr(g), st), "dfq_i8_conv")
         return y, acc
 
     def _run_slice(self, xq, out, g, N, OH, OW):
@@ -387,9 +396,10 @@ class _Int8Layer(_ConvLayer):
                 if isinstance(out, torch.Tensor) else type(out).__name__))
         d = np.zeros(1, _lib.I8_EPILOGUE_DT)
         d[0] = (0, 0, out.data_ptr(), s, lo, hi, -_INF, _INF)
-        _lib.check(_lib.load().dfq_i8_conv_slice(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
-                                                 _lib.table_ptr(d), coff, cstride, _lib.table_ptr(g), _lib.stream_ptr()),
-                   "dfq_i8_conv_slice (layer %s)" % self._who())
+        with _lib.launch(xq, self.weight_codes, out) as st:
+            _lib.check(_lib.load().dfq_i8_conv_slice(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                                     _lib.table_ptr(d), coff, cstride, _lib.table_ptr(g), st),
+                       "dfq_i8_conv_slice (layer %s)" % self._who())
         return out
 
     def _run_rows(self, xq, out, off, g, N, OH, OW):
@@ -397,9 +407,10 @@ class _Int8Layer(_ConvLayer):
         out, off = self._rows_out(out, off, N, OH, OW, xq.device)
         d = np.zeros(1, _lib.I8_EPILOGUE_DT)
         d[0] = (0, out.data_ptr(), 0, 0.0) + e.pre + e.post
-        _lib.check(_lib.load().dfq_i8_conv_nhwc(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
-                                                _lib.table_ptr(d), int(off), out[0].numel(), _lib.table_ptr(g),
-                                                _lib.stream_ptr()), "dfq_i8_conv_nhwc (layer %s)" % self._who())
+        with _lib.launch(xq, self.weight_codes, out) as st:
+            _lib.check(_lib.load().dfq_i8_conv_nhwc(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                                    _lib.table_ptr(d), int(off), out[0].numel(), _lib.table_ptr(g),
+                                                    st), "dfq_i8_conv_nhwc (layer %s)" % self._who())
         return out
 
     def _run_fused(self, xq, r, g, N, OH, OW):
@@ -413,9 +424,10 @@ class _Int8Layer(_ConvLayer):
         d[0] = (0 if r is None else r.data_ptr(), 0 if y is None else y.data_ptr(), 0 if yq is None else yq.data_ptr(),
                 0.0 if e.out_scale is None else e.out_scale) + e.pre + e.post
         lib = _lib.load()
-        _lib.check(lib.dfq_i8_conv_fused(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
-                                         _lib.table_ptr(d), _lib.table_ptr(g), _lib.stream_ptr()),
-                   "dfq_i8_conv_fused (layer %s)" % self._who())
+        with _lib.launch(xq, self.weight_codes, r, y, yq) as st:
+            _lib.check(lib.dfq_i8_conv_fused(_ptr(xq), _ptr(self.weight_codes), _ptr(self.dq), _ptr(self.bias),
+                                             _lib.table_ptr(d), _lib.table_ptr(g), st),
+                       "dfq_i8_conv_fused (layer %s)" % self._who())
         return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
 
 
@@ -557,13 +569,14 @@ class _AffineInt8Layer(_ConvLayer):
     def _pack(self, w, mw, mx):
         """Pack the codes at the first candidate scale whose round trip reproduces every weight; returns it."""
         g = self._pack_geometry()
-        lib, st = _lib.load(), _lib.stream_ptr()
+        lib = _lib.load()
         n_bad = torch.zeros(1, dtype=torch.int32, device=w.device)
         fewest = None
         for fw in weight_grid_candidates(mw, mx, self.w_bits):
-            _lib.check(lib.dfq_i8_affine_pack(_ptr(w), C.c_float(mw), C.c_float(fw), self.w_bits, _ptr(self.weight_codes),
-                                              _ptr(self.tap_table) if self.tap_table.numel() else None, _ptr(n_bad),
-                                              _lib.table_ptr(g), st), "dfq_i8_affine_pack (layer %s)" % self._who())
+            with _lib.launch(w, self.weight_codes) as st:
+                _lib.check(lib.dfq_i8_affine_pack(_ptr(w), C.c_float(mw), C.c_float(fw), self.w_bits, _ptr(self.weight_codes),
+                                                  _ptr(self.tap_table) if self.tap_table.numel() else None, _ptr(n_bad),
+                                                  _lib.table_ptr(g), st), "dfq_i8_affine_pack (layer %s)" % self._who())
             bad = int(n_bad.item())
             if bad == 0:
                 return fw
@@ -649,7 +662,7 @@ class _AffineInt8Layer(_ConvLayer):
 
     def _input(self, x):
         """(codes, S | None, N, H, W) of the input: quantized here from fp32, or the pair a codes_in layer takes."""
-        lib, st = _lib.load(), _lib.stream_ptr()
+        lib = _lib.load()
         if self.codes_in:
             xq, S = x if isinstance(x, tuple) and len(x) == 2 else (x, None)
             if not isinstance(xq, torch.Tensor) or xq.dtype != torch.int8 or xq.dim() != 4 or xq.shape[3] != self.cpad:
@@ -662,6 +675,7 @@ class _AffineInt8Layer(_ConvLayer):
                                     % (self._who(), N, H, W))
             if not xq.is_cuda:
                 raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s" % xq.device)
+            self._same_device(xq)
             return xq.contiguous(), None if S is None else S.contiguous(), N, H, W
         if not isinstance(x, torch.Tensor) or x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != self.in_channels:
             raise _lib.DfqError("int8 layer expects fp32 [N, %d, H, W], got %s" % (
@@ -669,14 +683,21 @@ class _AffineInt8Layer(_ConvLayer):
         if not x.is_cuda or not self.bias.is_cuda:
             raise _lib.DfqError("int8 layers run on the GPU only (no CPU fallback): input on %s, layer on %s"
                                 % (x.device, self.bias.device))
+        self._same_device(x)
         x = x.contiguous()
         N, _, H, W = x.shape
         xq = torch.empty(N * H * W * self.cpad, dtype=torch.int8, device=x.device)
         S = torch.empty(N * H * W, dtype=torch.int32, device=x.device)
-        _lib.check(lib.dfq_i8_affine_quantize(_ptr(x), _ptr(xq), _ptr(S), N, self.in_channels, H, W, self.cpad,
-                                              C.c_float(self.act_min), C.c_float(self.act_max), self.act_bits, st),
-                   "dfq_i8_affine_quantize (layer %s)" % self._who())
+        with _lib.launch(x, self.bias) as st:
+            _lib.check(lib.dfq_i8_affine_quantize(_ptr(x), _ptr(xq), _ptr(S), N, self.in_channels, H, W, self.cpad,
+                                                  C.c_float(self.act_min), C.c_float(self.act_max), self.act_bits, st),
+                       "dfq_i8_affine_quantize (layer %s)" % self._who())
         return xq, S, N, H, W
+
+    def _same_device(self, x):
+        if x.device != self.bias.device:
+            raise _lib.DfqError("layer %s is on %s, its input on %s: an int8 layer runs on its own device"
+                                % (self._who(), self.bias.device, x.device))
 
     def run(self, x, with_acc=False, residual=None, out=None, off=0):
         """(y, P | None) for x fp32 [N, C, H, W] on the GPU; P = the int32 sums of the shifted codes.  In the chained modes
@@ -696,13 +717,14 @@ class _AffineInt8Layer(_ConvLayer):
             return self._run_rows(xq, S, out, off, g, N, OH, OW), None
         if self.epilogue is not None or self.pad_code is not None:
             return self._run_fused(xq, S, residual, g, N, OH, OW, out), None
-        lib, st = _lib.load(), _lib.stream_ptr()
+        lib = _lib.load()
         y = torch.empty((N, self.out_channels, OH, OW), dtype=torch.float32, device=xq.device)
         acc = torch.empty(y.shape, dtype=torch.int32, device=xq.device) if with_acc else None
-        _lib.check(lib.dfq_i8_affine_conv(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
-                                          _ptr(self.tap_table) if self.tap_table.numel() else None,
-                                          _lib.table_ptr(self.constants), _ptr(self.bias), _ptr(y), _ptr(acc),
-                                          _lib.table_ptr(g), st), "dfq_i8_affine_conv (layer %s)" % self._who())
+        with _lib.launch(xq, self.weight_codes) as st:
+            _lib.check(lib.dfq_i8_affine_conv(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                              _ptr(self.tap_table) if self.tap_table.numel() else None,
+                                              _lib.table_ptr(self.constants), _ptr(self.bias), _ptr(y), _ptr(acc),
+                                              _lib.table_ptr(g), st), "dfq_i8_affine_conv (layer %s)" % self._who())
         return y, acc
 
     def _run_fused(self, xq, S, r, g, N, OH, OW, out=None):
@@ -731,19 +753,22 @@ class _AffineInt8Layer(_ConvLayer):
             lay = np.zeros(1, _lib.I8_AFFINE_LAYOUT_DT)
             lay[0] = (self.out_slice or (0, (self.out_channels + 15) // 16 * 16)) + (
                 int(self.out_slice is not None), int(self.pad_code is not None), self.pad_code or 0)
-            _lib.check(lib.dfq_i8_affine_conv_layout(*args, None if o is None else _lib.table_ptr(o), _lib.table_ptr(lay),
-                                                     _lib.table_ptr(g), _lib.stream_ptr()),
-                       "dfq_i8_affine_conv_layout (layer %s)" % self._who())
+            with _lib.launch(xq, self.weight_codes, r, y, yq, S_out) as st:
+                _lib.check(lib.dfq_i8_affine_conv_layout(*args, None if o is None else _lib.table_ptr(o), _lib.table_ptr(lay),
+                                                         _lib.table_ptr(g), st),
+                           "dfq_i8_affine_conv_layout (layer %s)" % self._who())
             if self.out_slice is not None:
                 return yq, S_out
         elif obs is None and res is None:
-            _lib.check(lib.dfq_i8_affine_conv_fused(*args, _lib.table_ptr(g), _lib.stream_ptr()),
-                       "dfq_i8_affine_conv_fused (layer %s)" % self._who())
+            with _lib.launch(xq, self.weight_codes, r, y, yq, S_out) as st:
+                _lib.check(lib.dfq_i8_affine_conv_fused(*args, _lib.table_ptr(g), st),
+                           "dfq_i8_affine_conv_fused (layer %s)" % self._who())
         else:
             o = np.zeros(1, _lib.I8_AFFINE_OBSERVE_DT)
             o[0] = (obs or (0.0, 0.0, 0)) + (res or (0.0, 0.0, 0))
-            _lib.check(lib.dfq_i8_affine_conv_observed(*args, _lib.table_ptr(o), _lib.table_ptr(g), _lib.stream_ptr()),
-                       "dfq_i8_affine_conv_observed (layer %s)" % self._who())
+            with _lib.launch(xq, self.weight_codes, r, y, yq, S_out) as st:
+                _lib.check(lib.dfq_i8_affine_conv_observed(*args, _lib.table_ptr(o), _lib.table_ptr(g), st),
+                           "dfq_i8_affine_conv_observed (layer %s)" % self._who())
         codes = None if yq is None else (yq, S_out)
         return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
 
@@ -752,11 +777,12 @@ class _AffineInt8Layer(_ConvLayer):
         e, (obs, _), tail = self.epilogue, self.observers, self.tail_observer
         r = np.zeros(1, _lib.I8_AFFINE_ROWS_DT)
         r[0] = (out.data_ptr(), int(off), out[0].numel()) + e.pre + e.post + (obs or (0.0, 0.0, 0)) + (tail or (0.0, 0.0, 0))
-        _lib.check(_lib.load().dfq_i8_affine_conv_rows(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
-                                                       _ptr(self.tap_table) if self.tap_table.numel() else None,
-                                                       _lib.table_ptr(self.constants), _ptr(self.bias), _lib.table_ptr(r),
-                                                       _lib.table_ptr(g), _lib.stream_ptr()),
-                   "dfq_i8_affine_conv_rows (layer %s)" % self._who())
+        with _lib.launch(xq, self.weight_codes, out) as st:
+            _lib.check(_lib.load().dfq_i8_affine_conv_rows(_ptr(xq), _ptr(S), _ptr(self.weight_codes),
+                                                           _ptr(self.tap_table) if self.tap_table.numel() else None,
+                                                           _lib.table_ptr(self.constants), _ptr(self.bias), _lib.table_ptr(r),
+                                                           _lib.table_ptr(g), st),
+                       "dfq_i8_affine_conv_rows (layer %s)" % self._who())
         return out
 
     def _slice_buffers(self, out, N, OH, OW, dev):
@@ -893,9 +919,10 @@ class Int8MaxPool2d(nn.Module):
 
     def forward(self, x):
         x, g, y, yq = self._launch_args(x)
-        _lib.check(_lib.load().dfq_i8_maxpool(_ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y),
-                                              _ptr(yq), C.c_float(self.out_scale or 0.0), _lib.table_ptr(g),
-                                              _lib.stream_ptr()), "dfq_i8_maxpool (%s)" % self.layer_name)
+        with _lib.launch(x) as st:
+            _lib.check(_lib.load().dfq_i8_maxpool(_ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y),
+                                                  _ptr(yq), C.c_float(self.out_scale or 0.0), _lib.table_ptr(g),
+                                                  st), "dfq_i8_maxpool (%s)" % self.layer_name)
         return (yq, y) if yq is not None and y is not None else (y if yq is None else yq)
 
     def _launch_args(self, x):
@@ -951,9 +978,10 @@ class AffineInt8MaxPool2d(Int8MaxPool2d):
         x, g, y, yq = self._launch_args(x)
         S = torch.empty(yq.shape[:3], dtype=torch.int32, device=x.device) if yq is not None and self.sums else None
         lo, hi, bits = self.out_scale or (0.0, 0.0, 0)
-        _lib.check(_lib.load().dfq_i8_affine_maxpool(
-            _ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y), _ptr(yq), _ptr(S), C.c_float(lo),
-            C.c_float(hi), bits, _lib.table_ptr(g), _lib.stream_ptr()), "dfq_i8_affine_maxpool (%s)" % self.layer_name)
+        with _lib.launch(x) as st:
+            _lib.check(_lib.load().dfq_i8_affine_maxpool(
+                _ptr(x) if self.codes_in else None, None if self.codes_in else _ptr(x), _ptr(y), _ptr(yq), _ptr(S), C.c_float(lo),
+                C.c_float(hi), bits, _lib.table_ptr(g), st), "dfq_i8_affine_maxpool (%s)" % self.layer_name)
         codes = None if yq is None else (yq, S)
         return (codes, y) if codes is not None and y is not None else (y if codes is None else codes)
 
@@ -1013,8 +1041,9 @@ class Int8UpsampleBilinear(nn.Module):
         x = x.contiguous()
         g = np.zeros(1, _lib.I8_RESIZE_DT)
         g[0] = (N, self.channels, H, W, OH, OW, int(self.align_corners), coff, cstride, self.out_scale) + self.clamp
-        _lib.check(_lib.load().dfq_i8_upsample_bilinear(_ptr(x), None, _ptr(out), _lib.table_ptr(g), _lib.stream_ptr()),
-                   "dfq_i8_upsample_bilinear (%s)" % self.layer_name)
+        with _lib.launch(x, out) as st:
+            _lib.check(_lib.load().dfq_i8_upsample_bilinear(_ptr(x), None, _ptr(out), _lib.table_ptr(g), st),
+                       "dfq_i8_upsample_bilinear (%s)" % self.layer_name)
         return out
 
     def extra_repr(self):
@@ -1047,9 +1076,10 @@ class AffineInt8UpsampleBilinear(nn.Module):
         g = np.zeros(1, _lib.I8_AFFINE_RESIZE_DT)
         g[0] = (N, self.channels, H, W, OH, OW, int(self.align_corners), coff, cstride) + self.pre + \
             (self.obs or (0.0, 0.0, 0)) + self.post + self.out
-        _lib.check(_lib.load().dfq_i8_affine_upsample_bilinear(_ptr(x), _ptr(codes), _ptr(S), _lib.table_ptr(g),
-                                                               _lib.stream_ptr()),
-                   "dfq_i8_affine_upsample_bilinear (%s)" % self.layer_name)
+        with _lib.launch(x) as st:
+            _lib.check(_lib.load().dfq_i8_affine_upsample_bilinear(_ptr(x), _ptr(codes), _ptr(S), _lib.table_ptr(g),
+                                                                   st),
+                       "dfq_i8_affine_upsample_bilinear (%s)" % self.layer_name)
         return codes, S
 
     def extra_repr(self):

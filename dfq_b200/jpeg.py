@@ -19,6 +19,7 @@ import ctypes as C
 import dataclasses
 import functools
 import struct
+import threading
 
 import numpy as np
 import torch
@@ -326,7 +327,8 @@ def parse(items, what="images"):
 def decode(items) -> list:
     """uint8 [H, W, 3] device tensors, one per JPEG of items (a list of bytes), each equal to Pillow's
     np.asarray(Image.open(BytesIO(b)).convert("RGB")).  One host-to-device copy, and no host synchronisation; a corrupt
-    entropy-coded segment is reported by the next check().  The tensors are views of one device block."""
+    entropy-coded segment is reported by the next check().  The tensors are views of one device block, on the current device,
+    decoded on its current stream."""
     from . import preprocess
     if isinstance(items, (bytes, bytearray, memoryview)) or not hasattr(items, "__len__") or len(items) == 0:
         raise _lib.DfqError("decode takes a non-empty list of JPEG bytes")
@@ -343,18 +345,21 @@ def decode(items) -> list:
 
 
 def check(device=None) -> None:
-    """Wait for the device decodes enqueued so far on device (default: every device used) and raise DfqError for the first
-    corrupt entropy-coded segment found since the last check().  The image's pixels are unspecified; the rest of its batch
-    is decoded."""
+    """Wait for the decodes enqueued so far on the current stream of device (default: every device used) and raise DfqError
+    for the first corrupt entropy-coded segment found since the last check().  The image's pixels are unspecified;
+    the rest of its batch is decoded.  The error word is one per device, shared by every thread and stream decoding
+    there, and is read on that device's current stream: wait for decodes enqueued on other streams (wait_stream)
+    before calling check()."""
     devs = [torch.device(device)] if device is not None else list(_state)
     for dev in devs:
         st = _state.get(dev)
         if st is None:
             continue
-        w = st["word"].cpu().tolist()
-        calls = st["calls"]
-        st["word"].copy_(torch.tensor(_CLEAR), non_blocking=False)
-        st["calls"] = 0
+        with _state_lock:
+            w = st["word"].cpu().tolist()
+            calls = st["calls"]
+            st["word"].copy_(torch.tensor(_CLEAR), non_blocking=False)
+            st["calls"] = 0
         if w[0] != _CLEAR[0]:
             call, image = w[0] >> 32, w[0] & 0xFFFFFFFF
             why = ", ".join(v for k, v in _ERRORS.items() if w[1] & k) or "error 0x%x" % w[1]
@@ -364,7 +369,10 @@ def check(device=None) -> None:
 
 # ---- batch packing and launch ---------------------------------------------------------------------------------------------
 _CLEAR = [(1 << 63) - 1, 0]
-_state = {}       # device -> {"word": int64 [2] (first corrupt (call << 32 | image), reason bits), "calls": decodes since check}
+# device -> {"word": int64 [2] (first corrupt (call << 32 | image), reason bits), "calls": decodes since check}: one word per
+# device, shared by every thread and stream decoding there; _state_lock guards the entries and the call count
+_state = {}
+_state_lock = threading.Lock()
 
 
 class _Batch:
@@ -403,12 +411,15 @@ class _Batch:
             a = np.array(self.segs, np.int64)
             sg["begin"], sg["end"], sg["image"], sg["mcu0"], sg["mcus"] = a.T
         dev = blob.device
-        st = _state.get(dev)
-        if st is None:
-            st = _state[dev] = {"word": torch.tensor(_CLEAR, dtype=torch.int64, device=dev), "calls": 0}
+        with _state_lock:
+            st = _state.get(dev)
+            if st is None:
+                st = _state[dev] = {"word": torch.tensor(_CLEAR, dtype=torch.int64, device=dev), "calls": 0}
+            call = st["calls"]
+            st["calls"] += 1
         p = np.zeros(1, _lib.JPEG_DECODE_DT)
-        p["n"], p["nseg"], p["blob_bytes"], p["call"] = len(self.images), len(self.segs), blob.numel(), st["calls"]
-        st["calls"] += 1
-        _lib.check(lib.dfq_jpeg_decode(_lib.table_ptr(p), _lib.table_ptr(im), _lib.table_ptr(sg),
-                                       C.c_void_p(blob.data_ptr()), C.c_void_p(st["word"].data_ptr()),
-                                       _lib.stream_ptr()), "dfq_jpeg_decode")
+        p["n"], p["nseg"], p["blob_bytes"], p["call"] = len(self.images), len(self.segs), blob.numel(), call
+        with _lib.launch(blob) as s:
+            _lib.check(lib.dfq_jpeg_decode(_lib.table_ptr(p), _lib.table_ptr(im), _lib.table_ptr(sg),
+                                           C.c_void_p(blob.data_ptr()), C.c_void_p(st["word"].data_ptr()), s),
+                       "dfq_jpeg_decode")

@@ -255,7 +255,8 @@ class PlaneMean(nn.Module):
     """ncnn's mean of each (image, channel) plane of x [N, C, ...] (dfq_i8_plane_mean): a sequential fp32 sum from 0.f in
     plane order, then * fp32(1 / P) (Reduction MEAN, divide=False) or / P (Pooling global average, divide=True); returns
     fp32 [N, C].  It is not torch's mean, which sums in another order.  With out_scale (set by chain_int8 only) it returns
-    the consumer's int8 codes [N, 1, 1, round_up(C, 16)] instead, q8 at out_scale."""
+    the consumer's int8 codes [N, 1, 1, round_up(C, 16)] instead, q8 at out_scale.  Runs on x's device and its current
+    stream, whichever device is current."""
 
     def __init__(self, divide, out_scale=None, name=None):
         super().__init__()
@@ -276,9 +277,10 @@ class PlaneMean(nn.Module):
             y = torch.empty((N, Cn), dtype=torch.float32, device=x.device)
         else:
             yq = torch.empty((N, 1, 1, (Cn + 15) // 16 * 16), dtype=torch.int8, device=x.device)
-        _lib.check(_lib.load().dfq_i8_plane_mean(I._ptr(x), I._ptr(y), I._ptr(yq), N, Cn, P, int(self.divide),
-                                                 C.c_float(0.0 if self.out_scale is None else self.out_scale),
-                                                 _lib.stream_ptr()), "dfq_i8_plane_mean (layer %s)" % self.layer_name)
+        with _lib.launch(x) as st:
+            _lib.check(_lib.load().dfq_i8_plane_mean(I._ptr(x), I._ptr(y), I._ptr(yq), N, Cn, P, int(self.divide),
+                                                     C.c_float(0.0 if self.out_scale is None else self.out_scale),
+                                                     st), "dfq_i8_plane_mean (layer %s)" % self.layer_name)
         return y if yq is None else yq
 
     def extra_repr(self):

@@ -18,6 +18,7 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 import struct
+import threading
 import zlib
 
 import numpy as np
@@ -169,7 +170,7 @@ def parse(items, what="labels"):
 def decode(items) -> list:
     """uint8 [H, W] device tensors, one per PNG of items (a list of bytes), each equal to np.array(Image.open(BytesIO(b))).
     One host-to-device copy, and no host synchronisation; a corrupt stream is reported by the next check().  The tensors
-    are views of one device block."""
+    are views of one device block, on the current device, decoded on its current stream."""
     from . import preprocess
     if isinstance(items, (bytes, bytearray, memoryview)) or not hasattr(items, "__len__") or len(items) == 0:
         raise _lib.DfqError("decode takes a non-empty list of PNG bytes")
@@ -187,18 +188,22 @@ def decode(items) -> list:
 
 
 def check(device=None) -> None:
-    """Wait for the device decodes enqueued so far on device (default: every device used) and raise DfqError for the first
-    corrupt stream found since the last check().  That image's label is unspecified; the rest of its batch is decoded.  The
-    reasons name every fault found in that image: a row with a bad filter type can precede a fault in the compressed data."""
+    """Wait for the decodes enqueued so far on the current stream of device (default: every device used) and raise DfqError
+    for the first corrupt stream found since the last check().  That image's label is unspecified; the rest of its
+    batch is decoded.  The reasons name every fault found in that image: a row with a bad filter type can precede a
+    fault in the compressed data.  The error word is one per device, shared by every thread and stream decoding
+    there, and is read on that device's current stream: wait for decodes enqueued on other streams (wait_stream)
+    before calling check()."""
     devs = [torch.device(device)] if device is not None else list(_state)
     for dev in devs:
         st = _state.get(dev)
         if st is None:
             continue
-        w = st["word"].cpu().tolist()
-        calls = st["calls"]
-        st["word"].copy_(torch.tensor(_CLEAR), non_blocking=False)
-        st["calls"] = 0
+        with _state_lock:
+            w = st["word"].cpu().tolist()
+            calls = st["calls"]
+            st["word"].copy_(torch.tensor(_CLEAR), non_blocking=False)
+            st["calls"] = 0
         if w[0] != _CLEAR[0]:
             call, image = w[0] >> 32, w[0] & 0xFFFFFFFF
             why = ", ".join(v for k, v in _ERRORS.items() if w[1] & k) or "error 0x%x" % w[1]
@@ -208,7 +213,10 @@ def check(device=None) -> None:
 
 # ---- batch packing and launch ---------------------------------------------------------------------------------------------
 _CLEAR = [(1 << 63) - 1, 0]
-_state = {}       # device -> {"word": int64 [2] (first corrupt (call << 32 | image), reason bits), "calls": decodes since check}
+# device -> {"word": int64 [2] (first corrupt (call << 32 | image), reason bits), "calls": decodes since check}: one word per
+# device, shared by every thread and stream decoding there; _state_lock guards the entries and the call count
+_state = {}
+_state_lock = threading.Lock()
 
 
 def _round(n):
@@ -246,11 +254,14 @@ class _Batch:
             im[k]["work"], im[k]["dst"] = at + work, at + dst
             im[k]["H"], im[k]["W"] = p.shape
         dev = blob.device
-        st = _state.get(dev)
-        if st is None:
-            st = _state[dev] = {"word": torch.tensor(_CLEAR, dtype=torch.int64, device=dev), "calls": 0}
+        with _state_lock:
+            st = _state.get(dev)
+            if st is None:
+                st = _state[dev] = {"word": torch.tensor(_CLEAR, dtype=torch.int64, device=dev), "calls": 0}
+            call = st["calls"]
+            st["calls"] += 1
         d = np.zeros(1, _lib.PNG_DECODE_DT)
-        d["n"], d["blob_bytes"], d["call"] = len(self.images), blob.numel(), st["calls"]
-        st["calls"] += 1
-        _lib.check(lib.dfq_png_decode(_lib.table_ptr(d), _lib.table_ptr(im), C.c_void_p(blob.data_ptr()),
-                                      C.c_void_p(st["word"].data_ptr()), _lib.stream_ptr()), "dfq_png_decode")
+        d["n"], d["blob_bytes"], d["call"] = len(self.images), blob.numel(), call
+        with _lib.launch(blob) as s:
+            _lib.check(lib.dfq_png_decode(_lib.table_ptr(d), _lib.table_ptr(im), C.c_void_p(blob.data_ptr()),
+                                          C.c_void_p(st["word"].data_ptr()), s), "dfq_png_decode")

@@ -236,9 +236,10 @@ def _launch(images, labels, xtaps, ytaps, near, filt, norm, out_h, out_w, mean, 
     p["mean"], p["std"], p["mean64"], p["std64"] = mean, std, mean, std
     out = torch.empty(n, 3, out_h, out_w, dtype=torch.float32, device=dev)
     lab = torch.empty(n, out_h, out_w, dtype=torch.float32, device=dev) if labels is not None else None
-    _lib.check(lib.dfq_pre_resample(_lib.table_ptr(p), _lib.table_ptr(desc), C.c_void_p(blob.data_ptr()),
-                                    C.c_void_p(out.data_ptr()), C.c_void_p(lab.data_ptr()) if lab is not None else None,
-                                    _lib.stream_ptr()), "dfq_pre_resample")
+    with _lib.launch(blob) as st:
+        _lib.check(lib.dfq_pre_resample(_lib.table_ptr(p), _lib.table_ptr(desc), C.c_void_p(blob.data_ptr()),
+                                        C.c_void_p(out.data_ptr()), C.c_void_p(lab.data_ptr()) if lab is not None else None,
+                                        st), "dfq_pre_resample")
     return out, lab
 
 

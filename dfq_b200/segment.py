@@ -68,14 +68,16 @@ def _run(logits, labels, pred, count, OH, OW, ac, label_type):
     N, C_, H, W = logits.shape
     d = np.zeros(1, _lib.SEG_ARGMAX_DT)
     d[0] = (N, C_, H, W, OH, OW, ac, label_type)
-    _lib.check(_lib.load().dfq_seg_argmax(_ptr(logits), _ptr(labels), _ptr(pred), _ptr(count), _lib.table_ptr(d),
-                                          _lib.stream_ptr()), "dfq_seg_argmax")
+    with _lib.launch(logits, labels, pred, count) as st:
+        _lib.check(_lib.load().dfq_seg_argmax(_ptr(logits), _ptr(labels), _ptr(pred), _ptr(count), _lib.table_ptr(d), st),
+                   "dfq_seg_argmax")
 
 
 def predict(logits, size=None, align_corners=None) -> torch.Tensor:
     """int64 [N, OH, OW]: torch.max(F.interpolate(logits, size, mode="bilinear", align_corners=align_corners), 1)[1] bit for
     bit, or torch.max(logits, 1)[1] when size is None or logits' own [H, W].  logits: contiguous fp32 [N, C, H, W] on the
-    GPU, C at most 160.  align_corners must be True or False when the size changes.  Does not synchronise with the host."""
+    GPU, C at most 160.  align_corners must be True or False when the size changes.  Runs on logits' device and its current
+    stream, the result on that device, whichever device is current.  Does not synchronise with the host."""
     N, C_, H, W = _logits(logits).shape
     OH, OW, ac = _size(size, H, W, align_corners)
     pred = torch.empty(N, OH, OW, dtype=torch.int64, device=logits.device)
@@ -87,7 +89,8 @@ class Evaluator:
     """utils/metrics.py Evaluator with the counting on the GPU.  add_logits counts a batch from the network's logits;
     confusion_matrix and the four metrics read the matrix back, and are what the reference's methods compute on the same
     matrix, NaN included.  The matrix is kept as int64 [num_class, num_class] on the device of the first batch and never
-    leaves it between batches."""
+    leaves it between batches; add_logits counts on that device's current stream, whichever device is current, and a batch
+    on another device raises DfqError."""
 
     def __init__(self, num_class):
         if not isinstance(num_class, int) or isinstance(num_class, bool) or not 1 <= num_class <= MAX_CLASSES:

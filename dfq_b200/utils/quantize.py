@@ -73,9 +73,10 @@ def fake_quant_explicit(x, num_bits, min_value, max_value, symmetric=False, out=
     else:
         yd = torch.empty_like(xd)
     if xd.numel():
-        _lib.check(lib.dfq_quant_dequant(_ptr(xd), _ptr(yd), xd.numel(), C.c_float(mn), C.c_double(scale),
-                                         C.c_float(qmin), C.c_float(qmax), int(div_mode), None, _lib.stream_ptr()),
-                   "dfq_quant_dequant")
+        with _lib.launch(xd) as st:
+            _lib.check(lib.dfq_quant_dequant(_ptr(xd), _ptr(yd), xd.numel(), C.c_float(mn), C.c_double(scale),
+                                             C.c_float(qmin), C.c_float(qmax), int(div_mode), None, st),
+                       "dfq_quant_dequant")
     if out is not None and yd is not out:
         out.copy_(yd.view(out.shape))
         return out
@@ -92,9 +93,10 @@ def fake_quant_device_range(x, num_bits, min_t, max_t, symmetric=False, prologue
     mx = max_t.detach().reshape(-1)[:1].to(device=xd.device, dtype=torch.float32).contiguous()
     yd = out if (out is not None and out.is_cuda and out.is_contiguous()) else torch.empty_like(xd)
     if xd.numel():
-        _lib.check(lib.dfq_quant_dequant_dev(_ptr(xd), _ptr(yd), xd.numel(), _ptr(mn), _ptr(mx), int(num_bits),
-                                             1 if symmetric else 0, int(div_mode), int(prologue), None,
-                                             _lib.stream_ptr()), "dfq_quant_dequant_dev")
+        with _lib.launch(xd) as st:
+            _lib.check(lib.dfq_quant_dequant_dev(_ptr(xd), _ptr(yd), xd.numel(), _ptr(mn), _ptr(mx), int(num_bits),
+                                                 1 if symmetric else 0, int(div_mode), int(prologue), None,
+                                                 st), "dfq_quant_dequant_dev")
     if out is not None and yd is not out:
         out.copy_(yd.view(out.shape))
         return out
@@ -106,7 +108,8 @@ def tensor_minmax(x):
     lib = _lib.load()
     xd, _ = _dev_f32(x.detach())
     out = xd.new_empty((2,))
-    _lib.check(lib.dfq_minmax(_ptr(xd), xd.numel(), _ptr(out), _lib.stream_ptr()), "dfq_minmax")
+    with _lib.launch(xd) as st:
+        _lib.check(lib.dfq_minmax(_ptr(xd), xd.numel(), _ptr(out), st), "dfq_minmax")
     return out
 
 
@@ -139,8 +142,9 @@ def per_sample_minmax_mean(x, batch=None):
     per = _per_sample(xd.numel(), batch)
     out = xd.new_empty((2,))
     scratch = xd.new_empty((2 * batch,))
-    _lib.check(lib.dfq_act_minmax_per_sample(_ptr(xd), batch, per, _ptr(out), _ptr(scratch), _lib.stream_ptr()),
-               "dfq_act_minmax_per_sample")
+    with _lib.launch(xd) as st:
+        _lib.check(lib.dfq_act_minmax_per_sample(_ptr(xd), batch, per, _ptr(out), _ptr(scratch), st),
+                   "dfq_act_minmax_per_sample")
     return out
 
 
@@ -163,11 +167,12 @@ def observe_and_quant(x, num_bits, flags, running_min=None, running_max=None, mo
     rmax, rmax_back = _running_buffer(running_max, xd.device, "running_max") if running_max is not None else (None, None)
     yd = out if (out is not None and out.is_cuda and out.is_contiguous()) else torch.empty_like(xd)
     if xd.numel():
-        _lib.check(lib.dfq_observe_quant(_ptr(xd), _ptr(yd), batch, per,
-                                         _ptr(rmin) if rmin is not None else None,
-                                         _ptr(rmax) if rmax is not None else None, None, int(flags),
-                                         C.c_double(momentum), int(num_bits), 1 if symmetric else 0, int(div_mode), int(prologue),
-                                         _lib.stream_ptr()), "dfq_observe_quant")
+        with _lib.launch(xd) as st:
+            _lib.check(lib.dfq_observe_quant(_ptr(xd), _ptr(yd), batch, per,
+                                             _ptr(rmin) if rmin is not None else None,
+                                             _ptr(rmax) if rmax is not None else None, None, int(flags),
+                                             C.c_double(momentum), int(num_bits), 1 if symmetric else 0, int(div_mode), int(prologue),
+                                             st), "dfq_observe_quant")
     for back, buf in ((rmin_back, rmin), (rmax_back, rmax)):
         if back is not None:
             back.copy_(buf.view(back.shape))

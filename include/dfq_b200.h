@@ -896,7 +896,7 @@ int dfq_cls_count(const float* logits, const int64_t* labels, int64_t* pred, uin
  * descending rank bits (-0.0 equal to +0.0, NaN last) and flags[t] = DFQ_MAP_IGNORED / _TP / _FP; pass keys and flags
  * offset to where the batch is appended.  Checks needing device data set bits of *error (atomicOr) instead of failing:
  * a detection label outside 1 .. C-1, a ground-truth label outside 0 .. C-1, offsets that do not run from 0 up to T
- * (resp. G) without decreasing; an image with bad offsets is skipped.  Does not synchronise.  DFQ_E_ARG, with a reason
+ * (resp. G) without decreasing; with bad offsets nothing of the batch is matched.  Does not synchronise.  DFQ_E_ARG, with a reason
  * and before any write: C < 2, N < 1, T or G < 0, a NULL pointer that is needed (the detection buffers when T > 0, the
  * ground-truth buffers when G > 0), boxes not 16-byte aligned.  DFQ_E_UNSUPPORTED: C above 4096, T above INT32_MAX. */
 int dfq_map_match(const float* det_boxes, const int64_t* det_labels, const float* det_probs, const int64_t* det_offsets,
