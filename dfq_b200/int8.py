@@ -2502,8 +2502,8 @@ class _Rewriter:
             self.hand_over(pp, u, u.name)
             return u.name, "codes", ("codes",)
         codes_node, y_node = _split(g, u)
-        for v in pp.codes:
-            v.replace_input_with(u, codes_node)
+        for v in pp.codes:                                      # the input only: its residual may be the pool's fp32
+            v.update_arg(0, codes_node)
         u.replace_all_uses_with(y_node, delete_user_cb=lambda x: x not in (y_node, codes_node))
         self.edges += [(u.name, v.target, pp.clamp) for v in pp.codes if v in self.convs]
         return u.name, "fp32", ("fp32", "codes")

@@ -188,6 +188,24 @@ def test_resnet_style_stem_pools_in_fp32_mode(monkeypatch):
     assert [a[:3] for a in gm.fused_adds] == [("b", "add", "pool")]
 
 
+def test_fp32_pool_whose_codes_consumer_adds_the_pool_as_its_residual(monkeypatch):
+    """conv -> relu -> maxpool -> {b, residual of b's own add}: b reads the pool's codes and adds its fp32 output.  Only
+    b's input may become the codes: its residual, the same pool node, stays the pool's fp32 output."""
+    class M(nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.stem, self.pool = nn.Conv2d(3, 16, 3, 1, 1), nn.MaxPool2d(2, 2)
+            self.b, self.z = nn.Conv2d(16, 16, 3, 1, 1), nn.Conv2d(16, 8, 1)
+
+        def forward(self, x):
+            t = self.pool(F.relu(self.stem(x)))
+            return self.z(torch.relu(F.relu6(self.b(t)) + t))
+    gm, _ = _chain(monkeypatch, M(), _x(), {"stem": 7.0, "b": 3.0, "z": 2.0})
+    assert gm.fused_pools == [("pool", "fp32", ("fp32", "codes"))]
+    assert ("pool", "b", (0.0, INF)) in gm.requantized_edges
+    assert [a[:3] for a in gm.fused_adds] == [("b", "add", "pool")]
+
+
 def test_pool_cat_needs_residual():
     from dfq_b200 import _lib, int8
     with pytest.raises(_lib.DfqError, match="pool_cat=True builds on residual=True"):
